@@ -122,6 +122,7 @@ def _load():
         "glic_debug_geom": (i32, [i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "glic_debug_binning": (i32, [i32, vp, i64, i64, vp, vp, vp, vp]),
         "glic_debug_image": (i32, [i32, i32, vp, vp, vp, vp, vp, C.POINTER(i64), vp]),
+        "glic_debug_spans": (i32, [i32, vp, C.POINTER(u32), vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)

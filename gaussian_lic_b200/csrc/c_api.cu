@@ -39,6 +39,12 @@ static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t
 static int check_view(const glic_view* v) {
     if (!v || !v->viewmatrix || !v->projmatrix || !v->campos) { set_error("view: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (v->width <= 0 || v->height <= 0) { set_error("view: non-positive image size"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const int64_t T = (int64_t)((v->width + TILE - 1) / TILE) * ((v->height + TILE - 1) / TILE);
+    if (T > GLIC_MAX_TILES) {
+        set_error("view: " + std::to_string(v->width) + "x" + std::to_string(v->height) + " has " + std::to_string(T) +
+                  " tiles of 16x16, more than GLIC_MAX_TILES = " + std::to_string(GLIC_MAX_TILES));
+        return GLIC_ERR_INVALID_ARGUMENT;
+    }
     return GLIC_OK;
 }
 
@@ -190,7 +196,7 @@ int glic_forward_render(int P, const glic_view* view, int no_color, int64_t R, v
 
     int cur = 0;
     if (R > 0) {
-        const int bit = (int)higher_msb((uint32_t)T);                       // rasterizer_impl.cu:417
+        const int bit = tile_sort_bits(T);                                  // rasterizer_impl.cu:417
         { StageTimer _t(GLIC_STAGE_EMIT, s);
           if (int e = sort_prepare(R, bit, bin.sort_temp, s)) return e;      // emit builds the tile sort's digit histograms
           if (int e = launch_emit_keys(P, vp, g, bin.keys[0], bin.vals[0], R, sort_hist(bin.sort_temp), bit, s)) return e; }
@@ -262,7 +268,7 @@ int glic_forward(int P, int sh_degree, int M, const float* means3D, const float*
       const int cur0 = launch_sort_pairs32(P, 32, g.depth_keys, g.order, g.sort_temp, g.sort_temp_size, s, nullptr, /*hist_ready=*/true);
       if (cur0 < 0) return cur0;
       if (int e = launch_depth_scan(P, g, g.order[cur0], cap, s)) return e; }
-    const int bit = (int)higher_msb((uint32_t)T);
+    const int bit = tile_sort_bits(T);
     { StageTimer _t(GLIC_STAGE_EMIT, s);
       if (int e = sort_prepare(cap, bit, bin.sort_temp, s)) return e;        // emit builds the tile sort's digit histograms
       if (int e = launch_emit_keys(P, vp, g, bin.keys[0], bin.vals[0], cap, sort_hist(bin.sort_temp), bit, s)) return e; }
@@ -312,7 +318,7 @@ int glic_backward(int P, int sh_degree, int M, const float* means3D, const float
         SampleState smp = SampleState::carve(const_cast<void*>(sample_ws), max_buckets);
         // the sort's ping-pong parity is a pure function of the pass count
         const int T = vp.grid_x * vp.grid_y;
-        const int passes = ((int)higher_msb((uint32_t)T) + 7) / 8;
+        const int passes = (tile_sort_bits(T) + 7) / 8;
         const int cur = passes & 1;
         StageTimer _t(GLIC_STAGE_RENDER_BWD, s);
         if (int e = launch_render_backward(P, vp, max_buckets, bin.vals[cur], g, img, smp, dL_dpix, dL_dmeans2D, dL_dconic,
@@ -354,7 +360,7 @@ int glic_backward_compact_internal(int P, int sh_degree, int M, const float* mea
         const int64_t max_buckets = glic_max_buckets(R, vp.W, vp.H);
         SampleState smp = SampleState::carve(const_cast<void*>(sample_ws), max_buckets);
         const int T = vp.grid_x * vp.grid_y;
-        const int passes = ((int)higher_msb((uint32_t)T) + 7) / 8;
+        const int passes = (tile_sort_bits(T) + 7) / 8;
         const int cur = passes & 1;
         StageTimer _t(GLIC_STAGE_RENDER_BWD, s);
         if (int e = launch_render_backward(P, vp, max_buckets, bin.vals[cur], g, img, smp, dL_dpix, dL_dmeans2D, dL_dconic,
@@ -390,6 +396,21 @@ int glic_debug_geom(int P, const void* geom_ws, float* depth, float* xy, float* 
     GeomState g = GeomState::carve(const_cast<void*>(geom_ws), P);
     debug_geom_kernel<<<(P + 255) / 256, 256, 0, (cudaStream_t)stream>>>(P, g, depth, xy, conic_opacity, rgb, tiles_touched, offsets, clamped);
     GLIC_LAUNCH_CHECK();
+    return GLIC_OK;
+}
+
+int glic_debug_spans(int P, const void* geom_ws, uint32_t* count_cap_host, void* stream) {
+    if (!count_cap_host) { set_error("debug_spans: null output"); return GLIC_ERR_INVALID_ARGUMENT; }
+    count_cap_host[0] = count_cap_host[1] = 0;
+    if (P <= 0) return GLIC_OK;
+    if (!geom_ws) { set_error("debug_spans: null workspace"); return GLIC_ERR_WORKSPACE; }
+    cudaStream_t s = (cudaStream_t)stream;
+    GeomState g = GeomState::carve(const_cast<void*>(geom_ws), P);
+    unsigned int count = 0;
+    GLIC_CUDA_TRY(cudaMemcpyAsync(&count, &g.hdr->span_count, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    count_cap_host[0] = count;
+    count_cap_host[1] = g.span_cap;
     return GLIC_OK;
 }
 

@@ -221,6 +221,11 @@ inline uint32_t higher_msb(uint32_t n) {
     return msb;
 }
 
+// Key bits of the tile sort.  Tile ids 0 .. T-1 need higher_msb(T - 1) bits; the reference's higher_msb(T) is one bit more
+// when T is a power of two, which at T = GLIC_MAX_TILES would exceed the 16 bits the key emission histograms.  The sorted
+// order is the same either way (a stable sort on a bit every key has clear).
+inline int tile_sort_bits(int T) { return (int)higher_msb((uint32_t)(T - 1)); }
+
 // View parameters passed by value to kernels (pointers stay device pointers).
 struct ViewParams {
     const float* view;

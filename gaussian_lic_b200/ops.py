@@ -356,8 +356,11 @@ class CRasterizer:
         capi.check(lib.glic_debug_image(W, H, capi.ptr(self.image_ws), capi.ptr(d["ranges"]),
                                         capi.ptr(d["bucket_offsets"]), capi.ptr(d["n_contrib"]),
                                         capi.ptr(d["max_contrib"]), cnt, None), "debug_image")
+        spans = (C.c_uint32 * 2)()
+        capi.check(lib.glic_debug_spans(P, capi.ptr(self.geom_ws), spans, None), "debug_spans")
         torch.cuda.synchronize(dev)
         d["R"], d["B"] = int(cnt[0]), int(cnt[1])
+        d["span_count"], d["span_cap"] = int(spans[0]), int(spans[1])
         return d
 
 

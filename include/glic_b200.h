@@ -50,6 +50,10 @@ typedef enum glic_status {
 /* Tile geometry is part of the parity contract (rasterizer/cuda_rasterizer/config.h:16-17). */
 #define GLIC_TILE 16
 #define GLIC_BUCKET 32 /* checkpoint period of the per-splat backward (forward.cu:412) */
+/* Largest frame: ceil(width/16) * ceil(height/16) <= GLIC_MAX_TILES (4096x4096 is the largest square frame).  Tile ids are
+ * sorted on at most 16 bits.  Every call that takes a glic_view refuses a larger frame with GLIC_ERR_INVALID_ARGUMENT
+ * before it enqueues any work. */
+#define GLIC_MAX_TILES 65536
 
 GLIC_API const char* glic_last_error(void);
 GLIC_API int glic_abi_version(void);
@@ -257,6 +261,10 @@ GLIC_API int glic_debug_binning(int P, const void* geom_ws, int64_t num_rendered
                                 uint32_t* point_list, uint64_t* keys_sorted, void* stream);
 GLIC_API int glic_debug_image(int width, int height, const void* image_ws, uint32_t* ranges, uint32_t* bucket_offsets,
                      uint32_t* n_contrib, uint32_t* max_contrib, int64_t* counters2_host /* {R,B}, HOST pointer */, void* stream);
+/* Fill level of the row-span arena of the last forward: count_cap_host[2] = {rows requested, capacity} (HOST pointer;
+ * synchronises `stream`).  Rects of more than 32 tiles store one span per row while the arena has room; when requested >
+ * capacity, the later rects had their rows recomputed by the key emission instead. */
+GLIC_API int glic_debug_spans(int P, const void* geom_ws, uint32_t* count_cap_host, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Multi-GPU exchange step (no counterpart in the reference, which is single-GPU): in-place MEAN all-reduce of the

@@ -78,6 +78,38 @@ def grad_close(a, b, what, rtol=GRAD_RTOL, el_rtol=EL_RTOL, el_atol=EL_ATOL, el_
     assert frac <= el_frac, "%s: %.3e of the entries fail the element-wise bound (allowed %.1e)" % (what, frac, el_frac)
 
 
+# ---- path predicates of the stress scenes (tests/test_stress_scenes.py, tests/test_gpu_stress.py) ------------------------------
+def hy_fallbacks(conic_opacity, vis):
+    """Visible Gaussians whose render row cull takes the 1.11 * radius + 1 fallback: the conic's determinant cancels,
+    dcon <= 1e-3 * prod (preprocess.cu, where hy is computed; f32 as there)."""
+    co = np.asarray(conic_opacity, np.float32)
+    prod = (co[:, 0] * co[:, 2]).astype(np.float32)
+    dcon = (prod - (co[:, 1] * co[:, 1]).astype(np.float32)).astype(np.float32)
+    return int((vis & ~(dcon > np.float32(1e-3) * prod)).sum())
+
+
+def tile_rects(xy, radii, W, H):
+    """getRect of every Gaussian: (x0, y0, x1, y1) in tiles, clamped to the grid (f32 arithmetic, truncation)"""
+    gx, gy = (W + 15) // 16, (H + 15) // 16
+    x, y = np.asarray(xy, np.float32)[:, 0], np.asarray(xy, np.float32)[:, 1]
+    r = np.asarray(radii).astype(np.float32)
+    q = np.float32(0.0625)
+
+    def cl(v, hi):
+        return np.clip(np.trunc(v).astype(np.int64), 0, hi)
+    return (cl((x - r) * q, gx), cl((y - r) * q, gy), cl((x + r + np.float32(16) - np.float32(1)) * q, gx),
+            cl((y + r + np.float32(16) - np.float32(1)) * q, gy))
+
+
+def big_rect_rows(xy, radii, W, H):
+    """rows of the rects of more than 32 tiles: what the counting walk asks of the 4P-entry span arena"""
+    x0, y0, x1, y1 = tile_rects(xy, radii, W, H)
+    n = (x1 - x0) * (y1 - y0)
+    vis = np.asarray(radii) > 0
+    return int((y1 - y0)[vis & (n > 32)].sum())
+
+
+
 # ---- golden vectors of the reference itself (tests/golden/make_reference_pins.py) ------------------------------------------
 # The reference's outputs at the sizes of the reference-pin tests are stored compactly: integer outputs as SHA-256 digests,
 # images and gradients as a seeded sample plus whole-tensor statistics.
