@@ -75,6 +75,8 @@ def _load():
         "glic_fused_ssim": (i32, [i32, i32, i32, i32, f32, f32, vp, vp, vp, vp, vp, vp, vp]),
         "glic_fused_ssim_backward": (i32, [i32, i32, i32, i32, f32, f32, vp, vp, vp, vp, vp, vp, vp, vp]),
         "glic_l1_ssim_loss": (i32, [i32, i32, i32, f32, vp, vp, vp, vp, vp, sz, vp]),
+        "glic_loss_exposure_scratch_bytes": (sz, [i32, i32]),
+        "glic_l1_ssim_loss_exposure": (i32, [i32, i32, f32, vp, vp, vp, vp, vp, vp, vp, sz, vp]),
         "glic_knn_mean_dist2": (i32, [i32, vp, vp, vp, sz, vp]),
         "glic_extend_bytes": (sz, [i32, i32, i32]),
         "glic_extend": (i32, [i32, vp, vp, vp, C.POINTER(f32), C.POINTER(f32), f32, f32, f32, f32, i32, i32, vp, f32, vp, sz, vp, vp,
@@ -119,6 +121,10 @@ def _load():
         "glic_mapper_connect": (i32, [vp, C.c_char_p]),
         "glic_mapper_synchronize": (i32, [vp]),
         "glic_mapper_set_option": (i32, [vp, i32, i32]),
+        "glic_mapper_enable_exposure": (i32, [vp, f32]),
+        "glic_mapper_exposure_get": (i32, [vp, i32, C.POINTER(f32)]),
+        "glic_mapper_exposure_set": (i32, [vp, i32, C.POINTER(f32)]),
+        "glic_mapper_exposure_adam_state": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32), C.POINTER(i32)]),
         "glic_debug_geom": (i32, [i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "glic_debug_binning": (i32, [i32, vp, i64, i64, vp, vp, vp, vp]),
         "glic_debug_image": (i32, [i32, i32, vp, vp, vp, vp, vp, C.POINTER(i64), vp]),

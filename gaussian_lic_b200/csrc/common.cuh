@@ -311,4 +311,11 @@ int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, 
                         int n_slots, float grad_scale, float color_scale, float b1, float b2, float eps, const unsigned int* skip_flag,
                         unsigned int* visible_count, cudaStream_t s);
 int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flags, cudaStream_t s);
+// per-keyframe exposure (ssim.cu): one Adam step of every keyframe of a batch of S <= EXPO_MAX_SLOTS slots; slot_grads[S][12]
+constexpr int EXPO_MAX_SLOTS = 32;
+int launch_exposure_adam(int S, const int* kf_of_slot_host, const float* slot_grads, float* E, float* exp_avg, float* exp_avg_sq,
+                         int* steps, float lr, const unsigned int* skip_flag, cudaStream_t s);
+// glic_eval_psnr_ssim with an optional exposure E (3 channels) applied to img before the clamp
+int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, const float* E, float* out2, void* scratch,
+                   size_t scratch_bytes, void* stream);
 }  // namespace glic

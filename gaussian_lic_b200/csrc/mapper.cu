@@ -26,6 +26,7 @@ using namespace glic;
 namespace {
 
 constexpr int MAX_SLOTS = 32;        // world * views_per_rank
+static_assert(MAX_SLOTS <= EXPO_MAX_SLOTS, "the exposure step takes every slot of a batch");
 constexpr int RING = 8;              // pinned result ring (loss, binning counters)
 
 struct CamBlock {                    // what the rasterizer gets per view (camera.h:38-110, renderer.cpp:31-54)
@@ -94,8 +95,9 @@ struct glic_mapper {
     int* radii = nullptr;
     float *g_mean2D = nullptr, *g_conic = nullptr, *g_opacity = nullptr;
     void* geom_ws = nullptr; size_t geom_bytes = 0;
-    // ---- exchange block: geo[11*Pcap + 4] | flags words | colour slots [2][S][Pcap][3] | flag bytes [2][S][Pcap] ----
-    char* xblock = nullptr; size_t xbytes = 0, off_col = 0, off_flags = 0;
+    // ---- exchange block: geo[11*Pcap + 4] | flags words | colour slots [2][S][Pcap][3] | flag bytes [2][S][Pcap] |
+    //      exposure gradient slots [2][S][12] ----
+    char* xblock = nullptr; size_t xbytes = 0, off_col = 0, off_flags = 0, off_expo = 0;
     size_t n_geo = 0;                // floats in the reduced region (11*Pcap + 4; the tail holds the collective overflow word)
     void* peers[8] = {nullptr};
     bool connected = false;
@@ -116,6 +118,12 @@ struct glic_mapper {
     uint64_t view_counter = 0;
     glic_mapper_stats st{};
     bool run_optimizer = true;            // GLIC_MAPPER_OPT_OPTIMIZER (benchmarks time the rasterization step alone with it off)
+    // ---- per-training-keyframe exposure (glic_mapper_enable_exposure): E, Adam moments [expo_cap][12], step counts ----
+    bool expo_on = false;
+    float expo_lr = 0.f;
+    float *expo_E = nullptr, *expo_m = nullptr, *expo_v = nullptr;
+    int* expo_t = nullptr;
+    size_t expo_cap = 0;
 };
 
 namespace {
@@ -143,6 +151,9 @@ float* col_slot(const glic_mapper* m, int parity, int slot) {
 uint8_t* flag_slot(const glic_mapper* m, int parity, int slot) {
     return reinterpret_cast<uint8_t*>(m->xblock + m->off_flags) + ((size_t)parity * m->S + slot) * (size_t)m->Pcap;
 }
+float* expo_slot(const glic_mapper* m, int parity, int slot) {
+    return reinterpret_cast<float*>(m->xblock + m->off_expo) + ((size_t)parity * m->S + slot) * 12;
+}
 
 size_t xblock_layout(glic_mapper* m, uint32_t cap) {
     m->n_geo = (size_t)11 * cap + 4;
@@ -151,7 +162,8 @@ size_t xblock_layout(glic_mapper* m, uint32_t cap) {
     const size_t flag_off = sl[5];
     m->off_col = flag_off + 256;
     m->off_flags = m->off_col + (((size_t)2 * m->S * cap * 3 * sizeof(float) + 255) & ~size_t(255));
-    return m->off_flags + (((size_t)2 * m->S * cap + 255) & ~size_t(255));
+    m->off_expo = m->off_flags + (((size_t)2 * m->S * cap + 255) & ~size_t(255));
+    return m->off_expo + (((size_t)2 * m->S * 12 * sizeof(float) + 255) & ~size_t(255));
 }
 
 // (re)allocates everything whose size depends on the Gaussian capacity; copies the live rows of the arenas
@@ -185,6 +197,43 @@ int set_capacity(glic_mapper* m, uint32_t cap) {
     m->peers[m->cfg.rank] = m->xblock;
     m->Pcap = cap;
     m->st.capacity = cap;
+    return GLIC_OK;
+}
+
+// room for the exposure state of n training keyframes (keeps the existing rows)
+int expo_reserve(glic_mapper* m, size_t n) {
+    if (n <= m->expo_cap) return GLIC_OK;
+    const size_t cap = std::max<size_t>({n, 2 * m->expo_cap, 64});
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    float *E = nullptr, *m1 = nullptr, *v = nullptr;
+    int* t = nullptr;
+    MAP_TRY(dev_alloc((void**)&E, cap * 12 * sizeof(float))); MAP_TRY(dev_alloc((void**)&m1, cap * 12 * sizeof(float)));
+    MAP_TRY(dev_alloc((void**)&v, cap * 12 * sizeof(float))); MAP_TRY(dev_alloc((void**)&t, cap * sizeof(int)));
+    if (m->expo_cap) {
+        GLIC_CUDA_TRY(cudaMemcpyAsync(E, m->expo_E, m->expo_cap * 12 * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+        GLIC_CUDA_TRY(cudaMemcpyAsync(m1, m->expo_m, m->expo_cap * 12 * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+        GLIC_CUDA_TRY(cudaMemcpyAsync(v, m->expo_v, m->expo_cap * 12 * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+        GLIC_CUDA_TRY(cudaMemcpyAsync(t, m->expo_t, m->expo_cap * sizeof(int), cudaMemcpyDeviceToDevice, m->stream));
+        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    }
+    void* old[] = {m->expo_E, m->expo_m, m->expo_v, m->expo_t};
+    for (void* p : old) if (p) cudaFree(p);
+    m->expo_E = E; m->expo_m = m1; m->expo_v = v; m->expo_t = t;
+    m->expo_cap = cap;
+    return GLIC_OK;
+}
+
+// keyframes [first, last): E = [I | 0], zero moments and step counts (on the mapper's stream, which is then drained: the
+// legacy-stream cudaMemcpy / cudaMemset would not be ordered before the iterations that read these rows)
+int expo_reset(glic_mapper* m, size_t first, size_t last) {
+    if (last <= first) return GLIC_OK;
+    std::vector<float> id(12 * (last - first), 0.0f);
+    for (size_t k = 0; k < last - first; ++k) id[12 * k] = id[12 * k + 5] = id[12 * k + 10] = 1.0f;
+    GLIC_CUDA_TRY(cudaMemcpyAsync(m->expo_E + 12 * first, id.data(), id.size() * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->expo_m + 12 * first, 0, id.size() * sizeof(float), m->stream));
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->expo_v + 12 * first, 0, id.size() * sizeof(float), m->stream));
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->expo_t + first, 0, (last - first) * sizeof(int), m->stream));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     return GLIC_OK;
 }
 
@@ -281,7 +330,11 @@ int iteration(glic_mapper* m, const int* views) {
         }
         GLIC_CUDA_TRY(cudaStreamWaitEvent(s, m->gt_ready[buf], 0));
         // loss of this view (the pinned ring keeps the last local view's value for the statistics)
-        MAP_TRY(glic_l1_ssim_loss(3, H, W, m->cfg.lambda_dssim, m->color, m->gt_dev[buf], m->loss_dev + 1, m->dL_dpix, m->loss_scratch, m->loss_bytes, s));
+        if (m->expo_on)
+            MAP_TRY(glic_l1_ssim_loss_exposure(H, W, m->cfg.lambda_dssim, m->color, m->gt_dev[buf], m->expo_E + 12 * (size_t)views[slot], m->loss_dev + 1,
+                                               m->dL_dpix, expo_slot(m, parity, slot), m->loss_scratch, m->loss_bytes, s));
+        else
+            MAP_TRY(glic_l1_ssim_loss(3, H, W, m->cfg.lambda_dssim, m->color, m->gt_dev[buf], m->loss_dev + 1, m->dL_dpix, m->loss_scratch, m->loss_bytes, s));
         GLIC_CUDA_TRY(cudaEventRecord(m->gt_free[buf], s));
         CompactGrads cg;
         cg.g_rot = reinterpret_cast<float4*>(geo + goff[0]); cg.g_xyz = geo + goff[1]; cg.g_scale = geo + goff[2]; cg.g_opacity = geo + goff[3];
@@ -296,6 +349,11 @@ int iteration(glic_mapper* m, const int* views) {
                 if (q == m->cfg.rank) continue;
                 char* dst = static_cast<char*>(m->peers[q]) + (reinterpret_cast<char*>(col) - m->xblock);
                 GLIC_CUDA_TRY(cudaMemcpyAsync(dst, col, sizeof(float) * 3 * (size_t)m->P, cudaMemcpyDeviceToDevice, m->push_stream));
+                if (m->expo_on) {                  // this slot's dL/dE (the loss wrote it before the render backward ran)
+                    float* eg = expo_slot(m, parity, slot);
+                    char* edst = static_cast<char*>(m->peers[q]) + (reinterpret_cast<char*>(eg) - m->xblock);
+                    GLIC_CUDA_TRY(cudaMemcpyAsync(edst, eg, sizeof(float) * 12, cudaMemcpyDeviceToDevice, m->push_stream));
+                }
             }
         }
     }
@@ -313,6 +371,10 @@ int iteration(glic_mapper* m, const int* views) {
     if (m->run_optimizer)
     MAP_TRY(launch_adam_compact(m->P, m->Pcap, m->D, m->M, m->params, m->m1, m->m2, geo, m->Pcap, lr6, col_slot(m, parity, 0), flag_slot(m, parity, 0),
                                 campos, m->S, 1.0f / (float)m->k, color_scale, 0.9f, 0.999f, 1e-15f, reinterpret_cast<const unsigned int*>(geo_tail), m->vis_acc, s));
+    // every replica steps the batch's exposures from the same S slot gradients, in slot order
+    if (m->run_optimizer && m->expo_on)
+        MAP_TRY(launch_exposure_adam(m->S, views, expo_slot(m, parity, 0), m->expo_E, m->expo_m, m->expo_v, m->expo_t, m->expo_lr,
+                                     reinterpret_cast<const unsigned int*>(geo_tail), s));
     GLIC_CUDA_TRY(cudaMemcpyAsync(m->loss_host + r, m->loss_dev + 1, sizeof(float), cudaMemcpyDeviceToHost, s));
     GLIC_CUDA_TRY(cudaEventRecord(m->ring_ev[r], s));
     m->ring_used[r] = true;
@@ -382,6 +444,8 @@ int glic_mapper_destroy(glic_mapper* m) {
                     m->xblock, m->image_ws, m->binning_ws, m->sample_ws, m->loss_scratch, m->eval_scratch, m->extend_ws, m->color, m->final_T, m->dL_dpix,
                     m->gt_dev[0], m->gt_dev[1], m->loss_dev, m->eval_out, m->vis_acc};
     for (void* p : bufs) if (p) cudaFree(p);
+    void* expo[] = {m->expo_E, m->expo_m, m->expo_v, m->expo_t};
+    for (void* p : expo) if (p) cudaFree(p);
     for (auto& kf : m->train) if (kf.cam_dev) cudaFree(kf.cam_dev);
     for (auto& kf : m->test) if (kf.cam_dev) cudaFree(kf.cam_dev);
     if (m->counters_host) cudaFreeHost(m->counters_host);
@@ -431,6 +495,10 @@ int glic_mapper_add_keyframe(glic_mapper* m, const glic_keyframe* kfi, int is_tr
     kf.view.tan_fovx = kf.cam.tanfovx; kf.view.tan_fovy = kf.cam.tanfovy;
     kf.view.limx_neg = kf.cam.lim[0]; kf.view.limx_pos = kf.cam.lim[1]; kf.view.limy_neg = kf.cam.lim[2]; kf.view.limy_pos = kf.cam.lim[3];
     kf.view.width = m->cfg.width; kf.view.height = m->cfg.height;
+    if (is_train && m->expo_on) {
+        MAP_TRY(expo_reserve(m, m->train.size() + 1));
+        MAP_TRY(expo_reset(m, m->train.size(), m->train.size() + 1));
+    }
     (is_train ? m->train : m->test).push_back(kf);
     return GLIC_OK;
 }
@@ -559,7 +627,8 @@ int glic_mapper_evaluate(glic_mapper* m, int is_train, int index, float* psnr, f
         MAP_TRY(set_bin_capacity(m, cnt[0] + cnt[0] / 4));
     }
     GLIC_CUDA_TRY(cudaMemcpyAsync(m->gt_dev[0], kf.image, sizeof(float) * 3 * (size_t)W * H, cudaMemcpyHostToDevice, s));
-    MAP_TRY(glic_eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], m->eval_out, m->eval_scratch, m->eval_bytes, s));
+    const float* E = (is_train && m->expo_on) ? m->expo_E + 12 * (size_t)index : nullptr;      // held-out views: identity
+    MAP_TRY(eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], E, m->eval_out, m->eval_scratch, m->eval_bytes, s));
     float out2[2] = {0.f, 0.f};
     GLIC_CUDA_TRY(cudaMemcpyAsync(out2, m->eval_out, sizeof(out2), cudaMemcpyDeviceToHost, s));
     GLIC_CUDA_TRY(cudaStreamSynchronize(s));
@@ -616,6 +685,59 @@ int glic_mapper_set_option(glic_mapper* m, int option, int value) {
             return set_bin_capacity(m, value, /*exact=*/true);
         default: set_error("mapper_set_option: unknown option"); return GLIC_ERR_INVALID_ARGUMENT;
     }
+}
+
+int glic_mapper_enable_exposure(glic_mapper* m, float exposure_lr) {
+    if (!m) { set_error("mapper_enable_exposure: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!(exposure_lr >= 0.0f) || !std::isfinite(exposure_lr)) { set_error("mapper_enable_exposure: exposure_lr must be finite and >= 0"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!m->expo_on) {
+        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+        const size_t need = glic_loss_exposure_scratch_bytes(m->cfg.height, m->cfg.width);
+        if (need > m->loss_bytes) {
+            cudaFree(m->loss_scratch);
+            m->loss_scratch = nullptr;
+            MAP_TRY(dev_alloc(&m->loss_scratch, need, false));
+            m->loss_bytes = need;
+        }
+        MAP_TRY(expo_reserve(m, m->train.size()));
+        MAP_TRY(expo_reset(m, 0, m->train.size()));
+        m->expo_on = true;
+    }
+    m->expo_lr = exposure_lr;
+    return GLIC_OK;
+}
+
+static int expo_index_check(glic_mapper* m, int index, const void* buf, const char* what) {
+    if (!m || !buf) { set_error(std::string(what) + ": null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!m->expo_on) { set_error(std::string(what) + ": exposure is not enabled (glic_mapper_enable_exposure)"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (index < 0 || index >= (int)m->train.size()) { set_error(std::string(what) + ": training keyframe index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
+    return GLIC_OK;
+}
+
+int glic_mapper_exposure_get(glic_mapper* m, int index, float* out12) {
+    MAP_TRY(expo_index_check(m, index, out12, "mapper_exposure_get"));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    GLIC_CUDA_TRY(cudaMemcpy(out12, m->expo_E + 12 * (size_t)index, 12 * sizeof(float), cudaMemcpyDeviceToHost));
+    return GLIC_OK;
+}
+
+int glic_mapper_exposure_set(glic_mapper* m, int index, const float* in12) {
+    MAP_TRY(expo_index_check(m, index, in12, "mapper_exposure_set"));
+    for (int j = 0; j < 12; ++j)
+        if (!std::isfinite(in12[j])) { set_error("mapper_exposure_set: non-finite entry"); return GLIC_ERR_INVALID_ARGUMENT; }
+    GLIC_CUDA_TRY(cudaMemcpyAsync(m->expo_E + 12 * (size_t)index, in12, 12 * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    return GLIC_OK;
+}
+
+int glic_mapper_exposure_adam_state(glic_mapper* m, int index, float* exp_avg12, float* exp_avg_sq12, int* step) {
+    MAP_TRY(expo_index_check(m, index, step, "mapper_exposure_adam_state"));
+    if (!exp_avg12 || !exp_avg_sq12) { set_error("mapper_exposure_adam_state: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    GLIC_CUDA_TRY(cudaMemcpy(exp_avg12, m->expo_m + 12 * (size_t)index, 12 * sizeof(float), cudaMemcpyDeviceToHost));
+    GLIC_CUDA_TRY(cudaMemcpy(exp_avg_sq12, m->expo_v + 12 * (size_t)index, 12 * sizeof(float), cudaMemcpyDeviceToHost));
+    GLIC_CUDA_TRY(cudaMemcpy(step, m->expo_t + index, sizeof(int), cudaMemcpyDeviceToHost));
+    return GLIC_OK;
 }
 
 int glic_mapper_synchronize(glic_mapper* m) {

@@ -37,15 +37,34 @@ __device__ __forceinline__ float pix_or_zero(const float* __restrict__ img, int 
     return (x >= 0 && y >= 0 && x < W && y < H) ? img[(size_t)y * W + x] : 0.0f;
 }
 
+// Per-image affine exposure (glic_l1_ssim_loss_exposure): E is 3x4 row-major and output channel c is
+//   out_c = E[0][c]*r + E[1][c]*g + E[2][c]*b + E[c][3]
+// (Inria 3DGS: matmul(img_hwc, E[:3,:3]) + E[:3,3]), evaluated in this fixed fma order so that E = [I | 0] gives out == img
+// exactly for finite non-negative images.
+struct ExpoCoef { float e0, e1, e2, e3; };
+
+__device__ __forceinline__ ExpoCoef expo_coef(const float* __restrict__ E, int c) { return {E[c], E[4 + c], E[8 + c], E[4 * c + 3]}; }
+
+// i: pixel index within a plane; img: the three planes of the rendered image, HW floats apart
+__device__ __forceinline__ float expose(const float* __restrict__ img, size_t HW, size_t i, ExpoCoef e) {
+    float acc = e.e3;
+    acc = fmaf(img[i], e.e0, acc);
+    acc = fmaf(img[HW + i], e.e1, acc);
+    return fmaf(img[2 * HW + i], e.e2, acc);
+}
+
 // Register-tiled separable 11-tap convolution.  Horizontal pass: one work item = 4 consecutive outputs
 // of one halo row (14 loads per image instead of 44); vertical pass: one thread = 4 consecutive rows of
 // one column (14 loads per moment instead of 44).  Row strides 43 / 33 keep both passes bank-conflict free.
 // LOSS = true: additionally accumulates (1-lambda)*|a-b| - lambda*ssim, scaled by 1/N, into *loss.
-template <bool LOSS>
-__global__ void __launch_bounds__(ST)
-ssim_forward_kernel(int H, int W, float C1, float C2, const float* __restrict__ img1, const float* __restrict__ img2,
-                    float* __restrict__ ssim_map, float* __restrict__ dm_dmu1, float* __restrict__ dm_dsigma1_sq,
-                    float* __restrict__ dm_dsigma12, float lambda_dssim, float inv_n, float* __restrict__ loss) {
+// EXPO = true: img1 is the three planes of the rendered image and the tile's channel of the exposed image is formed in the
+// halo load (it never exists in global memory); SSIM, its partial maps and the L1 term are those of the exposed image.
+template <bool LOSS, bool EXPO>
+__device__ __forceinline__ void
+ssim_forward_tile(int H, int W, float C1, float C2, const float* __restrict__ img1, const float* __restrict__ img2,
+                  float* __restrict__ ssim_map, float* __restrict__ dm_dmu1, float* __restrict__ dm_dsigma1_sq,
+                  float* __restrict__ dm_dsigma12, float lambda_dssim, float inv_n, float* __restrict__ loss,
+                  const float* __restrict__ E) {
     __shared__ float s1[SH_][SH_ + 1];
     __shared__ float s2[SH_][SH_ + 1];
     __shared__ float2 h01[SH_][SB + 1];          // horizontal pass of (x, y)
@@ -54,14 +73,24 @@ ssim_forward_kernel(int H, int W, float C1, float C2, const float* __restrict__ 
     __shared__ float red[ST / 32];
     const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
     const size_t plane = (size_t)blockIdx.z * H * W;
-    const float* a = img1 + plane;
+    const float* a = img1 + (EXPO ? 0 : plane);
     const float* b = img2 + plane;
     const int x0 = blockIdx.x * SB, y0 = blockIdx.y * SB;
 
-    for (int i = tid; i < SH_ * SH_; i += ST) {
-        const int ly = i / SH_, lx = i % SH_;
-        s1[ly][lx] = pix_or_zero(a, y0 + ly - HALO, x0 + lx - HALO, H, W);
-        s2[ly][lx] = pix_or_zero(b, y0 + ly - HALO, x0 + lx - HALO, H, W);
+    if (EXPO) {
+        const ExpoCoef e = expo_coef(E, blockIdx.z);
+        for (int i = tid; i < SH_ * SH_; i += ST) {
+            const int ly = i / SH_, lx = i % SH_;
+            const int y = y0 + ly - HALO, x = x0 + lx - HALO;
+            s1[ly][lx] = (x >= 0 && y >= 0 && x < W && y < H) ? expose(a, (size_t)H * W, (size_t)y * W + x, e) : 0.0f;
+            s2[ly][lx] = pix_or_zero(b, y, x, H, W);
+        }
+    } else {
+        for (int i = tid; i < SH_ * SH_; i += ST) {
+            const int ly = i / SH_, lx = i % SH_;
+            s1[ly][lx] = pix_or_zero(a, y0 + ly - HALO, x0 + lx - HALO, H, W);
+            s2[ly][lx] = pix_or_zero(b, y0 + ly - HALO, x0 + lx - HALO, H, W);
+        }
     }
     __syncthreads();
     for (int i = tid; i < SH_ * (SB / RPT); i += ST) {
@@ -158,14 +187,32 @@ ssim_forward_kernel(int H, int W, float C1, float C2, const float* __restrict__ 
     }
 }
 
+template <bool LOSS>
+__global__ void __launch_bounds__(ST)
+ssim_forward_kernel(int H, int W, float C1, float C2, const float* __restrict__ img1, const float* __restrict__ img2,
+                    float* __restrict__ ssim_map, float* __restrict__ dm_dmu1, float* __restrict__ dm_dsigma1_sq,
+                    float* __restrict__ dm_dsigma12, float lambda_dssim, float inv_n, float* __restrict__ loss) {
+    ssim_forward_tile<LOSS, false>(H, W, C1, C2, img1, img2, ssim_map, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, lambda_dssim, inv_n,
+                                   loss, nullptr);
+}
+
+// forward of the exposed loss: the partial maps of SSIM(out, gt) and the loss of out
+__global__ void __launch_bounds__(ST)
+ssim_loss_exposure_forward_kernel(int H, int W, float C1, float C2, const float* __restrict__ img, const float* __restrict__ gt,
+                                  const float* __restrict__ E, float* __restrict__ dm_dmu1, float* __restrict__ dm_dsigma1_sq,
+                                  float* __restrict__ dm_dsigma12, float lambda_dssim, float inv_n, float* __restrict__ loss) {
+    ssim_forward_tile<true, true>(H, W, C1, C2, img, gt, nullptr, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, lambda_dssim, inv_n, loss, E);
+}
+
 // dL/dimg1 = conv(dL*dm_dmu1) + 2*img1*conv(dL*dm_dsigma1_sq) + img2*conv(dL*dm_dsigma12)
 // CONST_DL: dL_dmap is the constant `dl_const` (fused loss) and the L1 sign term is added.
-template <bool CONST_DL>
-__global__ void __launch_bounds__(ST)
-ssim_backward_kernel(int H, int W, const float* __restrict__ img1, const float* __restrict__ img2,
-                     const float* __restrict__ dL_dmap, const float* __restrict__ dm_dmu1,
-                     const float* __restrict__ dm_dsigma1_sq, const float* __restrict__ dm_dsigma12,
-                     float* __restrict__ dL_dimg1, float dl_const, float l1_scale) {
+// EXPO: img1 is the three planes of the rendered image; the result is dL/dout at the exposed image out (see expose()).
+template <bool CONST_DL, bool EXPO>
+__device__ __forceinline__ void
+ssim_backward_tile(int H, int W, const float* __restrict__ img1, const float* __restrict__ img2,
+                   const float* __restrict__ dL_dmap, const float* __restrict__ dm_dmu1,
+                   const float* __restrict__ dm_dsigma1_sq, const float* __restrict__ dm_dsigma12,
+                   float* __restrict__ dL_dimg1, float dl_const, float l1_scale, const float* __restrict__ E) {
     __shared__ float s[3][SH_][SH_ + 1];
     __shared__ float h[3][SH_][SB + 1];
     const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
@@ -220,7 +267,8 @@ ssim_backward_kernel(int H, int W, const float* __restrict__ img1, const float* 
         const int py = y0 + ty * RPT + j;
         if (px < W && py < H) {
             const size_t gi = plane + (size_t)py * W + px;
-            const float p1 = img1[gi], p2 = img2[gi];
+            const float p1 = EXPO ? expose(img1, (size_t)H * W, (size_t)py * W + px, expo_coef(E, blockIdx.z)) : img1[gi];
+            const float p2 = img2[gi];
             float out = c[0][j];
             out += p1 * 2.0f * c[1][j];
             out += p2 * c[2][j];
@@ -231,6 +279,121 @@ ssim_backward_kernel(int H, int W, const float* __restrict__ img1, const float* 
             dL_dimg1[gi] = out;
         }
     }
+}
+
+template <bool CONST_DL>
+__global__ void __launch_bounds__(ST)
+ssim_backward_kernel(int H, int W, const float* __restrict__ img1, const float* __restrict__ img2,
+                     const float* __restrict__ dL_dmap, const float* __restrict__ dm_dmu1,
+                     const float* __restrict__ dm_dsigma1_sq, const float* __restrict__ dm_dsigma12,
+                     float* __restrict__ dL_dimg1, float dl_const, float l1_scale) {
+    ssim_backward_tile<CONST_DL, false>(H, W, img1, img2, dL_dmap, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, dL_dimg1, dl_const, l1_scale,
+                                        nullptr);
+}
+
+// backward of the exposed loss: dL/dout (3 planes) into dL_dout
+__global__ void __launch_bounds__(ST)
+ssim_loss_exposure_backward_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
+                                   const float* __restrict__ E, const float* __restrict__ dm_dmu1,
+                                   const float* __restrict__ dm_dsigma1_sq, const float* __restrict__ dm_dsigma12,
+                                   float* __restrict__ dL_dout, float dl_const, float l1_scale) {
+    ssim_backward_tile<true, true>(H, W, img, gt, nullptr, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, dL_dout, dl_const, l1_scale, E);
+}
+
+constexpr int XT = 256;             // threads of the exposure mix kernel
+
+// CTAs of the exposure mix kernel: a function of the frame size alone, so the partial sums (and their fixed-order total)
+// are the same on every call and every replica
+inline unsigned expo_blocks(size_t HW) { return (unsigned)std::min<size_t>((HW + XT - 1) / XT, (size_t)NUM_SMS * 4); }
+
+// In place, per pixel: dL/dimg_k = sum_c E[k][c] * dL/dout_c.  Also the CTA's partial sums (float64, fixed order) of
+//   dL/dE[k][c] = sum_px img_k * dL/dout_c (k < 3),   dL/dE[c][3] = sum_px dL/dout_c,
+// stored at partials[12 * blockIdx.x + (4k + c)] (the layout of E).
+__global__ void __launch_bounds__(XT)
+exposure_mix_kernel(size_t HW, const float* __restrict__ img, const float* __restrict__ E, float* __restrict__ dL,
+                    double* __restrict__ partials) {
+    __shared__ double red[XT / 32][12];
+    float e[12];
+#pragma unroll
+    for (int j = 0; j < 12; ++j) e[j] = E[j];
+    double acc[12];
+#pragma unroll
+    for (int j = 0; j < 12; ++j) acc[j] = 0.0;
+    for (size_t i = (size_t)blockIdx.x * XT + threadIdx.x; i < HW; i += (size_t)gridDim.x * XT) {
+        const float x[3] = {img[i], img[HW + i], img[2 * HW + i]};
+        const float d[3] = {dL[i], dL[HW + i], dL[2 * HW + i]};
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            float g = e[4 * k] * d[0];
+            g = fmaf(e[4 * k + 1], d[1], g);
+            dL[k * HW + i] = fmaf(e[4 * k + 2], d[2], g);
+#pragma unroll
+            for (int c = 0; c < 3; ++c) acc[4 * k + c] = fma((double)x[k], (double)d[c], acc[4 * k + c]);
+            acc[4 * k + 3] += (double)d[k];
+        }
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int j = 0; j < 12; ++j) {
+        double v = acc[j];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) red[warp][j] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < 12) {
+        double t = 0.0;
+#pragma unroll
+        for (int w = 0; w < XT / 32; ++w) t += red[w][threadIdx.x];
+        partials[12 * (size_t)blockIdx.x + threadIdx.x] = t;
+    }
+}
+
+// dL/dE[j] = fixed-order float64 sum of the G partials: warp j sums entry j (lane-strided, then a shuffle tree)
+__global__ void __launch_bounds__(384)
+exposure_grad_finish_kernel(unsigned G, const double* __restrict__ partials, float* __restrict__ dL_dE) {
+    const int j = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double s = 0.0;
+    for (unsigned b = lane; b < G; b += 32) s += partials[12 * (size_t)b + j];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) dL_dE[j] = (float)s;
+}
+
+struct ExpoBatch { int kf[EXPO_MAX_SLOTS]; };
+
+// One exposure step per batch (torch::optim::Adam: betas (0.9, 0.999), eps 1e-8, no weight decay, bias correction from
+// the keyframe's own step count).  Thread (slot s, entry j); the first slot that holds a keyframe steps it with
+//   g = (1/S) * sum over the slots holding it (slot order, float64) of the slot's dL/dE.
+// A set overflow word (the batch was skipped on the device) leaves E, m, v and t as they are.
+__global__ void __launch_bounds__(EXPO_MAX_SLOTS * 12)
+exposure_adam_kernel(int S, ExpoBatch batch, const float* __restrict__ slot_grads, float* __restrict__ E, float* __restrict__ m,
+                     float* __restrict__ v, int* __restrict__ t, float lr, const unsigned int* __restrict__ skip) {
+    if (*skip) return;
+    const int s = threadIdx.x / 12, j = threadIdx.x % 12;
+    bool first = s < S;
+    const int kf = first ? batch.kf[s] : 0;
+    for (int q = 0; q < s && first; ++q) first = batch.kf[q] != kf;
+    int step = 0;
+    if (first) step = t[kf] + 1;
+    __syncthreads();                                     // every thread has read its keyframe's old step count
+    if (!first) return;
+    double acc = 0.0;
+    for (int q = s; q < S; ++q)
+        if (batch.kf[q] == kf) acc += (double)slot_grads[12 * q + j];
+    const float g = (float)(acc / (double)S);
+    const float b1 = 0.9f, b2 = 0.999f, eps = 1e-8f;
+    const double bc1 = 1.0 - pow(0.9, (double)step), bc2 = 1.0 - pow(0.999, (double)step);
+    const size_t i = 12 * (size_t)kf + j;
+    // every operation rounded on its own (no contraction), so that a CPU restatement (tests/exposure_oracle.py) can follow it
+    const float m1 = fmaf(1.0f - b1, g, __fmul_rn(b1, m[i]));
+    const float v1 = fmaf(1.0f - b2, __fmul_rn(g, g), __fmul_rn(b2, v[i]));
+    const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v1), (float)sqrt(bc2)), eps);
+    const float step_size = (float)((double)lr / bc1);
+    E[i] = __fadd_rn(E[i], __fmul_rn(-step_size, __fdiv_rn(m1, denom)));
+    m[i] = m1;
+    v[i] = v1;
+    if (j == 0) t[kf] = step;
 }
 
 }  // namespace
@@ -295,18 +458,81 @@ extern "C" int glic_l1_ssim_loss(int CH, int H, int W, float lambda_dssim, const
     return GLIC_OK;
 }
 
+// scratch: the three partial maps (9 HW floats) | the mix kernel's float64 partial sums (12 per CTA)
+static size_t expo_partials_offset(int H, int W) { return ((sizeof(float) * 9 * (size_t)H * W) + 255) & ~size_t(255); }
+
+extern "C" size_t glic_loss_exposure_scratch_bytes(int H, int W) {
+    if (H <= 0 || W <= 0) return 0;
+    return expo_partials_offset(H, W) + sizeof(double) * 12 * (size_t)expo_blocks((size_t)H * W) + 256;
+}
+
+extern "C" int glic_l1_ssim_loss_exposure(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E,
+                                          float* loss_out, float* dL_dimg, float* dL_dE, void* scratch, size_t scratch_bytes,
+                                          void* stream) {
+    if (H <= 0 || W <= 0 || !img || !gt || !E || !loss_out || !scratch) { set_error("l1_ssim_loss_exposure: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if ((dL_dimg == nullptr) != (dL_dE == nullptr)) {
+        set_error("l1_ssim_loss_exposure: dL_dimg and dL_dE must be both NULL (loss only) or both non-NULL"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (scratch_bytes < glic_loss_exposure_scratch_bytes(H, W)) { set_error("l1_ssim_loss_exposure: scratch too small"); return GLIC_ERR_WORKSPACE; }
+    const size_t HW = (size_t)H * W, N = 3 * HW;
+    float* d1 = static_cast<float*>(scratch);
+    float* d2 = d1 + N;
+    float* d3 = d2 + N;
+    double* partials = reinterpret_cast<double*>(static_cast<char*>(scratch) + expo_partials_offset(H, W));
+    const float C1 = 0.01f * 0.01f, C2 = 0.03f * 0.03f;
+    const float inv_n = (float)(1.0 / (double)N);
+    cudaStream_t s = (cudaStream_t)stream;
+    GLIC_CUDA_TRY(cudaMemsetAsync(loss_out, 0, sizeof(float), s));
+    dim3 grid((W + SB - 1) / SB, (H + SB - 1) / SB, 3), block(ST);
+    { StageTimer _t(GLIC_STAGE_LOSS_FWD, s);
+    ssim_loss_exposure_forward_kernel<<<grid, block, 0, s>>>(H, W, C1, C2, img, gt, E, d1, d2, d3, lambda_dssim, inv_n, loss_out); }
+    GLIC_LAUNCH_CHECK();
+    if (dL_dimg) {
+        StageTimer _t(GLIC_STAGE_LOSS_BWD, s);
+        ssim_loss_exposure_backward_kernel<<<grid, block, 0, s>>>(H, W, img, gt, E, d1, d2, d3, dL_dimg, -lambda_dssim * inv_n,
+                                                                  (1.0f - lambda_dssim) * inv_n);
+        GLIC_LAUNCH_CHECK();
+        const unsigned G = expo_blocks(HW);
+        exposure_mix_kernel<<<G, XT, 0, s>>>(HW, img, E, dL_dimg, partials);
+        GLIC_LAUNCH_CHECK();
+        exposure_grad_finish_kernel<<<1, 384, 0, s>>>(G, partials, dL_dE);
+        GLIC_LAUNCH_CHECK();
+    }
+    return GLIC_OK;
+}
+
+namespace glic {
+int launch_exposure_adam(int S, const int* kf_of_slot, const float* slot_grads, float* E, float* m, float* v, int* t, float lr,
+                         const unsigned int* skip_flag, cudaStream_t s) {
+    if (S < 1 || S > EXPO_MAX_SLOTS) { set_error("exposure_adam: bad batch size"); return GLIC_ERR_INVALID_ARGUMENT; }
+    ExpoBatch b{};
+    for (int q = 0; q < S; ++q) b.kf[q] = kf_of_slot[q];
+    StageTimer _t(GLIC_STAGE_ADAM, s);
+    exposure_adam_kernel<<<1, EXPO_MAX_SLOTS * 12, 0, s>>>(S, b, slot_grads, E, m, v, t, lr, skip_flag);
+    GLIC_LAUNCH_CHECK();
+    return GLIC_OK;
+}
+}  // namespace glic
+
 
 // ---- evaluation metrics (evaluateVisualQuality, gaussian.cpp:756-760,795-799; loss_utils.h:35-39,84-127) --------------
 namespace glic {
 namespace {
 
-// clamp both images to [0,1] (gaussian.cpp:756-757) into scratch copies and accumulate the squared error
+// clamp both images to [0,1] (gaussian.cpp:756-757) into scratch copies and accumulate the squared error.
+// E (optional, 3 channels): the image is exposed first (see expose()); HW = pixels per plane.
 __global__ void __launch_bounds__(256)
 eval_clamp_mse_kernel(size_t N, const float* __restrict__ img, const float* __restrict__ gt, float* __restrict__ a,
-                      float* __restrict__ b, double* __restrict__ acc2) {
+                      float* __restrict__ b, double* __restrict__ acc2, const float* __restrict__ E, size_t HW) {
     double se = 0.0;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += (size_t)gridDim.x * blockDim.x) {
-        const float x = fminf(fmaxf(img[i], 0.f), 1.f), y = fminf(fmaxf(gt[i], 0.f), 1.f);
+        float x = img[i];
+        if (E) {
+            const int c = (int)(i / HW);
+            x = expose(img, HW, i - (size_t)c * HW, expo_coef(E, c));
+        }
+        x = fminf(fmaxf(x, 0.f), 1.f);
+        const float y = fminf(fmaxf(gt[i], 0.f), 1.f);
         a[i] = x; b[i] = y;
         const float d = x - y;
         se += (double)(d * d);
@@ -336,9 +562,10 @@ __global__ void eval_finish_kernel(size_t N, const double* __restrict__ acc2, fl
 
 extern "C" size_t glic_eval_scratch_bytes(int CH, int H, int W) { return sizeof(float) * 3 * (size_t)CH * H * W + 256; }
 
-extern "C" int glic_eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, float* out2, void* scratch,
-                                   size_t scratch_bytes, void* stream) {
-    if (CH <= 0 || H <= 0 || W <= 0 || !img || !gt || !out2 || !scratch) { set_error("eval_psnr_ssim: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
+namespace glic {
+int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, const float* E, float* out2, void* scratch,
+                   size_t scratch_bytes, void* stream) {
+    if (CH <= 0 || H <= 0 || W <= 0 || !img || !gt || !out2 || !scratch || (E && CH != 3)) { set_error("eval_psnr_ssim: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (scratch_bytes < glic_eval_scratch_bytes(CH, H, W)) { set_error("eval_psnr_ssim: scratch too small"); return GLIC_ERR_WORKSPACE; }
     const size_t N = (size_t)CH * H * W;
     cudaStream_t s = (cudaStream_t)stream;
@@ -348,7 +575,7 @@ extern "C" int glic_eval_psnr_ssim(int CH, int H, int W, const float* img, const
     float* map = b + N;
     GLIC_CUDA_TRY(cudaMemsetAsync(acc2, 0, 2 * sizeof(double), s));
     const unsigned blocks = (unsigned)std::min<size_t>((N + 255) / 256, (size_t)NUM_SMS * 8);
-    eval_clamp_mse_kernel<<<blocks, 256, 0, s>>>(N, img, gt, a, b, acc2);
+    eval_clamp_mse_kernel<<<blocks, 256, 0, s>>>(N, img, gt, a, b, acc2, E, (size_t)H * W);
     GLIC_LAUNCH_CHECK();
     if (int e = glic_fused_ssim(1, CH, H, W, 0.01f * 0.01f, 0.03f * 0.03f, a, b, map, nullptr, nullptr, nullptr, stream)) return e;
     eval_sum_kernel<<<blocks, 256, 0, s>>>(N, map, acc2);
@@ -356,4 +583,10 @@ extern "C" int glic_eval_psnr_ssim(int CH, int H, int W, const float* img, const
     eval_finish_kernel<<<1, 1, 0, s>>>(N, acc2, out2);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
+}
+}  // namespace glic
+
+extern "C" int glic_eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, float* out2, void* scratch,
+                                   size_t scratch_bytes, void* stream) {
+    return eval_psnr_ssim(CH, H, W, img, gt, nullptr, out2, scratch, scratch_bytes, stream);
 }

@@ -119,6 +119,27 @@ class Mapper:
     def set_binning_pairs(self, pairs):
         capi.check(capi.lib.glic_mapper_set_option(self._h, 2, int(pairs)), "mapper_set_option")
 
+    def enable_exposure(self, exposure_lr=0.001):
+        """Train a 3x4 affine exposure per training keyframe from now on (config/fastlivo.yaml:25-26: exposure_lr 0.001)."""
+        capi.check(capi.lib.glic_mapper_enable_exposure(self._h, float(exposure_lr)), "mapper_enable_exposure")
+
+    def exposure(self, index):
+        """E of training keyframe `index` as a [3,4] float32 array (out_c = E[0][c] r + E[1][c] g + E[2][c] b + E[c][3])."""
+        out = (C.c_float * 12)()
+        capi.check(capi.lib.glic_mapper_exposure_get(self._h, int(index), out), "mapper_exposure_get")
+        return np.array(out[:], np.float32).reshape(3, 4)
+
+    def set_exposure(self, index, E):
+        """Overwrite E of training keyframe `index`; its Adam state is kept."""
+        e = np.asarray(E, np.float32).reshape(12)
+        capi.check(capi.lib.glic_mapper_exposure_set(self._h, int(index), (C.c_float * 12)(*[float(x) for x in e])), "mapper_exposure_set")
+
+    def exposure_state(self, index):
+        """(E [3,4], exp_avg [3,4], exp_avg_sq [3,4], step count) of training keyframe `index`"""
+        m1, m2, t = (C.c_float * 12)(), (C.c_float * 12)(), C.c_int()
+        capi.check(capi.lib.glic_mapper_exposure_adam_state(self._h, int(index), m1, m2, C.byref(t)), "mapper_exposure_adam_state")
+        return self.exposure(index), np.array(m1[:], np.float32).reshape(3, 4), np.array(m2[:], np.float32).reshape(3, 4), int(t.value)
+
     def synchronize(self):
         capi.check(capi.lib.glic_mapper_synchronize(self._h), "mapper_synchronize")
 

@@ -145,6 +145,25 @@ def fused_ssim(img1, img2):
     return FusedSSIMMap.apply(SSIM_C1, SSIM_C2, img1, img2).mean()
 
 
+def l1_ssim_loss_exposure(img, gt, E, lambda_dssim=0.2, grad=True, scratch=None, stream=None):
+    """The photometric loss on the exposed image out_c = E[0][c] r + E[1][c] g + E[2][c] b + E[c][3] (glic_l1_ssim_loss_exposure).
+    img, gt: [3,H,W] float32 CUDA tensors; E: [3,4] (or 12) float32 CUDA tensor.  Returns (loss[1], dL_dimg[3,H,W], dL_dE[3,4]);
+    the two gradients are None when grad is False.  dL_dE is deterministic (fixed-order float64 sums)."""
+    _, H, W = img.shape
+    assert img.shape[0] == 3 and gt.shape == img.shape and E.numel() == 12
+    need = capi.lib.glic_loss_exposure_scratch_bytes(H, W)
+    if scratch is None or scratch.numel() < need:
+        scratch = torch.empty(need, dtype=torch.uint8, device=img.device)
+    f32 = dict(dtype=torch.float32, device=img.device)
+    loss = torch.empty(1, **f32)
+    dL_dimg = torch.empty(3, H, W, **f32) if grad else None
+    dL_dE = torch.empty(3, 4, **f32) if grad else None
+    capi.check(capi.lib.glic_l1_ssim_loss_exposure(H, W, lambda_dssim, capi.ptr(img), capi.ptr(gt), capi.ptr(E.contiguous()),
+                                                   capi.ptr(loss), capi.ptr(dL_dimg), capi.ptr(dL_dE), capi.ptr(scratch),
+                                                   scratch.numel(), stream), "l1_ssim_loss_exposure")
+    return loss, dL_dimg, dL_dE
+
+
 # ---- render() and the model getters it uses (rasterizer/renderer.cpp:21-88; gaussian.cpp:147-175) ------------------
 class GaussianParams:
     """The six raw parameter tensors of GaussianModel with its activation getters (sigmoid / exp / normalize)."""

@@ -238,6 +238,22 @@ GLIC_API size_t glic_loss_scratch_bytes(int CH, int H, int W);
 GLIC_API int glic_l1_ssim_loss(int CH, int H, int W, float lambda_dssim, const float* img, const float* gt,
                       float* loss_out, float* dL_dimg, void* scratch, size_t scratch_bytes, void* stream);
 
+/* The same loss on an exposed image (Inria 3DGS's trained exposure; no counterpart in the reference, whose render()
+ * ignores use_trained_exposure).  E_dev: 12 device floats, a 3x4 row-major matrix; the loss and its gradients are those
+ * of out[3,H,W],
+ *     out_c = E[0][c]*r + E[1][c]*g + E[2][c]*b + E[c][3]          (matmul(img_hwc, E[:3,:3]) + E[:3,3])
+ * evaluated as acc = E[c][3], then fmaf with r, g, b in that order: E = [I | 0] gives out == img exactly for the
+ * non-negative finite images the renderer produces.  out is formed inside the loss kernels and never written.
+ *   dL_dimg[3,H,W] = sum_c E[k][c] * dL/dout_c;  dL_dE_dev[12]: dL/dE[k][c] = sum_px img_k * dL/dout_c (k < 3) and
+ *   dL/dE[c][3] = sum_px dL/dout_c, summed in float64 in a fixed order (per-CTA partials, then one fixed-order total, no
+ *   atomics): two identical calls give identical bits.  dL_dimg and dL_dE_dev are both NULL (loss only) or both set.
+ *   img: 3 channels; scratch: glic_loss_exposure_scratch_bytes(H, W).  Profiled as GLIC_STAGE_LOSS_FWD / GLIC_STAGE_LOSS_BWD
+ *   (the dL/dE kernels are part of the latter); the mapper's exposure step is timed under GLIC_STAGE_ADAM. */
+GLIC_API size_t glic_loss_exposure_scratch_bytes(int H, int W);
+GLIC_API int glic_l1_ssim_loss_exposure(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E_dev,
+                                        float* loss_out, float* dL_dimg, float* dL_dE_dev, void* scratch, size_t scratch_bytes,
+                                        void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * simple-knn.  Replaces SimpleKNN::knn (simple-knn/simple_knn.cu:185-221): mean of the three
  * smallest squared distances to other points.  points[P,3] -> mean_dists[P].
@@ -404,6 +420,27 @@ GLIC_API int glic_mapper_synchronize(glic_mapper* m);
  * (the copy uses cudaMemcpyDefault): that is how "inputs resident in HBM" is measured. */
 enum { GLIC_MAPPER_OPT_OPTIMIZER = 1, GLIC_MAPPER_OPT_BINNING_PAIRS = 2 /* (tile, Gaussian) pairs the binning workspace holds; grows by itself on overflow */ };
 GLIC_API int glic_mapper_set_option(glic_mapper* m, int option, int value);
+/* Per-keyframe exposure (the reference's apply_exposure / exposure_lr, config/fastlivo.yaml:25-26, which its render()
+ * never applies).  Off by default.  glic_mapper_enable_exposure(m, lr) may be called before or between optimize() calls:
+ * from then on every training keyframe k has a 3x4 affine colour transform E_k (row-major, see glic_l1_ssim_loss_exposure),
+ * starting at [I | 0] (keyframes added later start there too).  Each iteration's loss is taken on E_k applied to the
+ * rendered image of every view of keyframe k; after the Gaussian step one launch steps the batch's keyframes with
+ * torch::optim::Adam's rule (betas 0.9 / 0.999, eps 1e-8, no weight decay, lr = exposure_lr, bias correction from the
+ * keyframe's own step count t, which rises by one per batch that holds the keyframe):
+ *     g = (1/S) * sum over the batch slots holding k of dL/dE,  m = b1 m + (1-b1) g,  v = b2 v + (1-b2) g^2,
+ *     E -= (lr / (1 - b1^t)) * m / (sqrt(v) / sqrt(1 - b2^t) + eps).
+ * An iteration skipped for a binning overflow leaves E, m, v and t unchanged; GLIC_MAPPER_OPT_OPTIMIZER = 0 leaves the
+ * exposure step out too.  With world > 1 every rank pushes its slots' 12-float dL/dE to its peers and every replica
+ * applies the same step: E, m, v and t stay bit-identical across ranks (call enable / set identically on every rank).
+ * glic_mapper_evaluate(is_train = 1) applies the keyframe's E before the [0,1] clamp; held-out keyframes (is_train = 0)
+ * are evaluated with the identity, since no exposure was ever fitted for them; extend() renders alpha only and is not
+ * affected.  exposure_get / exposure_set read and write E of training keyframe `index` (host arrays of 12 floats; they
+ * synchronise and need exposure enabled); set leaves that keyframe's Adam state (m, v, t) alone. */
+GLIC_API int glic_mapper_enable_exposure(glic_mapper* m, float exposure_lr);
+GLIC_API int glic_mapper_exposure_get(glic_mapper* m, int index, float* out12);
+GLIC_API int glic_mapper_exposure_set(glic_mapper* m, int index, const float* in12);
+/* the exposure's Adam state of training keyframe `index`: both moments (12 floats each) and the step count; synchronises */
+GLIC_API int glic_mapper_exposure_adam_state(glic_mapper* m, int index, float* exp_avg12, float* exp_avg_sq12, int* step);
 /* Camera (camera.h:38-110) in closed form, as the mapper derives it from a keyframe pose: out41 = view[16] (column-major
  * Rt) | proj[16] (column-major P*Rt) | campos[3] | tan_fovx, tan_fovy | limx_neg, limx_pos, limy_neg, limy_pos. */
 GLIC_API int glic_camera_block(int width, int height, float fx, float fy, float cx, float cy, const float* R_wc /*[9] row-major*/,
