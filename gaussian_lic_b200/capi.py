@@ -125,6 +125,10 @@ def _load():
         "glic_mapper_exposure_get": (i32, [vp, i32, C.POINTER(f32)]),
         "glic_mapper_exposure_set": (i32, [vp, i32, C.POINTER(f32)]),
         "glic_mapper_exposure_adam_state": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32), C.POINTER(i32)]),
+        "glic_mapper_enable_pose_refinement": (i32, [vp, f32, f32]),
+        "glic_mapper_pose_get": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32), C.POINTER(f32)]),
+        "glic_mapper_pose_set": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32)]),
+        "glic_mapper_pose_adam_state": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32), C.POINTER(i32)]),
         "glic_debug_geom": (i32, [i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "glic_debug_binning": (i32, [i32, vp, i64, i64, vp, vp, vp, vp]),
         "glic_debug_image": (i32, [i32, i32, vp, vp, vp, vp, vp, C.POINTER(i64), vp]),

@@ -258,7 +258,12 @@ struct CompactGrads {
     const float* dL_dopacity; // [P]   dL/d(activated opacity) from the render backward
     const float4* rot_raw;    // [P]   raw (un-normalised) rotation
     int accumulate;           // 0: overwrite the geometric gradients, 1: add to them (second and later views of a rank)
+    // camera-pose gradient of the view (preprocess_backward.cu, POSE); both NULL: not computed
+    double* pose_partials;    // [ceil(P/128)][6] per-CTA float64 partial sums (pose_partials_count(capacity) doubles)
+    float* pose_grad;         // [6] dL/d(rho, omega) of the view, written by the finish kernel
 };
+// doubles of the pose-gradient scratch for up to Pcap Gaussians
+size_t pose_partials_count(uint32_t Pcap);
 
 // ---- stage launchers (defined in the .cu files) ------------------------------------------
 int launch_preprocess_forward(int P, int D, int M, const float* means, const float* scales, float mod,
@@ -309,7 +314,9 @@ namespace glic {
 int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, float* exp_avg, float* exp_avg_sq, const float* g_geo,
                         uint32_t Pcap_geo, const float* lr6, const float* g_color, const uint8_t* flags, const float* campos4,
                         int n_slots, float grad_scale, float color_scale, float b1, float b2, float eps, const unsigned int* skip_flag,
-                        unsigned int* visible_count, cudaStream_t s);
+                        unsigned int* visible_count, cudaStream_t s, const float* const* campos_dev = nullptr);
+// campos_dev (optional, n_slots host-held device pointers): each slot's camera centre is read on the device from there
+// (campos4 is then unused)
 int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flags, cudaStream_t s);
 // per-keyframe exposure (ssim.cu): one Adam step of every keyframe of a batch of S <= EXPO_MAX_SLOTS slots; slot_grads[S][12]
 constexpr int EXPO_MAX_SLOTS = 32;

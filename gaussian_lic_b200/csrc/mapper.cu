@@ -34,8 +34,25 @@ struct CamBlock {                    // what the rasterizer gets per view (camer
     float tanfovx, tanfovy, lim[4];
 };
 
+// the pose-independent projection P of camera.h (row-major), with the FoV from the intrinsics (float members)
+void proj_matrix(int W, int H, double fx, double fy, double cx, double cy, float* Pm, float* fov2) {
+    const float fovx = (float)(2.0 * std::atan(W / (2.0 * fx))), fovy = (float)(2.0 * std::atan(H / (2.0 * fy)));
+    const float znear = 0.01f, zfar = 100.0f;
+    for (int i = 0; i < 16; ++i) Pm[i] = 0.0f;
+    Pm[0] = (float)(1.0 / std::tan((double)fovx / 2));
+    Pm[5] = (float)(1.0 / std::tan((double)fovy / 2));
+    Pm[2] = (2.0f * (float)cx - (float)W) / (float)W;
+    Pm[6] = (2.0f * (float)cy - (float)H) / (float)H;
+    Pm[14] = 1.0f;
+    Pm[10] = zfar / (zfar - znear);
+    Pm[11] = -(zfar * znear) / (zfar - znear);
+    fov2[0] = fovx; fov2[1] = fovy;
+}
+
 // camera.h:38-110 in closed form: FoV from the intrinsics (float members), world->view matrix Rt, projection P, both handed
 // to the kernels transposed (column-major), camera centre = -R_cw^T t_cw, the asymmetric clamp limits of :63-66.
+// Compiled for x86-64 without FMA, every operation below is one IEEE double / float operation: pose_step_kernel repeats the
+// pose-dependent part on the device bit for bit (cam_rebuild), so keep the two in step.
 void camera_block(int W, int H, double fx, double fy, double cx, double cy, const float* R_wc, const float* t_wc, CamBlock& o) {
     double Rcw[9], tcw[3];
     for (int i = 0; i < 3; ++i)
@@ -44,16 +61,9 @@ void camera_block(int W, int H, double fx, double fy, double cx, double cy, cons
     float Rt[16] = {0};
     for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) Rt[4 * i + j] = (float)Rcw[3 * i + j]; Rt[4 * i + 3] = (float)tcw[i]; }
     Rt[15] = 1.0f;
-    const float fovx = (float)(2.0 * std::atan(W / (2.0 * fx))), fovy = (float)(2.0 * std::atan(H / (2.0 * fy)));
-    const float znear = 0.01f, zfar = 100.0f;
-    float Pm[16] = {0};
-    Pm[0] = (float)(1.0 / std::tan((double)fovx / 2));
-    Pm[5] = (float)(1.0 / std::tan((double)fovy / 2));
-    Pm[2] = (2.0f * (float)cx - (float)W) / (float)W;
-    Pm[6] = (2.0f * (float)cy - (float)H) / (float)H;
-    Pm[14] = 1.0f;
-    Pm[10] = zfar / (zfar - znear);
-    Pm[11] = -(zfar * znear) / (zfar - znear);
+    float Pm[16], fov2[2];
+    proj_matrix(W, H, fx, fy, cx, cy, Pm, fov2);
+    const float fovx = fov2[0], fovy = fov2[1];
     float full[16];
     for (int i = 0; i < 4; ++i)
         for (int j = 0; j < 4; ++j) {
@@ -82,6 +92,128 @@ struct Keyframe {
 
 inline uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
 
+// ---- pose refinement (glic_mapper_enable_pose_refinement) ---------------------------------------------------------------
+// Keyframe k's pose is T_cw = [R_cw | t_cw] (float64 master, R_cw row-major), perturbed as Exp(delta) T_cw with
+// delta = (rho, omega) in the camera frame.  Each step: torch::optim::Adam on the 6-vector (as the exposure step), then
+// T_cw <- Exp(u) T_cw, the float pose (R_wc = R_cw^T, t_wc = -R_cw^T t_cw) re-derived from it, and the device camera block
+// (view16 | proj16 | campos4) rebuilt from those floats exactly as camera_block() does.
+
+// SE(3) exponential of u = (rho, omega): R = I + A K + B K^2, V = I + B K + C K^2, K = [omega]_x; t = V rho
+__device__ void se3_exp(const double u[6], double R[9], double t[3]) {
+    const double wx = u[3], wy = u[4], wz = u[5];
+    const double th2 = wx * wx + wy * wy + wz * wz;
+    double A, B, C;
+    if (th2 < 1e-4) {                     // theta < 1e-2: Taylor series to theta^6 (the next terms are below 1e-21)
+        A = 1.0 - th2 / 6.0 * (1.0 - th2 / 20.0 * (1.0 - th2 / 42.0));
+        B = 0.5 * (1.0 - th2 / 12.0 * (1.0 - th2 / 30.0 * (1.0 - th2 / 56.0)));
+        C = (1.0 / 6.0) * (1.0 - th2 / 20.0 * (1.0 - th2 / 42.0 * (1.0 - th2 / 72.0)));
+    } else {
+        const double th = sqrt(th2), s = sin(th), sh = sin(0.5 * th);
+        A = s / th;
+        B = 2.0 * sh * sh / th2;
+        C = (th - s) / (th2 * th);
+    }
+    const double K[9] = {0.0, -wz, wy, wz, 0.0, -wx, -wy, wx, 0.0};
+    double K2[9];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) K2[3 * i + j] = K[3 * i] * K[j] + K[3 * i + 1] * K[3 + j] + K[3 * i + 2] * K[6 + j];
+    double V[9];
+    for (int e = 0; e < 9; ++e) {
+        const double I = (e % 4 == 0) ? 1.0 : 0.0;
+        R[e] = I + A * K[e] + B * K2[e];
+        V[e] = I + B * K[e] + C * K2[e];
+    }
+    for (int i = 0; i < 3; ++i) t[i] = V[3 * i] * u[0] + V[3 * i + 1] * u[1] + V[3 * i + 2] * u[2];
+}
+
+// camera_block()'s pose-dependent part, operation for operation (no contraction): view16 | proj16 | campos4 from the float pose
+__device__ void cam_rebuild(const float* R_wc, const float* t_wc, const float* Pm, float* out36) {
+    double Rcw[9], tcw[3];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) Rcw[3 * i + j] = (double)R_wc[3 * j + i];
+    for (int i = 0; i < 3; ++i)
+        tcw[i] = -__dadd_rn(__dadd_rn(__dmul_rn(Rcw[3 * i], (double)t_wc[0]), __dmul_rn(Rcw[3 * i + 1], (double)t_wc[1])),
+                            __dmul_rn(Rcw[3 * i + 2], (double)t_wc[2]));
+    float Rt[16];
+    for (int e = 0; e < 16; ++e) Rt[e] = 0.0f;
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) Rt[4 * i + j] = __double2float_rn(Rcw[3 * i + j]);
+        Rt[4 * i + 3] = __double2float_rn(tcw[i]);
+    }
+    Rt[15] = 1.0f;
+    for (int i = 0; i < 4; ++i)
+        for (int j = 0; j < 4; ++j) {
+            float acc = 0.f;
+            for (int k = 0; k < 4; ++k) acc = __fadd_rn(acc, __fmul_rn(Pm[4 * i + k], Rt[4 * k + j]));
+            out36[16 + 4 * j + i] = acc;                                   // proj, column-major
+        }
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) out36[4 * c + r] = Rt[4 * r + c];      // view, column-major
+    for (int i = 0; i < 3; ++i)
+        out36[32 + i] = __double2float_rn(-__dadd_rn(__dadd_rn(__dmul_rn(Rcw[i], tcw[0]), __dmul_rn(Rcw[3 + i], tcw[1])),
+                                                     __dmul_rn(Rcw[6 + i], tcw[2])));
+    out36[35] = 0.f;
+}
+
+struct PoseBatch {
+    int kf[MAX_SLOTS];                // keyframe of each slot
+    float* cam[MAX_SLOTS];            // its device camera block
+    float Pm[16];                     // the pose-independent projection (row-major)
+};
+
+// One thread per slot; the first slot that holds a keyframe steps it with g = (1/S) * sum over the slots holding it (slot
+// order, float64) of the slot's dL/d(rho, omega), by exposure_adam_kernel's arithmetic.  A set overflow word leaves the pose,
+// m, v and t unchanged; an update of exactly zero leaves the pose and its camera block unchanged.
+__global__ void __launch_bounds__(MAX_SLOTS)
+pose_step_kernel(int S, PoseBatch b, const float* __restrict__ slot_grads /* [S][8] */, double* __restrict__ T /* [kf][12] */,
+                 float* __restrict__ pose_f /* [kf][12] */, float* __restrict__ m, float* __restrict__ v, int* __restrict__ t,
+                 float lr_rho, float lr_omega, const unsigned int* __restrict__ skip) {
+    if (*skip) return;
+    const int s = threadIdx.x;
+    if (s >= S) return;
+    const int kf = b.kf[s];
+    for (int q = 0; q < s; ++q) if (b.kf[q] == kf) return;
+    const int step = t[kf] + 1;
+    const float b1 = 0.9f, b2 = 0.999f, eps = 1e-8f;
+    const double bc1 = 1.0 - pow(0.9, (double)step), bc2 = 1.0 - pow(0.999, (double)step);
+    double u[6];
+    bool moved = false;
+    for (int j = 0; j < 6; ++j) {
+        double acc = 0.0;
+        for (int q = s; q < S; ++q)
+            if (b.kf[q] == kf) acc += (double)slot_grads[8 * q + j];
+        const float g = (float)(acc / (double)S);
+        const size_t i = 6 * (size_t)kf + j;
+        const float m1 = fmaf(1.0f - b1, g, __fmul_rn(b1, m[i]));
+        const float v1 = fmaf(1.0f - b2, __fmul_rn(g, g), __fmul_rn(b2, v[i]));
+        const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v1), (float)sqrt(bc2)), eps);
+        const float step_size = (float)((double)(j < 3 ? lr_rho : lr_omega) / bc1);
+        const float uj = __fmul_rn(-step_size, __fdiv_rn(m1, denom));
+        m[i] = m1;
+        v[i] = v1;
+        u[j] = (double)uj;
+        moved |= uj != 0.0f;
+    }
+    t[kf] = step;
+    if (!moved) return;
+    double R[9], tu[3];
+    se3_exp(u, R, tu);
+    double* Tk = T + 12 * (size_t)kf;
+    double Rn[9], tn[3];
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) Rn[3 * i + j] = R[3 * i] * Tk[j] + R[3 * i + 1] * Tk[3 + j] + R[3 * i + 2] * Tk[6 + j];
+        tn[i] = R[3 * i] * Tk[9] + R[3 * i + 1] * Tk[10] + R[3 * i + 2] * Tk[11] + tu[i];
+    }
+    for (int e = 0; e < 9; ++e) Tk[e] = Rn[e];
+    for (int i = 0; i < 3; ++i) Tk[9 + i] = tn[i];
+    float* f = pose_f + 12 * (size_t)kf;
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) f[3 * i + j] = (float)Rn[3 * j + i];
+        f[9 + i] = (float)(-(Rn[i] * tn[0] + Rn[3 + i] * tn[1] + Rn[6 + i] * tn[2]));
+    }
+    cam_rebuild(f, f + 9, b.Pm, b.cam[s]);
+}
+
 }  // namespace
 
 struct glic_mapper {
@@ -96,8 +228,8 @@ struct glic_mapper {
     float *g_mean2D = nullptr, *g_conic = nullptr, *g_opacity = nullptr;
     void* geom_ws = nullptr; size_t geom_bytes = 0;
     // ---- exchange block: geo[11*Pcap + 4] | flags words | colour slots [2][S][Pcap][3] | flag bytes [2][S][Pcap] |
-    //      exposure gradient slots [2][S][12] ----
-    char* xblock = nullptr; size_t xbytes = 0, off_col = 0, off_flags = 0, off_expo = 0;
+    //      exposure gradient slots [2][S][12] | pose gradient slots [2][S][8] (dL/d(rho, omega), 2 unused) ----
+    char* xblock = nullptr; size_t xbytes = 0, off_col = 0, off_flags = 0, off_expo = 0, off_pose = 0;
     size_t n_geo = 0;                // floats in the reduced region (11*Pcap + 4; the tail holds the collective overflow word)
     void* peers[8] = {nullptr};
     bool connected = false;
@@ -124,6 +256,16 @@ struct glic_mapper {
     float *expo_E = nullptr, *expo_m = nullptr, *expo_v = nullptr;
     int* expo_t = nullptr;
     size_t expo_cap = 0;
+    // ---- per-training-keyframe pose refinement (glic_mapper_enable_pose_refinement): float64 T_cw [pose_cap][12]
+    //      (R_cw row-major | t_cw), the float pose [pose_cap][12] (R_wc | t_wc), Adam moments [pose_cap][6], step counts ----
+    bool pose_on = false;
+    float pose_lr_rho = 0.f, pose_lr_omega = 0.f;
+    double* pose_T = nullptr;
+    float *pose_f = nullptr, *pose_m = nullptr, *pose_v = nullptr;
+    int* pose_t = nullptr;
+    size_t pose_cap = 0;
+    double* pose_part = nullptr;          // per-CTA partials of the pose-gradient reduction (pose_partials_count(Pcap))
+    cudaEvent_t ev_pose{};
 };
 
 namespace {
@@ -163,7 +305,11 @@ size_t xblock_layout(glic_mapper* m, uint32_t cap) {
     m->off_col = flag_off + 256;
     m->off_flags = m->off_col + (((size_t)2 * m->S * cap * 3 * sizeof(float) + 255) & ~size_t(255));
     m->off_expo = m->off_flags + (((size_t)2 * m->S * cap + 255) & ~size_t(255));
-    return m->off_expo + (((size_t)2 * m->S * 12 * sizeof(float) + 255) & ~size_t(255));
+    m->off_pose = m->off_expo + (((size_t)2 * m->S * 12 * sizeof(float) + 255) & ~size_t(255));
+    return m->off_pose + (((size_t)2 * m->S * 8 * sizeof(float) + 255) & ~size_t(255));
+}
+float* pose_slot(const glic_mapper* m, int parity, int slot) {
+    return reinterpret_cast<float*>(m->xblock + m->off_pose) + ((size_t)parity * m->S + slot) * 8;
 }
 
 // (re)allocates everything whose size depends on the Gaussian capacity; copies the live rows of the arenas
@@ -181,8 +327,9 @@ int set_capacity(glic_mapper* m, uint32_t cap) {
         MAP_TRY(glic_arena_regrow(m->m2, m->Pcap, n2, cap, (uint32_t)m->M, m->P, m->stream));
         GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     }
-    void* old[] = {m->params, m->m1, m->m2, m->act_opacity, m->act_scales, m->act_rots, m->radii, m->g_conic, m->geom_ws, m->xblock};
+    void* old[] = {m->params, m->m1, m->m2, m->act_opacity, m->act_scales, m->act_rots, m->radii, m->g_conic, m->geom_ws, m->xblock, m->pose_part};
     for (void* p : old) if (p) cudaFree(p);
+    MAP_TRY(dev_alloc((void**)&m->pose_part, pose_partials_count(cap) * sizeof(double), false));
     m->params = np; m->m1 = n1; m->m2 = n2;
     MAP_TRY(dev_alloc((void**)&m->act_opacity, (size_t)cap * 4)); MAP_TRY(dev_alloc((void**)&m->act_scales, (size_t)cap * 12));
     MAP_TRY(dev_alloc((void**)&m->act_rots, (size_t)cap * 16)); MAP_TRY(dev_alloc((void**)&m->radii, (size_t)cap * 4));
@@ -234,6 +381,77 @@ int expo_reset(glic_mapper* m, size_t first, size_t last) {
     GLIC_CUDA_TRY(cudaMemsetAsync(m->expo_v + 12 * first, 0, id.size() * sizeof(float), m->stream));
     GLIC_CUDA_TRY(cudaMemsetAsync(m->expo_t + first, 0, (last - first) * sizeof(int), m->stream));
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    return GLIC_OK;
+}
+
+// room for the pose state of n training keyframes (keeps the existing rows)
+int pose_reserve(glic_mapper* m, size_t n) {
+    if (n <= m->pose_cap) return GLIC_OK;
+    const size_t cap = std::max<size_t>({n, 2 * m->pose_cap, 64});
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    double* T = nullptr;
+    float *f = nullptr, *m1 = nullptr, *v = nullptr;
+    int* t = nullptr;
+    MAP_TRY(dev_alloc((void**)&T, cap * 12 * sizeof(double))); MAP_TRY(dev_alloc((void**)&f, cap * 12 * sizeof(float)));
+    MAP_TRY(dev_alloc((void**)&m1, cap * 6 * sizeof(float))); MAP_TRY(dev_alloc((void**)&v, cap * 6 * sizeof(float)));
+    MAP_TRY(dev_alloc((void**)&t, cap * sizeof(int)));
+    if (m->pose_cap) {
+        GLIC_CUDA_TRY(cudaMemcpyAsync(T, m->pose_T, m->pose_cap * 12 * sizeof(double), cudaMemcpyDeviceToDevice, m->stream));
+        GLIC_CUDA_TRY(cudaMemcpyAsync(f, m->pose_f, m->pose_cap * 12 * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+        GLIC_CUDA_TRY(cudaMemcpyAsync(m1, m->pose_m, m->pose_cap * 6 * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+        GLIC_CUDA_TRY(cudaMemcpyAsync(v, m->pose_v, m->pose_cap * 6 * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+        GLIC_CUDA_TRY(cudaMemcpyAsync(t, m->pose_t, m->pose_cap * sizeof(int), cudaMemcpyDeviceToDevice, m->stream));
+        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    }
+    void* old[] = {m->pose_T, m->pose_f, m->pose_m, m->pose_v, m->pose_t};
+    for (void* p : old) if (p) cudaFree(p);
+    m->pose_T = T; m->pose_f = f; m->pose_m = m1; m->pose_v = v; m->pose_t = t;
+    m->pose_cap = cap;
+    return GLIC_OK;
+}
+
+// float64 T_cw of a float pose, exactly as camera_block() forms R_cw and t_cw
+void pose_master(const float* R_wc, const float* t_wc, double* T12) {
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) T12[3 * i + j] = (double)R_wc[3 * j + i];
+    for (int i = 0; i < 3; ++i) T12[9 + i] = -(T12[3 * i] * t_wc[0] + T12[3 * i + 1] * t_wc[1] + T12[3 * i + 2] * t_wc[2]);
+}
+
+// writes keyframe k's float pose (host copy, master pose, device float pose, camera block); `reset` also zeroes its Adam
+// state.  Drains the mapper's stream (see expo_reset).
+int pose_write(glic_mapper* m, size_t k, const float* R_wc, const float* t_wc, bool reset) {
+    Keyframe& kf = m->train[k];
+    float R[9], t[3];
+    std::memcpy(R, R_wc, sizeof(R)); std::memcpy(t, t_wc, sizeof(t));
+    std::memcpy(kf.R_wc, R, sizeof(R)); std::memcpy(kf.t_wc, t, sizeof(t));
+    camera_block(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, kf.R_wc, kf.t_wc, kf.cam);
+    double T12[12];
+    pose_master(kf.R_wc, kf.t_wc, T12);
+    float f12[12];
+    std::memcpy(f12, kf.R_wc, 36); std::memcpy(f12 + 9, kf.t_wc, 12);
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    GLIC_CUDA_TRY(cudaMemcpyAsync(kf.cam_dev, kf.cam.view, 36 * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    GLIC_CUDA_TRY(cudaMemcpyAsync(m->pose_T + 12 * k, T12, sizeof(T12), cudaMemcpyHostToDevice, m->stream));
+    GLIC_CUDA_TRY(cudaMemcpyAsync(m->pose_f + 12 * k, f12, sizeof(f12), cudaMemcpyHostToDevice, m->stream));
+    if (reset) {
+        GLIC_CUDA_TRY(cudaMemsetAsync(m->pose_m + 6 * k, 0, 6 * sizeof(float), m->stream));
+        GLIC_CUDA_TRY(cudaMemsetAsync(m->pose_v + 6 * k, 0, 6 * sizeof(float), m->stream));
+        GLIC_CUDA_TRY(cudaMemsetAsync(m->pose_t + k, 0, sizeof(int), m->stream));
+    }
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    return GLIC_OK;
+}
+
+int launch_pose_step(glic_mapper* m, const int* views, int parity) {
+    PoseBatch b{};
+    for (int sl = 0; sl < m->S; ++sl) { b.kf[sl] = views[sl]; b.cam[sl] = m->train[views[sl]].cam_dev; }
+    float fov2[2];
+    proj_matrix(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, b.Pm, fov2);
+    StageTimer _t(GLIC_STAGE_ADAM, m->stream);
+    pose_step_kernel<<<1, MAX_SLOTS, 0, m->stream>>>(m->S, b, pose_slot(m, parity, 0), m->pose_T, m->pose_f, m->pose_m, m->pose_v,
+                                                     m->pose_t, m->pose_lr_rho, m->pose_lr_omega,
+                                                     reinterpret_cast<const unsigned int*>(geo_ptr(m) + (size_t)11 * m->Pcap));
+    GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }
 
@@ -340,9 +558,12 @@ int iteration(glic_mapper* m, const int* views) {
         cg.g_rot = reinterpret_cast<float4*>(geo + goff[0]); cg.g_xyz = geo + goff[1]; cg.g_scale = geo + goff[2]; cg.g_opacity = geo + goff[3];
         cg.opacity = m->act_opacity; cg.dL_dopacity = m->g_opacity; cg.rot_raw = reinterpret_cast<const float4*>(g[0]);
         cg.accumulate = j > 0;
+        cg.pose_partials = m->pose_on ? m->pose_part : nullptr;        // this view's dL/d(rho, omega), fused into the backward
+        cg.pose_grad = m->pose_on ? pose_slot(m, parity, slot) : nullptr;
         MAP_TRY(glic_backward_compact_internal((int)m->P, m->D, m->M, g[1], m->act_scales, m->act_rots, m->M ? g[5] : nullptr, &kf.view, m->radii,
                                                m->bin_cap, m->geom_ws, m->binning_ws, m->image_ws, m->sample_ws, m->dL_dpix, m->g_mean2D,
                                                m->g_conic, m->g_opacity, col, &cg, m->cfg.world > 1 ? (void*)m->ev_col : nullptr, s));
+        if (m->cfg.world > 1 && m->pose_on) GLIC_CUDA_TRY(cudaEventRecord(m->ev_pose, s));   // after the pose finish kernel
         if (m->cfg.world > 1) {
             GLIC_CUDA_TRY(cudaStreamWaitEvent(m->push_stream, m->ev_col, 0));
             for (int q = 0; q < m->cfg.world; ++q) {
@@ -353,6 +574,15 @@ int iteration(glic_mapper* m, const int* views) {
                     float* eg = expo_slot(m, parity, slot);
                     char* edst = static_cast<char*>(m->peers[q]) + (reinterpret_cast<char*>(eg) - m->xblock);
                     GLIC_CUDA_TRY(cudaMemcpyAsync(edst, eg, sizeof(float) * 12, cudaMemcpyDeviceToDevice, m->push_stream));
+                }
+            }
+            if (m->pose_on) {                      // this slot's dL/d(rho, omega): ev_col fired before the per-Gaussian backward
+                GLIC_CUDA_TRY(cudaStreamWaitEvent(m->push_stream, m->ev_pose, 0));
+                float* pg = pose_slot(m, parity, slot);
+                for (int q = 0; q < m->cfg.world; ++q) {
+                    if (q == m->cfg.rank) continue;
+                    char* pdst = static_cast<char*>(m->peers[q]) + (reinterpret_cast<char*>(pg) - m->xblock);
+                    GLIC_CUDA_TRY(cudaMemcpyAsync(pdst, pg, sizeof(float) * 6, cudaMemcpyDeviceToDevice, m->push_stream));
                 }
             }
         }
@@ -368,13 +598,19 @@ int iteration(glic_mapper* m, const int* views) {
     const float color_scale = m->M ? 1.0f / (float)m->S : 0.0f;
     float campos[MAX_SLOTS * 4];
     for (int sl = 0; sl < m->S; ++sl) std::memcpy(campos + 4 * sl, m->train[views[sl]].cam.campos, 16);
+    // pose refinement moves the camera blocks on the device: the SH rebuild reads each slot's centre from there
+    const float* campos_dev[MAX_SLOTS];
+    for (int sl = 0; sl < m->S; ++sl) campos_dev[sl] = m->train[views[sl]].cam_dev + 32;
     if (m->run_optimizer)
     MAP_TRY(launch_adam_compact(m->P, m->Pcap, m->D, m->M, m->params, m->m1, m->m2, geo, m->Pcap, lr6, col_slot(m, parity, 0), flag_slot(m, parity, 0),
-                                campos, m->S, 1.0f / (float)m->k, color_scale, 0.9f, 0.999f, 1e-15f, reinterpret_cast<const unsigned int*>(geo_tail), m->vis_acc, s));
+                                campos, m->S, 1.0f / (float)m->k, color_scale, 0.9f, 0.999f, 1e-15f, reinterpret_cast<const unsigned int*>(geo_tail), m->vis_acc, s,
+                                m->pose_on ? campos_dev : nullptr));
     // every replica steps the batch's exposures from the same S slot gradients, in slot order
     if (m->run_optimizer && m->expo_on)
         MAP_TRY(launch_exposure_adam(m->S, views, expo_slot(m, parity, 0), m->expo_E, m->expo_m, m->expo_v, m->expo_t, m->expo_lr,
                                      reinterpret_cast<const unsigned int*>(geo_tail), s));
+    // ... and their poses, after the Gaussians (whose SH rebuild above used the centres the batch was rendered from)
+    if (m->run_optimizer && m->pose_on) MAP_TRY(launch_pose_step(m, views, parity));
     GLIC_CUDA_TRY(cudaMemcpyAsync(m->loss_host + r, m->loss_dev + 1, sizeof(float), cudaMemcpyDeviceToHost, s));
     GLIC_CUDA_TRY(cudaEventRecord(m->ring_ev[r], s));
     m->ring_used[r] = true;
@@ -411,7 +647,7 @@ int glic_mapper_create(const glic_mapper_config* cfg, glic_mapper** out) {
     if (cudaGetDevice(&m->dev) != cudaSuccess) { set_error("mapper_create: no CUDA device"); return fail(GLIC_ERR_NO_DEVICE); }
     if (cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) != cudaSuccess || cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaStreamCreateWithFlags(&m->push_stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("mapper_create: stream creation failed"); return fail(GLIC_ERR_CUDA); }
-    cudaEvent_t* evs[] = {&m->gt_free[0], &m->gt_free[1], &m->gt_ready[0], &m->gt_ready[1], &m->ev_flags, &m->ev_col, &m->ev_push};
+    cudaEvent_t* evs[] = {&m->gt_free[0], &m->gt_free[1], &m->gt_ready[0], &m->gt_ready[1], &m->ev_flags, &m->ev_col, &m->ev_push, &m->ev_pose};
     for (cudaEvent_t* e : evs) if (cudaEventCreateWithFlags(e, cudaEventDisableTiming) != cudaSuccess) { set_error("mapper_create: event creation failed"); return fail(GLIC_ERR_CUDA); }
     for (int r = 0; r < RING; ++r) if (cudaEventCreateWithFlags(&m->ring_ev[r], cudaEventDisableTiming) != cudaSuccess) return fail(GLIC_ERR_CUDA);
     if (cudaEventCreate(&m->t0) != cudaSuccess || cudaEventCreate(&m->t1) != cudaSuccess) return fail(GLIC_ERR_CUDA);
@@ -446,11 +682,13 @@ int glic_mapper_destroy(glic_mapper* m) {
     for (void* p : bufs) if (p) cudaFree(p);
     void* expo[] = {m->expo_E, m->expo_m, m->expo_v, m->expo_t};
     for (void* p : expo) if (p) cudaFree(p);
+    void* pose[] = {m->pose_T, m->pose_f, m->pose_m, m->pose_v, m->pose_t, m->pose_part};
+    for (void* p : pose) if (p) cudaFree(p);
     for (auto& kf : m->train) if (kf.cam_dev) cudaFree(kf.cam_dev);
     for (auto& kf : m->test) if (kf.cam_dev) cudaFree(kf.cam_dev);
     if (m->counters_host) cudaFreeHost(m->counters_host);
     if (m->loss_host) cudaFreeHost(m->loss_host);
-    cudaEvent_t evs[] = {m->gt_free[0], m->gt_free[1], m->gt_ready[0], m->gt_ready[1], m->ev_flags, m->ev_col, m->ev_push, m->t0, m->t1};
+    cudaEvent_t evs[] = {m->gt_free[0], m->gt_free[1], m->gt_ready[0], m->gt_ready[1], m->ev_flags, m->ev_col, m->ev_push, m->ev_pose, m->t0, m->t1};
     for (cudaEvent_t e : evs) if (e) cudaEventDestroy(e);
     for (int r = 0; r < RING; ++r) if (m->ring_ev[r]) cudaEventDestroy(m->ring_ev[r]);
     if (m->stream) cudaStreamDestroy(m->stream);
@@ -500,6 +738,10 @@ int glic_mapper_add_keyframe(glic_mapper* m, const glic_keyframe* kfi, int is_tr
         MAP_TRY(expo_reset(m, m->train.size(), m->train.size() + 1));
     }
     (is_train ? m->train : m->test).push_back(kf);
+    if (is_train && m->pose_on) {                  // starts at its given pose with zero state
+        MAP_TRY(pose_reserve(m, m->train.size()));
+        MAP_TRY(pose_write(m, m->train.size() - 1, kf.R_wc, kf.t_wc, true));
+    }
     return GLIC_OK;
 }
 
@@ -546,9 +788,15 @@ int glic_mapper_extend(glic_mapper* m, int n, const float* points, const float* 
         GLIC_CUDA_TRY(cudaMemcpyAsync(m->final_T, ones.data(), sizeof(float) * ones.size(), cudaMemcpyHostToDevice, s));
         GLIC_CUDA_TRY(cudaStreamSynchronize(s));
     }
+    float view[16];
+    std::memcpy(view, kf.cam.view, sizeof(view));
+    if (m->pose_on) {                               // the keyframe's current (possibly refined) pose: its device camera block
+        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+        GLIC_CUDA_TRY(cudaMemcpy(view, kf.cam_dev, sizeof(view), cudaMemcpyDeviceToHost));
+    }
     float Rcw[9], tcw[3];
-    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Rcw[3 * i + j] = kf.cam.view[4 * j + i];   // view is column-major Rt
-    for (int i = 0; i < 3; ++i) tcw[i] = kf.cam.view[12 + i];
+    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Rcw[3 * i + j] = view[4 * j + i];   // view is column-major Rt
+    for (int i = 0; i < 3; ++i) tcw[i] = view[12 + i];
     int count = 0;
     MAP_TRY(glic_extend(n, d_pts, d_col, d_dep, Rcw, tcw, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, W, H, m->final_T, m->cfg.scaling_scale,
                         d_ws, glic_extend_bytes(n, W, H), d_keep, d_xyz, d_dc, d_ls, d_rot, d_op, &count, s));
@@ -737,6 +985,68 @@ int glic_mapper_exposure_adam_state(glic_mapper* m, int index, float* exp_avg12,
     GLIC_CUDA_TRY(cudaMemcpy(exp_avg12, m->expo_m + 12 * (size_t)index, 12 * sizeof(float), cudaMemcpyDeviceToHost));
     GLIC_CUDA_TRY(cudaMemcpy(exp_avg_sq12, m->expo_v + 12 * (size_t)index, 12 * sizeof(float), cudaMemcpyDeviceToHost));
     GLIC_CUDA_TRY(cudaMemcpy(step, m->expo_t + index, sizeof(int), cudaMemcpyDeviceToHost));
+    return GLIC_OK;
+}
+
+int glic_mapper_enable_pose_refinement(glic_mapper* m, float lr_translation, float lr_rotation) {
+    if (!m) { set_error("mapper_enable_pose_refinement: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!(lr_translation >= 0.0f) || !std::isfinite(lr_translation) || !(lr_rotation >= 0.0f) || !std::isfinite(lr_rotation)) {
+        set_error("mapper_enable_pose_refinement: the learning rates must be finite and >= 0"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (!m->pose_on) {                               // every training keyframe starts at its given pose with zero state
+        MAP_TRY(pose_reserve(m, m->train.size()));
+        for (size_t k = 0; k < m->train.size(); ++k) MAP_TRY(pose_write(m, k, m->train[k].R_wc, m->train[k].t_wc, true));
+        m->pose_on = true;
+    }
+    m->pose_lr_rho = lr_translation;
+    m->pose_lr_omega = lr_rotation;
+    return GLIC_OK;
+}
+
+static int pose_index_check(glic_mapper* m, int index, const void* buf, const char* what) {
+    if (!m || !buf) { set_error(std::string(what) + ": null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!m->pose_on) { set_error(std::string(what) + ": pose refinement is not enabled (glic_mapper_enable_pose_refinement)"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (index < 0 || index >= (int)m->train.size()) { set_error(std::string(what) + ": training keyframe index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
+    return GLIC_OK;
+}
+
+int glic_mapper_pose_get(glic_mapper* m, int index, float* R_wc9, float* t_wc3, float* cam41) {
+    MAP_TRY(pose_index_check(m, index, R_wc9, "mapper_pose_get"));
+    if (!t_wc3) { set_error("mapper_pose_get: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    float f12[12];
+    GLIC_CUDA_TRY(cudaMemcpy(f12, m->pose_f + 12 * (size_t)index, sizeof(f12), cudaMemcpyDeviceToHost));
+    std::memcpy(R_wc9, f12, 36); std::memcpy(t_wc3, f12 + 9, 12);
+    if (cam41) {
+        const Keyframe& kf = m->train[index];
+        GLIC_CUDA_TRY(cudaMemcpy(cam41, kf.cam_dev, 35 * sizeof(float), cudaMemcpyDeviceToHost));   // view | proj | campos[3]
+        cam41[35] = kf.cam.tanfovx; cam41[36] = kf.cam.tanfovy; std::memcpy(cam41 + 37, kf.cam.lim, 16);
+    }
+    return GLIC_OK;
+}
+
+int glic_mapper_pose_set(glic_mapper* m, int index, const float* R_wc9, const float* t_wc3) {
+    MAP_TRY(pose_index_check(m, index, R_wc9, "mapper_pose_set"));
+    if (!t_wc3) { set_error("mapper_pose_set: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    for (int j = 0; j < 9; ++j) if (!std::isfinite(R_wc9[j])) { set_error("mapper_pose_set: non-finite entry"); return GLIC_ERR_INVALID_ARGUMENT; }
+    for (int j = 0; j < 3; ++j) if (!std::isfinite(t_wc3[j])) { set_error("mapper_pose_set: non-finite entry"); return GLIC_ERR_INVALID_ARGUMENT; }
+    // a rotation: R^T R = I to float precision and det R = +1
+    double R[9], err = 0.0;
+    for (int j = 0; j < 9; ++j) R[j] = R_wc9[j];
+    for (int a = 0; a < 3; ++a)
+        for (int b = 0; b < 3; ++b) err = std::max(err, std::fabs(R[a] * R[b] + R[3 + a] * R[3 + b] + R[6 + a] * R[6 + b] - (a == b ? 1.0 : 0.0)));
+    const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) + R[2] * (R[3] * R[7] - R[4] * R[6]);
+    if (err > 1e-5 || det < 0.0) { set_error("mapper_pose_set: R_wc is not a rotation (orthonormal, det +1)"); return GLIC_ERR_INVALID_ARGUMENT; }
+    return pose_write(m, (size_t)index, R_wc9, t_wc3, false);
+}
+
+int glic_mapper_pose_adam_state(glic_mapper* m, int index, float* exp_avg6, float* exp_avg_sq6, int* step) {
+    MAP_TRY(pose_index_check(m, index, step, "mapper_pose_adam_state"));
+    if (!exp_avg6 || !exp_avg_sq6) { set_error("mapper_pose_adam_state: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    GLIC_CUDA_TRY(cudaMemcpy(exp_avg6, m->pose_m + 6 * (size_t)index, 6 * sizeof(float), cudaMemcpyDeviceToHost));
+    GLIC_CUDA_TRY(cudaMemcpy(exp_avg_sq6, m->pose_v + 6 * (size_t)index, 6 * sizeof(float), cudaMemcpyDeviceToHost));
+    GLIC_CUDA_TRY(cudaMemcpy(step, m->pose_t + index, sizeof(int), cudaMemcpyDeviceToHost));
     return GLIC_OK;
 }
 

@@ -14,6 +14,18 @@
 //          expressions of activations_backward_kernel -- written or ACCUMULATED over a rank's views.  dL/d(dc, sh-rest) are
 //          not materialised: they are linear in the clamp-masked dL/dcolour (the render backward's output + the forward's
 //          clamp bits) and are rebuilt inside the Adam kernel (model_step.cu).
+//
+// POSE (only with COMPACT; glic_mapper_enable_pose_refinement): the same pass also reduces the view's camera-pose gradient
+// g = dL/d(rho, omega) of T_cw(delta) = Exp(delta) T_cw at delta = 0 (delta in the camera frame, translation first).  With
+// W the rotation block of `view`, per visible Gaussian i
+//     g_view,i = dL/dp_view through J (dtx, dty, dtz) + W * (the projection adjoint, a world-frame vector),
+//     G_i      = J_i^T dL/dT_i  (= dL/dW through T = J W),
+//     d_i      = the SH view-direction adjoint (world frame; zero when M = 0, as the colour backward is skipped then),
+//     dL/drho   = sum_i g_view,i + W d_i                        (the camera centre moves by -W^T rho)
+//     dL/domega = sum_i p_view,i x g_view,i + sum_c W[:,c] x G_i[:,c]   (the camera centre does not move under omega).
+// Each Gaussian forms its six terms in fp32; the CTA adds them in float64 in a fixed order (warp shuffles, then the four
+// warps in order) and writes one partial per CTA; pose_grad_finish_kernel adds the partials in a fixed order.  No atomics:
+// two runs give the same bits.
 #include "geom_math.cuh"
 #include "sh_math.cuh"
 #include "warp_rows.cuh"
@@ -22,7 +34,7 @@ namespace glic {
 
 constexpr int PB_THREADS = 128;
 
-template <bool COMPACT>
+template <bool COMPACT, bool POSE = false>
 __global__ void __launch_bounds__(PB_THREADS)
 preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means, const float* __restrict__ scales,
                            float mod, const float4* __restrict__ rots, const float* __restrict__ sh, ViewParams vp,
@@ -33,6 +45,7 @@ preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means,
                            float* __restrict__ dL_dscales, float4* __restrict__ dL_drots, CompactGrads cg) {
     __shared__ float s_view[16], s_proj[16], s_cam[3];
     __shared__ __align__(16) float s_sh[PB_THREADS / 32][32 * SH_ROW_MAX];    // SH rows in, dL/dSH rows out
+    static_assert(COMPACT || !POSE, "the pose gradient is a compact-form output");
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (tid < 16) s_view[tid] = vp.view[tid];
     else if (tid < 32) s_proj[tid - 16] = vp.proj[tid - 16];
@@ -43,9 +56,10 @@ preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means,
     const bool staged = K > 0 && K <= SH_ROW_MAX && sh != nullptr;
     const int wfirst = blockIdx.x * blockDim.x + warp * 32;
     const int wcnt = min(32, P - wfirst);
-    if (wcnt <= 0) return;                                         // whole warp beyond P (warp-uniform)
+    if (wcnt <= 0 && !POSE) return;                                // whole warp beyond P (warp-uniform; POSE: stays for the CTA sum)
     float* slab = s_sh[warp];
-    if (staged && D > 0) warp_load_rows(sh, (size_t)wfirst, wcnt, K, slab, lane);
+    if (staged && D > 0 && (!POSE || wcnt > 0)) warp_load_rows(sh, (size_t)wfirst, wcnt, K, slab, lane);
+    float pose6[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};               // POSE: this Gaussian's dL/d(rho, omega)
     // dL/dSH row of this thread: shared-memory slab (written back coalesced below) or global memory
     float* dsh = staged ? (slab + lane * K) : (dL_dsh + (size_t)(idx < P ? idx : 0) * K);
     const bool visible = idx < P && radii[idx] > 0;
@@ -139,6 +153,7 @@ preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means,
     // reference (`if (shs)`, backward.cu:352) the whole colour backward -- dL/ddc included -- is skipped when no SH-rest
     // tensor is bound (M == 0). ----------------------------------------------------------------------------------
     float dRGB[3] = {0.f, 0.f, 0.f};
+    float dsx = 0.f, dsy = 0.f, dsz = 0.f;                         // POSE: the view-direction adjoint d_i
     if (sh == nullptr) {
         if (!COMPACT) { dL_ddc[3 * idx] = 0.f; dL_ddc[3 * idx + 1] = 0.f; dL_ddc[3 * idx + 2] = 0.f; }
     } else {
@@ -189,6 +204,44 @@ preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means,
         dmx += ((+sum2 - ox * ox) * ddx - oy * ox * ddy - oz * ox * ddz) * invsum32;
         dmy += (-ox * oy * ddx + (sum2 - oy * oy) * ddy - oz * oy * ddz) * invsum32;
         dmz += (-ox * oz * ddx - oy * oz * ddy + (sum2 - oz * oz) * ddz) * invsum32;
+        if constexpr (POSE) {
+            dsx = ((+sum2 - ox * ox) * ddx - oy * ox * ddy - oz * ox * ddz) * invsum32;
+            dsy = (-ox * oy * ddx + (sum2 - oy * oy) * ddy - oz * oy * ddz) * invsum32;
+            dsz = (-ox * oz * ddx - oy * oz * ddy + (sum2 - oz * oz) * ddz) * invsum32;
+        }
+    }
+    if constexpr (POSE) {
+        // the projection adjoint of the block above, rotated into the view frame, plus the part through J
+        const float* pr = s_proj;
+        const float hx = xform_row(pr, 0, px, py, pz), hy = xform_row(pr, 1, px, py, pz), hw = xform_row(pr, 3, px, py, pz);
+        const float m_w = 1.0f / (hw + 0.0000001f);
+        const float mul1 = hx * m_w * m_w, mul2 = hy * m_w * m_w;
+        const float g2x = dL_dmean2D[3 * idx], g2y = dL_dmean2D[3 * idx + 1];
+        const float pjx = (pr[0] * m_w - pr[3] * mul1) * g2x + (pr[1] * m_w - pr[3] * mul2) * g2y;
+        const float pjy = (pr[4] * m_w - pr[7] * mul1) * g2x + (pr[5] * m_w - pr[7] * mul2) * g2y;
+        const float pjz = (pr[8] * m_w - pr[11] * mul1) * g2x + (pr[9] * m_w - pr[11] * mul2) * g2y;
+        // W[r][c] = v[4c + r]; (W x)_r = v[r] x0 + v[4 + r] x1 + v[8 + r] x2
+        const float ux = pjx + dsx, uy = pjy + dsy, uz = pjz + dsz;
+        const float gvx = dtx + (v[0] * pjx + v[4] * pjy + v[8] * pjz);
+        const float gvy = dty + (v[1] * pjx + v[5] * pjy + v[9] * pjz);
+        const float gvz = dtz + (v[2] * pjx + v[6] * pjy + v[10] * pjz);
+        pose6[0] = dtx + (v[0] * ux + v[4] * uy + v[8] * uz);
+        pose6[1] = dty + (v[1] * ux + v[5] * uy + v[9] * uz);
+        pose6[2] = dtz + (v[2] * ux + v[6] * uy + v[10] * uz);
+        const float vx = xform_row(v, 0, px, py, pz), vy = xform_row(v, 1, px, py, pz), vz = tz;   // p_view
+        // G = J^T dT with J = [[fx/tz, 0, -fx lx/tz], [0, fy/tz, -fy ly/tz]] (the clamped lx, ly of cov2d_project)
+        const float J00 = fx * itz, J11 = fy * itz, J02 = -fx * c2.lx * itz, J12 = -fy * c2.ly * itz;
+        const float dT[2][3] = {{dT00, dT01, dT02}, {dT10, dT11, dT12}};
+        float wx = vy * gvz - vz * gvy, wy = vz * gvx - vx * gvz, wz = vx * gvy - vy * gvx;
+#pragma unroll
+        for (int cc = 0; cc < 3; ++cc) {
+            const float G0 = J00 * dT[0][cc], G1 = J11 * dT[1][cc], G2 = J02 * dT[0][cc] + J12 * dT[1][cc];
+            const float a0 = v[4 * cc], a1 = v[4 * cc + 1], a2 = v[4 * cc + 2];
+            wx += a1 * G2 - a2 * G1;
+            wy += a2 * G0 - a0 * G2;
+            wz += a0 * G1 - a1 * G0;
+        }
+        pose6[3] = wx; pose6[4] = wy; pose6[5] = wz;
     }
 
     // ---- cov3D backward (computeCov3D's adjoint, backward.cu:257-310): Sigma = M^T M, M = S R ------------------------
@@ -264,6 +317,38 @@ preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means,
     }
     }   // visible
     if (!COMPACT && staged) warp_store_rows(dL_dsh, (size_t)wfirst, wcnt, K, slab, lane);
+    if constexpr (POSE) {
+        __shared__ double s_pose[PB_THREADS / 32][6];
+        double r6[6];
+#pragma unroll
+        for (int j = 0; j < 6; ++j) {
+            r6[j] = (double)pose6[j];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) r6[j] += __shfl_down_sync(0xffffffffu, r6[j], o);
+        }
+        if (lane == 0) {
+#pragma unroll
+            for (int j = 0; j < 6; ++j) s_pose[warp][j] = r6[j];
+        }
+        __syncthreads();
+        if (tid < 6) {
+            double acc = 0.0;
+#pragma unroll
+            for (int w = 0; w < PB_THREADS / 32; ++w) acc += s_pose[w][tid];
+            cg.pose_partials[6 * (size_t)blockIdx.x + tid] = acc;
+        }
+    }
+}
+
+// one CTA: warp j adds component j of the G per-CTA partials (lane-strided, then a butterfly; a fixed order)
+__global__ void __launch_bounds__(192)
+pose_grad_finish_kernel(unsigned G, const double* __restrict__ partials, float* __restrict__ out6) {
+    const int j = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double s = 0.0;
+    for (unsigned b = lane; b < G; b += 32) s += partials[6 * (size_t)b + j];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) out6[j] = (float)s;
 }
 
 int launch_preprocess_backward(int P, int D, int M, const float* means, const float* scales, float mod,
@@ -283,11 +368,23 @@ int launch_preprocess_backward_compact(int P, int D, int M, const float* means, 
                                        const float* rots, const float* sh, const ViewParams& vp, const int* radii, GeomState g,
                                        const float* dL_dmean2D, const float* dL_dconic, const float* dL_dcolors,
                                        const CompactGrads& cg, cudaStream_t s) {
+    const unsigned blocks = (P + PB_THREADS - 1) / PB_THREADS;
+    if (cg.pose_partials) {
+        preprocess_backward_kernel<true, true><<<blocks, PB_THREADS, 0, s>>>(
+            P, D, M, means, scales, mod, reinterpret_cast<const float4*>(rots), sh, vp, radii, g.clamped, 0.0f,
+            dL_dmean2D, dL_dconic, dL_dcolors, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cg);
+        GLIC_LAUNCH_CHECK();
+        pose_grad_finish_kernel<<<1, 192, 0, s>>>(blocks, cg.pose_partials, cg.pose_grad);
+        GLIC_LAUNCH_CHECK();
+        return GLIC_OK;
+    }
     preprocess_backward_kernel<true><<<(P + PB_THREADS - 1) / PB_THREADS, PB_THREADS, 0, s>>>(
         P, D, M, means, scales, mod, reinterpret_cast<const float4*>(rots), sh, vp, radii, g.clamped, 0.0f,
         dL_dmean2D, dL_dconic, dL_dcolors, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cg);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }
+
+size_t pose_partials_count(uint32_t Pcap) { return 6 * (size_t)((Pcap + PB_THREADS - 1) / PB_THREADS); }
 
 }  // namespace glic

@@ -140,6 +140,35 @@ class Mapper:
         capi.check(capi.lib.glic_mapper_exposure_adam_state(self._h, int(index), m1, m2, C.byref(t)), "mapper_exposure_adam_state")
         return self.exposure(index), np.array(m1[:], np.float32).reshape(3, 4), np.array(m2[:], np.float32).reshape(3, 4), int(t.value)
 
+    def enable_pose_refinement(self, lr_translation, lr_rotation):
+        """Refine every training keyframe's pose from now on: T_cw <- Exp(u) T_cw, u from Adam on dL/d(rho, omega)."""
+        capi.check(capi.lib.glic_mapper_enable_pose_refinement(self._h, float(lr_translation), float(lr_rotation)),
+                   "mapper_enable_pose_refinement")
+
+    def pose(self, index, camera=False):
+        """(R_wc [3,3], t_wc [3]) float32 of training keyframe `index`; camera=True adds its device camera block as a dict
+        shaped like camera_block()'s."""
+        R, t, cam = (C.c_float * 9)(), (C.c_float * 3)(), (C.c_float * 41)()
+        capi.check(capi.lib.glic_mapper_pose_get(self._h, int(index), R, t, cam if camera else None), "mapper_pose_get")
+        out = (np.array(R[:], np.float32).reshape(3, 3), np.array(t[:], np.float32))
+        if not camera:
+            return out
+        o = np.array(cam[:], np.float32)
+        return out + (dict(W=self.W, H=self.H, view=o[:16].copy(), proj=o[16:32].copy(), campos=o[32:35].copy(),
+                           tanfovx=float(o[35]), tanfovy=float(o[36]), lims=o[37:41].copy()),)
+
+    def set_pose(self, index, R_wc, t_wc):
+        """Overwrite the pose of training keyframe `index`; its Adam state is kept."""
+        R = (C.c_float * 9)(*[float(x) for x in np.asarray(R_wc, np.float32).reshape(9)])
+        t = (C.c_float * 3)(*[float(x) for x in np.asarray(t_wc, np.float32).reshape(3)])
+        capi.check(capi.lib.glic_mapper_pose_set(self._h, int(index), R, t), "mapper_pose_set")
+
+    def pose_state(self, index):
+        """(exp_avg [6], exp_avg_sq [6], step count) of training keyframe `index`'s pose (rho then omega)"""
+        m1, m2, t = (C.c_float * 6)(), (C.c_float * 6)(), C.c_int()
+        capi.check(capi.lib.glic_mapper_pose_adam_state(self._h, int(index), m1, m2, C.byref(t)), "mapper_pose_adam_state")
+        return np.array(m1[:], np.float32), np.array(m2[:], np.float32), int(t.value)
+
     def synchronize(self):
         capi.check(capi.lib.glic_mapper_synchronize(self._h), "mapper_synchronize")
 

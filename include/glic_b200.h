@@ -441,6 +441,29 @@ GLIC_API int glic_mapper_exposure_get(glic_mapper* m, int index, float* out12);
 GLIC_API int glic_mapper_exposure_set(glic_mapper* m, int index, const float* in12);
 /* the exposure's Adam state of training keyframe `index`: both moments (12 floats each) and the step count; synchronises */
 GLIC_API int glic_mapper_exposure_adam_state(glic_mapper* m, int index, float* exp_avg12, float* exp_avg_sq12, int* step);
+/* Per-keyframe pose refinement (no counterpart in the reference, which takes every odometry pose as exact).  Off by default.
+ * glic_mapper_enable_pose_refinement(m, lr_translation, lr_rotation) may be called before or between optimize() calls; a
+ * repeated call changes the rates only.  Training keyframe k's pose (R_wc, t_wc) defines T_cw = [R_wc^T | -R_wc^T t_wc]
+ * (kept in float64, initialised exactly from the floats), perturbed as T_cw(delta) = Exp(delta) T_cw with
+ * delta = (rho, omega) in the camera frame, translation first, Exp the SE(3) exponential.  Its gradient at delta = 0 is
+ *     g_k = (1/S) * sum over the batch slots holding k of dL_view/ddelta,
+ * computed inside the per-Gaussian backward.  After the Gaussian step one launch steps the batch's keyframes with
+ * torch::optim::Adam's rule (betas 0.9 / 0.999, eps 1e-8, bias correction from the keyframe's own step count t, lr =
+ * lr_translation for rho and lr_rotation for omega), then T_cw <- Exp(u) T_cw for the update u, re-derives the float
+ * (R_wc, t_wc) and rebuilds the keyframe's camera block from them: that block always equals glic_camera_block(R_wc, t_wc)
+ * of the current float pose, bit for bit, and an update of exactly zero leaves it unchanged.  The moments persist when the
+ * pose moves.  An iteration skipped for a binning overflow leaves pose, m, v and t unchanged; GLIC_MAPPER_OPT_OPTIMIZER = 0
+ * leaves the pose step out too.  With world > 1 each rank pushes its slots' 6-float gradients to its peers and every replica
+ * applies the same step.  Training keyframes are rendered, evaluated and (extend(), on the newest) projected with their
+ * current pose; held-out keyframes keep theirs; keyframes added later start at their given pose with zero state.
+ * pose_get returns the current float pose of training keyframe `index` and, if cam41 is not NULL, its camera block in
+ * glic_camera_block's layout, read back from the device.  pose_set rejects non-finite input and an R_wc that is not a
+ * rotation; it leaves the Adam state alone.  These calls synchronise and need pose refinement enabled. */
+GLIC_API int glic_mapper_enable_pose_refinement(glic_mapper* m, float lr_translation, float lr_rotation);
+GLIC_API int glic_mapper_pose_get(glic_mapper* m, int index, float* R_wc9, float* t_wc3, float* cam41_or_null);
+GLIC_API int glic_mapper_pose_set(glic_mapper* m, int index, const float* R_wc9, const float* t_wc3);
+/* the pose's Adam state of training keyframe `index`: both moments (6 floats each, rho then omega) and the step count */
+GLIC_API int glic_mapper_pose_adam_state(glic_mapper* m, int index, float* exp_avg6, float* exp_avg_sq6, int* step);
 /* Camera (camera.h:38-110) in closed form, as the mapper derives it from a keyframe pose: out41 = view[16] (column-major
  * Rt) | proj[16] (column-major P*Rt) | campos[3] | tan_fovx, tan_fovy | limx_neg, limx_pos, limy_neg, limy_pos. */
 GLIC_API int glic_camera_block(int width, int height, float fx, float fy, float cx, float cy, const float* R_wc /*[9] row-major*/,

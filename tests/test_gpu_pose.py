@@ -1,0 +1,403 @@
+"""Per-keyframe pose refinement in the native mapper (glic_mapper_enable_pose_refinement) on the GPU: the pose gradient fused
+into the per-Gaussian backward, recovered from the pose's Adam moments and compared with the CPU restatement (pose_oracle.py)
+on the mapper's own image and dL/dpixel; the bit contract of the rebuilt camera blocks; the recovery of perturbed poses with
+frozen Gaussians; the overflow skip; two ranks against one; evaluation and extend() at the refined pose; and pose refinement
+together with exposure.
+
+Pose: T_cw(delta) = Exp(delta) T_cw, delta = (rho, omega) in the camera frame; g = (1/S) sum over the batch slots holding the
+keyframe of dL_view/ddelta.  The first Adam step from zero moments stores m' = fl((1 - b1) g), so g = m' / fl(1 - b1) to
+0.5 ulp, as in test_gpu_mapper_grads.py."""
+import os
+import socket
+
+import numpy as np
+import pytest
+
+from pose_oracle import pose_gradient
+from test_gpu_exposure import E_STAR, _render
+from test_gpu_mapper_grads import (C1, F, GROUPS, H, W, _compare, _keyframes, _mapper, _raw, _recovered, _reference, _scene,
+                                   _state)
+
+pytestmark = pytest.mark.gpu
+torch = pytest.importorskip("torch")
+
+LR_T, LR_R = 1e-3, 1e-3
+B1 = np.float32(0.9)
+
+
+def _pose_reference(raw, cams, gts, batch, oracles, Es=None):
+    """{keyframe: mean over the batch's slots of dL/d(rho, omega)} per oracle dtype, on the image and (exposed) dL/dpixel the
+    mapper's kernels produce for the raw parameters `raw` at the cameras `cams`"""
+    from gaussian_lic_b200 import model, ops
+    dev = torch.device("cuda:0")
+    mdl = model.PackedModel(raw, dev)
+    mdl.activate()
+    rast = ops.CRasterizer(W, H, dev)
+    out = {o.dtype.name: {} for o in oracles}
+    loss = None
+    for v in batch:
+        color, _, _ = rast.forward(mdl.inputs, rast.make_view(cams[v]))
+        gt = torch.as_tensor(gts[v]).to(dev)
+        if Es is None:
+            loss, dL = rast.loss(color, gt, 0.2)
+        else:
+            loss, dL, _ = ops.l1_ssim_loss_exposure(color, gt, torch.as_tensor(Es[v]).to(dev))
+        torch.cuda.synchronize()
+        dL = dL.cpu().numpy()
+        for o in oracles:
+            op, sc, rot = o.activations(raw["opacity_logits"], raw["log_scales"], raw["rots"])
+            g = dict(means=raw["means"], scales=sc, rots=rot, opacity=op, dc=raw["dc"], sh=raw["sh"], degree=raw["degree"])
+            f = o.forward(g, cams[v])
+            b = o.backward(f, dL)
+            gr = pose_gradient(g, cams[v], f, b)
+            o.free(f)
+            acc = out[o.dtype.name]
+            acc[v] = acc.get(v, 0.0) + gr / len(batch)
+    return out, float(loss.item())
+
+
+def _check_pose_grad(got, ref, what, tol=2e-3):
+    """relative norm error against the f64 restatement; the f32 oracle's distance is printed as the yardstick"""
+    want, yard = ref["float64"], ref["float32"]
+    worst = 0.0
+    for k, w in want.items():
+        err = np.linalg.norm(got[k] - w) / np.linalg.norm(w)
+        ye = np.linalg.norm(yard[k] - w) / np.linalg.norm(w)
+        print("%s: keyframe %d dL/d(rho, omega) recovered %s\n  f64 restatement %s\n  |diff|/|ref| = %.2e (f32 oracle: %.2e)" % (
+            what, k, got[k], w, err, ye))
+        worst = max(worst, err)
+        assert err <= tol, (what, k, err)
+    return worst
+
+
+# ---- gradient ---------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("deg", [0, 3])
+@pytest.mark.parametrize("batch", [[0], [0, 1], [1, 1]], ids=["one_view", "two_views", "same_view_twice"])
+def test_pose_gradient_matches_restatement(oracle32, oracle64, deg, batch):
+    raw = _scene(deg)
+    poses, cams, gts = _keyframes(seed=17)
+    m = _mapper(raw, poses, gts, views_per_rank=len(batch))
+    m.enable_pose_refinement(LR_T, LR_R)
+    before = _state(m)
+    assert all(t == 0 and not a.any() and not b.any() for a, b, t in (m.pose_state(i) for i in range(3)))
+    m.optimize(batch)
+    what = "pose, degree %d, views %s" % (deg, batch)
+    ref, loss = _pose_reference(_raw(before), cams, gts, batch, [oracle32, oracle64])
+    assert abs(m.stats().last_loss - loss) <= 1e-5 * loss
+    got = {}
+    for k in range(3):
+        m1, v1, t1 = m.pose_state(k)
+        if k not in batch:
+            assert t1 == 0 and not m1.any() and not v1.any(), (what, k)
+            R, t = m.pose(k)
+            assert np.array_equal(R, poses[k][0].astype(np.float32)) and np.array_equal(t, poses[k][1].astype(np.float32))
+            continue
+        assert t1 == 1, (what, k, t1)                                             # [1, 1]: one step for the two slots
+        got[k] = m1.astype(np.float64) / C1
+    _check_pose_grad(got, ref, what)
+    m.close()
+
+
+def test_second_step_uses_the_refined_pose(oracle32, oracle64):
+    """Step 2 renders keyframe 0 at its refined pose: its pose gradient there matches the restatement at the camera block
+    pose_get returns, and the Gaussians' dc / SH gradients (rebuilt in the Adam kernel from the slot's camera centre) match
+    the oracle at that camera -- not at the keyframe's original one."""
+    raw = _scene(3)
+    poses, cams, gts = _keyframes(seed=19)
+    m = _mapper(raw, poses, gts)
+    m.enable_pose_refinement(LR_T, LR_R)
+    m.optimize([0])
+    R1, t1, cam1 = m.pose(0, camera=True)
+    assert not np.array_equal(cam1["campos"], cams[0]["campos"])
+    mid = _state(m)
+    m_1, _, _ = m.pose_state(0)
+    m.optimize([0])
+    after = _state(m)
+    m_2, _, t2 = m.pose_state(0)
+    assert t2 == 2
+    what = "second step on the moved pose"
+    ref, loss = _pose_reference(_raw(mid), [cam1], gts, [0], [oracle32, oracle64])
+    got = {0: (m_2.astype(np.float64) - (B1 * m_1).astype(np.float64)) / C1}
+    _check_pose_grad(got, ref, what)
+    gref = _reference(_raw(mid), [cam1], gts, [0], [oracle32, oracle64])
+    rec = _recovered(mid, after)
+    rows = np.flatnonzero(gref["vis"])
+    _compare(rec, gref, rows, what, groups=("dc", "sh", "means"))
+    stale = _reference(_raw(mid), cams, gts, [0], [oracle64])
+    d_fresh = np.abs(rec["sh"][rows] - gref["grads"]["float64"]["sh"][rows]).max()
+    d_stale = np.abs(rec["sh"][rows] - stale["grads"]["float64"]["sh"][rows]).max()
+    print("%s: sh gradient vs oracle at the refined camera %.3e, at the original camera %.3e" % (what, d_fresh, d_stale))
+    assert d_stale > 10 * d_fresh
+    m.close()
+
+
+def test_pose_gradient_with_exposure(oracle32, oracle64):
+    raw = _scene(3)
+    poses, cams, gts = _keyframes(seed=23)
+    batch = [0, 1]
+    m = _mapper(raw, poses, gts, views_per_rank=2)
+    m.enable_exposure(0.001)
+    m.enable_pose_refinement(LR_T, LR_R)
+    for i in range(3):
+        m.set_exposure(i, E_STAR[i])
+    before = _state(m)
+    m.optimize(batch)
+    ref, loss = _pose_reference(_raw(before), cams, gts, batch, [oracle32, oracle64], Es=E_STAR)
+    assert abs(m.stats().last_loss - loss) <= 1e-5 * loss
+    got = {k: m.pose_state(k)[0].astype(np.float64) / C1 for k in batch}
+    _check_pose_grad(got, ref, "pose with exposure")
+    assert all(m.exposure_state(k)[3] == 1 for k in batch)
+    m.close()
+
+
+# ---- the bit contract --------------------------------------------------------------------------------------------------------
+def test_camera_block_is_the_camera_of_the_float_pose():
+    from gaussian_lic_b200 import mapper
+    raw = _scene(2)
+    poses, cams, gts = _keyframes(seed=29)
+    m = _mapper(raw, poses, gts, views_per_rank=2)
+    m.enable_pose_refinement(LR_T, LR_R)
+    m.optimize([0, 1, 2, 0, 2, 2, 1, 0])
+    for k in range(3):
+        R, t, cam = m.pose(k, camera=True)
+        want = mapper.camera_block(W, H, F, F, W / 2.0, H / 2.0, R, t)
+        assert m.pose_state(k)[2] > 0
+        assert not np.array_equal(cam["view"], cams[k]["view"])                  # it moved
+        for key in ("view", "proj", "campos", "lims"):
+            assert np.array_equal(cam[key].view(np.uint32), np.asarray(want[key], np.float32).view(np.uint32)), (k, key)
+        assert cam["tanfovx"] == want["tanfovx"] and cam["tanfovy"] == want["tanfovy"]
+        assert np.abs(R.astype(np.float64).T @ R - np.eye(3)).max() < 1e-6
+    m.close()
+    # both rates zero: every update is exactly zero, the blocks keep their original bits (the Adam state still advances)
+    m = _mapper(raw, poses, gts)
+    m.enable_pose_refinement(0.0, 0.0)
+    m.optimize([0, 1, 2, 1])
+    for k in range(3):
+        R, t, cam = m.pose(k, camera=True)
+        assert np.array_equal(R, poses[k][0].astype(np.float32)) and np.array_equal(t, poses[k][1].astype(np.float32))
+        for key in ("view", "proj", "campos"):
+            assert np.array_equal(cam[key].view(np.uint32), np.asarray(cams[k][key], np.float32).view(np.uint32)), (k, key)
+    assert m.pose_state(1)[2] == 2
+    m.close()
+
+
+# ---- recovery of perturbed poses -------------------------------------------------------------------------------------------
+REC_ITERS = 300
+REC_FACTOR = 20.0            # both errors must shrink at least this much (H100 run: 0.019 rad -> 1.9e-4, 0.039 -> 7.7e-5)
+
+
+def _rot_angle(Ra, Rb):
+    c = (np.trace(np.asarray(Ra, np.float64).T @ np.asarray(Rb, np.float64)) - 1.0) / 2.0
+    return float(np.arccos(np.clip(c, -1.0, 1.0)))
+
+
+def test_pose_refinement_recovers_perturbed_poses():
+    """Gaussians frozen (all five learning rates 0, exact: p + (-0)); targets rendered at the true poses; the two rig views
+    (keyframes 1 and 2) added at poses perturbed by ~0.6 degrees and ~2 cm.  Optimising the poses alone must shrink the
+    rotation and translation errors.  Keyframe 0 (the identity view, in whose frame this scene is generated: Gaussians down to
+    z = -1, through the near plane and outside the clamp limits) keeps its true pose and is not optimised: a recorded run
+    that optimised it too drifted to 0.11 rad while keyframes 1 and 2 converged."""
+    from gaussian_lic_b200 import mapper
+    raw = _scene(3)
+    poses, cams, _ = _keyframes()
+    gts = _render(raw, cams)
+    rng = np.random.default_rng(3)
+    frozen = dict(position_lr=0.0, feature_lr=0.0, opacity_lr=0.0, scaling_lr=0.0, rotation_lr=0.0)
+    m = mapper.Mapper(W, H, F, F, W / 2.0, H / 2.0, sh_degree=3, **frozen)
+    m.initialize(raw)
+    m.enable_pose_refinement(LR_T, LR_R)
+    from scipy.spatial.transform import Rotation
+    for k, ((R, t), img) in enumerate(zip(poses, gts)):
+        dR = Rotation.from_rotvec(rng.normal(size=3) * 0.01 / np.sqrt(3)).as_matrix() if k else np.eye(3)
+        m.add_keyframe(dR @ R, t + (rng.normal(size=3) * 0.02 / np.sqrt(3) if k else 0.0), img)
+    p0 = _state(m)["p"]
+
+    def errs():
+        out = []
+        for k, (R, t) in list(enumerate(poses))[1:]:
+            Rk, tk = m.pose(k)
+            out.append((_rot_angle(Rk, R), float(np.linalg.norm(tk - t))))
+        return np.array(out)
+
+    e0 = errs()
+    first = m.optimize([1, 2]).last_loss
+    m.optimize([1, 2] * (REC_ITERS - 1))
+    last = m.stats().last_loss
+    e1 = errs()
+    print("pose recovery: loss %.5f -> %.5f\n  rotation error (rad) %s -> %s\n  translation error %s -> %s" % (
+        first, last, e0[:, 0], e1[:, 0], e0[:, 1], e1[:, 1]))
+    p1 = _state(m)["p"]
+    assert all(np.array_equal(p0[g], p1[g]) for g in GROUPS)                    # the Gaussians did not move
+    assert e1[:, 0].max() * REC_FACTOR <= e0[:, 0].max()
+    assert e1[:, 1].max() * REC_FACTOR <= e0[:, 1].max()
+    assert last < 0.5 * first
+    assert m.pose_state(0)[2] == 0
+    m.close()
+
+
+# ---- overflow -------------------------------------------------------------------------------------------------------------
+def test_overflowed_iteration_leaves_the_pose_unchanged():
+    raw = _scene(1)
+    poses, cams, gts = _keyframes()
+    m = _mapper(raw, poses, gts)
+    m.enable_pose_refinement(LR_T, LR_R)
+    m.optimize([0])
+    s0 = [(m.pose(k, camera=True), m.pose_state(k)) for k in range(3)]
+    m.set_binning_pairs(1000)
+    st = m.optimize([0])
+    assert st.overflow_regrows >= 1 and st.iterations == 2
+    s1 = [(m.pose(k, camera=True), m.pose_state(k)) for k in range(3)]
+    for (pa, sa), (pb, sb) in zip(s0, s1):
+        assert np.array_equal(pa[0], pb[0]) and np.array_equal(pa[1], pb[1])
+        assert np.array_equal(pa[2]["view"], pb[2]["view"]) and np.array_equal(pa[2]["proj"], pb[2]["proj"])
+        for x, y in zip(sa[:2], sb[:2]):
+            assert np.array_equal(x.view(np.uint32), y.view(np.uint32))
+        assert sa[2] == sb[2]
+    assert s1[0][1][2] == 1
+    m.optimize([0])
+    assert m.pose_state(0)[2] == 2
+    m.close()
+
+
+# ---- evaluation and extend at the refined pose -------------------------------------------------------------------------------
+def test_evaluate_and_extend_use_the_refined_pose():
+    from gaussian_lic_b200 import mapper
+    raw = _scene(2)
+    poses, cams, _ = _keyframes()
+    imgs = _render(raw, cams)
+    m = mapper.Mapper(W, H, F, F, W / 2.0, H / 2.0, sh_degree=2)
+    m.initialize(raw)
+    m.enable_pose_refinement(LR_T, LR_R)
+    m.add_keyframe(*poses[0], imgs[1])                           # training keyframe 0 at pose 0 with the image of pose 1
+    m.add_keyframe(*poses[0], imgs[1], train=False)              # held-out: the same
+    before = m.evaluate(0, train=True)
+    m.set_pose(0, *poses[1])
+    after = m.evaluate(0, train=True)
+    held = m.evaluate(0, train=False)
+    print("evaluate: PSNR at the given pose %.2f, after set_pose %.2f, held-out %.2f" % (before[0], after[0], held[0]))
+    assert abs(held[0] - before[0]) < 1e-3                       # the held-out keyframe keeps its pose
+    assert after[0] > before[0] + 10
+    m.close()
+    # extend() on the newest keyframe after set_pose selects and initialises what a keyframe given at that pose does
+    rng = np.random.default_rng(4)
+    R1, t1 = poses[1]
+    pc = np.stack([rng.uniform(-1.2, 1.2, 4000), rng.uniform(-0.8, 0.8, 4000), rng.uniform(2.0, 12.0, 4000)], 1)
+    pts = (pc @ np.asarray(R1).T + np.asarray(t1)).astype(np.float32)          # world points in front of pose 1
+    cols = rng.uniform(0, 1, (4000, 3)).astype(np.float32)
+    rsp = rng.uniform(0.5, 2.0, 4000).astype(np.float32)
+    out = []
+    for refined in (True, False):
+        mm = mapper.Mapper(W, H, F, F, W / 2.0, H / 2.0, sh_degree=2)
+        mm.initialize(raw)
+        if refined:
+            mm.enable_pose_refinement(LR_T, LR_R)
+            mm.add_keyframe(*poses[0], imgs[0])
+            mm.set_pose(0, R1, t1)
+        else:
+            mm.add_keyframe(R1, t1, imgs[0])
+        n = mm.extend(pts, cols, rsp)
+        out.append((n, mm.download()))
+        mm.close()
+    print("extend at the refined pose: %d inserted (keyframe given at that pose: %d)" % (out[0][0], out[1][0]))
+    assert out[0][0] == out[1][0] > 0
+    for key in out[0][1]:
+        assert np.array_equal(out[0][1][key], out[1][1][key]), key
+
+
+def test_pose_calls_validate():
+    from gaussian_lic_b200 import capi
+    raw = _scene(0)
+    poses, cams, gts = _keyframes()
+    m = _mapper(raw, poses, gts)
+    with pytest.raises(capi.GlicError):
+        m.pose(0)                                                  # not enabled
+    with pytest.raises(capi.GlicError):
+        m.enable_pose_refinement(float("nan"), 1e-3)
+    m.enable_pose_refinement(LR_T, LR_R)
+    with pytest.raises(capi.GlicError):
+        m.pose(3)
+    bad = np.eye(3) * 1.01
+    with pytest.raises(capi.GlicError):
+        m.set_pose(0, bad, np.zeros(3))
+    with pytest.raises(capi.GlicError):
+        m.set_pose(0, np.diag([1.0, 1.0, -1.0]), np.zeros(3))       # a reflection
+    with pytest.raises(capi.GlicError):
+        m.set_pose(0, np.eye(3), np.array([0.0, np.inf, 0.0]))
+    m.enable_pose_refinement(2e-3, 0.0)                            # rates only
+    R, t = m.pose(1)
+    assert np.array_equal(R, poses[1][0].astype(np.float32))
+    m.close()
+
+
+# ---- two ranks --------------------------------------------------------------------------------------------------------------
+BATCHES_2R = [1, 2, 0, 1, 2, 2]
+
+
+def _pose_run(rank, world, k, exchange=None):
+    raw = _scene(3)
+    poses, cams, gts = _keyframes(seed=31)
+    from test_gpu_mapper_grads import P
+    m = _mapper(raw, poses, gts, capacity=P, rank=rank, world=world, views_per_rank=k)
+    if world > 1:
+        m.connect(exchange(m.export_handle()))
+    m.enable_pose_refinement(LR_T, LR_R)
+    m.optimize(BATCHES_2R)
+    out = dict(state=_state(m), pose=[m.pose(i, camera=True) for i in range(3)], adam=[m.pose_state(i) for i in range(3)])
+    return m, out
+
+
+def _pose_rank_worker(rank, world, port, q):
+    try:
+        import torch.distributed as dist
+        os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
+        dist.init_process_group("gloo", rank=rank, world_size=world)
+        torch.cuda.set_device(rank % torch.cuda.device_count())
+
+        def exchange(mine):
+            got = [None] * world
+            dist.all_gather_object(got, mine)
+            return got
+
+        m, out = _pose_run(rank, world, 1, exchange)
+        dist.barrier()
+        m.close()
+        dist.destroy_process_group()
+        q.put((rank, "ok", out))
+    except Exception as e:          # noqa: BLE001 - reported to the parent
+        import traceback
+        q.put((rank, "%r\n%s" % (e, traceback.format_exc()), None))
+
+
+@pytest.mark.timeout(300)
+def test_two_ranks_pose_replicas_and_one_rank_accumulation():
+    import torch.multiprocessing as mp
+    ctx = mp.get_context("spawn")
+    with socket.socket() as s:
+        s.bind(("127.0.0.1", 0))
+        port = s.getsockname()[1]
+    q = ctx.Queue()
+    procs = [ctx.Process(target=_pose_rank_worker, args=(r, 2, port, q)) for r in range(2)]
+    for p_ in procs:
+        p_.start()
+    res = sorted([q.get(timeout=240) for _ in procs], key=lambda r: r[0])
+    for p_ in procs:
+        p_.join(timeout=30)
+    assert all(r[1] == "ok" for r in res), [r[1] for r in res]
+    a, b = res[0][2], res[1][2]
+    for key in ("p", "m", "v"):
+        for g in GROUPS:
+            assert np.array_equal(a["state"][key][g], b["state"][key][g]), "replicas diverged in %s / %s" % (key, g)
+    for k in range(3):
+        for x, y in zip(a["pose"][k][:2] + a["adam"][k][:2], b["pose"][k][:2] + b["adam"][k][:2]):
+            assert np.array_equal(x.view(np.uint32), y.view(np.uint32)), "replicas diverged in keyframe %d's pose" % k
+        assert np.array_equal(a["pose"][k][2]["view"], b["pose"][k][2]["view"])
+        assert a["adam"][k][2] == b["adam"][k][2]
+    assert [a["adam"][k][2] for k in range(3)] == [1, 2, 2]
+    m, one = _pose_run(0, 1, 2)
+    m.close()
+    worst_r = max(np.abs(a["pose"][k][0].astype(np.float64) - one["pose"][k][0]).max() for k in range(3))
+    worst_t = max(np.abs(a["pose"][k][1].astype(np.float64) - one["pose"][k][1]).max() for k in range(3))
+    print("2 ranks vs 1 rank x 2 views: max |R diff| = %.3e, max |t diff| = %.3e (lr %.0e)" % (worst_r, worst_t, LR_T))
+    for k in range(3):
+        assert one["adam"][k][2] == a["adam"][k][2]
+    assert worst_r <= 0.02 * LR_R and worst_t <= 0.02 * LR_T
