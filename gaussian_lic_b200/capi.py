@@ -71,6 +71,7 @@ def _load():
         "glic_backward": (i32, [i32, i32, i32, vp, vp, f32, vp, vp, vp, C.POINTER(View), vp, i64, vp, vp, vp, vp, vp, f32,
                                 vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "glic_sort_pairs_u64_u32": (i32, [i64, i32, vp, vp, vp, vp, vp, sz, vp]),
+        "glic_debug_sort_pairs_u32": (i32, [i64, i32, vp, vp, vp, vp, vp, vp, sz, vp]),
         "glic_adam_update": (i32, [vp, vp, vp, vp, vp, f32, f32, f32, f32, u32, u32, vp]),
         "glic_fused_ssim": (i32, [i32, i32, i32, i32, f32, f32, vp, vp, vp, vp, vp, vp, vp]),
         "glic_fused_ssim_backward": (i32, [i32, i32, i32, i32, f32, f32, vp, vp, vp, vp, vp, vp, vp, vp]),

@@ -318,8 +318,7 @@ int glic_backward(int P, int sh_degree, int M, const float* means3D, const float
         SampleState smp = SampleState::carve(const_cast<void*>(sample_ws), max_buckets);
         // the sort's ping-pong parity is a pure function of the pass count
         const int T = vp.grid_x * vp.grid_y;
-        const int passes = (tile_sort_bits(T) + 7) / 8;
-        const int cur = passes & 1;
+        const int cur = tile_sort_passes(T) & 1;
         StageTimer _t(GLIC_STAGE_RENDER_BWD, s);
         if (int e = launch_render_backward(P, vp, max_buckets, bin.vals[cur], g, img, smp, dL_dpix, dL_dmeans2D, dL_dconic,
                                            dL_dopacity, dL_dcolors, s)) return e;
@@ -360,8 +359,7 @@ int glic_backward_compact_internal(int P, int sh_degree, int M, const float* mea
         const int64_t max_buckets = glic_max_buckets(R, vp.W, vp.H);
         SampleState smp = SampleState::carve(const_cast<void*>(sample_ws), max_buckets);
         const int T = vp.grid_x * vp.grid_y;
-        const int passes = (tile_sort_bits(T) + 7) / 8;
-        const int cur = passes & 1;
+        const int cur = tile_sort_passes(T) & 1;
         StageTimer _t(GLIC_STAGE_RENDER_BWD, s);
         if (int e = launch_render_backward(P, vp, max_buckets, bin.vals[cur], g, img, smp, dL_dpix, dL_dmeans2D, dL_dconic,
                                            dL_dopacity, dL_dcolors, s)) return e;
@@ -387,6 +385,14 @@ int glic_sort_pairs_u64_u32(int64_t n, int end_bit, uint64_t* keys_in, uint32_t*
         GLIC_CUDA_TRY(cudaMemcpyAsync(vals_out, vals_in, sizeof(uint32_t) * (size_t)n, cudaMemcpyDeviceToDevice, s));
     }
     return GLIC_OK;
+}
+
+int glic_debug_sort_pairs_u32(int64_t n, int end_bit, uint32_t* keys, uint32_t* vals, uint32_t* keys_alt, uint32_t* vals_alt,
+                              const unsigned int* n_dev, void* temp, size_t temp_bytes, void* stream) {
+    if (n < 0 || (n > 0 && (!keys || !vals || !keys_alt || !vals_alt || !temp))) { set_error("debug_sort_pairs_u32: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
+    uint32_t* k[2] = {keys, keys_alt};
+    uint32_t* v[2] = {vals, vals_alt};
+    return launch_sort_pairs32(n, end_bit, k, v, temp, temp_bytes, (cudaStream_t)stream, n_dev, false);
 }
 
 int glic_debug_geom(int P, const void* geom_ws, float* depth, float* xy, float* conic_opacity, float* rgb,

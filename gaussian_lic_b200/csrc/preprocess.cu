@@ -163,11 +163,12 @@ template <bool EMIT>
 GLIC_DI uint32_t block_tile_walk(WalkSmem& w, int n, float mx, float my, float cox, float coy, float coz, float thr, int x0,
                                  int y0, int rw, int grid_x, uint32_t idx, uint32_t off, uint32_t* __restrict__ keys,
                                  uint32_t* __restrict__ vals, SpanStore ss, uint32_t& mask_or_base, uint32_t* s_hist = nullptr,
-                                 uint32_t hi_mask = 0) {
-    // EMIT: every key written also counts into the CTA's two digit histograms of the tile sort (bits [0,8) and [8,..))
+                                 int lo_bits = 8, uint32_t hi_mask = 0) {
+    // EMIT: every key written also counts into the CTA's two digit histograms of the tile sort (bits [0,lo_bits) and
+    // [lo_bits,..))
     auto count_key = [&](uint32_t key) {
-        atomicAdd(&s_hist[key & 255u], 1u);
-        if (hi_mask) atomicAdd(&s_hist[256 + ((key >> 8) & hi_mask)], 1u);
+        atomicAdd(&s_hist[key & ((1u << lo_bits) - 1u)], 1u);
+        if (hi_mask) atomicAdd(&s_hist[256 + ((key >> lo_bits) & hi_mask)], 1u);
     };
     constexpr unsigned FULL = 0xffffffffu;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -627,7 +628,7 @@ depth_scan_kernel(int P, GeomState g, const uint32_t* __restrict__ order, unsign
 // slot range [offsets[idx] - tiles, offsets[idx]); the tile sort's digit histograms are counted on the way.
 __global__ void __launch_bounds__(PRE_THREADS)
 emit_keys_kernel(int P, ViewParams vp, GeomState g, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals, unsigned int capacity,
-                 uint32_t* __restrict__ sort_hist, uint32_t hi_mask) {
+                 uint32_t* __restrict__ sort_hist, int lo_bits, uint32_t hi_mask) {
     __shared__ WalkSmem walk;
     __shared__ uint32_t s_hist[2 * 256];
     for (int i = threadIdx.x; i < 2 * 256; i += PRE_THREADS) s_hist[i] = 0;
@@ -656,7 +657,7 @@ emit_keys_kernel(int P, ViewParams vp, GeomState g, uint32_t* __restrict__ keys,
     }
     const SpanStore ss{g.spans, g.span_cap, &g.hdr->span_count};
     block_tile_walk<true>(walk, skip ? 0 : n, mx, my, cox, coy, coz, thr, x0, y0, rw, vp.grid_x, (uint32_t)idx, off, keys, vals, ss, mask_or_base,
-                          s_hist, hi_mask);
+                          s_hist, lo_bits, hi_mask);
     __syncthreads();
     for (int i = threadIdx.x; i < 2 * 256; i += PRE_THREADS) {
         const uint32_t v = s_hist[i];
@@ -697,8 +698,11 @@ int launch_emit_keys(int P, const ViewParams& vp, GeomState g, uint32_t* tile_ke
                      int end_bit, cudaStream_t s) {
     const unsigned int cap = (unsigned int)std::min<int64_t>(capacity, 0xFFFFFFFFll);
     if (end_bit > 16) { set_error("emit_keys: more than 16 tile bits"); return GLIC_ERR_INVALID_ARGUMENT; }
-    const uint32_t hi_mask = end_bit > 8 ? (1u << (end_bit - 8)) - 1u : 0u;
-    emit_keys_kernel<<<(P + PRE_THREADS - 1) / PRE_THREADS, PRE_THREADS, 0, s>>>(P, vp, g, tile_keys, vals, cap, sort_hist_out, hi_mask);
+    // the sort's digit split: one pass of end_bit bits, or two of sort_pass_bits(end_bit, 0) + sort_pass_bits(end_bit, 1)
+    const int lo_bits = sort_pass_bits(end_bit, 0);
+    const uint32_t hi_mask = sort_passes(end_bit) > 1 ? (1u << sort_pass_bits(end_bit, 1)) - 1u : 0u;
+    emit_keys_kernel<<<(P + PRE_THREADS - 1) / PRE_THREADS, PRE_THREADS, 0, s>>>(P, vp, g, tile_keys, vals, cap, sort_hist_out, lo_bits,
+                                                                                  hi_mask);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }

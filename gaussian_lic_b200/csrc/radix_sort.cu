@@ -4,14 +4,17 @@
 // Replaces cub::DeviceRadixSort::SortPairs(begin_bit = 0, end_bit = 32 + bit) as called at
 // reference rasterizer_impl.cu:417-424 (and the Morton sort of simple_knn.cu:210-213).
 //
-// Structure (8-bit digits, ceil(end_bit/8) passes):
+// Structure (ceil(end_bit/8) passes, the key bits split evenly over them -- sort_pass_bits(): 13 -> 7 + 6, 45 -> 8,8,8,7,7,7 --
+// so that no pass carries digits that cannot occur):
 //   1. one histogram kernel builds the global digit histogram of EVERY pass in a single read of
 //      the keys (8 B/pair);
 //   2. a tiny kernel turns each histogram into exclusive digit offsets;
-//   3. one kernel per pass: each CTA ranks a 4096-pair tile (warp-synchronous ranking, stable: a cascade of `bits`
-//      ballots -- MATCH.ANY measured ~2x slower on passes whose 256 digits are all populated), resolves its global digit offsets with a per-digit decoupled look-back chain over
-//      dynamically ordered CTAs (no second read of the data), stages the tile in shared memory in
-//      sorted order and writes digit runs out coalesced (24 B/pair/pass).
+//   3. one kernel per pass: each CTA loads a 4096-pair tile (keys into registers, values straight into shared memory with
+//      cp.async), counts its digits in shared memory and publishes those counts at once, ranks the tile (warp-synchronous,
+//      stable: a branch-free cascade of one ballot per digit bit, then a leaderless update of the warp's digit counters --
+//      MATCH.ANY measured slower), resolves its global digit
+//      offsets with a per-digit decoupled look-back over dynamically ordered CTAs (no second read of the data), stages the
+//      tile in shared memory in sorted order and writes digit runs out coalesced (24 B/pair/pass).
 // Algorithmic HBM traffic: (8 + 24*passes) B per pair (152 B @ 45 bits).
 #include "common.cuh"
 #include <algorithm>
@@ -19,13 +22,10 @@
 
 namespace glic {
 
-int sort_prepare(int64_t n, int end_bit, void* temp, cudaStream_t s, int digit_bits);
 size_t sort_temp_bytes(int64_t n);
 
 namespace {
 
-constexpr int RADIX_BITS = 8;                          // digit width of the 32-bit-key sorts (and of producer-built histograms)
-constexpr int RADIX = 1 << RADIX_BITS;
 constexpr int RADIX_BITS_MAX = 9;                      // the 64-bit-key sort takes 9-bit digits when that saves a pass (45 bits: 5 instead of 6)
 constexpr int RADIX_MAX = 1 << RADIX_BITS_MAX;
 constexpr int SORT_THREADS = 256;
@@ -40,14 +40,21 @@ constexpr uint32_t FLAG_PREFIX = 2u << 30;
 constexpr uint32_t VALUE_MASK = (1u << 30) - 1;
 
 struct SortTemp {
-    uint32_t* hist;     // [MAX_PASSES][RADIX]  digit histograms -> exclusive offsets
+    uint32_t* hist;     // [MAX_PASSES][1 << max digit bits]  digit histograms -> exclusive offsets
     uint32_t* tickets;  // [MAX_PASSES]
-    uint32_t* status;   // [passes][blocks][RADIX]
+    uint32_t* status;   // per pass p: [blocks][1 << sort_pass_bits(p)], passes packed back to back
 };
 
 __host__ inline int sort_items(int64_t n) { return n < SORT_SMALL_LIMIT ? SORT_ITEMS_SMALL : SORT_ITEMS_BIG; }
 __host__ inline int64_t sort_blocks(int64_t n) { const int64_t tile = (int64_t)SORT_THREADS * sort_items(n); return (n + tile - 1) / tile; }
 __host__ inline int64_t sort_blocks_big(int64_t n) { const int64_t tile = (int64_t)SORT_THREADS * SORT_ITEMS_BIG; return (n + tile - 1) / tile; }
+
+// live digits of all passes together: the status words one CTA needs over the whole sort
+__host__ inline int64_t sort_live_digits(int end_bit, int max_bits) {
+    int64_t d = 0;
+    for (int p = 0; p < sort_passes(end_bit, max_bits); ++p) d += (int64_t)1 << sort_pass_bits(end_bit, p, max_bits);
+    return d;
+}
 
 __host__ inline SortTemp carve_sort_temp(void* temp) {
     char* p = static_cast<char*>(temp);
@@ -66,13 +73,19 @@ __device__ __forceinline__ uint32_t ld_volatile(const uint32_t* p) {
 __device__ __forceinline__ void st_volatile(uint32_t* p, uint32_t v) {
     asm volatile("st.volatile.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
+// 4-byte global -> shared copy that holds no register while in flight (LDGSTS); completed by cp_async_wait_all()
+__device__ __forceinline__ void cp_async4(void* smem_dst, const void* gmem_src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gmem_src)
+                 : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // ---- 1. all-pass histogram --------------------------------------------------------------
 template <typename KeyT, int RB>
 __global__ void __launch_bounds__(256)
 sort_histogram_kernel(const KeyT* __restrict__ keys, int64_t n, const unsigned int* __restrict__ n_dev, int passes, int end_bit,
                       uint32_t* __restrict__ hist) {
-    constexpr int RADIX_BITS = RB, RADIX = 1 << RB;
+    constexpr int RADIX = 1 << RB;
     if (n_dev) n = min(n, (int64_t)*n_dev);
     __shared__ uint32_t sh[MAX_PASSES * RADIX];
     for (int i = threadIdx.x; i < passes * RADIX; i += blockDim.x) sh[i] = 0;
@@ -81,9 +94,8 @@ sort_histogram_kernel(const KeyT* __restrict__ keys, int64_t n, const unsigned i
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
         const KeyT k = keys[i];
         for (int p = 0; p < passes; ++p) {
-            const int shift = p * RADIX_BITS;
-            const int bits = min(RADIX_BITS, end_bit - shift);
-            const uint32_t d = (uint32_t)(k >> shift) & ((1u << bits) - 1u);
+            const int bits = sort_pass_bits(end_bit, p, RB);
+            const uint32_t d = (uint32_t)(k >> sort_pass_shift(end_bit, p, RB)) & ((1u << bits) - 1u);
             atomicAdd(&sh[p * RADIX + d], 1u);
         }
     }
@@ -94,10 +106,10 @@ sort_histogram_kernel(const KeyT* __restrict__ keys, int64_t n, const unsigned i
     }
 }
 
-// ---- 2. exclusive scan of each pass's 256 bins --------------------------------------------
+// ---- 2. exclusive scan of each pass's bins --------------------------------------------
 __global__ void __launch_bounds__(RADIX_MAX) sort_scan_hist_kernel(uint32_t* __restrict__ hist) {
     __shared__ uint32_t warp_tot[RADIX_MAX / 32];
-    uint32_t* h = hist + blockIdx.x * blockDim.x;          // blockDim.x = bins of this sort's digit
+    uint32_t* h = hist + blockIdx.x * blockDim.x;          // blockDim.x = bins of this sort's widest digit
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t v = h[tid];
     uint32_t incl = v;
@@ -121,14 +133,17 @@ struct __align__(16) PassSmem {
     KeyT keys[SORT_TILE];
     uint32_t vals[SORT_TILE];
     uint32_t warp_cnt[SORT_WARPS][RADIX];
+    uint32_t tile_cnt[RADIX];
     uint32_t digit_excl[RADIX];
     uint32_t global_base[RADIX];
     uint32_t warp_tot[SORT_WARPS];
     uint32_t block_id;
 };
 
+// RB: widest digit the kernel is built for (8, or 9 for the opt-in 64-bit variant); `bits` <= RB: this pass's digit width.
+// Only the 1 << bits live digits are counted, published and looked back on; `status` holds [blocks][1 << bits] words.
 template <typename KeyT, int SORT_ITEMS, int RB>
-__global__ void __launch_bounds__(SORT_THREADS, SORT_ITEMS <= 4 ? 6 : (sizeof(KeyT) == 4 ? 5 : 3))
+__global__ void __launch_bounds__(SORT_THREADS, SORT_ITEMS <= 4 ? 6 : (sizeof(KeyT) == 4 ? 4 : 3))
 onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restrict__ vals_in,
                      KeyT* __restrict__ keys_out, uint32_t* __restrict__ vals_out, int64_t n, const unsigned int* __restrict__ n_dev,
                      int shift, int bits, const uint32_t* __restrict__ digit_base, uint32_t* __restrict__ status,
@@ -136,13 +151,15 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr int SORT_TILE = SORT_THREADS * SORT_ITEMS;
     constexpr int RADIX_BITS = RB, RADIX = 1 << RB;
-    constexpr int DPT = RADIX / SORT_THREADS;               // digits owned by one thread in the per-digit phase (1 or 2)
+    constexpr int DPT = RADIX > SORT_THREADS ? RADIX / SORT_THREADS : 1;   // digits owned by one thread in the per-digit phase
     PassSmem<KeyT, SORT_ITEMS, RB>& sm = *reinterpret_cast<PassSmem<KeyT, SORT_ITEMS, RB>*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t dmask = (1u << bits) - 1u;
+    const int nd = 1 << bits;                               // live digits of this pass
+    const uint32_t dmask = (uint32_t)nd - 1u;
 
     if (tid == 0) sm.block_id = atomicAdd(ticket, 1u);
     for (int i = tid; i < SORT_WARPS * RADIX; i += SORT_THREADS) (&sm.warp_cnt[0][0])[i] = 0;
+    for (int i = tid; i < RADIX; i += SORT_THREADS) sm.tile_cnt[i] = 0;
     __syncthreads();
     if (n_dev) n = min(n, (int64_t)*n_dev);   // capacity-sized launch: the true count lives on the device
     const int64_t block = sm.block_id;
@@ -150,15 +167,30 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
     if (tile_base >= n) return;                 // (CTA-uniform) nothing for this ticket
     const int count = (int)min((int64_t)SORT_TILE, n - tile_base);
 
-    // -- load (warp-striped: lane l, item j <-> element warp*512 + j*32 + l; order-preserving)
+    // -- load keys (warp-striped: lane l, item j <-> element warp*512 + j*32 + l; order-preserving) and count the tile's
+    //    digits; the values travel to shared memory (tile order) asynchronously meanwhile, in no register
     KeyT k[SORT_ITEMS];
     uint32_t rank[SORT_ITEMS];
     const int wbase = warp * (32 * SORT_ITEMS);
 #pragma unroll
     for (int j = 0; j < SORT_ITEMS; ++j) {
         const int li = wbase + j * 32 + lane;
+        if (li < count) cp_async4(&sm.vals[li], vals_in + tile_base + li);
         k[j] = li < count ? keys_in[tile_base + li] : (KeyT)~(KeyT)0;
     }
+#pragma unroll
+    for (int j = 0; j < SORT_ITEMS; ++j)
+        if (wbase + j * 32 + lane < count) atomicAdd(&sm.tile_cnt[(uint32_t)(k[j] >> shift) & dmask], 1u);
+    __syncthreads();
+    // -- publish the tile's digit counts before ranking it: successors' look-backs need not wait for this CTA's ranking
+    uint32_t tot[DPT];
+#pragma unroll
+    for (int e = 0; e < DPT; ++e) {
+        const int d = tid * DPT + e;
+        tot[e] = d < nd ? sm.tile_cnt[d] : 0u;
+        if (d < nd) st_volatile(status + (size_t)block * nd + d, (block == 0 ? FLAG_PREFIX : FLAG_AGG) | tot[e]);
+    }
+
     // -- stable rank inside the warp's digit streams
     const uint32_t lt_mask = (1u << lane) - 1u;
 #pragma unroll
@@ -168,50 +200,45 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
         const uint32_t d = (uint32_t)(k[j] >> shift) & dmask;
         const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
         uint32_t r = 0;
+        // peers from RB ballots, with no branch on `bits` (the bits past it are clear in every d and change nothing): the
+        // branch-free cascade measured faster than skipping the dead ballots.  Cost is independent of the digit
+        // distribution; MATCH.ANY measured ~1.35x slower per pass on H100
         uint32_t bpeers = vmask;
-        {   // peers from `bits` ballots: cost independent of the digit distribution (MATCH.ANY stalls longer on
-            // passes whose 256 digits are all populated)
 #pragma unroll
-            for (int b = 0; b < RADIX_BITS; ++b) {
-                if (b < bits) {
-                    const bool bit = (d >> b) & 1u;
-                    const uint32_t bal = __ballot_sync(0xffffffffu, bit && valid);
-                    bpeers &= bit ? bal : ~bal;
-                }
-            }
+        for (int b = 0; b < RADIX_BITS; ++b) {
+            const bool bit = (d >> b) & 1u;
+            const uint32_t bal = __ballot_sync(0xffffffffu, bit && valid);
+            bpeers &= bit ? bal : ~bal;
         }
+        // every peer reads its digit's running count and writes back the same new value: no leader election, no shuffle,
+        // no divergent branch in the per-item chain
+        const uint32_t c = sm.warp_cnt[warp][d];
+        __syncwarp();
         if (valid) {
-            const uint32_t peers = bpeers;
-            const int leader = __ffs(peers) - 1;
-            uint32_t c = 0;
-            if (lane == leader) {
-                c = sm.warp_cnt[warp][d];
-                sm.warp_cnt[warp][d] = c + __popc(peers);
-            }
-            c = __shfl_sync(peers, c, leader);
-            r = c + __popc(peers & lt_mask);
+            sm.warp_cnt[warp][d] = c + __popc(bpeers);
+            r = c + __popc(bpeers & lt_mask);
         }
         rank[j] = r;
         __syncwarp();
     }
     __syncthreads();
 
-    // -- per digit (thread t owns digits t*DPT .. t*DPT + DPT-1): warp bases, CTA total, look-back
+    // -- per digit (thread t owns digits t*DPT .. t*DPT + DPT-1): warp bases, CTA-local placement, look-back
     {
-        uint32_t tot[DPT];
         uint32_t mine = 0;
 #pragma unroll
         for (int e = 0; e < DPT; ++e) {
             const int d = tid * DPT + e;
-            uint32_t t = 0;
+            if (d < nd) {
+                uint32_t t = 0;
 #pragma unroll
-            for (int w = 0; w < SORT_WARPS; ++w) {
-                const uint32_t c = sm.warp_cnt[w][d];
-                sm.warp_cnt[w][d] = t;
-                t += c;
+                for (int w = 0; w < SORT_WARPS; ++w) {
+                    const uint32_t c = sm.warp_cnt[w][d];
+                    sm.warp_cnt[w][d] = t;
+                    t += c;
+                }
             }
-            tot[e] = t;
-            mine += t;
+            mine += tot[e];
         }
         // CTA-local exclusive scan over digits (placement inside the staged tile)
         uint32_t incl = mine;
@@ -228,18 +255,15 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
 #pragma unroll
         for (int e = 0; e < DPT; ++e) {
             const int d = tid * DPT + e;
+            if (d >= nd) break;
             sm.digit_excl[d] = excl;
-            // decoupled look-back for this digit
-            uint32_t* my = status + (size_t)block * RADIX + d;
+            // decoupled look-back for this digit (its aggregate went out before the ranking)
             uint32_t prev = 0;
-            if (block == 0) {
-                st_volatile(my, FLAG_PREFIX | tot[e]);
-            } else {
-                st_volatile(my, FLAG_AGG | tot[e]);
+            if (block > 0) {
                 int64_t b = block - 1;
                 unsigned spins = 0;
                 while (true) {
-                    const uint32_t s = ld_volatile(status + (size_t)b * RADIX + d);
+                    const uint32_t s = ld_volatile(status + (size_t)b * nd + d);
                     const uint32_t f = s & ~VALUE_MASK;
                     if (f == 0) {
                         if (++spins > (1u << 26)) __trap();   // fail loudly rather than hang the GPU
@@ -249,7 +273,7 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
                     if (f == FLAG_PREFIX) break;
                     --b;
                 }
-                st_volatile(my, FLAG_PREFIX | (prev + tot[e]));
+                st_volatile(status + (size_t)block * nd + d, FLAG_PREFIX | (prev + tot[e]));
             }
             sm.global_base[d] = digit_base[d] + prev - excl;
             excl += tot[e];
@@ -257,26 +281,42 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
     }
     __syncthreads();
 
-    // -- stage the tile in sorted order
+    // -- stage the tile in sorted order: keys straight from registers (their ranks become positions), then the values,
+    //    which sit in the same buffer in tile order, through registers
 #pragma unroll
     for (int j = 0; j < SORT_ITEMS; ++j) {
         const int li = wbase + j * 32 + lane;
         if (li < count) {
             const uint32_t d = (uint32_t)(k[j] >> shift) & dmask;
-            const uint32_t pos = sm.digit_excl[d] + sm.warp_cnt[warp][d] + rank[j];
-            sm.keys[pos] = k[j];
-            sm.vals[pos] = vals_in[tile_base + li];
+            rank[j] += sm.digit_excl[d] + sm.warp_cnt[warp][d];
+            sm.keys[rank[j]] = k[j];
         }
     }
+    cp_async_wait_all();
+    __syncthreads();
+    uint32_t v[SORT_ITEMS];
+#pragma unroll
+    for (int j = 0; j < SORT_ITEMS; ++j) {
+        const int li = wbase + j * 32 + lane;
+        v[j] = li < count ? sm.vals[li] : 0u;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < SORT_ITEMS; ++j)
+        if (wbase + j * 32 + lane < count) sm.vals[rank[j]] = v[j];
     __syncthreads();
 
     // -- coalesced write-out of digit runs
-    for (int i = tid; i < count; i += SORT_THREADS) {
-        const KeyT key = sm.keys[i];
-        const uint32_t d = (uint32_t)(key >> shift) & dmask;
-        const size_t dst = (size_t)sm.global_base[d] + i;
-        keys_out[dst] = key;
-        vals_out[dst] = sm.vals[i];
+#pragma unroll
+    for (int j = 0; j < SORT_ITEMS; ++j) {
+        const int i = j * SORT_THREADS + tid;
+        if (i < count) {
+            const KeyT key = sm.keys[i];
+            const uint32_t d = (uint32_t)(key >> shift) & dmask;
+            const size_t dst = (size_t)sm.global_base[d] + i;
+            keys_out[dst] = key;
+            vals_out[dst] = sm.vals[i];
+        }
     }
 }
 
@@ -285,8 +325,7 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
 // zeroes the histograms, tickets and look-back status words of a sort of n pairs on bits [0, end_bit)
 int sort_prepare(int64_t n, int end_bit, void* temp, cudaStream_t s, int digit_bits) {
     if (n <= 0) return GLIC_OK;
-    const int passes = (end_bit + digit_bits - 1) / digit_bits;
-    const size_t used = sizeof(uint32_t) * (MAX_PASSES * RADIX_MAX + 32 + (size_t)passes * sort_blocks(n) * ((size_t)1 << digit_bits));
+    const size_t used = sizeof(uint32_t) * (MAX_PASSES * RADIX_MAX + 32 + (size_t)sort_blocks(n) * sort_live_digits(end_bit, digit_bits));
     GLIC_CUDA_TRY(cudaMemsetAsync(temp, 0, used, s));
     return GLIC_OK;
 }
@@ -308,31 +347,33 @@ static int run_passes(int64_t n, int passes, int end_bit, int64_t blocks, KeyT* 
                                            (int)sizeof(PassSmem<KeyT, ITEMS, RB>)));
     }
     int cur = 0;
+    uint32_t* status = t.status;
     for (int p = 0; p < passes; ++p) {
-        const int shift = p * RB;
-        const int bits = min(RB, end_bit - shift);
+        const int bits = sort_pass_bits(end_bit, p, RB);
         onesweep_pass_kernel<KeyT, ITEMS, RB><<<(unsigned)blocks, SORT_THREADS, sizeof(PassSmem<KeyT, ITEMS, RB>), s>>>(
-            keys[cur], vals[cur], keys[cur ^ 1], vals[cur ^ 1], n, n_dev, shift, bits, t.hist + p * BINS,
-            t.status + (size_t)p * blocks * BINS, t.tickets + p);
+            keys[cur], vals[cur], keys[cur ^ 1], vals[cur ^ 1], n, n_dev, sort_pass_shift(end_bit, p, RB), bits, t.hist + p * BINS,
+            status, t.tickets + p);
         GLIC_LAUNCH_CHECK();
+        status += (size_t)blocks << bits;     // each pass's status words cover its live digits only
         cur ^= 1;
     }
     return cur;
 }
 
-// Digit width of a sort.  The pass kernel is generic (8- or 9-bit digits; GLIC_SORT_DIGIT_BITS=9 selects the wider one for
-// 64-bit keys when it saves a pass), but 8 stays the default: a pass is bound by the warp-synchronous ranking (one ballot per
-// digit bit and item) and by the per-digit look-back, not by its 24 B/pair of HBM traffic, so a wider digit costs more than
-// the saved pass returns.
+// Widest digit of a sort.  The pass kernel is generic (up to 8- or 9-bit digits; GLIC_SORT_DIGIT_BITS=9 selects the wider
+// one for 64-bit keys when it saves a pass), but 8 stays the default: a pass is bound by the warp-synchronous ranking (one
+// ballot per digit bit and item), not by its 24 B/pair of HBM traffic, so a wider digit costs more than the saved pass
+// returns.
 template <typename KeyT>
 static inline int sort_digit_bits(int end_bit) {
     static const int want = getenv("GLIC_SORT_DIGIT_BITS") ? atoi(getenv("GLIC_SORT_DIGIT_BITS")) : 8;
-    if (want == 9 && sizeof(KeyT) == 8 && (end_bit + 8) / 9 < (end_bit + 7) / 8) return 9;
+    if (want == 9 && sizeof(KeyT) == 8 && sort_passes(end_bit, 9) < sort_passes(end_bit, 8)) return 9;
     return 8;
 }
 
 // hist_ready: the caller zeroed the temp block with sort_prepare() and a producer kernel already accumulated the digit
-// histograms of every pass into sort_hist(temp) (8-bit digits): the histogram kernel -- one more read of all keys -- is skipped.
+// histograms of every pass into sort_hist(temp) (digits of sort_pass_bits(end_bit, p)): the histogram kernel -- one more
+// read of all keys -- is skipped.
 template <typename KeyT>
 static int launch_sort_pairs_t(int64_t n, int end_bit, KeyT* keys[2], uint32_t* vals[2], void* temp, size_t temp_bytes,
                                cudaStream_t s, const unsigned int* n_dev = nullptr, bool hist_ready = false) {
@@ -340,7 +381,7 @@ static int launch_sort_pairs_t(int64_t n, int end_bit, KeyT* keys[2], uint32_t* 
     if (n >= (int64_t)VALUE_MASK) { set_error("sort: n too large"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (n <= 0) return 0;
     const int rb = hist_ready ? 8 : sort_digit_bits<KeyT>(end_bit);
-    const int passes = (end_bit + rb - 1) / rb;
+    const int passes = sort_passes(end_bit, rb);
     if (passes > MAX_PASSES) { set_error("sort: too many passes"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (temp_bytes < sort_temp_bytes(n)) { set_error("sort: temp too small"); return GLIC_ERR_WORKSPACE; }
     const int64_t blocks = sort_blocks(n);

@@ -158,6 +158,13 @@ GLIC_API size_t glic_sort_temp_bytes(int64_t n);
 GLIC_API int glic_sort_pairs_u64_u32(int64_t n, int end_bit, uint64_t* keys_in, uint32_t* vals_in,
                             uint64_t* keys_out, uint32_t* vals_out, void* temp, size_t temp_bytes,
                             void* stream);
+/* Test hook: the 32-bit-key sort of the binning (depth keys, tile ids) on key bits [0, end_bit), ping-ponging between
+ * (keys, vals) and (keys_alt, vals_alt).  n_dev (optional, device memory): the true count <= n; the kernels are launched
+ * for n, as the forward launches its capacity-sized tile sort.  Returns 0/1 = which pair holds the result (1: the _alt
+ * pair), < 0 on error. */
+GLIC_API int glic_debug_sort_pairs_u32(int64_t n, int end_bit, uint32_t* keys, uint32_t* vals, uint32_t* keys_alt,
+                                       uint32_t* vals_alt, const unsigned int* n_dev, void* temp, size_t temp_bytes,
+                                       void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Visibility-masked Adam.  Replaces ADAM::adamUpdate (rasterizer/cuda_rasterizer/adam.cu:9-67,
