@@ -280,6 +280,19 @@ struct CompactGrads {
 // doubles of the pose-gradient scratch for up to Pcap Gaussians
 size_t pose_partials_count(uint32_t Pcap);
 
+// out[j] = the G per-CTA float64 partials [G][N] summed in a fixed order (no atomics: two runs give the same bits).  One CTA of
+// N warps, <<<1, 32 * N>>>: warp j sums component j lane-strided, then an xor butterfly.
+template <int N>
+__global__ void __launch_bounds__(32 * N)
+partials_finish_kernel(unsigned G, const double* __restrict__ partials, float* __restrict__ out) {
+    const int j = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double s = 0.0;
+    for (unsigned b = lane; b < G; b += 32) s += partials[N * (size_t)b + j];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) out[j] = (float)s;
+}
+
 // ---- stage launchers (defined in the .cu files) ------------------------------------------
 int launch_preprocess_forward(int P, int D, int M, const float* means, const float* scales, float mod,
                               const float* rots, const float* opac, const float* dc, const float* sh,
@@ -328,11 +341,10 @@ extern "C" int glic_backward_compact_internal(int P, int sh_degree, int M, const
                                               void* after_render_event, void* stream);
 namespace glic {
 int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, float* exp_avg, float* exp_avg_sq, const float* g_geo,
-                        uint32_t Pcap_geo, const float* lr6, const float* g_color, const uint8_t* flags, const float* campos4,
+                        uint32_t Pcap_geo, const float* lr6, const float* g_color, const uint8_t* flags, const float* const* campos_dev,
                         int n_slots, float grad_scale, float color_scale, float b1, float b2, float eps, const unsigned int* skip_flag,
-                        unsigned int* visible_count, cudaStream_t s, const float* const* campos_dev = nullptr);
-// campos_dev (optional, n_slots host-held device pointers): each slot's camera centre is read on the device from there
-// (campos4 is then unused)
+                        unsigned int* visible_count, cudaStream_t s);
+// campos_dev: n_slots host-held device pointers, each slot's camera centre (read on the device)
 int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flags, cudaStream_t s);
 // per-keyframe exposure (ssim.cu): one Adam step of every keyframe of a batch of S <= EXPO_MAX_SLOTS slots; slot_grads[S][12]
 constexpr int EXPO_MAX_SLOTS = 32;

@@ -14,11 +14,15 @@
 //     the 11 geometric floats are mean-reduced in place by the two-shot kernel of p2p.cu; every replica then runs the same
 //     Adam launch on the same bytes.
 #include "common.cuh"
+#include "adam_math.cuh"
 
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <initializer_list>
+#include <nv/target>
 #include <random>
+#include <utility>
 #include <vector>
 
 using namespace glic;
@@ -49,34 +53,56 @@ void proj_matrix(int W, int H, double fx, double fy, double cx, double cy, float
     fov2[0] = fovx; fov2[1] = fovy;
 }
 
-// camera.h:38-110 in closed form: FoV from the intrinsics (float members), world->view matrix Rt, projection P, both handed
-// to the kernels transposed (column-major), camera centre = -R_cw^T t_cw, the asymmetric clamp limits of :63-66.
-// Compiled for x86-64 without FMA, every operation below is one IEEE double / float operation: pose_step_kernel repeats the
-// pose-dependent part on the device bit for bit (cam_rebuild), so keep the two in step.
-void camera_block(int W, int H, double fx, double fy, double cx, double cy, const float* R_wc, const float* t_wc, CamBlock& o) {
+// One IEEE double / float operation each, on the device and on the host alike: the _rn intrinsics keep nvcc from contracting
+// them into FMAs, and x86-64 host code is compiled without FMA.
+__host__ __device__ inline double dmul(double a, double b) { NV_IF_ELSE_TARGET(NV_IS_DEVICE, (return __dmul_rn(a, b);), (return a * b;)) }
+__host__ __device__ inline double dadd(double a, double b) { NV_IF_ELSE_TARGET(NV_IS_DEVICE, (return __dadd_rn(a, b);), (return a + b;)) }
+__host__ __device__ inline float fmul(float a, float b) { NV_IF_ELSE_TARGET(NV_IS_DEVICE, (return __fmul_rn(a, b);), (return a * b;)) }
+__host__ __device__ inline float fadd(float a, float b) { NV_IF_ELSE_TARGET(NV_IS_DEVICE, (return __fadd_rn(a, b);), (return a + b;)) }
+__host__ __device__ inline float d2f(double a) { NV_IF_ELSE_TARGET(NV_IS_DEVICE, (return __double2float_rn(a);), (return (float)a;)) }
+
+// The pose-dependent part of camera.h:38-110 from a float pose: the world->view matrix Rt and the full projection P Rt, both
+// handed to the kernels transposed (column-major), and the camera centre -R_cw^T t_cw, into cam36 = view16 | proj16 | campos4;
+// T12 (optional) = the float64 T_cw = R_cw (row-major) | t_cw they are formed from.  The host (camera_block) and the pose step
+// on the device both build the block here, so a refined keyframe's block equals glic_camera_block of its float pose bit for bit.
+__host__ __device__ void pose_camera(const float* R_wc, const float* t_wc, const float* Pm, float* cam36, double* T12) {
     double Rcw[9], tcw[3];
     for (int i = 0; i < 3; ++i)
         for (int j = 0; j < 3; ++j) Rcw[3 * i + j] = (double)R_wc[3 * j + i];
-    for (int i = 0; i < 3; ++i) tcw[i] = -(Rcw[3 * i] * t_wc[0] + Rcw[3 * i + 1] * t_wc[1] + Rcw[3 * i + 2] * t_wc[2]);
-    float Rt[16] = {0};
-    for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) Rt[4 * i + j] = (float)Rcw[3 * i + j]; Rt[4 * i + 3] = (float)tcw[i]; }
+    for (int i = 0; i < 3; ++i)
+        tcw[i] = -dadd(dadd(dmul(Rcw[3 * i], (double)t_wc[0]), dmul(Rcw[3 * i + 1], (double)t_wc[1])), dmul(Rcw[3 * i + 2], (double)t_wc[2]));
+    float Rt[16];
+    for (int e = 0; e < 16; ++e) Rt[e] = 0.0f;
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) Rt[4 * i + j] = d2f(Rcw[3 * i + j]);
+        Rt[4 * i + 3] = d2f(tcw[i]);
+    }
     Rt[15] = 1.0f;
-    float Pm[16], fov2[2];
-    proj_matrix(W, H, fx, fy, cx, cy, Pm, fov2);
-    const float fovx = fov2[0], fovy = fov2[1];
-    float full[16];
     for (int i = 0; i < 4; ++i)
         for (int j = 0; j < 4; ++j) {
             float acc = 0.f;
-            for (int k = 0; k < 4; ++k) acc += Pm[4 * i + k] * Rt[4 * k + j];
-            full[4 * i + j] = acc;
+            for (int k = 0; k < 4; ++k) acc = fadd(acc, fmul(Pm[4 * i + k], Rt[4 * k + j]));
+            cam36[16 + 4 * j + i] = acc;                                   // proj, column-major
         }
     for (int r = 0; r < 4; ++r)
-        for (int c = 0; c < 4; ++c) { o.view[4 * c + r] = Rt[4 * r + c]; o.proj[4 * c + r] = full[4 * r + c]; }
-    for (int i = 0; i < 3; ++i) o.campos[i] = (float)(-(Rcw[i] * tcw[0] + Rcw[3 + i] * tcw[1] + Rcw[6 + i] * tcw[2]));
-    o.campos[3] = 0.f;
-    o.tanfovx = std::tan(fovx * 0.5f);
-    o.tanfovy = std::tan(fovy * 0.5f);
+        for (int c = 0; c < 4; ++c) cam36[4 * c + r] = Rt[4 * r + c];      // view, column-major
+    for (int i = 0; i < 3; ++i)
+        cam36[32 + i] = d2f(-dadd(dadd(dmul(Rcw[i], tcw[0]), dmul(Rcw[3 + i], tcw[1])), dmul(Rcw[6 + i], tcw[2])));
+    cam36[35] = 0.f;
+    if (T12) {
+        for (int e = 0; e < 9; ++e) T12[e] = Rcw[e];
+        for (int i = 0; i < 3; ++i) T12[9 + i] = tcw[i];
+    }
+}
+
+// camera.h:38-110 in closed form: FoV from the intrinsics (float members), pose_camera, the asymmetric clamp limits of :63-66
+void camera_block(int W, int H, double fx, double fy, double cx, double cy, const float* R_wc, const float* t_wc, CamBlock& o,
+                  double* T12 = nullptr) {
+    float Pm[16], fov2[2];
+    proj_matrix(W, H, fx, fy, cx, cy, Pm, fov2);
+    pose_camera(R_wc, t_wc, Pm, o.view, T12);                         // view | proj | campos are contiguous
+    o.tanfovx = std::tan(fov2[0] * 0.5f);
+    o.tanfovy = std::tan(fov2[1] * 0.5f);
     const float ffx = (float)fx, ffy = (float)fy, fcx = (float)cx, fcy = (float)cy;
     o.lim[0] = -0.15f * W / ffx - fcx / ffx; o.lim[1] = 1.15f * W / ffx - fcx / ffx;
     o.lim[2] = -0.15f * H / ffy - fcy / ffy; o.lim[3] = 1.15f * H / ffy - fcy / ffy;
@@ -96,7 +122,7 @@ inline uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
 // Keyframe k's pose is T_cw = [R_cw | t_cw] (float64 master, R_cw row-major), perturbed as Exp(delta) T_cw with
 // delta = (rho, omega) in the camera frame.  Each step: torch::optim::Adam on the 6-vector (as the exposure step), then
 // T_cw <- Exp(u) T_cw, the float pose (R_wc = R_cw^T, t_wc = -R_cw^T t_cw) re-derived from it, and the device camera block
-// (view16 | proj16 | campos4) rebuilt from those floats exactly as camera_block() does.
+// (view16 | proj16 | campos4) rebuilt from those floats by pose_camera.
 
 // SE(3) exponential of u = (rho, omega): R = I + A K + B K^2, V = I + B K + C K^2, K = [omega]_x; t = V rho
 __device__ void se3_exp(const double u[6], double R[9], double t[3]) {
@@ -126,71 +152,30 @@ __device__ void se3_exp(const double u[6], double R[9], double t[3]) {
     for (int i = 0; i < 3; ++i) t[i] = V[3 * i] * u[0] + V[3 * i + 1] * u[1] + V[3 * i + 2] * u[2];
 }
 
-// camera_block()'s pose-dependent part, operation for operation (no contraction): view16 | proj16 | campos4 from the float pose
-__device__ void cam_rebuild(const float* R_wc, const float* t_wc, const float* Pm, float* out36) {
-    double Rcw[9], tcw[3];
-    for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 3; ++j) Rcw[3 * i + j] = (double)R_wc[3 * j + i];
-    for (int i = 0; i < 3; ++i)
-        tcw[i] = -__dadd_rn(__dadd_rn(__dmul_rn(Rcw[3 * i], (double)t_wc[0]), __dmul_rn(Rcw[3 * i + 1], (double)t_wc[1])),
-                            __dmul_rn(Rcw[3 * i + 2], (double)t_wc[2]));
-    float Rt[16];
-    for (int e = 0; e < 16; ++e) Rt[e] = 0.0f;
-    for (int i = 0; i < 3; ++i) {
-        for (int j = 0; j < 3; ++j) Rt[4 * i + j] = __double2float_rn(Rcw[3 * i + j]);
-        Rt[4 * i + 3] = __double2float_rn(tcw[i]);
-    }
-    Rt[15] = 1.0f;
-    for (int i = 0; i < 4; ++i)
-        for (int j = 0; j < 4; ++j) {
-            float acc = 0.f;
-            for (int k = 0; k < 4; ++k) acc = __fadd_rn(acc, __fmul_rn(Pm[4 * i + k], Rt[4 * k + j]));
-            out36[16 + 4 * j + i] = acc;                                   // proj, column-major
-        }
-    for (int r = 0; r < 4; ++r)
-        for (int c = 0; c < 4; ++c) out36[4 * c + r] = Rt[4 * r + c];      // view, column-major
-    for (int i = 0; i < 3; ++i)
-        out36[32 + i] = __double2float_rn(-__dadd_rn(__dadd_rn(__dmul_rn(Rcw[i], tcw[0]), __dmul_rn(Rcw[3 + i], tcw[1])),
-                                                     __dmul_rn(Rcw[6 + i], tcw[2])));
-    out36[35] = 0.f;
-}
-
 struct PoseBatch {
     int kf[MAX_SLOTS];                // keyframe of each slot
     float* cam[MAX_SLOTS];            // its device camera block
     float Pm[16];                     // the pose-independent projection (row-major)
 };
 
-// One thread per slot; the first slot that holds a keyframe steps it with g = (1/S) * sum over the slots holding it (slot
-// order, float64) of the slot's dL/d(rho, omega), by exposure_adam_kernel's arithmetic.  A set overflow word leaves the pose,
-// m, v and t unchanged; an update of exactly zero leaves the pose and its camera block unchanged.
+// One thread per slot; the first slot that holds a keyframe steps it with the batch gradient of keyframe_batch_grad and
+// torch_adam_delta, as the exposure step does.  A set overflow word leaves the pose, m, v and t unchanged; an update of
+// exactly zero leaves the pose and its camera block unchanged.
 __global__ void __launch_bounds__(MAX_SLOTS)
 pose_step_kernel(int S, PoseBatch b, const float* __restrict__ slot_grads /* [S][8] */, double* __restrict__ T /* [kf][12] */,
                  float* __restrict__ pose_f /* [kf][12] */, float* __restrict__ m, float* __restrict__ v, int* __restrict__ t,
                  float lr_rho, float lr_omega, const unsigned int* __restrict__ skip) {
     if (*skip) return;
     const int s = threadIdx.x;
-    if (s >= S) return;
+    if (s >= S || !first_slot_of_keyframe(b.kf, s)) return;
     const int kf = b.kf[s];
-    for (int q = 0; q < s; ++q) if (b.kf[q] == kf) return;
     const int step = t[kf] + 1;
-    const float b1 = 0.9f, b2 = 0.999f, eps = 1e-8f;
-    const double bc1 = 1.0 - pow(0.9, (double)step), bc2 = 1.0 - pow(0.999, (double)step);
     double u[6];
     bool moved = false;
     for (int j = 0; j < 6; ++j) {
-        double acc = 0.0;
-        for (int q = s; q < S; ++q)
-            if (b.kf[q] == kf) acc += (double)slot_grads[8 * q + j];
-        const float g = (float)(acc / (double)S);
+        const float g = keyframe_batch_grad(b.kf, S, s, slot_grads, 8, j);
         const size_t i = 6 * (size_t)kf + j;
-        const float m1 = fmaf(1.0f - b1, g, __fmul_rn(b1, m[i]));
-        const float v1 = fmaf(1.0f - b2, __fmul_rn(g, g), __fmul_rn(b2, v[i]));
-        const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v1), (float)sqrt(bc2)), eps);
-        const float step_size = (float)((double)(j < 3 ? lr_rho : lr_omega) / bc1);
-        const float uj = __fmul_rn(-step_size, __fdiv_rn(m1, denom));
-        m[i] = m1;
-        v[i] = v1;
+        const float uj = torch_adam_delta(g, m[i], v[i], j < 3 ? lr_rho : lr_omega, step);
         u[j] = (double)uj;
         moved |= uj != 0.0f;
     }
@@ -211,8 +196,18 @@ pose_step_kernel(int S, PoseBatch b, const float* __restrict__ slot_grads /* [S]
         for (int j = 0; j < 3; ++j) f[3 * i + j] = (float)Rn[3 * j + i];
         f[9 + i] = (float)(-(Rn[i] * tn[0] + Rn[3 + i] * tn[1] + Rn[6 + i] * tn[2]));
     }
-    cam_rebuild(f, f + 9, b.Pm, b.cam[s]);
+    pose_camera(f, f + 9, b.Pm, b.cam[s], nullptr);
 }
+
+// Regions of the exchange block that hold one slot per (parity, view slot), in layout order
+enum SlotRegion { COLOUR, FLAGS, EXPOSURE, POSE, N_REGIONS };
+
+// Adam state of a per-training-keyframe parameter of `width` floats: moments [cap][width], step counts [cap]
+struct KeyframeAdam {
+    int width;
+    float *m = nullptr, *v = nullptr;
+    int* t = nullptr;
+};
 
 }  // namespace
 
@@ -227,9 +222,8 @@ struct glic_mapper {
     int* radii = nullptr;
     float *g_mean2D = nullptr, *g_conic = nullptr, *g_opacity = nullptr;
     void* geom_ws = nullptr; size_t geom_bytes = 0;
-    // ---- exchange block: geo[11*Pcap + 4] | flags words | colour slots [2][S][Pcap][3] | flag bytes [2][S][Pcap] |
-    //      exposure gradient slots [2][S][12] | pose gradient slots [2][S][8] (dL/d(rho, omega), 2 unused) ----
-    char* xblock = nullptr; size_t xbytes = 0, off_col = 0, off_flags = 0, off_expo = 0, off_pose = 0;
+    // ---- exchange block: geo[11*Pcap + 4] | flags words | one region [2][S] of slots per SlotRegion (xblock_layout) ----
+    char* xblock = nullptr; size_t xbytes = 0, slot_off[N_REGIONS] = {}, slot_bytes[N_REGIONS] = {};
     size_t n_geo = 0;                // floats in the reduced region (11*Pcap + 4; the tail holds the collective overflow word)
     void* peers[8] = {nullptr};
     bool connected = false;
@@ -250,19 +244,19 @@ struct glic_mapper {
     uint64_t view_counter = 0;
     glic_mapper_stats st{};
     bool run_optimizer = true;            // GLIC_MAPPER_OPT_OPTIMIZER (benchmarks time the rasterization step alone with it off)
-    // ---- per-training-keyframe exposure (glic_mapper_enable_exposure): E, Adam moments [expo_cap][12], step counts ----
+    // ---- per-training-keyframe exposure (glic_mapper_enable_exposure): E [expo_cap][12] and its Adam state ----
     bool expo_on = false;
     float expo_lr = 0.f;
-    float *expo_E = nullptr, *expo_m = nullptr, *expo_v = nullptr;
-    int* expo_t = nullptr;
+    float* expo_E = nullptr;
+    KeyframeAdam expo_adam{12};
     size_t expo_cap = 0;
     // ---- per-training-keyframe pose refinement (glic_mapper_enable_pose_refinement): float64 T_cw [pose_cap][12]
-    //      (R_cw row-major | t_cw), the float pose [pose_cap][12] (R_wc | t_wc), Adam moments [pose_cap][6], step counts ----
+    //      (R_cw row-major | t_cw), the float pose [pose_cap][12] (R_wc | t_wc) and the Adam state of the 6-vector ----
     bool pose_on = false;
     float pose_lr_rho = 0.f, pose_lr_omega = 0.f;
     double* pose_T = nullptr;
-    float *pose_f = nullptr, *pose_m = nullptr, *pose_v = nullptr;
-    int* pose_t = nullptr;
+    float* pose_f = nullptr;
+    KeyframeAdam pose_adam{6};
     size_t pose_cap = 0;
     double* pose_part = nullptr;          // per-CTA partials of the pose-gradient reduction (pose_partials_count(Pcap))
     cudaEvent_t ev_pose{};
@@ -287,29 +281,37 @@ void arena_ptrs(const glic_mapper* m, float* base, uint32_t cap, float* out6[6])
 }
 
 float* geo_ptr(const glic_mapper* m) { return reinterpret_cast<float*>(m->xblock); }
-float* col_slot(const glic_mapper* m, int parity, int slot) {
-    return reinterpret_cast<float*>(m->xblock + m->off_col) + ((size_t)parity * m->S + slot) * (size_t)m->Pcap * 3;
-}
-uint8_t* flag_slot(const glic_mapper* m, int parity, int slot) {
-    return reinterpret_cast<uint8_t*>(m->xblock + m->off_flags) + ((size_t)parity * m->S + slot) * (size_t)m->Pcap;
-}
-float* expo_slot(const glic_mapper* m, int parity, int slot) {
-    return reinterpret_cast<float*>(m->xblock + m->off_expo) + ((size_t)parity * m->S + slot) * 12;
+
+// view slot s of parity `parity` in region r of the exchange block
+template <typename T = float>
+T* slot(const glic_mapper* m, SlotRegion r, int parity, int s) {
+    return reinterpret_cast<T*>(m->xblock + m->slot_off[r] + ((size_t)parity * m->S + s) * m->slot_bytes[r]);
 }
 
+// The slot regions follow the flags words, each [2][S] slots rounded up to 256 bytes: colour gradients [cap][3] floats, flag
+// bytes [cap], dL/dE [12] floats, dL/d(rho, omega) [8] floats (2 unused).  Returns the block's size.
 size_t xblock_layout(glic_mapper* m, uint32_t cap) {
     m->n_geo = (size_t)11 * cap + 4;
     size_t sl[6];
     glic_p2p_slice(0, 1, m->n_geo, 0, sl);
-    const size_t flag_off = sl[5];
-    m->off_col = flag_off + 256;
-    m->off_flags = m->off_col + (((size_t)2 * m->S * cap * 3 * sizeof(float) + 255) & ~size_t(255));
-    m->off_expo = m->off_flags + (((size_t)2 * m->S * cap + 255) & ~size_t(255));
-    m->off_pose = m->off_expo + (((size_t)2 * m->S * 12 * sizeof(float) + 255) & ~size_t(255));
-    return m->off_pose + (((size_t)2 * m->S * 8 * sizeof(float) + 255) & ~size_t(255));
+    const size_t bytes[N_REGIONS] = {(size_t)cap * 3 * sizeof(float), cap, 12 * sizeof(float), 8 * sizeof(float)};
+    size_t off = sl[5] + 256;
+    for (int r = 0; r < N_REGIONS; ++r) {
+        m->slot_off[r] = off;
+        m->slot_bytes[r] = bytes[r];
+        off += ((size_t)2 * m->S * bytes[r] + 255) & ~size_t(255);
+    }
+    return off;
 }
-float* pose_slot(const glic_mapper* m, int parity, int slot) {
-    return reinterpret_cast<float*>(m->xblock + m->off_pose) + ((size_t)parity * m->S + slot) * 8;
+
+// copies [local, local + bytes) of this rank's exchange block to the same offset in every peer's, on the push stream
+int push_to_peers(glic_mapper* m, const void* local, size_t bytes) {
+    const size_t off = static_cast<const char*>(local) - m->xblock;
+    for (int q = 0; q < m->cfg.world; ++q) {
+        if (q == m->cfg.rank) continue;
+        GLIC_CUDA_TRY(cudaMemcpyAsync(static_cast<char*>(m->peers[q]) + off, local, bytes, cudaMemcpyDeviceToDevice, m->push_stream));
+    }
+    return GLIC_OK;
 }
 
 // (re)allocates everything whose size depends on the Gaussian capacity; copies the live rows of the arenas
@@ -347,26 +349,56 @@ int set_capacity(glic_mapper* m, uint32_t cap) {
     return GLIC_OK;
 }
 
+// Grows per-training-keyframe device arrays from old_cap to cap rows, keeping rows [0, old_cap): each entry is the address of
+// an array and its bytes per row.  New rows are zero.
+int grow_keyframe_rows(glic_mapper* m, std::initializer_list<std::pair<void**, size_t>> arrays, size_t old_cap, size_t cap) {
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    std::vector<void*> grown(arrays.size(), nullptr);
+    size_t i = 0;
+    for (const auto& a : arrays) MAP_TRY(dev_alloc(&grown[i++], cap * a.second));
+    if (old_cap) {
+        i = 0;
+        for (const auto& a : arrays)
+            GLIC_CUDA_TRY(cudaMemcpyAsync(grown[i++], *a.first, old_cap * a.second, cudaMemcpyDeviceToDevice, m->stream));
+        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    }
+    i = 0;
+    for (const auto& a : arrays) {
+        if (*a.first) cudaFree(*a.first);
+        *a.first = grown[i++];
+    }
+    return GLIC_OK;
+}
+
 // room for the exposure state of n training keyframes (keeps the existing rows)
 int expo_reserve(glic_mapper* m, size_t n) {
     if (n <= m->expo_cap) return GLIC_OK;
     const size_t cap = std::max<size_t>({n, 2 * m->expo_cap, 64});
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    float *E = nullptr, *m1 = nullptr, *v = nullptr;
-    int* t = nullptr;
-    MAP_TRY(dev_alloc((void**)&E, cap * 12 * sizeof(float))); MAP_TRY(dev_alloc((void**)&m1, cap * 12 * sizeof(float)));
-    MAP_TRY(dev_alloc((void**)&v, cap * 12 * sizeof(float))); MAP_TRY(dev_alloc((void**)&t, cap * sizeof(int)));
-    if (m->expo_cap) {
-        GLIC_CUDA_TRY(cudaMemcpyAsync(E, m->expo_E, m->expo_cap * 12 * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-        GLIC_CUDA_TRY(cudaMemcpyAsync(m1, m->expo_m, m->expo_cap * 12 * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-        GLIC_CUDA_TRY(cudaMemcpyAsync(v, m->expo_v, m->expo_cap * 12 * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-        GLIC_CUDA_TRY(cudaMemcpyAsync(t, m->expo_t, m->expo_cap * sizeof(int), cudaMemcpyDeviceToDevice, m->stream));
-        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    }
-    void* old[] = {m->expo_E, m->expo_m, m->expo_v, m->expo_t};
-    for (void* p : old) if (p) cudaFree(p);
-    m->expo_E = E; m->expo_m = m1; m->expo_v = v; m->expo_t = t;
+    KeyframeAdam& a = m->expo_adam;
+    MAP_TRY(grow_keyframe_rows(m, {{(void**)&m->expo_E, 12 * sizeof(float)}, {(void**)&a.m, 12 * sizeof(float)},
+                                   {(void**)&a.v, 12 * sizeof(float)}, {(void**)&a.t, sizeof(int)}}, m->expo_cap, cap));
     m->expo_cap = cap;
+    return GLIC_OK;
+}
+
+// room for the pose state of n training keyframes (keeps the existing rows)
+int pose_reserve(glic_mapper* m, size_t n) {
+    if (n <= m->pose_cap) return GLIC_OK;
+    const size_t cap = std::max<size_t>({n, 2 * m->pose_cap, 64});
+    KeyframeAdam& a = m->pose_adam;
+    MAP_TRY(grow_keyframe_rows(m, {{(void**)&m->pose_T, 12 * sizeof(double)}, {(void**)&m->pose_f, 12 * sizeof(float)},
+                                   {(void**)&a.m, 6 * sizeof(float)}, {(void**)&a.v, 6 * sizeof(float)}, {(void**)&a.t, sizeof(int)}},
+                               m->pose_cap, cap));
+    m->pose_cap = cap;
+    return GLIC_OK;
+}
+
+// zero moments and step counts of keyframes [first, last), on the mapper's stream
+int adam_reset(glic_mapper* m, const KeyframeAdam& a, size_t first, size_t last) {
+    const size_t row = a.width * sizeof(float);
+    GLIC_CUDA_TRY(cudaMemsetAsync(a.m + a.width * first, 0, (last - first) * row, m->stream));
+    GLIC_CUDA_TRY(cudaMemsetAsync(a.v + a.width * first, 0, (last - first) * row, m->stream));
+    GLIC_CUDA_TRY(cudaMemsetAsync(a.t + first, 0, (last - first) * sizeof(int), m->stream));
     return GLIC_OK;
 }
 
@@ -377,44 +409,9 @@ int expo_reset(glic_mapper* m, size_t first, size_t last) {
     std::vector<float> id(12 * (last - first), 0.0f);
     for (size_t k = 0; k < last - first; ++k) id[12 * k] = id[12 * k + 5] = id[12 * k + 10] = 1.0f;
     GLIC_CUDA_TRY(cudaMemcpyAsync(m->expo_E + 12 * first, id.data(), id.size() * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->expo_m + 12 * first, 0, id.size() * sizeof(float), m->stream));
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->expo_v + 12 * first, 0, id.size() * sizeof(float), m->stream));
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->expo_t + first, 0, (last - first) * sizeof(int), m->stream));
+    MAP_TRY(adam_reset(m, m->expo_adam, first, last));
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     return GLIC_OK;
-}
-
-// room for the pose state of n training keyframes (keeps the existing rows)
-int pose_reserve(glic_mapper* m, size_t n) {
-    if (n <= m->pose_cap) return GLIC_OK;
-    const size_t cap = std::max<size_t>({n, 2 * m->pose_cap, 64});
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    double* T = nullptr;
-    float *f = nullptr, *m1 = nullptr, *v = nullptr;
-    int* t = nullptr;
-    MAP_TRY(dev_alloc((void**)&T, cap * 12 * sizeof(double))); MAP_TRY(dev_alloc((void**)&f, cap * 12 * sizeof(float)));
-    MAP_TRY(dev_alloc((void**)&m1, cap * 6 * sizeof(float))); MAP_TRY(dev_alloc((void**)&v, cap * 6 * sizeof(float)));
-    MAP_TRY(dev_alloc((void**)&t, cap * sizeof(int)));
-    if (m->pose_cap) {
-        GLIC_CUDA_TRY(cudaMemcpyAsync(T, m->pose_T, m->pose_cap * 12 * sizeof(double), cudaMemcpyDeviceToDevice, m->stream));
-        GLIC_CUDA_TRY(cudaMemcpyAsync(f, m->pose_f, m->pose_cap * 12 * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-        GLIC_CUDA_TRY(cudaMemcpyAsync(m1, m->pose_m, m->pose_cap * 6 * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-        GLIC_CUDA_TRY(cudaMemcpyAsync(v, m->pose_v, m->pose_cap * 6 * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-        GLIC_CUDA_TRY(cudaMemcpyAsync(t, m->pose_t, m->pose_cap * sizeof(int), cudaMemcpyDeviceToDevice, m->stream));
-        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    }
-    void* old[] = {m->pose_T, m->pose_f, m->pose_m, m->pose_v, m->pose_t};
-    for (void* p : old) if (p) cudaFree(p);
-    m->pose_T = T; m->pose_f = f; m->pose_m = m1; m->pose_v = v; m->pose_t = t;
-    m->pose_cap = cap;
-    return GLIC_OK;
-}
-
-// float64 T_cw of a float pose, exactly as camera_block() forms R_cw and t_cw
-void pose_master(const float* R_wc, const float* t_wc, double* T12) {
-    for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 3; ++j) T12[3 * i + j] = (double)R_wc[3 * j + i];
-    for (int i = 0; i < 3; ++i) T12[9 + i] = -(T12[3 * i] * t_wc[0] + T12[3 * i + 1] * t_wc[1] + T12[3 * i + 2] * t_wc[2]);
 }
 
 // writes keyframe k's float pose (host copy, master pose, device float pose, camera block); `reset` also zeroes its Adam
@@ -424,20 +421,15 @@ int pose_write(glic_mapper* m, size_t k, const float* R_wc, const float* t_wc, b
     float R[9], t[3];
     std::memcpy(R, R_wc, sizeof(R)); std::memcpy(t, t_wc, sizeof(t));
     std::memcpy(kf.R_wc, R, sizeof(R)); std::memcpy(kf.t_wc, t, sizeof(t));
-    camera_block(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, kf.R_wc, kf.t_wc, kf.cam);
     double T12[12];
-    pose_master(kf.R_wc, kf.t_wc, T12);
+    camera_block(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, kf.R_wc, kf.t_wc, kf.cam, T12);
     float f12[12];
     std::memcpy(f12, kf.R_wc, 36); std::memcpy(f12 + 9, kf.t_wc, 12);
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     GLIC_CUDA_TRY(cudaMemcpyAsync(kf.cam_dev, kf.cam.view, 36 * sizeof(float), cudaMemcpyHostToDevice, m->stream));
     GLIC_CUDA_TRY(cudaMemcpyAsync(m->pose_T + 12 * k, T12, sizeof(T12), cudaMemcpyHostToDevice, m->stream));
     GLIC_CUDA_TRY(cudaMemcpyAsync(m->pose_f + 12 * k, f12, sizeof(f12), cudaMemcpyHostToDevice, m->stream));
-    if (reset) {
-        GLIC_CUDA_TRY(cudaMemsetAsync(m->pose_m + 6 * k, 0, 6 * sizeof(float), m->stream));
-        GLIC_CUDA_TRY(cudaMemsetAsync(m->pose_v + 6 * k, 0, 6 * sizeof(float), m->stream));
-        GLIC_CUDA_TRY(cudaMemsetAsync(m->pose_t + k, 0, sizeof(int), m->stream));
-    }
+    if (reset) MAP_TRY(adam_reset(m, m->pose_adam, k, k + 1));
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     return GLIC_OK;
 }
@@ -448,8 +440,9 @@ int launch_pose_step(glic_mapper* m, const int* views, int parity) {
     float fov2[2];
     proj_matrix(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, b.Pm, fov2);
     StageTimer _t(GLIC_STAGE_ADAM, m->stream);
-    pose_step_kernel<<<1, MAX_SLOTS, 0, m->stream>>>(m->S, b, pose_slot(m, parity, 0), m->pose_T, m->pose_f, m->pose_m, m->pose_v,
-                                                     m->pose_t, m->pose_lr_rho, m->pose_lr_omega,
+    const KeyframeAdam& a = m->pose_adam;
+    pose_step_kernel<<<1, MAX_SLOTS, 0, m->stream>>>(m->S, b, slot(m, POSE, parity, 0), m->pose_T, m->pose_f, a.m, a.v, a.t,
+                                                     m->pose_lr_rho, m->pose_lr_omega,
                                                      reinterpret_cast<const unsigned int*>(geo_ptr(m) + (size_t)11 * m->Pcap));
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
@@ -500,6 +493,21 @@ int forward_view(glic_mapper* m, const Keyframe& kf, int no_color, long long* co
                         m->sample_ws, m->sample_bytes, m->color, m->final_T, (int64_t*)counters, m->stream);
 }
 
+// activations and a synchronous forward of kf: a binning overflow grows the workspace and renders again, up to 4 attempts.
+// The caller has drained the ring (poll_ring(wait)), so ring slot 0's pinned counters are free.
+int forward_settled(glic_mapper* m, const Keyframe& kf, int no_color) {
+    MAP_TRY(activate(m));
+    for (int attempt = 0; attempt < 4; ++attempt) {
+        long long* cnt = m->counters_host;
+        MAP_TRY(forward_view(m, kf, no_color, cnt));
+        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+        if (!cnt[2]) break;
+        ++m->st.overflow_regrows;
+        MAP_TRY(set_bin_capacity(m, cnt[0] + cnt[0] / 4));
+    }
+    return GLIC_OK;
+}
+
 __global__ void overflow_word_kernel(const GeomHeader* ghdr, float* word) { if (ghdr->overflow) *word = 1.0f; }
 
 // one optimiser step over the view batch `views` (S keyframe indices, slot-major); this rank renders slots [rank*k, rank*k + k)
@@ -524,33 +532,29 @@ int iteration(glic_mapper* m, const int* views) {
     size_t goff[6];
     glic_packed_offsets(m->Pcap, 0, goff);
     for (int j = 0; j < m->k; ++j) {
-        const int slot = m->cfg.rank * m->k + j;
-        const Keyframe& kf = m->train[views[slot]];
+        const int sl = m->cfg.rank * m->k + j;
+        const Keyframe& kf = m->train[views[sl]];
         const int buf = (int)(m->view_counter++ & 1);
         // keyframe image H2D on the copy stream (gaussian.cpp:678), overlapping the previous view's backward / Adam
         GLIC_CUDA_TRY(cudaStreamWaitEvent(m->copy_stream, m->gt_free[buf], 0));
         GLIC_CUDA_TRY(cudaMemcpyAsync(m->gt_dev[buf], kf.image, sizeof(float) * 3 * (size_t)W * H, cudaMemcpyDefault, m->copy_stream));
         GLIC_CUDA_TRY(cudaEventRecord(m->gt_ready[buf], m->copy_stream));
         MAP_TRY(forward_view(m, kf, 0, j == m->k - 1 ? m->counters_host + 4 * r : nullptr));
-        uint8_t* fl = flag_slot(m, parity, slot);
-        float* col = col_slot(m, parity, slot);
+        uint8_t* fl = slot<uint8_t>(m, FLAGS, parity, sl);
+        float* col = slot(m, COLOUR, parity, sl);
         MAP_TRY(launch_view_flags((int)m->P, m->radii, GeomState::carve(m->geom_ws, (int)m->P), fl, s));
         overflow_word_kernel<<<1, 1, 0, s>>>(GeomState::carve(m->geom_ws, (int)m->P).hdr, geo_tail);
         GLIC_LAUNCH_CHECK();
         if (m->cfg.world > 1) {
             GLIC_CUDA_TRY(cudaEventRecord(m->ev_flags, s));
             GLIC_CUDA_TRY(cudaStreamWaitEvent(m->push_stream, m->ev_flags, 0));
-            for (int q = 0; q < m->cfg.world; ++q) {
-                if (q == m->cfg.rank) continue;
-                uint8_t* dst = static_cast<uint8_t*>(m->peers[q]) + (fl - reinterpret_cast<uint8_t*>(m->xblock));
-                GLIC_CUDA_TRY(cudaMemcpyAsync(dst, fl, m->P, cudaMemcpyDeviceToDevice, m->push_stream));
-            }
+            MAP_TRY(push_to_peers(m, fl, m->P));
         }
         GLIC_CUDA_TRY(cudaStreamWaitEvent(s, m->gt_ready[buf], 0));
         // loss of this view (the pinned ring keeps the last local view's value for the statistics)
         if (m->expo_on)
-            MAP_TRY(glic_l1_ssim_loss_exposure(H, W, m->cfg.lambda_dssim, m->color, m->gt_dev[buf], m->expo_E + 12 * (size_t)views[slot], m->loss_dev + 1,
-                                               m->dL_dpix, expo_slot(m, parity, slot), m->loss_scratch, m->loss_bytes, s));
+            MAP_TRY(glic_l1_ssim_loss_exposure(H, W, m->cfg.lambda_dssim, m->color, m->gt_dev[buf], m->expo_E + 12 * (size_t)views[sl], m->loss_dev + 1,
+                                               m->dL_dpix, slot(m, EXPOSURE, parity, sl), m->loss_scratch, m->loss_bytes, s));
         else
             MAP_TRY(glic_l1_ssim_loss(3, H, W, m->cfg.lambda_dssim, m->color, m->gt_dev[buf], m->loss_dev + 1, m->dL_dpix, m->loss_scratch, m->loss_bytes, s));
         GLIC_CUDA_TRY(cudaEventRecord(m->gt_free[buf], s));
@@ -559,31 +563,19 @@ int iteration(glic_mapper* m, const int* views) {
         cg.opacity = m->act_opacity; cg.dL_dopacity = m->g_opacity; cg.rot_raw = reinterpret_cast<const float4*>(g[0]);
         cg.accumulate = j > 0;
         cg.pose_partials = m->pose_on ? m->pose_part : nullptr;        // this view's dL/d(rho, omega), fused into the backward
-        cg.pose_grad = m->pose_on ? pose_slot(m, parity, slot) : nullptr;
+        cg.pose_grad = m->pose_on ? slot(m, POSE, parity, sl) : nullptr;
         MAP_TRY(glic_backward_compact_internal((int)m->P, m->D, m->M, g[1], m->act_scales, m->act_rots, m->M ? g[5] : nullptr, &kf.view, m->radii,
                                                m->bin_cap, m->geom_ws, m->binning_ws, m->image_ws, m->sample_ws, m->dL_dpix, m->g_mean2D,
                                                m->g_conic, m->g_opacity, col, &cg, m->cfg.world > 1 ? (void*)m->ev_col : nullptr, s));
         if (m->cfg.world > 1 && m->pose_on) GLIC_CUDA_TRY(cudaEventRecord(m->ev_pose, s));   // after the pose finish kernel
         if (m->cfg.world > 1) {
             GLIC_CUDA_TRY(cudaStreamWaitEvent(m->push_stream, m->ev_col, 0));
-            for (int q = 0; q < m->cfg.world; ++q) {
-                if (q == m->cfg.rank) continue;
-                char* dst = static_cast<char*>(m->peers[q]) + (reinterpret_cast<char*>(col) - m->xblock);
-                GLIC_CUDA_TRY(cudaMemcpyAsync(dst, col, sizeof(float) * 3 * (size_t)m->P, cudaMemcpyDeviceToDevice, m->push_stream));
-                if (m->expo_on) {                  // this slot's dL/dE (the loss wrote it before the render backward ran)
-                    float* eg = expo_slot(m, parity, slot);
-                    char* edst = static_cast<char*>(m->peers[q]) + (reinterpret_cast<char*>(eg) - m->xblock);
-                    GLIC_CUDA_TRY(cudaMemcpyAsync(edst, eg, sizeof(float) * 12, cudaMemcpyDeviceToDevice, m->push_stream));
-                }
-            }
+            MAP_TRY(push_to_peers(m, col, sizeof(float) * 3 * (size_t)m->P));
+            // this slot's dL/dE (the loss wrote it before the render backward ran)
+            if (m->expo_on) MAP_TRY(push_to_peers(m, slot(m, EXPOSURE, parity, sl), sizeof(float) * 12));
             if (m->pose_on) {                      // this slot's dL/d(rho, omega): ev_col fired before the per-Gaussian backward
                 GLIC_CUDA_TRY(cudaStreamWaitEvent(m->push_stream, m->ev_pose, 0));
-                float* pg = pose_slot(m, parity, slot);
-                for (int q = 0; q < m->cfg.world; ++q) {
-                    if (q == m->cfg.rank) continue;
-                    char* pdst = static_cast<char*>(m->peers[q]) + (reinterpret_cast<char*>(pg) - m->xblock);
-                    GLIC_CUDA_TRY(cudaMemcpyAsync(pdst, pg, sizeof(float) * 6, cudaMemcpyDeviceToDevice, m->push_stream));
-                }
+                MAP_TRY(push_to_peers(m, slot(m, POSE, parity, sl), sizeof(float) * 6));
             }
         }
     }
@@ -596,18 +588,16 @@ int iteration(glic_mapper* m, const int* views) {
     // Reference quirk kept for parity (backward.cu:352 `if (shs)`): with no SH-rest tensor bound (degree 0, M = 0) the whole
     // colour backward is skipped, dL/ddc included, so dc never trains.
     const float color_scale = m->M ? 1.0f / (float)m->S : 0.0f;
-    float campos[MAX_SLOTS * 4];
-    for (int sl = 0; sl < m->S; ++sl) std::memcpy(campos + 4 * sl, m->train[views[sl]].cam.campos, 16);
-    // pose refinement moves the camera blocks on the device: the SH rebuild reads each slot's centre from there
-    const float* campos_dev[MAX_SLOTS];
-    for (int sl = 0; sl < m->S; ++sl) campos_dev[sl] = m->train[views[sl]].cam_dev + 32;
+    // the SH rebuild reads each slot's camera centre from its device camera block (pose refinement moves the blocks there)
+    const float* campos[MAX_SLOTS];
+    for (int sl = 0; sl < m->S; ++sl) campos[sl] = m->train[views[sl]].cam_dev + 32;
     if (m->run_optimizer)
-    MAP_TRY(launch_adam_compact(m->P, m->Pcap, m->D, m->M, m->params, m->m1, m->m2, geo, m->Pcap, lr6, col_slot(m, parity, 0), flag_slot(m, parity, 0),
-                                campos, m->S, 1.0f / (float)m->k, color_scale, 0.9f, 0.999f, 1e-15f, reinterpret_cast<const unsigned int*>(geo_tail), m->vis_acc, s,
-                                m->pose_on ? campos_dev : nullptr));
+    MAP_TRY(launch_adam_compact(m->P, m->Pcap, m->D, m->M, m->params, m->m1, m->m2, geo, m->Pcap, lr6, slot(m, COLOUR, parity, 0),
+                                slot<uint8_t>(m, FLAGS, parity, 0), campos, m->S, 1.0f / (float)m->k, color_scale, 0.9f, 0.999f, 1e-15f,
+                                reinterpret_cast<const unsigned int*>(geo_tail), m->vis_acc, s));
     // every replica steps the batch's exposures from the same S slot gradients, in slot order
     if (m->run_optimizer && m->expo_on)
-        MAP_TRY(launch_exposure_adam(m->S, views, expo_slot(m, parity, 0), m->expo_E, m->expo_m, m->expo_v, m->expo_t, m->expo_lr,
+        MAP_TRY(launch_exposure_adam(m->S, views, slot(m, EXPOSURE, parity, 0), m->expo_E, m->expo_adam.m, m->expo_adam.v, m->expo_adam.t, m->expo_lr,
                                      reinterpret_cast<const unsigned int*>(geo_tail), s));
     // ... and their poses, after the Gaussians (whose SH rebuild above used the centres the batch was rendered from)
     if (m->run_optimizer && m->pose_on) MAP_TRY(launch_pose_step(m, views, parity));
@@ -615,6 +605,31 @@ int iteration(glic_mapper* m, const int* views) {
     GLIC_CUDA_TRY(cudaEventRecord(m->ring_ev[r], s));
     m->ring_used[r] = true;
     ++m->st.iterations;
+    return GLIC_OK;
+}
+
+// the checks of the per-keyframe getters and setters: a mapper and a buffer, the feature (pose or exposure) enabled, a training
+// keyframe index in range
+int keyframe_index_check(glic_mapper* m, bool pose, int index, const void* buf, const char* what) {
+    if (!m || !buf) { set_error(std::string(what) + ": null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!(pose ? m->pose_on : m->expo_on)) {
+        set_error(std::string(what) + (pose ? ": pose refinement is not enabled (glic_mapper_enable_pose_refinement)"
+                                            : ": exposure is not enabled (glic_mapper_enable_exposure)"));
+        return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (index < 0 || index >= (int)m->train.size()) { set_error(std::string(what) + ": training keyframe index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
+    return GLIC_OK;
+}
+
+// moments and step count of a training keyframe's pose or exposure
+int keyframe_adam_state(glic_mapper* m, bool pose, int index, float* exp_avg, float* exp_avg_sq, int* step, const char* what) {
+    MAP_TRY(keyframe_index_check(m, pose, index, step, what));
+    if (!exp_avg || !exp_avg_sq) { set_error(std::string(what) + ": null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const KeyframeAdam& a = pose ? m->pose_adam : m->expo_adam;
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    GLIC_CUDA_TRY(cudaMemcpy(exp_avg, a.m + a.width * (size_t)index, a.width * sizeof(float), cudaMemcpyDeviceToHost));
+    GLIC_CUDA_TRY(cudaMemcpy(exp_avg_sq, a.v + a.width * (size_t)index, a.width * sizeof(float), cudaMemcpyDeviceToHost));
+    GLIC_CUDA_TRY(cudaMemcpy(step, a.t + index, sizeof(int), cudaMemcpyDeviceToHost));
     return GLIC_OK;
 }
 
@@ -680,10 +695,9 @@ int glic_mapper_destroy(glic_mapper* m) {
                     m->xblock, m->image_ws, m->binning_ws, m->sample_ws, m->loss_scratch, m->eval_scratch, m->extend_ws, m->color, m->final_T, m->dL_dpix,
                     m->gt_dev[0], m->gt_dev[1], m->loss_dev, m->eval_out, m->vis_acc};
     for (void* p : bufs) if (p) cudaFree(p);
-    void* expo[] = {m->expo_E, m->expo_m, m->expo_v, m->expo_t};
-    for (void* p : expo) if (p) cudaFree(p);
-    void* pose[] = {m->pose_T, m->pose_f, m->pose_m, m->pose_v, m->pose_t, m->pose_part};
-    for (void* p : pose) if (p) cudaFree(p);
+    void* keyframe_state[] = {m->expo_E, m->expo_adam.m, m->expo_adam.v, m->expo_adam.t, m->pose_T, m->pose_f, m->pose_adam.m,
+                              m->pose_adam.v, m->pose_adam.t, m->pose_part};
+    for (void* p : keyframe_state) if (p) cudaFree(p);
     for (auto& kf : m->train) if (kf.cam_dev) cudaFree(kf.cam_dev);
     for (auto& kf : m->test) if (kf.cam_dev) cudaFree(kf.cam_dev);
     if (m->counters_host) cudaFreeHost(m->counters_host);
@@ -774,15 +788,7 @@ int glic_mapper_extend(glic_mapper* m, int n, const float* points, const float* 
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_dep, depth_rsp, sizeof(float) * n, cudaMemcpyHostToDevice, s));
     // alpha-only render of the newest keyframe (gaussian.cpp:506-507); the binning capacity is settled synchronously here
     if (m->P) {
-        MAP_TRY(activate(m));
-        for (int attempt = 0; attempt < 4; ++attempt) {
-            long long* cnt = m->counters_host;              // ring slot 0 is free: poll_ring(wait) drained the ring
-            MAP_TRY(forward_view(m, kf, 1, cnt));
-            GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-            if (!cnt[2]) break;
-            ++m->st.overflow_regrows;
-            MAP_TRY(set_bin_capacity(m, cnt[0] + cnt[0] / 4));
-        }
+        MAP_TRY(forward_settled(m, kf, 1));
     } else {
         std::vector<float> ones((size_t)W * H, 1.0f);                                       // empty model: alpha = 1 - T = 0
         GLIC_CUDA_TRY(cudaMemcpyAsync(m->final_T, ones.data(), sizeof(float) * ones.size(), cudaMemcpyHostToDevice, s));
@@ -865,15 +871,7 @@ int glic_mapper_evaluate(glic_mapper* m, int is_train, int index, float* psnr, f
     const Keyframe& kf = list[index];
     cudaStream_t s = m->stream;
     const int W = m->cfg.width, H = m->cfg.height;
-    MAP_TRY(activate(m));
-    for (int attempt = 0; attempt < 4; ++attempt) {
-        long long* cnt = m->counters_host;
-        MAP_TRY(forward_view(m, kf, 0, cnt));
-        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-        if (!cnt[2]) break;
-        ++m->st.overflow_regrows;
-        MAP_TRY(set_bin_capacity(m, cnt[0] + cnt[0] / 4));
-    }
+    MAP_TRY(forward_settled(m, kf, 0));
     GLIC_CUDA_TRY(cudaMemcpyAsync(m->gt_dev[0], kf.image, sizeof(float) * 3 * (size_t)W * H, cudaMemcpyHostToDevice, s));
     const float* E = (is_train && m->expo_on) ? m->expo_E + 12 * (size_t)index : nullptr;      // held-out views: identity
     MAP_TRY(eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], E, m->eval_out, m->eval_scratch, m->eval_bytes, s));
@@ -955,22 +953,15 @@ int glic_mapper_enable_exposure(glic_mapper* m, float exposure_lr) {
     return GLIC_OK;
 }
 
-static int expo_index_check(glic_mapper* m, int index, const void* buf, const char* what) {
-    if (!m || !buf) { set_error(std::string(what) + ": null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!m->expo_on) { set_error(std::string(what) + ": exposure is not enabled (glic_mapper_enable_exposure)"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (index < 0 || index >= (int)m->train.size()) { set_error(std::string(what) + ": training keyframe index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
-    return GLIC_OK;
-}
-
 int glic_mapper_exposure_get(glic_mapper* m, int index, float* out12) {
-    MAP_TRY(expo_index_check(m, index, out12, "mapper_exposure_get"));
+    MAP_TRY(keyframe_index_check(m, false, index, out12, "mapper_exposure_get"));
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     GLIC_CUDA_TRY(cudaMemcpy(out12, m->expo_E + 12 * (size_t)index, 12 * sizeof(float), cudaMemcpyDeviceToHost));
     return GLIC_OK;
 }
 
 int glic_mapper_exposure_set(glic_mapper* m, int index, const float* in12) {
-    MAP_TRY(expo_index_check(m, index, in12, "mapper_exposure_set"));
+    MAP_TRY(keyframe_index_check(m, false, index, in12, "mapper_exposure_set"));
     for (int j = 0; j < 12; ++j)
         if (!std::isfinite(in12[j])) { set_error("mapper_exposure_set: non-finite entry"); return GLIC_ERR_INVALID_ARGUMENT; }
     GLIC_CUDA_TRY(cudaMemcpyAsync(m->expo_E + 12 * (size_t)index, in12, 12 * sizeof(float), cudaMemcpyHostToDevice, m->stream));
@@ -979,13 +970,7 @@ int glic_mapper_exposure_set(glic_mapper* m, int index, const float* in12) {
 }
 
 int glic_mapper_exposure_adam_state(glic_mapper* m, int index, float* exp_avg12, float* exp_avg_sq12, int* step) {
-    MAP_TRY(expo_index_check(m, index, step, "mapper_exposure_adam_state"));
-    if (!exp_avg12 || !exp_avg_sq12) { set_error("mapper_exposure_adam_state: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    GLIC_CUDA_TRY(cudaMemcpy(exp_avg12, m->expo_m + 12 * (size_t)index, 12 * sizeof(float), cudaMemcpyDeviceToHost));
-    GLIC_CUDA_TRY(cudaMemcpy(exp_avg_sq12, m->expo_v + 12 * (size_t)index, 12 * sizeof(float), cudaMemcpyDeviceToHost));
-    GLIC_CUDA_TRY(cudaMemcpy(step, m->expo_t + index, sizeof(int), cudaMemcpyDeviceToHost));
-    return GLIC_OK;
+    return keyframe_adam_state(m, false, index, exp_avg12, exp_avg_sq12, step, "mapper_exposure_adam_state");
 }
 
 int glic_mapper_enable_pose_refinement(glic_mapper* m, float lr_translation, float lr_rotation) {
@@ -1003,15 +988,8 @@ int glic_mapper_enable_pose_refinement(glic_mapper* m, float lr_translation, flo
     return GLIC_OK;
 }
 
-static int pose_index_check(glic_mapper* m, int index, const void* buf, const char* what) {
-    if (!m || !buf) { set_error(std::string(what) + ": null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!m->pose_on) { set_error(std::string(what) + ": pose refinement is not enabled (glic_mapper_enable_pose_refinement)"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (index < 0 || index >= (int)m->train.size()) { set_error(std::string(what) + ": training keyframe index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
-    return GLIC_OK;
-}
-
 int glic_mapper_pose_get(glic_mapper* m, int index, float* R_wc9, float* t_wc3, float* cam41) {
-    MAP_TRY(pose_index_check(m, index, R_wc9, "mapper_pose_get"));
+    MAP_TRY(keyframe_index_check(m, true, index, R_wc9, "mapper_pose_get"));
     if (!t_wc3) { set_error("mapper_pose_get: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     float f12[12];
@@ -1026,7 +1004,7 @@ int glic_mapper_pose_get(glic_mapper* m, int index, float* R_wc9, float* t_wc3, 
 }
 
 int glic_mapper_pose_set(glic_mapper* m, int index, const float* R_wc9, const float* t_wc3) {
-    MAP_TRY(pose_index_check(m, index, R_wc9, "mapper_pose_set"));
+    MAP_TRY(keyframe_index_check(m, true, index, R_wc9, "mapper_pose_set"));
     if (!t_wc3) { set_error("mapper_pose_set: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
     for (int j = 0; j < 9; ++j) if (!std::isfinite(R_wc9[j])) { set_error("mapper_pose_set: non-finite entry"); return GLIC_ERR_INVALID_ARGUMENT; }
     for (int j = 0; j < 3; ++j) if (!std::isfinite(t_wc3[j])) { set_error("mapper_pose_set: non-finite entry"); return GLIC_ERR_INVALID_ARGUMENT; }
@@ -1041,13 +1019,7 @@ int glic_mapper_pose_set(glic_mapper* m, int index, const float* R_wc9, const fl
 }
 
 int glic_mapper_pose_adam_state(glic_mapper* m, int index, float* exp_avg6, float* exp_avg_sq6, int* step) {
-    MAP_TRY(pose_index_check(m, index, step, "mapper_pose_adam_state"));
-    if (!exp_avg6 || !exp_avg_sq6) { set_error("mapper_pose_adam_state: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    GLIC_CUDA_TRY(cudaMemcpy(exp_avg6, m->pose_m + 6 * (size_t)index, 6 * sizeof(float), cudaMemcpyDeviceToHost));
-    GLIC_CUDA_TRY(cudaMemcpy(exp_avg_sq6, m->pose_v + 6 * (size_t)index, 6 * sizeof(float), cudaMemcpyDeviceToHost));
-    GLIC_CUDA_TRY(cudaMemcpy(step, m->pose_t + index, sizeof(int), cudaMemcpyDeviceToHost));
-    return GLIC_OK;
+    return keyframe_adam_state(m, true, index, exp_avg6, exp_avg_sq6, step, "mapper_pose_adam_state");
 }
 
 int glic_mapper_synchronize(glic_mapper* m) {

@@ -101,23 +101,18 @@ struct ArenaLayout {
 struct ViewSlots {
     const float* g_color;    // [n_slots][stride][3] dL/dcolour per view as the render backward left it (before the clamp mask)
     const uint8_t* visible;  // [n_slots][stride] per-view flags: 0x80 = radii > 0, bits 0..2 = colour channel clamped (forward.cu:70-75)
-    float campos[32 * 4];    // [n_slots][4] camera centres of the batch's views, by value (n_slots <= 32)
+    const float* campos[32]; // [n_slots] camera centre of each slot's view, in its device camera block (n_slots <= 32)
     size_t stride;           // Gaussians per slot (the arena capacity)
     int n_slots;
 };
 
-// DEV_CAMPOS: the camera centres are read from the slots' device camera blocks instead (pose refinement moves them on the
-// device, so a host copy would be stale)
-struct SlotCampos { const float* p[32]; };
-
 constexpr int ADAM_WARPS = 4;
 
-template <bool DEV_CAMPOS>
 __global__ void __launch_bounds__(ADAM_WARPS * 32)
 adam_compact_kernel(uint32_t P, int D, int M, float* __restrict__ params, float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
                     const float* __restrict__ g_geo /* arena-shaped: rotation | xyz | log-scale | opacity */, ArenaLayout L,
                     ArenaLayout Lg, ViewSlots vs, float grad_scale, float color_scale, float b1, float b2, float eps,
-                    const unsigned int* __restrict__ skip_flag, unsigned int* __restrict__ visible_count, SlotCampos cdev) {
+                    const unsigned int* __restrict__ skip_flag, unsigned int* __restrict__ visible_count) {
     __shared__ float s_g[ADAM_WARPS][32 * (SH_ROW_MAX + 3)];      // rebuilt gradients of the warp's 32 Gaussians: dc[32][3] | sh-rest[32][K]
     __shared__ uint8_t s_row[ADAM_WARPS][32];                      // compacted list of the warp's visible rows
     if (skip_flag && *skip_flag) return;                          // binning overflow: the frame was empty, do not step (ADVICE r1)
@@ -152,9 +147,7 @@ adam_compact_kernel(uint32_t P, int D, int M, float* __restrict__ params, float*
             const float g0 = (fl & 1u) ? 0.f : gc[0], g1 = (fl & 2u) ? 0.f : gc[1], g2 = (fl & 4u) ? 0.f : gc[2];
             gdc[0] += kSH0 * g0; gdc[1] += kSH0 * g1; gdc[2] += kSH0 * g2;
             if (nb > 0) {
-                float cx, cy, cz;
-                if constexpr (DEV_CAMPOS) { cx = cdev.p[v][0]; cy = cdev.p[v][1]; cz = cdev.p[v][2]; }
-                else { cx = vs.campos[4 * v]; cy = vs.campos[4 * v + 1]; cz = vs.campos[4 * v + 2]; }
+                const float cx = vs.campos[v][0], cy = vs.campos[v][1], cz = vs.campos[v][2];
                 const float ox = px - cx, oy = py - cy, oz = pz - cz;
                 const float inv = 1.0f / sqrtf(ox * ox + oy * oy + oz * oz);
                 float bs[15];
@@ -359,9 +352,9 @@ int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flag
 }
 
 int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, float* exp_avg, float* exp_avg_sq, const float* g_geo,
-                        uint32_t Pcap_geo, const float* lr6, const float* g_color, const uint8_t* flags, const float* campos4,
+                        uint32_t Pcap_geo, const float* lr6, const float* g_color, const uint8_t* flags, const float* const* campos_dev,
                         int n_slots, float grad_scale, float color_scale, float b1, float b2, float eps, const unsigned int* skip_flag,
-                        unsigned int* visible_count, cudaStream_t s, const float* const* campos_dev) {
+                        unsigned int* visible_count, cudaStream_t s) {
     if (P == 0) return GLIC_OK;
     ArenaLayout L, Lg;
     size_t off6[6];
@@ -370,19 +363,13 @@ int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, 
     glic_packed_offsets(Pcap_geo, 0, off6);                         // geometric arena: rotation | xyz | log-scale | opacity
     for (int q = 0; q < 6; ++q) { Lg.off[q] = off6[q]; Lg.lr[q] = 0.f; }
     ViewSlots vs;
-    if (n_slots < 1 || n_slots > 32 || (!campos4 && !campos_dev)) { set_error("adam_compact: 1..32 view slots"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (n_slots < 1 || n_slots > 32 || !campos_dev) { set_error("adam_compact: 1..32 view slots"); return GLIC_ERR_INVALID_ARGUMENT; }
     vs.g_color = g_color; vs.visible = flags; vs.stride = Pcap_geo; vs.n_slots = n_slots;
-    SlotCampos cdev{};
-    if (campos_dev) for (int i = 0; i < n_slots; ++i) cdev.p[i] = campos_dev[i];
-    else for (int i = 0; i < 4 * n_slots; ++i) vs.campos[i] = campos4[i];
+    for (int i = 0; i < n_slots; ++i) vs.campos[i] = campos_dev[i];
     const unsigned warps = (P + 31) / 32;
     StageTimer _t(GLIC_STAGE_ADAM, s);
-    if (campos_dev)
-        adam_compact_kernel<true><<<(warps + ADAM_WARPS - 1) / ADAM_WARPS, ADAM_WARPS * 32, 0, s>>>(
-            P, D, M, params, exp_avg, exp_avg_sq, g_geo, L, Lg, vs, grad_scale, color_scale, b1, b2, eps, skip_flag, visible_count, cdev);
-    else
-        adam_compact_kernel<false><<<(warps + ADAM_WARPS - 1) / ADAM_WARPS, ADAM_WARPS * 32, 0, s>>>(
-            P, D, M, params, exp_avg, exp_avg_sq, g_geo, L, Lg, vs, grad_scale, color_scale, b1, b2, eps, skip_flag, visible_count, cdev);
+    adam_compact_kernel<<<(warps + ADAM_WARPS - 1) / ADAM_WARPS, ADAM_WARPS * 32, 0, s>>>(
+        P, D, M, params, exp_avg, exp_avg_sq, g_geo, L, Lg, vs, grad_scale, color_scale, b1, b2, eps, skip_flag, visible_count);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }

@@ -24,7 +24,7 @@
 //     dL/drho   = sum_i g_view,i + W d_i                        (the camera centre moves by -W^T rho)
 //     dL/domega = sum_i p_view,i x g_view,i + sum_c W[:,c] x G_i[:,c]   (the camera centre does not move under omega).
 // Each Gaussian forms its six terms in fp32; the CTA adds them in float64 in a fixed order (warp shuffles, then the four
-// warps in order) and writes one partial per CTA; pose_grad_finish_kernel adds the partials in a fixed order.  No atomics:
+// warps in order) and writes one partial per CTA; partials_finish_kernel adds the partials in a fixed order.  No atomics:
 // two runs give the same bits.
 #include "geom_math.cuh"
 #include "sh_math.cuh"
@@ -340,17 +340,6 @@ preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means,
     }
 }
 
-// one CTA: warp j adds component j of the G per-CTA partials (lane-strided, then a butterfly; a fixed order)
-__global__ void __launch_bounds__(192)
-pose_grad_finish_kernel(unsigned G, const double* __restrict__ partials, float* __restrict__ out6) {
-    const int j = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    double s = 0.0;
-    for (unsigned b = lane; b < G; b += 32) s += partials[6 * (size_t)b + j];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane == 0) out6[j] = (float)s;
-}
-
 int launch_preprocess_backward(int P, int D, int M, const float* means, const float* scales, float mod,
                                const float* rots, const float* sh, const ViewParams& vp, const int* radii, GeomState g,
                                float lambda_erank, const float* dL_dmean2D, const float* dL_dconic,
@@ -374,7 +363,7 @@ int launch_preprocess_backward_compact(int P, int D, int M, const float* means, 
             P, D, M, means, scales, mod, reinterpret_cast<const float4*>(rots), sh, vp, radii, g.clamped, 0.0f,
             dL_dmean2D, dL_dconic, dL_dcolors, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cg);
         GLIC_LAUNCH_CHECK();
-        pose_grad_finish_kernel<<<1, 192, 0, s>>>(blocks, cg.pose_partials, cg.pose_grad);
+        partials_finish_kernel<6><<<1, 6 * 32, 0, s>>>(blocks, cg.pose_partials, cg.pose_grad);
         GLIC_LAUNCH_CHECK();
         return GLIC_OK;
     }

@@ -15,6 +15,7 @@
 // fetches both.  Each half is the same fmaf(g, v, acc) chain as the scalar form: bit-identical results.  The backward
 // (3 maps) stays scalar: its 64-bit shared-memory traffic would cost more than pairing saves.
 #include "common.cuh"
+#include "adam_math.cuh"
 #include "f32x2.cuh"
 #include <algorithm>
 
@@ -349,50 +350,25 @@ exposure_mix_kernel(size_t HW, const float* __restrict__ img, const float* __res
     }
 }
 
-// dL/dE[j] = fixed-order float64 sum of the G partials: warp j sums entry j (lane-strided, then a shuffle tree)
-__global__ void __launch_bounds__(384)
-exposure_grad_finish_kernel(unsigned G, const double* __restrict__ partials, float* __restrict__ dL_dE) {
-    const int j = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    double s = 0.0;
-    for (unsigned b = lane; b < G; b += 32) s += partials[12 * (size_t)b + j];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane == 0) dL_dE[j] = (float)s;
-}
-
 struct ExpoBatch { int kf[EXPO_MAX_SLOTS]; };
 
-// One exposure step per batch (torch::optim::Adam: betas (0.9, 0.999), eps 1e-8, no weight decay, bias correction from
-// the keyframe's own step count).  Thread (slot s, entry j); the first slot that holds a keyframe steps it with
-//   g = (1/S) * sum over the slots holding it (slot order, float64) of the slot's dL/dE.
+// One exposure step per batch (torch_adam_delta, bias correction from the keyframe's own step count).  Thread (slot s,
+// entry j); the first slot that holds a keyframe steps it with the batch gradient of keyframe_batch_grad.
 // A set overflow word (the batch was skipped on the device) leaves E, m, v and t as they are.
 __global__ void __launch_bounds__(EXPO_MAX_SLOTS * 12)
 exposure_adam_kernel(int S, ExpoBatch batch, const float* __restrict__ slot_grads, float* __restrict__ E, float* __restrict__ m,
                      float* __restrict__ v, int* __restrict__ t, float lr, const unsigned int* __restrict__ skip) {
     if (*skip) return;
     const int s = threadIdx.x / 12, j = threadIdx.x % 12;
-    bool first = s < S;
+    const bool first = s < S && first_slot_of_keyframe(batch.kf, s);
     const int kf = first ? batch.kf[s] : 0;
-    for (int q = 0; q < s && first; ++q) first = batch.kf[q] != kf;
     int step = 0;
     if (first) step = t[kf] + 1;
     __syncthreads();                                     // every thread has read its keyframe's old step count
     if (!first) return;
-    double acc = 0.0;
-    for (int q = s; q < S; ++q)
-        if (batch.kf[q] == kf) acc += (double)slot_grads[12 * q + j];
-    const float g = (float)(acc / (double)S);
-    const float b1 = 0.9f, b2 = 0.999f, eps = 1e-8f;
-    const double bc1 = 1.0 - pow(0.9, (double)step), bc2 = 1.0 - pow(0.999, (double)step);
+    const float g = keyframe_batch_grad(batch.kf, S, s, slot_grads, 12, j);
     const size_t i = 12 * (size_t)kf + j;
-    // every operation rounded on its own (no contraction), so that a CPU restatement (tests/exposure_oracle.py) can follow it
-    const float m1 = fmaf(1.0f - b1, g, __fmul_rn(b1, m[i]));
-    const float v1 = fmaf(1.0f - b2, __fmul_rn(g, g), __fmul_rn(b2, v[i]));
-    const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v1), (float)sqrt(bc2)), eps);
-    const float step_size = (float)((double)lr / bc1);
-    E[i] = __fadd_rn(E[i], __fmul_rn(-step_size, __fdiv_rn(m1, denom)));
-    m[i] = m1;
-    v[i] = v1;
+    E[i] = __fadd_rn(E[i], torch_adam_delta(g, m[i], v[i], lr, step));
     if (j == 0) t[kf] = step;
 }
 
@@ -495,7 +471,7 @@ extern "C" int glic_l1_ssim_loss_exposure(int H, int W, float lambda_dssim, cons
         const unsigned G = expo_blocks(HW);
         exposure_mix_kernel<<<G, XT, 0, s>>>(HW, img, E, dL_dimg, partials);
         GLIC_LAUNCH_CHECK();
-        exposure_grad_finish_kernel<<<1, 384, 0, s>>>(G, partials, dL_dE);
+        partials_finish_kernel<12><<<1, 12 * 32, 0, s>>>(G, partials, dL_dE);
         GLIC_LAUNCH_CHECK();
     }
     return GLIC_OK;

@@ -3,7 +3,7 @@
 Two native mappers on the same scene and keyframes run bench.py's mapping_iter_native step: one view per iteration from eight
 pinned-host keyframes (image H2D, activations, forward, fused L1 + D-SSIM loss, backward, Gaussian Adam).  One mapper never
 enables pose refinement; the other trains the keyframe poses (the pose gradient fused into the per-Gaussian backward, its
-finish kernel, the pose Adam step and camera rebuild, and the Adam kernel's device-side camera centres).  Their timed windows alternate in this one call, so
+finish kernel, the pose Adam step and camera rebuild).  Their timed windows alternate in this one call, so
 both see the same machine state; each window is device time on the mapper's stream over `--steps` iterations.
 
     python scripts/pose_bench.py [--steps 50] [--windows 9] [--config cfg2]
