@@ -104,6 +104,10 @@ def _load():
         "glic_p2p_check": (i32, [vp, sz, sz, vp]),
         "glic_eval_scratch_bytes": (sz, [i32, i32, i32]),
         "glic_eval_psnr_ssim": (i32, [i32, i32, i32, vp, vp, vp, vp, sz, vp]),
+        "glic_lpips_weight_floats": (sz, []),
+        "glic_lpips_read_weights": (i32, [C.c_char_p, vp]),
+        "glic_lpips_scratch_bytes": (sz, [i32, i32]),
+        "glic_lpips": (i32, [i32, i32, vp, vp, vp, vp, vp, sz, vp]),
         "glic_arena_append": (i32, [vp, vp, vp, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp]),
         "glic_arena_regrow": (i32, [vp, u32, vp, u32, u32, u32, vp]),
         "glic_camera_block": (i32, [i32, i32, f32, f32, f32, f32, C.POINTER(f32), C.POINTER(f32), C.POINTER(f32)]),
@@ -115,6 +119,9 @@ def _load():
         "glic_mapper_optimize": (i32, [vp, C.POINTER(i32), i32]),
         "glic_mapper_sample_views": (i32, [vp, C.POINTER(i32), C.POINTER(i32)]),
         "glic_mapper_evaluate": (i32, [vp, i32, i32, C.POINTER(f32), C.POINTER(f32)]),
+        "glic_mapper_load_lpips": (i32, [vp, C.c_char_p]),
+        "glic_mapper_evaluate_lpips": (i32, [vp, i32, i32, C.POINTER(f32), C.POINTER(f32), C.POINTER(f32)]),
+        "glic_mapper_render": (i32, [vp, i32, i32, vp]),
         "glic_mapper_save_map": (i32, [vp, C.c_char_p]),
         "glic_mapper_stats_get": (i32, [vp, C.POINTER(MapperStats)]),
         "glic_mapper_download": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp]),

@@ -353,4 +353,6 @@ int launch_exposure_adam(int S, const int* kf_of_slot_host, const float* slot_gr
 // glic_eval_psnr_ssim with an optional exposure E (3 channels) applied to img before the clamp
 int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, const float* E, float* out2, void* scratch,
                    size_t scratch_bytes, void* stream);
+// the clamped (and exposed) images eval_psnr_ssim scored, left in its scratch: which = 0 the image, 1 the ground truth
+const float* eval_clamped(const void* scratch, int CH, int H, int W, int which);
 }  // namespace glic

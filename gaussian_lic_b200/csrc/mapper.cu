@@ -260,6 +260,10 @@ struct glic_mapper {
     size_t pose_cap = 0;
     double* pose_part = nullptr;          // per-CTA partials of the pose-gradient reduction (pose_partials_count(Pcap))
     cudaEvent_t ev_pose{};
+    // ---- LPIPS of the evaluation (glic_mapper_load_lpips): weight payload and glic_lpips's scratch, sized on first use ----
+    float* lpips_w = nullptr;
+    void* lpips_scratch = nullptr;
+    size_t lpips_bytes = 0;
 };
 
 namespace {
@@ -633,6 +637,29 @@ int keyframe_adam_state(glic_mapper* m, bool pose, int index, float* exp_avg, fl
     return GLIC_OK;
 }
 
+// renders keyframe `index` and scores it (evaluateVisualQuality, gaussian.cpp:754-760): PSNR / SSIM land in eval_out[0..1], and
+// the clamped image (a training keyframe's E applied first; held-out views: identity) and the clamped ground truth stay in the
+// evaluation scratch (eval_clamped).  Asynchronous after the settled forward.
+int render_scored(glic_mapper* m, int is_train, int index, const char* what) {
+    auto& list = is_train ? m->train : m->test;
+    if (index < 0 || index >= (int)list.size()) { set_error(std::string(what) + ": keyframe index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
+    MAP_TRY(poll_ring(m, true));
+    const Keyframe& kf = list[index];
+    cudaStream_t s = m->stream;
+    const int W = m->cfg.width, H = m->cfg.height;
+    MAP_TRY(forward_settled(m, kf, 0));
+    GLIC_CUDA_TRY(cudaMemcpyAsync(m->gt_dev[0], kf.image, sizeof(float) * 3 * (size_t)W * H, cudaMemcpyHostToDevice, s));
+    const float* E = (is_train && m->expo_on) ? m->expo_E + 12 * (size_t)index : nullptr;
+    return eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], E, m->eval_out, m->eval_scratch, m->eval_bytes, s);
+}
+
+// copies n floats of eval_out to the host and waits for them
+int read_eval_out(glic_mapper* m, float* out, int n) {
+    GLIC_CUDA_TRY(cudaMemcpyAsync(out, m->eval_out, sizeof(float) * n, cudaMemcpyDeviceToHost, m->stream));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    return GLIC_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -696,7 +723,7 @@ int glic_mapper_destroy(glic_mapper* m) {
                     m->gt_dev[0], m->gt_dev[1], m->loss_dev, m->eval_out, m->vis_acc};
     for (void* p : bufs) if (p) cudaFree(p);
     void* keyframe_state[] = {m->expo_E, m->expo_adam.m, m->expo_adam.v, m->expo_adam.t, m->pose_T, m->pose_f, m->pose_adam.m,
-                              m->pose_adam.v, m->pose_adam.t, m->pose_part};
+                              m->pose_adam.v, m->pose_adam.t, m->pose_part, m->lpips_w, m->lpips_scratch};
     for (void* p : keyframe_state) if (p) cudaFree(p);
     for (auto& kf : m->train) if (kf.cam_dev) cudaFree(kf.cam_dev);
     for (auto& kf : m->test) if (kf.cam_dev) cudaFree(kf.cam_dev);
@@ -865,20 +892,49 @@ int glic_mapper_optimize(glic_mapper* m, const int* views_host, int n_views) {
 
 int glic_mapper_evaluate(glic_mapper* m, int is_train, int index, float* psnr, float* ssim) {
     if (!m || !psnr || !ssim) { set_error("mapper_evaluate: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    auto& list = is_train ? m->train : m->test;
-    if (index < 0 || index >= (int)list.size()) { set_error("mapper_evaluate: keyframe index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
-    MAP_TRY(poll_ring(m, true));
-    const Keyframe& kf = list[index];
-    cudaStream_t s = m->stream;
-    const int W = m->cfg.width, H = m->cfg.height;
-    MAP_TRY(forward_settled(m, kf, 0));
-    GLIC_CUDA_TRY(cudaMemcpyAsync(m->gt_dev[0], kf.image, sizeof(float) * 3 * (size_t)W * H, cudaMemcpyHostToDevice, s));
-    const float* E = (is_train && m->expo_on) ? m->expo_E + 12 * (size_t)index : nullptr;      // held-out views: identity
-    MAP_TRY(eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], E, m->eval_out, m->eval_scratch, m->eval_bytes, s));
+    MAP_TRY(render_scored(m, is_train, index, "mapper_evaluate"));
     float out2[2] = {0.f, 0.f};
-    GLIC_CUDA_TRY(cudaMemcpyAsync(out2, m->eval_out, sizeof(out2), cudaMemcpyDeviceToHost, s));
-    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    MAP_TRY(read_eval_out(m, out2, 2));
     *psnr = out2[0]; *ssim = out2[1];
+    return GLIC_OK;
+}
+
+int glic_mapper_load_lpips(glic_mapper* m, const char* path) {
+    if (!m || !path) { set_error("mapper_load_lpips: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    std::vector<float> w(glic_lpips_weight_floats());
+    MAP_TRY(glic_lpips_read_weights(path, w.data()));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    if (!m->lpips_w) MAP_TRY(dev_alloc((void**)&m->lpips_w, w.size() * sizeof(float), false));
+    GLIC_CUDA_TRY(cudaMemcpy(m->lpips_w, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice));
+    return GLIC_OK;
+}
+
+int glic_mapper_evaluate_lpips(glic_mapper* m, int is_train, int index, float* psnr, float* ssim, float* lpips) {
+    if (!m || !psnr || !ssim || !lpips) { set_error("mapper_evaluate_lpips: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!m->lpips_w) { set_error("mapper_evaluate_lpips: no LPIPS weights loaded (glic_mapper_load_lpips)"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const int W = m->cfg.width, H = m->cfg.height;
+    const size_t need = glic_lpips_scratch_bytes(H, W);
+    if (!need) { set_error("mapper_evaluate_lpips: LPIPS needs a frame of at least 31x31"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!m->lpips_scratch) {
+        MAP_TRY(dev_alloc(&m->lpips_scratch, need, false));
+        m->lpips_bytes = need;
+    }
+    MAP_TRY(render_scored(m, is_train, index, "mapper_evaluate_lpips"));
+    MAP_TRY(glic_lpips(H, W, eval_clamped(m->eval_scratch, 3, H, W, 0), eval_clamped(m->eval_scratch, 3, H, W, 1), m->lpips_w,
+                       m->eval_out + 2, m->lpips_scratch, m->lpips_bytes, m->stream));
+    float out3[3] = {0.f, 0.f, 0.f};
+    MAP_TRY(read_eval_out(m, out3, 3));
+    *psnr = out3[0]; *ssim = out3[1]; *lpips = out3[2];
+    return GLIC_OK;
+}
+
+int glic_mapper_render(glic_mapper* m, int is_train, int index, float* rgb_host) {
+    if (!m || !rgb_host) { set_error("mapper_render: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const int W = m->cfg.width, H = m->cfg.height;
+    MAP_TRY(render_scored(m, is_train, index, "mapper_render"));
+    GLIC_CUDA_TRY(cudaMemcpyAsync(rgb_host, eval_clamped(m->eval_scratch, 3, H, W, 0), sizeof(float) * 3 * (size_t)W * H,
+                                  cudaMemcpyDeviceToHost, m->stream));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     return GLIC_OK;
 }
 

@@ -560,6 +560,10 @@ int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, cons
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }
+
+const float* eval_clamped(const void* scratch, int CH, int H, int W, int which) {
+    return reinterpret_cast<const float*>(static_cast<const char*>(scratch) + 256) + (size_t)which * CH * H * W;
+}
 }  // namespace glic
 
 extern "C" int glic_eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, float* out2, void* scratch,

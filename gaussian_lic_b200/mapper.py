@@ -105,6 +105,24 @@ class Mapper:
         capi.check(capi.lib.glic_mapper_evaluate(self._h, int(bool(train)), int(index), C.byref(a), C.byref(b)), "mapper_evaluate")
         return a.value, b.value
 
+    def load_lpips(self, path):
+        """Load a glic_lpips weight file (gaussian_lic_b200.lpips_weights.convert makes one from lpips_alex.pt)."""
+        capi.check(capi.lib.glic_mapper_load_lpips(self._h, str(path).encode()), "mapper_load_lpips")
+
+    def evaluate_lpips(self, index, train=True):
+        """(PSNR, SSIM, LPIPS) of one keyframe from one render; PSNR and SSIM are evaluate()'s, bit for bit."""
+        a, b, c = C.c_float(), C.c_float(), C.c_float()
+        capi.check(capi.lib.glic_mapper_evaluate_lpips(self._h, int(bool(train)), int(index), C.byref(a), C.byref(b), C.byref(c)),
+                   "mapper_evaluate_lpips")
+        return a.value, b.value, c.value
+
+    def render(self, index, train=True):
+        """The [3,H,W] float32 image evaluation scores: drawn at the keyframe's current pose, a training keyframe's exposure
+        applied, clamped to [0,1]."""
+        out = np.empty((3, self.H, self.W), np.float32)
+        capi.check(capi.lib.glic_mapper_render(self._h, int(bool(train)), int(index), _p(out)), "mapper_render")
+        return out
+
     def save_map(self, path):
         capi.check(capi.lib.glic_mapper_save_map(self._h, str(path).encode()), "mapper_save_map")
 

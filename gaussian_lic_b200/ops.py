@@ -164,6 +164,20 @@ def l1_ssim_loss_exposure(img, gt, E, lambda_dssim=0.2, grad=True, scratch=None,
     return loss, dL_dimg, dL_dE
 
 
+def lpips(img, gt, weights, scratch=None, stream=None):
+    """LPIPS (AlexNet) of two [3,H,W] float32 CUDA tensors (glic_lpips; both are clamped to [0,1] inside).  weights: the float32
+    CUDA payload of a weight file (lpips_weights.read).  Returns a [1] tensor; no host synchronisation."""
+    _, H, W = img.shape
+    assert img.shape[0] == 3 and gt.shape == img.shape
+    need = capi.lib.glic_lpips_scratch_bytes(H, W)
+    if scratch is None or scratch.numel() < need:
+        scratch = torch.empty(max(need, 1), dtype=torch.uint8, device=img.device)
+    out = torch.empty(1, dtype=torch.float32, device=img.device)
+    capi.check(capi.lib.glic_lpips(H, W, capi.ptr(img.contiguous()), capi.ptr(gt.contiguous()), capi.ptr(weights), capi.ptr(out),
+                                   capi.ptr(scratch), scratch.numel(), stream), "lpips")
+    return out
+
+
 # ---- render() and the model getters it uses (rasterizer/renderer.cpp:21-88; gaussian.cpp:147-175) ------------------
 class GaussianParams:
     """The six raw parameter tensors of GaussianModel with its activation getters (sigmoid / exp / normalize)."""

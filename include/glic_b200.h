@@ -324,11 +324,29 @@ GLIC_API int glic_p2p_reduce_adam(int rank, int world, void* const* bufs_host, u
  * Evaluation metrics (SURVEY 8f rank 4; evaluateVisualQuality, gaussian.cpp:721-830 with loss_utils.h:35-39,
  * 84-127): both images are clamped to [0,1]; PSNR = 10 log10(1 / mean((a-b)^2)); SSIM = mean of the 11x11 /
  * sigma 1.5 zero-padded SSIM map (the conv2d formulation, same window as the fused kernel).  out2[0] = PSNR,
- * out2[1] = SSIM (device floats).  scratch: glic_eval_scratch_bytes.  LPIPS stays TorchScript (out of scope).
+ * out2[1] = SSIM (device floats).  scratch: glic_eval_scratch_bytes.  LPIPS: glic_lpips below.
  * ------------------------------------------------------------------------------------- */
 GLIC_API size_t glic_eval_scratch_bytes(int CH, int H, int W);
 GLIC_API int glic_eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, float* out2, void* scratch,
                                  size_t scratch_bytes, void* stream);
+
+/* LPIPS with the AlexNet trunk, exactly the TorchScript module evaluateVisualQuality loads (src/lpips/lpips_alex.pt,
+ * gaussian.cpp:741-800; lpipsPyTorch/modules/{lpips,networks,utils}.py): both [3,H,W] images are clamped to [0,1] (not
+ * rescaled to [-1,1]), normalised with the file's mean / std, run through conv0/3/6/8/10 (+ReLU; 3/2 max pool after the first
+ * two), and each of the five taps contributes mean_px sum_c lin_c (x_c/(|x|+1e-10) - y_c/(|y|+1e-10))^2.
+ *   Weights: a flat little-endian file, 16-byte header (uint32 magic "LPIP", version 1, float count, 0) followed by
+ *   glic_lpips_weight_floats() floats: mean[3] std[3] | conv0 OIHW weight, bias | conv3 .. | conv6 .. | conv8 .. | conv10 .. |
+ *   lin0[64] lin1[192] lin2[384] lin3[256] lin4[256].  gaussian_lic_b200.lpips_weights converts the .pt file.
+ *   glic_lpips_read_weights (host) fills `host` with the payload and fails on a wrong magic, version, count or file size.
+ *   glic_lpips: device pointers; `weights` holds the payload; out1: 1 device float.  Frames from 31x31 (the smallest the network
+ *   accepts) to 8192x8192; anything else is refused with GLIC_ERR_INVALID_ARGUMENT before any launch, and
+ *   glic_lpips_scratch_bytes returns 0 for it.  No host synchronisation; per-CTA float64 partials added in a fixed order, so two
+ *   identical calls give identical bits and identical images give exactly 0. */
+GLIC_API size_t glic_lpips_weight_floats(void);
+GLIC_API int glic_lpips_read_weights(const char* path, float* host);
+GLIC_API size_t glic_lpips_scratch_bytes(int H, int W);
+GLIC_API int glic_lpips(int H, int W, const float* img, const float* gt, const float* weights, float* out1, void* scratch,
+                        size_t scratch_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Capacity-laid-out model arena (SURVEY 8f rank 1; replaces the torch::cat re-allocation of all parameters and Adam
@@ -412,6 +430,14 @@ GLIC_API int glic_mapper_optimize(glic_mapper* m, const int* views_host, int n_v
 GLIC_API int glic_mapper_sample_views(glic_mapper* m, int* views_host, int* count);
 /* PSNR / SSIM of one keyframe (train = 1: training list, 0: held-out list); synchronises */
 GLIC_API int glic_mapper_evaluate(glic_mapper* m, int is_train, int index, float* psnr, float* ssim);
+/* evaluateVisualQuality's three metrics.  load_lpips reads a glic_lpips weight file and uploads it (the mapper owns the copy;
+ * a second call replaces it).  evaluate_lpips renders the keyframe once and returns the PSNR and SSIM glic_mapper_evaluate
+ * returns, bit for bit, plus the LPIPS of the same clamped image against the keyframe's image; without weights loaded, or on
+ * a frame under 31x31, it returns GLIC_ERR_INVALID_ARGUMENT.  render writes that scored image to rgb_host[3,H,W] (host): the
+ * keyframe drawn at its current pose, a training keyframe's exposure E applied, clamped to [0,1].  All three synchronise. */
+GLIC_API int glic_mapper_load_lpips(glic_mapper* m, const char* path);
+GLIC_API int glic_mapper_evaluate_lpips(glic_mapper* m, int is_train, int index, float* psnr, float* ssim, float* lpips);
+GLIC_API int glic_mapper_render(glic_mapper* m, int is_train, int index, float* rgb_host);
 GLIC_API int glic_mapper_save_map(glic_mapper* m, const char* path);
 GLIC_API int glic_mapper_stats_get(glic_mapper* m, glic_mapper_stats* out);
 /* live rows of the arena copied to host arrays shaped like glic_mapper_initialize's (any pointer may be NULL); synchronises */
