@@ -870,6 +870,10 @@ int glic_mapper_optimize(glic_mapper* m, const int* views_host, int n_views) {
         MAP_TRY(glic_mapper_sample_views(m, list.data(), &cnt));
         list.resize((size_t)cnt);
     }
+    // every index is checked before the first batch is enqueued: a bad index in a later batch (say slot 31 of the second
+    // batch of 32) would otherwise return the error with the earlier batches already stepped
+    for (int v : list)
+        if (v < 0 || v >= (int)m->train.size()) { set_error("mapper_optimize: view index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (list.empty() || m->P == 0) return GLIC_OK;
     GLIC_CUDA_TRY(cudaMemsetAsync(m->vis_acc, 0, sizeof(unsigned int), m->stream));
     GLIC_CUDA_TRY(cudaEventRecord(m->t0, m->stream));
