@@ -82,6 +82,9 @@ def _load():
         "glic_extend_bytes": (sz, [i32, i32, i32]),
         "glic_extend": (i32, [i32, vp, vp, vp, C.POINTER(f32), C.POINTER(f32), f32, f32, f32, f32, i32, i32, vp, f32, vp, sz, vp, vp,
                               vp, vp, vp, vp, C.POINTER(i32), vp]),
+        "glic_lidar_init": (i32, [i32, vp, vp, vp, C.c_double, C.c_double, vp, vp, vp, vp, vp, vp]),
+        "glic_skybox_init_bytes": (sz, [i32]),
+        "glic_skybox_init": (i32, [i32, i32, C.c_uint64, vp, sz, vp, vp, vp, vp, vp, vp, vp]),
         "glic_ply_bytes": (sz, [u32, u32]),
         "glic_ply_write": (i32, [C.c_char_p, u32, u32, vp, vp, vp, vp, vp, vp]),
         "glic_ply_write_packed": (i32, [C.c_char_p, u32, u32, vp]),
@@ -114,6 +117,8 @@ def _load():
         "glic_mapper_create": (i32, [C.POINTER(MapperConfig), C.POINTER(vp)]),
         "glic_mapper_destroy": (i32, [vp]),
         "glic_mapper_initialize": (i32, [vp, u32, vp, vp, vp, vp, vp, vp]),
+        "glic_mapper_initialize_lidar": (i32, [vp, i32, vp, vp, vp, C.c_double, i32, i32]),
+        "glic_mapper_sky_rows": (i32, [vp, C.POINTER(u32)]),
         "glic_mapper_add_keyframe": (i32, [vp, C.POINTER(Keyframe), i32]),
         "glic_mapper_extend": (i32, [vp, i32, vp, vp, vp]),
         "glic_mapper_optimize": (i32, [vp, C.POINTER(i32), i32]),

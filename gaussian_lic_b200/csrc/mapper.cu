@@ -217,6 +217,7 @@ struct glic_mapper {
     cudaStream_t stream = nullptr, copy_stream = nullptr, push_stream = nullptr;
     // ---- arenas (capacity Pcap) ----
     uint32_t P = 0, Pcap = 0;
+    uint32_t n_sky = 0;                   // rows [0, n_sky) are the skybox (glic_mapper_initialize_lidar): left out of save_map
     float *params = nullptr, *m1 = nullptr, *m2 = nullptr;
     float *act_opacity = nullptr, *act_scales = nullptr, *act_rots = nullptr;
     int* radii = nullptr;
@@ -273,6 +274,18 @@ namespace {
 int dev_alloc(void** p, size_t bytes, bool zero = true) {
     GLIC_CUDA_TRY(cudaMalloc(p, bytes ? bytes : 256));
     if (zero) GLIC_CUDA_TRY(cudaMemset(*p, 0, bytes ? bytes : 256));
+    return GLIC_OK;
+}
+
+// grows the staging buffer of the host inputs of extend() and initialize_lidar() to at least `need` bytes (contents lost)
+int reserve_staging(glic_mapper* m, size_t need) {
+    if (need <= m->extend_bytes) return GLIC_OK;
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    if (m->extend_ws) cudaFree(m->extend_ws);
+    m->extend_ws = nullptr;
+    m->extend_bytes = 0;
+    MAP_TRY(dev_alloc(&m->extend_ws, need, false));
+    m->extend_bytes = need;
     return GLIC_OK;
 }
 
@@ -757,8 +770,53 @@ int glic_mapper_initialize(glic_mapper* m, uint32_t P, const float* xyz, const f
         if (P && kk[q] && src[q]) GLIC_CUDA_TRY(cudaMemcpyAsync(g[q], src[q], sizeof(float) * kk[q] * P, cudaMemcpyHostToDevice, s));
     GLIC_CUDA_TRY(cudaStreamSynchronize(s));
     m->P = P;
+    m->n_sky = 0;
     m->st.num_gaussians = P;
     if ((int64_t)16 * P > m->bin_cap) MAP_TRY(set_bin_capacity(m, (int64_t)16 * P));
+    return GLIC_OK;
+}
+
+int glic_mapper_initialize_lidar(glic_mapper* m, int n, const float* points, const double* colors, const float* depth_rsp, double focal,
+                                 int sky_points, int sky_radius) {
+    if (!m || !points || !colors || !depth_rsp) { set_error("mapper_initialize_lidar: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    // n > 0 is the reference's assert(num > 0) (gaussian.cpp:216)
+    if (n < 1 || sky_points < 0 || (sky_points > 0 && sky_radius <= 0) || (int64_t)n + sky_points > INT32_MAX / 4) {
+        set_error("mapper_initialize_lidar: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    const uint32_t S = (uint32_t)sky_points, P = S + (uint32_t)n;
+    MAP_TRY(set_capacity(m, P));
+    cudaStream_t s = m->stream;
+    // staging: points | colors | depth | the sky's dist2 and knn workspace
+    Carver c(nullptr);
+    c.take<float>((size_t)3 * n); c.take<double>((size_t)3 * n); c.take<float>(n); c.take<char>(glic_skybox_init_bytes(sky_points));
+    MAP_TRY(reserve_staging(m, c.total()));
+    c = Carver(m->extend_ws);
+    float* d_pts = c.take<float>((size_t)3 * n); double* d_col = c.take<double>((size_t)3 * n); float* d_dep = c.take<float>(n);
+    const size_t sky_bytes = glic_skybox_init_bytes(sky_points);
+    void* d_sky = c.take<char>(sky_bytes);
+    const size_t nfl = arena_floats(m, m->Pcap);
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->params, 0, nfl * 4, s));
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->m1, 0, nfl * 4, s));
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->m2, 0, nfl * 4, s));
+    GLIC_CUDA_TRY(cudaMemcpyAsync(d_pts, points, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, s));
+    GLIC_CUDA_TRY(cudaMemcpyAsync(d_col, colors, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, s));
+    GLIC_CUDA_TRY(cudaMemcpyAsync(d_dep, depth_rsp, sizeof(float) * n, cudaMemcpyHostToDevice, s));
+    float* g[6];                                    // rot, xyz, log-scale, opacity, f_dc, f_rest
+    arena_ptrs(m, m->params, m->Pcap, g);
+    MAP_TRY(glic_skybox_init(sky_points, sky_radius, m->cfg.seed, d_sky, sky_bytes, g[1], g[4], g[2], g[0], g[3], nullptr, s));
+    MAP_TRY(glic_lidar_init(n, d_pts, d_col, d_dep, (double)m->cfg.scaling_scale, focal, g[1] + 3 * (size_t)S, g[4] + 3 * (size_t)S,
+                            g[2] + 3 * (size_t)S, g[0] + 4 * (size_t)S, g[3] + S, s));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    m->P = P;
+    m->n_sky = S;
+    m->st.num_gaussians = P;
+    if ((int64_t)16 * P > m->bin_cap) MAP_TRY(set_bin_capacity(m, (int64_t)16 * P));
+    return GLIC_OK;
+}
+
+int glic_mapper_sky_rows(glic_mapper* m, uint32_t* out) {
+    if (!m || !out) { set_error("mapper_sky_rows: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    *out = m->n_sky;
     return GLIC_OK;
 }
 
@@ -797,13 +855,7 @@ int glic_mapper_extend(glic_mapper* m, int n, const float* points, const float* 
     const int W = m->cfg.width, H = m->cfg.height;
     const Keyframe& kf = m->train.back();
     // staging: points | colors | depth | outputs (keep_idx, xyz, f_dc, log_scale, rot, opacity) | glic_extend's own workspace
-    const size_t need = glic_extend_bytes(n, W, H) + (size_t)n * (3 + 3 + 1 + 1 + 3 + 3 + 3 + 4 + 1) * 4 + 4096;
-    if (need > m->extend_bytes) {
-        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-        if (m->extend_ws) cudaFree(m->extend_ws);
-        MAP_TRY(dev_alloc(&m->extend_ws, need, false));
-        m->extend_bytes = need;
-    }
+    MAP_TRY(reserve_staging(m, glic_extend_bytes(n, W, H) + (size_t)n * (3 + 3 + 1 + 1 + 3 + 3 + 3 + 4 + 1) * 4 + 4096));
     Carver c(m->extend_ws);
     float* d_pts = c.take<float>((size_t)3 * n); float* d_col = c.take<float>((size_t)3 * n); float* d_dep = c.take<float>(n);
     int* d_keep = c.take<int>(n); float* d_xyz = c.take<float>((size_t)3 * n); float* d_dc = c.take<float>((size_t)3 * n);
@@ -969,10 +1021,14 @@ int glic_mapper_download(glic_mapper* m, float* xyz, float* f_dc, float* f_rest,
 
 int glic_mapper_save_map(glic_mapper* m, const char* path) {
     if (!m || !path) { set_error("mapper_save_map: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    const size_t P = m->P, M = (size_t)m->M;
+    const size_t P = m->P, M = (size_t)m->M, S = m->n_sky;
     std::vector<float> xyz(3 * P), dc(3 * P), rest(3 * M * P), op(P), ls(3 * P), rot(4 * P);
     MAP_TRY(glic_mapper_download(m, xyz.data(), dc.data(), M ? rest.data() : nullptr, op.data(), ls.data(), rot.data(), nullptr, nullptr));
-    return glic_ply_write(path, (uint32_t)P, (uint32_t)M, xyz.data(), dc.data(), rest.data(), op.data(), ls.data(), rot.data());
+    // rows [S, P): saveMap slices the sky off every tensor (gaussian.cpp:310-316).  It hands tinyply the unsliced row count
+    // for f_dc and f_rest, but tinyply keeps the count of the element's first property (xyz, sliced), so the reference's file
+    // is the consistently sliced one.
+    return glic_ply_write(path, (uint32_t)(P - S), (uint32_t)M, xyz.data() + 3 * S, dc.data() + 3 * S, rest.data() + 3 * M * S, op.data() + S,
+                          ls.data() + 3 * S, rot.data() + 4 * S);
 }
 
 int glic_mapper_stats_get(glic_mapper* m, glic_mapper_stats* out) {

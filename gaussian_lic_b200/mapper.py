@@ -67,6 +67,21 @@ class Mapper:
         a = [_f32(g["means"]), _f32(g["dc"]).reshape(P, 3), _f32(g["sh"]), _f32(g["opacity_logits"]), _f32(g["log_scales"]), _f32(g["rots"])]
         capi.check(capi.lib.glic_mapper_initialize(self._h, P, *[_p(x) for x in a]), "mapper_initialize")
 
+    def initialize_lidar(self, points, colors, depth_rsp, focal, sky_points=0, sky_radius=0):
+        """initialize() (gaussian.cpp:212-304) on the GPU: sky_points sky rows keyed by the seed, then the first scan's LiDAR
+        points in order.  colors are the Dataset's doubles (rgb / 255.0); focal = (fx + fy) / 2 of the configuration."""
+        pts, dep = _f32(points), _f32(depth_rsp)
+        col = np.ascontiguousarray(colors, dtype=np.float64)
+        n = int(pts.shape[0])
+        capi.check(capi.lib.glic_mapper_initialize_lidar(self._h, n, _p(pts), _p(col), _p(dep), float(focal), int(sky_points),
+                                                         int(sky_radius)), "mapper_initialize_lidar")
+
+    def sky_rows(self):
+        """How many leading rows are the skybox (save_map leaves them out)."""
+        out = C.c_uint32()
+        capi.check(capi.lib.glic_mapper_sky_rows(self._h, C.byref(out)), "mapper_sky_rows")
+        return int(out.value)
+
     def add_keyframe(self, R_wc, t_wc, image, train=True, pinned=None):
         """image: [3,H,W] float32 numpy array, or a pinned torch tensor (kept alive here)."""
         kf = capi.Keyframe()

@@ -178,6 +178,38 @@ def lpips(img, gt, weights, scratch=None, stream=None):
     return out
 
 
+def lidar_init(points, colors, depth_rsp, scaling_scale, focal, stream=None):
+    """initialize()'s LiDAR rows (glic_lidar_init).  points [n,3] float32, colors [n,3] float64 (rgb / 255.0), depth_rsp [n]
+    float32, all CUDA tensors; scaling_scale and focal = (fx + fy) / 2 are doubles.  Returns the raw parameters
+    dict(xyz [n,3], f_dc [n,3], log_scale [n,3], rot [n,4], opacity_logit [n]); f_rest is zero and not returned."""
+    n = int(points.shape[0])
+    assert points.dtype == torch.float32 and colors.dtype == torch.float64 and depth_rsp.dtype == torch.float32
+    f32 = dict(dtype=torch.float32, device=points.device)
+    out = dict(xyz=torch.empty(n, 3, **f32), f_dc=torch.empty(n, 3, **f32), log_scale=torch.empty(n, 3, **f32),
+               rot=torch.empty(n, 4, **f32), opacity_logit=torch.empty(n, **f32))
+    capi.check(capi.lib.glic_lidar_init(n, capi.ptr(points.contiguous()), capi.ptr(colors.contiguous()), capi.ptr(depth_rsp.contiguous()),
+                                        float(scaling_scale), float(focal), *[capi.ptr(out[k]) for k in ("xyz", "f_dc", "log_scale", "rot",
+                                                                                                          "opacity_logit")], stream),
+               "lidar_init")
+    return out
+
+
+def skybox_init(n, radius, seed, device="cuda:0", uniforms=False, stream=None):
+    """initialize()'s n sky rows (glic_skybox_init) keyed by seed, as the raw-parameter dict lidar_init returns; uniforms=True
+    adds the generator's draws as uv [n,2] (u1, u2 per row)."""
+    f32 = dict(dtype=torch.float32, device=device)
+    out = dict(xyz=torch.empty(n, 3, **f32), f_dc=torch.empty(n, 3, **f32), log_scale=torch.empty(n, 3, **f32),
+               rot=torch.empty(n, 4, **f32), opacity_logit=torch.empty(n, **f32))
+    if uniforms:
+        out["uv"] = torch.empty(n, 2, **f32)
+    need = capi.lib.glic_skybox_init_bytes(int(n))
+    ws = torch.empty(max(need, 1), dtype=torch.uint8, device=device)
+    capi.check(capi.lib.glic_skybox_init(int(n), int(radius), int(seed), capi.ptr(ws), need,
+                                         *[capi.ptr(out[k]) for k in ("xyz", "f_dc", "log_scale", "rot", "opacity_logit")],
+                                         capi.ptr(out.get("uv")), stream), "skybox_init")
+    return out
+
+
 # ---- render() and the model getters it uses (rasterizer/renderer.cpp:21-88; gaussian.cpp:147-175) ------------------
 class GaussianParams:
     """The six raw parameter tensors of GaussianModel with its activation getters (sigmoid / exp / normalize)."""

@@ -212,6 +212,27 @@ GLIC_API int glic_extend(int n, const float* points, const float* colors, const 
                          float* f_dc, float* log_scale, float* rot, float* opacity_logit, int* count_host, void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * initialize() on the GPU (gaussian.cpp:212-304): the first map's rows, written where the caller points (device pointers;
+ * rot 16-byte aligned).  Neither call touches f_rest or Adam moments (the reference's are zero).  Both are asynchronous on
+ * `stream`.  glic_mapper_initialize_lidar wires them to the model: sky rows [0, S), then the LiDAR rows in input order.
+ *   glic_lidar_init: xyz = points; f_dc = (float)((colors - 0.5) / C0) in double (colors: the Dataset's rgb / 255.0
+ *   doubles); log_scale = (float)log(scaling_scale * depth_rsp / focal) in double on all three axes, focal = (fx + fy) / 2
+ *   from the configuration's doubles; rot = (1, 0, 0, 0); opacity_logit = log(0.1 / 0.9) in float.
+ *   glic_skybox_init: n points on the cap z > -0.4 of the sphere of radius 10 * radius, positions in torch's float order
+ *   from two uniforms per row drawn by a counter-based generator keyed by (seed, row) -- the SplitMix64 output seed +
+ *   (row + 1) * 0x9E3779B97F4A7C15 through the SplitMix64 finaliser; u1 = its top 24 bits * 2^-24, u2 = bits 16..39 *
+ *   2^-24 --; f_dc = (0.7, 0.8, 0.95) raw; log_scale = logf(sqrtf(fmaxf(d2, 1e-7f))) with d2 = glic_knn_mean_dist2 over
+ *   the n sky points alone; rot = (1, 0, 0, 0); opacity_logit = log(0.7 / 0.3) in float.  uv (optional, device, [n][2])
+ *   receives the uniforms.  ws: glic_skybox_init_bytes(n) bytes of device memory.
+ * ------------------------------------------------------------------------------------- */
+GLIC_API int glic_lidar_init(int n, const float* points, const double* colors, const float* depth_rsp, double scaling_scale,
+                             double focal, float* xyz, float* f_dc, float* log_scale, float* rot, float* opacity_logit,
+                             void* stream);
+GLIC_API size_t glic_skybox_init_bytes(int n);
+GLIC_API int glic_skybox_init(int n, int radius, uint64_t seed, void* ws, size_t ws_bytes, float* xyz, float* f_dc,
+                              float* log_scale, float* rot, float* opacity_logit, float* uv, void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * On-disk map (SURVEY 8f rank 4).  Replaces GaussianModel::saveMap (gaussian.cpp:305-397, through tinyply.h:588-703):
  * binary little-endian PLY, element vertex, float properties x y z | f_dc_0..2 | f_rest_0..3M-1 | opacity | scale_0..2 |
  * rot_0..3; RAW parameters; f_rest channel-major.  The file is byte-identical to the reference's for the same tensors
@@ -368,7 +389,8 @@ GLIC_API int glic_arena_regrow(const float* src, uint32_t Pcap_src, float* dst, 
  * torch, no Python.  The mapper OWNS its device memory (arena, Adam state, workspaces, keyframe images stay pinned on
  * the host like Camera::original_image_, gaussian.cpp:80): it is the host of the loop, not an operator.
  *
- *   create -> initialize(raw parameters) -> { add_keyframe -> [extend] -> optimize }* -> evaluate / save_map
+ *   create -> initialize(raw parameters) | initialize_lidar(first scan) -> { add_keyframe -> [extend] -> optimize }*
+ *          -> evaluate / save_map
  *
  * One iteration (gaussian.cpp:674-716) = for each of this rank's views: H2D of the pinned image (copy stream,
  * double-buffered), fused activations, forward (capacity-sized binning, no host sync), fused L1/D-SSIM loss, backward
@@ -419,6 +441,16 @@ GLIC_API int glic_mapper_destroy(glic_mapper* m);
 /* raw parameters (host): xyz[P,3] f_dc[P,3] f_rest[P,M,3] (may be NULL: zeros) opacity_logit[P] log_scale[P,3] rot[P,4] */
 GLIC_API int glic_mapper_initialize(glic_mapper* m, uint32_t P, const float* xyz, const float* f_dc, const float* f_rest,
                                     const float* opacity_logit, const float* log_scale, const float* rot);
+/* initialize() (gaussian.cpp:212-304) from the first scan, on the GPU (glic_skybox_init, glic_lidar_init): replaces the model
+ * like glic_mapper_initialize, with sky_points sky rows [0, S) followed by the n LiDAR rows in input order; P = S + n, all
+ * Adam moments zero.  points[n,3] colors[n,3] (doubles, rgb / 255.0) depth_rsp[n] are host arrays; focal = (fx + fy) / 2 of
+ * the configuration in double; the sky is keyed by cfg.seed (the view sampler's state is left alone).  n < 1,
+ * sky_points < 0, sky_radius <= 0 with sky_points > 0 or a NULL pointer return GLIC_ERR_INVALID_ARGUMENT and change
+ * nothing.  Synchronises.  save_map writes rows [S, P) only (saveMap, gaussian.cpp:310-316); every other call sees every
+ * row.  glic_mapper_sky_rows returns S (0 after glic_mapper_initialize). */
+GLIC_API int glic_mapper_initialize_lidar(glic_mapper* m, int n, const float* points, const double* colors, const float* depth_rsp,
+                                          double focal, int sky_points, int sky_radius);
+GLIC_API int glic_mapper_sky_rows(glic_mapper* m, uint32_t* out);
 GLIC_API int glic_mapper_add_keyframe(glic_mapper* m, const glic_keyframe* kf, int is_train);
 /* extend() (gaussian.cpp:499-638) on the newest training keyframe: alpha-only render, z-buffer de-duplication of the n
  * LiDAR points, filter, initialisation, in-place append.  points[n,3] colors[n,3] depth_rsp[n] are host arrays. */
