@@ -35,6 +35,16 @@ class Keyframe(C.Structure):
     _fields_ = [("R_wc", C.c_float * 9), ("t_wc", C.c_float * 3), ("image", C.c_void_p)]
 
 
+class Frame(C.Structure):
+    _fields_ = [("q_wc", C.c_double * 4), ("t_wc", C.c_double * 3), ("bgr", C.c_void_p), ("row_bytes", C.c_size_t), ("n_points", C.c_int),
+                ("xyz", C.c_void_p), ("rgb", C.c_void_p)]
+
+
+class FrameStats(C.Structure):
+    _fields_ = [("frames", C.c_uint32), ("train", C.c_uint32), ("test", C.c_uint32), ("pending_points", C.c_uint32),
+                ("image_bytes", C.c_uint64)]
+
+
 class MapperStats(C.Structure):
     _fields_ = [("num_gaussians", C.c_uint32), ("capacity", C.c_uint32), ("iterations", C.c_uint64), ("last_inserted", C.c_uint32),
                 ("last_loss", C.c_float), ("mean_visible", C.c_double), ("overflow_regrows", C.c_uint32), ("ms_extend", C.c_float),
@@ -85,6 +95,7 @@ def _load():
         "glic_lidar_init": (i32, [i32, vp, vp, vp, C.c_double, C.c_double, vp, vp, vp, vp, vp, vp]),
         "glic_skybox_init_bytes": (sz, [i32]),
         "glic_skybox_init": (i32, [i32, i32, C.c_uint64, vp, sz, vp, vp, vp, vp, vp, vp, vp]),
+        "glic_decode_bgr8": (i32, [i32, i32, vp, vp, vp]),
         "glic_ply_bytes": (sz, [u32, u32]),
         "glic_ply_write": (i32, [C.c_char_p, u32, u32, vp, vp, vp, vp, vp, vp]),
         "glic_ply_write_packed": (i32, [C.c_char_p, u32, u32, vp]),
@@ -142,6 +153,10 @@ def _load():
         "glic_mapper_pose_get": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32), C.POINTER(f32)]),
         "glic_mapper_pose_set": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32)]),
         "glic_mapper_pose_adam_state": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32), C.POINTER(i32)]),
+        "glic_mapper_enable_frames": (i32, [vp, i32, i32, i32]),
+        "glic_mapper_add_frame": (i32, [vp, C.POINTER(Frame), C.POINTER(i32)]),
+        "glic_mapper_keyframe_image": (i32, [vp, i32, i32, vp]),
+        "glic_mapper_frames_get": (i32, [vp, C.POINTER(FrameStats)]),
         "glic_debug_geom": (i32, [i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "glic_debug_binning": (i32, [i32, vp, i64, i64, vp, vp, vp, vp]),
         "glic_debug_image": (i32, [i32, i32, vp, vp, vp, vp, vp, C.POINTER(i64), vp]),

@@ -111,6 +111,7 @@ void camera_block(int W, int H, double fx, double fy, double cx, double cy, cons
 struct Keyframe {
     float R_wc[9], t_wc[3];
     const float* image;
+    const uint8_t* bgr = nullptr;    // add_frame keyframes: packed HWC BGR8 in the frame store, decoded where `image` is copied
     CamBlock cam;
     float* cam_dev;                  // view16 | proj16 | campos4
     glic_view view;
@@ -199,6 +200,41 @@ pose_step_kernel(int S, PoseBatch b, const float* __restrict__ slot_grads /* [S]
     pose_camera(f, f + 9, b.Pm, b.cam[s], nullptr);
 }
 
+// ---- raw frames (glic_mapper_add_frame; Dataset::addFrame, gaussian.cpp:41-111) -------------------------------------------
+constexpr size_t FRAME_CHUNK = 8;    // frames per device allocation of the 8-bit image store
+
+// Eigen::Quaterniond(w, x, y, z).toRotationMatrix() in Eigen's operation order, without normalisation; q = (x, y, z, w).
+// Host code: x86-64 is compiled without FMA, so every operation rounds once.
+void quat_rotation(const double q[4], double R[9]) {
+    const double x = q[0], y = q[1], z = q[2], w = q[3];
+    const double tx = 2.0 * x, ty = 2.0 * y, tz = 2.0 * z;
+    const double twx = tx * w, twy = ty * w, twz = tz * w;
+    const double txx = tx * x, txy = ty * x, txz = tz * x;
+    const double tyy = ty * y, tyz = tz * y, tzz = tz * z;
+    R[0] = 1.0 - (tyy + tzz); R[1] = txy - twz;         R[2] = txz + twy;
+    R[3] = txy + twz;         R[4] = 1.0 - (txx + tzz); R[5] = tyz - twx;
+    R[6] = txz - twy;         R[7] = tyz + twx;         R[8] = 1.0 - (txx + tyy);
+}
+
+// gaussian.cpp:66-70: each new point's depth in its own frame's camera, Eigen's fixed-size product without FMA,
+// (float)(((Rcw20 p0 + Rcw21 p1) + Rcw22 p2) + tcw2) with p the point in double
+__global__ void __launch_bounds__(256)
+scan_depth_kernel(int n, const float* __restrict__ xyz, double r0, double r1, double r2, double t2, float* __restrict__ depth) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float* p = xyz + 3 * (size_t)i;
+    const double d = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(r0, (double)p[0]), __dmul_rn(r1, (double)p[1])), __dmul_rn(r2, (double)p[2])), t2);
+    depth[i] = __double2float_rn(d);
+}
+
+// the Dataset's colours, rgb / 255.0 in double (gaussian.cpp:65): initialize() reads the doubles, extend() floats of them
+// (gaussian.cpp:517-519)
+template <typename T>
+__global__ void __launch_bounds__(256) scan_colour_kernel(int n3, const uint8_t* __restrict__ rgb, T* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n3) out[i] = (T)__ddiv_rn((double)rgb[i], 255.0);
+}
+
 // Regions of the exchange block that hold one slot per (parity, view slot), in layout order
 enum SlotRegion { COLOUR, FLAGS, EXPOSURE, POSE, N_REGIONS };
 
@@ -265,6 +301,18 @@ struct glic_mapper {
     float* lpips_w = nullptr;
     void* lpips_scratch = nullptr;
     size_t lpips_bytes = 0;
+    // ---- raw frames (glic_mapper_enable_frames / add_frame): the 8-bit image store, chunks of FRAME_CHUNK frames of
+    //      frame_stride bytes that never move, and the scan of the frames since the last training keyframe (device arrays
+    //      of scan_cap points, grown by doubling) ----
+    bool initialized = false;             // initialize or initialize_lidar has run (the next scan extends the map)
+    bool frames_on = false;
+    int frame_k = 1, frame_sky_points = 0, frame_sky_radius = 0;
+    std::vector<uint8_t*> frame_chunks;
+    size_t frame_stride = 0;
+    float *scan_xyz = nullptr, *scan_depth = nullptr;
+    uint8_t* scan_rgb = nullptr;
+    size_t scan_cap = 0;
+    glic_frame_stats fst{};
 };
 
 namespace {
@@ -525,6 +573,15 @@ int forward_settled(glic_mapper* m, const Keyframe& kf, int no_color) {
     return GLIC_OK;
 }
 
+// keyframe kf's float image [3,H,W] into dst on stream s: an add_frame keyframe's 8-bit image decoded from the frame store,
+// any other keyframe's float image copied with `kind`
+int load_gt(glic_mapper* m, const Keyframe& kf, float* dst, cudaMemcpyKind kind, cudaStream_t s) {
+    const int W = m->cfg.width, H = m->cfg.height;
+    if (kf.bgr) return glic_decode_bgr8(H, W, kf.bgr, dst, s);
+    GLIC_CUDA_TRY(cudaMemcpyAsync(dst, kf.image, sizeof(float) * 3 * (size_t)W * H, kind, s));
+    return GLIC_OK;
+}
+
 __global__ void overflow_word_kernel(const GeomHeader* ghdr, float* word) { if (ghdr->overflow) *word = 1.0f; }
 
 // one optimiser step over the view batch `views` (S keyframe indices, slot-major); this rank renders slots [rank*k, rank*k + k)
@@ -552,9 +609,10 @@ int iteration(glic_mapper* m, const int* views) {
         const int sl = m->cfg.rank * m->k + j;
         const Keyframe& kf = m->train[views[sl]];
         const int buf = (int)(m->view_counter++ & 1);
-        // keyframe image H2D on the copy stream (gaussian.cpp:678), overlapping the previous view's backward / Adam
+        // keyframe image H2D (gaussian.cpp:678), or the 8-bit frame's decode, on the copy stream, overlapping the previous
+        // view's backward / Adam
         GLIC_CUDA_TRY(cudaStreamWaitEvent(m->copy_stream, m->gt_free[buf], 0));
-        GLIC_CUDA_TRY(cudaMemcpyAsync(m->gt_dev[buf], kf.image, sizeof(float) * 3 * (size_t)W * H, cudaMemcpyDefault, m->copy_stream));
+        MAP_TRY(load_gt(m, kf, m->gt_dev[buf], cudaMemcpyDefault, m->copy_stream));
         GLIC_CUDA_TRY(cudaEventRecord(m->gt_ready[buf], m->copy_stream));
         MAP_TRY(forward_view(m, kf, 0, j == m->k - 1 ? m->counters_host + 4 * r : nullptr));
         uint8_t* fl = slot<uint8_t>(m, FLAGS, parity, sl);
@@ -661,7 +719,7 @@ int render_scored(glic_mapper* m, int is_train, int index, const char* what) {
     cudaStream_t s = m->stream;
     const int W = m->cfg.width, H = m->cfg.height;
     MAP_TRY(forward_settled(m, kf, 0));
-    GLIC_CUDA_TRY(cudaMemcpyAsync(m->gt_dev[0], kf.image, sizeof(float) * 3 * (size_t)W * H, cudaMemcpyHostToDevice, s));
+    MAP_TRY(load_gt(m, kf, m->gt_dev[0], cudaMemcpyHostToDevice, s));
     const float* E = (is_train && m->expo_on) ? m->expo_E + 12 * (size_t)index : nullptr;
     return eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], E, m->eval_out, m->eval_scratch, m->eval_bytes, s);
 }
@@ -670,6 +728,205 @@ int render_scored(glic_mapper* m, int is_train, int index, const char* what) {
 int read_eval_out(glic_mapper* m, float* out, int n) {
     GLIC_CUDA_TRY(cudaMemcpyAsync(out, m->eval_out, sizeof(float) * n, cudaMemcpyDeviceToHost, m->stream));
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    return GLIC_OK;
+}
+
+// initialize() (gaussian.cpp:212-304) from device arrays: the sky rows, then the n LiDAR rows.  The caller has validated the
+// arguments, sized the arena for sky_points + n rows and hands sky_ws of glic_skybox_init_bytes(sky_points) bytes.
+int initialize_lidar_core(glic_mapper* m, int n, const float* d_pts, const double* d_col, const float* d_dep, double focal, int sky_points,
+                          int sky_radius, void* sky_ws) {
+    const uint32_t S = (uint32_t)sky_points, P = S + (uint32_t)n;
+    cudaStream_t s = m->stream;
+    const size_t nfl = arena_floats(m, m->Pcap);
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->params, 0, nfl * 4, s));
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->m1, 0, nfl * 4, s));
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->m2, 0, nfl * 4, s));
+    float* g[6];                                    // rot, xyz, log-scale, opacity, f_dc, f_rest
+    arena_ptrs(m, m->params, m->Pcap, g);
+    MAP_TRY(glic_skybox_init(sky_points, sky_radius, m->cfg.seed, sky_ws, glic_skybox_init_bytes(sky_points), g[1], g[4], g[2], g[0], g[3], nullptr, s));
+    MAP_TRY(glic_lidar_init(n, d_pts, d_col, d_dep, (double)m->cfg.scaling_scale, focal, g[1] + 3 * (size_t)S, g[4] + 3 * (size_t)S,
+                            g[2] + 3 * (size_t)S, g[0] + 4 * (size_t)S, g[3] + S, s));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    m->P = P;
+    m->n_sky = S;
+    m->st.num_gaussians = P;
+    m->initialized = true;
+    if ((int64_t)16 * P > m->bin_cap) MAP_TRY(set_bin_capacity(m, (int64_t)16 * P));
+    return GLIC_OK;
+}
+
+// extend()'s workspace after its inputs: outputs (keep_idx, xyz, f_dc, log_scale, rot, opacity) | glic_extend's own
+size_t extend_core_carve(void* ws, int n, int W, int H, int** keep, float** out5, void** ext_ws) {
+    Carver c(ws);
+    int* k = c.take<int>(n);
+    const size_t width[5] = {3, 3, 3, 4, 1};
+    for (int q = 0; q < 5; ++q) {
+        float* p = c.take<float>(width[q] * n);
+        if (out5) out5[q] = p;
+    }
+    void* e = c.take<char>(glic_extend_bytes(n, W, H));
+    if (keep) *keep = k;
+    if (ext_ws) *ext_ws = e;
+    return c.total();
+}
+
+// extend() (gaussian.cpp:499-638) on the newest training keyframe from device arrays of n > 0 points.  The caller has
+// drained the ring, sized the arena for P + n rows, recorded m->t0 before staging its inputs and hands ws of
+// extend_core_carve(nullptr, n, W, H, ...) bytes.
+int extend_core(glic_mapper* m, int n, const float* d_pts, const float* d_col, const float* d_dep, void* ws) {
+    cudaStream_t s = m->stream;
+    const int W = m->cfg.width, H = m->cfg.height;
+    const Keyframe& kf = m->train.back();
+    int* d_keep = nullptr;
+    float* o[5];
+    void* d_ws = nullptr;
+    extend_core_carve(ws, n, W, H, &d_keep, o, &d_ws);
+    float *d_xyz = o[0], *d_dc = o[1], *d_ls = o[2], *d_rot = o[3], *d_op = o[4];
+    // alpha-only render of the newest keyframe (gaussian.cpp:506-507); the binning capacity is settled synchronously here
+    if (m->P) {
+        MAP_TRY(forward_settled(m, kf, 1));
+    } else {
+        std::vector<float> ones((size_t)W * H, 1.0f);                                       // empty model: alpha = 1 - T = 0
+        GLIC_CUDA_TRY(cudaMemcpyAsync(m->final_T, ones.data(), sizeof(float) * ones.size(), cudaMemcpyHostToDevice, s));
+        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    }
+    float view[16];
+    std::memcpy(view, kf.cam.view, sizeof(view));
+    if (m->pose_on) {                               // the keyframe's current (possibly refined) pose: its device camera block
+        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+        GLIC_CUDA_TRY(cudaMemcpy(view, kf.cam_dev, sizeof(view), cudaMemcpyDeviceToHost));
+    }
+    float Rcw[9], tcw[3];
+    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Rcw[3 * i + j] = view[4 * j + i];   // view is column-major Rt
+    for (int i = 0; i < 3; ++i) tcw[i] = view[12 + i];
+    int count = 0;
+    MAP_TRY(glic_extend(n, d_pts, d_col, d_dep, Rcw, tcw, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, W, H, m->final_T, m->cfg.scaling_scale,
+                        d_ws, glic_extend_bytes(n, W, H), d_keep, d_xyz, d_dc, d_ls, d_rot, d_op, &count, s));
+    MAP_TRY(glic_arena_append(m->params, m->m1, m->m2, m->P, m->Pcap, (uint32_t)m->M, (uint32_t)count, d_xyz, d_dc, d_ls, d_rot, d_op, s));
+    GLIC_CUDA_TRY(cudaEventRecord(m->t1, s));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    cudaEventElapsedTime(&m->st.ms_extend, m->t0, m->t1);
+    m->P += (uint32_t)count;
+    m->st.num_gaussians = m->P;
+    m->st.last_inserted = (uint32_t)count;
+    return GLIC_OK;
+}
+
+// room in the extend() staging for n points and the arena for P + n rows (ring drained first)
+int extend_prepare(glic_mapper* m, int n, size_t input_bytes) {
+    MAP_TRY(poll_ring(m, true));
+    MAP_TRY(set_capacity(m, std::max<uint32_t>(m->P + (uint32_t)n, m->Pcap < m->P + (uint32_t)n ? 2 * m->Pcap : 0)));
+    return reserve_staging(m, input_bytes + extend_core_carve(nullptr, n, m->cfg.width, m->cfg.height, nullptr, nullptr, nullptr));
+}
+
+// glic_mapper_add_keyframe's body; a keyframe of add_frame has image = nullptr and its 8-bit image in the frame store
+int add_keyframe_core(glic_mapper* m, const float* R_wc, const float* t_wc, const float* image, const uint8_t* bgr, int is_train) {
+    Keyframe kf;
+    std::memcpy(kf.R_wc, R_wc, sizeof(kf.R_wc)); std::memcpy(kf.t_wc, t_wc, sizeof(kf.t_wc));
+    kf.image = image;
+    kf.bgr = bgr;
+    camera_block(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, kf.R_wc, kf.t_wc, kf.cam);
+    MAP_TRY(dev_alloc((void**)&kf.cam_dev, 36 * sizeof(float), false));
+    GLIC_CUDA_TRY(cudaMemcpy(kf.cam_dev, kf.cam.view, 36 * sizeof(float), cudaMemcpyHostToDevice));   // view | proj | campos are contiguous
+    kf.view.viewmatrix = kf.cam_dev; kf.view.projmatrix = kf.cam_dev + 16; kf.view.campos = kf.cam_dev + 32;
+    kf.view.tan_fovx = kf.cam.tanfovx; kf.view.tan_fovy = kf.cam.tanfovy;
+    kf.view.limx_neg = kf.cam.lim[0]; kf.view.limx_pos = kf.cam.lim[1]; kf.view.limy_neg = kf.cam.lim[2]; kf.view.limy_pos = kf.cam.lim[3];
+    kf.view.width = m->cfg.width; kf.view.height = m->cfg.height;
+    if (is_train && m->expo_on) {
+        MAP_TRY(expo_reserve(m, m->train.size() + 1));
+        MAP_TRY(expo_reset(m, m->train.size(), m->train.size() + 1));
+    }
+    (is_train ? m->train : m->test).push_back(kf);
+    if (is_train && m->pose_on) {                  // starts at its given pose with zero state
+        MAP_TRY(pose_reserve(m, m->train.size()));
+        MAP_TRY(pose_write(m, m->train.size() - 1, kf.R_wc, kf.t_wc, true));
+    }
+    return GLIC_OK;
+}
+
+// copies frame f's image into the next slot of the frame store (a new chunk when the last one is full), dropping the row
+// padding; returns the slot
+int frame_store_push(glic_mapper* m, const glic_frame* f, const uint8_t** slot_out) {
+    const size_t W3 = 3 * (size_t)m->cfg.width, H = (size_t)m->cfg.height, idx = m->fst.frames;
+    if (idx / FRAME_CHUNK >= m->frame_chunks.size()) {
+        void* chunk = nullptr;
+        MAP_TRY(dev_alloc(&chunk, FRAME_CHUNK * m->frame_stride, false));
+        m->frame_chunks.push_back(static_cast<uint8_t*>(chunk));
+        m->fst.image_bytes += FRAME_CHUNK * m->frame_stride;
+    }
+    uint8_t* dst = m->frame_chunks[idx / FRAME_CHUNK] + (idx % FRAME_CHUNK) * m->frame_stride;
+    GLIC_CUDA_TRY(cudaMemcpy2DAsync(dst, W3, f->bgr, f->row_bytes, W3, H, cudaMemcpyHostToDevice, m->stream));
+    *slot_out = dst;
+    return GLIC_OK;
+}
+
+// appends frame f's points to the scan buffer (grown by doubling) with their depths in the frame's camera, R = R_wc in double
+int scan_append(glic_mapper* m, const glic_frame* f, const double R[9]) {
+    const size_t n = (size_t)f->n_points, have = m->fst.pending_points;
+    if (n == 0) return GLIC_OK;
+    cudaStream_t s = m->stream;
+    if (have + n > m->scan_cap) {
+        const size_t cap = std::max<size_t>({have + n, 2 * m->scan_cap, 4096});
+        float *xyz = nullptr, *dep = nullptr;
+        uint8_t* rgb = nullptr;
+        MAP_TRY(dev_alloc((void**)&xyz, cap * 3 * sizeof(float), false));
+        MAP_TRY(dev_alloc((void**)&rgb, cap * 3, false));
+        MAP_TRY(dev_alloc((void**)&dep, cap * sizeof(float), false));
+        if (have) {
+            GLIC_CUDA_TRY(cudaMemcpyAsync(xyz, m->scan_xyz, have * 3 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+            GLIC_CUDA_TRY(cudaMemcpyAsync(rgb, m->scan_rgb, have * 3, cudaMemcpyDeviceToDevice, s));
+            GLIC_CUDA_TRY(cudaMemcpyAsync(dep, m->scan_depth, have * sizeof(float), cudaMemcpyDeviceToDevice, s));
+        }
+        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+        cudaFree(m->scan_xyz); cudaFree(m->scan_rgb); cudaFree(m->scan_depth);
+        m->scan_xyz = xyz; m->scan_rgb = rgb; m->scan_depth = dep;
+        m->scan_cap = cap;
+    }
+    GLIC_CUDA_TRY(cudaMemcpyAsync(m->scan_xyz + 3 * have, f->xyz, n * 3 * sizeof(float), cudaMemcpyHostToDevice, s));
+    GLIC_CUDA_TRY(cudaMemcpyAsync(m->scan_rgb + 3 * have, f->rgb, n * 3, cudaMemcpyHostToDevice, s));
+    // R_cw = R^T; t_cw = -R_cw t_wc in the product's order (gaussian.cpp:66-67)
+    const double* t = f->t_wc;
+    const double tcw2 = -(((R[2] * t[0]) + (R[5] * t[1])) + (R[8] * t[2]));
+    scan_depth_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((int)n, m->scan_xyz + 3 * have, R[2], R[5], R[8], tcw2, m->scan_depth + have);
+    GLIC_LAUNCH_CHECK();
+    m->fst.pending_points = (uint32_t)(have + n);
+    return GLIC_OK;
+}
+
+// mapping.cpp:158-174 at a training keyframe: the accumulated scan initializes the map, or extends it; then it is emptied
+int scan_handoff(glic_mapper* m) {
+    const int n = (int)m->fst.pending_points;
+    cudaStream_t s = m->stream;
+    const unsigned blocks = (unsigned)((3 * (size_t)n + 255) / 256);
+    if (!m->initialized) {
+        const int S = m->frame_sky_points;
+        MAP_TRY(set_capacity(m, (uint32_t)S + (uint32_t)n));
+        Carver c(nullptr);
+        c.take<double>((size_t)3 * n); c.take<char>(glic_skybox_init_bytes(S));
+        MAP_TRY(reserve_staging(m, c.total()));
+        c = Carver(m->extend_ws);
+        double* d_col = c.take<double>((size_t)3 * n);
+        void* sky_ws = c.take<char>(glic_skybox_init_bytes(S));
+        scan_colour_kernel<double><<<blocks, 256, 0, s>>>(3 * n, m->scan_rgb, d_col);
+        GLIC_LAUNCH_CHECK();
+        const double focal = ((double)m->cfg.fx + (double)m->cfg.fy) / 2;
+        MAP_TRY(initialize_lidar_core(m, n, m->scan_xyz, d_col, m->scan_depth, focal, S, m->frame_sky_radius, sky_ws));
+    } else {
+        m->st.last_inserted = 0;
+        if (n > 0) {
+            Carver c(nullptr);
+            c.take<float>((size_t)3 * n);
+            MAP_TRY(extend_prepare(m, n, c.total()));
+            c = Carver(m->extend_ws);
+            float* d_col = c.take<float>((size_t)3 * n);
+            void* ws = c.take<char>(0);
+            GLIC_CUDA_TRY(cudaEventRecord(m->t0, s));
+            scan_colour_kernel<float><<<blocks, 256, 0, s>>>(3 * n, m->scan_rgb, d_col);
+            GLIC_LAUNCH_CHECK();
+            MAP_TRY(extend_core(m, n, m->scan_xyz, d_col, m->scan_depth, ws));
+        }
+    }
+    m->fst.pending_points = 0;
     return GLIC_OK;
 }
 
@@ -738,6 +995,9 @@ int glic_mapper_destroy(glic_mapper* m) {
     void* keyframe_state[] = {m->expo_E, m->expo_adam.m, m->expo_adam.v, m->expo_adam.t, m->pose_T, m->pose_f, m->pose_adam.m,
                               m->pose_adam.v, m->pose_adam.t, m->pose_part, m->lpips_w, m->lpips_scratch};
     for (void* p : keyframe_state) if (p) cudaFree(p);
+    for (uint8_t* p : m->frame_chunks) cudaFree(p);
+    void* scan[] = {m->scan_xyz, m->scan_rgb, m->scan_depth};
+    for (void* p : scan) if (p) cudaFree(p);
     for (auto& kf : m->train) if (kf.cam_dev) cudaFree(kf.cam_dev);
     for (auto& kf : m->test) if (kf.cam_dev) cudaFree(kf.cam_dev);
     if (m->counters_host) cudaFreeHost(m->counters_host);
@@ -772,6 +1032,7 @@ int glic_mapper_initialize(glic_mapper* m, uint32_t P, const float* xyz, const f
     m->P = P;
     m->n_sky = 0;
     m->st.num_gaussians = P;
+    m->initialized = true;
     if ((int64_t)16 * P > m->bin_cap) MAP_TRY(set_bin_capacity(m, (int64_t)16 * P));
     return GLIC_OK;
 }
@@ -783,8 +1044,7 @@ int glic_mapper_initialize_lidar(glic_mapper* m, int n, const float* points, con
     if (n < 1 || sky_points < 0 || (sky_points > 0 && sky_radius <= 0) || (int64_t)n + sky_points > INT32_MAX / 4) {
         set_error("mapper_initialize_lidar: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT;
     }
-    const uint32_t S = (uint32_t)sky_points, P = S + (uint32_t)n;
-    MAP_TRY(set_capacity(m, P));
+    MAP_TRY(set_capacity(m, (uint32_t)sky_points + (uint32_t)n));
     cudaStream_t s = m->stream;
     // staging: points | colors | depth | the sky's dist2 and knn workspace
     Carver c(nullptr);
@@ -792,26 +1052,11 @@ int glic_mapper_initialize_lidar(glic_mapper* m, int n, const float* points, con
     MAP_TRY(reserve_staging(m, c.total()));
     c = Carver(m->extend_ws);
     float* d_pts = c.take<float>((size_t)3 * n); double* d_col = c.take<double>((size_t)3 * n); float* d_dep = c.take<float>(n);
-    const size_t sky_bytes = glic_skybox_init_bytes(sky_points);
-    void* d_sky = c.take<char>(sky_bytes);
-    const size_t nfl = arena_floats(m, m->Pcap);
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->params, 0, nfl * 4, s));
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->m1, 0, nfl * 4, s));
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->m2, 0, nfl * 4, s));
+    void* d_sky = c.take<char>(glic_skybox_init_bytes(sky_points));
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_pts, points, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, s));
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_col, colors, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, s));
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_dep, depth_rsp, sizeof(float) * n, cudaMemcpyHostToDevice, s));
-    float* g[6];                                    // rot, xyz, log-scale, opacity, f_dc, f_rest
-    arena_ptrs(m, m->params, m->Pcap, g);
-    MAP_TRY(glic_skybox_init(sky_points, sky_radius, m->cfg.seed, d_sky, sky_bytes, g[1], g[4], g[2], g[0], g[3], nullptr, s));
-    MAP_TRY(glic_lidar_init(n, d_pts, d_col, d_dep, (double)m->cfg.scaling_scale, focal, g[1] + 3 * (size_t)S, g[4] + 3 * (size_t)S,
-                            g[2] + 3 * (size_t)S, g[0] + 4 * (size_t)S, g[3] + S, s));
-    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-    m->P = P;
-    m->n_sky = S;
-    m->st.num_gaussians = P;
-    if ((int64_t)16 * P > m->bin_cap) MAP_TRY(set_bin_capacity(m, (int64_t)16 * P));
-    return GLIC_OK;
+    return initialize_lidar_core(m, n, d_pts, d_col, d_dep, focal, sky_points, sky_radius, d_sky);
 }
 
 int glic_mapper_sky_rows(glic_mapper* m, uint32_t* out) {
@@ -822,26 +1067,7 @@ int glic_mapper_sky_rows(glic_mapper* m, uint32_t* out) {
 
 int glic_mapper_add_keyframe(glic_mapper* m, const glic_keyframe* kfi, int is_train) {
     if (!m || !kfi || !kfi->image) { set_error("mapper_add_keyframe: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    Keyframe kf;
-    std::memcpy(kf.R_wc, kfi->R_wc, sizeof(kf.R_wc)); std::memcpy(kf.t_wc, kfi->t_wc, sizeof(kf.t_wc));
-    kf.image = kfi->image;
-    camera_block(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, kf.R_wc, kf.t_wc, kf.cam);
-    MAP_TRY(dev_alloc((void**)&kf.cam_dev, 36 * sizeof(float), false));
-    GLIC_CUDA_TRY(cudaMemcpy(kf.cam_dev, kf.cam.view, 36 * sizeof(float), cudaMemcpyHostToDevice));   // view | proj | campos are contiguous
-    kf.view.viewmatrix = kf.cam_dev; kf.view.projmatrix = kf.cam_dev + 16; kf.view.campos = kf.cam_dev + 32;
-    kf.view.tan_fovx = kf.cam.tanfovx; kf.view.tan_fovy = kf.cam.tanfovy;
-    kf.view.limx_neg = kf.cam.lim[0]; kf.view.limx_pos = kf.cam.lim[1]; kf.view.limy_neg = kf.cam.lim[2]; kf.view.limy_pos = kf.cam.lim[3];
-    kf.view.width = m->cfg.width; kf.view.height = m->cfg.height;
-    if (is_train && m->expo_on) {
-        MAP_TRY(expo_reserve(m, m->train.size() + 1));
-        MAP_TRY(expo_reset(m, m->train.size(), m->train.size() + 1));
-    }
-    (is_train ? m->train : m->test).push_back(kf);
-    if (is_train && m->pose_on) {                  // starts at its given pose with zero state
-        MAP_TRY(pose_reserve(m, m->train.size()));
-        MAP_TRY(pose_write(m, m->train.size() - 1, kf.R_wc, kf.t_wc, true));
-    }
-    return GLIC_OK;
+    return add_keyframe_core(m, kfi->R_wc, kfi->t_wc, kfi->image, nullptr, is_train);
 }
 
 int glic_mapper_extend(glic_mapper* m, int n, const float* points, const float* colors, const float* depth_rsp) {
@@ -849,49 +1075,81 @@ int glic_mapper_extend(glic_mapper* m, int n, const float* points, const float* 
     m->st.last_inserted = 0;
     if (n == 0) return GLIC_OK;
     if (m->train.empty()) { set_error("mapper_extend: no training keyframe yet"); return GLIC_ERR_INVALID_ARGUMENT; }
-    MAP_TRY(poll_ring(m, true));
-    MAP_TRY(set_capacity(m, std::max<uint32_t>(m->P + (uint32_t)n, m->Pcap < m->P + (uint32_t)n ? 2 * m->Pcap : 0)));
-    cudaStream_t s = m->stream;
-    const int W = m->cfg.width, H = m->cfg.height;
-    const Keyframe& kf = m->train.back();
-    // staging: points | colors | depth | outputs (keep_idx, xyz, f_dc, log_scale, rot, opacity) | glic_extend's own workspace
-    MAP_TRY(reserve_staging(m, glic_extend_bytes(n, W, H) + (size_t)n * (3 + 3 + 1 + 1 + 3 + 3 + 3 + 4 + 1) * 4 + 4096));
-    Carver c(m->extend_ws);
+    // staging: points | colors | depth | extend_core's workspace
+    Carver c(nullptr);
+    c.take<float>((size_t)3 * n); c.take<float>((size_t)3 * n); c.take<float>(n);
+    MAP_TRY(extend_prepare(m, n, c.total()));
+    c = Carver(m->extend_ws);
     float* d_pts = c.take<float>((size_t)3 * n); float* d_col = c.take<float>((size_t)3 * n); float* d_dep = c.take<float>(n);
-    int* d_keep = c.take<int>(n); float* d_xyz = c.take<float>((size_t)3 * n); float* d_dc = c.take<float>((size_t)3 * n);
-    float* d_ls = c.take<float>((size_t)3 * n); float* d_rot = c.take<float>((size_t)4 * n); float* d_op = c.take<float>(n);
-    void* d_ws = c.take<char>(glic_extend_bytes(n, W, H));
+    void* ws = c.take<char>(0);
+    cudaStream_t s = m->stream;
     GLIC_CUDA_TRY(cudaEventRecord(m->t0, s));
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_pts, points, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, s));
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_col, colors, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, s));
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_dep, depth_rsp, sizeof(float) * n, cudaMemcpyHostToDevice, s));
-    // alpha-only render of the newest keyframe (gaussian.cpp:506-507); the binning capacity is settled synchronously here
-    if (m->P) {
-        MAP_TRY(forward_settled(m, kf, 1));
-    } else {
-        std::vector<float> ones((size_t)W * H, 1.0f);                                       // empty model: alpha = 1 - T = 0
-        GLIC_CUDA_TRY(cudaMemcpyAsync(m->final_T, ones.data(), sizeof(float) * ones.size(), cudaMemcpyHostToDevice, s));
-        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    return extend_core(m, n, d_pts, d_col, d_dep, ws);
+}
+
+int glic_mapper_enable_frames(glic_mapper* m, int select_every_k_frame, int sky_points, int sky_radius) {
+    if (!m) { set_error("mapper_enable_frames: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (m->frames_on) { set_error("mapper_enable_frames: frames are already enabled"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (select_every_k_frame < 1 || sky_points < 0 || (sky_points > 0 && sky_radius <= 0) || sky_points > INT32_MAX / 4) {
+        set_error("mapper_enable_frames: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT;
     }
-    float view[16];
-    std::memcpy(view, kf.cam.view, sizeof(view));
-    if (m->pose_on) {                               // the keyframe's current (possibly refined) pose: its device camera block
-        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-        GLIC_CUDA_TRY(cudaMemcpy(view, kf.cam_dev, sizeof(view), cudaMemcpyDeviceToHost));
+    m->frames_on = true;
+    m->frame_k = select_every_k_frame;
+    m->frame_sky_points = sky_points;
+    m->frame_sky_radius = sky_radius;
+    m->frame_stride = ((size_t)3 * m->cfg.width * m->cfg.height + 255) & ~size_t(255);
+    return GLIC_OK;
+}
+
+int glic_mapper_add_frame(glic_mapper* m, const glic_frame* f, int* is_keyframe) {
+    if (!m || !f || !f->bgr || (f->n_points > 0 && (!f->xyz || !f->rgb))) { set_error("mapper_add_frame: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!m->frames_on) { set_error("mapper_add_frame: frames are not enabled (glic_mapper_enable_frames)"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (f->row_bytes < 3 * (size_t)m->cfg.width || f->n_points < 0) { set_error("mapper_add_frame: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const size_t pending = (size_t)m->fst.pending_points + (size_t)f->n_points;
+    if (pending + (size_t)m->frame_sky_points > INT32_MAX / 4) { set_error("mapper_add_frame: too many scan points before a keyframe"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const int train = (m->fst.frames + 1) % (uint32_t)m->frame_k == 0;
+    // the reference's assert(num > 0) of initialize() (gaussian.cpp:216)
+    if (train && !m->initialized && pending == 0) { set_error("mapper_add_frame: the first keyframe has no scan points"); return GLIC_ERR_INVALID_ARGUMENT; }
+    double R[9];
+    quat_rotation(f->q_wc, R);
+    float R_wc[9], t_wc[3];
+    for (int e = 0; e < 9; ++e) R_wc[e] = (float)R[e];
+    for (int i = 0; i < 3; ++i) t_wc[i] = (float)f->t_wc[i];
+    const uint8_t* bgr = nullptr;
+    MAP_TRY(frame_store_push(m, f, &bgr));
+    MAP_TRY(scan_append(m, f, R));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));      // the caller's buffers are free again
+    MAP_TRY(add_keyframe_core(m, R_wc, t_wc, nullptr, bgr, train));
+    ++m->fst.frames;
+    ++(train ? m->fst.train : m->fst.test);
+    if (train) MAP_TRY(scan_handoff(m));
+    if (is_keyframe) *is_keyframe = train;
+    return GLIC_OK;
+}
+
+int glic_mapper_keyframe_image(glic_mapper* m, int is_train, int index, float* rgb_host) {
+    if (!m || !rgb_host) { set_error("mapper_keyframe_image: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const auto& list = is_train ? m->train : m->test;
+    if (index < 0 || index >= (int)list.size()) { set_error("mapper_keyframe_image: keyframe index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const Keyframe& kf = list[index];
+    const size_t bytes = sizeof(float) * 3 * (size_t)m->cfg.width * m->cfg.height;
+    if (!kf.bgr) {
+        GLIC_CUDA_TRY(cudaMemcpy(rgb_host, kf.image, bytes, cudaMemcpyDefault));
+        return GLIC_OK;
     }
-    float Rcw[9], tcw[3];
-    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Rcw[3 * i + j] = view[4 * j + i];   // view is column-major Rt
-    for (int i = 0; i < 3; ++i) tcw[i] = view[12 + i];
-    int count = 0;
-    MAP_TRY(glic_extend(n, d_pts, d_col, d_dep, Rcw, tcw, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, W, H, m->final_T, m->cfg.scaling_scale,
-                        d_ws, glic_extend_bytes(n, W, H), d_keep, d_xyz, d_dc, d_ls, d_rot, d_op, &count, s));
-    MAP_TRY(glic_arena_append(m->params, m->m1, m->m2, m->P, m->Pcap, (uint32_t)m->M, (uint32_t)count, d_xyz, d_dc, d_ls, d_rot, d_op, s));
-    GLIC_CUDA_TRY(cudaEventRecord(m->t1, s));
-    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-    cudaEventElapsedTime(&m->st.ms_extend, m->t0, m->t1);
-    m->P += (uint32_t)count;
-    m->st.num_gaussians = m->P;
-    m->st.last_inserted = (uint32_t)count;
+    MAP_TRY(poll_ring(m, true));                          // the iterations' use of gt_dev[0] has finished (see render_scored)
+    MAP_TRY(load_gt(m, kf, m->gt_dev[0], cudaMemcpyHostToDevice, m->stream));
+    GLIC_CUDA_TRY(cudaMemcpyAsync(rgb_host, m->gt_dev[0], bytes, cudaMemcpyDeviceToHost, m->stream));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    return GLIC_OK;
+}
+
+int glic_mapper_frames_get(glic_mapper* m, glic_frame_stats* out) {
+    if (!m || !out) { set_error("mapper_frames_get: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    *out = m->fst;
     return GLIC_OK;
 }
 

@@ -96,6 +96,43 @@ class Mapper:
             kf.image = img.ctypes.data
         capi.check(capi.lib.glic_mapper_add_keyframe(self._h, C.byref(kf), int(bool(train))), "mapper_add_keyframe")
 
+    def enable_frames(self, select_every_k_frame=5, sky_points=0, sky_radius=0):
+        """Accept raw frames through add_frame (config/*.yaml: select_every_k_frame, skybox_points_num, skybox_radius)."""
+        capi.check(capi.lib.glic_mapper_enable_frames(self._h, int(select_every_k_frame), int(sky_points), int(sky_radius)),
+                   "mapper_enable_frames")
+
+    def add_frame(self, q_wc, t_wc, bgr, xyz, rgb):
+        """Dataset::addFrame (gaussian.cpp:41-111) and the keyframe hand-off of mapping.cpp:158-174 on the GPU.  q_wc: (x, y, z, w)
+        odometry orientation; t_wc: position; bgr: [H,W,3] uint8 BGR8 image (a row-padded view such as a[:, :W] of a wider
+        array is passed with its row stride); xyz: [n,3] float32 world points; rgb: [n,3] uint8.  Returns True for a
+        training keyframe, False for a held-out one."""
+        f = capi.Frame()
+        f.q_wc[:] = [float(x) for x in np.asarray(q_wc, np.float64).reshape(4)]
+        f.t_wc[:] = [float(x) for x in np.asarray(t_wc, np.float64).reshape(3)]
+        img = np.asarray(bgr)
+        if img.dtype != np.uint8 or img.ndim != 3 or img.shape != (self.H, self.W, 3) or img.strides[1:] != (3, 1):
+            raise ValueError("bgr must be a [%d,%d,3] uint8 array with packed pixels" % (self.H, self.W))
+        f.bgr, f.row_bytes = img.ctypes.data, int(img.strides[0])
+        pts = _f32(xyz).reshape(-1, 3)
+        col = np.ascontiguousarray(rgb, dtype=np.uint8).reshape(-1, 3)
+        if pts.shape[0] != col.shape[0]:
+            raise ValueError("xyz and rgb must have the same number of points")
+        f.n_points, f.xyz, f.rgb = int(pts.shape[0]), _p(pts), _p(col)
+        out = C.c_int()
+        capi.check(capi.lib.glic_mapper_add_frame(self._h, C.byref(f), C.byref(out)), "mapper_add_frame")
+        return bool(out.value)
+
+    def keyframe_image(self, index, train=True):
+        """The [3,H,W] float32 image the loss sees for a keyframe (decoded from 8 bits for add_frame keyframes)."""
+        out = np.empty((3, self.H, self.W), np.float32)
+        capi.check(capi.lib.glic_mapper_keyframe_image(self._h, int(bool(train)), int(index), _p(out)), "mapper_keyframe_image")
+        return out
+
+    def frames_get(self):
+        st = capi.FrameStats()
+        capi.check(capi.lib.glic_mapper_frames_get(self._h, C.byref(st)), "mapper_frames_get")
+        return st
+
     def extend(self, points, colors, depth_rsp):
         pts, col, dep = _f32(points), _f32(colors), _f32(depth_rsp)
         capi.check(capi.lib.glic_mapper_extend(self._h, int(pts.shape[0]), _p(pts), _p(col), _p(dep)), "mapper_extend")

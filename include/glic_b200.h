@@ -232,6 +232,13 @@ GLIC_API size_t glic_skybox_init_bytes(int n);
 GLIC_API int glic_skybox_init(int n, int radius, uint64_t seed, void* ws, size_t ws_bytes, float* xyz, float* f_dc,
                               float* log_scale, float* rot, float* opacity_logit, float* uv, void* stream);
 
+/* 8-bit camera frame -> the float image the loss sees (Dataset::addFrame, gaussian.cpp:44-49: cv_bridge BGR8,
+ * cvtColor(BGR2RGB), convertTo(CV_32FC3, 1.0f / 255.0f)).  bgr: packed [H][W][3] bytes (B, G, R); rgb: [3][H][W] floats,
+ *     rgb[c][y][x] = __fmul_rn((float)bgr[y][x][2 - c], 1.0f / 255.0f)
+ * one rounding of x * fl32(1/255), which is what OpenCV's 8U -> 32F convertTo computes; it is not (float)(x / 255.0), which
+ * differs for 126 of the 256 byte values.  No host synchronisation. */
+GLIC_API int glic_decode_bgr8(int H, int W, const uint8_t* bgr, float* rgb, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * On-disk map (SURVEY 8f rank 4).  Replaces GaussianModel::saveMap (gaussian.cpp:305-397, through tinyply.h:588-703):
  * binary little-endian PLY, element vertex, float properties x y z | f_dc_0..2 | f_rest_0..3M-1 | opacity | scale_0..2 |
@@ -386,8 +393,9 @@ GLIC_API int glic_arena_regrow(const float* src, uint32_t Pcap_src, float* dst, 
 /* ---------------------------------------------------------------------------------------
  * Native mapping host (SURVEY 8f ranks 1-4): the C++ counterpart of GaussianModel + extend() + optimize() +
  * evaluateVisualQuality() + saveMap() (gaussian.cpp:113-830) on top of the kernels above -- one object per GPU, no
- * torch, no Python.  The mapper OWNS its device memory (arena, Adam state, workspaces, keyframe images stay pinned on
- * the host like Camera::original_image_, gaussian.cpp:80): it is the host of the loop, not an operator.
+ * torch, no Python.  The mapper OWNS its device memory (arena, Adam state, workspaces; float keyframe images stay pinned on
+ * the host like Camera::original_image_, gaussian.cpp:80, frames of glic_mapper_add_frame are kept as 8 bits on the device):
+ * it is the host of the loop, not an operator.
  *
  *   create -> initialize(raw parameters) | initialize_lidar(first scan) -> { add_keyframe -> [extend] -> optimize }*
  *          -> evaluate / save_map
@@ -533,6 +541,50 @@ GLIC_API int glic_mapper_pose_adam_state(glic_mapper* m, int index, float* exp_a
  * Rt) | proj[16] (column-major P*Rt) | campos[3] | tan_fovx, tan_fovy | limx_neg, limx_pos, limy_neg, limy_pos. */
 GLIC_API int glic_camera_block(int width, int height, float fx, float fy, float cx, float cy, const float* R_wc /*[9] row-major*/,
                                const float* t_wc /*[3]*/, float* out41);
+/* Raw frames (Dataset::addFrame, gaussian.cpp:41-111, and the keyframe hand-off of mapping.cpp:158-174): the host feeds every
+ * aligned camera frame with its odometry pose and LiDAR scan; the mapper selects the keyframes, keeps each image as 8 bits
+ * in HBM and builds or extends the map on the GPU.  optimize() stays the caller's call (mapping.cpp:178).
+ *   glic_mapper_enable_frames(m, k, sky_points, sky_radius): select_every_k_frame (>= 1) and the skybox settings of the
+ *   initial map (skybox_points_num, skybox_radius; sky_radius > 0 when sky_points > 0).  Once per mapper, before the first
+ *   add_frame; a second call returns GLIC_ERR_INVALID_ARGUMENT.
+ *   glic_mapper_add_frame(m, f, is_keyframe):
+ *   - R = Eigen::Quaterniond(w, x, y, z).toRotationMatrix() in double, Eigen's formula and operation order, no normalisation;
+ *     the keyframe's float pose is R_wc = (float)R, t_wc = (float)t, and its camera block is glic_camera_block of those
+ *     floats (the reference's Camera rounds t_cw from the doubles instead: t_cw may differ by 1 ulp);
+ *   - the image is copied once into a mapper-owned device store (packed HWC BGR8, row padding dropped, allocated in chunks
+ *     that never move); the mapper keeps no host pointer;
+ *   - the points are appended to a device scan buffer with depth_rsp = (float)(((Rcw20 p0 + Rcw21 p1) + Rcw22 p2) + tcw2) in
+ *     double without FMA, p = (double)xyz, R_cw = R^T, t_cw = -R_cw t_wc in the same order (gaussian.cpp:64-70);
+ *   - the frame is a training keyframe iff (frames added before it + 1) % k == 0, a held-out keyframe otherwise;
+ *   - at a training keyframe the accumulated scan initializes the map (glic_mapper_initialize_lidar with the enable_frames
+ *     sky, colours (double)c / 255.0, focal = ((double)fx + (double)fy) / 2 of the configuration) if neither initialize
+ *     nor initialize_lidar has run, and extends it otherwise (glic_mapper_extend with colours (float)((double)c / 255.0));
+ *     either way the scan buffer is emptied.
+ *   A NULL mapper, frame or pointer (xyz / rgb may be NULL when n_points is 0), row_bytes < 3 W, n_points < 0, frames not
+ *   enabled, or a first training keyframe with an empty accumulated scan return GLIC_ERR_INVALID_ARGUMENT and change
+ *   nothing.  Synchronises.  *is_keyframe (optional) is 1 for a training keyframe, 0 for a held-out one.
+ *   Frame keyframes train, evaluate and render like glic_keyframe ones: the 8-bit image is decoded on the device
+ *   (glic_decode_bgr8) where the float image would be copied, so an iteration moves no image bytes over PCIe.
+ *   glic_mapper_keyframe_image writes the float [3,H,W] image the loss sees of any keyframe to rgb_host (synchronises).
+ *   glic_mapper_frames_get returns the counters below. */
+typedef struct glic_frame {
+    double q_wc[4];                /* odometry orientation, geometry_msgs order (x, y, z, w) */
+    double t_wc[3];
+    const uint8_t* bgr;            /* host [H][row_bytes]: BGR8 rows of 3 W bytes (sensor_msgs/Image "bgr8", cv_bridge BGR8) */
+    size_t row_bytes;              /* >= 3 W */
+    int n_points;                  /* >= 0 */
+    const float* xyz;              /* host [n,3], world frame (PCL PointXYZRGB x, y, z) */
+    const uint8_t* rgb;            /* host [n,3] (PCL r, g, b) */
+} glic_frame;
+typedef struct glic_frame_stats {
+    uint32_t frames, train, test;  /* frames added so far, and how many became training / held-out keyframes */
+    uint32_t pending_points;       /* scan points waiting for the next training keyframe */
+    uint64_t image_bytes;          /* device bytes held by the 8-bit frame store */
+} glic_frame_stats;
+GLIC_API int glic_mapper_enable_frames(glic_mapper* m, int select_every_k_frame, int sky_points, int sky_radius);
+GLIC_API int glic_mapper_add_frame(glic_mapper* m, const glic_frame* f, int* is_keyframe /* may be NULL */);
+GLIC_API int glic_mapper_keyframe_image(glic_mapper* m, int is_train, int index, float* rgb_host /* [3,H,W] */);
+GLIC_API int glic_mapper_frames_get(glic_mapper* m, glic_frame_stats* out);
 
 /* ---------------------------------------------------------------------------------------
  * Stage timing (cudaEvent pairs recorded on the launching stream around each stage; off by
