@@ -81,11 +81,15 @@ def _cov3d(scales, rots):
     return np.einsum("pij,pj,pkj->pik", R, s2, R)
 
 
-def pose_gradient(g, cam, fwd, bwd, parts=False):
+def pose_gradient(g, cam, fwd, bwd, parts=False, rows=None, magnitude=False):
     """dL/d(rho, omega) [6] float64 of one view, from the oracle's forward (radii) and backward (dL_dmeans2D, dL_dconic,
     dL_dmeans3D).  g: the activated Gaussians handed to Oracle.forward.  parts=True also returns the translation identity's
-    right-hand side W * sum_i dL_dmeans3D_i."""
+    right-hand side W * sum_i dL_dmeans3D_i.  rows: sum only over these Gaussians (indices; default all), e.g. the sky rows
+    alone.  magnitude=True returns [2, 6] instead: the gradient and sum_i |term_i| over its per-Gaussian terms, the scale of
+    the rounding error of a float32 evaluation of each term."""
     vis = np.flatnonzero(np.asarray(fwd["radii"])[:int(np.asarray(g["means"]).shape[0])] > 0)
+    if rows is not None:
+        vis = np.intersect1d(vis, np.asarray(rows))
     view = np.asarray(cam["view"], np.float64).reshape(4, 4).T       # row-major Rt
     Wm, tv = view[:3, :3], view[:3, 3]
     pr = np.asarray(cam["proj"], np.float64)                         # column-major
@@ -138,6 +142,10 @@ def pose_gradient(g, cam, fwd, bwd, parts=False):
     rho = gview.sum(0) + Wm @ d.sum(0)
     omega = np.cross(pv, gview).sum(0) + np.cross(np.broadcast_to(Wm.T[None], G.shape), G.transpose(0, 2, 1)).sum((0, 1))
     out = np.concatenate([rho, omega])
+    if magnitude:
+        terms = np.concatenate([gview + d @ Wm.T, np.cross(pv, gview)
+                                + np.cross(np.broadcast_to(Wm.T[None], G.shape), G.transpose(0, 2, 1)).sum(1)], 1)
+        return np.stack([out, np.abs(terms).sum(0)])
     if parts:
         return out, Wm @ dm3.sum(0)
     return out

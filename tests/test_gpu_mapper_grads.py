@@ -152,9 +152,10 @@ def _yardstick(ref, rows, what):
     print("%s: f32 oracle vs f64 oracle, max|diff|/max|ref|: %s" % (what, {g: "%.2e" % x for g, x in d.items()}))
 
 
-def _compare(got, ref, rows, what, groups=GROUPS):
+def _compare(got, ref, rows, what, groups=GROUPS, rtol=None):
     """grad_close (test_gpu_parity.py's tolerances) on every group over the rows that stepped; the edge rows are kept out of
-    the rotation group, whose scale the 1e12 factor of the tiny quaternion would set."""
+    the rotation group, whose scale the 1e12 factor of the tiny quaternion would set.  rtol: {group: norm tolerance} where a
+    caller has measured that the f32 oracle itself is further than GRAD_RTOL from the f64 one (default GRAD_RTOL)."""
     want = ref["grads"]["float64"]
     n_or = int((np.any([r > 0 for r in ref["oracle_radii"]], axis=0) != ref["vis"]).sum())
     print("%s: %d Gaussians stepped, %d differ in visibility between the GPU and the f64 oracle" % (what, rows.size, n_or))
@@ -162,7 +163,7 @@ def _compare(got, ref, rows, what, groups=GROUPS):
     for g in groups:
         r = np.setdiff1d(rows, EDGE) if g == "rots" else rows
         if want[g][r].size:
-            grad_close(got[g][r], want[g][r], "%s: d %s" % (what, g))
+            grad_close(got[g][r], want[g][r], "%s: d %s" % (what, g), **({} if rtol is None else dict(rtol=rtol[g])))
 
 
 def _recovery_bound(after):

@@ -101,9 +101,11 @@ def _batch_reference(raw, cams, gts, Es, batch, oracles):
     return out
 
 
-def _step_against_oracle(m, batch, n_train, gts, oracles, what):
+def _step_against_oracle(m, batch, n_train, gts, oracles, what, groups=GROUPS, rtol=None):
     """One optimiser step over `batch` (S slots, exposure and pose refinement on), checked against the f64 oracle at the
-    cameras and exposures the keyframes had before it"""
+    cameras and exposures the keyframes had before it.  groups: the Gaussians' parameter groups compared with _compare (a
+    map of isotropic, unrotated rows only has a rotation gradient of rounding noise, which the caller bounds itself);
+    rtol: _compare's per-group tolerances"""
     before, it0 = _state(m), m.stats().iterations
     pre = [_kf_state(m, k) for k in range(n_train)]
     kfs = list(dict.fromkeys(batch))
@@ -118,7 +120,7 @@ def _step_against_oracle(m, batch, n_train, gts, oracles, what):
     assert abs(st.last_loss - want_loss) <= 1e-5 * want_loss, (what, st.last_loss, want_loss)
     got = _recovered(before, after)
     rows = np.flatnonzero(ref["vis"])
-    _compare(got, ref, rows, what)
+    _compare(got, ref, rows, what, groups, rtol)
     _check_step(before, after, got, rows, _lr6(), what)
     _check_untouched(before, after, ~ref["vis"], what)
     got_pose = {}

@@ -25,9 +25,9 @@ LR_T, LR_R = 1e-3, 1e-3
 B1 = np.float32(0.9)
 
 
-def _pose_reference(raw, cams, gts, batch, oracles, Es=None):
+def _pose_reference(raw, cams, gts, batch, oracles, Es=None, **kw):
     """{keyframe: mean over the batch's slots of dL/d(rho, omega)} per oracle dtype, on the image and (exposed) dL/dpixel the
-    mapper's kernels produce for the raw parameters `raw` at the cameras `cams`"""
+    mapper's kernels produce for the raw parameters `raw` at the cameras `cams`; kw go to pose_gradient (rows, magnitude)"""
     from gaussian_lic_b200 import model, ops
     dev = torch.device("cuda:0")
     mdl = model.PackedModel(raw, dev)
@@ -49,7 +49,7 @@ def _pose_reference(raw, cams, gts, batch, oracles, Es=None):
             g = dict(means=raw["means"], scales=sc, rots=rot, opacity=op, dc=raw["dc"], sh=raw["sh"], degree=raw["degree"])
             f = o.forward(g, cams[v])
             b = o.backward(f, dL)
-            gr = pose_gradient(g, cams[v], f, b)
+            gr = pose_gradient(g, cams[v], f, b, **kw)
             o.free(f)
             acc = out[o.dtype.name]
             acc[v] = acc.get(v, 0.0) + gr / len(batch)
