@@ -161,6 +161,7 @@ def _load():
         "glic_debug_binning": (i32, [i32, vp, i64, i64, vp, vp, vp, vp]),
         "glic_debug_image": (i32, [i32, i32, vp, vp, vp, vp, vp, C.POINTER(i64), vp]),
         "glic_debug_spans": (i32, [i32, vp, C.POINTER(u32), vp]),
+        "glic_debug_render_backward": (i32, [i32, C.POINTER(View), i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)

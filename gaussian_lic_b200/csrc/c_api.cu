@@ -395,6 +395,26 @@ int glic_debug_sort_pairs_u32(int64_t n, int end_bit, uint32_t* keys, uint32_t* 
     return launch_sort_pairs32(n, end_bit, k, v, temp, temp_bytes, (cudaStream_t)stream, n_dev, false);
 }
 
+int glic_debug_render_backward(int P, const glic_view* view, int64_t R, const void* geom_ws, const void* binning_ws,
+                               const void* image_ws, const void* sample_ws, const float* dL_dpix, float* dL_dmeans2D,
+                               float* dL_dconic, float* dL_dopacity, float* dL_dcolors, int exact, unsigned long long* counters,
+                               void* stream) {
+    if (int e = check_view(view)) return e;
+    if (P < 0 || R < 0) { set_error("debug_render_backward: bad sizes"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (P == 0 || R == 0) return GLIC_OK;
+    if (!dL_dpix || !dL_dmeans2D || !dL_dconic || !dL_dopacity || !dL_dcolors) { set_error("debug_render_backward: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!geom_ws || !image_ws || !binning_ws || !sample_ws) { set_error("debug_render_backward: missing saved workspace"); return GLIC_ERR_WORKSPACE; }
+    const ViewParams vp = make_view_params(view);
+    GeomState g = GeomState::carve(const_cast<void*>(geom_ws), P);
+    ImageState img = ImageState::carve(const_cast<void*>(image_ws), vp.W, vp.H);
+    BinningState bin = BinningState::carve(const_cast<void*>(binning_ws), R);
+    const int64_t max_buckets = glic_max_buckets(R, vp.W, vp.H);
+    SampleState smp = SampleState::carve(const_cast<void*>(sample_ws), max_buckets);
+    const int cur = tile_sort_passes(vp.grid_x * vp.grid_y) & 1;
+    return launch_render_backward(P, vp, max_buckets, bin.vals[cur], g, img, smp, dL_dpix, dL_dmeans2D, dL_dconic, dL_dopacity,
+                                  dL_dcolors, (cudaStream_t)stream, exact != 0, counters);
+}
+
 int glic_debug_geom(int P, const void* geom_ws, float* depth, float* xy, float* conic_opacity, float* rgb,
                     uint32_t* tiles_touched, uint32_t* offsets, uint8_t* clamped, void* stream) {
     if (P <= 0) return GLIC_OK;

@@ -318,7 +318,9 @@ int launch_render_forward(const ViewParams& vp, bool no_color, const uint32_t* p
                           SampleState smp, float* out_color, float* out_final_T, cudaStream_t s);
 int launch_render_backward(int P, const ViewParams& vp, int64_t max_buckets, const uint32_t* point_list, GeomState g,
                            ImageState img, SampleState smp, const float* dL_dpix, float* dL_dmean2D /*[P,3]*/,
-                           float* dL_dconic /*[P,4]*/, float* dL_dopacity, float* dL_dcolors, cudaStream_t s);
+                           float* dL_dconic /*[P,4]*/, float* dL_dopacity, float* dL_dcolors, cudaStream_t s,
+                           bool exact = false /* expf for every pixel, no visit skip (tests) */,
+                           unsigned long long* counters = nullptr /* [8], device: the counting form (render.cu BwdCount) */);
 int launch_preprocess_backward(int P, int D, int M, const float* means, const float* scales, float mod,
                                const float* rots, const float* sh, const ViewParams& vp, const int* radii, GeomState g,
                                float lambda_erank, const float* dL_dmean2D, const float* dL_dconic,

@@ -316,7 +316,16 @@ constexpr int BWD_WARPS = 4;              // warps per CTA; every warp owns one 
 // the warp by one reduce-scatter (8 values in 3 halving exchanges + 2 butterflies; the 9th by butterfly) and leave as
 // 9 RED per splat and bucket -- the same global-atomic count as the reference's per-splat formulation, without its
 // 287-step shuffle pipeline (4 shuffles + bookkeeping per pixel-splat pair).
-template <int BWD_ROWPAIRS, int MIN_CTAS>
+//
+// FAST (the production form) takes G = 2^(power * log2 e) from one MUFU.EX2 instead of the bit-exact expf (8 instructions),
+// and falls back to expf for a pixel whose fast alpha lies within a guard band of 1/255, so every take/skip decision stays
+// the forward's.  It also carries one colour suffix per pixel (sum_c a_c dL/dpix_c) instead of three, which halves the
+// dL/dalpha arithmetic and frees the 16 registers that let 6 CTAs (24 warps) per SM fit in 80 registers without spilling
+// (the former body needs 96 and runs at 5).  !FAST is the former body (expf for every pixel, three suffixes); tests compare the two.  COUNT adds work counters
+// (BwdCount) and is used by tests and scripts/render_bwd_bench.py only.  No visit is skipped for want of a taking pixel:
+// at cfg2, 98 % of the (splat, two row pairs) visits have one, and a per-visit ballot cost more than it saved.
+enum BwdCount { BC_LIVE, BC_SPLATS, BC_SPLATS_TAKEN, BC_VISITS, BC_VISITS_TAKEN, BC_CAND, BC_TAKEN, BC_FALLBACK, BC_N };
+template <int BWD_ROWPAIRS, int MIN_CTAS, bool FAST, bool COUNT>
 __global__ void __launch_bounds__(BWD_WARPS * 32, MIN_CTAS)
 render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr, const uint2* __restrict__ ranges,
                        const uint32_t* __restrict__ point_list, const float4* __restrict__ rec,
@@ -324,7 +333,7 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
                        const float4* __restrict__ ckpt, const uint32_t* __restrict__ n_contrib,
                        const float* __restrict__ pixel_colors, const float* __restrict__ dL_dpix,
                        float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic, float* __restrict__ dL_dopacity,
-                       float* __restrict__ dL_dcolors) {
+                       float* __restrict__ dL_dcolors, unsigned long long* __restrict__ counters) {
     __shared__ float4 s_sp[BWD_WARPS][BUCKET][3];            // the bucket's splat records, per warp
     __shared__ uint32_t s_gid[BWD_WARPS][BUCKET];
     __shared__ uint32_t s_rows[BWD_WARPS][BUCKET];           // row pairs each splat can reach (8-bit mask)
@@ -347,6 +356,7 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
     else if (slot < 5) { dst_base = dL_dconic; dst_stride = 4; dst_off = slot == 4 ? 3 : slot - 2; f_op = -0.5f; f_one = 0.f; }
     else { dst_base = dL_dcolors; dst_stride = 3; dst_off = slot - 5; f_op = 0.f; f_one = 1.f; }
     const bool i_write = (lane & 3) == 0 || lane == 1;
+    unsigned ctr[BC_N] = {};                                     // COUNT only: this lane's share of the counters
 
     constexpr int PARTS = (TILE / 2) / BWD_ROWPAIRS;
     // work items are handed out dynamically (one ticket per warp and item): buckets differ by more than 10x in cost
@@ -383,7 +393,8 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
         // inside this bucket (0 = never got here) and the restart state, kept as fp32 pairs (f32x2.cuh)
         constexpr int NP = BWD_ROWPAIRS / 2;
         int rel[BWD_ROWPAIRS];
-        f2 Tr[NP], a0[NP], a1[NP], a2[NP];
+        // FAST keeps one suffix per pixel, Ag = sum_c a_c dL/dpix_c, instead of the three a_c: dL/dalpha only needs that sum
+        f2 Tr[NP], a0[NP], a1[NP], a2[NP], Ag[NP];
         const float qy0f = (float)qy0;
         int rel_max[BWD_ROWPAIRS];                            // warp-uniform: deepest pixel of each row pair
         int n_max = 0;
@@ -411,6 +422,7 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
             }
             Tr[p] = f2_pack(st[0][0], st[1][0]);
             a0[p] = f2_pack(st[0][1], st[1][1]); a1[p] = f2_pack(st[0][2], st[1][2]); a2[p] = f2_pack(st[0][3], st[1][3]);
+            Ag[p] = f2_fma(a2[p], f2_pack(st[0][6], st[1][6]), f2_fma(a1[p], f2_pack(st[0][5], st[1][5]), f2_mul(a0[p], f2_pack(st[0][4], st[1][4]))));
             s_g[warp][p][0][lane] = make_float2(st[0][4], st[1][4]);
             s_g[warp][p][1][lane] = make_float2(st[0][5], st[1][5]);
             s_g[warp][p][2][lane] = make_float2(st[0][6], st[1][6]);
@@ -438,6 +450,7 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
         }
 
         uint32_t todo = __ballot_sync(0xffffffffu, s_rows[warp][lane] != 0);
+        if (COUNT && lane == 0) ctr[BC_SPLATS] += __popc(todo);
         while (todo) {
             const int k = __ffs(todo) - 1;
             todo &= todo - 1;
@@ -462,12 +475,53 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
                 const f2 power = f2_sub(f2_mul(f2_fma(dx, cxdx, f2_mul(dy, f2_mul(dy, b.x))), -0.5f), f2_mul(dy, cydx));
                 float p0, p1;
                 f2_unpack(power, p0, p1);
-                const float G0 = expf(fminf(p0, 0.0f)), G1 = expf(fminf(p1, 0.0f));
-                float x0, x1;
-                f2_unpack(f2_mul(f2_pack(G0, G1), b.y), x0, x1);
-                x0 = fminf(0.99f, x0); x1 = fminf(0.99f, x1);
-                const bool take0 = ((two & 1u) != 0) & (k < rel[2 * p]) & (p0 <= 0.0f) & (x0 >= (1.0f / 255.0f));
-                const bool take1 = ((two & 2u) != 0) & (k < rel[2 * p + 1]) & (p1 <= 0.0f) & (x1 >= (1.0f / 255.0f));
+                const bool cand0 = ((two & 1u) != 0) & (k < rel[2 * p]) & (p0 <= 0.0f);
+                const bool cand1 = ((two & 2u) != 0) & (k < rel[2 * p + 1]) & (p1 <= 0.0f);
+                float G0, G1, x0, x1;
+                bool take0, take1;
+                if (FAST) {
+                    // G = 2^(power log2 e) by MUFU.EX2.  The decision x = o G >= 1/255 must be the forward's, which computes
+                    // x from the libdevice expf.  Only a pixel with x near 1/255 can be decided differently, and there
+                    // G ~ 1/(255 o), so |power| ~ ln(255 o) <= ln 255 (o <= 1 is a sigmoid) and |y| = |power log2 e| <= 8.
+                    // Relative distance between the fast x and the forward's x:
+                    //   y = fl(power * fl(log2 e)): |dy| <= 8 * (2^-24 + 2^-24.5)   -> 2^y off by <= ln 2 * 2^-20.4 = 2^-20.9
+                    //   ex2.approx.ftz.f32 <= 2 ulp = 2^-22, libdevice expf <= 2 ulp = 2^-22, the two products with o 2^-24 each
+                    // in all < 2^-19.7.  A pixel whose fast x lies within 2^-16 (relative) of 1/255 is decided from the
+                    // exact expf instead, so every decision is the forward's with a margin of 8x.  (o > 1 only widens
+                    // |y| to log2(255 o): the band still covers that up to o ~ 2^56.)  Subnormal G flushes to 0, far
+                    // below the band.  The fast G feeds the gradient terms: 2^-19.7 relative, far inside fp32 atomics noise.
+                    float e0, e1;
+                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(fmul(fminf(p0, 0.0f), 1.44269504088896341f)));
+                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(fmul(fminf(p1, 0.0f), 1.44269504088896341f)));
+                    G0 = e0; G1 = e1;
+                    f2_unpack(f2_mul(f2_pack(G0, G1), b.y), x0, x1);
+                    constexpr float thr = 1.0f / 255.0f, band = (1.0f / 255.0f) * (1.0f / 65536.0f);
+                    const bool near0 = cand0 & (fabsf(x0 - thr) <= band), near1 = cand1 & (fabsf(x1 - thr) <= band);
+                    if (near0 | near1) {                                  // rare: the forward's expf for these pixels
+                        if (near0) { G0 = expf(p0); x0 = fmul(G0, b.y); }
+                        if (near1) { G1 = expf(p1); x1 = fmul(G1, b.y); }
+                    }
+                    if (COUNT) ctr[BC_FALLBACK] += (unsigned)near0 + (unsigned)near1;
+                    x0 = fminf(0.99f, x0); x1 = fminf(0.99f, x1);
+                    take0 = cand0 & (x0 >= thr);
+                    take1 = cand1 & (x1 >= thr);
+                    if (COUNT) {
+                        const bool any = __any_sync(0xffffffffu, take0 | take1);
+                        if (lane == 0) { ++ctr[BC_VISITS]; ctr[BC_VISITS_TAKEN] += any; }
+                        ctr[BC_CAND] += (unsigned)cand0 + (unsigned)cand1; ctr[BC_TAKEN] += (unsigned)take0 + (unsigned)take1;
+                    }
+                } else {
+                    G0 = expf(fminf(p0, 0.0f)); G1 = expf(fminf(p1, 0.0f));
+                    f2_unpack(f2_mul(f2_pack(G0, G1), b.y), x0, x1);
+                    x0 = fminf(0.99f, x0); x1 = fminf(0.99f, x1);
+                    take0 = cand0 & (x0 >= (1.0f / 255.0f));
+                    take1 = cand1 & (x1 >= (1.0f / 255.0f));
+                    if (COUNT) {
+                        const bool any = __any_sync(0xffffffffu, take0 | take1);
+                        if (lane == 0) { ++ctr[BC_VISITS]; ctr[BC_VISITS_TAKEN] += any; }
+                        ctr[BC_CAND] += (unsigned)cand0 + (unsigned)cand1; ctr[BC_TAKEN] += (unsigned)take0 + (unsigned)take1;
+                    }
+                }
                 const f2 G = f2_pack(take0 ? G0 : 0.0f, take1 ? G1 : 0.0f);
                 const f2 alpha = f2_pack(take0 ? x0 : 0.0f, take1 ? x1 : 0.0f);
                 const f2 one_m = f2_sub(f2_bcast(1.0f), alpha);
@@ -480,12 +534,22 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
                 const f2 ainv = f2_pack(i0, i1);
                 const float2 gr = s_g[warp][p][0][lane], gg = s_g[warp][p][1][lane], gb = s_g[warp][p][2][lane];
                 const f2 g0 = f2_pack(gr.x, gr.y), g1 = f2_pack(gg.x, gg.y), g2 = f2_pack(gb.x, gb.y);
-                a0[p] = f2_fma(dch, f2_bcast(b.z), a0[p]); c0s = f2_fma(dch, g0, c0s);
-                f2 dLa = f2_mul(f2_fma(ainv, a0[p], f2_mul(T, b.z)), g0);
-                a1[p] = f2_fma(dch, f2_bcast(b.w), a1[p]); c1s = f2_fma(dch, g1, c1s);
-                dLa = f2_fma(f2_fma(ainv, a1[p], f2_mul(T, b.w)), g1, dLa);
-                a2[p] = f2_fma(dch, f2_bcast(c2), a2[p]); c2s = f2_fma(dch, g2, c2s);
-                dLa = f2_fma(f2_fma(ainv, a2[p], f2_mul(T, c2)), g2, dLa);
+                c0s = f2_fma(dch, g0, c0s); c1s = f2_fma(dch, g1, c1s); c2s = f2_fma(dch, g2, c2s);
+                f2 dLa;
+                if (FAST) {
+                    // dL/dalpha = sum_c (a_c' / (1 - alpha) + T c_c) g_c with a_c' = a_c + dch c_c, so with cg = sum_c c_c g_c:
+                    // Ag' = Ag + dch cg and dL/dalpha = Ag' / (1 - alpha) + T cg (6 operations per pixel instead of 12)
+                    const f2 cg = f2_fma(g2, c2, f2_fma(g1, b.w, f2_mul(g0, b.z)));
+                    Ag[p] = f2_fma(dch, cg, Ag[p]);
+                    dLa = f2_fma(ainv, Ag[p], f2_mul(T, cg));
+                } else {
+                    a0[p] = f2_fma(dch, f2_bcast(b.z), a0[p]);
+                    dLa = f2_mul(f2_fma(ainv, a0[p], f2_mul(T, b.z)), g0);
+                    a1[p] = f2_fma(dch, f2_bcast(b.w), a1[p]);
+                    dLa = f2_fma(f2_fma(ainv, a1[p], f2_mul(T, b.w)), g1, dLa);
+                    a2[p] = f2_fma(dch, f2_bcast(c2), a2[p]);
+                    dLa = f2_fma(f2_fma(ainv, a2[p], f2_mul(T, c2)), g2, dLa);
+                }
                 Tr[p] = f2_mul(T, one_m);
                 // constant factors (opacity, 0.5*W, 0.5*H, -0.5) are applied once per splat below
                 const f2 w = f2_mul(G, dLa);                              // = dL_dG / opacity
@@ -498,6 +562,7 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
             float v_c0 = f2_lo(c0s) + f2_hi(c0s), v_c1 = f2_lo(c1s) + f2_hi(c1s), v_c2 = f2_lo(c2s) + f2_hi(c2s);
             // every sum of the lane is an exact 0 when no pixel contributed (w = 0 and dch = 0 term by term): skipping is exact
             if (!__any_sync(0xffffffffu, v_o != 0.f || v_c0 != 0.f || v_c1 != 0.f || v_c2 != 0.f)) continue;
+            if (COUNT && lane == 0) ++ctr[BC_SPLATS_TAKEN];
             const float s1 = f2_lo(S1) + f2_hi(S1), s2 = f2_lo(S2) + f2_hi(S2);
             const float sx = dx * v_o;                                   // sum w dx
             const float v_mx = sx * a.z + s1 * a.w;                      // -> * (-opacity * 0.5 * W)
@@ -526,6 +591,14 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
                 const float val = lane == 1 ? v_o : w0;
                 atomicAdd(dst_base + dst_stride * gid + dst_off, val * (f_op * b.y + f_one));
             }
+        }
+    }
+    if (COUNT) {
+        if (blockIdx.x == 0 && threadIdx.x == 0) counters[BC_LIVE] = n_live;
+#pragma unroll
+        for (int c = BC_SPLATS; c < BC_N; ++c) {
+            const unsigned s = __reduce_add_sync(0xffffffffu, ctr[c]);
+            if (lane == 0 && s) atomicAdd(counters + c, (unsigned long long)s);
         }
     }
 }
@@ -557,34 +630,39 @@ int launch_render_forward(const ViewParams& vp, bool no_color, const uint32_t* p
 
 int launch_render_backward(int P, const ViewParams& vp, int64_t max_buckets, const uint32_t* point_list, GeomState g,
                            ImageState img, SampleState smp, const float* dL_dpix, float* dL_dmean2D, float* dL_dconic,
-                           float* dL_dopacity, float* dL_dcolors, cudaStream_t s) {
+                           float* dL_dopacity, float* dL_dcolors, cudaStream_t s, bool exact, unsigned long long* counters) {
     (void)P; (void)smp.bucket_to_tile;
     if (max_buckets <= 0) return GLIC_OK;
     const int T = vp.grid_x * vp.grid_y;
     live_scan_kernel<<<1, 1024, 0, s>>>(T, img.max_contrib, img.live_offsets, img.hdr);
     GLIC_LAUNCH_CHECK();
-    // RP = row pairs per lane (8: one warp per bucket's whole tile, 4: two warps share it).  The occupancy-derived grid size
-    // is a property of the DEVICE: cached per device, not per process.
+    // RP = row pairs per lane (8: one warp per bucket's whole tile, 4: two warps share it; the exact and counting forms exist
+    // for RP = 8 only).  The occupancy-derived grid size is a property of the DEVICE and the kernel: cached per device.
     static const int rp = getenv("GLIC_BWD_RP") ? atoi(getenv("GLIC_BWD_RP")) : 8;
     using Kern = void (*)(ViewParams, int, ImageHeader*, const uint2*, const uint32_t*, const float4*, const uint32_t*,
-                          const uint32_t*, const float4*, const uint32_t*, const float*, const float*, float*, float*, float*, float*);
-    const Kern kern = rp == 8 ? render_backward_kernel<8, 5> : render_backward_kernel<4, 6>;
-    static int blocks_per_device[64] = {};
+                          const uint32_t*, const float4*, const uint32_t*, const float*, const float*, float*, float*, float*, float*,
+                          unsigned long long*);
+    const int form = exact || counters ? 2 * (int)exact + (counters != nullptr) : rp == 8 ? 0 : 4;
+    const Kern kerns[5] = {render_backward_kernel<8, 6, true, false>, render_backward_kernel<8, 6, true, true>,
+                           render_backward_kernel<8, 5, false, false>, render_backward_kernel<8, 5, false, true>,
+                           render_backward_kernel<4, 6, true, false>};
+    const Kern kern = kerns[form];
+    static int blocks_per_device[5][64] = {};
     int dev = 0;
     GLIC_CUDA_TRY(cudaGetDevice(&dev));
     if (dev < 0 || dev >= 64) { set_error("render_backward: device index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!blocks_per_device[dev]) {
+    if (!blocks_per_device[form][dev]) {
         int sms = NUM_SMS, per_sm = 4;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, BWD_WARPS * 32, 0);
-        blocks_per_device[dev] = sms * (per_sm > 0 ? per_sm : 1);
+        blocks_per_device[form][dev] = sms * (per_sm > 0 ? per_sm : 1);
     }
-    const int blocks = blocks_per_device[dev];
-    const int parts = rp == 8 ? 1 : 2;
+    const int blocks = blocks_per_device[form][dev];
+    const int parts = form == 4 ? 2 : 1;
     const int64_t need = (max_buckets * parts + BWD_WARPS - 1) / BWD_WARPS;
     kern<<<(unsigned)std::min<int64_t>(blocks, need), BWD_WARPS * 32, 0, s>>>(
         vp, T, img.hdr, img.ranges, point_list, g.rec, img.bucket_offsets, img.live_offsets, smp.ckpt, img.n_contrib,
-        img.pixel_colors, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors);
+        img.pixel_colors, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors, counters);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }

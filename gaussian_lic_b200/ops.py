@@ -396,6 +396,19 @@ class CRasterizer:
                                               self.loss_scratch.numel(), self.stream), "l1_ssim_loss")
         return loss_out, dL_dimg
 
+    BWD_COUNTERS = ("live_buckets", "splats", "splats_taken", "visits", "visits_taken", "candidate_pixels", "taken_pixels",
+                    "fallback_pixels")
+
+    def render_backward(self, view, dL_dpix, grads, exact=False, counters=None):
+        """The render backward alone on the saved state of the last forward (glic_debug_render_backward), accumulating into
+        grads' four 2-D gradient tensors (zero them first).  exact=True: the former kernel body.  counters: a zeroed [8]
+        int64 device tensor selects the counting form, which adds BWD_COUNTERS to it."""
+        capi.check(self.lib.glic_debug_render_backward(
+            self.P, C.byref(view), self.cap, capi.ptr(self.geom_ws), capi.ptr(self.binning_ws), capi.ptr(self.image_ws),
+            capi.ptr(self.sample_ws), capi.ptr(dL_dpix), capi.ptr(grads["dL_dmeans2D"]), capi.ptr(grads["dL_dconic"]),
+            capi.ptr(grads["dL_dopacity"]), capi.ptr(grads["dL_dcolors"]), int(exact), capi.ptr(counters), self.stream),
+            "debug_render_backward")
+
     # ---- introspection for parity tests -------------------------------------------------------------------
     def debug_state(self):
         lib, P, R, W, H = self.lib, self.P, self.R, self.W, self.H

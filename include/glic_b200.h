@@ -316,6 +316,15 @@ GLIC_API int glic_debug_image(int width, int height, const void* image_ws, uint3
  * synchronises `stream`).  Rects of more than 32 tiles store one span per row while the arena has room; when requested >
  * capacity, the later rects had their rows recomputed by the key emission instead. */
 GLIC_API int glic_debug_spans(int P, const void* geom_ws, uint32_t* count_cap_host, void* stream);
+/* The render backward alone on the saved state of the last glic_forward (R = its binning capacity), ACCUMULATING into the
+ * four 2-D gradient buffers (the caller zeroes them).  exact != 0: the former kernel body (expf for every pixel) instead
+ * of the production one.  counters (optional, DEVICE, 8 x uint64, zeroed by the caller): the
+ * counting form of the same kernel adds {live buckets, splats walked, splats with a taker, (splat, two row pairs) visits,
+ * visits with a taker, candidate pixels, pixel-splat pairs taken, pixels decided by the exact expf fallback}. */
+GLIC_API int glic_debug_render_backward(int P, const glic_view* view, int64_t R, const void* geom_ws, const void* binning_ws,
+                                        const void* image_ws, const void* sample_ws, const float* dL_dpix, float* dL_dmeans2D,
+                                        float* dL_dconic, float* dL_dopacity, float* dL_dcolors, int exact,
+                                        unsigned long long* counters, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Multi-GPU exchange step (no counterpart in the reference, which is single-GPU): in-place MEAN all-reduce of the
