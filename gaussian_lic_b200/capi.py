@@ -141,6 +141,7 @@ def _load():
         "glic_mapper_save_map": (i32, [vp, C.c_char_p]),
         "glic_mapper_stats_get": (i32, [vp, C.POINTER(MapperStats)]),
         "glic_mapper_download": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+        "glic_mapper_prune": (i32, [vp, f32, i32, C.POINTER(u32)]),
         "glic_mapper_export": (i32, [vp, C.c_char_p]),
         "glic_mapper_connect": (i32, [vp, C.c_char_p]),
         "glic_mapper_synchronize": (i32, [vp]),

@@ -24,6 +24,10 @@ constexpr int BUCKET = GLIC_BUCKET;     // 32 splats per checkpoint bucket
 constexpr int PRE_THREADS = 256;        // Gaussians per preprocess CTA
 constexpr int NUM_SMS = 132;            // H100 SXM: sizes the grid-stride launches (a grid cap, never a correctness bound)
 
+// torch::sigmoid of an opacity logit (GaussianModel::getOpacity, gaussian.cpp:147-150) as the activation kernel evaluates it;
+// glic_mapper_prune decides with the same expression, so its 1/255 cut is the preprocess's o < 1/255 test bit for bit
+__device__ __forceinline__ float opacity_activation(float logit) { return 1.0f / (1.0f + expf(-logit)); }
+
 // ---- error plumbing --------------------------------------------------------------------
 void set_error(const std::string& s);
 extern unsigned long long g_launches;
@@ -357,4 +361,11 @@ int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, cons
                    size_t scratch_bytes, void* stream);
 // the clamped (and exposed) images eval_psnr_ssim scored, left in its scratch: which = 0 the image, 1 the ground truth
 const float* eval_clamped(const void* scratch, int CH, int H, int W, int which);
+// stable compaction of the arenas (prune.cu).  select: which of rows [0, P) keep opacity_activation(logit) >= min_opacity;
+// result_host[2] = {kept rows, kept rows among [0, n_sky)}, synchronises s.  gather: output rows [0, P_old) of every group of
+// dst = the kept rows of src in order, then zeros; src and dst are arenas of capacity Pcap.  Both take the select's scratch.
+size_t prune_scratch_bytes(uint32_t P);
+int launch_prune_select(uint32_t P, uint32_t n_sky, const float* opacity_logit, float min_opacity, void* scratch, uint32_t* result_host,
+                        cudaStream_t s);
+int launch_prune_gather(const float* src, float* dst, uint32_t Pcap, int M, uint32_t P_old, uint32_t P_new, const void* scratch, cudaStream_t s);
 }  // namespace glic

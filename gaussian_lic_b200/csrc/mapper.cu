@@ -325,7 +325,8 @@ int dev_alloc(void** p, size_t bytes, bool zero = true) {
     return GLIC_OK;
 }
 
-// grows the staging buffer of the host inputs of extend() and initialize_lidar() to at least `need` bytes (contents lost)
+// grows the staging buffer of the host inputs of extend() and initialize_lidar() (also prune()'s selection scratch) to at least
+// `need` bytes (contents lost)
 int reserve_staging(glic_mapper* m, size_t need) {
     if (need <= m->extend_bytes) return GLIC_OK;
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
@@ -1275,6 +1276,59 @@ int glic_mapper_download(glic_mapper* m, float* xyz, float* f_dc, float* f_rest,
         }
     }
     return GLIC_OK;
+}
+
+// Stable compaction (prune.cu): select the kept rows, then gather each arena into a spare one of the same capacity and swap.
+// The spare is allocated once, before anything changes, and rotates: params -> spare, the old params buffer then takes m1, the
+// old m1 buffer m2, and the old m2 buffer is freed.  Peak extra memory: one arena (glic_packed_floats(Pcap, M) floats); the
+// selection's scratch (4 B per row) lives in the extend() staging buffer, which keeps it.  The gather writes output rows
+// [0, P_old); rows [P_old, Pcap) of every arena are zero already (allocation, initialize, append and regrow keep them so), so
+// the vacated rows end up zero like them.
+int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, uint32_t* removed) {
+    if (!m) { set_error("mapper_prune: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!std::isfinite(min_opacity) || min_opacity < 0.0f || min_opacity > 1.0f) {
+        set_error("mapper_prune: min_opacity must be finite and in [0, 1]"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    MAP_TRY(poll_ring(m, true));
+    const uint32_t P = m->P;
+    if (P == 0) {
+        if (removed) *removed = 0;
+        return GLIC_OK;
+    }
+    cudaStream_t s = m->stream;
+    MAP_TRY(reserve_staging(m, prune_scratch_bytes(P)));            // the selection's scratch: the idle extend() staging
+    void* scratch = m->extend_ws;
+    float* g[6];
+    arena_ptrs(m, m->params, m->Pcap, g);
+    uint32_t kept[2] = {0, 0};
+    int e = launch_prune_select(P, m->n_sky, g[3], min_opacity, scratch, kept, s);
+    if (e == GLIC_OK && kept[0] == 0) {
+        set_error("mapper_prune: the threshold removes every row (an empty map cannot be trained)");
+        e = GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (e == GLIC_OK && !dry_run && kept[0] < P) {
+        float* spare = nullptr;
+        const size_t bytes = arena_floats(m, m->Pcap) * sizeof(float);
+        e = dev_alloc((void**)&spare, bytes, false);
+        if (e == GLIC_OK) {
+            if (cudaMemsetAsync(spare, 0, bytes, s) != cudaSuccess) { set_error("mapper_prune: cudaMemsetAsync failed"); e = GLIC_ERR_CUDA; }
+            for (float** arena : {&m->params, &m->m1, &m->m2}) {
+                if (e != GLIC_OK) break;
+                e = launch_prune_gather(*arena, spare, m->Pcap, m->M, P, kept[0], scratch, s);
+                if (e == GLIC_OK) std::swap(*arena, spare);
+            }
+            if (e == GLIC_OK && cudaStreamSynchronize(s) != cudaSuccess) { set_error("mapper_prune: synchronisation failed"); e = GLIC_ERR_CUDA; }
+            cudaFree(spare);
+        }
+        if (e == GLIC_OK) {
+            m->P = kept[0];
+            m->n_sky = kept[1];
+            m->st.num_gaussians = kept[0];
+        }
+    }
+    if (e == GLIC_OK && removed) *removed = P - kept[0];
+    return e;
 }
 
 int glic_mapper_save_map(glic_mapper* m, const char* path) {

@@ -26,7 +26,7 @@ activations_forward_kernel(int P, const float* __restrict__ opacity_logit, const
                            float4* __restrict__ rot) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P) return;
-    opacity[i] = 1.0f / (1.0f + expf(-opacity_logit[i]));
+    opacity[i] = opacity_activation(opacity_logit[i]);
 #pragma unroll
     for (int c = 0; c < 3; ++c) scale[3 * (size_t)i + c] = expf(log_scale[3 * (size_t)i + c]);
     const float4 q = rot_raw[i];

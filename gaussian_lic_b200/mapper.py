@@ -12,6 +12,7 @@ from . import capi
 
 FASTLIVO = dict(position_lr=1.6e-4, feature_lr=2.5e-3, opacity_lr=0.05, scaling_lr=0.005, rotation_lr=0.001,
                 lambda_dssim=0.2, scaling_scale=1.0)                  # config/fastlivo.yaml:15-24
+DEAD_OPACITY = float(np.float32(1.0) / np.float32(255.0))             # GLIC_MAPPER_DEAD_OPACITY: the preprocess's o < 1/255 cull
 
 
 def _f32(a):
@@ -253,6 +254,14 @@ class Mapper:
         if moments:
             out["exp_avg"], out["exp_avg_sq"] = m1, m2
         return out
+
+    def prune(self, min_opacity=DEAD_OPACITY, dry_run=False):
+        """Remove every row whose activated opacity is below min_opacity (stable: survivors keep their order, parameters and
+        Adam moments; the surviving sky rows stay in front).  The default removes exactly the rows the preprocess culls in every
+        view.  dry_run only counts.  Returns the number of rows removed (or that would be)."""
+        out = C.c_uint32()
+        capi.check(capi.lib.glic_mapper_prune(self._h, float(min_opacity), int(bool(dry_run)), C.byref(out)), "mapper_prune")
+        return int(out.value)
 
     # ---- multi-GPU wiring: torch.distributed (or anything else) only carries the 64-byte handles --------------------------
     def export_handle(self):

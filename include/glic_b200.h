@@ -492,6 +492,22 @@ GLIC_API int glic_mapper_stats_get(glic_mapper* m, glic_mapper_stats* out);
 /* live rows of the arena copied to host arrays shaped like glic_mapper_initialize's (any pointer may be NULL); synchronises */
 GLIC_API int glic_mapper_download(glic_mapper* m, float* xyz, float* f_dc, float* f_rest, float* opacity_logit,
                                   float* log_scale, float* rot, float* exp_avg_packed, float* exp_avg_sq_packed);
+/* Removes every row whose activated opacity is below min_opacity; *removed (may be NULL) gets the count.
+ *   A row goes iff act(logit) < min_opacity, act the activation kernel's own float expression 1 / (1 + expf(-logit)) (a NaN
+ *   logit stays).  At GLIC_MAPPER_DEAD_OPACITY that is the preprocess's o < 1/255 cull bit for bit: such a row is culled in
+ *   every view, so it is never visible, the masked Adam never steps it and it can never render or train again.
+ *   The compaction is stable: survivors keep their relative order, and their six parameter groups and both Adam moments move
+ *   with them bit for bit.  Sky rows stay in front; glic_mapper_sky_rows becomes the number of surviving sky rows, so save_map
+ *   still writes exactly the non-sky survivors.  P and stats.num_gaussians drop, the capacity is unchanged, and the vacated rows
+ *   [P_new, P_old) of the parameter and moment arenas are zeroed.  Keyframes, exposure and pose state are untouched.
+ *   dry_run != 0 only counts.  A NULL mapper, a non-finite min_opacity or one outside [0, 1], and a prune that would remove
+ *   every row (dry run or not) return GLIC_ERR_INVALID_ARGUMENT and change nothing; a mapper with no rows returns GLIC_OK with
+ *   0 removed.  The call drains the iteration pipeline first (as download / save_map, including the lagged overflow ring) and
+ *   synchronises.  It needs one spare arena of the capacity (glic_packed_floats(capacity, M) floats) while it runs.
+ *   world > 1: every rank must make the same call between the same optimize() calls; replicas are bit-identical, so they remove
+ *   the same rows and stay identical without any exchange. */
+#define GLIC_MAPPER_DEAD_OPACITY (1.0f / 255.0f)
+GLIC_API int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, uint32_t* removed);
 /* multi-GPU wiring: every rank exports the 64-byte IPC handle of its exchange block, the caller all-gathers them
  * (torch.distributed / MPI / a file: plumbing) and hands all `world` handles back. */
 GLIC_API int glic_mapper_export(glic_mapper* m, unsigned char* handle64);
