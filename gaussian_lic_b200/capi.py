@@ -163,6 +163,8 @@ def _load():
         "glic_debug_image": (i32, [i32, i32, vp, vp, vp, vp, vp, C.POINTER(i64), vp]),
         "glic_debug_spans": (i32, [i32, vp, C.POINTER(u32), vp]),
         "glic_debug_render_backward": (i32, [i32, C.POINTER(View), i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, vp]),
+        "glic_debug_fail_allocation": (i32, [i32]),
+        "glic_debug_mapper_allocations": (i64, []),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)

@@ -17,9 +17,12 @@
 #include "adam_math.cuh"
 
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstring>
+#include <functional>
 #include <initializer_list>
+#include <memory>
 #include <nv/target>
 #include <random>
 #include <utility>
@@ -108,12 +111,77 @@ void camera_block(int W, int H, double fx, double fy, double cx, double cy, cons
     o.lim[2] = -0.15f * H / ffy - fcy / ffy; o.lim[3] = 1.15f * H / ffy - fcy / ffy;
 }
 
-struct Keyframe {
+// ---- ownership: every CUDA resource of a mapper is a member of one of the two types below, and only they allocate or release
+// one.  The members release themselves, so destroying a mapper is a drain and a delete, and a failed create needs no cleanup.
+std::atomic<int> fail_countdown{0};          // glic_debug_fail_allocation
+std::atomic<int64_t> live_allocations{0};    // glic_debug_mapper_allocations
+
+// One device (or pinned host) allocation of a known size, move-only, released by its destructor
+class Buf {
+public:
+    Buf() = default;
+    Buf(Buf&& o) noexcept { *this = std::move(o); }
+    Buf& operator=(Buf&& o) noexcept {
+        if (this != &o) { release(); p_ = std::exchange(o.p_, nullptr); bytes_ = std::exchange(o.bytes_, 0); pinned_ = o.pinned_; }
+        return *this;
+    }
+    ~Buf() { release(); }
+    void* raw() const { return p_; }
+    size_t bytes() const { return bytes_; }
+    // on an empty Buf: `bytes` of device memory (of pinned host memory with `pinned`), not initialised
+    int allocate(size_t bytes, bool pinned = false) {
+        int n = fail_countdown.load();
+        while (n > 0 && !fail_countdown.compare_exchange_weak(n, n - 1)) {}
+        const cudaError_t e = n == 1 ? cudaErrorMemoryAllocation
+                            : pinned ? cudaHostAlloc(&p_, bytes, cudaHostAllocDefault) : cudaMalloc(&p_, bytes ? bytes : 256);
+        if (e != cudaSuccess) {
+            p_ = nullptr;
+            cudaGetLastError();                      // not left for the next launch check to report
+            set_error("mapper: allocation of " + std::to_string(bytes) + " bytes failed: " + cudaGetErrorString(e));
+            return GLIC_ERR_CUDA;
+        }
+        bytes_ = bytes; pinned_ = pinned; ++live_allocations;
+        return GLIC_OK;
+    }
+private:
+    void release() {
+        if (!p_) return;
+        if (pinned_) cudaFreeHost(p_); else cudaFree(p_);
+        --live_allocations; p_ = nullptr; bytes_ = 0;
+    }
+    void* p_ = nullptr;
+    size_t bytes_ = 0;
+    bool pinned_ = false;
+};
+// a Buf of T that converts to T*, so the launches take it as they would a raw pointer
+template <typename T>
+struct Dev : Buf {
+    operator T*() const { return static_cast<T*>(raw()); }
+};
+
+// a stream, an event or an IPC mapping, move-only, destroyed by its destructor
+template <typename H, cudaError_t (*Destroy)(H)>
+class Handle {
+public:
+    Handle() = default;
+    explicit Handle(H h) : h_(h) {}
+    Handle(Handle&& o) noexcept : h_(std::exchange(o.h_, nullptr)) {}
+    Handle& operator=(Handle&& o) noexcept { std::swap(h_, o.h_); return *this; }
+    ~Handle() { if (h_) Destroy(h_); }
+    operator H() const { return h_; }
+private:
+    H h_ = nullptr;
+};
+using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
+using Event = Handle<cudaEvent_t, cudaEventDestroy>;
+using IpcMapping = Handle<void*, cudaIpcCloseMemHandle>;
+
+struct Keyframe {                    // move-only: it owns its device camera block
     float R_wc[9], t_wc[3];
-    const float* image;
+    const float* image = nullptr;
     const uint8_t* bgr = nullptr;    // add_frame keyframes: packed HWC BGR8 in the frame store, decoded where `image` is copied
     CamBlock cam;
-    float* cam_dev;                  // view16 | proj16 | campos4
+    Dev<float> cam_dev;              // view16 | proj16 | campos4
     glic_view view;
 };
 
@@ -241,8 +309,14 @@ enum SlotRegion { COLOUR, FLAGS, EXPOSURE, POSE, N_REGIONS };
 // Adam state of a per-training-keyframe parameter of `width` floats: moments [cap][width], step counts [cap]
 struct KeyframeAdam {
     int width;
-    float *m = nullptr, *v = nullptr;
-    int* t = nullptr;
+    Dev<float> m, v;
+    Dev<int> t;
+};
+
+// The exchange block: geo[11*Pcap + 4] | flags words | one region [2][S] of slots per SlotRegion
+struct XLayout {
+    size_t n_geo = 0;                // floats in the reduced region (11*Pcap + 4; the tail holds the collective overflow word)
+    size_t bytes = 0, slot_off[N_REGIONS] = {}, slot_bytes[N_REGIONS] = {};
 };
 
 }  // namespace
@@ -250,30 +324,29 @@ struct KeyframeAdam {
 struct glic_mapper {
     glic_mapper_config cfg{};
     int dev = 0, D = 0, M = 0, S = 1, k = 1;
-    cudaStream_t stream = nullptr, copy_stream = nullptr, push_stream = nullptr;
+    Stream stream, copy_stream, push_stream;
     // ---- arenas (capacity Pcap) ----
     uint32_t P = 0, Pcap = 0;
     uint32_t n_sky = 0;                   // rows [0, n_sky) are the skybox (glic_mapper_initialize_lidar): left out of save_map
-    float *params = nullptr, *m1 = nullptr, *m2 = nullptr;
-    float *act_opacity = nullptr, *act_scales = nullptr, *act_rots = nullptr;
-    int* radii = nullptr;
-    float *g_mean2D = nullptr, *g_conic = nullptr, *g_opacity = nullptr;
-    void* geom_ws = nullptr; size_t geom_bytes = 0;
-    // ---- exchange block: geo[11*Pcap + 4] | flags words | one region [2][S] of slots per SlotRegion (xblock_layout) ----
-    char* xblock = nullptr; size_t xbytes = 0, slot_off[N_REGIONS] = {}, slot_bytes[N_REGIONS] = {};
-    size_t n_geo = 0;                // floats in the reduced region (11*Pcap + 4; the tail holds the collective overflow word)
+    Dev<float> params, m1, m2;
+    Dev<float> act_opacity, act_scales, act_rots;
+    Dev<int> radii;
+    Dev<float> g_conic;                   // the render backward's 2-D gradient accumulators: conic [4 Pcap] | mean2D [3 Pcap] | opacity
+    float *g_mean2D = nullptr, *g_opacity = nullptr;
+    Dev<void> geom_ws;
+    Dev<char> xblock;
+    XLayout x;
     void* peers[8] = {nullptr};
     bool connected = false;
-    std::vector<void*> opened;
+    std::vector<IpcMapping> opened;
     // ---- per-image buffers ----
-    void *image_ws = nullptr, *binning_ws = nullptr, *sample_ws = nullptr, *loss_scratch = nullptr, *eval_scratch = nullptr, *extend_ws = nullptr;
-    size_t image_bytes = 0, binning_bytes = 0, sample_bytes = 0, loss_bytes = 0, eval_bytes = 0, extend_bytes = 0;
+    Dev<void> image_ws, binning_ws, sample_ws, loss_scratch, eval_scratch, extend_ws;
     int64_t bin_cap = 0;
-    float *color = nullptr, *final_T = nullptr, *dL_dpix = nullptr, *gt_dev[2] = {nullptr, nullptr}, *loss_dev = nullptr, *eval_out = nullptr;
-    unsigned int* vis_acc = nullptr;
-    cudaEvent_t gt_free[2]{}, gt_ready[2]{}, ev_flags{}, ev_col{}, ev_push{}, ring_ev[RING]{}, t0{}, t1{};
-    long long* counters_host = nullptr;   // pinned [RING][4]
-    float* loss_host = nullptr;           // pinned [RING]
+    Dev<float> color, final_T, dL_dpix, gt_dev[2], loss_dev, eval_out;
+    Dev<unsigned int> vis_acc;
+    Event gt_free[2], gt_ready[2], ev_flags, ev_col, ev_push, ring_ev[RING], t0, t1;
+    Dev<long long> counters_host;         // pinned [RING][4]
+    Dev<float> loss_host;                 // pinned [RING]
     bool ring_used[RING] = {false};
     // ---- keyframes ----
     std::vector<Keyframe> train, test;
@@ -281,36 +354,36 @@ struct glic_mapper {
     uint64_t view_counter = 0;
     glic_mapper_stats st{};
     bool run_optimizer = true;            // GLIC_MAPPER_OPT_OPTIMIZER (benchmarks time the rasterization step alone with it off)
-    // ---- per-training-keyframe exposure (glic_mapper_enable_exposure): E [expo_cap][12] and its Adam state ----
+    // ---- per-training-keyframe rows of the exposure and the pose refinement, kf_cap of each, allocated for both features
+    //      once either is enabled (enabling one initialises its rows of the existing keyframes) ----
+    size_t kf_cap = 0;
+    // exposure (glic_mapper_enable_exposure): E [kf_cap][12] and its Adam state
     bool expo_on = false;
     float expo_lr = 0.f;
-    float* expo_E = nullptr;
+    Dev<float> expo_E;
     KeyframeAdam expo_adam{12};
-    size_t expo_cap = 0;
-    // ---- per-training-keyframe pose refinement (glic_mapper_enable_pose_refinement): float64 T_cw [pose_cap][12]
-    //      (R_cw row-major | t_cw), the float pose [pose_cap][12] (R_wc | t_wc) and the Adam state of the 6-vector ----
+    // pose refinement (glic_mapper_enable_pose_refinement): float64 T_cw [kf_cap][12] (R_cw row-major | t_cw), the float pose
+    // [kf_cap][12] (R_wc | t_wc) and the Adam state of the 6-vector
     bool pose_on = false;
     float pose_lr_rho = 0.f, pose_lr_omega = 0.f;
-    double* pose_T = nullptr;
-    float* pose_f = nullptr;
+    Dev<double> pose_T;
+    Dev<float> pose_f;
     KeyframeAdam pose_adam{6};
-    size_t pose_cap = 0;
-    double* pose_part = nullptr;          // per-CTA partials of the pose-gradient reduction (pose_partials_count(Pcap))
-    cudaEvent_t ev_pose{};
+    Dev<double> pose_part;                // per-CTA partials of the pose-gradient reduction (pose_partials_count(Pcap))
+    Event ev_pose;
     // ---- LPIPS of the evaluation (glic_mapper_load_lpips): weight payload and glic_lpips's scratch, sized on first use ----
-    float* lpips_w = nullptr;
-    void* lpips_scratch = nullptr;
-    size_t lpips_bytes = 0;
+    Dev<float> lpips_w;
+    Dev<void> lpips_scratch;
     // ---- raw frames (glic_mapper_enable_frames / add_frame): the 8-bit image store, chunks of FRAME_CHUNK frames of
     //      frame_stride bytes that never move, and the scan of the frames since the last training keyframe (device arrays
     //      of scan_cap points, grown by doubling) ----
     bool initialized = false;             // initialize or initialize_lidar has run (the next scan extends the map)
     bool frames_on = false;
     int frame_k = 1, frame_sky_points = 0, frame_sky_radius = 0;
-    std::vector<uint8_t*> frame_chunks;
+    std::vector<Dev<uint8_t>> frame_chunks;
     size_t frame_stride = 0;
-    float *scan_xyz = nullptr, *scan_depth = nullptr;
-    uint8_t* scan_rgb = nullptr;
+    Dev<float> scan_xyz, scan_depth;
+    Dev<uint8_t> scan_rgb;
     size_t scan_cap = 0;
     glic_frame_stats fst{};
 };
@@ -319,24 +392,31 @@ namespace {
 
 #define MAP_TRY(expr) do { int _e = (expr); if (_e != GLIC_OK) return _e; } while (0)
 
-int dev_alloc(void** p, size_t bytes, bool zero = true) {
-    GLIC_CUDA_TRY(cudaMalloc(p, bytes ? bytes : 256));
-    if (zero) GLIC_CUDA_TRY(cudaMemset(*p, 0, bytes ? bytes : 256));
+// One buffer of a growth: its new size, the prefix of its old contents it keeps, and whether it starts zeroed
+struct Grow { Buf& buf; size_t bytes, keep = 0; bool zero = false; };
+
+// The one way a mapper's buffers grow: allocate every new buffer; on the mapper's stream zero those that start zeroed and copy the
+// kept prefixes (then `fill`, which set_capacity uses to regrow the arenas into the new buffers); synchronise; only then swap the
+// new buffers in and release the old.  A failed allocation leaves every buffer as it was.
+int grow(glic_mapper* m, std::initializer_list<Grow> list, const std::function<int(Buf*)>& fill = nullptr) {
+    std::vector<Buf> fresh(list.size());
+    Buf* b = fresh.data();
+    for (const Grow& g : list) MAP_TRY((b++)->allocate(g.bytes));
+    b = fresh.data();
+    for (const Grow& g : list) {
+        if (g.zero) GLIC_CUDA_TRY(cudaMemsetAsync(b->raw(), 0, g.bytes, m->stream));
+        if (g.keep) GLIC_CUDA_TRY(cudaMemcpyAsync(b->raw(), g.buf.raw(), g.keep, cudaMemcpyDeviceToDevice, m->stream));
+        ++b;
+    }
+    if (fill) MAP_TRY(fill(fresh.data()));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    b = fresh.data();
+    for (const Grow& g : list) g.buf = std::move(*b++);
     return GLIC_OK;
 }
 
-// grows the staging buffer of the host inputs of extend() and initialize_lidar() (also prune()'s selection scratch) to at least
-// `need` bytes (contents lost)
-int reserve_staging(glic_mapper* m, size_t need) {
-    if (need <= m->extend_bytes) return GLIC_OK;
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    if (m->extend_ws) cudaFree(m->extend_ws);
-    m->extend_ws = nullptr;
-    m->extend_bytes = 0;
-    MAP_TRY(dev_alloc(&m->extend_ws, need, false));
-    m->extend_bytes = need;
-    return GLIC_OK;
-}
+// grows b to at least `need` bytes without keeping its contents
+int reserve(glic_mapper* m, Buf& b, size_t need) { return need <= b.bytes() ? GLIC_OK : grow(m, {{b, need}}); }
 
 size_t arena_floats(const glic_mapper* m, uint32_t cap) { return glic_packed_floats(cap, (uint32_t)m->M); }
 
@@ -346,28 +426,29 @@ void arena_ptrs(const glic_mapper* m, float* base, uint32_t cap, float* out6[6])
     for (int q = 0; q < 6; ++q) out6[q] = base + off[q];
 }
 
-float* geo_ptr(const glic_mapper* m) { return reinterpret_cast<float*>(m->xblock); }
+float* geo_ptr(const glic_mapper* m) { return static_cast<float*>(m->xblock.raw()); }
 
 // view slot s of parity `parity` in region r of the exchange block
 template <typename T = float>
 T* slot(const glic_mapper* m, SlotRegion r, int parity, int s) {
-    return reinterpret_cast<T*>(m->xblock + m->slot_off[r] + ((size_t)parity * m->S + s) * m->slot_bytes[r]);
+    return reinterpret_cast<T*>(m->xblock + m->x.slot_off[r] + ((size_t)parity * m->S + s) * m->x.slot_bytes[r]);
 }
 
 // The slot regions follow the flags words, each [2][S] slots rounded up to 256 bytes: colour gradients [cap][3] floats, flag
-// bytes [cap], dL/dE [12] floats, dL/d(rho, omega) [8] floats (2 unused).  Returns the block's size.
-size_t xblock_layout(glic_mapper* m, uint32_t cap) {
-    m->n_geo = (size_t)11 * cap + 4;
+// bytes [cap], dL/dE [12] floats, dL/d(rho, omega) [8] floats (2 unused).
+XLayout xblock_layout(int S, uint32_t cap) {
+    XLayout x;
+    x.n_geo = (size_t)11 * cap + 4;
     size_t sl[6];
-    glic_p2p_slice(0, 1, m->n_geo, 0, sl);
+    glic_p2p_slice(0, 1, x.n_geo, 0, sl);
     const size_t bytes[N_REGIONS] = {(size_t)cap * 3 * sizeof(float), cap, 12 * sizeof(float), 8 * sizeof(float)};
-    size_t off = sl[5] + 256;
+    x.bytes = sl[5] + 256;
     for (int r = 0; r < N_REGIONS; ++r) {
-        m->slot_off[r] = off;
-        m->slot_bytes[r] = bytes[r];
-        off += ((size_t)2 * m->S * bytes[r] + 255) & ~size_t(255);
+        x.slot_off[r] = x.bytes;
+        x.slot_bytes[r] = bytes[r];
+        x.bytes += ((size_t)2 * S * bytes[r] + 255) & ~size_t(255);
     }
-    return off;
+    return x;
 }
 
 // copies [local, local + bytes) of this rank's exchange block to the same offset in every peer's, on the push stream
@@ -380,82 +461,43 @@ int push_to_peers(glic_mapper* m, const void* local, size_t bytes) {
     return GLIC_OK;
 }
 
-// (re)allocates everything whose size depends on the Gaussian capacity; copies the live rows of the arenas
+// grows everything whose size depends on the Gaussian capacity, all of it allocated before any old buffer is released; the
+// arenas keep their live rows and every new buffer but pose_part starts zeroed, so rows [P, Pcap) of the arenas stay zero
 int set_capacity(glic_mapper* m, uint32_t cap) {
     cap = round_up(std::max<uint32_t>(cap, 256), 256);
     if (cap <= m->Pcap) return GLIC_OK;
     if (m->connected) { set_error("mapper: the arena capacity is fixed once the exchange blocks are connected (world > 1); create the mapper with a larger capacity"); return GLIC_ERR_WORKSPACE; }
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    const size_t nfl = arena_floats(m, cap);
-    float *np = nullptr, *n1 = nullptr, *n2 = nullptr;
-    MAP_TRY(dev_alloc((void**)&np, nfl * 4)); MAP_TRY(dev_alloc((void**)&n1, nfl * 4)); MAP_TRY(dev_alloc((void**)&n2, nfl * 4));
-    if (m->P) {
-        MAP_TRY(glic_arena_regrow(m->params, m->Pcap, np, cap, (uint32_t)m->M, m->P, m->stream));
-        MAP_TRY(glic_arena_regrow(m->m1, m->Pcap, n1, cap, (uint32_t)m->M, m->P, m->stream));
-        MAP_TRY(glic_arena_regrow(m->m2, m->Pcap, n2, cap, (uint32_t)m->M, m->P, m->stream));
-        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    }
-    void* old[] = {m->params, m->m1, m->m2, m->act_opacity, m->act_scales, m->act_rots, m->radii, m->g_conic, m->geom_ws, m->xblock, m->pose_part};
-    for (void* p : old) if (p) cudaFree(p);
-    MAP_TRY(dev_alloc((void**)&m->pose_part, pose_partials_count(cap) * sizeof(double), false));
-    m->params = np; m->m1 = n1; m->m2 = n2;
-    MAP_TRY(dev_alloc((void**)&m->act_opacity, (size_t)cap * 4)); MAP_TRY(dev_alloc((void**)&m->act_scales, (size_t)cap * 12));
-    MAP_TRY(dev_alloc((void**)&m->act_rots, (size_t)cap * 16)); MAP_TRY(dev_alloc((void**)&m->radii, (size_t)cap * 4));
-    // the three 2-D gradient accumulators the render backward adds into: one block (conic first: float4-aligned)
-    MAP_TRY(dev_alloc((void**)&m->g_conic, (size_t)cap * (16 + 12 + 4)));
-    m->g_mean2D = m->g_conic + (size_t)cap * 4;
+    const size_t arena = arena_floats(m, cap) * sizeof(float);
+    const XLayout x = xblock_layout(m->S, cap);
+    auto regrow = [&](Buf* fresh) -> int {
+        const float* old[3] = {m->params, m->m1, m->m2};
+        for (int a = 0; a < 3 && m->P; ++a)
+            MAP_TRY(glic_arena_regrow(old[a], m->Pcap, static_cast<float*>(fresh[a].raw()), cap, (uint32_t)m->M, m->P, m->stream));
+        return GLIC_OK;
+    };
+    MAP_TRY(grow(m, {{m->params, arena, 0, true}, {m->m1, arena, 0, true}, {m->m2, arena, 0, true},
+                     {m->act_opacity, (size_t)cap * 4, 0, true}, {m->act_scales, (size_t)cap * 12, 0, true},
+                     {m->act_rots, (size_t)cap * 16, 0, true}, {m->radii, (size_t)cap * 4, 0, true},
+                     {m->g_conic, (size_t)cap * (16 + 12 + 4), 0, true}, {m->geom_ws, glic_geom_bytes((int)cap), 0, true},
+                     {m->xblock, x.bytes, 0, true}, {m->pose_part, pose_partials_count(cap) * sizeof(double)}}, regrow));
+    m->g_mean2D = m->g_conic + (size_t)cap * 4;           // conic first: float4-aligned
     m->g_opacity = m->g_mean2D + (size_t)cap * 3;
-    m->geom_bytes = glic_geom_bytes((int)cap);
-    MAP_TRY(dev_alloc(&m->geom_ws, m->geom_bytes));
-    m->xbytes = xblock_layout(m, cap);
-    MAP_TRY(dev_alloc((void**)&m->xblock, m->xbytes));
+    m->x = x;
     m->peers[m->cfg.rank] = m->xblock;
     m->Pcap = cap;
     m->st.capacity = cap;
     return GLIC_OK;
 }
 
-// Grows per-training-keyframe device arrays from old_cap to cap rows, keeping rows [0, old_cap): each entry is the address of
-// an array and its bytes per row.  New rows are zero.
-int grow_keyframe_rows(glic_mapper* m, std::initializer_list<std::pair<void**, size_t>> arrays, size_t old_cap, size_t cap) {
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    std::vector<void*> grown(arrays.size(), nullptr);
-    size_t i = 0;
-    for (const auto& a : arrays) MAP_TRY(dev_alloc(&grown[i++], cap * a.second));
-    if (old_cap) {
-        i = 0;
-        for (const auto& a : arrays)
-            GLIC_CUDA_TRY(cudaMemcpyAsync(grown[i++], *a.first, old_cap * a.second, cudaMemcpyDeviceToDevice, m->stream));
-        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    }
-    i = 0;
-    for (const auto& a : arrays) {
-        if (*a.first) cudaFree(*a.first);
-        *a.first = grown[i++];
-    }
-    return GLIC_OK;
-}
-
-// room for the exposure state of n training keyframes (keeps the existing rows)
-int expo_reserve(glic_mapper* m, size_t n) {
-    if (n <= m->expo_cap) return GLIC_OK;
-    const size_t cap = std::max<size_t>({n, 2 * m->expo_cap, 64});
-    KeyframeAdam& a = m->expo_adam;
-    MAP_TRY(grow_keyframe_rows(m, {{(void**)&m->expo_E, 12 * sizeof(float)}, {(void**)&a.m, 12 * sizeof(float)},
-                                   {(void**)&a.v, 12 * sizeof(float)}, {(void**)&a.t, sizeof(int)}}, m->expo_cap, cap));
-    m->expo_cap = cap;
-    return GLIC_OK;
-}
-
-// room for the pose state of n training keyframes (keeps the existing rows)
-int pose_reserve(glic_mapper* m, size_t n) {
-    if (n <= m->pose_cap) return GLIC_OK;
-    const size_t cap = std::max<size_t>({n, 2 * m->pose_cap, 64});
-    KeyframeAdam& a = m->pose_adam;
-    MAP_TRY(grow_keyframe_rows(m, {{(void**)&m->pose_T, 12 * sizeof(double)}, {(void**)&m->pose_f, 12 * sizeof(float)},
-                                   {(void**)&a.m, 6 * sizeof(float)}, {(void**)&a.v, 6 * sizeof(float)}, {(void**)&a.t, sizeof(int)}},
-                               m->pose_cap, cap));
-    m->pose_cap = cap;
+// room for the exposure and pose rows of n training keyframes: existing rows are kept, new rows are zero
+int reserve_keyframe_rows(glic_mapper* m, size_t n) {
+    if (n <= m->kf_cap) return GLIC_OK;
+    const size_t cap = std::max<size_t>({n, 2 * m->kf_cap, 64}), old = m->kf_cap;
+    auto rows = [&](Buf& b, size_t row_bytes) { return Grow{b, cap * row_bytes, old * row_bytes, true}; };
+    MAP_TRY(grow(m, {rows(m->expo_E, 12 * sizeof(float)), rows(m->expo_adam.m, 12 * sizeof(float)), rows(m->expo_adam.v, 12 * sizeof(float)),
+                     rows(m->expo_adam.t, sizeof(int)), rows(m->pose_T, 12 * sizeof(double)), rows(m->pose_f, 12 * sizeof(float)),
+                     rows(m->pose_adam.m, 6 * sizeof(float)), rows(m->pose_adam.v, 6 * sizeof(float)), rows(m->pose_adam.t, sizeof(int))}));
+    m->kf_cap = cap;
     return GLIC_OK;
 }
 
@@ -516,14 +558,9 @@ int launch_pose_step(glic_mapper* m, const int* views, int parity) {
 
 int set_bin_capacity(glic_mapper* m, int64_t pairs, bool exact = false) {
     if (!exact && pairs <= m->bin_cap) return GLIC_OK;
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    if (m->binning_ws) cudaFree(m->binning_ws);
-    if (m->sample_ws) cudaFree(m->sample_ws);
-    m->binning_bytes = glic_binning_bytes(pairs);
-    m->sample_bytes = glic_sample_bytes(pairs, m->cfg.width, m->cfg.height);
-    MAP_TRY(dev_alloc(&m->binning_ws, m->binning_bytes, false));
-    MAP_TRY(dev_alloc(&m->sample_ws, m->sample_bytes, false));
-    m->bin_cap = glic_binning_capacity(m->binning_bytes, m->sample_bytes, m->cfg.width, m->cfg.height, 0);
+    const size_t binning_bytes = glic_binning_bytes(pairs), sample_bytes = glic_sample_bytes(pairs, m->cfg.width, m->cfg.height);
+    MAP_TRY(grow(m, {{m->binning_ws, binning_bytes}, {m->sample_ws, sample_bytes}}));
+    m->bin_cap = glic_binning_capacity(binning_bytes, sample_bytes, m->cfg.width, m->cfg.height, 0);
     return GLIC_OK;
 }
 
@@ -538,8 +575,8 @@ int poll_ring(glic_mapper* m, bool wait) {
         const long long* c = m->counters_host + 4 * r;
         m->st.last_loss = m->loss_host[r];
         if (c[2]) {                                        // this frame overflowed the binning workspace: it was skipped on the device
-            ++m->st.overflow_regrows;
             MAP_TRY(set_bin_capacity(m, std::max<int64_t>(c[0] + c[0] / 4, m->bin_cap * 3 / 2)));
+            ++m->st.overflow_regrows;
         }
     }
     return GLIC_OK;
@@ -555,8 +592,8 @@ int forward_view(glic_mapper* m, const Keyframe& kf, int no_color, long long* co
     float* g[6];
     arena_ptrs(m, m->params, m->Pcap, g);
     return glic_forward((int)m->P, m->D, m->M, g[1], m->act_scales, 1.0f, m->act_rots, m->act_opacity, g[4], m->M ? g[5] : nullptr, &kf.view,
-                        no_color, m->radii, m->geom_ws, m->geom_bytes, m->image_ws, m->image_bytes, m->binning_ws, m->binning_bytes,
-                        m->sample_ws, m->sample_bytes, m->color, m->final_T, (int64_t*)counters, m->stream);
+                        no_color, m->radii, m->geom_ws, m->geom_ws.bytes(), m->image_ws, m->image_ws.bytes(), m->binning_ws,
+                        m->binning_ws.bytes(), m->sample_ws, m->sample_ws.bytes(), m->color, m->final_T, (int64_t*)counters, m->stream);
 }
 
 // activations and a synchronous forward of kf: a binning overflow grows the workspace and renders again, up to 4 attempts.
@@ -568,8 +605,8 @@ int forward_settled(glic_mapper* m, const Keyframe& kf, int no_color) {
         MAP_TRY(forward_view(m, kf, no_color, cnt));
         GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
         if (!cnt[2]) break;
-        ++m->st.overflow_regrows;
         MAP_TRY(set_bin_capacity(m, cnt[0] + cnt[0] / 4));
+        ++m->st.overflow_regrows;
     }
     return GLIC_OK;
 }
@@ -630,15 +667,15 @@ int iteration(glic_mapper* m, const int* views) {
         // loss of this view (the pinned ring keeps the last local view's value for the statistics)
         if (m->expo_on)
             MAP_TRY(glic_l1_ssim_loss_exposure(H, W, m->cfg.lambda_dssim, m->color, m->gt_dev[buf], m->expo_E + 12 * (size_t)views[sl], m->loss_dev + 1,
-                                               m->dL_dpix, slot(m, EXPOSURE, parity, sl), m->loss_scratch, m->loss_bytes, s));
+                                               m->dL_dpix, slot(m, EXPOSURE, parity, sl), m->loss_scratch, m->loss_scratch.bytes(), s));
         else
-            MAP_TRY(glic_l1_ssim_loss(3, H, W, m->cfg.lambda_dssim, m->color, m->gt_dev[buf], m->loss_dev + 1, m->dL_dpix, m->loss_scratch, m->loss_bytes, s));
+            MAP_TRY(glic_l1_ssim_loss(3, H, W, m->cfg.lambda_dssim, m->color, m->gt_dev[buf], m->loss_dev + 1, m->dL_dpix, m->loss_scratch, m->loss_scratch.bytes(), s));
         GLIC_CUDA_TRY(cudaEventRecord(m->gt_free[buf], s));
         CompactGrads cg;
         cg.g_rot = reinterpret_cast<float4*>(geo + goff[0]); cg.g_xyz = geo + goff[1]; cg.g_scale = geo + goff[2]; cg.g_opacity = geo + goff[3];
         cg.opacity = m->act_opacity; cg.dL_dopacity = m->g_opacity; cg.rot_raw = reinterpret_cast<const float4*>(g[0]);
         cg.accumulate = j > 0;
-        cg.pose_partials = m->pose_on ? m->pose_part : nullptr;        // this view's dL/d(rho, omega), fused into the backward
+        cg.pose_partials = m->pose_on ? (double*)m->pose_part : nullptr;        // this view's dL/d(rho, omega), fused into the backward
         cg.pose_grad = m->pose_on ? slot(m, POSE, parity, sl) : nullptr;
         MAP_TRY(glic_backward_compact_internal((int)m->P, m->D, m->M, g[1], m->act_scales, m->act_rots, m->M ? g[5] : nullptr, &kf.view, m->radii,
                                                m->bin_cap, m->geom_ws, m->binning_ws, m->image_ws, m->sample_ws, m->dL_dpix, m->g_mean2D,
@@ -658,7 +695,7 @@ int iteration(glic_mapper* m, const int* views) {
     if (m->cfg.world > 1) {
         GLIC_CUDA_TRY(cudaEventRecord(m->ev_push, m->push_stream));
         GLIC_CUDA_TRY(cudaStreamWaitEvent(s, m->ev_push, 0));
-        MAP_TRY(glic_p2p_allreduce_mean(m->cfg.rank, m->cfg.world, m->peers, m->n_geo, 0, s));
+        MAP_TRY(glic_p2p_allreduce_mean(m->cfg.rank, m->cfg.world, m->peers, m->x.n_geo, 0, s));
     }
     float lr6[6] = {m->cfg.rotation_lr, m->cfg.position_lr, m->cfg.scaling_lr, m->cfg.opacity_lr, m->cfg.feature_lr, m->cfg.feature_lr / 20.0f};
     // Reference quirk kept for parity (backward.cu:352 `if (shs)`): with no SH-rest tensor bound (degree 0, M = 0) the whole
@@ -722,7 +759,7 @@ int render_scored(glic_mapper* m, int is_train, int index, const char* what) {
     MAP_TRY(forward_settled(m, kf, 0));
     MAP_TRY(load_gt(m, kf, m->gt_dev[0], cudaMemcpyHostToDevice, s));
     const float* E = (is_train && m->expo_on) ? m->expo_E + 12 * (size_t)index : nullptr;
-    return eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], E, m->eval_out, m->eval_scratch, m->eval_bytes, s);
+    return eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], E, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s);
 }
 
 // copies n floats of eval_out to the host and waits for them
@@ -737,6 +774,7 @@ int read_eval_out(glic_mapper* m, float* out, int n) {
 int initialize_lidar_core(glic_mapper* m, int n, const float* d_pts, const double* d_col, const float* d_dep, double focal, int sky_points,
                           int sky_radius, void* sky_ws) {
     const uint32_t S = (uint32_t)sky_points, P = S + (uint32_t)n;
+    MAP_TRY(set_bin_capacity(m, (int64_t)16 * P));  // before the map is replaced: a failure leaves it as it was
     cudaStream_t s = m->stream;
     const size_t nfl = arena_floats(m, m->Pcap);
     GLIC_CUDA_TRY(cudaMemsetAsync(m->params, 0, nfl * 4, s));
@@ -752,7 +790,6 @@ int initialize_lidar_core(glic_mapper* m, int n, const float* d_pts, const doubl
     m->n_sky = S;
     m->st.num_gaussians = P;
     m->initialized = true;
-    if ((int64_t)16 * P > m->bin_cap) MAP_TRY(set_bin_capacity(m, (int64_t)16 * P));
     return GLIC_OK;
 }
 
@@ -771,13 +808,12 @@ size_t extend_core_carve(void* ws, int n, int W, int H, int** keep, float** out5
     return c.total();
 }
 
-// extend() (gaussian.cpp:499-638) on the newest training keyframe from device arrays of n > 0 points.  The caller has
+// extend() (gaussian.cpp:499-638) on training keyframe kf, the newest, from device arrays of n > 0 points.  The caller has
 // drained the ring, sized the arena for P + n rows, recorded m->t0 before staging its inputs and hands ws of
 // extend_core_carve(nullptr, n, W, H, ...) bytes.
-int extend_core(glic_mapper* m, int n, const float* d_pts, const float* d_col, const float* d_dep, void* ws) {
+int extend_core(glic_mapper* m, const Keyframe& kf, int n, const float* d_pts, const float* d_col, const float* d_dep, void* ws) {
     cudaStream_t s = m->stream;
     const int W = m->cfg.width, H = m->cfg.height;
-    const Keyframe& kf = m->train.back();
     int* d_keep = nullptr;
     float* o[5];
     void* d_ws = nullptr;
@@ -817,118 +853,74 @@ int extend_core(glic_mapper* m, int n, const float* d_pts, const float* d_col, c
 int extend_prepare(glic_mapper* m, int n, size_t input_bytes) {
     MAP_TRY(poll_ring(m, true));
     MAP_TRY(set_capacity(m, std::max<uint32_t>(m->P + (uint32_t)n, m->Pcap < m->P + (uint32_t)n ? 2 * m->Pcap : 0)));
-    return reserve_staging(m, input_bytes + extend_core_carve(nullptr, n, m->cfg.width, m->cfg.height, nullptr, nullptr, nullptr));
+    return reserve(m, m->extend_ws, input_bytes + extend_core_carve(nullptr, n, m->cfg.width, m->cfg.height, nullptr, nullptr, nullptr));
 }
 
-// glic_mapper_add_keyframe's body; a keyframe of add_frame has image = nullptr and its 8-bit image in the frame store
-int add_keyframe_core(glic_mapper* m, const float* R_wc, const float* t_wc, const float* image, const uint8_t* bgr, int is_train) {
-    Keyframe kf;
+// a keyframe at pose (R_wc, t_wc) with its device camera block, not yet in a list; a keyframe of add_frame has image = nullptr
+// and its 8-bit image in the frame store
+int make_keyframe(glic_mapper* m, const float* R_wc, const float* t_wc, const float* image, const uint8_t* bgr, Keyframe& kf) {
     std::memcpy(kf.R_wc, R_wc, sizeof(kf.R_wc)); std::memcpy(kf.t_wc, t_wc, sizeof(kf.t_wc));
     kf.image = image;
     kf.bgr = bgr;
     camera_block(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, kf.R_wc, kf.t_wc, kf.cam);
-    MAP_TRY(dev_alloc((void**)&kf.cam_dev, 36 * sizeof(float), false));
-    GLIC_CUDA_TRY(cudaMemcpy(kf.cam_dev, kf.cam.view, 36 * sizeof(float), cudaMemcpyHostToDevice));   // view | proj | campos are contiguous
+    MAP_TRY(kf.cam_dev.allocate(36 * sizeof(float)));
+    // view | proj | campos are contiguous; ordered before every use of the block, all of which are on the mapper's stream or after
+    // a synchronisation of it
+    GLIC_CUDA_TRY(cudaMemcpyAsync(kf.cam_dev, kf.cam.view, 36 * sizeof(float), cudaMemcpyHostToDevice, m->stream));
     kf.view.viewmatrix = kf.cam_dev; kf.view.projmatrix = kf.cam_dev + 16; kf.view.campos = kf.cam_dev + 32;
     kf.view.tan_fovx = kf.cam.tanfovx; kf.view.tan_fovy = kf.cam.tanfovy;
     kf.view.limx_neg = kf.cam.lim[0]; kf.view.limx_pos = kf.cam.lim[1]; kf.view.limy_neg = kf.cam.lim[2]; kf.view.limy_pos = kf.cam.lim[3];
     kf.view.width = m->cfg.width; kf.view.height = m->cfg.height;
-    if (is_train && m->expo_on) {
-        MAP_TRY(expo_reserve(m, m->train.size() + 1));
-        MAP_TRY(expo_reset(m, m->train.size(), m->train.size() + 1));
-    }
-    (is_train ? m->train : m->test).push_back(kf);
-    if (is_train && m->pose_on) {                  // starts at its given pose with zero state
-        MAP_TRY(pose_reserve(m, m->train.size()));
-        MAP_TRY(pose_write(m, m->train.size() - 1, kf.R_wc, kf.t_wc, true));
-    }
     return GLIC_OK;
 }
 
-// copies frame f's image into the next slot of the frame store (a new chunk when the last one is full), dropping the row
-// padding; returns the slot
-int frame_store_push(glic_mapper* m, const glic_frame* f, const uint8_t** slot_out) {
-    const size_t W3 = 3 * (size_t)m->cfg.width, H = (size_t)m->cfg.height, idx = m->fst.frames;
-    if (idx / FRAME_CHUNK >= m->frame_chunks.size()) {
-        void* chunk = nullptr;
-        MAP_TRY(dev_alloc(&chunk, FRAME_CHUNK * m->frame_stride, false));
-        m->frame_chunks.push_back(static_cast<uint8_t*>(chunk));
-        m->fst.image_bytes += FRAME_CHUNK * m->frame_stride;
-    }
-    uint8_t* dst = m->frame_chunks[idx / FRAME_CHUNK] + (idx % FRAME_CHUNK) * m->frame_stride;
-    GLIC_CUDA_TRY(cudaMemcpy2DAsync(dst, W3, f->bgr, f->row_bytes, W3, H, cudaMemcpyHostToDevice, m->stream));
-    *slot_out = dst;
+// appends kf to its list.  A training keyframe's rows (reserve_keyframe_rows, by the caller) start at E = [I | 0] and at its
+// given pose, with zero Adam state, for the features that are enabled.
+int push_keyframe(glic_mapper* m, Keyframe&& kf, int is_train) {
+    (is_train ? m->train : m->test).push_back(std::move(kf));
+    if (!is_train) return GLIC_OK;
+    const size_t k = m->train.size() - 1;
+    if (m->expo_on) MAP_TRY(expo_reset(m, k, k + 1));
+    if (m->pose_on) MAP_TRY(pose_write(m, k, m->train[k].R_wc, m->train[k].t_wc, true));
     return GLIC_OK;
 }
 
-// appends frame f's points to the scan buffer (grown by doubling) with their depths in the frame's camera, R = R_wc in double
-int scan_append(glic_mapper* m, const glic_frame* f, const double R[9]) {
-    const size_t n = (size_t)f->n_points, have = m->fst.pending_points;
-    if (n == 0) return GLIC_OK;
-    cudaStream_t s = m->stream;
-    if (have + n > m->scan_cap) {
-        const size_t cap = std::max<size_t>({have + n, 2 * m->scan_cap, 4096});
-        float *xyz = nullptr, *dep = nullptr;
-        uint8_t* rgb = nullptr;
-        MAP_TRY(dev_alloc((void**)&xyz, cap * 3 * sizeof(float), false));
-        MAP_TRY(dev_alloc((void**)&rgb, cap * 3, false));
-        MAP_TRY(dev_alloc((void**)&dep, cap * sizeof(float), false));
-        if (have) {
-            GLIC_CUDA_TRY(cudaMemcpyAsync(xyz, m->scan_xyz, have * 3 * sizeof(float), cudaMemcpyDeviceToDevice, s));
-            GLIC_CUDA_TRY(cudaMemcpyAsync(rgb, m->scan_rgb, have * 3, cudaMemcpyDeviceToDevice, s));
-            GLIC_CUDA_TRY(cudaMemcpyAsync(dep, m->scan_depth, have * sizeof(float), cudaMemcpyDeviceToDevice, s));
-        }
-        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-        cudaFree(m->scan_xyz); cudaFree(m->scan_rgb); cudaFree(m->scan_depth);
-        m->scan_xyz = xyz; m->scan_rgb = rgb; m->scan_depth = dep;
-        m->scan_cap = cap;
+// Reserves what the hand-off of n scan points will need: the arena for the first map's sky and LiDAR rows, or for n more rows
+// of extend(), and the staging of their colours and workspace
+int handoff_reserve(glic_mapper* m, int n) {
+    Carver c(nullptr);
+    if (m->initialized) {
+        if (n == 0) return GLIC_OK;
+        c.take<float>((size_t)3 * n);
+        return extend_prepare(m, n, c.total());
     }
-    GLIC_CUDA_TRY(cudaMemcpyAsync(m->scan_xyz + 3 * have, f->xyz, n * 3 * sizeof(float), cudaMemcpyHostToDevice, s));
-    GLIC_CUDA_TRY(cudaMemcpyAsync(m->scan_rgb + 3 * have, f->rgb, n * 3, cudaMemcpyHostToDevice, s));
-    // R_cw = R^T; t_cw = -R_cw t_wc in the product's order (gaussian.cpp:66-67)
-    const double* t = f->t_wc;
-    const double tcw2 = -(((R[2] * t[0]) + (R[5] * t[1])) + (R[8] * t[2]));
-    scan_depth_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((int)n, m->scan_xyz + 3 * have, R[2], R[5], R[8], tcw2, m->scan_depth + have);
-    GLIC_LAUNCH_CHECK();
-    m->fst.pending_points = (uint32_t)(have + n);
-    return GLIC_OK;
+    MAP_TRY(set_capacity(m, (uint32_t)m->frame_sky_points + (uint32_t)n));
+    c.take<double>((size_t)3 * n); c.take<char>(glic_skybox_init_bytes(m->frame_sky_points));
+    return reserve(m, m->extend_ws, c.total());
 }
 
-// mapping.cpp:158-174 at a training keyframe: the accumulated scan initializes the map, or extends it; then it is emptied
-int scan_handoff(glic_mapper* m) {
-    const int n = (int)m->fst.pending_points;
+// mapping.cpp:158-174 at training keyframe kf: the n accumulated scan points initialize the map, or extend it.  Everything is
+// reserved (handoff_reserve); the one allocation left is a binning regrow, which comes before the map changes.
+int scan_handoff(glic_mapper* m, const Keyframe& kf, int n) {
     cudaStream_t s = m->stream;
     const unsigned blocks = (unsigned)((3 * (size_t)n + 255) / 256);
+    Carver c(m->extend_ws);
     if (!m->initialized) {
         const int S = m->frame_sky_points;
-        MAP_TRY(set_capacity(m, (uint32_t)S + (uint32_t)n));
-        Carver c(nullptr);
-        c.take<double>((size_t)3 * n); c.take<char>(glic_skybox_init_bytes(S));
-        MAP_TRY(reserve_staging(m, c.total()));
-        c = Carver(m->extend_ws);
         double* d_col = c.take<double>((size_t)3 * n);
         void* sky_ws = c.take<char>(glic_skybox_init_bytes(S));
         scan_colour_kernel<double><<<blocks, 256, 0, s>>>(3 * n, m->scan_rgb, d_col);
         GLIC_LAUNCH_CHECK();
         const double focal = ((double)m->cfg.fx + (double)m->cfg.fy) / 2;
-        MAP_TRY(initialize_lidar_core(m, n, m->scan_xyz, d_col, m->scan_depth, focal, S, m->frame_sky_radius, sky_ws));
-    } else {
-        m->st.last_inserted = 0;
-        if (n > 0) {
-            Carver c(nullptr);
-            c.take<float>((size_t)3 * n);
-            MAP_TRY(extend_prepare(m, n, c.total()));
-            c = Carver(m->extend_ws);
-            float* d_col = c.take<float>((size_t)3 * n);
-            void* ws = c.take<char>(0);
-            GLIC_CUDA_TRY(cudaEventRecord(m->t0, s));
-            scan_colour_kernel<float><<<blocks, 256, 0, s>>>(3 * n, m->scan_rgb, d_col);
-            GLIC_LAUNCH_CHECK();
-            MAP_TRY(extend_core(m, n, m->scan_xyz, d_col, m->scan_depth, ws));
-        }
+        return initialize_lidar_core(m, n, m->scan_xyz, d_col, m->scan_depth, focal, S, m->frame_sky_radius, sky_ws);
     }
-    m->fst.pending_points = 0;
-    return GLIC_OK;
+    if (n == 0) { m->st.last_inserted = 0; return GLIC_OK; }
+    float* d_col = c.take<float>((size_t)3 * n);
+    void* ws = c.take<char>(0);
+    GLIC_CUDA_TRY(cudaEventRecord(m->t0, s));
+    scan_colour_kernel<float><<<blocks, 256, 0, s>>>(3 * n, m->scan_rgb, d_col);
+    GLIC_LAUNCH_CHECK();
+    return extend_core(m, kf, n, m->scan_xyz, d_col, m->scan_depth, ws);
 }
 
 }  // namespace
@@ -950,67 +942,43 @@ int glic_mapper_create(const glic_mapper_config* cfg, glic_mapper** out) {
         cfg->rank >= cfg->world || cfg->views_per_rank < 1 || cfg->world * cfg->views_per_rank > MAX_SLOTS) {
         set_error("mapper_create: bad configuration"); return GLIC_ERR_INVALID_ARGUMENT;
     }
-    glic_mapper* m = new glic_mapper();
+    std::unique_ptr<glic_mapper> m(new glic_mapper());     // on a failure its members release whatever was made
     m->cfg = *cfg;
     if (m->cfg.max_iters <= 0) m->cfg.max_iters = 100;
     m->D = cfg->sh_degree; m->M = (m->D + 1) * (m->D + 1) - 1;
     m->k = cfg->views_per_rank; m->S = cfg->world * cfg->views_per_rank;
     m->rng.seed(cfg->seed);
-    auto fail = [&](int e) { glic_mapper_destroy(m); return e; };
-    if (cudaGetDevice(&m->dev) != cudaSuccess) { set_error("mapper_create: no CUDA device"); return fail(GLIC_ERR_NO_DEVICE); }
-    if (cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) != cudaSuccess || cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&m->push_stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("mapper_create: stream creation failed"); return fail(GLIC_ERR_CUDA); }
-    cudaEvent_t* evs[] = {&m->gt_free[0], &m->gt_free[1], &m->gt_ready[0], &m->gt_ready[1], &m->ev_flags, &m->ev_col, &m->ev_push, &m->ev_pose};
-    for (cudaEvent_t* e : evs) if (cudaEventCreateWithFlags(e, cudaEventDisableTiming) != cudaSuccess) { set_error("mapper_create: event creation failed"); return fail(GLIC_ERR_CUDA); }
-    for (int r = 0; r < RING; ++r) if (cudaEventCreateWithFlags(&m->ring_ev[r], cudaEventDisableTiming) != cudaSuccess) return fail(GLIC_ERR_CUDA);
-    if (cudaEventCreate(&m->t0) != cudaSuccess || cudaEventCreate(&m->t1) != cudaSuccess) return fail(GLIC_ERR_CUDA);
+    if (cudaGetDevice(&m->dev) != cudaSuccess) { set_error("mapper_create: no CUDA device"); return GLIC_ERR_NO_DEVICE; }
+    cudaStream_t sh = nullptr;
+    cudaEvent_t eh = nullptr;
+    for (Stream* s : {&m->stream, &m->copy_stream, &m->push_stream}) { GLIC_CUDA_TRY(cudaStreamCreateWithFlags(&sh, cudaStreamNonBlocking)); *s = Stream(sh); }
+    std::vector<Event*> evs = {&m->gt_free[0], &m->gt_free[1], &m->gt_ready[0], &m->gt_ready[1], &m->ev_flags, &m->ev_col, &m->ev_push, &m->ev_pose};
+    for (Event& e : m->ring_ev) evs.push_back(&e);
+    for (Event* e : evs) { GLIC_CUDA_TRY(cudaEventCreateWithFlags(&eh, cudaEventDisableTiming)); *e = Event(eh); }
+    for (Event* e : {&m->t0, &m->t1}) { GLIC_CUDA_TRY(cudaEventCreate(&eh)); *e = Event(eh); }
     const int W = cfg->width, H = cfg->height;
     const size_t HW = (size_t)W * H;
-    if (int e = set_capacity(m, cfg->capacity ? cfg->capacity : 1u << 20)) return fail(e);
-    m->image_bytes = glic_image_bytes(W, H);
-    m->loss_bytes = glic_loss_scratch_bytes(3, H, W);
-    m->eval_bytes = glic_eval_scratch_bytes(3, H, W);
-    int e = GLIC_OK;
-    if ((e = dev_alloc(&m->image_ws, m->image_bytes)) || (e = dev_alloc(&m->loss_scratch, m->loss_bytes, false)) || (e = dev_alloc(&m->eval_scratch, m->eval_bytes, false)) ||
-        (e = dev_alloc((void**)&m->color, HW * 12)) || (e = dev_alloc((void**)&m->final_T, HW * 4)) || (e = dev_alloc((void**)&m->dL_dpix, HW * 12)) ||
-        (e = dev_alloc((void**)&m->gt_dev[0], HW * 12)) || (e = dev_alloc((void**)&m->gt_dev[1], HW * 12)) || (e = dev_alloc((void**)&m->loss_dev, 64)) ||
-        (e = dev_alloc((void**)&m->eval_out, 64)) || (e = dev_alloc((void**)&m->vis_acc, 64))) return fail(e);
-    if (cudaHostAlloc((void**)&m->counters_host, sizeof(long long) * 4 * RING, cudaHostAllocDefault) != cudaSuccess ||
-        cudaHostAlloc((void**)&m->loss_host, sizeof(float) * RING, cudaHostAllocDefault) != cudaSuccess) { set_error("mapper_create: pinned allocation failed"); return fail(GLIC_ERR_CUDA); }
+    MAP_TRY(set_capacity(m.get(), cfg->capacity ? cfg->capacity : 1u << 20));
+    MAP_TRY(grow(m.get(), {{m->image_ws, glic_image_bytes(W, H), 0, true}, {m->loss_scratch, glic_loss_scratch_bytes(3, H, W)},
+                           {m->eval_scratch, glic_eval_scratch_bytes(3, H, W)}, {m->color, HW * 12, 0, true}, {m->final_T, HW * 4, 0, true},
+                           {m->dL_dpix, HW * 12, 0, true}, {m->gt_dev[0], HW * 12, 0, true}, {m->gt_dev[1], HW * 12, 0, true},
+                           {m->loss_dev, 64, 0, true}, {m->eval_out, 64, 0, true}, {m->vis_acc, 64, 0, true}}));
+    MAP_TRY(m->counters_host.allocate(sizeof(long long) * 4 * RING, true));
+    MAP_TRY(m->loss_host.allocate(sizeof(float) * RING, true));
     std::memset(m->counters_host, 0, sizeof(long long) * 4 * RING);
     std::memset(m->loss_host, 0, sizeof(float) * RING);
-    if ((e = set_bin_capacity(m, std::max<int64_t>((int64_t)16 * m->Pcap, (int64_t)1 << 22)))) return fail(e);
+    MAP_TRY(set_bin_capacity(m.get(), std::max<int64_t>((int64_t)16 * m->Pcap, (int64_t)1 << 22)));
     cudaEventRecord(m->gt_free[0], m->stream); cudaEventRecord(m->gt_free[1], m->stream);
-    *out = m;
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));       // the copy and push streams and the peers see the zeroed buffers
+    *out = m.release();
     return GLIC_OK;
 }
 
 int glic_mapper_destroy(glic_mapper* m) {
     if (!m) return GLIC_OK;
-    cudaDeviceSynchronize();
-    for (void* p : m->opened) cudaIpcCloseMemHandle(p);
-    void* bufs[] = {m->params, m->m1, m->m2, m->act_opacity, m->act_scales, m->act_rots, m->radii, m->g_conic, m->geom_ws,
-                    m->xblock, m->image_ws, m->binning_ws, m->sample_ws, m->loss_scratch, m->eval_scratch, m->extend_ws, m->color, m->final_T, m->dL_dpix,
-                    m->gt_dev[0], m->gt_dev[1], m->loss_dev, m->eval_out, m->vis_acc};
-    for (void* p : bufs) if (p) cudaFree(p);
-    void* keyframe_state[] = {m->expo_E, m->expo_adam.m, m->expo_adam.v, m->expo_adam.t, m->pose_T, m->pose_f, m->pose_adam.m,
-                              m->pose_adam.v, m->pose_adam.t, m->pose_part, m->lpips_w, m->lpips_scratch};
-    for (void* p : keyframe_state) if (p) cudaFree(p);
-    for (uint8_t* p : m->frame_chunks) cudaFree(p);
-    void* scan[] = {m->scan_xyz, m->scan_rgb, m->scan_depth};
-    for (void* p : scan) if (p) cudaFree(p);
-    for (auto& kf : m->train) if (kf.cam_dev) cudaFree(kf.cam_dev);
-    for (auto& kf : m->test) if (kf.cam_dev) cudaFree(kf.cam_dev);
-    if (m->counters_host) cudaFreeHost(m->counters_host);
-    if (m->loss_host) cudaFreeHost(m->loss_host);
-    cudaEvent_t evs[] = {m->gt_free[0], m->gt_free[1], m->gt_ready[0], m->gt_ready[1], m->ev_flags, m->ev_col, m->ev_push, m->ev_pose, m->t0, m->t1};
-    for (cudaEvent_t e : evs) if (e) cudaEventDestroy(e);
-    for (int r = 0; r < RING; ++r) if (m->ring_ev[r]) cudaEventDestroy(m->ring_ev[r]);
-    if (m->stream) cudaStreamDestroy(m->stream);
-    if (m->copy_stream) cudaStreamDestroy(m->copy_stream);
-    if (m->push_stream) cudaStreamDestroy(m->push_stream);
-    cudaGetLastError();
+    cudaDeviceSynchronize();                               // nothing in flight may still use what the members release
     delete m;
+    cudaGetLastError();
     return GLIC_OK;
 }
 
@@ -1018,6 +986,7 @@ int glic_mapper_initialize(glic_mapper* m, uint32_t P, const float* xyz, const f
                            const float* log_scale, const float* rot) {
     if (!m || (P && (!xyz || !f_dc || !opacity_logit || !log_scale || !rot))) { set_error("mapper_initialize: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
     MAP_TRY(set_capacity(m, P));
+    MAP_TRY(set_bin_capacity(m, (int64_t)16 * P));
     cudaStream_t s = m->stream;
     const size_t nfl = arena_floats(m, m->Pcap);
     GLIC_CUDA_TRY(cudaMemsetAsync(m->params, 0, nfl * 4, s));
@@ -1034,7 +1003,6 @@ int glic_mapper_initialize(glic_mapper* m, uint32_t P, const float* xyz, const f
     m->n_sky = 0;
     m->st.num_gaussians = P;
     m->initialized = true;
-    if ((int64_t)16 * P > m->bin_cap) MAP_TRY(set_bin_capacity(m, (int64_t)16 * P));
     return GLIC_OK;
 }
 
@@ -1050,7 +1018,7 @@ int glic_mapper_initialize_lidar(glic_mapper* m, int n, const float* points, con
     // staging: points | colors | depth | the sky's dist2 and knn workspace
     Carver c(nullptr);
     c.take<float>((size_t)3 * n); c.take<double>((size_t)3 * n); c.take<float>(n); c.take<char>(glic_skybox_init_bytes(sky_points));
-    MAP_TRY(reserve_staging(m, c.total()));
+    MAP_TRY(reserve(m, m->extend_ws, c.total()));
     c = Carver(m->extend_ws);
     float* d_pts = c.take<float>((size_t)3 * n); double* d_col = c.take<double>((size_t)3 * n); float* d_dep = c.take<float>(n);
     void* d_sky = c.take<char>(glic_skybox_init_bytes(sky_points));
@@ -1068,13 +1036,15 @@ int glic_mapper_sky_rows(glic_mapper* m, uint32_t* out) {
 
 int glic_mapper_add_keyframe(glic_mapper* m, const glic_keyframe* kfi, int is_train) {
     if (!m || !kfi || !kfi->image) { set_error("mapper_add_keyframe: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    return add_keyframe_core(m, kfi->R_wc, kfi->t_wc, kfi->image, nullptr, is_train);
+    Keyframe kf;
+    MAP_TRY(make_keyframe(m, kfi->R_wc, kfi->t_wc, kfi->image, nullptr, kf));
+    if (is_train && (m->expo_on || m->pose_on)) MAP_TRY(reserve_keyframe_rows(m, m->train.size() + 1));
+    return push_keyframe(m, std::move(kf), is_train);
 }
 
 int glic_mapper_extend(glic_mapper* m, int n, const float* points, const float* colors, const float* depth_rsp) {
     if (!m || n < 0 || (n && (!points || !colors || !depth_rsp))) { set_error("mapper_extend: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
-    m->st.last_inserted = 0;
-    if (n == 0) return GLIC_OK;
+    if (n == 0) { m->st.last_inserted = 0; return GLIC_OK; }
     if (m->train.empty()) { set_error("mapper_extend: no training keyframe yet"); return GLIC_ERR_INVALID_ARGUMENT; }
     // staging: points | colors | depth | extend_core's workspace
     Carver c(nullptr);
@@ -1088,7 +1058,7 @@ int glic_mapper_extend(glic_mapper* m, int n, const float* points, const float* 
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_pts, points, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, s));
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_col, colors, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, s));
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_dep, depth_rsp, sizeof(float) * n, cudaMemcpyHostToDevice, s));
-    return extend_core(m, n, d_pts, d_col, d_dep, ws);
+    return extend_core(m, m->train.back(), n, d_pts, d_col, d_dep, ws);
 }
 
 int glic_mapper_enable_frames(glic_mapper* m, int select_every_k_frame, int sky_points, int sky_radius) {
@@ -1119,14 +1089,49 @@ int glic_mapper_add_frame(glic_mapper* m, const glic_frame* f, int* is_keyframe)
     float R_wc[9], t_wc[3];
     for (int e = 0; e < 9; ++e) R_wc[e] = (float)R[e];
     for (int i = 0; i < 3; ++i) t_wc[i] = (float)f->t_wc[i];
-    const uint8_t* bgr = nullptr;
-    MAP_TRY(frame_store_push(m, f, &bgr));
-    MAP_TRY(scan_append(m, f, R));
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));      // the caller's buffers are free again
-    MAP_TRY(add_keyframe_core(m, R_wc, t_wc, nullptr, bgr, train));
+    // Reserve everything first: the frame store's next slot (a new chunk when the last one is full), room in the scan buffers
+    // (grown by doubling), the keyframe and, at a training keyframe, its rows and what the hand-off needs
+    const size_t idx = m->fst.frames, have = m->fst.pending_points, n = (size_t)f->n_points;
+    if (idx / FRAME_CHUNK >= m->frame_chunks.size()) {
+        Dev<uint8_t> chunk;
+        MAP_TRY(chunk.allocate(FRAME_CHUNK * m->frame_stride));
+        m->frame_chunks.push_back(std::move(chunk));
+    }
+    if (pending > m->scan_cap) {
+        const size_t cap = std::max<size_t>({pending, 2 * m->scan_cap, 4096});
+        MAP_TRY(grow(m, {{m->scan_xyz, cap * 3 * sizeof(float), have * 3 * sizeof(float)}, {m->scan_rgb, cap * 3, have * 3},
+                         {m->scan_depth, cap * sizeof(float), have * sizeof(float)}}));
+        m->scan_cap = cap;
+    }
+    uint8_t* dst = m->frame_chunks[idx / FRAME_CHUNK] + (idx % FRAME_CHUNK) * m->frame_stride;
+    Keyframe kf;
+    MAP_TRY(make_keyframe(m, R_wc, t_wc, nullptr, dst, kf));
+    if (train) {
+        if (m->expo_on || m->pose_on) MAP_TRY(reserve_keyframe_rows(m, m->train.size() + 1));
+        MAP_TRY(handoff_reserve(m, (int)pending));
+    }
+    // the image without its row padding, and the points after the pending ones with their depths in the frame's camera
+    cudaStream_t s = m->stream;
+    const size_t W3 = 3 * (size_t)m->cfg.width;
+    GLIC_CUDA_TRY(cudaMemcpy2DAsync(dst, W3, f->bgr, f->row_bytes, W3, (size_t)m->cfg.height, cudaMemcpyHostToDevice, s));
+    if (n) {
+        GLIC_CUDA_TRY(cudaMemcpyAsync(m->scan_xyz + 3 * have, f->xyz, n * 3 * sizeof(float), cudaMemcpyHostToDevice, s));
+        GLIC_CUDA_TRY(cudaMemcpyAsync(m->scan_rgb + 3 * have, f->rgb, n * 3, cudaMemcpyHostToDevice, s));
+        // R_cw = R^T; t_cw = -R_cw t_wc in the product's order (gaussian.cpp:66-67)
+        const double* t = f->t_wc;
+        const double tcw2 = -(((R[2] * t[0]) + (R[5] * t[1])) + (R[8] * t[2]));
+        scan_depth_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((int)n, m->scan_xyz + 3 * have, R[2], R[5], R[8], tcw2, m->scan_depth + have);
+        GLIC_LAUNCH_CHECK();
+    }
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));              // the caller's buffers are free again
+    // The hand-off runs before the keyframe joins its list, so that its one possible allocation failure (a binning regrow, before
+    // the map changes) leaves nothing to undo.  It draws the keyframe as it will be pushed: the pose it starts at.
+    if (train) MAP_TRY(scan_handoff(m, kf, (int)pending));
+    MAP_TRY(push_keyframe(m, std::move(kf), train));
+    m->fst.pending_points = train ? 0 : (uint32_t)pending;
     ++m->fst.frames;
     ++(train ? m->fst.train : m->fst.test);
-    if (train) MAP_TRY(scan_handoff(m));
+    m->fst.image_bytes = m->frame_chunks.size() * FRAME_CHUNK * m->frame_stride;
     if (is_keyframe) *is_keyframe = train;
     return GLIC_OK;
 }
@@ -1201,7 +1206,7 @@ int glic_mapper_optimize(glic_mapper* m, const int* views_host, int n_views) {
     MAP_TRY(poll_ring(m, true));
     cudaEventElapsedTime(&m->st.ms_optimize, m->t0, m->t1);
     m->st.mean_visible = (double)vis / (double)iters;
-    if (m->connected) MAP_TRY(glic_p2p_check(m->xblock, m->n_geo, 0, m->stream));
+    if (m->connected) MAP_TRY(glic_p2p_check(m->xblock, m->x.n_geo, 0, m->stream));
     return GLIC_OK;
 }
 
@@ -1218,9 +1223,9 @@ int glic_mapper_load_lpips(glic_mapper* m, const char* path) {
     if (!m || !path) { set_error("mapper_load_lpips: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
     std::vector<float> w(glic_lpips_weight_floats());
     MAP_TRY(glic_lpips_read_weights(path, w.data()));
+    MAP_TRY(reserve(m, m->lpips_w, w.size() * sizeof(float)));
+    GLIC_CUDA_TRY(cudaMemcpyAsync(m->lpips_w, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice, m->stream));
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    if (!m->lpips_w) MAP_TRY(dev_alloc((void**)&m->lpips_w, w.size() * sizeof(float), false));
-    GLIC_CUDA_TRY(cudaMemcpy(m->lpips_w, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice));
     return GLIC_OK;
 }
 
@@ -1230,13 +1235,10 @@ int glic_mapper_evaluate_lpips(glic_mapper* m, int is_train, int index, float* p
     const int W = m->cfg.width, H = m->cfg.height;
     const size_t need = glic_lpips_scratch_bytes(H, W);
     if (!need) { set_error("mapper_evaluate_lpips: LPIPS needs a frame of at least 31x31"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!m->lpips_scratch) {
-        MAP_TRY(dev_alloc(&m->lpips_scratch, need, false));
-        m->lpips_bytes = need;
-    }
+    MAP_TRY(reserve(m, m->lpips_scratch, need));
     MAP_TRY(render_scored(m, is_train, index, "mapper_evaluate_lpips"));
     MAP_TRY(glic_lpips(H, W, eval_clamped(m->eval_scratch, 3, H, W, 0), eval_clamped(m->eval_scratch, 3, H, W, 1), m->lpips_w,
-                       m->eval_out + 2, m->lpips_scratch, m->lpips_bytes, m->stream));
+                       m->eval_out + 2, m->lpips_scratch, m->lpips_scratch.bytes(), m->stream));
     float out3[3] = {0.f, 0.f, 0.f};
     MAP_TRY(read_eval_out(m, out3, 3));
     *psnr = out3[0]; *ssim = out3[1]; *lpips = out3[2];
@@ -1297,38 +1299,29 @@ int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, uint32_t* 
         return GLIC_OK;
     }
     cudaStream_t s = m->stream;
-    MAP_TRY(reserve_staging(m, prune_scratch_bytes(P)));            // the selection's scratch: the idle extend() staging
+    MAP_TRY(reserve(m, m->extend_ws, prune_scratch_bytes(P)));  // the selection's scratch: the idle extend() staging
     void* scratch = m->extend_ws;
     float* g[6];
     arena_ptrs(m, m->params, m->Pcap, g);
     uint32_t kept[2] = {0, 0};
-    int e = launch_prune_select(P, m->n_sky, g[3], min_opacity, scratch, kept, s);
-    if (e == GLIC_OK && kept[0] == 0) {
-        set_error("mapper_prune: the threshold removes every row (an empty map cannot be trained)");
-        e = GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (e == GLIC_OK && !dry_run && kept[0] < P) {
-        float* spare = nullptr;
+    MAP_TRY(launch_prune_select(P, m->n_sky, g[3], min_opacity, scratch, kept, s));
+    if (kept[0] == 0) { set_error("mapper_prune: the threshold removes every row (an empty map cannot be trained)"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!dry_run && kept[0] < P) {
+        Dev<float> spare;
         const size_t bytes = arena_floats(m, m->Pcap) * sizeof(float);
-        e = dev_alloc((void**)&spare, bytes, false);
-        if (e == GLIC_OK) {
-            if (cudaMemsetAsync(spare, 0, bytes, s) != cudaSuccess) { set_error("mapper_prune: cudaMemsetAsync failed"); e = GLIC_ERR_CUDA; }
-            for (float** arena : {&m->params, &m->m1, &m->m2}) {
-                if (e != GLIC_OK) break;
-                e = launch_prune_gather(*arena, spare, m->Pcap, m->M, P, kept[0], scratch, s);
-                if (e == GLIC_OK) std::swap(*arena, spare);
-            }
-            if (e == GLIC_OK && cudaStreamSynchronize(s) != cudaSuccess) { set_error("mapper_prune: synchronisation failed"); e = GLIC_ERR_CUDA; }
-            cudaFree(spare);
+        MAP_TRY(spare.allocate(bytes));
+        GLIC_CUDA_TRY(cudaMemsetAsync(spare, 0, bytes, s));
+        for (Dev<float>* arena : {&m->params, &m->m1, &m->m2}) {
+            MAP_TRY(launch_prune_gather(*arena, spare, m->Pcap, m->M, P, kept[0], scratch, s));
+            std::swap(*arena, spare);
         }
-        if (e == GLIC_OK) {
-            m->P = kept[0];
-            m->n_sky = kept[1];
-            m->st.num_gaussians = kept[0];
-        }
+        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+        m->P = kept[0];
+        m->n_sky = kept[1];
+        m->st.num_gaussians = kept[0];
     }
-    if (e == GLIC_OK && removed) *removed = P - kept[0];
-    return e;
+    if (removed) *removed = P - kept[0];
+    return GLIC_OK;
 }
 
 int glic_mapper_save_map(glic_mapper* m, const char* path) {
@@ -1365,15 +1358,8 @@ int glic_mapper_enable_exposure(glic_mapper* m, float exposure_lr) {
     if (!m) { set_error("mapper_enable_exposure: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (!(exposure_lr >= 0.0f) || !std::isfinite(exposure_lr)) { set_error("mapper_enable_exposure: exposure_lr must be finite and >= 0"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (!m->expo_on) {
-        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-        const size_t need = glic_loss_exposure_scratch_bytes(m->cfg.height, m->cfg.width);
-        if (need > m->loss_bytes) {
-            cudaFree(m->loss_scratch);
-            m->loss_scratch = nullptr;
-            MAP_TRY(dev_alloc(&m->loss_scratch, need, false));
-            m->loss_bytes = need;
-        }
-        MAP_TRY(expo_reserve(m, m->train.size()));
+        MAP_TRY(reserve(m, m->loss_scratch, glic_loss_exposure_scratch_bytes(m->cfg.height, m->cfg.width)));
+        MAP_TRY(reserve_keyframe_rows(m, m->train.size()));
         MAP_TRY(expo_reset(m, 0, m->train.size()));
         m->expo_on = true;
     }
@@ -1407,7 +1393,7 @@ int glic_mapper_enable_pose_refinement(glic_mapper* m, float lr_translation, flo
         set_error("mapper_enable_pose_refinement: the learning rates must be finite and >= 0"); return GLIC_ERR_INVALID_ARGUMENT;
     }
     if (!m->pose_on) {                               // every training keyframe starts at its given pose with zero state
-        MAP_TRY(pose_reserve(m, m->train.size()));
+        MAP_TRY(reserve_keyframe_rows(m, m->train.size()));
         for (size_t k = 0; k < m->train.size(); ++k) MAP_TRY(pose_write(m, k, m->train[k].R_wc, m->train[k].t_wc, true));
         m->pose_on = true;
     }
@@ -1473,10 +1459,18 @@ int glic_mapper_connect(glic_mapper* m, const unsigned char* handles) {
         void* p = nullptr;
         GLIC_CUDA_TRY(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
         m->peers[q] = p;
-        m->opened.push_back(p);
+        m->opened.emplace_back(p);
     }
     m->connected = true;
     return GLIC_OK;
 }
+
+int glic_debug_fail_allocation(int n) {
+    if (n < 0) { set_error("debug_fail_allocation: n must be >= 0"); return GLIC_ERR_INVALID_ARGUMENT; }
+    fail_countdown = n;
+    return GLIC_OK;
+}
+
+int64_t glic_debug_mapper_allocations(void) { return live_allocations; }
 
 }  // extern "C"

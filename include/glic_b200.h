@@ -325,6 +325,11 @@ GLIC_API int glic_debug_render_backward(int P, const glic_view* view, int64_t R,
                                         const void* image_ws, const void* sample_ws, const float* dL_dpix, float* dL_dmeans2D,
                                         float* dL_dconic, float* dL_dopacity, float* dL_dcolors, int exact,
                                         unsigned long long* counters, void* stream);
+/* Allocation failures of the native mapper, simulated on the host (no CUDA call is made for the failing one): the n-th device
+ * or pinned allocation a mapper makes from now on returns cudaErrorMemoryAllocation; n = 0 disarms it, n < 0 is refused.
+ * glic_debug_mapper_allocations is the number of allocations the mappers of this process hold right now. */
+GLIC_API int glic_debug_fail_allocation(int n);
+GLIC_API int64_t glic_debug_mapper_allocations(void);
 
 /* ---------------------------------------------------------------------------------------
  * Multi-GPU exchange step (no counterpart in the reference, which is single-GPU): in-place MEAN all-reduce of the
@@ -420,6 +425,10 @@ GLIC_API int glic_arena_regrow(const float* src, uint32_t Pcap_src, float* dst, 
  * then applies the identical Adam step (replicas stay bit-identical).  Semantics: mean of the per-view losses over all
  * world * views_per_rank views, one optimiser step per batch.
  * All host pointers unless stated.  Status codes as everywhere; the mapper never throws.
+ * Failure contract: a mapper call that cannot allocate returns GLIC_ERR_CUDA and leaves everything the getters return unchanged,
+ * except that capacities (stats.capacity, the workspaces) may have grown; the host may free memory (glic_mapper_prune) and call
+ * again.  glic_mapper_optimize is the one exception: a binning regrow that fails between its batches returns the error with the
+ * old workspace intact, and the batches already enqueued stand, as they do for any error in the middle of the list.
  * ------------------------------------------------------------------------------------- */
 typedef struct glic_mapper glic_mapper;
 
