@@ -142,6 +142,10 @@ def _load():
         "glic_mapper_stats_get": (i32, [vp, C.POINTER(MapperStats)]),
         "glic_mapper_download": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "glic_mapper_prune": (i32, [vp, f32, i32, C.POINTER(u32)]),
+        "glic_mapper_enable_densification": (i32, [vp]),
+        "glic_mapper_densify": (i32, [vp, f32, f32, f32, i32, C.POINTER(u32), C.POINTER(u32)]),
+        "glic_mapper_densify_stats": (i32, [vp, vp, vp]),
+        "glic_densify_split": (i32, [i32, vp, vp, vp, C.c_uint64, C.c_uint64, u32, vp, vp, vp]),
         "glic_mapper_export": (i32, [vp, C.c_char_p]),
         "glic_mapper_connect": (i32, [vp, C.c_char_p]),
         "glic_mapper_synchronize": (i32, [vp]),

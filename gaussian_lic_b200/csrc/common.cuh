@@ -27,6 +27,19 @@ constexpr int NUM_SMS = 132;            // H100 SXM: sizes the grid-stride launc
 // torch::sigmoid of an opacity logit (GaussianModel::getOpacity, gaussian.cpp:147-150) as the activation kernel evaluates it;
 // glic_mapper_prune decides with the same expression, so its 1/255 cut is the preprocess's o < 1/255 test bit for bit
 __device__ __forceinline__ float opacity_activation(float logit) { return 1.0f / (1.0f + expf(-logit)); }
+// the SplitMix64 finaliser (Steele, Lea, Flood, OOPSLA 2014): the counter-based generators of the skybox and the split children
+__device__ __forceinline__ uint64_t splitmix64_mix(uint64_t z) {
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+// torch::exp of a log-scale and normalize (p = 2, eps = 1e-12) of a raw rotation (getScaling / getRotation) as the activation
+// kernel evaluates them; glic_mapper_densify decides and places the split children with the same expressions
+__device__ __forceinline__ float scale_activation(float log_scale) { return expf(log_scale); }
+__device__ __forceinline__ float4 rotation_activation(float4 q) {
+    const float n = fmaxf(sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w), 1e-12f);
+    return make_float4(q.x / n, q.y / n, q.z / n, q.w / n);
+}
 
 // ---- error plumbing --------------------------------------------------------------------
 void set_error(const std::string& s);
@@ -280,6 +293,10 @@ struct CompactGrads {
     // camera-pose gradient of the view (preprocess_backward.cu, POSE); both NULL: not computed
     double* pose_partials;    // [ceil(P/128)][6] per-CTA float64 partial sums (pose_partials_count(capacity) doubles)
     float* pose_grad;         // [6] dL/d(rho, omega) of the view, written by the finish kernel
+    // densification statistics of the view (glic_mapper_enable_densification); both NULL: not computed.  Written or accumulated
+    // like the geometric gradients: |(dL/dmean2D.x, .y)| and 1 for a visible row, 0 and 0 for a culled one
+    float* dens_norm;         // [P]
+    float* dens_count;        // [P]
 };
 // doubles of the pose-gradient scratch for up to Pcap Gaussians
 size_t pose_partials_count(uint32_t Pcap);
@@ -349,7 +366,10 @@ namespace glic {
 int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, float* exp_avg, float* exp_avg_sq, const float* g_geo,
                         uint32_t Pcap_geo, const float* lr6, const float* g_color, const uint8_t* flags, const float* const* campos_dev,
                         int n_slots, float grad_scale, float color_scale, float b1, float b2, float eps, const unsigned int* skip_flag,
-                        unsigned int* visible_count, cudaStream_t s);
+                        unsigned int* visible_count, cudaStream_t s, const float* g_dens = nullptr, float* dens_accum = nullptr,
+                        float* dens_denom = nullptr, float dens_scale = 1.0f);
+// g_dens (optional): the densification statistics of the batch in the gradient block, norms [Pcap_geo] | counts [Pcap_geo]; the
+// Adam launch adds dens_scale times them to dens_accum / dens_denom for every row visible in some slot, unless skip_flag is set
 // campos_dev: n_slots host-held device pointers, each slot's camera centre (read on the device)
 int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flags, cudaStream_t s);
 // per-keyframe exposure (ssim.cu): one Adam step of every keyframe of a batch of S <= EXPO_MAX_SLOTS slots; slot_grads[S][12]
@@ -368,4 +388,20 @@ size_t prune_scratch_bytes(uint32_t P);
 int launch_prune_select(uint32_t P, uint32_t n_sky, const float* opacity_logit, float min_opacity, void* scratch, uint32_t* result_host,
                         cudaStream_t s);
 int launch_prune_gather(const float* src, float* dst, uint32_t Pcap, int M, uint32_t P_old, uint32_t P_new, const void* scratch, cudaStream_t s);
+// the select's index map: idx[new] = old for the P_new kept rows
+const uint32_t* prune_index(const void* scratch, uint32_t P);
+// dst[r] = r < rows_valid ? src[idx[r]] : 0 for r < rows_out (one float per row)
+int launch_gather_floats(const float* src, float* dst, uint32_t rows_out, uint32_t rows_valid, const uint32_t* idx, cudaStream_t s);
+// output rows [0, rows_out) of every group of dst: row r < rows_valid takes row idx[r] of src, the others are zero
+int launch_gather_rows(const float* src, float* dst, uint32_t Pcap, int M, uint32_t rows_out, uint32_t rows_valid, const uint32_t* idx,
+                       cudaStream_t s);
+// densification (prune.cu, glic_mapper_densify).  select: classes of rows [0, P) (keep, clone, split; rows below n_sky are
+// kept) from the statistics and the log-scale group; result_host[2] = {clones, splits}, synchronises s; the scratch then
+// holds the index map of the result rows (densify_index).  children: rows [first, first + n) of the arena, copies of their
+// parents, become split children in place (xyz and log-scale).
+size_t densify_scratch_bytes(uint32_t P);
+int launch_densify_select(uint32_t P, uint32_t n_sky, const float* accum, const float* denom, const float* log_scale, float grad_threshold,
+                          float clone_max_scale, void* scratch, uint32_t* result_host, cudaStream_t s);
+const uint32_t* densify_index(const void* scratch, uint32_t P);
+int launch_densify_children(float* params, uint32_t Pcap, int M, uint32_t first, uint32_t n, uint64_t seed, uint64_t call, cudaStream_t s);
 }  // namespace glic

@@ -14,14 +14,8 @@
 namespace glic {
 namespace {
 
-__device__ __forceinline__ uint64_t sky_mix64(uint64_t z) {
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    return z ^ (z >> 31);
-}
-
 __device__ __forceinline__ void sky_uniforms(uint64_t seed, uint32_t row, float& u1, float& u2) {
-    const uint64_t r = sky_mix64(seed + ((uint64_t)row + 1) * 0x9E3779B97F4A7C15ull);
+    const uint64_t r = splitmix64_mix(seed + ((uint64_t)row + 1) * 0x9E3779B97F4A7C15ull);
     u1 = __fmul_rn((float)(uint32_t)(r >> 40), 5.9604644775390625e-08f);               // * 2^-24: exact
     u2 = __fmul_rn((float)(uint32_t)((r >> 16) & 0xFFFFFFu), 5.9604644775390625e-08f);
 }

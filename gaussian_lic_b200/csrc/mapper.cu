@@ -12,7 +12,7 @@
 //   * multi-GPU (view-sharded): per-view colour gradients + flag bytes are PUSHED to every peer's exchange block by the
 //     copy engines over NVLink as soon as the render backward has produced them (overlapping the per-Gaussian backward),
 //     the 11 geometric floats are mean-reduced in place by the two-shot kernel of p2p.cu; every replica then runs the same
-//     Adam launch on the same bytes.
+//     Adam launch on the same bytes.  With densification on, the view's statistics ride along as two more rows (13 floats).
 #include "common.cuh"
 #include "adam_math.cuh"
 
@@ -313,7 +313,8 @@ struct KeyframeAdam {
     Dev<int> t;
 };
 
-// The exchange block: geo[11*Pcap + 4] | flags words | one region [2][S] of slots per SlotRegion
+// The exchange block: geo[11*Pcap + 4 (+ 2*Pcap)] | flags words | one region [2][S] of slots per SlotRegion.  With densification
+// on, the reduced region ends in the batch's statistics rows: norms [Pcap] | view counts [Pcap], at 11*Pcap + 4.
 struct XLayout {
     size_t n_geo = 0;                // floats in the reduced region (11*Pcap + 4; the tail holds the collective overflow word)
     size_t bytes = 0, slot_off[N_REGIONS] = {}, slot_bytes[N_REGIONS] = {};
@@ -386,6 +387,12 @@ struct glic_mapper {
     Dev<uint8_t> scan_rgb;
     size_t scan_cap = 0;
     glic_frame_stats fst{};
+    // ---- densification (glic_mapper_enable_densification): per-row statistics [Pcap] each, and the number of real densify
+    //      calls so far (the key of the split children's generator) ----
+    bool dens_on = false;
+    bool exported = false;                // glic_mapper_export has run: the exchange block can no longer move
+    Dev<float> dens_accum, dens_denom;
+    uint64_t dens_calls = 0;
 };
 
 namespace {
@@ -398,7 +405,7 @@ struct Grow { Buf& buf; size_t bytes, keep = 0; bool zero = false; };
 // The one way a mapper's buffers grow: allocate every new buffer; on the mapper's stream zero those that start zeroed and copy the
 // kept prefixes (then `fill`, which set_capacity uses to regrow the arenas into the new buffers); synchronise; only then swap the
 // new buffers in and release the old.  A failed allocation leaves every buffer as it was.
-int grow(glic_mapper* m, std::initializer_list<Grow> list, const std::function<int(Buf*)>& fill = nullptr) {
+int grow(glic_mapper* m, const std::vector<Grow>& list, const std::function<int(Buf*)>& fill = nullptr) {
     std::vector<Buf> fresh(list.size());
     Buf* b = fresh.data();
     for (const Grow& g : list) MAP_TRY((b++)->allocate(g.bytes));
@@ -416,7 +423,7 @@ int grow(glic_mapper* m, std::initializer_list<Grow> list, const std::function<i
 }
 
 // grows b to at least `need` bytes without keeping its contents
-int reserve(glic_mapper* m, Buf& b, size_t need) { return need <= b.bytes() ? GLIC_OK : grow(m, {{b, need}}); }
+int reserve(glic_mapper* m, Buf& b, size_t need) { return need <= b.bytes() ? GLIC_OK : grow(m, {Grow{b, need}}); }
 
 size_t arena_floats(const glic_mapper* m, uint32_t cap) { return glic_packed_floats(cap, (uint32_t)m->M); }
 
@@ -436,9 +443,9 @@ T* slot(const glic_mapper* m, SlotRegion r, int parity, int s) {
 
 // The slot regions follow the flags words, each [2][S] slots rounded up to 256 bytes: colour gradients [cap][3] floats, flag
 // bytes [cap], dL/dE [12] floats, dL/d(rho, omega) [8] floats (2 unused).
-XLayout xblock_layout(int S, uint32_t cap) {
+XLayout xblock_layout(int S, uint32_t cap, bool dens) {
     XLayout x;
-    x.n_geo = (size_t)11 * cap + 4;
+    x.n_geo = (size_t)(dens ? 13 : 11) * cap + 4;
     size_t sl[6];
     glic_p2p_slice(0, 1, x.n_geo, 0, sl);
     const size_t bytes[N_REGIONS] = {(size_t)cap * 3 * sizeof(float), cap, 12 * sizeof(float), 8 * sizeof(float)};
@@ -468,18 +475,21 @@ int set_capacity(glic_mapper* m, uint32_t cap) {
     if (cap <= m->Pcap) return GLIC_OK;
     if (m->connected) { set_error("mapper: the arena capacity is fixed once the exchange blocks are connected (world > 1); create the mapper with a larger capacity"); return GLIC_ERR_WORKSPACE; }
     const size_t arena = arena_floats(m, cap) * sizeof(float);
-    const XLayout x = xblock_layout(m->S, cap);
+    const XLayout x = xblock_layout(m->S, cap, m->dens_on);
     auto regrow = [&](Buf* fresh) -> int {
         const float* old[3] = {m->params, m->m1, m->m2};
         for (int a = 0; a < 3 && m->P; ++a)
             MAP_TRY(glic_arena_regrow(old[a], m->Pcap, static_cast<float*>(fresh[a].raw()), cap, (uint32_t)m->M, m->P, m->stream));
         return GLIC_OK;
     };
-    MAP_TRY(grow(m, {{m->params, arena, 0, true}, {m->m1, arena, 0, true}, {m->m2, arena, 0, true},
-                     {m->act_opacity, (size_t)cap * 4, 0, true}, {m->act_scales, (size_t)cap * 12, 0, true},
-                     {m->act_rots, (size_t)cap * 16, 0, true}, {m->radii, (size_t)cap * 4, 0, true},
-                     {m->g_conic, (size_t)cap * (16 + 12 + 4), 0, true}, {m->geom_ws, glic_geom_bytes((int)cap), 0, true},
-                     {m->xblock, x.bytes, 0, true}, {m->pose_part, pose_partials_count(cap) * sizeof(double)}}, regrow));
+    std::vector<Grow> list = {{m->params, arena, 0, true}, {m->m1, arena, 0, true}, {m->m2, arena, 0, true},
+                              {m->act_opacity, (size_t)cap * 4, 0, true}, {m->act_scales, (size_t)cap * 12, 0, true},
+                              {m->act_rots, (size_t)cap * 16, 0, true}, {m->radii, (size_t)cap * 4, 0, true},
+                              {m->g_conic, (size_t)cap * (16 + 12 + 4), 0, true}, {m->geom_ws, glic_geom_bytes((int)cap), 0, true},
+                              {m->xblock, x.bytes, 0, true}, {m->pose_part, pose_partials_count(cap) * sizeof(double)}};
+    if (m->dens_on)                                       // the statistics keep their live rows
+        for (Buf* b : {(Buf*)&m->dens_accum, (Buf*)&m->dens_denom}) list.push_back({*b, (size_t)cap * 4, (size_t)m->P * 4, true});
+    MAP_TRY(grow(m, list, regrow));
     m->g_mean2D = m->g_conic + (size_t)cap * 4;           // conic first: float4-aligned
     m->g_opacity = m->g_mean2D + (size_t)cap * 3;
     m->x = x;
@@ -539,6 +549,14 @@ int pose_write(glic_mapper* m, size_t k, const float* R_wc, const float* t_wc, b
     GLIC_CUDA_TRY(cudaMemcpyAsync(m->pose_f + 12 * k, f12, sizeof(f12), cudaMemcpyHostToDevice, m->stream));
     if (reset) MAP_TRY(adam_reset(m, m->pose_adam, k, k + 1));
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    return GLIC_OK;
+}
+
+// zero statistics for every row, on the mapper's stream (a no-op with densification off)
+int dens_reset(glic_mapper* m) {
+    if (!m->dens_on) return GLIC_OK;
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->dens_accum, 0, (size_t)m->Pcap * 4, m->stream));
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->dens_denom, 0, (size_t)m->Pcap * 4, m->stream));
     return GLIC_OK;
 }
 
@@ -677,6 +695,8 @@ int iteration(glic_mapper* m, const int* views) {
         cg.accumulate = j > 0;
         cg.pose_partials = m->pose_on ? (double*)m->pose_part : nullptr;        // this view's dL/d(rho, omega), fused into the backward
         cg.pose_grad = m->pose_on ? slot(m, POSE, parity, sl) : nullptr;
+        cg.dens_norm = m->dens_on ? geo_tail + 4 : nullptr;                        // this view's statistics, summed over the rank's views
+        cg.dens_count = m->dens_on ? geo_tail + 4 + m->Pcap : nullptr;
         MAP_TRY(glic_backward_compact_internal((int)m->P, m->D, m->M, g[1], m->act_scales, m->act_rots, m->M ? g[5] : nullptr, &kf.view, m->radii,
                                                m->bin_cap, m->geom_ws, m->binning_ws, m->image_ws, m->sample_ws, m->dL_dpix, m->g_mean2D,
                                                m->g_conic, m->g_opacity, col, &cg, m->cfg.world > 1 ? (void*)m->ev_col : nullptr, s));
@@ -707,7 +727,8 @@ int iteration(glic_mapper* m, const int* views) {
     if (m->run_optimizer)
     MAP_TRY(launch_adam_compact(m->P, m->Pcap, m->D, m->M, m->params, m->m1, m->m2, geo, m->Pcap, lr6, slot(m, COLOUR, parity, 0),
                                 slot<uint8_t>(m, FLAGS, parity, 0), campos, m->S, 1.0f / (float)m->k, color_scale, 0.9f, 0.999f, 1e-15f,
-                                reinterpret_cast<const unsigned int*>(geo_tail), m->vis_acc, s));
+                                reinterpret_cast<const unsigned int*>(geo_tail), m->vis_acc, s, m->dens_on ? geo_tail + 4 : nullptr,
+                                m->dens_accum, m->dens_denom, (float)m->cfg.world));
     // every replica steps the batch's exposures from the same S slot gradients, in slot order
     if (m->run_optimizer && m->expo_on)
         MAP_TRY(launch_exposure_adam(m->S, views, slot(m, EXPOSURE, parity, 0), m->expo_E, m->expo_adam.m, m->expo_adam.v, m->expo_adam.t, m->expo_lr,
@@ -780,6 +801,7 @@ int initialize_lidar_core(glic_mapper* m, int n, const float* d_pts, const doubl
     GLIC_CUDA_TRY(cudaMemsetAsync(m->params, 0, nfl * 4, s));
     GLIC_CUDA_TRY(cudaMemsetAsync(m->m1, 0, nfl * 4, s));
     GLIC_CUDA_TRY(cudaMemsetAsync(m->m2, 0, nfl * 4, s));
+    MAP_TRY(dens_reset(m));
     float* g[6];                                    // rot, xyz, log-scale, opacity, f_dc, f_rest
     arena_ptrs(m, m->params, m->Pcap, g);
     MAP_TRY(glic_skybox_init(sky_points, sky_radius, m->cfg.seed, sky_ws, glic_skybox_init_bytes(sky_points), g[1], g[4], g[2], g[0], g[3], nullptr, s));
@@ -992,6 +1014,7 @@ int glic_mapper_initialize(glic_mapper* m, uint32_t P, const float* xyz, const f
     GLIC_CUDA_TRY(cudaMemsetAsync(m->params, 0, nfl * 4, s));
     GLIC_CUDA_TRY(cudaMemsetAsync(m->m1, 0, nfl * 4, s));
     GLIC_CUDA_TRY(cudaMemsetAsync(m->m2, 0, nfl * 4, s));
+    MAP_TRY(dens_reset(m));
     float* g[6];
     arena_ptrs(m, m->params, m->Pcap, g);
     const float* src[6] = {rot, xyz, log_scale, opacity_logit, f_dc, f_rest};
@@ -1307,13 +1330,23 @@ int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, uint32_t* 
     MAP_TRY(launch_prune_select(P, m->n_sky, g[3], min_opacity, scratch, kept, s));
     if (kept[0] == 0) { set_error("mapper_prune: the threshold removes every row (an empty map cannot be trained)"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (!dry_run && kept[0] < P) {
-        Dev<float> spare;
+        Dev<float> spare, spare_stats[2];
         const size_t bytes = arena_floats(m, m->Pcap) * sizeof(float);
         MAP_TRY(spare.allocate(bytes));
+        if (m->dens_on)                                    // the statistics move with their rows (and their spares are zero)
+            for (Dev<float>& b : spare_stats) MAP_TRY(b.allocate((size_t)m->Pcap * 4));
         GLIC_CUDA_TRY(cudaMemsetAsync(spare, 0, bytes, s));
         for (Dev<float>* arena : {&m->params, &m->m1, &m->m2}) {
             MAP_TRY(launch_prune_gather(*arena, spare, m->Pcap, m->M, P, kept[0], scratch, s));
             std::swap(*arena, spare);
+        }
+        if (m->dens_on) {
+            Dev<float>* stats[2] = {&m->dens_accum, &m->dens_denom};
+            for (int q = 0; q < 2; ++q) {
+                GLIC_CUDA_TRY(cudaMemsetAsync(spare_stats[q], 0, (size_t)m->Pcap * 4, s));
+                MAP_TRY(launch_gather_floats(*stats[q], spare_stats[q], P, kept[0], prune_index(scratch, P), s));
+                std::swap(*stats[q], spare_stats[q]);
+            }
         }
         GLIC_CUDA_TRY(cudaStreamSynchronize(s));
         m->P = kept[0];
@@ -1321,6 +1354,92 @@ int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, uint32_t* 
         m->st.num_gaussians = kept[0];
     }
     if (removed) *removed = P - kept[0];
+    return GLIC_OK;
+}
+
+int glic_mapper_enable_densification(glic_mapper* m) {
+    if (!m) { set_error("mapper_enable_densification: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (m->dens_on) return GLIC_OK;
+    if (m->cfg.world > 1 && (m->exported || m->connected)) {
+        set_error("mapper_enable_densification: with world > 1 it must come before glic_mapper_export (the exchange block grows)");
+        return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    MAP_TRY(poll_ring(m, true));
+    // the exchange block gains the two statistics rows; every new buffer starts zeroed
+    const XLayout x = xblock_layout(m->S, m->Pcap, true);
+    MAP_TRY(grow(m, {{m->xblock, x.bytes, 0, true}, {m->dens_accum, (size_t)m->Pcap * 4, 0, true}, {m->dens_denom, (size_t)m->Pcap * 4, 0, true}}));
+    m->x = x;
+    m->peers[m->cfg.rank] = m->xblock;
+    m->dens_on = true;
+    return GLIC_OK;
+}
+
+// Inria's densify_and_clone + densify_and_split (N = 2) as one three-way compaction (prune.cu): select, reserve (capacity, then
+// one spare arena), gather every arena into the spare in rotation as prune does (the moments keep only the kept rows: the new
+// rows' moments are zero), write the children's xyz and log-scale, zero the statistics.
+int glic_mapper_densify(glic_mapper* m, float grad_threshold, float percent_dense, float scene_extent, int dry_run, uint32_t* cloned,
+                        uint32_t* split) {
+    if (!m) { set_error("mapper_densify: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!m->dens_on) { set_error("mapper_densify: densification is not enabled (glic_mapper_enable_densification)"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!std::isfinite(grad_threshold) || grad_threshold < 0.0f || !std::isfinite(percent_dense) || percent_dense < 0.0f ||
+        !std::isfinite(scene_extent) || !(scene_extent > 0.0f)) {
+        set_error("mapper_densify: grad_threshold and percent_dense must be finite and >= 0, scene_extent finite and > 0");
+        return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    MAP_TRY(poll_ring(m, true));
+    const uint32_t P = m->P;
+    uint32_t cnt[2] = {0, 0};                                      // clones, splits
+    cudaStream_t s = m->stream;
+    if (P) {
+        MAP_TRY(reserve(m, m->extend_ws, densify_scratch_bytes(P)));   // the selection's scratch: the idle extend() staging
+        float* g[6];
+        arena_ptrs(m, m->params, m->Pcap, g);
+        const float clone_max = percent_dense * scene_extent;
+        MAP_TRY(launch_densify_select(P, m->n_sky, m->dens_accum, m->dens_denom, g[2], grad_threshold, clone_max, m->extend_ws, cnt, s));
+    }
+    const uint32_t n_clone = cnt[0], n_split = cnt[1];
+    const uint64_t total = (uint64_t)P + n_clone + n_split;
+    if (!dry_run && total > P) {
+        if (total > m->Pcap) {
+            if (m->connected) {
+                set_error("mapper_densify: the result does not fit the capacity, which is fixed once the exchange blocks are connected (world > 1); prune first");
+                return GLIC_ERR_WORKSPACE;
+            }
+            MAP_TRY(set_capacity(m, std::max<uint32_t>((uint32_t)total, 2 * m->Pcap)));
+        }
+        Dev<float> spare;
+        const size_t bytes = arena_floats(m, m->Pcap) * sizeof(float);
+        MAP_TRY(spare.allocate(bytes));
+        GLIC_CUDA_TRY(cudaMemsetAsync(spare, 0, bytes, s));
+        const uint32_t* idx = densify_index(m->extend_ws, P);
+        const uint32_t kept = P - n_split;
+        for (Dev<float>* arena : {&m->params, &m->m1, &m->m2}) {
+            MAP_TRY(launch_gather_rows(*arena, spare, m->Pcap, m->M, (uint32_t)total, arena == &m->params ? (uint32_t)total : kept, idx, s));
+            std::swap(*arena, spare);
+        }
+        MAP_TRY(launch_densify_children(m->params, m->Pcap, m->M, kept + n_clone, 2 * n_split, m->cfg.seed, m->dens_calls, s));
+        m->P = (uint32_t)total;
+        m->st.num_gaussians = m->P;
+    }
+    if (!dry_run) {
+        MAP_TRY(dens_reset(m));                                    // densification_postfix: the statistics start again
+        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+        ++m->dens_calls;
+    }
+    if (cloned) *cloned = n_clone;
+    if (split) *split = n_split;
+    return GLIC_OK;
+}
+
+int glic_mapper_densify_stats(glic_mapper* m, float* grad_accum, float* denom) {
+    if (!m || !grad_accum || !denom) { set_error("mapper_densify_stats: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!m->dens_on) { set_error("mapper_densify_stats: densification is not enabled (glic_mapper_enable_densification)"); return GLIC_ERR_INVALID_ARGUMENT; }
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    if (!m->P) return GLIC_OK;
+    GLIC_CUDA_TRY(cudaMemcpy(grad_accum, m->dens_accum, (size_t)m->P * 4, cudaMemcpyDeviceToHost));
+    GLIC_CUDA_TRY(cudaMemcpy(denom, m->dens_denom, (size_t)m->P * 4, cudaMemcpyDeviceToHost));
     return GLIC_OK;
 }
 
@@ -1447,6 +1566,7 @@ int glic_mapper_export(glic_mapper* m, unsigned char* handle64) {
     cudaIpcMemHandle_t h;
     GLIC_CUDA_TRY(cudaIpcGetMemHandle(&h, m->xblock));
     std::memcpy(handle64, &h, 64);
+    m->exported = true;
     return GLIC_OK;
 }
 

@@ -28,10 +28,8 @@ activations_forward_kernel(int P, const float* __restrict__ opacity_logit, const
     if (i >= P) return;
     opacity[i] = opacity_activation(opacity_logit[i]);
 #pragma unroll
-    for (int c = 0; c < 3; ++c) scale[3 * (size_t)i + c] = expf(log_scale[3 * (size_t)i + c]);
-    const float4 q = rot_raw[i];
-    const float n = fmaxf(sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w), 1e-12f);
-    rot[i] = make_float4(q.x / n, q.y / n, q.z / n, q.w / n);
+    for (int c = 0; c < 3; ++c) scale[3 * (size_t)i + c] = scale_activation(log_scale[3 * (size_t)i + c]);
+    rot[i] = rotation_activation(rot_raw[i]);
 }
 
 // dL/d(activated) -> dL/d(raw), in place: sigmoid' = s(1-s); exp' = exp; normalize: (g - q (q.g)) / |r| (|r| > eps)
@@ -93,6 +91,8 @@ adam_packed_kernel(float* __restrict__ param, const float* __restrict__ grad, fl
 // (warp-cooperative): all six groups of the warp's visible rows stream through once with coalesced accesses, the geometric
 // gradients (already summed over the rank's views and mean-reduced over the ranks) read from the arena-shaped gradient block,
 // dc / sh-rest from the slab.
+// Densification (g_dens set): lane = Gaussian, every row visible in some slot adds dens_scale times the batch's statistics
+// (norm sum, view count; dens_scale = world undoes the exchange's mean) to its running sums.  A set skip flag leaves them.
 struct ArenaLayout {
     size_t off[6];       // float offset of each group in the arena: rotation, xyz, log-scale, opacity, dc, sh-rest
     float lr[6];
@@ -112,7 +112,8 @@ __global__ void __launch_bounds__(ADAM_WARPS * 32)
 adam_compact_kernel(uint32_t P, int D, int M, float* __restrict__ params, float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
                     const float* __restrict__ g_geo /* arena-shaped: rotation | xyz | log-scale | opacity */, ArenaLayout L,
                     ArenaLayout Lg, ViewSlots vs, float grad_scale, float color_scale, float b1, float b2, float eps,
-                    const unsigned int* __restrict__ skip_flag, unsigned int* __restrict__ visible_count) {
+                    const unsigned int* __restrict__ skip_flag, unsigned int* __restrict__ visible_count,
+                    const float* __restrict__ g_dens, float* __restrict__ dens_accum, float* __restrict__ dens_denom, float dens_scale) {
     __shared__ float s_g[ADAM_WARPS][32 * (SH_ROW_MAX + 3)];      // rebuilt gradients of the warp's 32 Gaussians: dc[32][3] | sh-rest[32][K]
     __shared__ uint8_t s_row[ADAM_WARPS][32];                      // compacted list of the warp's visible rows
     if (skip_flag && *skip_flag) return;                          // binning overflow: the frame was empty, do not step (ADVICE r1)
@@ -126,6 +127,10 @@ adam_compact_kernel(uint32_t P, int D, int M, float* __restrict__ params, float*
     bool vis = false;
     if (i < P) {
         for (int v = 0; v < vs.n_slots; ++v) vis |= (vs.visible[(size_t)v * vs.stride + i] & 0x80u) != 0;
+    }
+    if (g_dens && vis) {
+        dens_accum[i] = __fadd_rn(dens_accum[i], __fmul_rn(g_dens[i], dens_scale));
+        dens_denom[i] = __fadd_rn(dens_denom[i], __fmul_rn(g_dens[vs.stride + i], dens_scale));
     }
     const unsigned any = __ballot_sync(0xffffffffu, vis);
     if (!any) return;
@@ -354,7 +359,8 @@ int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flag
 int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, float* exp_avg, float* exp_avg_sq, const float* g_geo,
                         uint32_t Pcap_geo, const float* lr6, const float* g_color, const uint8_t* flags, const float* const* campos_dev,
                         int n_slots, float grad_scale, float color_scale, float b1, float b2, float eps, const unsigned int* skip_flag,
-                        unsigned int* visible_count, cudaStream_t s) {
+                        unsigned int* visible_count, cudaStream_t s, const float* g_dens, float* dens_accum, float* dens_denom,
+                        float dens_scale) {
     if (P == 0) return GLIC_OK;
     ArenaLayout L, Lg;
     size_t off6[6];
@@ -369,7 +375,8 @@ int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, 
     const unsigned warps = (P + 31) / 32;
     StageTimer _t(GLIC_STAGE_ADAM, s);
     adam_compact_kernel<<<(warps + ADAM_WARPS - 1) / ADAM_WARPS, ADAM_WARPS * 32, 0, s>>>(
-        P, D, M, params, exp_avg, exp_avg_sq, g_geo, L, Lg, vs, grad_scale, color_scale, b1, b2, eps, skip_flag, visible_count);
+        P, D, M, params, exp_avg, exp_avg_sq, g_geo, L, Lg, vs, grad_scale, color_scale, b1, b2, eps, skip_flag, visible_count, g_dens,
+        dens_accum, dens_denom, dens_scale);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }

@@ -26,6 +26,10 @@
 // Each Gaussian forms its six terms in fp32; the CTA adds them in float64 in a fixed order (warp shuffles, then the four
 // warps in order) and writes one partial per CTA; partials_finish_kernel adds the partials in a fixed order.  No atomics:
 // two runs give the same bits.
+//
+// DENS (only with COMPACT; glic_mapper_enable_densification): the same pass writes (or, for the later views of a rank, adds)
+// the view's densification statistics of each row: |(dL/dmean2D.x, dL/dmean2D.y)| and 1 when it is visible, 0 and 0 when it is
+// culled.  One thread owns a row, so there are no atomics.
 #include "geom_math.cuh"
 #include "sh_math.cuh"
 #include "warp_rows.cuh"
@@ -34,7 +38,7 @@ namespace glic {
 
 constexpr int PB_THREADS = 128;
 
-template <bool COMPACT, bool POSE = false>
+template <bool COMPACT, bool POSE = false, bool DENS = false>
 __global__ void __launch_bounds__(PB_THREADS)
 preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means, const float* __restrict__ scales,
                            float mod, const float4* __restrict__ rots, const float* __restrict__ sh, ViewParams vp,
@@ -46,6 +50,7 @@ preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means,
     __shared__ float s_view[16], s_proj[16], s_cam[3];
     __shared__ __align__(16) float s_sh[PB_THREADS / 32][32 * SH_ROW_MAX];    // SH rows in, dL/dSH rows out
     static_assert(COMPACT || !POSE, "the pose gradient is a compact-form output");
+    static_assert(COMPACT || !DENS, "the densification statistics are a compact-form output");
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (tid < 16) s_view[tid] = vp.view[tid];
     else if (tid < 32) s_proj[tid - 16] = vp.proj[tid - 16];
@@ -71,6 +76,7 @@ preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means,
                     for (int k = 0; k < 3; ++k) { cg.g_xyz[3 * idx + k] = 0.f; cg.g_scale[3 * idx + k] = 0.f; }
                     cg.g_rot[idx] = make_float4(0.f, 0.f, 0.f, 0.f);
                     cg.g_opacity[idx] = 0.f;
+                    if constexpr (DENS) { cg.dens_norm[idx] = 0.f; cg.dens_count[idx] = 0.f; }
                 }
             } else {
 #pragma unroll
@@ -314,6 +320,12 @@ preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means,
             cg.g_rot[idx] = g_r;
             cg.g_opacity[idx] = g_o;
         }
+        if constexpr (DENS) {
+            const float g2x = dL_dmean2D[3 * idx], g2y = dL_dmean2D[3 * idx + 1];
+            const float nrm = sqrtf(g2x * g2x + g2y * g2y);
+            if (cg.accumulate) { cg.dens_norm[idx] += nrm; cg.dens_count[idx] += 1.0f; }
+            else { cg.dens_norm[idx] = nrm; cg.dens_count[idx] = 1.0f; }
+        }
     }
     }   // visible
     if (!COMPACT && staged) warp_store_rows(dL_dsh, (size_t)wfirst, wcnt, K, slab, lane);
@@ -353,13 +365,13 @@ int launch_preprocess_backward(int P, int D, int M, const float* means, const fl
     return GLIC_OK;
 }
 
-int launch_preprocess_backward_compact(int P, int D, int M, const float* means, const float* scales, float mod,
-                                       const float* rots, const float* sh, const ViewParams& vp, const int* radii, GeomState g,
-                                       const float* dL_dmean2D, const float* dL_dconic, const float* dL_dcolors,
-                                       const CompactGrads& cg, cudaStream_t s) {
+template <bool DENS>
+static int launch_compact(int P, int D, int M, const float* means, const float* scales, float mod, const float* rots, const float* sh,
+                   const ViewParams& vp, const int* radii, GeomState g, const float* dL_dmean2D, const float* dL_dconic,
+                   const float* dL_dcolors, const CompactGrads& cg, cudaStream_t s) {
     const unsigned blocks = (P + PB_THREADS - 1) / PB_THREADS;
     if (cg.pose_partials) {
-        preprocess_backward_kernel<true, true><<<blocks, PB_THREADS, 0, s>>>(
+        preprocess_backward_kernel<true, true, DENS><<<blocks, PB_THREADS, 0, s>>>(
             P, D, M, means, scales, mod, reinterpret_cast<const float4*>(rots), sh, vp, radii, g.clamped, 0.0f,
             dL_dmean2D, dL_dconic, dL_dcolors, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cg);
         GLIC_LAUNCH_CHECK();
@@ -367,11 +379,19 @@ int launch_preprocess_backward_compact(int P, int D, int M, const float* means, 
         GLIC_LAUNCH_CHECK();
         return GLIC_OK;
     }
-    preprocess_backward_kernel<true><<<(P + PB_THREADS - 1) / PB_THREADS, PB_THREADS, 0, s>>>(
+    preprocess_backward_kernel<true, false, DENS><<<(P + PB_THREADS - 1) / PB_THREADS, PB_THREADS, 0, s>>>(
         P, D, M, means, scales, mod, reinterpret_cast<const float4*>(rots), sh, vp, radii, g.clamped, 0.0f,
         dL_dmean2D, dL_dconic, dL_dcolors, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cg);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
+}
+
+int launch_preprocess_backward_compact(int P, int D, int M, const float* means, const float* scales, float mod,
+                                       const float* rots, const float* sh, const ViewParams& vp, const int* radii, GeomState g,
+                                       const float* dL_dmean2D, const float* dL_dconic, const float* dL_dcolors,
+                                       const CompactGrads& cg, cudaStream_t s) {
+    return cg.dens_norm ? launch_compact<true>(P, D, M, means, scales, mod, rots, sh, vp, radii, g, dL_dmean2D, dL_dconic, dL_dcolors, cg, s)
+                        : launch_compact<false>(P, D, M, means, scales, mod, rots, sh, vp, radii, g, dL_dmean2D, dL_dconic, dL_dcolors, cg, s);
 }
 
 size_t pose_partials_count(uint32_t Pcap) { return 6 * (size_t)((Pcap + PB_THREADS - 1) / PB_THREADS); }

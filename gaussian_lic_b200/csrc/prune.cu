@@ -11,6 +11,17 @@
 //      group offsets are multiples of Pcap floats, Pcap a multiple of 256); its four source floats are consecutive whenever
 //      their rows are, so loads coalesce across a run of kept rows.
 // The keep decision is opacity_activation(logit) >= min_opacity, the activation kernel's own expression (common.cuh).
+//
+// Densification (glic_mapper_densify) is a three-way version of the same compaction.  Each row is kept, cloned (kept and
+// copied once) or split (replaced by two children):
+//   1. densify_count_kernel: per tile, the clones and the splits;
+//   2. prune_scan_kernel, once per count: tile offsets and the two totals;
+//   3. densify_index_kernel: idx[new] = old for the kept rows (rows that are not split, in order), then the clones, then the
+//      first child of every split row, then the second; the children's rows start as copies of their parent;
+//   4. prune_gather_kernel per arena (the moments take only the kept rows; every new row gets zero moments);
+//   5. densify_children_kernel: each child row, a copy of its parent, gets its own xyz and the parent's log-scale - log(1.6).
+// The decisions use the activation kernel's expf (scale_activation) and the child geometry its normalisation
+// (rotation_activation); glic_densify_split evaluates the same child geometry on its own.
 #include "common.cuh"
 
 namespace glic {
@@ -198,9 +209,17 @@ int launch_prune_select(uint32_t P, uint32_t n_sky, const float* opacity_logit, 
     return GLIC_OK;
 }
 
+const uint32_t* prune_index(const void* scratch, uint32_t P) {
+    const uint32_t tiles = (P + PRUNE_TILE - 1) / PRUNE_TILE;
+    return reinterpret_cast<const uint32_t*>(static_cast<const char*>(scratch) + 256 + (((size_t)tiles * 4 + 255) & ~size_t(255)));
+}
+
 int launch_prune_gather(const float* src, float* dst, uint32_t Pcap, int M, uint32_t P_old, uint32_t P_new, const void* scratch, cudaStream_t s) {
-    const uint32_t tiles = (P_old + PRUNE_TILE - 1) / PRUNE_TILE;
-    const uint32_t* idx = reinterpret_cast<const uint32_t*>(static_cast<const char*>(scratch) + 256 + (((size_t)tiles * 4 + 255) & ~size_t(255)));
+    return launch_gather_rows(src, dst, Pcap, M, P_old, P_new, prune_index(scratch, P_old), s);
+}
+
+int launch_gather_rows(const float* src, float* dst, uint32_t Pcap, int M, uint32_t P_old, uint32_t P_new, const uint32_t* idx,
+                       cudaStream_t s) {
     GatherPlan g;
     glic_packed_offsets(Pcap, (uint32_t)M, g.off);
     const int k[6] = {4, 3, 3, 1, 3, 3 * M};
@@ -215,4 +234,235 @@ int launch_prune_gather(const float* src, float* dst, uint32_t Pcap, int M, uint
     return GLIC_OK;
 }
 
+// ---- densification ---------------------------------------------------------------------------------------------------
+namespace {
+
+constexpr float SPLIT_LOG_SCALE = 0x1.e148a2p-2f;              // (float)log(1.6): log(exp(ls) / (0.8 * 2)) = ls - log(1.6)
+
+// 0 keep, 1 clone, 2 split (glic_mapper_densify): sky rows are kept; grad = accum / denom (0 without a view);
+// selected iff grad >= threshold; a selected row is cloned iff its largest activated scale is <= clone_max_scale
+__device__ __forceinline__ int densify_class(uint32_t r, uint32_t n_sky, const float* __restrict__ accum, const float* __restrict__ denom,
+                                             const float* __restrict__ log_scale, float thr, float clone_max) {
+    if (r < n_sky) return 0;
+    const float d = denom[r];
+    const float grad = d > 0.0f ? __fdiv_rn(accum[r], d) : 0.0f;
+    if (!(grad >= thr)) return 0;
+    const float* ls = log_scale + 3 * (size_t)r;
+    const float smax = fmaxf(fmaxf(scale_activation(ls[0]), scale_activation(ls[1])), scale_activation(ls[2]));
+    return smax <= clone_max ? 1 : 2;
+}
+
+__global__ void __launch_bounds__(PRUNE_THREADS)
+densify_count_kernel(uint32_t P, uint32_t n_sky, const float* __restrict__ accum, const float* __restrict__ denom,
+                     const float* __restrict__ log_scale, float thr, float clone_max, uint32_t* __restrict__ tile_clone,
+                     uint32_t* __restrict__ tile_split) {
+    const uint32_t r0 = blockIdx.x * PRUNE_TILE + PRUNE_ROWS * threadIdx.x;
+    uint32_t n = 0;                                            // clones | splits << 16 (at most PRUNE_TILE each)
+#pragma unroll
+    for (int e = 0; e < PRUNE_ROWS; ++e) {
+        if (r0 + e >= P) break;
+        const int c = densify_class(r0 + e, n_sky, accum, denom, log_scale, thr, clone_max);
+        n += c == 1 ? 1u : c == 2 ? (1u << 16) : 0u;
+    }
+    __shared__ uint32_t warp_n[PRUNE_THREADS / 32];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+    if ((threadIdx.x & 31) == 0) warp_n[threadIdx.x >> 5] = n;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t t = 0;
+        for (int w = 0; w < PRUNE_THREADS / 32; ++w) t += warp_n[w];
+        tile_clone[blockIdx.x] = t & 0xFFFFu;
+        tile_split[blockIdx.x] = t >> 16;
+    }
+}
+
+// totals[2] = {clones, splits} (the scans' totals); places every result row's source row in idx
+__global__ void __launch_bounds__(PRUNE_THREADS)
+densify_index_kernel(uint32_t P, uint32_t n_sky, const float* __restrict__ accum, const float* __restrict__ denom,
+                     const float* __restrict__ log_scale, float thr, float clone_max, const uint32_t* __restrict__ clone_offset,
+                     const uint32_t* __restrict__ split_offset, const uint32_t* __restrict__ totals, uint32_t* __restrict__ idx) {
+    const uint32_t r0 = blockIdx.x * PRUNE_TILE + PRUNE_ROWS * threadIdx.x;
+    int cls[PRUNE_ROWS];
+    uint32_t n = 0;
+#pragma unroll
+    for (int e = 0; e < PRUNE_ROWS; ++e) {
+        cls[e] = r0 + e < P ? densify_class(r0 + e, n_sky, accum, denom, log_scale, thr, clone_max) : -1;
+        n += cls[e] == 1 ? 1u : cls[e] == 2 ? (1u << 16) : 0u;
+    }
+    // exclusive scan of the packed counts over the CTA, in thread (= row) order
+    __shared__ uint32_t warp_tot[PRUNE_THREADS / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t incl = n;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+    }
+    if (lane == 31) warp_tot[warp] = incl;
+    __syncthreads();
+    uint32_t before = 0;
+    for (int w = 0; w < warp; ++w) before += warp_tot[w];
+    const uint32_t excl = before + incl - n;
+    uint32_t clones = clone_offset[blockIdx.x] + (excl & 0xFFFFu), splits = split_offset[blockIdx.x] + (excl >> 16);
+    const uint32_t n_clone = totals[0], n_split = totals[1];
+    const uint32_t kept = P - n_split, first_child = kept + n_clone;
+#pragma unroll
+    for (int e = 0; e < PRUNE_ROWS; ++e) {
+        const uint32_t r = r0 + e;
+        if (cls[e] < 0) break;
+        if (cls[e] == 2) {
+            idx[first_child + splits] = r;
+            idx[first_child + n_split + splits] = r;
+            ++splits;
+        } else {
+            idx[r - splits] = r;
+            if (cls[e] == 1) idx[kept + clones++] = r;
+        }
+    }
+}
+
+// child `row` of densify call `call`, axis a: the uniforms of the skybox's generator at counter
+// k = ((call + 1) * 2^32 + row) * 3 + a, then Box-Muller
+__device__ __forceinline__ float split_normal(uint64_t seed, uint64_t call, uint32_t row, int a) {
+    const uint64_t k = (((call + 1) << 32) + row) * 3 + (uint64_t)a;
+    const uint64_t r = splitmix64_mix(seed + (k + 1) * 0x9E3779B97F4A7C15ull);
+    const float u1 = __fmul_rn((float)(uint32_t)(r >> 40), 5.9604644775390625e-08f);               // * 2^-24: exact
+    const float u2 = __fmul_rn((float)(uint32_t)((r >> 16) & 0xFFFFFFu), 5.9604644775390625e-08f);
+    const float rad = sqrtf(__fmul_rn(-2.0f, logf(__fsub_rn(1.0f, u1))));
+    return __fmul_rn(rad, cospif(__fmul_rn(2.0f, u2)));
+}
+
+// xyz of a split child: p + R(q) (s * z), R = build_rotation of the normalised q = (r, x, y, z), every operation rounded once
+__device__ __forceinline__ void split_child(const float p[3], const float s[3], float4 q, const float z[3], float out[3]) {
+    const float r = q.x, x = q.y, y = q.z, w = q.w;
+    const float R[9] = {
+        __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(y, y), __fmul_rn(w, w)))),
+        __fmul_rn(2.0f, __fsub_rn(__fmul_rn(x, y), __fmul_rn(r, w))),
+        __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, w), __fmul_rn(r, y))),
+        __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, y), __fmul_rn(r, w))),
+        __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, x), __fmul_rn(w, w)))),
+        __fmul_rn(2.0f, __fsub_rn(__fmul_rn(y, w), __fmul_rn(r, x))),
+        __fmul_rn(2.0f, __fsub_rn(__fmul_rn(x, w), __fmul_rn(r, y))),
+        __fmul_rn(2.0f, __fadd_rn(__fmul_rn(y, w), __fmul_rn(r, x))),
+        __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y))))};
+    const float v[3] = {__fmul_rn(s[0], z[0]), __fmul_rn(s[1], z[1]), __fmul_rn(s[2], z[2])};
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+        out[i] = __fadd_rn(p[i], __fadd_rn(__fadd_rn(__fmul_rn(R[3 * i], v[0]), __fmul_rn(R[3 * i + 1], v[1])), __fmul_rn(R[3 * i + 2], v[2])));
+}
+
+// rows [first, first + n) of the arena (copies of their parents) become the split children: xyz and log-scale
+__global__ void __launch_bounds__(256)
+densify_children_kernel(float* __restrict__ params, size_t off_rot, size_t off_xyz, size_t off_ls, uint32_t first, uint32_t n, uint64_t seed,
+                        uint64_t call) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const uint32_t row = first + t;
+    float* xyz = params + off_xyz + 3 * (size_t)row;
+    float* ls = params + off_ls + 3 * (size_t)row;
+    const float4 q = rotation_activation(reinterpret_cast<const float4*>(params + off_rot)[row]);
+    float p[3], s[3], z[3], out[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        p[a] = xyz[a];
+        s[a] = scale_activation(ls[a]);
+        z[a] = split_normal(seed, call, row, a);
+    }
+    split_child(p, s, q, z, out);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        xyz[a] = out[a];
+        ls[a] = __fsub_rn(ls[a], SPLIT_LOG_SCALE);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+densify_split_kernel(int n, const float* __restrict__ xyz, const float* __restrict__ scale, const float4* __restrict__ rot, uint64_t seed,
+                     uint64_t call, uint32_t first_row, float* __restrict__ xyz_out, float* __restrict__ z_out) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    float p[3], s[3], z[3], out[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        p[a] = xyz[3 * (size_t)t + a];
+        s[a] = scale[3 * (size_t)t + a];
+        z[a] = split_normal(seed, call, first_row + (uint32_t)t, a);
+    }
+    split_child(p, s, rot[t], z, out);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        xyz_out[3 * (size_t)t + a] = out[a];
+        if (z_out) z_out[3 * (size_t)t + a] = z[a];
+    }
+}
+
+__global__ void __launch_bounds__(256)
+gather_floats_kernel(const float* __restrict__ src, float* __restrict__ dst, uint32_t rows_out, uint32_t rows_valid,
+                     const uint32_t* __restrict__ idx) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < rows_out) dst[r] = r < rows_valid ? src[idx[r]] : 0.0f;
+}
+
+// scratch: totals[2] (256 bytes) | clone tile counts | split tile counts | idx[2P]
+size_t tile_bytes(uint32_t P) { return (((size_t)(P + PRUNE_TILE - 1) / PRUNE_TILE) * 4 + 255) & ~size_t(255); }
+
+}  // namespace
+
+size_t densify_scratch_bytes(uint32_t P) { return 256 + 2 * tile_bytes(P) + (size_t)P * 8; }
+
+const uint32_t* densify_index(const void* scratch, uint32_t P) {
+    return reinterpret_cast<const uint32_t*>(static_cast<const char*>(scratch) + 256 + 2 * tile_bytes(P));
+}
+
+int launch_densify_select(uint32_t P, uint32_t n_sky, const float* accum, const float* denom, const float* log_scale, float grad_threshold,
+                          float clone_max_scale, void* scratch, uint32_t* result_host, cudaStream_t s) {
+    const uint32_t tiles = (P + PRUNE_TILE - 1) / PRUNE_TILE;
+    char* base = static_cast<char*>(scratch);
+    uint32_t* totals = reinterpret_cast<uint32_t*>(base);
+    uint32_t* tile_clone = reinterpret_cast<uint32_t*>(base + 256);
+    uint32_t* tile_split = reinterpret_cast<uint32_t*>(base + 256 + tile_bytes(P));
+    uint32_t* idx = const_cast<uint32_t*>(densify_index(scratch, P));
+    densify_count_kernel<<<tiles, PRUNE_THREADS, 0, s>>>(P, n_sky, accum, denom, log_scale, grad_threshold, clone_max_scale, tile_clone, tile_split);
+    GLIC_LAUNCH_CHECK();
+    prune_scan_kernel<<<1, 1024, 0, s>>>(tiles, tile_clone, totals);
+    GLIC_LAUNCH_CHECK();
+    prune_scan_kernel<<<1, 1024, 0, s>>>(tiles, tile_split, totals + 1);
+    GLIC_LAUNCH_CHECK();
+    densify_index_kernel<<<tiles, PRUNE_THREADS, 0, s>>>(P, n_sky, accum, denom, log_scale, grad_threshold, clone_max_scale, tile_clone,
+                                                         tile_split, totals, idx);
+    GLIC_LAUNCH_CHECK();
+    GLIC_CUDA_TRY(cudaMemcpyAsync(result_host, totals, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    return GLIC_OK;
+}
+
+int launch_densify_children(float* params, uint32_t Pcap, int M, uint32_t first, uint32_t n, uint64_t seed, uint64_t call, cudaStream_t s) {
+    if (n == 0) return GLIC_OK;
+    size_t off[6];
+    glic_packed_offsets(Pcap, (uint32_t)M, off);
+    densify_children_kernel<<<(n + 255) / 256, 256, 0, s>>>(params, off[0], off[1], off[2], first, n, seed, call);
+    GLIC_LAUNCH_CHECK();
+    return GLIC_OK;
+}
+
+int launch_gather_floats(const float* src, float* dst, uint32_t rows_out, uint32_t rows_valid, const uint32_t* idx, cudaStream_t s) {
+    if (rows_out == 0) return GLIC_OK;
+    gather_floats_kernel<<<(rows_out + 255) / 256, 256, 0, s>>>(src, dst, rows_out, rows_valid, idx);
+    GLIC_LAUNCH_CHECK();
+    return GLIC_OK;
+}
+
 }  // namespace glic
+
+extern "C" int glic_densify_split(int n, const float* xyz, const float* scale, const float* rot, uint64_t seed, uint64_t call,
+                                  uint32_t first_row, float* xyz_out, float* z_out, void* stream) {
+    if (n < 0) { glic::set_error("densify_split: n must be >= 0"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (n == 0) return GLIC_OK;
+    if (!xyz || !scale || !rot || !xyz_out) { glic::set_error("densify_split: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if ((reinterpret_cast<uintptr_t>(rot) & 15u) != 0) { glic::set_error("densify_split: rot must be 16-byte aligned"); return GLIC_ERR_INVALID_ARGUMENT; }
+    glic::densify_split_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(n, xyz, scale, reinterpret_cast<const float4*>(rot), seed,
+                                                                                  call, first_row, xyz_out, z_out);
+    GLIC_LAUNCH_CHECK();
+    return GLIC_OK;
+}

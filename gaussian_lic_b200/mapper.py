@@ -13,6 +13,8 @@ from . import capi
 FASTLIVO = dict(position_lr=1.6e-4, feature_lr=2.5e-3, opacity_lr=0.05, scaling_lr=0.005, rotation_lr=0.001,
                 lambda_dssim=0.2, scaling_scale=1.0)                  # config/fastlivo.yaml:15-24
 DEAD_OPACITY = float(np.float32(1.0) / np.float32(255.0))             # GLIC_MAPPER_DEAD_OPACITY: the preprocess's o < 1/255 cull
+DENSIFY_GRAD_THRESHOLD = float(np.float32(0.0002))                   # GLIC_MAPPER_DENSIFY_GRAD_THRESHOLD (Inria's default)
+PERCENT_DENSE = float(np.float32(0.01))                              # GLIC_MAPPER_PERCENT_DENSE
 
 
 def _f32(a):
@@ -262,6 +264,27 @@ class Mapper:
         out = C.c_uint32()
         capi.check(capi.lib.glic_mapper_prune(self._h, float(min_opacity), int(bool(dry_run)), C.byref(out)), "mapper_prune")
         return int(out.value)
+
+    def enable_densification(self):
+        """Gather the view-space gradient statistics densify() selects on, from the next iteration on (world > 1: before
+        export_handle())."""
+        capi.check(capi.lib.glic_mapper_enable_densification(self._h), "mapper_enable_densification")
+
+    def densify(self, scene_extent, grad_threshold=DENSIFY_GRAD_THRESHOLD, percent_dense=PERCENT_DENSE, dry_run=False):
+        """Clone the selected small rows and split the selected large ones into two children (Inria's densify_and_clone /
+        densify_and_split); the statistics start again.  dry_run only counts.  Returns (cloned, split)."""
+        c, s = C.c_uint32(), C.c_uint32()
+        capi.check(capi.lib.glic_mapper_densify(self._h, float(grad_threshold), float(percent_dense), float(scene_extent),
+                                                int(bool(dry_run)), C.byref(c), C.byref(s)), "mapper_densify")
+        return int(c.value), int(s.value)
+
+    def densify_stats(self):
+        """(accum [P], denom [P]) float32: the summed view-space gradient norms and the number of views that saw each row."""
+        P = int(self.stats().num_gaussians)
+        acc, den = np.zeros(P, np.float32), np.zeros(P, np.float32)
+        capi.check(capi.lib.glic_mapper_densify_stats(self._h, _p(acc) if P else acc.ctypes.data_as(C.c_void_p),
+                                                      _p(den) if P else den.ctypes.data_as(C.c_void_p)), "mapper_densify_stats")
+        return acc, den
 
     # ---- multi-GPU wiring: torch.distributed (or anything else) only carries the 64-byte handles --------------------------
     def export_handle(self):

@@ -517,6 +517,62 @@ GLIC_API int glic_mapper_download(glic_mapper* m, float* xyz, float* f_dc, float
  *   the same rows and stay identical without any exchange. */
 #define GLIC_MAPPER_DEAD_OPACITY (1.0f / 255.0f)
 GLIC_API int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, uint32_t* removed);
+/* Densification: Inria 3DGS's densify_and_clone + densify_and_split (N = 2) driven by view-space gradients (no counterpart in
+ * the reference, whose densificationPostfix is only the concatenation extend() uses).  Off by default; with it never enabled an
+ * iteration enqueues the same work as before.
+ *   glic_mapper_enable_densification(m): from now on every row i keeps two floats, accum_i and denom_i, starting at 0.  In every
+ *   iteration that steps the Gaussians, for every view v of the batch (all world * views_per_rank of them) with radii_v,i > 0:
+ *       accum_i += |(g.x, g.y)|,   denom_i += 1,
+ *   g = that view's own dL_v/dmean2D (NDC-scaled, what glic_backward returns as dL_dmeans2D; not divided by the batch size, so
+ *   the threshold does not depend on world * views_per_rank).  The per-view values are summed over a rank's views inside the
+ *   per-Gaussian backward and committed by the Adam launch; an iteration skipped for a binning overflow leaves them unchanged,
+ *   and so does GLIC_MAPPER_OPT_OPTIMIZER = 0.  extend() appends rows with zero statistics, a capacity growth keeps them,
+ *   glic_mapper_prune moves them with their rows bit for bit, initialize / initialize_lidar zero them.  A second call does
+ *   nothing.  With world > 1 it must come before glic_mapper_export (GLIC_ERR_INVALID_ARGUMENT otherwise; the exchange block
+ *   gains two rows of Pcap floats, which the reduce carries: the committed statistics are world times the mean over the ranks,
+ *   exactly the sums over all views when world is a power of two).
+ *   glic_mapper_densify_stats(m, accum, denom): the P statistics of each kind to host arrays; synchronises.
+ *   glic_mapper_densify(m, grad_threshold, percent_dense, scene_extent, dry_run, &cloned, &split) (the counts may be NULL):
+ *   - candidates are the non-sky rows [S, P) (sky rows are never densified, so the sky prefix and save_map stay valid);
+ *     grad_i = denom_i > 0 ? accum_i / denom_i : 0 (one IEEE division), selected iff grad_i >= grad_threshold;
+ *     smax_i = the largest of the row's three activated scales (expf, the activation kernel's), cloned iff
+ *     smax_i <= percent_dense * scene_extent (the product in float), split otherwise;
+ *   - the result rows, in Inria's order: every row that is not split, in its order; the clones, in index order; the first child
+ *     of every split row in index order; then the second child of every split row.  Kept rows keep their parameters and both Adam
+ *     moments bit for bit; clones are bit-identical copies of their parent's six groups; children copy rotation, f_dc, f_rest
+ *     and opacity, take log_scale = __fsub_rn(ls, (float)log(1.6)) (Inria's log(exp(ls) / (0.8 * 2)) up to rounding), and
+ *     xyz = glic_densify_split of the parent's xyz, activated scale s and normalised rotation q (the activation kernel's) at
+ *     key (cfg.seed, call, row), row = the child's result row, call = the number of earlier real densify calls of this mapper;
+ *     every new row has zero moments; sky rows, n_sky, keyframes, exposure and pose state are untouched;
+ *   - a real call (dry_run == 0) then zeroes every row's statistics (densification_postfix) and advances `call`; a dry run only
+ *     counts, changes nothing and does not advance `call`;
+ *   - capacity: a result that does not fit grows the arenas like extend() (to max(rows, 2 * capacity)); with world > 1 and the
+ *     mapper connected it returns GLIC_ERR_WORKSPACE and changes nothing (the dry-run counts let the host prune first);
+ *   - densification not enabled, a NULL mapper, a non-finite or negative grad_threshold or percent_dense, or a scene_extent
+ *     that is not finite and > 0 return GLIC_ERR_INVALID_ARGUMENT and change nothing.  Allocation failures follow the failure
+ *     contract above.  The call drains the iteration pipeline (as prune does) and synchronises.  It needs one spare arena of the
+ *     capacity while it runs, and its selection scratch (8 B per row) lives in the extend() staging buffer.
+ *   - world > 1: every rank makes the same calls between the same optimize() calls; replicas stay bit-identical in parameters,
+ *     moments and statistics with no exchange.
+ * glic_densify_split(n, xyz, scale, rot, seed, call, first_row, xyz_out, z_out, stream): the children's geometry on its own, for
+ *   n children (device arrays; child t has parent xyz[t], activated scale[t], normalised rot[t] = (r, x, y, z), 16-byte aligned,
+ *   and result row first_row + t).  Per axis a the standard normal z_a comes from the skybox's counter-based generator
+ *   (glic_skybox_init) at counter k = ((call + 1) * 2^32 + row) * 3 + a (mod 2^64): r = mix64(seed + (k + 1) * 0x9E3779B97F4A7C15),
+ *   u1 = (r >> 40) * 2^-24, u2 = ((r >> 16) & 0xFFFFFF) * 2^-24, then Box-Muller
+ *       z_a = __fmul_rn(sqrtf(__fmul_rn(-2, logf(__fsub_rn(1, u1)))), cospif(__fmul_rn(2, u2))).
+ *   With v_a = __fmul_rn(s_a, z_a) and R = Inria's build_rotation(q), each entry one of
+ *       1 - 2 (y y + z z), 2 (x y - r z), 2 (x z + r y) / 2 (x y + r z), 1 - 2 (x x + z z), 2 (y z - r x) /
+ *       2 (x z - r y), 2 (y z + r x), 1 - 2 (x x + y y)
+ *   with every product, sum and difference rounded once (_rn), xyz_out_i = p_i + ((R_i0 v_0 + R_i1 v_1) + R_i2 v_2), rounded
+ *   in that order.  z_out (optional, [n][3]) receives the normals.  No host synchronisation. */
+#define GLIC_MAPPER_DENSIFY_GRAD_THRESHOLD 0.0002f   /* Inria's densify_grad_threshold */
+#define GLIC_MAPPER_PERCENT_DENSE 0.01f
+GLIC_API int glic_mapper_enable_densification(glic_mapper* m);
+GLIC_API int glic_mapper_densify(glic_mapper* m, float grad_threshold, float percent_dense, float scene_extent, int dry_run,
+                                 uint32_t* cloned, uint32_t* split);
+GLIC_API int glic_mapper_densify_stats(glic_mapper* m, float* grad_accum, float* denom);
+GLIC_API int glic_densify_split(int n, const float* xyz, const float* scale, const float* rot, uint64_t seed, uint64_t call,
+                                uint32_t first_row, float* xyz_out, float* z_out, void* stream);
 /* multi-GPU wiring: every rank exports the 64-byte IPC handle of its exchange block, the caller all-gathers them
  * (torch.distributed / MPI / a file: plumbing) and hands all `world` handles back. */
 GLIC_API int glic_mapper_export(glic_mapper* m, unsigned char* handle64);
