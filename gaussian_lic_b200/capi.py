@@ -51,6 +51,22 @@ class MapperStats(C.Structure):
                 ("ms_optimize", C.c_float)]
 
 
+class DensityParams(C.Structure):
+    _fields_ = [("grad_threshold", C.c_float), ("percent_dense", C.c_float), ("scene_extent", C.c_float), ("min_opacity", C.c_float),
+                ("max_screen_radius", C.c_int32), ("max_world_scale", C.c_float)]
+
+
+class DensityCounts(C.Structure):
+    _fields_ = [("cloned", C.c_uint32), ("split", C.c_uint32), ("pruned", C.c_uint32), ("rows", C.c_uint32)]
+
+
+class DensitySchedule(C.Structure):
+    _fields_ = [("densify_from", C.c_uint32), ("densify_until", C.c_uint32), ("densify_interval", C.c_uint32),
+                ("opacity_reset_interval", C.c_uint32), ("grad_threshold", C.c_float), ("percent_dense", C.c_float),
+                ("min_opacity", C.c_float), ("reset_opacity", C.c_float), ("screen_radius", C.c_int32),
+                ("world_scale_factor", C.c_float), ("scene_extent", C.c_float)]
+
+
 def _load():
     if not os.path.isfile(LIB_PATH):
         raise ImportError(
@@ -146,6 +162,12 @@ def _load():
         "glic_mapper_densify": (i32, [vp, f32, f32, f32, i32, C.POINTER(u32), C.POINTER(u32)]),
         "glic_mapper_densify_stats": (i32, [vp, vp, vp]),
         "glic_densify_split": (i32, [i32, vp, vp, vp, C.c_uint64, C.c_uint64, u32, vp, vp, vp]),
+        "glic_mapper_screen_radii": (i32, [vp, vp]),
+        "glic_mapper_reset_opacity": (i32, [vp, f32]),
+        "glic_mapper_densify_and_prune": (i32, [vp, C.POINTER(DensityParams), i32, C.POINTER(DensityCounts)]),
+        "glic_mapper_set_density_schedule": (i32, [vp, C.POINTER(DensitySchedule)]),
+        "glic_mapper_scene_extent": (i32, [vp, C.POINTER(f32)]),
+        "glic_mapper_density_totals": (i32, [vp, C.POINTER(DensityCounts), C.POINTER(u32), C.POINTER(u32)]),
         "glic_mapper_export": (i32, [vp, C.c_char_p]),
         "glic_mapper_connect": (i32, [vp, C.c_char_p]),
         "glic_mapper_synchronize": (i32, [vp]),

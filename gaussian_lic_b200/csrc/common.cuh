@@ -367,11 +367,13 @@ int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, 
                         uint32_t Pcap_geo, const float* lr6, const float* g_color, const uint8_t* flags, const float* const* campos_dev,
                         int n_slots, float grad_scale, float color_scale, float b1, float b2, float eps, const unsigned int* skip_flag,
                         unsigned int* visible_count, cudaStream_t s, const float* g_dens = nullptr, float* dens_accum = nullptr,
-                        float* dens_denom = nullptr, float dens_scale = 1.0f);
+                        float* dens_denom = nullptr, float dens_scale = 1.0f, const int* radii = nullptr, int* dens_maxr = nullptr);
 // g_dens (optional): the densification statistics of the batch in the gradient block, norms [Pcap_geo] | counts [Pcap_geo]; the
-// Adam launch adds dens_scale times them to dens_accum / dens_denom for every row visible in some slot, unless skip_flag is set
+// Adam launch adds dens_scale times them to dens_accum / dens_denom for every row visible in some slot, unless skip_flag is set.
+// radii (with g_dens): [n_slots][Pcap_geo] each slot's screen radii; dens_maxr takes their max over the slots that see the row
 // campos_dev: n_slots host-held device pointers, each slot's camera centre (read on the device)
-int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flags, cudaStream_t s);
+// radii_out (optional): the view's radii copied next to its flags (the densification's screen-radius slot)
+int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flags, cudaStream_t s, int* radii_out = nullptr);
 // per-keyframe exposure (ssim.cu): one Adam step of every keyframe of a batch of S <= EXPO_MAX_SLOTS slots; slot_grads[S][12]
 constexpr int EXPO_MAX_SLOTS = 32;
 int launch_exposure_adam(int S, const int* kf_of_slot_host, const float* slot_grads, float* E, float* exp_avg, float* exp_avg_sq,
@@ -390,18 +392,30 @@ int launch_prune_select(uint32_t P, uint32_t n_sky, const float* opacity_logit, 
 int launch_prune_gather(const float* src, float* dst, uint32_t Pcap, int M, uint32_t P_old, uint32_t P_new, const void* scratch, cudaStream_t s);
 // the select's index map: idx[new] = old for the P_new kept rows
 const uint32_t* prune_index(const void* scratch, uint32_t P);
-// dst[r] = r < rows_valid ? src[idx[r]] : 0 for r < rows_out (one float per row)
-int launch_gather_floats(const float* src, float* dst, uint32_t rows_out, uint32_t rows_valid, const uint32_t* idx, cudaStream_t s);
+// dst[r] = r < rows_valid ? src[idx[r]] : 0 for r < rows_out (one 32-bit word per row)
+int launch_gather_words(const void* src, void* dst, uint32_t rows_out, uint32_t rows_valid, const uint32_t* idx, cudaStream_t s);
 // output rows [0, rows_out) of every group of dst: row r < rows_valid takes row idx[r] of src, the others are zero
 int launch_gather_rows(const float* src, float* dst, uint32_t Pcap, int M, uint32_t rows_out, uint32_t rows_valid, const uint32_t* idx,
                        cudaStream_t s);
-// densification (prune.cu, glic_mapper_densify).  select: classes of rows [0, P) (keep, clone, split; rows below n_sky are
-// kept) from the statistics and the log-scale group; result_host[2] = {clones, splits}, synchronises s; the scratch then
-// holds the index map of the result rows (densify_index).  children: rows [first, first + n) of the arena, copies of their
-// parents, become split children in place (xyz and log-scale).
-size_t densify_scratch_bytes(uint32_t P);
-int launch_densify_select(uint32_t P, uint32_t n_sky, const float* accum, const float* denom, const float* log_scale, float grad_threshold,
-                          float clone_max_scale, void* scratch, uint32_t* result_host, cudaStream_t s);
-const uint32_t* densify_index(const void* scratch, uint32_t P);
-int launch_densify_children(float* params, uint32_t Pcap, int M, uint32_t first, uint32_t n, uint64_t seed, uint64_t call, cudaStream_t s);
+// densify-and-prune (prune.cu, glic_mapper_densify_and_prune): the selection's inputs (device pointers of rows [0, P)) and
+// parameters, as the header states them
+struct DensitySelect {
+    uint32_t P, n_sky;
+    const float *accum, *denom, *log_scale, *logit;
+    const int* maxr;                 // read only when max_screen_radius > 0
+    float grad_threshold, clone_max, min_opacity, max_world_scale;
+    int max_screen_radius;
+};
+// select: the fate of every row; result_host[6] = {clones, splits, surviving kept rows, surviving clones, surviving split rows,
+// surviving sky rows}, synchronises s; the scratch then holds the index map of the surviving rows (density_index) and the
+// children's keys.  children: rows [first, first + 2 n) of the arena, copies of the n surviving split rows' parents, become
+// their children in place (xyz and log-scale); P_select is the P the selection ran on, n_split its splits.
+size_t density_scratch_bytes(uint32_t P);
+int launch_density_select(const DensitySelect& a, void* scratch, uint32_t* result_host, cudaStream_t s);
+const uint32_t* density_index(const void* scratch, uint32_t P);
+int launch_densify_children(float* params, uint32_t Pcap, int M, uint32_t first, uint32_t n, const void* scratch, uint32_t P_select,
+                            uint32_t n_split, uint64_t seed, uint64_t call, cudaStream_t s);
+// glic_mapper_reset_opacity on rows [first, P) of the opacity group of the three arenas
+int launch_reset_opacity(uint32_t first, uint32_t P, uint32_t Pcap, int M, float* params, float* m1, float* m2, float max_opacity,
+                         float reset_logit, cudaStream_t s);
 }  // namespace glic

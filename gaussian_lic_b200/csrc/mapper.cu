@@ -304,7 +304,7 @@ __global__ void __launch_bounds__(256) scan_colour_kernel(int n3, const uint8_t*
 }
 
 // Regions of the exchange block that hold one slot per (parity, view slot), in layout order
-enum SlotRegion { COLOUR, FLAGS, EXPOSURE, POSE, N_REGIONS };
+enum SlotRegion { COLOUR, FLAGS, EXPOSURE, POSE, RADII, N_REGIONS };
 
 // Adam state of a per-training-keyframe parameter of `width` floats: moments [cap][width], step counts [cap]
 struct KeyframeAdam {
@@ -392,7 +392,13 @@ struct glic_mapper {
     bool dens_on = false;
     bool exported = false;                // glic_mapper_export has run: the exchange block can no longer move
     Dev<float> dens_accum, dens_denom;
+    Dev<int> dens_maxr;                   // the largest screen radius of each row since the statistics last restarted
     uint64_t dens_calls = 0;
+    // ---- the density-control schedule of optimize() (glic_mapper_set_density_schedule) and what it has done since it was set
+    bool sched_on = false;
+    glic_density_schedule sched{};
+    glic_density_counts sched_totals{};
+    uint32_t sched_steps = 0, sched_resets = 0;
 };
 
 namespace {
@@ -442,13 +448,15 @@ T* slot(const glic_mapper* m, SlotRegion r, int parity, int s) {
 }
 
 // The slot regions follow the flags words, each [2][S] slots rounded up to 256 bytes: colour gradients [cap][3] floats, flag
-// bytes [cap], dL/dE [12] floats, dL/d(rho, omega) [8] floats (2 unused).
+// bytes [cap], dL/dE [12] floats, dL/d(rho, omega) [8] floats (2 unused), and with densification on the screen radii [cap]
+// int32 (empty otherwise).
 XLayout xblock_layout(int S, uint32_t cap, bool dens) {
     XLayout x;
     x.n_geo = (size_t)(dens ? 13 : 11) * cap + 4;
     size_t sl[6];
     glic_p2p_slice(0, 1, x.n_geo, 0, sl);
-    const size_t bytes[N_REGIONS] = {(size_t)cap * 3 * sizeof(float), cap, 12 * sizeof(float), 8 * sizeof(float)};
+    const size_t bytes[N_REGIONS] = {(size_t)cap * 3 * sizeof(float), cap, 12 * sizeof(float), 8 * sizeof(float),
+                                     dens ? (size_t)cap * sizeof(int) : 0};
     x.bytes = sl[5] + 256;
     for (int r = 0; r < N_REGIONS; ++r) {
         x.slot_off[r] = x.bytes;
@@ -488,7 +496,7 @@ int set_capacity(glic_mapper* m, uint32_t cap) {
                               {m->g_conic, (size_t)cap * (16 + 12 + 4), 0, true}, {m->geom_ws, glic_geom_bytes((int)cap), 0, true},
                               {m->xblock, x.bytes, 0, true}, {m->pose_part, pose_partials_count(cap) * sizeof(double)}};
     if (m->dens_on)                                       // the statistics keep their live rows
-        for (Buf* b : {(Buf*)&m->dens_accum, (Buf*)&m->dens_denom}) list.push_back({*b, (size_t)cap * 4, (size_t)m->P * 4, true});
+        for (Buf* b : {(Buf*)&m->dens_accum, (Buf*)&m->dens_denom, (Buf*)&m->dens_maxr}) list.push_back({*b, (size_t)cap * 4, (size_t)m->P * 4, true});
     MAP_TRY(grow(m, list, regrow));
     m->g_mean2D = m->g_conic + (size_t)cap * 4;           // conic first: float4-aligned
     m->g_opacity = m->g_mean2D + (size_t)cap * 3;
@@ -557,6 +565,7 @@ int dens_reset(glic_mapper* m) {
     if (!m->dens_on) return GLIC_OK;
     GLIC_CUDA_TRY(cudaMemsetAsync(m->dens_accum, 0, (size_t)m->Pcap * 4, m->stream));
     GLIC_CUDA_TRY(cudaMemsetAsync(m->dens_denom, 0, (size_t)m->Pcap * 4, m->stream));
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->dens_maxr, 0, (size_t)m->Pcap * 4, m->stream));
     return GLIC_OK;
 }
 
@@ -673,13 +682,15 @@ int iteration(glic_mapper* m, const int* views) {
         MAP_TRY(forward_view(m, kf, 0, j == m->k - 1 ? m->counters_host + 4 * r : nullptr));
         uint8_t* fl = slot<uint8_t>(m, FLAGS, parity, sl);
         float* col = slot(m, COLOUR, parity, sl);
-        MAP_TRY(launch_view_flags((int)m->P, m->radii, GeomState::carve(m->geom_ws, (int)m->P), fl, s));
+        int* rad = m->dens_on ? slot<int>(m, RADII, parity, sl) : nullptr;           // this view's radii for the screen-size statistic
+        MAP_TRY(launch_view_flags((int)m->P, m->radii, GeomState::carve(m->geom_ws, (int)m->P), fl, s, rad));
         overflow_word_kernel<<<1, 1, 0, s>>>(GeomState::carve(m->geom_ws, (int)m->P).hdr, geo_tail);
         GLIC_LAUNCH_CHECK();
         if (m->cfg.world > 1) {
             GLIC_CUDA_TRY(cudaEventRecord(m->ev_flags, s));
             GLIC_CUDA_TRY(cudaStreamWaitEvent(m->push_stream, m->ev_flags, 0));
             MAP_TRY(push_to_peers(m, fl, m->P));
+            if (rad) MAP_TRY(push_to_peers(m, rad, sizeof(int) * (size_t)m->P));
         }
         GLIC_CUDA_TRY(cudaStreamWaitEvent(s, m->gt_ready[buf], 0));
         // loss of this view (the pinned ring keeps the last local view's value for the statistics)
@@ -728,7 +739,8 @@ int iteration(glic_mapper* m, const int* views) {
     MAP_TRY(launch_adam_compact(m->P, m->Pcap, m->D, m->M, m->params, m->m1, m->m2, geo, m->Pcap, lr6, slot(m, COLOUR, parity, 0),
                                 slot<uint8_t>(m, FLAGS, parity, 0), campos, m->S, 1.0f / (float)m->k, color_scale, 0.9f, 0.999f, 1e-15f,
                                 reinterpret_cast<const unsigned int*>(geo_tail), m->vis_acc, s, m->dens_on ? geo_tail + 4 : nullptr,
-                                m->dens_accum, m->dens_denom, (float)m->cfg.world));
+                                m->dens_accum, m->dens_denom, (float)m->cfg.world, m->dens_on ? slot<int>(m, RADII, parity, 0) : nullptr,
+                                m->dens_maxr));
     // every replica steps the batch's exposures from the same S slot gradients, in slot order
     if (m->run_optimizer && m->expo_on)
         MAP_TRY(launch_exposure_adam(m->S, views, slot(m, EXPOSURE, parity, 0), m->expo_E, m->expo_adam.m, m->expo_adam.v, m->expo_adam.t, m->expo_lr,
@@ -944,6 +956,8 @@ int scan_handoff(glic_mapper* m, const Keyframe& kf, int n) {
     GLIC_LAUNCH_CHECK();
     return extend_core(m, kf, n, m->scan_xyz, d_col, m->scan_depth, ws);
 }
+
+int scheduled_density_step(glic_mapper* m);    // optimize()'s density control, with glic_mapper_densify_and_prune below
 
 }  // namespace
 
@@ -1221,6 +1235,7 @@ int glic_mapper_optimize(glic_mapper* m, const int* views_host, int n_views) {
     for (size_t it = 0; it < iters; ++it) {
         for (int sl = 0; sl < m->S; ++sl) batch[sl] = list[(it * m->S + sl) % list.size()];     // the last batch wraps around
         MAP_TRY(iteration(m, batch.data()));
+        if (m->sched_on && m->run_optimizer) MAP_TRY(scheduled_density_step(m));
     }
     GLIC_CUDA_TRY(cudaEventRecord(m->t1, m->stream));
     unsigned int vis = 0;
@@ -1330,7 +1345,7 @@ int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, uint32_t* 
     MAP_TRY(launch_prune_select(P, m->n_sky, g[3], min_opacity, scratch, kept, s));
     if (kept[0] == 0) { set_error("mapper_prune: the threshold removes every row (an empty map cannot be trained)"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (!dry_run && kept[0] < P) {
-        Dev<float> spare, spare_stats[2];
+        Dev<float> spare, spare_stats[3];
         const size_t bytes = arena_floats(m, m->Pcap) * sizeof(float);
         MAP_TRY(spare.allocate(bytes));
         if (m->dens_on)                                    // the statistics move with their rows (and their spares are zero)
@@ -1341,11 +1356,11 @@ int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, uint32_t* 
             std::swap(*arena, spare);
         }
         if (m->dens_on) {
-            Dev<float>* stats[2] = {&m->dens_accum, &m->dens_denom};
-            for (int q = 0; q < 2; ++q) {
+            Buf* stats[3] = {&m->dens_accum, &m->dens_denom, &m->dens_maxr};
+            for (int q = 0; q < 3; ++q) {
                 GLIC_CUDA_TRY(cudaMemsetAsync(spare_stats[q], 0, (size_t)m->Pcap * 4, s));
-                MAP_TRY(launch_gather_floats(*stats[q], spare_stats[q], P, kept[0], prune_index(scratch, P), s));
-                std::swap(*stats[q], spare_stats[q]);
+                MAP_TRY(launch_gather_words(stats[q]->raw(), spare_stats[q], P, kept[0], prune_index(scratch, P), s));
+                std::swap(*stats[q], static_cast<Buf&>(spare_stats[q]));
             }
         }
         GLIC_CUDA_TRY(cudaStreamSynchronize(s));
@@ -1366,61 +1381,65 @@ int glic_mapper_enable_densification(glic_mapper* m) {
     }
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     MAP_TRY(poll_ring(m, true));
-    // the exchange block gains the two statistics rows; every new buffer starts zeroed
+    // the exchange block gains the two statistics rows and the radius slots; every new buffer starts zeroed
     const XLayout x = xblock_layout(m->S, m->Pcap, true);
-    MAP_TRY(grow(m, {{m->xblock, x.bytes, 0, true}, {m->dens_accum, (size_t)m->Pcap * 4, 0, true}, {m->dens_denom, (size_t)m->Pcap * 4, 0, true}}));
+    MAP_TRY(grow(m, {{m->xblock, x.bytes, 0, true}, {m->dens_accum, (size_t)m->Pcap * 4, 0, true}, {m->dens_denom, (size_t)m->Pcap * 4, 0, true},
+                     {m->dens_maxr, (size_t)m->Pcap * 4, 0, true}}));
     m->x = x;
     m->peers[m->cfg.rank] = m->xblock;
     m->dens_on = true;
     return GLIC_OK;
 }
 
-// Inria's densify_and_clone + densify_and_split (N = 2) as one three-way compaction (prune.cu): select, reserve (capacity, then
-// one spare arena), gather every arena into the spare in rotation as prune does (the moments keep only the kept rows: the new
-// rows' moments are zero), write the children's xyz and log-scale, zero the statistics.
-int glic_mapper_densify(glic_mapper* m, float grad_threshold, float percent_dense, float scene_extent, int dry_run, uint32_t* cloned,
-                        uint32_t* split) {
-    if (!m) { set_error("mapper_densify: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!m->dens_on) { set_error("mapper_densify: densification is not enabled (glic_mapper_enable_densification)"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!std::isfinite(grad_threshold) || grad_threshold < 0.0f || !std::isfinite(percent_dense) || percent_dense < 0.0f ||
-        !std::isfinite(scene_extent) || !(scene_extent > 0.0f)) {
-        set_error("mapper_densify: grad_threshold and percent_dense must be finite and >= 0, scene_extent finite and > 0");
-        return GLIC_ERR_INVALID_ARGUMENT;
-    }
+}  // extern "C"
+
+namespace {
+
+// glic_mapper_densify_and_prune (glic_mapper_densify: min_opacity 0, both size tests off) as one compaction (prune.cu): select,
+// reserve (capacity, then one spare arena), gather every arena into the spare in rotation as prune does (the moments keep only
+// the kept rows: the new rows' moments are zero), write the children's xyz and log-scale, zero the statistics.  The caller has
+// validated p.  reject_empty: a result without rows is an error (densify on an empty map is not).
+int density_step(glic_mapper* m, const glic_density_params& p, int dry_run, bool reject_empty, glic_density_counts* out, const char* what) {
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     MAP_TRY(poll_ring(m, true));
     const uint32_t P = m->P;
-    uint32_t cnt[2] = {0, 0};                                      // clones, splits
+    uint32_t r[6] = {0, 0, 0, 0, 0, 0};                // clones, splits, surviving kept rows, clones, split rows, sky rows
     cudaStream_t s = m->stream;
     if (P) {
-        MAP_TRY(reserve(m, m->extend_ws, densify_scratch_bytes(P)));   // the selection's scratch: the idle extend() staging
+        MAP_TRY(reserve(m, m->extend_ws, density_scratch_bytes(P)));   // the selection's scratch: the idle extend() staging
         float* g[6];
         arena_ptrs(m, m->params, m->Pcap, g);
-        const float clone_max = percent_dense * scene_extent;
-        MAP_TRY(launch_densify_select(P, m->n_sky, m->dens_accum, m->dens_denom, g[2], grad_threshold, clone_max, m->extend_ws, cnt, s));
+        const DensitySelect a{P, m->n_sky, m->dens_accum, m->dens_denom, g[2], g[3], m->dens_maxr, p.grad_threshold,
+                              p.percent_dense * p.scene_extent, p.min_opacity, p.max_world_scale, p.max_screen_radius};
+        MAP_TRY(launch_density_select(a, m->extend_ws, r, s));
     }
-    const uint32_t n_clone = cnt[0], n_split = cnt[1];
-    const uint64_t total = (uint64_t)P + n_clone + n_split;
-    if (!dry_run && total > P) {
-        if (total > m->Pcap) {
+    const uint32_t n_clone = r[0], n_split = r[1], kept = r[2], cloned = r[3], split = r[4];
+    const uint64_t unpruned = (uint64_t)P + n_clone + n_split, rows = (uint64_t)kept + cloned + 2 * (uint64_t)split;
+    if (reject_empty && rows == 0) {
+        set_error(std::string(what) + ": the result has no rows (an empty map cannot be trained)");
+        return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (!dry_run && (n_clone || n_split || rows != P)) {
+        if (rows > m->Pcap) {
             if (m->connected) {
-                set_error("mapper_densify: the result does not fit the capacity, which is fixed once the exchange blocks are connected (world > 1); prune first");
+                set_error(std::string(what) + ": the result does not fit the capacity, which is fixed once the exchange blocks are connected (world > 1); prune first");
                 return GLIC_ERR_WORKSPACE;
             }
-            MAP_TRY(set_capacity(m, std::max<uint32_t>((uint32_t)total, 2 * m->Pcap)));
+            MAP_TRY(set_capacity(m, std::max<uint32_t>((uint32_t)rows, 2 * m->Pcap)));
         }
         Dev<float> spare;
         const size_t bytes = arena_floats(m, m->Pcap) * sizeof(float);
         MAP_TRY(spare.allocate(bytes));
         GLIC_CUDA_TRY(cudaMemsetAsync(spare, 0, bytes, s));
-        const uint32_t* idx = densify_index(m->extend_ws, P);
-        const uint32_t kept = P - n_split;
+        const uint32_t* idx = density_index(m->extend_ws, P);
+        const uint32_t written = std::max<uint32_t>((uint32_t)rows, P);   // the rows a prune vacates become zero
         for (Dev<float>* arena : {&m->params, &m->m1, &m->m2}) {
-            MAP_TRY(launch_gather_rows(*arena, spare, m->Pcap, m->M, (uint32_t)total, arena == &m->params ? (uint32_t)total : kept, idx, s));
+            MAP_TRY(launch_gather_rows(*arena, spare, m->Pcap, m->M, written, arena == &m->params ? (uint32_t)rows : kept, idx, s));
             std::swap(*arena, spare);
         }
-        MAP_TRY(launch_densify_children(m->params, m->Pcap, m->M, kept + n_clone, 2 * n_split, m->cfg.seed, m->dens_calls, s));
-        m->P = (uint32_t)total;
+        MAP_TRY(launch_densify_children(m->params, m->Pcap, m->M, kept + cloned, split, m->extend_ws, P, n_split, m->cfg.seed, m->dens_calls, s));
+        m->P = (uint32_t)rows;
+        m->n_sky = r[5];
         m->st.num_gaussians = m->P;
     }
     if (!dry_run) {
@@ -1428,8 +1447,147 @@ int glic_mapper_densify(glic_mapper* m, float grad_threshold, float percent_dens
         GLIC_CUDA_TRY(cudaStreamSynchronize(s));
         ++m->dens_calls;
     }
-    if (cloned) *cloned = n_clone;
-    if (split) *split = n_split;
+    if (out) *out = glic_density_counts{n_clone, n_split, (uint32_t)(unpruned - rows), (uint32_t)rows};
+    return GLIC_OK;
+}
+
+// getNerfppNorm's radius over the training keyframes' camera centres (their device poses under pose refinement), in double
+int scene_extent(glic_mapper* m, float* out) {
+    const size_t n = m->train.size();
+    *out = 0.0f;
+    if (n == 0) return GLIC_OK;
+    std::vector<double> c(3 * n);
+    if (m->pose_on) {
+        std::vector<float> f12(12 * n);
+        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+        GLIC_CUDA_TRY(cudaMemcpy(f12.data(), m->pose_f, f12.size() * sizeof(float), cudaMemcpyDeviceToHost));
+        for (size_t k = 0; k < n; ++k) for (int i = 0; i < 3; ++i) c[3 * k + i] = f12[12 * k + 9 + i];
+    } else {
+        for (size_t k = 0; k < n; ++k) for (int i = 0; i < 3; ++i) c[3 * k + i] = m->train[k].t_wc[i];
+    }
+    double mean[3] = {0.0, 0.0, 0.0}, far = 0.0;
+    for (size_t k = 0; k < n; ++k) for (int i = 0; i < 3; ++i) mean[i] += c[3 * k + i];
+    for (int i = 0; i < 3; ++i) mean[i] /= (double)n;
+    for (size_t k = 0; k < n; ++k) {
+        const double dx = c[3 * k] - mean[0], dy = c[3 * k + 1] - mean[1], dz = c[3 * k + 2] - mean[2];
+        far = std::max(far, std::sqrt(dx * dx + dy * dy + dz * dz));
+    }
+    *out = (float)(1.1 * far);
+    return GLIC_OK;
+}
+
+// the schedule's work after the iteration that made stats.iterations = n (glic_mapper_set_density_schedule)
+int scheduled_density_step(glic_mapper* m) {
+    const glic_density_schedule& c = m->sched;
+    const uint64_t n = m->st.iterations;
+    if (c.densify_from < n && n < c.densify_until && n % c.densify_interval == 0) {
+        float extent = c.scene_extent;
+        if (!(extent > 0.0f)) MAP_TRY(scene_extent(m, &extent));
+        if (extent > 0.0f) {                                        // one keyframe, or all at one place: no step
+            const bool sizes = c.opacity_reset_interval > 0 && n > c.opacity_reset_interval;
+            const glic_density_params p{c.grad_threshold, c.percent_dense, extent, c.min_opacity, sizes ? c.screen_radius : 0,
+                                        sizes ? c.world_scale_factor * extent : 0.0f};
+            glic_density_counts k{};
+            MAP_TRY(glic_mapper_densify_and_prune(m, &p, 0, &k));
+            m->sched_totals.cloned += k.cloned;
+            m->sched_totals.split += k.split;
+            m->sched_totals.pruned += k.pruned;
+            m->sched_totals.rows = k.rows;
+            ++m->sched_steps;
+        }
+    }
+    if (c.opacity_reset_interval > 0 && n < c.densify_until && n % c.opacity_reset_interval == 0) {
+        MAP_TRY(glic_mapper_reset_opacity(m, c.reset_opacity));
+        ++m->sched_resets;
+    }
+    return GLIC_OK;
+}
+
+bool finite_at_least_zero(float x) { return std::isfinite(x) && x >= 0.0f; }
+
+}  // namespace
+
+extern "C" {
+
+int glic_mapper_densify(glic_mapper* m, float grad_threshold, float percent_dense, float scene_extent, int dry_run, uint32_t* cloned,
+                        uint32_t* split) {
+    if (!m) { set_error("mapper_densify: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!m->dens_on) { set_error("mapper_densify: densification is not enabled (glic_mapper_enable_densification)"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!finite_at_least_zero(grad_threshold) || !finite_at_least_zero(percent_dense) || !std::isfinite(scene_extent) || !(scene_extent > 0.0f)) {
+        set_error("mapper_densify: grad_threshold and percent_dense must be finite and >= 0, scene_extent finite and > 0");
+        return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    glic_density_counts k{};
+    MAP_TRY(density_step(m, glic_density_params{grad_threshold, percent_dense, scene_extent, 0.0f, 0, 0.0f}, dry_run, false, &k, "mapper_densify"));
+    if (cloned) *cloned = k.cloned;
+    if (split) *split = k.split;
+    return GLIC_OK;
+}
+
+int glic_mapper_densify_and_prune(glic_mapper* m, const glic_density_params* p, int dry_run, glic_density_counts* out) {
+    if (!m || !p) { set_error("mapper_densify_and_prune: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!m->dens_on) { set_error("mapper_densify_and_prune: densification is not enabled (glic_mapper_enable_densification)"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!finite_at_least_zero(p->grad_threshold) || !finite_at_least_zero(p->percent_dense) || !std::isfinite(p->scene_extent) ||
+        !(p->scene_extent > 0.0f) || !finite_at_least_zero(p->min_opacity) || p->min_opacity > 1.0f || p->max_screen_radius < 0 ||
+        !finite_at_least_zero(p->max_world_scale)) {
+        set_error("mapper_densify_and_prune: grad_threshold, percent_dense and max_world_scale must be finite and >= 0, scene_extent finite "
+                  "and > 0, min_opacity in [0, 1], max_screen_radius >= 0");
+        return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    return density_step(m, *p, dry_run, true, out, "mapper_densify_and_prune");
+}
+
+int glic_mapper_screen_radii(glic_mapper* m, int32_t* out) {
+    if (!m || !out) { set_error("mapper_screen_radii: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!m->dens_on) { set_error("mapper_screen_radii: densification is not enabled (glic_mapper_enable_densification)"); return GLIC_ERR_INVALID_ARGUMENT; }
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    if (m->P) GLIC_CUDA_TRY(cudaMemcpy(out, m->dens_maxr, (size_t)m->P * 4, cudaMemcpyDeviceToHost));
+    return GLIC_OK;
+}
+
+// Inria's reset_opacity on the non-sky rows: one kernel (prune.cu) after the pipeline drains
+int glic_mapper_reset_opacity(glic_mapper* m, float max_opacity) {
+    if (!m) { set_error("mapper_reset_opacity: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!std::isfinite(max_opacity) || !(max_opacity > 0.0f) || !(max_opacity < 1.0f)) {
+        set_error("mapper_reset_opacity: max_opacity must be finite and in (0, 1)"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    MAP_TRY(poll_ring(m, true));
+    const double r = (double)max_opacity;
+    MAP_TRY(launch_reset_opacity(m->n_sky, m->P, m->Pcap, m->M, m->params, m->m1, m->m2, max_opacity, (float)std::log(r / (1.0 - r)), m->stream));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    return GLIC_OK;
+}
+
+int glic_mapper_set_density_schedule(glic_mapper* m, const glic_density_schedule* c) {
+    if (!m) { set_error("mapper_set_density_schedule: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (c) {
+        if (!m->dens_on) { set_error("mapper_set_density_schedule: densification is not enabled (glic_mapper_enable_densification)"); return GLIC_ERR_INVALID_ARGUMENT; }
+        if (c->densify_interval == 0 || !finite_at_least_zero(c->grad_threshold) || !finite_at_least_zero(c->percent_dense) ||
+            !finite_at_least_zero(c->min_opacity) || c->min_opacity > 1.0f || !std::isfinite(c->reset_opacity) || !(c->reset_opacity > 0.0f) ||
+            !(c->reset_opacity < 1.0f) || c->screen_radius < 0 || !finite_at_least_zero(c->world_scale_factor) || !finite_at_least_zero(c->scene_extent)) {
+            set_error("mapper_set_density_schedule: densify_interval must be >= 1, grad_threshold, percent_dense, world_scale_factor and "
+                      "scene_extent finite and >= 0, min_opacity in [0, 1], reset_opacity in (0, 1), screen_radius >= 0");
+            return GLIC_ERR_INVALID_ARGUMENT;
+        }
+        m->sched = *c;
+    }
+    m->sched_on = c != nullptr;
+    m->sched_totals = glic_density_counts{};
+    m->sched_steps = m->sched_resets = 0;
+    return GLIC_OK;
+}
+
+int glic_mapper_scene_extent(glic_mapper* m, float* out) {
+    if (!m || !out) { set_error("mapper_scene_extent: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    return scene_extent(m, out);
+}
+
+int glic_mapper_density_totals(glic_mapper* m, glic_density_counts* out, uint32_t* steps, uint32_t* resets) {
+    if (!m) { set_error("mapper_density_totals: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (out) *out = m->sched_totals;
+    if (steps) *steps = m->sched_steps;
+    if (resets) *resets = m->sched_resets;
     return GLIC_OK;
 }
 

@@ -92,7 +92,9 @@ adam_packed_kernel(float* __restrict__ param, const float* __restrict__ grad, fl
 // gradients (already summed over the rank's views and mean-reduced over the ranks) read from the arena-shaped gradient block,
 // dc / sh-rest from the slab.
 // Densification (g_dens set): lane = Gaussian, every row visible in some slot adds dens_scale times the batch's statistics
-// (norm sum, view count; dens_scale = world undoes the exchange's mean) to its running sums.  A set skip flag leaves them.
+// (norm sum, view count; dens_scale = world undoes the exchange's mean) to its running sums, and raises its screen-radius
+// statistic to the largest radius of the slots that see it (vs.radii: each slot's radii, next to its flags).  A set skip flag
+// leaves them.
 struct ArenaLayout {
     size_t off[6];       // float offset of each group in the arena: rotation, xyz, log-scale, opacity, dc, sh-rest
     float lr[6];
@@ -102,6 +104,7 @@ struct ViewSlots {
     const float* g_color;    // [n_slots][stride][3] dL/dcolour per view as the render backward left it (before the clamp mask)
     const uint8_t* visible;  // [n_slots][stride] per-view flags: 0x80 = radii > 0, bits 0..2 = colour channel clamped (forward.cu:70-75)
     const float* campos[32]; // [n_slots] camera centre of each slot's view, in its device camera block (n_slots <= 32)
+    const int* radii;        // [n_slots][stride] per-view screen radii (densification only)
     size_t stride;           // Gaussians per slot (the arena capacity)
     int n_slots;
 };
@@ -113,7 +116,8 @@ adam_compact_kernel(uint32_t P, int D, int M, float* __restrict__ params, float*
                     const float* __restrict__ g_geo /* arena-shaped: rotation | xyz | log-scale | opacity */, ArenaLayout L,
                     ArenaLayout Lg, ViewSlots vs, float grad_scale, float color_scale, float b1, float b2, float eps,
                     const unsigned int* __restrict__ skip_flag, unsigned int* __restrict__ visible_count,
-                    const float* __restrict__ g_dens, float* __restrict__ dens_accum, float* __restrict__ dens_denom, float dens_scale) {
+                    const float* __restrict__ g_dens, float* __restrict__ dens_accum, float* __restrict__ dens_denom, float dens_scale,
+                    int* __restrict__ dens_maxr) {
     __shared__ float s_g[ADAM_WARPS][32 * (SH_ROW_MAX + 3)];      // rebuilt gradients of the warp's 32 Gaussians: dc[32][3] | sh-rest[32][K]
     __shared__ uint8_t s_row[ADAM_WARPS][32];                      // compacted list of the warp's visible rows
     if (skip_flag && *skip_flag) return;                          // binning overflow: the frame was empty, do not step (ADVICE r1)
@@ -131,6 +135,10 @@ adam_compact_kernel(uint32_t P, int D, int M, float* __restrict__ params, float*
     if (g_dens && vis) {
         dens_accum[i] = __fadd_rn(dens_accum[i], __fmul_rn(g_dens[i], dens_scale));
         dens_denom[i] = __fadd_rn(dens_denom[i], __fmul_rn(g_dens[vs.stride + i], dens_scale));
+        int r = dens_maxr[i];
+        for (int v = 0; v < vs.n_slots; ++v)
+            if (vs.visible[(size_t)v * vs.stride + i] & 0x80u) r = max(r, vs.radii[(size_t)v * vs.stride + i]);
+        dens_maxr[i] = r;
     }
     const unsigned any = __ballot_sync(0xffffffffu, vis);
     if (!any) return;
@@ -342,16 +350,20 @@ int glic_arena_regrow(const float* src, uint32_t Pcap_src, float* dst, uint32_t 
 namespace glic {
 namespace {
 __global__ void __launch_bounds__(256)
-view_flags_kernel(int P, const int* __restrict__ radii, const uint8_t* __restrict__ clamped, uint8_t* __restrict__ flags) {
+view_flags_kernel(int P, const int* __restrict__ radii, const uint8_t* __restrict__ clamped, uint8_t* __restrict__ flags,
+                  int* __restrict__ radii_out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < P) flags[i] = radii[i] > 0 ? (uint8_t)(0x80u | (clamped[i] & 7u)) : (uint8_t)0;
+    if (i >= P) return;
+    const int r = radii[i];
+    flags[i] = r > 0 ? (uint8_t)(0x80u | (clamped[i] & 7u)) : (uint8_t)0;
+    if (radii_out) radii_out[i] = r;
 }
 }  // namespace
 
 // per-view flags byte of the compact exchange: visibility + the forward's colour-clamp bits
-int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flags, cudaStream_t s) {
+int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flags, cudaStream_t s, int* radii_out) {
     if (P <= 0) return GLIC_OK;
-    view_flags_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, radii, g.clamped, flags);
+    view_flags_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, radii, g.clamped, flags, radii_out);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }
@@ -360,7 +372,7 @@ int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, 
                         uint32_t Pcap_geo, const float* lr6, const float* g_color, const uint8_t* flags, const float* const* campos_dev,
                         int n_slots, float grad_scale, float color_scale, float b1, float b2, float eps, const unsigned int* skip_flag,
                         unsigned int* visible_count, cudaStream_t s, const float* g_dens, float* dens_accum, float* dens_denom,
-                        float dens_scale) {
+                        float dens_scale, const int* radii, int* dens_maxr) {
     if (P == 0) return GLIC_OK;
     ArenaLayout L, Lg;
     size_t off6[6];
@@ -370,13 +382,14 @@ int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, 
     for (int q = 0; q < 6; ++q) { Lg.off[q] = off6[q]; Lg.lr[q] = 0.f; }
     ViewSlots vs;
     if (n_slots < 1 || n_slots > 32 || !campos_dev) { set_error("adam_compact: 1..32 view slots"); return GLIC_ERR_INVALID_ARGUMENT; }
-    vs.g_color = g_color; vs.visible = flags; vs.stride = Pcap_geo; vs.n_slots = n_slots;
+    if (g_dens && (!radii || !dens_maxr)) { set_error("adam_compact: the densification statistics need the radii"); return GLIC_ERR_INVALID_ARGUMENT; }
+    vs.g_color = g_color; vs.visible = flags; vs.radii = radii; vs.stride = Pcap_geo; vs.n_slots = n_slots;
     for (int i = 0; i < n_slots; ++i) vs.campos[i] = campos_dev[i];
     const unsigned warps = (P + 31) / 32;
     StageTimer _t(GLIC_STAGE_ADAM, s);
     adam_compact_kernel<<<(warps + ADAM_WARPS - 1) / ADAM_WARPS, ADAM_WARPS * 32, 0, s>>>(
         P, D, M, params, exp_avg, exp_avg_sq, g_geo, L, Lg, vs, grad_scale, color_scale, b1, b2, eps, skip_flag, visible_count, g_dens,
-        dens_accum, dens_denom, dens_scale);
+        dens_accum, dens_denom, dens_scale, dens_maxr);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }

@@ -12,14 +12,17 @@
 //      their rows are, so loads coalesce across a run of kept rows.
 // The keep decision is opacity_activation(logit) >= min_opacity, the activation kernel's own expression (common.cuh).
 //
-// Densification (glic_mapper_densify) is a three-way version of the same compaction.  Each row is kept, cloned (kept and
-// copied once) or split (replaced by two children):
-//   1. densify_count_kernel: per tile, the clones and the splits;
-//   2. prune_scan_kernel, once per count: tile offsets and the two totals;
-//   3. densify_index_kernel: idx[new] = old for the kept rows (rows that are not split, in order), then the clones, then the
-//      first child of every split row, then the second; the children's rows start as copies of their parent;
+// Densification (glic_mapper_densify_and_prune, and glic_mapper_densify, which is its case without a prune) is a five-way
+// version of the same compaction.  Each row is kept, cloned (kept and copied once) or split (replaced by two children), and
+// each of the rows it leaves in the densify result survives the prune predicate or not (row_fate):
+//   1. fate_count_kernel: per tile, the clones and the splits, and the survivors of each kind;
+//   2. prune_scan_kernel, one CTA per count: tile offsets and the five totals;
+//   3. fate_index_kernel: idx[new] = old for the surviving kept rows (rows that are not split, in order), then the surviving
+//      clones, then the first child of every surviving split row, then the second; the children's rows start as copies of their
+//      parent, and each child's key is the row it has in the densify result before the prune;
 //   4. prune_gather_kernel per arena (the moments take only the kept rows; every new row gets zero moments);
-//   5. densify_children_kernel: each child row, a copy of its parent, gets its own xyz and the parent's log-scale - log(1.6).
+//   5. densify_children_kernel: each child row, a copy of its parent, gets its own xyz (drawn at its key) and the parent's
+//      log-scale - log(1.6).
 // The decisions use the activation kernel's expf (scale_activation) and the child geometry its normalisation
 // (rotation_activation); glic_densify_split evaluates the same child geometry on its own.
 #include "common.cuh"
@@ -65,8 +68,11 @@ prune_count_kernel(uint32_t P, const float* __restrict__ logit, float min_opacit
     }
 }
 
-// exclusive scan of the tile counts in place, the total into *total
+// exclusive scan of the tile counts in place, the total into *total; CTA b scans the b-th of consecutive arrays of n_tiles
+// counts into total[b]
 __global__ void __launch_bounds__(1024) prune_scan_kernel(uint32_t n_tiles, uint32_t* __restrict__ tile, uint32_t* __restrict__ total) {
+    tile += (size_t)blockIdx.x * n_tiles;
+    total += blockIdx.x;
     __shared__ uint32_t warp_tot[32];
     __shared__ uint32_t carry;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -239,85 +245,135 @@ namespace {
 
 constexpr float SPLIT_LOG_SCALE = 0x1.e148a2p-2f;              // (float)log(1.6): log(exp(ls) / (0.8 * 2)) = ls - log(1.6)
 
-// 0 keep, 1 clone, 2 split (glic_mapper_densify): sky rows are kept; grad = accum / denom (0 without a view);
-// selected iff grad >= threshold; a selected row is cloned iff its largest activated scale is <= clone_max_scale
-__device__ __forceinline__ int densify_class(uint32_t r, uint32_t n_sky, const float* __restrict__ accum, const float* __restrict__ denom,
-                                             const float* __restrict__ log_scale, float thr, float clone_max) {
-    if (r < n_sky) return 0;
-    const float d = denom[r];
-    const float grad = d > 0.0f ? __fdiv_rn(accum[r], d) : 0.0f;
-    if (!(grad >= thr)) return 0;
-    const float* ls = log_scale + 3 * (size_t)r;
-    const float smax = fmaxf(fmaxf(scale_activation(ls[0]), scale_activation(ls[1])), scale_activation(ls[2]));
-    return smax <= clone_max ? 1 : 2;
+// The fate of row r in one densify-and-prune.  Bits 0-1, the densify class: 0 keep, 1 clone, 2 split.  Sky rows are kept;
+// grad = accum / denom (0 without a view); selected iff grad >= threshold; a selected row is cloned iff its largest activated
+// scale is <= clone_max, split otherwise.  Bits 2-4, which of the densify result's rows that come from r survive the prune
+// predicate: the row itself (kept or cloned), its clone, its two children (one logit and one log-scale: one fate).  The
+// predicate: act(logit) < min_opacity, or (non-sky rows) maxr > max_screen_radius > 0, or largest scale > max_world_scale > 0.
+// Clones and children have maxr 0, and the children's scale is their own (the parent's log-scale - log(1.6)).
+constexpr unsigned FATE_ROW = 4u, FATE_CLONE = 8u, FATE_CHILDREN = 16u;
+
+__device__ __forceinline__ float largest_scale(const float* ls) {
+    return fmaxf(fmaxf(scale_activation(ls[0]), scale_activation(ls[1])), scale_activation(ls[2]));
 }
 
+__device__ __forceinline__ unsigned row_fate(uint32_t r, const DensitySelect& a) {
+    const bool sky = r < a.n_sky;
+    const float* ls = a.log_scale + 3 * (size_t)r;
+    const bool world = a.max_world_scale > 0.0f;
+    unsigned cls = 0;
+    float smax = 0.0f;
+    if (!sky) {
+        const float d = a.denom[r];
+        const float grad = d > 0.0f ? __fdiv_rn(a.accum[r], d) : 0.0f;
+        if (grad >= a.grad_threshold) {
+            smax = largest_scale(ls);
+            cls = smax <= a.clone_max ? 1u : 2u;
+        } else if (world) {
+            smax = largest_scale(ls);
+        }
+    }
+    const bool faded = opacity_activation(a.logit[r]) < a.min_opacity;
+    if (cls == 2u) {
+        bool gone = faded;
+        if (!gone && world) {
+            const float child[3] = {__fsub_rn(ls[0], SPLIT_LOG_SCALE), __fsub_rn(ls[1], SPLIT_LOG_SCALE), __fsub_rn(ls[2], SPLIT_LOG_SCALE)};
+            gone = largest_scale(child) > a.max_world_scale;
+        }
+        return cls | (gone ? 0u : FATE_CHILDREN);
+    }
+    const bool copy_gone = faded || (!sky && world && smax > a.max_world_scale);
+    const bool row_gone = copy_gone || (!sky && a.max_screen_radius > 0 && a.maxr[r] > a.max_screen_radius);
+    return cls | (row_gone ? 0u : FATE_ROW) | (cls == 1u && !copy_gone ? FATE_CLONE : 0u);
+}
+
+// the counts of one row, two to a word (at most PRUNE_TILE = 1024 of each per CTA): A = clones | splits << 16 (of the densify
+// result), B = surviving kept rows | surviving clones << 16, C = surviving split rows
+__device__ __forceinline__ void fate_counts(unsigned f, uint32_t& A, uint32_t& B, uint32_t& C) {
+    const unsigned cls = f & 3u;
+    A += cls == 1u ? 1u : cls == 2u ? (1u << 16) : 0u;
+    if (cls == 2u) C += (f & FATE_CHILDREN) ? 1u : 0u;
+    else B += ((f & FATE_ROW) ? 1u : 0u) + ((f & FATE_CLONE) ? (1u << 16) : 0u);
+}
+
+// per tile: tile[q * n_tiles + tile] for q = clones, splits, surviving kept rows, surviving clones, surviving split rows
 __global__ void __launch_bounds__(PRUNE_THREADS)
-densify_count_kernel(uint32_t P, uint32_t n_sky, const float* __restrict__ accum, const float* __restrict__ denom,
-                     const float* __restrict__ log_scale, float thr, float clone_max, uint32_t* __restrict__ tile_clone,
-                     uint32_t* __restrict__ tile_split) {
+fate_count_kernel(DensitySelect a, uint32_t n_tiles, uint32_t* __restrict__ tile) {
     const uint32_t r0 = blockIdx.x * PRUNE_TILE + PRUNE_ROWS * threadIdx.x;
-    uint32_t n = 0;                                            // clones | splits << 16 (at most PRUNE_TILE each)
+    uint32_t A = 0, B = 0, Cn = 0;
 #pragma unroll
     for (int e = 0; e < PRUNE_ROWS; ++e) {
-        if (r0 + e >= P) break;
-        const int c = densify_class(r0 + e, n_sky, accum, denom, log_scale, thr, clone_max);
-        n += c == 1 ? 1u : c == 2 ? (1u << 16) : 0u;
+        if (r0 + e >= a.P) break;
+        fate_counts(row_fate(r0 + e, a), A, B, Cn);
     }
-    __shared__ uint32_t warp_n[PRUNE_THREADS / 32];
+    __shared__ uint32_t warp_n[3][PRUNE_THREADS / 32];
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
-    if ((threadIdx.x & 31) == 0) warp_n[threadIdx.x >> 5] = n;
+    for (int o = 16; o > 0; o >>= 1) {
+        A += __shfl_xor_sync(0xffffffffu, A, o);
+        B += __shfl_xor_sync(0xffffffffu, B, o);
+        Cn += __shfl_xor_sync(0xffffffffu, Cn, o);
+    }
+    if ((threadIdx.x & 31) == 0) { warp_n[0][threadIdx.x >> 5] = A; warp_n[1][threadIdx.x >> 5] = B; warp_n[2][threadIdx.x >> 5] = Cn; }
     __syncthreads();
     if (threadIdx.x == 0) {
-        uint32_t t = 0;
-        for (int w = 0; w < PRUNE_THREADS / 32; ++w) t += warp_n[w];
-        tile_clone[blockIdx.x] = t & 0xFFFFu;
-        tile_split[blockIdx.x] = t >> 16;
+        uint32_t ta = 0, tb = 0, tc = 0;
+        for (int w = 0; w < PRUNE_THREADS / 32; ++w) { ta += warp_n[0][w]; tb += warp_n[1][w]; tc += warp_n[2][w]; }
+        const uint32_t c[5] = {ta & 0xFFFFu, ta >> 16, tb & 0xFFFFu, tb >> 16, tc};
+        for (int q = 0; q < 5; ++q) tile[(size_t)q * n_tiles + blockIdx.x] = c[q];
     }
 }
 
-// totals[2] = {clones, splits} (the scans' totals); places every result row's source row in idx
+// totals[6] = {clones, splits, surviving kept, surviving clones, surviving split rows (the scans' totals), the new index of
+// row n_sky}.  Places every surviving row's source row in idx: the surviving kept rows, the surviving clones, the first then
+// the second children of the surviving split rows; key[j] = the row the first child of surviving split j has in the densify
+// result before the prune (its second child's is key[j] + splits)
 __global__ void __launch_bounds__(PRUNE_THREADS)
-densify_index_kernel(uint32_t P, uint32_t n_sky, const float* __restrict__ accum, const float* __restrict__ denom,
-                     const float* __restrict__ log_scale, float thr, float clone_max, const uint32_t* __restrict__ clone_offset,
-                     const uint32_t* __restrict__ split_offset, const uint32_t* __restrict__ totals, uint32_t* __restrict__ idx) {
+fate_index_kernel(DensitySelect a, uint32_t n_tiles, const uint32_t* __restrict__ tile_offset, uint32_t* __restrict__ totals,
+                  uint32_t* __restrict__ idx, uint32_t* __restrict__ key) {
     const uint32_t r0 = blockIdx.x * PRUNE_TILE + PRUNE_ROWS * threadIdx.x;
-    int cls[PRUNE_ROWS];
-    uint32_t n = 0;
+    unsigned f[PRUNE_ROWS];
+    uint32_t A = 0, B = 0, Cn = 0;
 #pragma unroll
     for (int e = 0; e < PRUNE_ROWS; ++e) {
-        cls[e] = r0 + e < P ? densify_class(r0 + e, n_sky, accum, denom, log_scale, thr, clone_max) : -1;
-        n += cls[e] == 1 ? 1u : cls[e] == 2 ? (1u << 16) : 0u;
+        f[e] = r0 + e < a.P ? row_fate(r0 + e, a) : 0u;
+        if (r0 + e < a.P) fate_counts(f[e], A, B, Cn);
     }
-    // exclusive scan of the packed counts over the CTA, in thread (= row) order
-    __shared__ uint32_t warp_tot[PRUNE_THREADS / 32];
+    // exclusive scans of the three count words over the CTA, in thread (= row) order
+    __shared__ uint32_t warp_tot[3][PRUNE_THREADS / 32];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t incl = n;
+    uint32_t ia = A, ib = B, ic = Cn;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += t;
+        const uint32_t ta = __shfl_up_sync(0xffffffffu, ia, o), tb = __shfl_up_sync(0xffffffffu, ib, o), tc = __shfl_up_sync(0xffffffffu, ic, o);
+        if (lane >= o) { ia += ta; ib += tb; ic += tc; }
     }
-    if (lane == 31) warp_tot[warp] = incl;
+    if (lane == 31) { warp_tot[0][warp] = ia; warp_tot[1][warp] = ib; warp_tot[2][warp] = ic; }
     __syncthreads();
-    uint32_t before = 0;
-    for (int w = 0; w < warp; ++w) before += warp_tot[w];
-    const uint32_t excl = before + incl - n;
-    uint32_t clones = clone_offset[blockIdx.x] + (excl & 0xFFFFu), splits = split_offset[blockIdx.x] + (excl >> 16);
-    const uint32_t n_clone = totals[0], n_split = totals[1];
-    const uint32_t kept = P - n_split, first_child = kept + n_clone;
+    uint32_t ba = 0, bb = 0, bc = 0;
+    for (int w = 0; w < warp; ++w) { ba += warp_tot[0][w]; bb += warp_tot[1][w]; bc += warp_tot[2][w]; }
+    const uint32_t ea = ba + ia - A, eb = bb + ib - B, ec = bc + ic - Cn;
+    const uint32_t n_clone = totals[0], n_split = totals[1], n_kept = totals[2], n_cloned = totals[3], n_split_s = totals[4];
+    uint32_t split = tile_offset[1 * (size_t)n_tiles + blockIdx.x] + (ea >> 16);
+    uint32_t kept = tile_offset[2 * (size_t)n_tiles + blockIdx.x] + (eb & 0xFFFFu);
+    uint32_t clone = tile_offset[3 * (size_t)n_tiles + blockIdx.x] + (eb >> 16);
+    uint32_t child = tile_offset[4 * (size_t)n_tiles + blockIdx.x] + ec;
+    const uint32_t first_child = a.P - n_split + n_clone;                  // before the prune
+    const uint32_t first_child_s = n_kept + n_cloned;                      // after it
 #pragma unroll
     for (int e = 0; e < PRUNE_ROWS; ++e) {
         const uint32_t r = r0 + e;
-        if (cls[e] < 0) break;
-        if (cls[e] == 2) {
-            idx[first_child + splits] = r;
-            idx[first_child + n_split + splits] = r;
-            ++splits;
+        if (r >= a.P) break;
+        if (r == a.n_sky) totals[5] = kept;
+        if ((f[e] & 3u) == 2u) {
+            if (f[e] & FATE_CHILDREN) {
+                idx[first_child_s + child] = r;
+                idx[first_child_s + n_split_s + child] = r;
+                key[child++] = first_child + split;
+            }
+            ++split;
         } else {
-            idx[r - splits] = r;
-            if (cls[e] == 1) idx[kept + clones++] = r;
+            if (f[e] & FATE_ROW) idx[kept++] = r;
+            if (f[e] & FATE_CLONE) idx[n_kept + clone++] = r;
         }
     }
 }
@@ -352,13 +408,15 @@ __device__ __forceinline__ void split_child(const float p[3], const float s[3], 
         out[i] = __fadd_rn(p[i], __fadd_rn(__fadd_rn(__fmul_rn(R[3 * i], v[0]), __fmul_rn(R[3 * i + 1], v[1])), __fmul_rn(R[3 * i + 2], v[2])));
 }
 
-// rows [first, first + n) of the arena (copies of their parents) become the split children: xyz and log-scale
+// rows [first, first + 2 n) of the arena (copies of their parents) become the split children: xyz and log-scale.  Child t
+// draws its normals at the row it has in the densify result before the prune: key[t] (first children, t < n), key[t - n] +
+// n_split (second children)
 __global__ void __launch_bounds__(256)
-densify_children_kernel(float* __restrict__ params, size_t off_rot, size_t off_xyz, size_t off_ls, uint32_t first, uint32_t n, uint64_t seed,
-                        uint64_t call) {
+densify_children_kernel(float* __restrict__ params, size_t off_rot, size_t off_xyz, size_t off_ls, uint32_t first, uint32_t n,
+                        const uint32_t* __restrict__ key, uint32_t n_split, uint64_t seed, uint64_t call) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= n) return;
-    const uint32_t row = first + t;
+    if (t >= 2 * n) return;
+    const uint32_t row = first + t, k = t < n ? key[t] : key[t - n] + n_split;
     float* xyz = params + off_xyz + 3 * (size_t)row;
     float* ls = params + off_ls + 3 * (size_t)row;
     const float4 q = rotation_activation(reinterpret_cast<const float4*>(params + off_rot)[row]);
@@ -367,7 +425,7 @@ densify_children_kernel(float* __restrict__ params, size_t off_rot, size_t off_x
     for (int a = 0; a < 3; ++a) {
         p[a] = xyz[a];
         s[a] = scale_activation(ls[a]);
-        z[a] = split_normal(seed, call, row, a);
+        z[a] = split_normal(seed, call, k, a);
     }
     split_child(p, s, q, z, out);
 #pragma unroll
@@ -398,57 +456,79 @@ densify_split_kernel(int n, const float* __restrict__ xyz, const float* __restri
 }
 
 __global__ void __launch_bounds__(256)
-gather_floats_kernel(const float* __restrict__ src, float* __restrict__ dst, uint32_t rows_out, uint32_t rows_valid,
-                     const uint32_t* __restrict__ idx) {
+gather_words_kernel(const uint32_t* __restrict__ src, uint32_t* __restrict__ dst, uint32_t rows_out, uint32_t rows_valid,
+                    const uint32_t* __restrict__ idx) {
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r < rows_out) dst[r] = r < rows_valid ? src[idx[r]] : 0.0f;
+    if (r < rows_out) dst[r] = r < rows_valid ? src[idx[r]] : 0u;
 }
 
-// scratch: totals[2] (256 bytes) | clone tile counts | split tile counts | idx[2P]
+// rows [first, P) (glic_mapper_reset_opacity): a logit whose activation is above max_opacity becomes `logit`; both moments of
+// the opacity group become zero
+__global__ void __launch_bounds__(256)
+reset_opacity_kernel(uint32_t first, uint32_t P, float* __restrict__ logit, float* __restrict__ m1, float* __restrict__ m2, float max_opacity,
+                     float reset_logit) {
+    const uint32_t r = first + blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= P) return;
+    if (opacity_activation(logit[r]) > max_opacity) logit[r] = reset_logit;
+    m1[r] = 0.0f;
+    m2[r] = 0.0f;
+}
+
+// scratch: totals[6] (256 bytes) | 5 arrays of tile counts | idx[2P] | key[P]
 size_t tile_bytes(uint32_t P) { return (((size_t)(P + PRUNE_TILE - 1) / PRUNE_TILE) * 4 + 255) & ~size_t(255); }
 
 }  // namespace
 
-size_t densify_scratch_bytes(uint32_t P) { return 256 + 2 * tile_bytes(P) + (size_t)P * 8; }
+size_t density_scratch_bytes(uint32_t P) { return 256 + 5 * tile_bytes(P) + (size_t)P * 12; }
 
-const uint32_t* densify_index(const void* scratch, uint32_t P) {
-    return reinterpret_cast<const uint32_t*>(static_cast<const char*>(scratch) + 256 + 2 * tile_bytes(P));
+const uint32_t* density_index(const void* scratch, uint32_t P) {
+    return reinterpret_cast<const uint32_t*>(static_cast<const char*>(scratch) + 256 + 5 * tile_bytes(P));
 }
 
-int launch_densify_select(uint32_t P, uint32_t n_sky, const float* accum, const float* denom, const float* log_scale, float grad_threshold,
-                          float clone_max_scale, void* scratch, uint32_t* result_host, cudaStream_t s) {
-    const uint32_t tiles = (P + PRUNE_TILE - 1) / PRUNE_TILE;
+int launch_density_select(const DensitySelect& a, void* scratch, uint32_t* result_host, cudaStream_t s) {
+    const uint32_t tiles = (a.P + PRUNE_TILE - 1) / PRUNE_TILE;
     char* base = static_cast<char*>(scratch);
     uint32_t* totals = reinterpret_cast<uint32_t*>(base);
-    uint32_t* tile_clone = reinterpret_cast<uint32_t*>(base + 256);
-    uint32_t* tile_split = reinterpret_cast<uint32_t*>(base + 256 + tile_bytes(P));
-    uint32_t* idx = const_cast<uint32_t*>(densify_index(scratch, P));
-    densify_count_kernel<<<tiles, PRUNE_THREADS, 0, s>>>(P, n_sky, accum, denom, log_scale, grad_threshold, clone_max_scale, tile_clone, tile_split);
+    uint32_t* tile = reinterpret_cast<uint32_t*>(base + 256);          // 5 arrays of `tiles` counts, within 5 * tile_bytes(P)
+    uint32_t* idx = const_cast<uint32_t*>(density_index(scratch, a.P));
+    GLIC_CUDA_TRY(cudaMemsetAsync(totals + 5, 0, sizeof(uint32_t), s));
+    fate_count_kernel<<<tiles, PRUNE_THREADS, 0, s>>>(a, tiles, tile);
     GLIC_LAUNCH_CHECK();
-    prune_scan_kernel<<<1, 1024, 0, s>>>(tiles, tile_clone, totals);
+    prune_scan_kernel<<<5, 1024, 0, s>>>(tiles, tile, totals);
     GLIC_LAUNCH_CHECK();
-    prune_scan_kernel<<<1, 1024, 0, s>>>(tiles, tile_split, totals + 1);
+    fate_index_kernel<<<tiles, PRUNE_THREADS, 0, s>>>(a, tiles, tile, totals, idx, idx + 2 * (size_t)a.P);
     GLIC_LAUNCH_CHECK();
-    densify_index_kernel<<<tiles, PRUNE_THREADS, 0, s>>>(P, n_sky, accum, denom, log_scale, grad_threshold, clone_max_scale, tile_clone,
-                                                         tile_split, totals, idx);
-    GLIC_LAUNCH_CHECK();
-    GLIC_CUDA_TRY(cudaMemcpyAsync(result_host, totals, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    GLIC_CUDA_TRY(cudaMemcpyAsync(result_host, totals, 6 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    if (a.n_sky >= a.P) result_host[5] = result_host[2];         // every row is sky: the surviving kept rows are
     return GLIC_OK;
 }
 
-int launch_densify_children(float* params, uint32_t Pcap, int M, uint32_t first, uint32_t n, uint64_t seed, uint64_t call, cudaStream_t s) {
+int launch_densify_children(float* params, uint32_t Pcap, int M, uint32_t first, uint32_t n, const void* scratch, uint32_t P_select,
+                            uint32_t n_split, uint64_t seed, uint64_t call, cudaStream_t s) {
     if (n == 0) return GLIC_OK;
     size_t off[6];
     glic_packed_offsets(Pcap, (uint32_t)M, off);
-    densify_children_kernel<<<(n + 255) / 256, 256, 0, s>>>(params, off[0], off[1], off[2], first, n, seed, call);
+    const uint32_t* key = density_index(scratch, P_select) + 2 * (size_t)P_select;
+    densify_children_kernel<<<(2 * n + 255) / 256, 256, 0, s>>>(params, off[0], off[1], off[2], first, n, key, n_split, seed, call);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }
 
-int launch_gather_floats(const float* src, float* dst, uint32_t rows_out, uint32_t rows_valid, const uint32_t* idx, cudaStream_t s) {
+int launch_gather_words(const void* src, void* dst, uint32_t rows_out, uint32_t rows_valid, const uint32_t* idx, cudaStream_t s) {
     if (rows_out == 0) return GLIC_OK;
-    gather_floats_kernel<<<(rows_out + 255) / 256, 256, 0, s>>>(src, dst, rows_out, rows_valid, idx);
+    gather_words_kernel<<<(rows_out + 255) / 256, 256, 0, s>>>(static_cast<const uint32_t*>(src), static_cast<uint32_t*>(dst), rows_out,
+                                                               rows_valid, idx);
+    GLIC_LAUNCH_CHECK();
+    return GLIC_OK;
+}
+
+int launch_reset_opacity(uint32_t first, uint32_t P, uint32_t Pcap, int M, float* params, float* m1, float* m2, float max_opacity,
+                         float reset_logit, cudaStream_t s) {
+    if (first >= P) return GLIC_OK;
+    size_t off[6];
+    glic_packed_offsets(Pcap, (uint32_t)M, off);
+    reset_opacity_kernel<<<(P - first + 255) / 256, 256, 0, s>>>(first, P, params + off[3], m1 + off[3], m2 + off[3], max_opacity, reset_logit);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }

@@ -15,6 +15,11 @@ FASTLIVO = dict(position_lr=1.6e-4, feature_lr=2.5e-3, opacity_lr=0.05, scaling_
 DEAD_OPACITY = float(np.float32(1.0) / np.float32(255.0))             # GLIC_MAPPER_DEAD_OPACITY: the preprocess's o < 1/255 cull
 DENSIFY_GRAD_THRESHOLD = float(np.float32(0.0002))                   # GLIC_MAPPER_DENSIFY_GRAD_THRESHOLD (Inria's default)
 PERCENT_DENSE = float(np.float32(0.01))                              # GLIC_MAPPER_PERCENT_DENSE
+RESET_OPACITY = float(np.float32(0.01))                              # GLIC_MAPPER_RESET_OPACITY
+# glic_density_schedule's fields at Inria's defaults (GLIC_MAPPER_DENSIFY_FROM ... ; scene_extent 0: derived at each step)
+DENSITY_SCHEDULE = dict(densify_from=500, densify_until=15000, densify_interval=100, opacity_reset_interval=3000,
+                        grad_threshold=DENSIFY_GRAD_THRESHOLD, percent_dense=PERCENT_DENSE, min_opacity=float(np.float32(0.005)),
+                        reset_opacity=RESET_OPACITY, screen_radius=20, world_scale_factor=float(np.float32(0.1)), scene_extent=0.0)
 
 
 def _f32(a):
@@ -285,6 +290,54 @@ class Mapper:
         capi.check(capi.lib.glic_mapper_densify_stats(self._h, _p(acc) if P else acc.ctypes.data_as(C.c_void_p),
                                                       _p(den) if P else den.ctypes.data_as(C.c_void_p)), "mapper_densify_stats")
         return acc, den
+
+    def screen_radii(self):
+        """maxr [P] int32: the largest screen radius each row has had in a stepped view since the statistics last restarted."""
+        P = int(self.stats().num_gaussians)
+        out = np.zeros(max(P, 1), np.int32)
+        capi.check(capi.lib.glic_mapper_screen_radii(self._h, out.ctypes.data_as(C.c_void_p)), "mapper_screen_radii")
+        return out[:P]
+
+    def reset_opacity(self, max_opacity=RESET_OPACITY):
+        """Inria's reset_opacity on the non-sky rows: logits above max_opacity drop to it, the opacity moments become zero."""
+        capi.check(capi.lib.glic_mapper_reset_opacity(self._h, float(max_opacity)), "mapper_reset_opacity")
+
+    def densify_and_prune(self, scene_extent, grad_threshold=DENSIFY_GRAD_THRESHOLD, percent_dense=PERCENT_DENSE, min_opacity=0.0,
+                          max_screen_radius=0, max_world_scale=0.0, dry_run=False):
+        """densify() and then the removal of the result's rows with act(logit) < min_opacity, or (non-sky) maxr >
+        max_screen_radius > 0, or largest scale > max_world_scale > 0, in one compaction.  dry_run only counts.  Returns
+        {cloned, split, pruned, rows}."""
+        p = capi.DensityParams(float(grad_threshold), float(percent_dense), float(scene_extent), float(min_opacity), int(max_screen_radius),
+                               float(max_world_scale))
+        out = capi.DensityCounts()
+        capi.check(capi.lib.glic_mapper_densify_and_prune(self._h, C.byref(p), int(bool(dry_run)), C.byref(out)), "mapper_densify_and_prune")
+        return {k: int(getattr(out, k)) for k, _ in capi.DensityCounts._fields_}
+
+    def set_density_schedule(self, **fields):
+        """Run density control inside optimize(): densify_and_prune every densify_interval iterations in (densify_from,
+        densify_until), reset_opacity every opacity_reset_interval.  Fields not given take Inria's defaults (DENSITY_SCHEDULE)."""
+        unknown = set(fields) - set(DENSITY_SCHEDULE)
+        if unknown:
+            raise TypeError("unknown schedule fields: %s" % sorted(unknown))
+        s = capi.DensitySchedule(**dict(DENSITY_SCHEDULE, **fields))
+        capi.check(capi.lib.glic_mapper_set_density_schedule(self._h, C.byref(s)), "mapper_set_density_schedule")
+
+    def clear_density_schedule(self):
+        capi.check(capi.lib.glic_mapper_set_density_schedule(self._h, None), "mapper_set_density_schedule")
+
+    def scene_extent(self):
+        """getNerfppNorm's radius over the training keyframes' current camera centres."""
+        out = C.c_float()
+        capi.check(capi.lib.glic_mapper_scene_extent(self._h, C.byref(out)), "mapper_scene_extent")
+        return out.value
+
+    def density_totals(self):
+        """What the schedule has done since it was set: {cloned, split, pruned, rows, steps, resets}."""
+        out, steps, resets = capi.DensityCounts(), C.c_uint32(), C.c_uint32()
+        capi.check(capi.lib.glic_mapper_density_totals(self._h, C.byref(out), C.byref(steps), C.byref(resets)), "mapper_density_totals")
+        d = {k: int(getattr(out, k)) for k, _ in capi.DensityCounts._fields_}
+        d.update(steps=int(steps.value), resets=int(resets.value))
+        return d
 
     # ---- multi-GPU wiring: torch.distributed (or anything else) only carries the 64-byte handles --------------------------
     def export_handle(self):

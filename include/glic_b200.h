@@ -531,7 +531,14 @@ GLIC_API int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, u
  *   nothing.  With world > 1 it must come before glic_mapper_export (GLIC_ERR_INVALID_ARGUMENT otherwise; the exchange block
  *   gains two rows of Pcap floats, which the reduce carries: the committed statistics are world times the mean over the ranks,
  *   exactly the sums over all views when world is a power of two).
+ *   Every row also keeps maxr_i, an int32 screen radius starting at 0 (Inria's max_radii2D): in every iteration that steps the
+ *   Gaussians, maxr_i = max(maxr_i, radii_v,i) over every view v of the batch with radii_v,i > 0, radii_v the forward's radii of
+ *   that view.  Each view's radii travel in a slot of the exchange block next to its flag byte (pushed to the peers with it
+ *   when world > 1); the max is order-free, so replicas agree exactly.  maxr follows the rules of accum / denom above (overflow
+ *   and OPT_OPTIMIZER = 0 leave it, extend() appends 0, growth keeps it, prune moves it, initialize zeroes it) and every real
+ *   densify zeroes it.  Memory: 4 B per row of capacity, plus 2 * S * 4 B per row of capacity in the exchange block.
  *   glic_mapper_densify_stats(m, accum, denom): the P statistics of each kind to host arrays; synchronises.
+ *   glic_mapper_screen_radii(m, out): the P values of maxr to a host array; densification must be enabled; synchronises.
  *   glic_mapper_densify(m, grad_threshold, percent_dense, scene_extent, dry_run, &cloned, &split) (the counts may be NULL):
  *   - candidates are the non-sky rows [S, P) (sky rows are never densified, so the sky prefix and save_map stay valid);
  *     grad_i = denom_i > 0 ? accum_i / denom_i : 0 (one IEEE division), selected iff grad_i >= grad_threshold;
@@ -551,7 +558,9 @@ GLIC_API int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, u
  *   - densification not enabled, a NULL mapper, a non-finite or negative grad_threshold or percent_dense, or a scene_extent
  *     that is not finite and > 0 return GLIC_ERR_INVALID_ARGUMENT and change nothing.  Allocation failures follow the failure
  *     contract above.  The call drains the iteration pipeline (as prune does) and synchronises.  It needs one spare arena of the
- *     capacity while it runs, and its selection scratch (8 B per row) lives in the extend() staging buffer.
+ *     capacity while it runs, and its selection scratch (12 B per row) lives in the extend() staging buffer.  It is
+ *     glic_mapper_densify_and_prune with min_opacity = 0 and both size tests off, which removes nothing (act(l) < 0 never holds),
+ *     except that a mapper without rows returns GLIC_OK with zero counts.
  *   - world > 1: every rank makes the same calls between the same optimize() calls; replicas stay bit-identical in parameters,
  *     moments and statistics with no exchange.
  * glic_densify_split(n, xyz, scale, rot, seed, call, first_row, xyz_out, z_out, stream): the children's geometry on its own, for
@@ -573,6 +582,88 @@ GLIC_API int glic_mapper_densify(glic_mapper* m, float grad_threshold, float per
 GLIC_API int glic_mapper_densify_stats(glic_mapper* m, float* grad_accum, float* denom);
 GLIC_API int glic_densify_split(int n, const float* xyz, const float* scale, const float* rot, uint64_t seed, uint64_t call,
                                 uint32_t first_row, float* xyz_out, float* z_out, void* stream);
+GLIC_API int glic_mapper_screen_radii(glic_mapper* m, int32_t* out);
+/* Opacity reset (Inria's reset_opacity).  glic_mapper_reset_opacity(m, max_opacity): every non-sky row [S, P) whose
+ * act(logit) > max_opacity (act as in glic_mapper_prune) gets logit = (float)log(r / (1 - r)), computed in double with
+ * r = (double)max_opacity; every other logit stays bit for bit.  (Inria's inverse_sigmoid(min(sigmoid(l), 0.01)) also moves
+ * the rows already below the cut, by rounding; this does not.)  Both Adam moments of the opacity group become zero for every
+ * non-sky row, as Inria's replace_tensor_to_optimizer does.  Sky rows, every other group and every other moment stay bit for
+ * bit.  A NULL mapper, or a max_opacity that is not finite or not in (0, 1), returns GLIC_ERR_INVALID_ARGUMENT and changes
+ * nothing.  Drains the iteration pipeline (as prune does) and synchronises.  world > 1: every rank makes the same call between
+ * the same optimize() calls; no exchange is needed. */
+#define GLIC_MAPPER_RESET_OPACITY 0.01f
+GLIC_API int glic_mapper_reset_opacity(glic_mapper* m, float max_opacity);
+/* Densify and prune in one compaction (Inria's densify_and_prune).  The result is defined in two steps:
+ *   1. exactly what glic_mapper_densify(grad_threshold, percent_dense, scene_extent) would produce: the same selection, row
+ *      order and bits;
+ *   2. every row of that result that meets the prune predicate is removed:
+ *        act(logit) < min_opacity (prune's own test; sky rows can go by it), or, for non-sky rows,
+ *        max_screen_radius > 0 and maxr > max_screen_radius, or
+ *        max_world_scale > 0 and the largest activated scale (expf of the row's own log-scale) > max_world_scale,
+ *      where maxr is the statistic gathered before the call for the rows that existed and 0 for clones and children, and a
+ *      split child is judged at its own, reduced scale.  (Inria's code compares max_radii2D after densification_postfix has
+ *      zeroed it, so its screen-size test never fires; here it does.)
+ * Survivors keep the result order.  A split child draws its xyz at the row it has in the unpruned densify result, so the call
+ * equals glic_mapper_densify followed by the predicate, bit for bit, children's xyz included.  Computed in one pass: one
+ * selection, one gather per arena into one spare arena (moments for the surviving kept rows only; new rows get zero moments).
+ * After a real call accum, denom and maxr are zero for every row, `call` advances (as in densify) and glic_mapper_sky_rows is
+ * the number of surviving sky rows.  *out (may be NULL): cloned and split as glic_mapper_densify counts them, pruned = the rows
+ * of the densify result the predicate removed, rows = the rows after the call.
+ * Capacity: only the final row count must fit; a result that does not grows the arenas like extend() when the mapper is not
+ * connected, and returns GLIC_ERR_WORKSPACE and changes nothing when it is (world > 1), so a connected mapper can densify
+ * whenever pruning makes room.  Rejected with GLIC_ERR_INVALID_ARGUMENT, changing nothing: what glic_mapper_densify rejects, a
+ * NULL p, min_opacity not finite or not in [0, 1], a negative max_screen_radius, max_world_scale not finite or negative, and a
+ * result with no rows (dry run or not).  dry_run != 0 only counts.  Allocation failures follow the failure contract.  Drains
+ * the iteration pipeline and synchronises.  world > 1: every rank makes the same calls between the same optimize() calls. */
+typedef struct glic_density_params {
+    float grad_threshold, percent_dense, scene_extent;   /* as glic_mapper_densify */
+    float min_opacity;                                    /* remove iff act(logit) < min_opacity (prune's own test) */
+    int32_t max_screen_radius;                            /* > 0: remove non-sky rows with maxr > it; 0: off */
+    float max_world_scale;                                /* > 0: remove non-sky rows whose largest activated scale > it; 0: off */
+} glic_density_params;
+typedef struct glic_density_counts { uint32_t cloned, split, pruned, rows; } glic_density_counts;
+GLIC_API int glic_mapper_densify_and_prune(glic_mapper* m, const glic_density_params* p, int dry_run, glic_density_counts* out);
+/* Density control inside optimize() (Inria's schedule).  glic_mapper_set_density_schedule(m, s) sets the schedule (NULL: off,
+ * the default) and restarts the totals; densification must be enabled to set one.  Rejected with GLIC_ERR_INVALID_ARGUMENT:
+ * densify_interval 0, grad_threshold, percent_dense, world_scale_factor or scene_extent not finite or negative, min_opacity not
+ * finite or not in [0, 1], reset_opacity not finite or not in (0, 1), a negative screen_radius.
+ * After each iteration optimize() enqueues, with n = stats.iterations after it (counted across calls, overflow-skipped
+ * iterations included):
+ *   - if densify_from < n < densify_until and n % densify_interval == 0: glic_mapper_densify_and_prune with the schedule's
+ *     grad_threshold, percent_dense and min_opacity, scene_extent = the schedule's when > 0, glic_mapper_scene_extent
+ *     otherwise, and, only when opacity_reset_interval > 0 and n > opacity_reset_interval (Inria enables them together),
+ *     max_screen_radius = screen_radius and max_world_scale = world_scale_factor * extent (in float); both off before.  A
+ *     derived extent that is not > 0 (one keyframe, or all at one place) skips this step and leaves the statistics;
+ *   - then, if opacity_reset_interval > 0, n < densify_until and n % opacity_reset_interval == 0: glic_mapper_reset_opacity
+ *     (reset_opacity).
+ * With GLIC_MAPPER_OPT_OPTIMIZER = 0 the schedule does nothing.  A scheduled step drains the pipeline (the only new
+ * synchronisation); one that fails (GLIC_ERR_WORKSPACE on a connected mapper, say) ends optimize() with its error, and the
+ * iterations before it stand.  stats.ms_optimize covers the whole call.
+ * glic_mapper_scene_extent(m, out): Inria's getNerfppNorm radius over the training keyframes' current camera centres c_k (the
+ * device poses under pose refinement, as glic_mapper_pose_get returns them): 1.1 * max_k |c_k - mean(c)| in double, rounded to
+ * float; 0 without keyframes.
+ * glic_mapper_density_totals(m, out, steps, resets) (each may be NULL): since the schedule was set, the summed cloned, split and
+ * pruned counts of its densify steps, rows = the rows after the latest one (0 before any), the number of densify steps and the
+ * number of opacity resets. */
+typedef struct glic_density_schedule {
+    uint32_t densify_from, densify_until, densify_interval;  /* Inria: 500, 15000, 100 */
+    uint32_t opacity_reset_interval;                         /* 3000; 0 = never */
+    float grad_threshold, percent_dense, min_opacity;        /* 0.0002, 0.01, 0.005 */
+    float reset_opacity;                                     /* 0.01 */
+    int32_t screen_radius;                                   /* 20 */
+    float world_scale_factor;                                /* 0.1 */
+    float scene_extent;                                      /* > 0: fixed; 0: derived at each step */
+} glic_density_schedule;
+#define GLIC_MAPPER_DENSIFY_FROM 500u
+#define GLIC_MAPPER_DENSIFY_UNTIL 15000u
+#define GLIC_MAPPER_DENSIFY_INTERVAL 100u
+#define GLIC_MAPPER_OPACITY_RESET_INTERVAL 3000u
+#define GLIC_MAPPER_MIN_OPACITY 0.005f
+#define GLIC_MAPPER_SCREEN_RADIUS 20
+#define GLIC_MAPPER_WORLD_SCALE_FACTOR 0.1f
+GLIC_API int glic_mapper_set_density_schedule(glic_mapper* m, const glic_density_schedule* s);
+GLIC_API int glic_mapper_scene_extent(glic_mapper* m, float* out);
+GLIC_API int glic_mapper_density_totals(glic_mapper* m, glic_density_counts* out, uint32_t* steps, uint32_t* resets);
 /* multi-GPU wiring: every rank exports the 64-byte IPC handle of its exchange block, the caller all-gathers them
  * (torch.distributed / MPI / a file: plumbing) and hands all `world` handles back. */
 GLIC_API int glic_mapper_export(glic_mapper* m, unsigned char* handle64);
