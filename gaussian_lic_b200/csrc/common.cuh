@@ -383,38 +383,32 @@ int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, cons
                    size_t scratch_bytes, void* stream);
 // the clamped (and exposed) images eval_psnr_ssim scored, left in its scratch: which = 0 the image, 1 the ground truth
 const float* eval_clamped(const void* scratch, int CH, int H, int W, int which);
-// stable compaction of the arenas (prune.cu).  select: which of rows [0, P) keep opacity_activation(logit) >= min_opacity;
-// result_host[2] = {kept rows, kept rows among [0, n_sky)}, synchronises s.  gather: output rows [0, P_old) of every group of
-// dst = the kept rows of src in order, then zeros; src and dst are arenas of capacity Pcap.  Both take the select's scratch.
-size_t prune_scratch_bytes(uint32_t P);
-int launch_prune_select(uint32_t P, uint32_t n_sky, const float* opacity_logit, float min_opacity, void* scratch, uint32_t* result_host,
-                        cudaStream_t s);
-int launch_prune_gather(const float* src, float* dst, uint32_t Pcap, int M, uint32_t P_old, uint32_t P_new, const void* scratch, cudaStream_t s);
-// the select's index map: idx[new] = old for the P_new kept rows
-const uint32_t* prune_index(const void* scratch, uint32_t P);
-// dst[r] = r < rows_valid ? src[idx[r]] : 0 for r < rows_out (one 32-bit word per row)
-int launch_gather_words(const void* src, void* dst, uint32_t rows_out, uint32_t rows_valid, const uint32_t* idx, cudaStream_t s);
-// output rows [0, rows_out) of every group of dst: row r < rows_valid takes row idx[r] of src, the others are zero
-int launch_gather_rows(const float* src, float* dst, uint32_t Pcap, int M, uint32_t rows_out, uint32_t rows_valid, const uint32_t* idx,
-                       cudaStream_t s);
-// densify-and-prune (prune.cu, glic_mapper_densify_and_prune): the selection's inputs (device pointers of rows [0, P)) and
-// parameters, as the header states them
+// stable compaction of the arenas (prune.cu): glic_mapper_densify_and_prune, glic_mapper_densify (nothing removed) and
+// glic_mapper_prune (nothing selected) select once and gather every arena by the selection's index map.
+// The selection's inputs (device pointers of rows [0, P)) and parameters, as the header states them
 struct DensitySelect {
     uint32_t P, n_sky;
-    const float *accum, *denom, *log_scale, *logit;
+    const float *accum, *denom;      // both null: no row is selected (class 0 for every row), and neither is read
+    const float *log_scale, *logit;  // log_scale is read only for a selected row, or when max_world_scale > 0
     const int* maxr;                 // read only when max_screen_radius > 0
     float grad_threshold, clone_max, min_opacity, max_world_scale;
     int max_screen_radius;
 };
 // select: the fate of every row; result_host[6] = {clones, splits, surviving kept rows, surviving clones, surviving split rows,
-// surviving sky rows}, synchronises s; the scratch then holds the index map of the surviving rows (density_index) and the
-// children's keys.  children: rows [first, first + 2 n) of the arena, copies of the n surviving split rows' parents, become
-// their children in place (xyz and log-scale); P_select is the P the selection ran on, n_split its splits.
+// surviving sky rows}, synchronises s; the scratch then holds the index map of the surviving rows (density_index: idx[new] = old)
+// and the children's keys.  children: rows [first, first + 2 n) of the arena, copies of the n surviving split rows' parents,
+// become their children in place (xyz and log-scale); P_select is the P the selection ran on, n_split its splits.
 size_t density_scratch_bytes(uint32_t P);
 int launch_density_select(const DensitySelect& a, void* scratch, uint32_t* result_host, cudaStream_t s);
 const uint32_t* density_index(const void* scratch, uint32_t P);
 int launch_densify_children(float* params, uint32_t Pcap, int M, uint32_t first, uint32_t n, const void* scratch, uint32_t P_select,
                             uint32_t n_split, uint64_t seed, uint64_t call, cudaStream_t s);
+// output rows [0, rows_out) of every group of dst: row r < rows_valid takes row idx[r] of src, the others are zero; src and dst
+// are arenas of capacity Pcap
+int launch_gather_rows(const float* src, float* dst, uint32_t Pcap, int M, uint32_t rows_out, uint32_t rows_valid, const uint32_t* idx,
+                       cudaStream_t s);
+// dst[r] = r < rows_valid ? src[idx[r]] : 0 for r < rows_out (one 32-bit word per row)
+int launch_gather_words(const void* src, void* dst, uint32_t rows_out, uint32_t rows_valid, const uint32_t* idx, cudaStream_t s);
 // glic_mapper_reset_opacity on rows [first, P) of the opacity group of the three arenas
 int launch_reset_opacity(uint32_t first, uint32_t P, uint32_t Pcap, int M, float* params, float* m1, float* m2, float max_opacity,
                          float reset_logit, cudaStream_t s);

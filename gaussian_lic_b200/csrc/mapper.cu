@@ -1318,60 +1318,6 @@ int glic_mapper_download(glic_mapper* m, float* xyz, float* f_dc, float* f_rest,
     return GLIC_OK;
 }
 
-// Stable compaction (prune.cu): select the kept rows, then gather each arena into a spare one of the same capacity and swap.
-// The spare is allocated once, before anything changes, and rotates: params -> spare, the old params buffer then takes m1, the
-// old m1 buffer m2, and the old m2 buffer is freed.  Peak extra memory: one arena (glic_packed_floats(Pcap, M) floats); the
-// selection's scratch (4 B per row) lives in the extend() staging buffer, which keeps it.  The gather writes output rows
-// [0, P_old); rows [P_old, Pcap) of every arena are zero already (allocation, initialize, append and regrow keep them so), so
-// the vacated rows end up zero like them.
-int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, uint32_t* removed) {
-    if (!m) { set_error("mapper_prune: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!std::isfinite(min_opacity) || min_opacity < 0.0f || min_opacity > 1.0f) {
-        set_error("mapper_prune: min_opacity must be finite and in [0, 1]"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    MAP_TRY(poll_ring(m, true));
-    const uint32_t P = m->P;
-    if (P == 0) {
-        if (removed) *removed = 0;
-        return GLIC_OK;
-    }
-    cudaStream_t s = m->stream;
-    MAP_TRY(reserve(m, m->extend_ws, prune_scratch_bytes(P)));  // the selection's scratch: the idle extend() staging
-    void* scratch = m->extend_ws;
-    float* g[6];
-    arena_ptrs(m, m->params, m->Pcap, g);
-    uint32_t kept[2] = {0, 0};
-    MAP_TRY(launch_prune_select(P, m->n_sky, g[3], min_opacity, scratch, kept, s));
-    if (kept[0] == 0) { set_error("mapper_prune: the threshold removes every row (an empty map cannot be trained)"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!dry_run && kept[0] < P) {
-        Dev<float> spare, spare_stats[3];
-        const size_t bytes = arena_floats(m, m->Pcap) * sizeof(float);
-        MAP_TRY(spare.allocate(bytes));
-        if (m->dens_on)                                    // the statistics move with their rows (and their spares are zero)
-            for (Dev<float>& b : spare_stats) MAP_TRY(b.allocate((size_t)m->Pcap * 4));
-        GLIC_CUDA_TRY(cudaMemsetAsync(spare, 0, bytes, s));
-        for (Dev<float>* arena : {&m->params, &m->m1, &m->m2}) {
-            MAP_TRY(launch_prune_gather(*arena, spare, m->Pcap, m->M, P, kept[0], scratch, s));
-            std::swap(*arena, spare);
-        }
-        if (m->dens_on) {
-            Buf* stats[3] = {&m->dens_accum, &m->dens_denom, &m->dens_maxr};
-            for (int q = 0; q < 3; ++q) {
-                GLIC_CUDA_TRY(cudaMemsetAsync(spare_stats[q], 0, (size_t)m->Pcap * 4, s));
-                MAP_TRY(launch_gather_words(stats[q]->raw(), spare_stats[q], P, kept[0], prune_index(scratch, P), s));
-                std::swap(*stats[q], static_cast<Buf&>(spare_stats[q]));
-            }
-        }
-        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-        m->P = kept[0];
-        m->n_sky = kept[1];
-        m->st.num_gaussians = kept[0];
-    }
-    if (removed) *removed = P - kept[0];
-    return GLIC_OK;
-}
-
 int glic_mapper_enable_densification(glic_mapper* m) {
     if (!m) { set_error("mapper_enable_densification: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (m->dens_on) return GLIC_OK;
@@ -1395,11 +1341,21 @@ int glic_mapper_enable_densification(glic_mapper* m) {
 
 namespace {
 
-// glic_mapper_densify_and_prune (glic_mapper_densify: min_opacity 0, both size tests off) as one compaction (prune.cu): select,
-// reserve (capacity, then one spare arena), gather every arena into the spare in rotation as prune does (the moments keep only
-// the kept rows: the new rows' moments are zero), write the children's xyz and log-scale, zero the statistics.  The caller has
-// validated p.  reject_empty: a result without rows is an error (densify on an empty map is not).
-int density_step(glic_mapper* m, const glic_density_params& p, int dry_run, bool reject_empty, glic_density_counts* out, const char* what) {
+// The one stable compaction of the arenas (prune.cu), behind glic_mapper_densify_and_prune, glic_mapper_densify (min_opacity 0,
+// both size tests off) and glic_mapper_prune (no row selected, both size tests off): select, reserve (capacity, then the
+// spares), gather each arena into a spare one of the same capacity and swap, write the children's xyz and log-scale.  The
+// spare is allocated once, before anything changes, and rotates: params -> spare, the old params buffer then takes m1, the old
+// m1 buffer m2, and the old m2 buffer is freed.  Peak extra memory: one arena (glic_packed_floats(Pcap, M) floats); the
+// selection's scratch (12 B per row and five counts per 1024 rows) lives in the extend() staging buffer, which keeps it.  The
+// params gather takes every result row, the moments only the kept rows (the new rows' moments are zero), and each writes output
+// rows [0, max(rows, P)): rows [P, Pcap) of every arena are zero already (allocation, initialize, append and regrow keep them
+// so), so the rows a prune vacates end up zero like them.
+// densify: the call densifies, so it selects by the statistics, zeroes them and advances dens_calls even when no row changes.
+// Otherwise it only prunes: no statistic is read, the statistics (with densification on) move with their rows, dens_calls
+// stays (it keys the children's draws of every later densify), and a call that removes nothing touches nothing.
+// The caller has validated p.  reject_empty: a result without rows is an error (densify on an empty map is not).
+int density_step(glic_mapper* m, const glic_density_params& p, bool densify, int dry_run, bool reject_empty, glic_density_counts* out,
+                 const char* what) {
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     MAP_TRY(poll_ring(m, true));
     const uint32_t P = m->P;
@@ -1409,8 +1365,9 @@ int density_step(glic_mapper* m, const glic_density_params& p, int dry_run, bool
         MAP_TRY(reserve(m, m->extend_ws, density_scratch_bytes(P)));   // the selection's scratch: the idle extend() staging
         float* g[6];
         arena_ptrs(m, m->params, m->Pcap, g);
-        const DensitySelect a{P, m->n_sky, m->dens_accum, m->dens_denom, g[2], g[3], m->dens_maxr, p.grad_threshold,
-                              p.percent_dense * p.scene_extent, p.min_opacity, p.max_world_scale, p.max_screen_radius};
+        const float* no_stats = nullptr;                   // a prune selects no row, with densification on or off
+        const DensitySelect a{P, m->n_sky, densify ? m->dens_accum : no_stats, densify ? m->dens_denom : no_stats, g[2], g[3], m->dens_maxr,
+                              p.grad_threshold, p.percent_dense * p.scene_extent, p.min_opacity, p.max_world_scale, p.max_screen_radius};
         MAP_TRY(launch_density_select(a, m->extend_ws, r, s));
     }
     const uint32_t n_clone = r[0], n_split = r[1], kept = r[2], cloned = r[3], split = r[4];
@@ -1427,9 +1384,12 @@ int density_step(glic_mapper* m, const glic_density_params& p, int dry_run, bool
             }
             MAP_TRY(set_capacity(m, std::max<uint32_t>((uint32_t)rows, 2 * m->Pcap)));
         }
-        Dev<float> spare;
+        Dev<float> spare, spare_stats[3];
+        const bool move_stats = !densify && m->dens_on;
         const size_t bytes = arena_floats(m, m->Pcap) * sizeof(float);
         MAP_TRY(spare.allocate(bytes));
+        if (move_stats)
+            for (Dev<float>& b : spare_stats) MAP_TRY(b.allocate((size_t)m->Pcap * 4));
         GLIC_CUDA_TRY(cudaMemsetAsync(spare, 0, bytes, s));
         const uint32_t* idx = density_index(m->extend_ws, P);
         const uint32_t written = std::max<uint32_t>((uint32_t)rows, P);   // the rows a prune vacates become zero
@@ -1438,14 +1398,22 @@ int density_step(glic_mapper* m, const glic_density_params& p, int dry_run, bool
             std::swap(*arena, spare);
         }
         MAP_TRY(launch_densify_children(m->params, m->Pcap, m->M, kept + cloned, split, m->extend_ws, P, n_split, m->cfg.seed, m->dens_calls, s));
+        if (move_stats) {                                  // the statistics move with their rows (and their spares are zero)
+            Buf* stats[3] = {&m->dens_accum, &m->dens_denom, &m->dens_maxr};
+            for (int q = 0; q < 3; ++q) {
+                GLIC_CUDA_TRY(cudaMemsetAsync(spare_stats[q], 0, (size_t)m->Pcap * 4, s));
+                MAP_TRY(launch_gather_words(stats[q]->raw(), spare_stats[q], written, kept, idx, s));
+                std::swap(*stats[q], static_cast<Buf&>(spare_stats[q]));
+            }
+        }
         m->P = (uint32_t)rows;
         m->n_sky = r[5];
         m->st.num_gaussians = m->P;
     }
     if (!dry_run) {
-        MAP_TRY(dens_reset(m));                                    // densification_postfix: the statistics start again
+        if (densify) MAP_TRY(dens_reset(m));                       // densification_postfix: the statistics start again
         GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-        ++m->dens_calls;
+        if (densify) ++m->dens_calls;
     }
     if (out) *out = glic_density_counts{n_clone, n_split, (uint32_t)(unpruned - rows), (uint32_t)rows};
     return GLIC_OK;
@@ -1509,6 +1477,18 @@ bool finite_at_least_zero(float x) { return std::isfinite(x) && x >= 0.0f; }
 
 extern "C" {
 
+// the compaction with no row selected and both size tests off; a mapper with no rows has nothing to remove (0, not an error)
+int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, uint32_t* removed) {
+    if (!m) { set_error("mapper_prune: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!std::isfinite(min_opacity) || min_opacity < 0.0f || min_opacity > 1.0f) {
+        set_error("mapper_prune: min_opacity must be finite and in [0, 1]"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    glic_density_counts k{};
+    MAP_TRY(density_step(m, glic_density_params{0.0f, 0.0f, 0.0f, min_opacity, 0, 0.0f}, false, dry_run, m->P != 0, &k, "mapper_prune"));
+    if (removed) *removed = k.pruned;
+    return GLIC_OK;
+}
+
 int glic_mapper_densify(glic_mapper* m, float grad_threshold, float percent_dense, float scene_extent, int dry_run, uint32_t* cloned,
                         uint32_t* split) {
     if (!m) { set_error("mapper_densify: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
@@ -1518,7 +1498,7 @@ int glic_mapper_densify(glic_mapper* m, float grad_threshold, float percent_dens
         return GLIC_ERR_INVALID_ARGUMENT;
     }
     glic_density_counts k{};
-    MAP_TRY(density_step(m, glic_density_params{grad_threshold, percent_dense, scene_extent, 0.0f, 0, 0.0f}, dry_run, false, &k, "mapper_densify"));
+    MAP_TRY(density_step(m, glic_density_params{grad_threshold, percent_dense, scene_extent, 0.0f, 0, 0.0f}, true, dry_run, false, &k, "mapper_densify"));
     if (cloned) *cloned = k.cloned;
     if (split) *split = k.split;
     return GLIC_OK;
@@ -1534,7 +1514,7 @@ int glic_mapper_densify_and_prune(glic_mapper* m, const glic_density_params* p, 
                   "and > 0, min_opacity in [0, 1], max_screen_radius >= 0");
         return GLIC_ERR_INVALID_ARGUMENT;
     }
-    return density_step(m, *p, dry_run, true, out, "mapper_densify_and_prune");
+    return density_step(m, *p, true, dry_run, true, out, "mapper_densify_and_prune");
 }
 
 int glic_mapper_screen_radii(glic_mapper* m, int32_t* out) {

@@ -1,30 +1,25 @@
-// prune.cu -- stable compaction of the mapper's arenas (glic_mapper_prune): every row whose activated opacity is below a
-// threshold is removed, the survivors keep their relative order, and all six parameter groups and both Adam moments move with
-// them bit for bit.  No CUB:
-//   1. prune_count_kernel: one CTA per tile of PRUNE_TILE rows counts the rows it keeps;
-//   2. prune_scan_kernel:  one CTA scans the per-tile counts (a two-level scan: rows within a tile in step 3, tiles here; at
-//      1024 rows per tile a 2 M-row map has 2048 tile counts) into tile offsets and the kept total;
-//   3. prune_index_kernel: each tile places its kept rows at their new index: idx[new] = old, and the new index of row n_sky,
-//      i.e. the number of kept rows before it (the surviving sky rows);
-//   4. prune_gather_kernel: per arena, one launch over all six groups writes output rows [0, P_old) of each group: row r < P_new
-//      takes source row idx[r], rows [P_new, P_old) become zero.  Each thread writes one float4 of a group (16-byte aligned:
-//      group offsets are multiples of Pcap floats, Pcap a multiple of 256); its four source floats are consecutive whenever
-//      their rows are, so loads coalesce across a run of kept rows.
-// The keep decision is opacity_activation(logit) >= min_opacity, the activation kernel's own expression (common.cuh).
-//
-// Densification (glic_mapper_densify_and_prune, and glic_mapper_densify, which is its case without a prune) is a five-way
-// version of the same compaction.  Each row is kept, cloned (kept and copied once) or split (replaced by two children), and
-// each of the rows it leaves in the densify result survives the prune predicate or not (row_fate):
-//   1. fate_count_kernel: per tile, the clones and the splits, and the survivors of each kind;
-//   2. prune_scan_kernel, one CTA per count: tile offsets and the five totals;
+// prune.cu -- the one stable compaction of the mapper's arenas, behind glic_mapper_prune, glic_mapper_densify and
+// glic_mapper_densify_and_prune.  Each row is kept, cloned (kept and copied once) or split (replaced by two children), and each
+// of the rows it leaves in the densify result survives the prune predicate or not (row_fate).  The survivors keep their relative
+// order, and all six parameter groups and both Adam moments move with them bit for bit.  glic_mapper_densify is the case without
+// a prune; glic_mapper_prune is the case in which no row is selected (no statistics are given, and none are read) and both
+// size tests are off, so a row's fate is its logit's alone.  No CUB:
+//   1. fate_count_kernel: one CTA per tile of PRUNE_TILE rows counts its clones and splits, and the survivors of each kind;
+//   2. prune_scan_kernel, one CTA per count: scans the per-tile counts (a two-level scan: rows within a tile in step 3, tiles
+//      here; at 1024 rows per tile a 2 M-row map has 2048 tile counts) into tile offsets and the five totals;
 //   3. fate_index_kernel: idx[new] = old for the surviving kept rows (rows that are not split, in order), then the surviving
 //      clones, then the first child of every surviving split row, then the second; the children's rows start as copies of their
-//      parent, and each child's key is the row it has in the densify result before the prune;
-//   4. prune_gather_kernel per arena (the moments take only the kept rows; every new row gets zero moments);
+//      parent, and each child's key is the row it has in the densify result before the prune.  It also finds the new index of
+//      row n_sky, i.e. the number of kept rows before it (the surviving sky rows);
+//   4. prune_gather_kernel: per arena, one launch over all six groups writes output rows [0, rows_out) of each group: row
+//      r < rows_valid takes source row idx[r], the others become zero (the rows a prune vacates; for the moments, every new
+//      row).  Each thread writes one float4 of a group (16-byte aligned: group offsets are multiples of Pcap floats, Pcap a
+//      multiple of 256); its four source floats are consecutive whenever their rows are, so loads coalesce across a run of
+//      kept rows;
 //   5. densify_children_kernel: each child row, a copy of its parent, gets its own xyz (drawn at its key) and the parent's
 //      log-scale - log(1.6).
-// The decisions use the activation kernel's expf (scale_activation) and the child geometry its normalisation
-// (rotation_activation); glic_densify_split evaluates the same child geometry on its own.
+// The decisions use the activation kernel's own expressions (opacity_activation, scale_activation: common.cuh) and the child
+// geometry its normalisation (rotation_activation); glic_densify_split evaluates the same child geometry on its own.
 #include "common.cuh"
 
 namespace glic {
@@ -33,40 +28,6 @@ namespace {
 constexpr int PRUNE_THREADS = 256;
 constexpr int PRUNE_ROWS = 4;                                  // consecutive rows per thread
 constexpr uint32_t PRUNE_TILE = PRUNE_THREADS * PRUNE_ROWS;    // rows per CTA of the count and index passes
-
-// the keep flags of this thread's rows [r0, r0 + 4): a float4 load when all four exist (r0 is a multiple of 4, the group
-// offset a multiple of Pcap floats)
-__device__ __forceinline__ void keep_flags(uint32_t P, const float* __restrict__ logit, float min_opacity, uint32_t r0, bool keep[PRUNE_ROWS]) {
-    float l[PRUNE_ROWS];
-    if (r0 + PRUNE_ROWS <= P) {
-        const float4 v = *reinterpret_cast<const float4*>(logit + r0);
-        l[0] = v.x; l[1] = v.y; l[2] = v.z; l[3] = v.w;
-    } else {
-#pragma unroll
-        for (int e = 0; e < PRUNE_ROWS; ++e) l[e] = r0 + e < P ? logit[r0 + e] : 0.0f;
-    }
-#pragma unroll
-    for (int e = 0; e < PRUNE_ROWS; ++e) keep[e] = r0 + e < P && !(opacity_activation(l[e]) < min_opacity);
-}
-
-__global__ void __launch_bounds__(PRUNE_THREADS)
-prune_count_kernel(uint32_t P, const float* __restrict__ logit, float min_opacity, uint32_t* __restrict__ tile_count) {
-    bool keep[PRUNE_ROWS];
-    keep_flags(P, logit, min_opacity, blockIdx.x * PRUNE_TILE + PRUNE_ROWS * threadIdx.x, keep);
-    int n = 0;
-#pragma unroll
-    for (int e = 0; e < PRUNE_ROWS; ++e) n += keep[e];
-    __shared__ int warp_n[PRUNE_THREADS / 32];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
-    if ((threadIdx.x & 31) == 0) warp_n[threadIdx.x >> 5] = n;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int t = 0;
-        for (int w = 0; w < PRUNE_THREADS / 32; ++w) t += warp_n[w];
-        tile_count[blockIdx.x] = (uint32_t)t;
-    }
-}
 
 // exclusive scan of the tile counts in place, the total into *total; CTA b scans the b-th of consecutive arrays of n_tiles
 // counts into total[b]
@@ -107,37 +68,6 @@ __global__ void __launch_bounds__(1024) prune_scan_kernel(uint32_t n_tiles, uint
         __syncthreads();
     }
     if (tid == 0) *total = carry;
-}
-
-// idx[new] = old for every kept row; *sky_new = the new index of row n_sky (written only when n_sky < P)
-__global__ void __launch_bounds__(PRUNE_THREADS)
-prune_index_kernel(uint32_t P, const float* __restrict__ logit, float min_opacity, const uint32_t* __restrict__ tile_offset, uint32_t n_sky,
-                   uint32_t* __restrict__ idx, uint32_t* __restrict__ sky_new) {
-    const uint32_t r0 = blockIdx.x * PRUNE_TILE + PRUNE_ROWS * threadIdx.x;
-    bool keep[PRUNE_ROWS];
-    keep_flags(P, logit, min_opacity, r0, keep);
-    uint32_t n = 0;
-#pragma unroll
-    for (int e = 0; e < PRUNE_ROWS; ++e) n += keep[e];
-    // exclusive scan of n over the CTA, in thread (= row) order
-    __shared__ uint32_t warp_tot[PRUNE_THREADS / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t incl = n;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += t;
-    }
-    if (lane == 31) warp_tot[warp] = incl;
-    __syncthreads();
-    uint32_t before = 0;
-    for (int w = 0; w < warp; ++w) before += warp_tot[w];
-    uint32_t pos = tile_offset[blockIdx.x] + before + incl - n;
-#pragma unroll
-    for (int e = 0; e < PRUNE_ROWS; ++e) {
-        if (r0 + e == n_sky) *sky_new = pos;
-        if (keep[e]) idx[pos++] = r0 + e;
-    }
 }
 
 struct GatherPlan {
@@ -190,40 +120,6 @@ prune_gather_kernel(const float* __restrict__ src, float* __restrict__ dst, cons
 
 }  // namespace
 
-size_t prune_scratch_bytes(uint32_t P) {
-    const uint32_t tiles = (P + PRUNE_TILE - 1) / PRUNE_TILE;
-    return 256 + (((size_t)tiles * 4 + 255) & ~size_t(255)) + (size_t)P * 4;
-}
-
-// scratch: result[2] = {P_new, sky_new} (256 bytes) | tile counts | idx[P]
-int launch_prune_select(uint32_t P, uint32_t n_sky, const float* opacity_logit, float min_opacity, void* scratch, uint32_t* result_host,
-                        cudaStream_t s) {
-    const uint32_t tiles = (P + PRUNE_TILE - 1) / PRUNE_TILE;
-    uint32_t* result = static_cast<uint32_t*>(scratch);
-    uint32_t* tile = reinterpret_cast<uint32_t*>(static_cast<char*>(scratch) + 256);
-    uint32_t* idx = reinterpret_cast<uint32_t*>(static_cast<char*>(scratch) + 256 + (((size_t)tiles * 4 + 255) & ~size_t(255)));
-    GLIC_CUDA_TRY(cudaMemsetAsync(result, 0, 2 * sizeof(uint32_t), s));
-    prune_count_kernel<<<tiles, PRUNE_THREADS, 0, s>>>(P, opacity_logit, min_opacity, tile);
-    GLIC_LAUNCH_CHECK();
-    prune_scan_kernel<<<1, 1024, 0, s>>>(tiles, tile, result);
-    GLIC_LAUNCH_CHECK();
-    prune_index_kernel<<<tiles, PRUNE_THREADS, 0, s>>>(P, opacity_logit, min_opacity, tile, n_sky, idx, result + 1);
-    GLIC_LAUNCH_CHECK();
-    GLIC_CUDA_TRY(cudaMemcpyAsync(result_host, result, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-    if (n_sky >= P) result_host[1] = result_host[0];            // every row is sky: the survivors are
-    return GLIC_OK;
-}
-
-const uint32_t* prune_index(const void* scratch, uint32_t P) {
-    const uint32_t tiles = (P + PRUNE_TILE - 1) / PRUNE_TILE;
-    return reinterpret_cast<const uint32_t*>(static_cast<const char*>(scratch) + 256 + (((size_t)tiles * 4 + 255) & ~size_t(255)));
-}
-
-int launch_prune_gather(const float* src, float* dst, uint32_t Pcap, int M, uint32_t P_old, uint32_t P_new, const void* scratch, cudaStream_t s) {
-    return launch_gather_rows(src, dst, Pcap, M, P_old, P_new, prune_index(scratch, P_old), s);
-}
-
 int launch_gather_rows(const float* src, float* dst, uint32_t Pcap, int M, uint32_t P_old, uint32_t P_new, const uint32_t* idx,
                        cudaStream_t s) {
     GatherPlan g;
@@ -251,6 +147,7 @@ constexpr float SPLIT_LOG_SCALE = 0x1.e148a2p-2f;              // (float)log(1.6
 // predicate: the row itself (kept or cloned), its clone, its two children (one logit and one log-scale: one fate).  The
 // predicate: act(logit) < min_opacity, or (non-sky rows) maxr > max_screen_radius > 0, or largest scale > max_world_scale > 0.
 // Clones and children have maxr 0, and the children's scale is their own (the parent's log-scale - log(1.6)).
+// Without statistics (a.accum null) no row is selected; then, with both size tests off, a row's logit is all that is read.
 constexpr unsigned FATE_ROW = 4u, FATE_CLONE = 8u, FATE_CHILDREN = 16u;
 
 __device__ __forceinline__ float largest_scale(const float* ls) {
@@ -264,9 +161,12 @@ __device__ __forceinline__ unsigned row_fate(uint32_t r, const DensitySelect& a)
     unsigned cls = 0;
     float smax = 0.0f;
     if (!sky) {
-        const float d = a.denom[r];
-        const float grad = d > 0.0f ? __fdiv_rn(a.accum[r], d) : 0.0f;
-        if (grad >= a.grad_threshold) {
+        bool selected = false;
+        if (a.accum) {
+            const float d = a.denom[r];
+            selected = (d > 0.0f ? __fdiv_rn(a.accum[r], d) : 0.0f) >= a.grad_threshold;
+        }
+        if (selected) {
             smax = largest_scale(ls);
             cls = smax <= a.clone_max ? 1u : 2u;
         } else if (world) {
@@ -474,29 +374,40 @@ reset_opacity_kernel(uint32_t first, uint32_t P, float* __restrict__ logit, floa
     m2[r] = 0.0f;
 }
 
-// scratch: totals[6] (256 bytes) | 5 arrays of tile counts | idx[2P] | key[P]
-size_t tile_bytes(uint32_t P) { return (((size_t)(P + PRUNE_TILE - 1) / PRUNE_TILE) * 4 + 255) & ~size_t(255); }
+// The selection's scratch for P rows, as byte offsets: totals[6] (256 bytes) | 5 arrays of `tiles` counts | idx[2P] | key[P]
+struct ScratchLayout {
+    uint32_t tiles;
+    size_t tile, idx, key, bytes;
+    explicit ScratchLayout(uint32_t P) : tiles((P + PRUNE_TILE - 1) / PRUNE_TILE) {
+        tile = 256;
+        idx = tile + 5 * (((size_t)tiles * 4 + 255) & ~size_t(255));
+        key = idx + (size_t)P * 8;
+        bytes = key + (size_t)P * 4;
+    }
+};
 
 }  // namespace
 
-size_t density_scratch_bytes(uint32_t P) { return 256 + 5 * tile_bytes(P) + (size_t)P * 12; }
+size_t density_scratch_bytes(uint32_t P) { return ScratchLayout(P).bytes; }
 
 const uint32_t* density_index(const void* scratch, uint32_t P) {
-    return reinterpret_cast<const uint32_t*>(static_cast<const char*>(scratch) + 256 + 5 * tile_bytes(P));
+    return reinterpret_cast<const uint32_t*>(static_cast<const char*>(scratch) + ScratchLayout(P).idx);
 }
 
 int launch_density_select(const DensitySelect& a, void* scratch, uint32_t* result_host, cudaStream_t s) {
-    const uint32_t tiles = (a.P + PRUNE_TILE - 1) / PRUNE_TILE;
+    const ScratchLayout l(a.P);
+    const uint32_t tiles = l.tiles;
     char* base = static_cast<char*>(scratch);
     uint32_t* totals = reinterpret_cast<uint32_t*>(base);
-    uint32_t* tile = reinterpret_cast<uint32_t*>(base + 256);          // 5 arrays of `tiles` counts, within 5 * tile_bytes(P)
-    uint32_t* idx = const_cast<uint32_t*>(density_index(scratch, a.P));
+    uint32_t* tile = reinterpret_cast<uint32_t*>(base + l.tile);
+    uint32_t* idx = reinterpret_cast<uint32_t*>(base + l.idx);
+    uint32_t* key = reinterpret_cast<uint32_t*>(base + l.key);
     GLIC_CUDA_TRY(cudaMemsetAsync(totals + 5, 0, sizeof(uint32_t), s));
     fate_count_kernel<<<tiles, PRUNE_THREADS, 0, s>>>(a, tiles, tile);
     GLIC_LAUNCH_CHECK();
     prune_scan_kernel<<<5, 1024, 0, s>>>(tiles, tile, totals);
     GLIC_LAUNCH_CHECK();
-    fate_index_kernel<<<tiles, PRUNE_THREADS, 0, s>>>(a, tiles, tile, totals, idx, idx + 2 * (size_t)a.P);
+    fate_index_kernel<<<tiles, PRUNE_THREADS, 0, s>>>(a, tiles, tile, totals, idx, key);
     GLIC_LAUNCH_CHECK();
     GLIC_CUDA_TRY(cudaMemcpyAsync(result_host, totals, 6 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     GLIC_CUDA_TRY(cudaStreamSynchronize(s));
@@ -509,7 +420,7 @@ int launch_densify_children(float* params, uint32_t Pcap, int M, uint32_t first,
     if (n == 0) return GLIC_OK;
     size_t off[6];
     glic_packed_offsets(Pcap, (uint32_t)M, off);
-    const uint32_t* key = density_index(scratch, P_select) + 2 * (size_t)P_select;
+    const uint32_t* key = reinterpret_cast<const uint32_t*>(static_cast<const char*>(scratch) + ScratchLayout(P_select).key);
     densify_children_kernel<<<(2 * n + 255) / 256, 256, 0, s>>>(params, off[0], off[1], off[2], first, n, key, n_split, seed, call);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
