@@ -67,6 +67,18 @@ class DensitySchedule(C.Structure):
                 ("world_scale_factor", C.c_float), ("scene_extent", C.c_float)]
 
 
+class AlignParams(C.Structure):
+    _fields_ = [("iterations", C.c_int), ("lr_translation", C.c_float), ("lr_rotation", C.c_float), ("exposure_lr", C.c_float),
+                ("split", C.c_int)]
+
+
+class AlignResult(C.Structure):
+    _fields_ = [("R_wc", C.c_float * 9), ("t_wc", C.c_float * 3), ("E", C.c_float * 12), ("psnr", C.c_float), ("ssim", C.c_float),
+                ("lpips", C.c_float), ("first_loss", C.c_float), ("last_loss", C.c_float), ("pose_exp_avg", C.c_float * 6),
+                ("pose_exp_avg_sq", C.c_float * 6), ("expo_exp_avg", C.c_float * 12), ("expo_exp_avg_sq", C.c_float * 12),
+                ("steps", C.c_int), ("skipped", C.c_int)]
+
+
 def _load():
     if not os.path.isfile(LIB_PATH):
         raise ImportError(
@@ -180,6 +192,7 @@ def _load():
         "glic_mapper_pose_get": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32), C.POINTER(f32)]),
         "glic_mapper_pose_set": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32)]),
         "glic_mapper_pose_adam_state": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32), C.POINTER(i32)]),
+        "glic_mapper_align": (i32, [vp, i32, i32, C.POINTER(AlignParams), C.POINTER(AlignResult), vp]),
         "glic_mapper_enable_frames": (i32, [vp, i32, i32, i32]),
         "glic_mapper_add_frame": (i32, [vp, C.POINTER(Frame), C.POINTER(i32)]),
         "glic_mapper_keyframe_image": (i32, [vp, i32, i32, vp]),
@@ -189,6 +202,8 @@ def _load():
         "glic_debug_image": (i32, [i32, i32, vp, vp, vp, vp, vp, C.POINTER(i64), vp]),
         "glic_debug_spans": (i32, [i32, vp, C.POINTER(u32), vp]),
         "glic_debug_render_backward": (i32, [i32, C.POINTER(View), i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, vp]),
+        "glic_debug_pose_backward": (i32, [i32, i32, i32, vp, vp, vp, vp, vp, vp, C.POINTER(View), vp, vp, vp, vp, vp, vp, i32, vp,
+                                           vp, vp, vp]),
         "glic_debug_fail_allocation": (i32, [i32]),
         "glic_debug_mapper_allocations": (i64, []),
     }

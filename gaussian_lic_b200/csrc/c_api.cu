@@ -371,6 +371,31 @@ int glic_backward_compact_internal(int P, int sh_degree, int M, const float* mea
                                               dL_dconic, dL_dcolors, *cg, s);
 }
 
+int glic_debug_pose_backward(int P, int sh_degree, int M, const float* means3D, const float* scales, const float* rotations,
+                             const float* rot_raw, const float* opacity, const float* sh, const glic_view* view, const int* radii,
+                             const void* geom_ws, const float* dL_dmeans2D, const float* dL_dconic, const float* dL_dopacity,
+                             const float* dL_dcolors, int pose_only, float* g_geo, void* partials, float* pose6, void* stream) {
+    if (int e = check_view(view)) return e;
+    if (P <= 0 || !means3D || !scales || !rotations || !radii || !geom_ws || !dL_dmeans2D || !dL_dconic || !dL_dcolors || !partials ||
+        !pose6 || (!pose_only && (!g_geo || !rot_raw || !opacity || !dL_dopacity))) {
+        set_error("debug_pose_backward: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    CompactGrads cg{};
+    if (!pose_only) {                                   // the mapper's compact block: rotation | xyz | log-scale | opacity logit
+        cg.g_rot = reinterpret_cast<float4*>(g_geo);
+        cg.g_xyz = g_geo + 4 * (size_t)P;
+        cg.g_scale = g_geo + 7 * (size_t)P;
+        cg.g_opacity = g_geo + 10 * (size_t)P;
+        cg.opacity = opacity; cg.dL_dopacity = dL_dopacity; cg.rot_raw = reinterpret_cast<const float4*>(rot_raw);
+    }
+    cg.pose_partials = static_cast<double*>(partials);
+    cg.pose_grad = pose6;
+    StageTimer _t(GLIC_STAGE_PREPROCESS_BWD, (cudaStream_t)stream);
+    return launch_preprocess_backward_compact(P, sh_degree, M, means3D, scales, 1.0f, rotations, sh, make_view_params(view), radii,
+                                              GeomState::carve(const_cast<void*>(geom_ws), P), dL_dmeans2D, dL_dconic, dL_dcolors, cg,
+                                              (cudaStream_t)stream);
+}
+
 int glic_sort_pairs_u64_u32(int64_t n, int end_bit, uint64_t* keys_in, uint32_t* vals_in, uint64_t* keys_out,
                             uint32_t* vals_out, void* temp, size_t temp_bytes, void* stream) {
     if (n < 0 || (n > 0 && (!keys_in || !vals_in || !keys_out || !vals_out || !temp))) { set_error("sort_pairs: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }

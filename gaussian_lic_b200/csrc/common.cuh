@@ -280,7 +280,9 @@ inline ViewParams make_view_params(const glic_view* v) {
     return p;
 }
 
-// Compact gradient outputs of the per-Gaussian backward (the mapper's form, see preprocess_backward.cu).
+// Compact gradient outputs of the per-Gaussian backward (the mapper's form, see preprocess_backward.cu).  Null row pointers
+// (g_xyz == NULL) with the two pose pointers set select the pose-only form: the view's pose gradient and nothing per row (the
+// other row inputs and the densification pointers are then not read and must be NULL).
 struct CompactGrads {
     float4* g_rot;            // [P] dL/d(raw rotation)
     float* g_xyz;             // [P,3]

@@ -22,6 +22,7 @@
 #include <cstring>
 #include <functional>
 #include <initializer_list>
+#include <limits>
 #include <memory>
 #include <nv/target>
 #include <random>
@@ -375,6 +376,8 @@ struct glic_mapper {
     // ---- LPIPS of the evaluation (glic_mapper_load_lpips): weight payload and glic_lpips's scratch, sized on first use ----
     Dev<float> lpips_w;
     Dev<void> lpips_scratch;
+    // ---- test-time alignment (glic_mapper_align): its workspace (align_carve), sized on first use ----
+    Dev<char> align_ws;
     // ---- raw frames (glic_mapper_enable_frames / add_frame): the 8-bit image store, chunks of FRAME_CHUNK frames of
     //      frame_stride bytes that never move, and the scan of the frames since the last training keyframe (device arrays
     //      of scan_cap points, grown by doubling) ----
@@ -1473,6 +1476,200 @@ int scheduled_density_step(glic_mapper* m) {
 
 bool finite_at_least_zero(float x) { return std::isfinite(x) && x >= 0.0f; }
 
+// ---- test-time alignment (glic_mapper_align) ------------------------------------------------------------------------------
+// The call's one-row state on the device: the pose and exposure being fitted with their Adam states, laid out as
+// pose_step_kernel and exposure_adam_kernel index them (keyframe 0 of one-row arrays); the last iteration's gradients, loss and
+// overflow word; and the tally of the iterations.
+struct AlignState {
+    double T[12];                     // float64 T_cw = R_cw (row-major) | t_cw
+    float pose_f[12];                 // R_wc | t_wc
+    float cam[36];                    // view16 | proj16 | campos4 of pose_f
+    float pose_m[6], pose_v[6];
+    float E[12], expo_m[12], expo_v[12];
+    float pose_grad[8];               // dL/d(rho, omega) (6 used)
+    float dE[12];                     // dL/dE
+    float loss;                       // fit-region loss
+    float overflow;                   // overflow_word_kernel's word: non-zero skips both steps
+    int pose_t, expo_t;
+    int steps, skipped;
+    float first_loss, last_loss;
+    unsigned int max_pairs;           // the largest (tile, Gaussian) pair count of a skipped iteration
+};
+
+// closes an alignment iteration: counted as stepped (with its loss) or skipped (with its pair count); the word is cleared
+__global__ void align_tally_kernel(const GeomHeader* __restrict__ ghdr, AlignState* __restrict__ st) {
+    if (st->overflow != 0.0f) {
+        ++st->skipped;
+        st->max_pairs = max(st->max_pairs, ghdr->total);
+    } else {
+        if (st->steps == 0) st->first_loss = st->loss;
+        st->last_loss = st->loss;
+        ++st->steps;
+    }
+    st->overflow = 0.0f;
+}
+
+// dst[3][H][w] = columns [x0, x0 + w) of src[3][H][W]
+__global__ void __launch_bounds__(256)
+crop_columns_kernel(int H, int W, int x0, int w, const float* __restrict__ src, float* __restrict__ dst) {
+    const size_t n = (size_t)3 * H * w;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t row = i / w;
+        dst[i] = src[row * W + x0 + (i - row * w)];
+    }
+}
+
+// dst[3][H][W] = src[3][H][w] in columns [0, w), zero in the others
+__global__ void __launch_bounds__(256)
+pad_columns_kernel(int H, int W, int w, const float* __restrict__ src, float* __restrict__ dst) {
+    const size_t n = (size_t)3 * H * W;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t row = i / W, x = i - row * W;
+        dst[i] = x < (size_t)w ? src[row * w + x] : 0.0f;
+    }
+}
+
+unsigned plane_blocks(size_t n) { return (unsigned)std::min<size_t>((n + 255) / 256, (size_t)NUM_SMS * 8); }
+
+// The workspace of glic_mapper_align: colour gradients [3 Pcap] | pose partials | with split, three planes [3][H][W - W/2]
+// (rendered and ground-truth crops, the fit crop's dL/dpixel) | the one-row state
+size_t align_carve(void* ws, uint32_t Pcap, int W, int H, bool split, float** col, double** part, float** crops, AlignState** st) {
+    Carver c(ws);
+    float* a = c.take<float>((size_t)3 * Pcap);
+    double* b = c.take<double>(pose_partials_count(Pcap));
+    for (int q = 0; q < 3; ++q) {
+        float* x = c.take<float>(split ? (size_t)3 * H * (W - W / 2) : 0);
+        if (crops) crops[q] = x;
+    }
+    AlignState* t = c.take<AlignState>(1);
+    if (col) *col = a;
+    if (part) *part = b;
+    if (st) *st = t;
+    return c.total();
+}
+
+// glic_mapper_align after its checks: reserve, start state, the fit loop (enqueued without a host synchronisation), the
+// overflow regrow, the scoring
+int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_align_params& p, glic_align_result* out, float* rgb_host) {
+    const int W = m->cfg.width, H = m->cfg.height;
+    const bool split = p.split != 0;
+    const int Wf = split ? W / 2 : W, x_score = split ? W / 2 : 0, Ws = W - x_score;     // fit and score columns
+    const bool use_expo = p.exposure_lr > 0.0f || (train && m->expo_on);                  // the loss applies E
+    cudaStream_t s = m->stream;
+    MAP_TRY(poll_ring(m, true));
+    MAP_TRY(reserve(m, m->align_ws, align_carve(nullptr, m->Pcap, W, H, split, nullptr, nullptr, nullptr, nullptr)));
+    if (use_expo) MAP_TRY(reserve(m, m->loss_scratch, glic_loss_exposure_scratch_bytes(H, Wf)));
+    if (m->lpips_w) MAP_TRY(reserve(m, m->lpips_scratch, glic_lpips_scratch_bytes(H, Ws)));
+    float *col = nullptr, *crops[3] = {nullptr, nullptr, nullptr};
+    double* part = nullptr;
+    AlignState* st = nullptr;
+    align_carve(m->align_ws, m->Pcap, W, H, split, &col, &part, crops, &st);
+    // start: the stored pose (its camera block is the keyframe's), or a training keyframe's refined one; E = [I | 0], or a
+    // training keyframe's trained E; zero moments and step counts
+    AlignState h{};
+    CamBlock cb;
+    camera_block(W, H, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, kf.R_wc, kf.t_wc, cb, h.T);
+    std::memcpy(h.pose_f, kf.R_wc, sizeof(kf.R_wc)); std::memcpy(h.pose_f + 9, kf.t_wc, sizeof(kf.t_wc));
+    std::memcpy(h.cam, cb.view, sizeof(h.cam));
+    h.E[0] = h.E[5] = h.E[10] = 1.0f;
+    h.first_loss = h.last_loss = std::numeric_limits<float>::quiet_NaN();
+    GLIC_CUDA_TRY(cudaMemcpyAsync(st, &h, sizeof(h), cudaMemcpyHostToDevice, s));
+    if (train && m->pose_on) {
+        GLIC_CUDA_TRY(cudaMemcpyAsync(st->T, m->pose_T + 12 * (size_t)index, sizeof(h.T), cudaMemcpyDeviceToDevice, s));
+        GLIC_CUDA_TRY(cudaMemcpyAsync(st->pose_f, m->pose_f + 12 * (size_t)index, sizeof(h.pose_f), cudaMemcpyDeviceToDevice, s));
+        GLIC_CUDA_TRY(cudaMemcpyAsync(st->cam, kf.cam_dev, sizeof(h.cam), cudaMemcpyDeviceToDevice, s));
+    }
+    if (train && m->expo_on) GLIC_CUDA_TRY(cudaMemcpyAsync(st->E, m->expo_E + 12 * (size_t)index, sizeof(h.E), cudaMemcpyDeviceToDevice, s));
+    Keyframe ak;                                    // the keyframe's view, drawn from the call's own camera block
+    ak.view = kf.view;
+    ak.view.viewmatrix = st->cam; ak.view.projmatrix = st->cam + 16; ak.view.campos = st->cam + 32;
+    MAP_TRY(load_gt(m, kf, m->gt_dev[0], cudaMemcpyHostToDevice, s));
+    const float* gt_fit = m->gt_dev[0];
+    if (split) {
+        crop_columns_kernel<<<plane_blocks((size_t)3 * H * Wf), 256, 0, s>>>(H, W, 0, Wf, m->gt_dev[0], crops[1]);
+        GLIC_LAUNCH_CHECK();
+        gt_fit = crops[1];
+    }
+    MAP_TRY(activate(m));
+    float* g[6];
+    arena_ptrs(m, m->params, m->Pcap, g);
+    PoseBatch b{};
+    b.cam[0] = st->cam;
+    float fov2[2];
+    proj_matrix(W, H, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, b.Pm, fov2);
+    const int slot_kf[1] = {0};
+    const unsigned int* skip = reinterpret_cast<const unsigned int*>(&st->overflow);
+    CompactGrads cg{};                              // null row pointers: the pose-only backward
+    cg.pose_partials = part;
+    cg.pose_grad = st->pose_grad;
+    const GeomHeader* ghdr = GeomState::carve(m->geom_ws, (int)m->P).hdr;
+    for (int it = 0; it < p.iterations; ++it) {
+        MAP_TRY(forward_view(m, ak, 0, nullptr));
+        overflow_word_kernel<<<1, 1, 0, s>>>(ghdr, &st->overflow);
+        GLIC_LAUNCH_CHECK();
+        const float* img_fit = m->color;
+        float* dL_fit = m->dL_dpix;
+        if (split) {
+            crop_columns_kernel<<<plane_blocks((size_t)3 * H * Wf), 256, 0, s>>>(H, W, 0, Wf, m->color, crops[0]);
+            GLIC_LAUNCH_CHECK();
+            img_fit = crops[0];
+            dL_fit = crops[2];
+        }
+        if (use_expo)
+            MAP_TRY(glic_l1_ssim_loss_exposure(H, Wf, m->cfg.lambda_dssim, img_fit, gt_fit, st->E, &st->loss, dL_fit, st->dE, m->loss_scratch,
+                                               m->loss_scratch.bytes(), s));
+        else
+            MAP_TRY(glic_l1_ssim_loss(3, H, Wf, m->cfg.lambda_dssim, img_fit, gt_fit, &st->loss, dL_fit, m->loss_scratch, m->loss_scratch.bytes(), s));
+        if (split) {
+            pad_columns_kernel<<<plane_blocks((size_t)3 * H * W), 256, 0, s>>>(H, W, Wf, crops[2], m->dL_dpix);
+            GLIC_LAUNCH_CHECK();
+        }
+        MAP_TRY(glic_backward_compact_internal((int)m->P, m->D, m->M, g[1], m->act_scales, m->act_rots, m->M ? g[5] : nullptr, &ak.view, m->radii,
+                                               m->bin_cap, m->geom_ws, m->binning_ws, m->image_ws, m->sample_ws, m->dL_dpix, m->g_mean2D,
+                                               m->g_conic, m->g_opacity, col, &cg, nullptr, s));
+        pose_step_kernel<<<1, MAX_SLOTS, 0, s>>>(1, b, st->pose_grad, st->T, st->pose_f, st->pose_m, st->pose_v, &st->pose_t,
+                                                 p.lr_translation, p.lr_rotation, skip);
+        GLIC_LAUNCH_CHECK();
+        if (p.exposure_lr > 0.0f)
+            MAP_TRY(launch_exposure_adam(1, slot_kf, st->dE, st->E, st->expo_m, st->expo_v, &st->expo_t, p.exposure_lr, skip, s));
+        align_tally_kernel<<<1, 1, 0, s>>>(ghdr, st);
+        GLIC_LAUNCH_CHECK();
+    }
+    GLIC_CUDA_TRY(cudaMemcpyAsync(&h, st, sizeof(h), cudaMemcpyDeviceToHost, s));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    if (h.skipped) {                                // as poll_ring grows it after an overflowed iteration
+        MAP_TRY(set_bin_capacity(m, std::max<int64_t>((int64_t)h.max_pairs + h.max_pairs / 4, m->bin_cap * 3 / 2)));
+        ++m->st.overflow_regrows;
+    }
+    // scoring at the fitted camera: the full clamped (exposed) frame, then with split its score columns
+    MAP_TRY(forward_settled(m, ak, 0));
+    MAP_TRY(eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], use_expo ? st->E : nullptr, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s));
+    if (rgb_host)
+        GLIC_CUDA_TRY(cudaMemcpyAsync(rgb_host, eval_clamped(m->eval_scratch, 3, H, W, 0), sizeof(float) * 3 * (size_t)W * H,
+                                      cudaMemcpyDeviceToHost, s));
+    if (split) {
+        for (int q = 0; q < 2; ++q) {
+            crop_columns_kernel<<<plane_blocks((size_t)3 * H * Ws), 256, 0, s>>>(H, W, x_score, Ws, eval_clamped(m->eval_scratch, 3, H, W, q), crops[q]);
+            GLIC_LAUNCH_CHECK();
+        }
+        MAP_TRY(eval_psnr_ssim(3, H, Ws, crops[0], crops[1], nullptr, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s));
+    }
+    if (m->lpips_w)
+        MAP_TRY(glic_lpips(H, Ws, eval_clamped(m->eval_scratch, 3, H, Ws, 0), eval_clamped(m->eval_scratch, 3, H, Ws, 1), m->lpips_w,
+                           m->eval_out + 2, m->lpips_scratch, m->lpips_scratch.bytes(), s));
+    float out3[3] = {0.f, 0.f, std::numeric_limits<float>::quiet_NaN()};
+    MAP_TRY(read_eval_out(m, out3, m->lpips_w ? 3 : 2));
+    glic_align_result& r = *out;
+    std::memcpy(r.R_wc, h.pose_f, sizeof(r.R_wc)); std::memcpy(r.t_wc, h.pose_f + 9, sizeof(r.t_wc));
+    std::memcpy(r.E, h.E, sizeof(r.E));
+    r.psnr = out3[0]; r.ssim = out3[1]; r.lpips = out3[2];
+    r.first_loss = h.first_loss; r.last_loss = h.last_loss;
+    std::memcpy(r.pose_exp_avg, h.pose_m, sizeof(r.pose_exp_avg)); std::memcpy(r.pose_exp_avg_sq, h.pose_v, sizeof(r.pose_exp_avg_sq));
+    std::memcpy(r.expo_exp_avg, h.expo_m, sizeof(r.expo_exp_avg)); std::memcpy(r.expo_exp_avg_sq, h.expo_v, sizeof(r.expo_exp_avg_sq));
+    r.steps = h.steps; r.skipped = h.skipped;
+    return GLIC_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1691,6 +1888,21 @@ int glic_mapper_pose_set(glic_mapper* m, int index, const float* R_wc9, const fl
 
 int glic_mapper_pose_adam_state(glic_mapper* m, int index, float* exp_avg6, float* exp_avg_sq6, int* step) {
     return keyframe_adam_state(m, true, index, exp_avg6, exp_avg_sq6, step, "mapper_pose_adam_state");
+}
+
+int glic_mapper_align(glic_mapper* m, int is_train, int index, const glic_align_params* p, glic_align_result* out, float* rgb_host) {
+    if (!m || !p || !out) { set_error("mapper_align: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const auto& list = is_train ? m->train : m->test;
+    if (index < 0 || index >= (int)list.size()) { set_error("mapper_align: keyframe index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (p->iterations < 0 || !finite_at_least_zero(p->lr_translation) || !finite_at_least_zero(p->lr_rotation) ||
+        !finite_at_least_zero(p->exposure_lr) || (p->split != 0 && p->split != 1)) {
+        set_error("mapper_align: iterations must be >= 0, the rates finite and >= 0, split 0 or 1"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    const int W = m->cfg.width, H = m->cfg.height, Ws = W - (p->split ? W / 2 : 0);
+    if (p->split && W < 2) { set_error("mapper_align: split needs a frame at least 2 columns wide"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (m->lpips_w && !glic_lpips_scratch_bytes(H, Ws)) { set_error("mapper_align: LPIPS needs a score region of at least 31x31"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (m->P == 0) { set_error("mapper_align: the map has no rows to align against"); return GLIC_ERR_INVALID_ARGUMENT; }
+    return align(m, list[index], is_train != 0, index, *p, out, rgb_host);
 }
 
 int glic_mapper_synchronize(glic_mapper* m) {

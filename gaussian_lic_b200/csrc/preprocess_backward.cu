@@ -27,6 +27,12 @@
 // warps in order) and writes one partial per CTA; partials_finish_kernel adds the partials in a fixed order.  No atomics:
 // two runs give the same bits.
 //
+// POSE_ONLY (with POSE, without DENS; glic_mapper_align): the six pose floats and nothing per row.  The same pass, the same
+// fp32 expressions for pose6 and the same fixed-order reduction, but no row of the compact block is written, the scale /
+// rotation chain rule and the opacity activation are not formed, and neither their inputs (opacity, dL/dopacity, the raw
+// rotation) nor the densification statistics are touched.  Given the same render-backward outputs its pose gradient is the
+// POSE form's, bit for bit.  Chosen by CompactGrads with null row pointers (g_xyz == NULL) and pose partials.
+//
 // DENS (only with COMPACT; glic_mapper_enable_densification): the same pass writes (or, for the later views of a rank, adds)
 // the view's densification statistics of each row: |(dL/dmean2D.x, dL/dmean2D.y)| and 1 when it is visible, 0 and 0 when it is
 // culled.  One thread owns a row, so there are no atomics.
@@ -38,7 +44,7 @@ namespace glic {
 
 constexpr int PB_THREADS = 128;
 
-template <bool COMPACT, bool POSE = false, bool DENS = false>
+template <bool COMPACT, bool POSE = false, bool DENS = false, bool POSE_ONLY = false>
 __global__ void __launch_bounds__(PB_THREADS)
 preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means, const float* __restrict__ scales,
                            float mod, const float4* __restrict__ rots, const float* __restrict__ sh, ViewParams vp,
@@ -51,6 +57,7 @@ preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means,
     __shared__ __align__(16) float s_sh[PB_THREADS / 32][32 * SH_ROW_MAX];    // SH rows in, dL/dSH rows out
     static_assert(COMPACT || !POSE, "the pose gradient is a compact-form output");
     static_assert(COMPACT || !DENS, "the densification statistics are a compact-form output");
+    static_assert(!POSE_ONLY || (POSE && !DENS), "the pose-only form writes the pose partials alone");
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (tid < 16) s_view[tid] = vp.view[tid];
     else if (tid < 32) s_proj[tid - 16] = vp.proj[tid - 16];
@@ -71,7 +78,7 @@ preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means,
     if (!visible) {
         if (idx < P) {
             if (COMPACT) {
-                if (!cg.accumulate) {
+                if (!POSE_ONLY && !cg.accumulate) {
 #pragma unroll
                     for (int k = 0; k < 3; ++k) { cg.g_xyz[3 * idx + k] = 0.f; cg.g_scale[3 * idx + k] = 0.f; }
                     cg.g_rot[idx] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -290,7 +297,7 @@ preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means,
         dL_dmeans3D[3 * idx] = dmx; dL_dmeans3D[3 * idx + 1] = dmy; dL_dmeans3D[3 * idx + 2] = dmz;
         dL_dscales[3 * idx] = ds[0]; dL_dscales[3 * idx + 1] = ds[1]; dL_dscales[3 * idx + 2] = ds[2];
         dL_drots[idx] = dq;
-    } else {
+    } else if constexpr (!POSE_ONLY) {
         // chain rule of the activations (same expressions as activations_backward_kernel, model_step.cu):
         //   sigmoid' = o (1 - o);  exp' = exp;  normalize: (g - q (q.g)) / |r|
         const float o = cg.opacity[idx];
@@ -365,13 +372,13 @@ int launch_preprocess_backward(int P, int D, int M, const float* means, const fl
     return GLIC_OK;
 }
 
-template <bool DENS>
+template <bool DENS, bool POSE_ONLY = false>
 static int launch_compact(int P, int D, int M, const float* means, const float* scales, float mod, const float* rots, const float* sh,
                    const ViewParams& vp, const int* radii, GeomState g, const float* dL_dmean2D, const float* dL_dconic,
                    const float* dL_dcolors, const CompactGrads& cg, cudaStream_t s) {
     const unsigned blocks = (P + PB_THREADS - 1) / PB_THREADS;
     if (cg.pose_partials) {
-        preprocess_backward_kernel<true, true, DENS><<<blocks, PB_THREADS, 0, s>>>(
+        preprocess_backward_kernel<true, true, DENS, POSE_ONLY><<<blocks, PB_THREADS, 0, s>>>(
             P, D, M, means, scales, mod, reinterpret_cast<const float4*>(rots), sh, vp, radii, g.clamped, 0.0f,
             dL_dmean2D, dL_dconic, dL_dcolors, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cg);
         GLIC_LAUNCH_CHECK();
@@ -390,6 +397,10 @@ int launch_preprocess_backward_compact(int P, int D, int M, const float* means, 
                                        const float* rots, const float* sh, const ViewParams& vp, const int* radii, GeomState g,
                                        const float* dL_dmean2D, const float* dL_dconic, const float* dL_dcolors,
                                        const CompactGrads& cg, cudaStream_t s) {
+    if (!cg.g_xyz) {                                               // the pose gradient alone (POSE_ONLY)
+        if (!cg.pose_partials || !cg.pose_grad || cg.dens_norm) { set_error("backward_compact: the pose-only form takes the pose outputs alone"); return GLIC_ERR_INVALID_ARGUMENT; }
+        return launch_compact<false, true>(P, D, M, means, scales, mod, rots, sh, vp, radii, g, dL_dmean2D, dL_dconic, dL_dcolors, cg, s);
+    }
     return cg.dens_norm ? launch_compact<true>(P, D, M, means, scales, mod, rots, sh, vp, radii, g, dL_dmean2D, dL_dconic, dL_dcolors, cg, s)
                         : launch_compact<false>(P, D, M, means, scales, mod, rots, sh, vp, radii, g, dL_dmean2D, dL_dconic, dL_dcolors, cg, s);
 }

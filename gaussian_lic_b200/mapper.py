@@ -247,6 +247,29 @@ class Mapper:
         capi.check(capi.lib.glic_mapper_pose_adam_state(self._h, int(index), m1, m2, C.byref(t)), "mapper_pose_adam_state")
         return np.array(m1[:], np.float32), np.array(m2[:], np.float32), int(t.value)
 
+    def align(self, index, train=False, iterations=100, lr_translation=1e-3, lr_rotation=1e-3, exposure_lr=0.0, split=False,
+              image=False):
+        """Fit keyframe `index`'s pose (and with exposure_lr > 0 its exposure) to its image against the frozen map, then score it
+        there (glic_mapper_align).  split=True fits on the left half and scores on the right half.  Returns a dict of the
+        result fields: R_wc [3,3], t_wc [3], E [3,4], psnr, ssim, lpips (NaN without load_lpips), first_loss, last_loss, the
+        Adam moments (pose_exp_avg [6], pose_exp_avg_sq [6], expo_exp_avg [3,4], expo_exp_avg_sq [3,4]), steps, skipped; and
+        with image=True the [3,H,W] clamped, exposed frame at the fitted camera under "image"."""
+        p = capi.AlignParams(int(iterations), float(lr_translation), float(lr_rotation), float(exposure_lr), int(bool(split)))
+        r = capi.AlignResult()
+        img = np.empty((3, self.H, self.W), np.float32) if image else None
+        capi.check(capi.lib.glic_mapper_align(self._h, int(bool(train)), int(index), C.byref(p), C.byref(r), _p(img)), "mapper_align")
+        shapes = dict(R_wc=(3, 3), E=(3, 4), expo_exp_avg=(3, 4), expo_exp_avg_sq=(3, 4))
+        out = {}
+        for k, _ in capi.AlignResult._fields_:
+            v = getattr(r, k)
+            if isinstance(v, C.Array):
+                out[k] = np.array(v[:], np.float32).reshape(shapes.get(k, (-1,)))
+            else:
+                out[k] = v
+        if image:
+            out["image"] = img
+        return out
+
     def synchronize(self):
         capi.check(capi.lib.glic_mapper_synchronize(self._h), "mapper_synchronize")
 

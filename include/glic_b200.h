@@ -325,6 +325,17 @@ GLIC_API int glic_debug_render_backward(int P, const glic_view* view, int64_t R,
                                         const void* image_ws, const void* sample_ws, const float* dL_dpix, float* dL_dmeans2D,
                                         float* dL_dconic, float* dL_dopacity, float* dL_dcolors, int exact,
                                         unsigned long long* counters, void* stream);
+/* The mapper's per-Gaussian backward alone, on the saved state of the last glic_forward and given render-backward outputs
+ * (device arrays; rotations activated, rot_raw the raw ones, opacity activated).  pose_only = 0: the COMPACT + POSE form of an
+ * iteration under pose refinement, writing the 11 geometric floats of every row to g_geo [11 P] (rotation [P,4] | xyz [P,3] |
+ * log-scale [P,3] | opacity logit [P]); pose_only = 1: the POSE_ONLY form of glic_mapper_align, which writes no row (g_geo,
+ * rot_raw, opacity and dL_dopacity may be NULL).  Both write dL/d(rho, omega) of the view to pose6 (device, 6 floats) through
+ * partials (device, 48 * ceil(P / 128) bytes).  Asynchronous on `stream`. */
+GLIC_API int glic_debug_pose_backward(int P, int sh_degree, int M, const float* means3D, const float* scales, const float* rotations,
+                                      const float* rot_raw, const float* opacity, const float* sh, const glic_view* view,
+                                      const int* radii, const void* geom_ws, const float* dL_dmeans2D, const float* dL_dconic,
+                                      const float* dL_dopacity, const float* dL_dcolors, int pose_only, float* g_geo,
+                                      void* partials, float* pose6, void* stream);
 /* Allocation failures of the native mapper, simulated on the host (no CUDA call is made for the failing one): the n-th device
  * or pinned allocation a mapper makes from now on returns cudaErrorMemoryAllocation; n = 0 disarms it, n < 0 is refused.
  * glic_debug_mapper_allocations is the number of allocations the mappers of this process hold right now. */
@@ -718,6 +729,59 @@ GLIC_API int glic_mapper_pose_get(glic_mapper* m, int index, float* R_wc9, float
 GLIC_API int glic_mapper_pose_set(glic_mapper* m, int index, const float* R_wc9, const float* t_wc3);
 /* the pose's Adam state of training keyframe `index`: both moments (6 floats each, rho then omega) and the step count */
 GLIC_API int glic_mapper_pose_adam_state(glic_mapper* m, int index, float* exp_avg6, float* exp_avg_sq6, int* step);
+/* Test-time alignment (BARF-style evaluation; Inria 3DGS's train_test_exp): fit one keyframe's camera pose and exposure to its
+ * image against the frozen map, then score it there.  glic_mapper_evaluate scores a held-out keyframe at its odometry pose
+ * with the identity exposure; once pose refinement and exposure have moved the training keyframes (and with them the map),
+ * that measures the drift and the brightness of the frame as well as the map.  glic_mapper_align(m, is_train, index, p, out,
+ * rgb_host) works on either list:
+ *   - start: the keyframe's current float pose (the refined pose of a training keyframe under pose refinement, the stored pose
+ *     otherwise; the float64 T_cw is the refined master, or derived from the floats as glic_camera_block does) and
+ *     E = the training keyframe's E when exposure is enabled, [I | 0] otherwise; zero Adam moments and step counts;
+ *   - each of p->iterations iterations: render at the current pose; the L1 + D-SSIM loss (cfg.lambda_dssim) on the fit region,
+ *     with E applied when exposure_lr > 0 or the start E is a trained one; the render backward and the pose-only per-Gaussian
+ *     backward on that region's dL/dpixel (zero elsewhere); one Adam step of the pose and, when exposure_lr > 0, one of E, with
+ *     the rules, betas, eps and bias correction of pose refinement and exposure above for a batch of one slot (T_cw <- Exp(u)
+ *     T_cw in float64, the float pose and camera block re-derived from it).  A zero rate leaves that part of the pose at its
+ *     start (its moments still advance, as in training); exposure_lr = 0 leaves E at its start and its moments at zero;
+ *   - fit region: split = 0 the whole frame; split = 1 columns [0, W/2), the loss taken on the cropped planes [3, H, W/2]
+ *     (SSIM pads at the crop edge as at a frame border).  Score region: the whole frame, or columns [W/2, W);
+ *   - an iteration whose forward overflows the binning workspace changes nothing and counts in `skipped`; after the loop the
+ *     workspace grows as it does after an overflowed training iteration (stats.overflow_regrows counts it);
+ *   - scoring, once at the end: the keyframe drawn at the fitted pose (as glic_mapper_evaluate draws, overflow redone), the
+ *     fitted E applied when it was in the loss, clamped to [0,1]; PSNR / SSIM as glic_mapper_evaluate computes them and LPIPS as
+ *     glic_mapper_evaluate_lpips does (NaN without glic_mapper_load_lpips), on the score region (with split = 1 the right-half
+ *     crops of the clamped frame and image, exactly glic_eval_psnr_ssim of those crops).  rgb_host (may be NULL) receives the
+ *     whole clamped, exposed frame [3,H,W] as glic_mapper_render writes it.  With no fit (iterations = 0, or all three rates 0)
+ *     and split = 0 the scores are glic_mapper_evaluate_lpips's and the image glic_mapper_render's, bit for bit;
+ *   - out: the fitted float pose, E, the scores, the fit loss of the first and of the last stepped iteration (NaN without one),
+ *     both Adam moments of the pose and of E (the first step from zero moments stores m = fl((1 - b1) g)), and the counts.
+ * The map is frozen: the call changes no parameter, moment, densification statistic, maxr, sky row count, keyframe, pose,
+ * camera block, E, Adam state, sampler state or density-control counter, and no stats field but overflow_regrows.  It drains
+ * the iteration pipeline (as glic_mapper_evaluate does), enqueues the iterations without a host synchronisation (the overflow
+ * skip stays on the device) and synchronises at the end.  With world > 1 it is rank-local: it reads and writes none of the
+ * exchange block the peers push into, so one rank may align between optimize() calls while the others do not.
+ * Memory: its workspace (kept for the next call) is 12 B per row of capacity (the colour gradients) + 6 doubles per 128 rows
+ * (the pose partials) + with split three planes of 12 * H * (W - W/2) B + a state row under 1 KB; the exposure loss's scratch and
+ * LPIPS's grow as for training and evaluation.  Everything is reserved before anything runs (failure contract above).
+ * Rejected with GLIC_ERR_INVALID_ARGUMENT, changing nothing: a NULL m, p or out; an index out of range; iterations < 0; a
+ * rate that is negative or not finite; split not 0 or 1; split = 1 on a frame under 2 columns; a score region under 31x31
+ * with LPIPS weights loaded; a mapper with no rows. */
+typedef struct glic_align_params {
+    int iterations;                    /* >= 0 */
+    float lr_translation, lr_rotation; /* pose Adam rates, >= 0; 0 leaves that part of the pose fixed */
+    float exposure_lr;                 /* >= 0; 0 leaves E fixed */
+    int split;                         /* 0: fit and score on the whole frame; 1: fit on columns [0, W/2), score on [W/2, W) */
+} glic_align_params;
+typedef struct glic_align_result {
+    float R_wc[9], t_wc[3];            /* the fitted float pose */
+    float E[12];                       /* the fitted exposure (row-major 3x4, as glic_mapper_exposure_get) */
+    float psnr, ssim, lpips;           /* at the fitted pose and E, on the score region; lpips is NaN without glic_mapper_load_lpips */
+    float first_loss, last_loss;       /* fit-region loss of the first and of the last stepped iteration */
+    float pose_exp_avg[6], pose_exp_avg_sq[6], expo_exp_avg[12], expo_exp_avg_sq[12];
+    int steps, skipped;                /* stepped iterations, and iterations skipped for a binning overflow */
+} glic_align_result;
+GLIC_API int glic_mapper_align(glic_mapper* m, int is_train, int index, const glic_align_params* p, glic_align_result* out,
+                               float* rgb_host /* [3,H,W] or NULL */);
 /* Camera (camera.h:38-110) in closed form, as the mapper derives it from a keyframe pose: out41 = view[16] (column-major
  * Rt) | proj[16] (column-major P*Rt) | campos[3] | tan_fovx, tan_fovy | limx_neg, limx_pos, limy_neg, limy_pos. */
 GLIC_API int glic_camera_block(int width, int height, float fx, float fy, float cx, float cy, const float* R_wc /*[9] row-major*/,
