@@ -79,6 +79,11 @@ class AlignResult(C.Structure):
                 ("steps", C.c_int), ("skipped", C.c_int)]
 
 
+class RenderCamera(C.Structure):
+    _fields_ = [("R_wc", C.c_float * 9), ("t_wc", C.c_float * 3), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float),
+                ("cy", C.c_float), ("width", C.c_int), ("height", C.c_int)]
+
+
 def _load():
     if not os.path.isfile(LIB_PATH):
         raise ImportError(
@@ -105,6 +110,8 @@ def _load():
         "glic_binning_capacity": (i64, [sz, sz, i32, i32, i32]),
         "glic_forward": (i32, [i32, i32, i32, vp, vp, f32, vp, vp, vp, vp, C.POINTER(View), i32, vp, vp, sz, vp, sz, vp, sz, vp, sz, vp, vp,
                                vp, vp]),
+        "glic_render": (i32, [i32, i32, i32, vp, vp, f32, vp, vp, vp, vp, C.POINTER(View), vp, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp,
+                              vp, vp]),
         "glic_forward_render": (i32, [i32, C.POINTER(View), i32, i64, vp, vp, vp, sz, vp, sz, vp, vp, C.POINTER(i64), vp]),
         "glic_backward": (i32, [i32, i32, i32, vp, vp, f32, vp, vp, vp, C.POINTER(View), vp, i64, vp, vp, vp, vp, vp, f32,
                                 vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
@@ -193,6 +200,7 @@ def _load():
         "glic_mapper_pose_set": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32)]),
         "glic_mapper_pose_adam_state": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32), C.POINTER(i32)]),
         "glic_mapper_align": (i32, [vp, i32, i32, C.POINTER(AlignParams), C.POINTER(AlignResult), vp]),
+        "glic_mapper_render_camera": (i32, [vp, C.POINTER(RenderCamera), i32, i32, vp, vp, vp, vp]),
         "glic_mapper_enable_frames": (i32, [vp, i32, i32, i32]),
         "glic_mapper_add_frame": (i32, [vp, C.POINTER(Frame), C.POINTER(i32)]),
         "glic_mapper_keyframe_image": (i32, [vp, i32, i32, vp]),

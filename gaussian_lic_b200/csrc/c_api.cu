@@ -63,11 +63,43 @@ __global__ void debug_geom_kernel(int P, GeomState g, float* depth, float* xy, f
     if (clamped) { const unsigned c = g.clamped[i]; clamped[3 * i] = c & 1u; clamped[3 * i + 1] = (c >> 1) & 1u; clamped[3 * i + 2] = (c >> 2) & 1u; }
 }
 
+__global__ void __launch_bounds__(256) fill_kernel(size_t n, float v, float* __restrict__ out) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) out[i] = v;
+}
+
 __global__ void debug_keys_kernel(long long R, GeomState g, const uint32_t* tile_keys, const uint32_t* point_list, uint64_t* out) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= R) return;
     const uint32_t gid = point_list[i];
     out[i] = ((uint64_t)tile_keys[i] << 32) | (uint64_t)__float_as_uint(g.rec[3 * (size_t)gid + 2].y);
+}
+
+// The stages of glic_forward and glic_render up to the blend, on workspaces carved for `cap` pairs: preprocess, depth sort and scan,
+// key emission, tile sort, tile ranges and, with `buckets`, the bucket offsets of the checkpoints.  Returns the ping-pong half that
+// holds the sorted list, < 0 on error.
+int bin_view(int P, int sh_degree, int M, const float* means3D, const float* scales, float scale_modifier, const float* rotations,
+             const float* opacities, const float* dc, const float* sh, const ViewParams& vp, bool no_color, int* radii, GeomState g,
+             BinningState bin, ImageState img, int64_t cap, bool buckets, cudaStream_t s) {
+    { StageTimer _t(GLIC_STAGE_PREPROCESS, s);
+      if (int e = launch_preprocess_forward(P, sh_degree, M, means3D, scales, scale_modifier, rotations, opacities, dc, sh, vp,
+                                            no_color, radii, g, s)) return e; }
+    { StageTimer _t(GLIC_STAGE_SORT, s);
+      const int cur0 = launch_sort_pairs32(P, 32, g.depth_keys, g.order, g.sort_temp, g.sort_temp_size, s, nullptr, /*hist_ready=*/true);
+      if (cur0 < 0) return cur0;
+      if (int e = launch_depth_scan(P, g, g.order[cur0], cap, s)) return e; }
+    const int bit = tile_sort_bits(vp.grid_x * vp.grid_y);
+    { StageTimer _t(GLIC_STAGE_EMIT, s);
+      if (int e = sort_prepare(cap, bit, bin.sort_temp, s)) return e;        // emit builds the tile sort's digit histograms
+      if (int e = launch_emit_keys(P, vp, g, bin.keys[0], bin.vals[0], cap, sort_hist(bin.sort_temp), bit, s)) return e; }
+    int cur;
+    { StageTimer _t(GLIC_STAGE_SORT, s);
+      cur = launch_sort_pairs32(cap, bit, bin.keys, bin.vals, bin.sort_temp, bin.sort_temp_size, s, &g.hdr->r_eff, true);
+      if (cur < 0) return cur; }
+    GLIC_CUDA_TRY(cudaMemsetAsync(&bin.hdr->sorted_in_b, cur, 1, s));       // 0/1 in the low byte (header is zero-padded)
+    GLIC_CUDA_TRY(cudaMemsetAsync(reinterpret_cast<char*>(&bin.hdr->sorted_in_b) + 1, 0, 3, s));
+    { StageTimer _t(GLIC_STAGE_RANGES, s);
+      if (int e = launch_tile_ranges(cap, g.hdr, bin.keys[cur], vp.grid_x * vp.grid_y, img, buckets, s)) return e; }
+    return cur;
 }
 
 }  // namespace glic
@@ -240,7 +272,6 @@ int glic_forward(int P, int sh_degree, int M, const float* means3D, const float*
     if (!out_final_T || (!no_color && !out_color)) { set_error("forward: null output"); return GLIC_ERR_INVALID_ARGUMENT; }
     cudaStream_t s = (cudaStream_t)stream;
     const ViewParams vp = make_view_params(view);
-    const int T = vp.grid_x * vp.grid_y;
     const size_t HW = (size_t)vp.W * vp.H;
     ImageState img = ImageState::carve(image_ws, vp.W, vp.H);
     if (P == 0) {
@@ -261,27 +292,54 @@ int glic_forward(int P, int sh_degree, int M, const float* means3D, const float*
     BinningState bin = BinningState::carve(binning_ws, cap);
     const int64_t max_buckets = no_color ? 0 : glic_max_buckets(cap, vp.W, vp.H);
     SampleState smp = SampleState::carve(no_color ? nullptr : sample_ws, max_buckets);
-    { StageTimer _t(GLIC_STAGE_PREPROCESS, s);
-      if (int e = launch_preprocess_forward(P, sh_degree, M, means3D, scales, scale_modifier, rotations, opacities, dc, sh, vp,
-                                            no_color != 0, radii, g, s)) return e; }
-    { StageTimer _t(GLIC_STAGE_SORT, s);
-      const int cur0 = launch_sort_pairs32(P, 32, g.depth_keys, g.order, g.sort_temp, g.sort_temp_size, s, nullptr, /*hist_ready=*/true);
-      if (cur0 < 0) return cur0;
-      if (int e = launch_depth_scan(P, g, g.order[cur0], cap, s)) return e; }
-    const int bit = tile_sort_bits(T);
-    { StageTimer _t(GLIC_STAGE_EMIT, s);
-      if (int e = sort_prepare(cap, bit, bin.sort_temp, s)) return e;        // emit builds the tile sort's digit histograms
-      if (int e = launch_emit_keys(P, vp, g, bin.keys[0], bin.vals[0], cap, sort_hist(bin.sort_temp), bit, s)) return e; }
-    int cur;
-    { StageTimer _t(GLIC_STAGE_SORT, s);
-      cur = launch_sort_pairs32(cap, bit, bin.keys, bin.vals, bin.sort_temp, bin.sort_temp_size, s, &g.hdr->r_eff, true);
-      if (cur < 0) return cur; }
-    GLIC_CUDA_TRY(cudaMemsetAsync(&bin.hdr->sorted_in_b, cur, 1, s));       // 0/1 in the low byte (header is zero-padded)
-    GLIC_CUDA_TRY(cudaMemsetAsync(reinterpret_cast<char*>(&bin.hdr->sorted_in_b) + 1, 0, 3, s));
-    { StageTimer _t(GLIC_STAGE_RANGES, s);
-      if (int e = launch_tile_ranges(cap, g.hdr, bin.keys[cur], T, img, !no_color, s)) return e; }
+    const int cur = bin_view(P, sh_degree, M, means3D, scales, scale_modifier, rotations, opacities, dc, sh, vp, no_color != 0, radii, g, bin,
+                             img, cap, !no_color, s);
+    if (cur < 0) return cur;
     { StageTimer _t(GLIC_STAGE_RENDER_FWD, s);
       if (int e = launch_render_forward(vp, no_color != 0, bin.vals[cur], g, img, smp, out_color, out_final_T, s)) return e; }
+    if (counters_host) GLIC_CUDA_TRY(cudaMemcpyAsync(counters_host, img.hdr->counters, 3 * sizeof(long long), cudaMemcpyDeviceToHost, s));
+    return GLIC_OK;
+}
+
+int glic_render(int P, int sh_degree, int M, const float* means3D, const float* scales, float scale_modifier,
+                const float* rotations, const float* opacities, const float* dc, const float* sh, const glic_view* view,
+                int* radii, void* geom_ws, size_t geom_bytes, void* image_ws, size_t image_bytes, void* binning_ws,
+                size_t binning_bytes, float* out_color, float* out_final_T, float* out_depth, float* out_median_depth,
+                int64_t* counters_host, void* stream) {
+    if (int e = check_view(view)) return e;
+    if (P < 0 || sh_degree < 0 || sh_degree > 3 || M < 0) { set_error("render: bad P / sh_degree / M"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if ((sh_degree + 1) * (sh_degree + 1) - 1 > M) { set_error("render: sh has fewer coefficients than sh_degree needs"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!image_ws || image_bytes < glic_image_bytes(view->width, view->height)) { set_error("render: image workspace too small"); return GLIC_ERR_WORKSPACE; }
+    if (!out_color || !out_final_T) { set_error("render: null output"); return GLIC_ERR_INVALID_ARGUMENT; }
+    cudaStream_t s = (cudaStream_t)stream;
+    const ViewParams vp = make_view_params(view);
+    const size_t HW = (size_t)vp.W * vp.H;
+    ImageState img = ImageState::carve(image_ws, vp.W, vp.H);
+    if (P == 0) {                                      // nothing to draw: T = 1 (nothing covers a pixel), every other plane 0
+        fill_kernel<<<(unsigned)std::min<size_t>((HW + 255) / 256, (size_t)NUM_SMS * 8), 256, 0, s>>>(HW, 1.0f, out_final_T);
+        GLIC_LAUNCH_CHECK();
+        GLIC_CUDA_TRY(cudaMemsetAsync(out_color, 0, sizeof(float) * 3 * HW, s));
+        if (out_depth) GLIC_CUDA_TRY(cudaMemsetAsync(out_depth, 0, sizeof(float) * HW, s));
+        if (out_median_depth) GLIC_CUDA_TRY(cudaMemsetAsync(out_median_depth, 0, sizeof(float) * HW, s));
+        GLIC_CUDA_TRY(cudaMemsetAsync(img.hdr, 0, sizeof(ImageHeader), s));
+        if (counters_host) GLIC_CUDA_TRY(cudaMemcpyAsync(counters_host, img.hdr->counters, 3 * sizeof(long long), cudaMemcpyDeviceToHost, s));
+        return GLIC_OK;
+    }
+    if (!means3D || !scales || !rotations || !opacities || !radii || !dc || (M > 0 && sh_degree > 0 && !sh)) {
+        set_error("render: null input pointer"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (!aligned16(rotations)) { set_error("render: rotations must be 16-byte aligned"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!geom_ws || geom_bytes < glic_geom_bytes(P)) { set_error("render: geometry workspace too small"); return GLIC_ERR_WORKSPACE; }
+    const int64_t cap = glic_binning_capacity(binning_bytes, 0, vp.W, vp.H, 1);     // no sample workspace: nothing is saved
+    if (!binning_ws || cap < 1) { set_error("render: binning workspace missing or too small"); return GLIC_ERR_WORKSPACE; }
+    GeomState g = GeomState::carve(geom_ws, P);
+    BinningState bin = BinningState::carve(binning_ws, cap);
+    // glic_forward's stages up to the blend, so the tile lists are its lists; no checkpoints, so no bucket offsets
+    const int cur = bin_view(P, sh_degree, M, means3D, scales, scale_modifier, rotations, opacities, dc, sh, vp, false, radii, g, bin, img,
+                             cap, false, s);
+    if (cur < 0) return cur;
+    { StageTimer _t(GLIC_STAGE_RENDER_FWD, s);
+      if (int e = launch_render_infer(vp, bin.vals[cur], g, img, out_color, out_final_T, out_depth, out_median_depth, s)) return e; }
     if (counters_host) GLIC_CUDA_TRY(cudaMemcpyAsync(counters_host, img.hdr->counters, 3 * sizeof(long long), cudaMemcpyDeviceToHost, s));
     return GLIC_OK;
 }

@@ -339,6 +339,9 @@ int launch_tile_ranges(int64_t R, const GeomHeader* ghdr, const uint32_t* tile_k
                        cudaStream_t s);
 int launch_render_forward(const ViewParams& vp, bool no_color, const uint32_t* point_list, GeomState g, ImageState img,
                           SampleState smp, float* out_color, float* out_final_T, cudaStream_t s);
+// the inference form of the blend (glic_render): colour, final T and, when non-null, expected and median depth; nothing else
+int launch_render_infer(const ViewParams& vp, const uint32_t* point_list, GeomState g, ImageState img, float* out_color,
+                        float* out_final_T, float* out_depth, float* out_median, cudaStream_t s);
 int launch_render_backward(int P, const ViewParams& vp, int64_t max_buckets, const uint32_t* point_list, GeomState g,
                            ImageState img, SampleState smp, const float* dL_dpix, float* dL_dmean2D /*[P,3]*/,
                            float* dL_dconic /*[P,4]*/, float* dL_dopacity, float* dL_dcolors, cudaStream_t s,
@@ -383,6 +386,8 @@ int launch_exposure_adam(int S, const int* kf_of_slot_host, const float* slot_gr
 // glic_eval_psnr_ssim with an optional exposure E (3 channels) applied to img before the clamp
 int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, const float* E, float* out2, void* scratch,
                    size_t scratch_bytes, void* stream);
+// out[3][H][W] = img exposed by E (optional) and clamped to [0,1], element for element the image eval_psnr_ssim scores
+int launch_scored_image(int H, int W, const float* img, const float* E, float* out, cudaStream_t s);
 // the clamped (and exposed) images eval_psnr_ssim scored, left in its scratch: which = 0 the image, 1 the ground truth
 const float* eval_clamped(const void* scratch, int CH, int H, int W, int which);
 // stable compaction of the arenas (prune.cu): glic_mapper_densify_and_prune, glic_mapper_densify (nothing removed) and

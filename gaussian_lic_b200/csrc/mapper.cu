@@ -378,6 +378,8 @@ struct glic_mapper {
     Dev<void> lpips_scratch;
     // ---- test-time alignment (glic_mapper_align): its workspace (align_carve), sized on first use ----
     Dev<char> align_ws;
+    // ---- rendering from a caller's camera (glic_mapper_render_camera): its workspace (render_carve) for the largest frame so far
+    Dev<char> render_ws;
     // ---- raw frames (glic_mapper_enable_frames / add_frame): the 8-bit image store, chunks of FRAME_CHUNK frames of
     //      frame_stride bytes that never move, and the scan of the frames since the last training keyframe (device arrays
     //      of scan_cap points, grown by doubling) ----
@@ -594,6 +596,15 @@ int set_bin_capacity(glic_mapper* m, int64_t pairs, bool exact = false) {
     return GLIC_OK;
 }
 
+// room for `pairs` in the binning workspace alone, for glic_render (which has no sample workspace); the sample workspace is left
+// as it is.  The training capacity is re-derived from both workspaces exactly as glic_forward derives it, so the backward keeps
+// carving the binning workspace with the capacity the forward used.
+int grow_render_binning(glic_mapper* m, int64_t pairs) {
+    MAP_TRY(reserve(m, m->binning_ws, glic_binning_bytes(pairs)));
+    m->bin_cap = glic_binning_capacity(m->binning_ws.bytes(), m->sample_ws.bytes(), m->cfg.width, m->cfg.height, 0);
+    return GLIC_OK;
+}
+
 // lagged, non-blocking look at the pinned binning counters of finished iterations
 int poll_ring(glic_mapper* m, bool wait) {
     for (int r = 0; r < RING; ++r) {
@@ -754,6 +765,19 @@ int iteration(glic_mapper* m, const int* views) {
     GLIC_CUDA_TRY(cudaEventRecord(m->ring_ev[r], s));
     m->ring_used[r] = true;
     ++m->st.iterations;
+    return GLIC_OK;
+}
+
+// glic_mapper_pose_set's test of a float pose: finite entries, R_wc a rotation (R^T R = I to float precision and det R = +1)
+int pose_check(const float* R_wc9, const float* t_wc3, const char* what) {
+    for (int j = 0; j < 9; ++j) if (!std::isfinite(R_wc9[j])) { set_error(std::string(what) + ": non-finite entry"); return GLIC_ERR_INVALID_ARGUMENT; }
+    for (int j = 0; j < 3; ++j) if (!std::isfinite(t_wc3[j])) { set_error(std::string(what) + ": non-finite entry"); return GLIC_ERR_INVALID_ARGUMENT; }
+    double R[9], err = 0.0;
+    for (int j = 0; j < 9; ++j) R[j] = R_wc9[j];
+    for (int a = 0; a < 3; ++a)
+        for (int b = 0; b < 3; ++b) err = std::max(err, std::fabs(R[a] * R[b] + R[3 + a] * R[3 + b] + R[6 + a] * R[6 + b] - (a == b ? 1.0 : 0.0)));
+    const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) + R[2] * (R[3] * R[7] - R[4] * R[6]);
+    if (err > 1e-5 || det < 0.0) { set_error(std::string(what) + ": R_wc is not a rotation (orthonormal, det +1)"); return GLIC_ERR_INVALID_ARGUMENT; }
     return GLIC_OK;
 }
 
@@ -1670,6 +1694,66 @@ int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_
     return GLIC_OK;
 }
 
+// The workspace of glic_mapper_render_camera: the camera block (view16 | proj16 | campos4) | an image workspace | glic_render's
+// colour, final T, depth and median depth planes | the scored colour
+struct RenderPlanes { float* cam; void* image_ws; float *color, *T, *depth, *median, *rgb; };
+size_t render_carve(void* ws, int W, int H, RenderPlanes* out) {
+    const size_t HW = (size_t)W * H;
+    Carver c(ws);
+    RenderPlanes r;
+    r.cam = c.take<float>(36);
+    r.image_ws = c.take<char>(glic_image_bytes(W, H));
+    r.color = c.take<float>(3 * HW);
+    r.T = c.take<float>(HW);
+    r.depth = c.take<float>(HW);
+    r.median = c.take<float>(HW);
+    r.rgb = c.take<float>(3 * HW);
+    if (out) *out = r;
+    return c.total();
+}
+
+// glic_mapper_render_camera after its checks: out = rgb, final_T, depth, median_depth (each may be NULL)
+int render_camera(glic_mapper* m, const glic_render_camera& c, int exposure_index, int with_sky, float* const out[4]) {
+    const int W = c.width, H = c.height;
+    const size_t HW = (size_t)W * H;
+    cudaStream_t s = m->stream;
+    MAP_TRY(poll_ring(m, true));
+    MAP_TRY(reserve(m, m->render_ws, render_carve(nullptr, W, H, nullptr)));
+    RenderPlanes r;
+    render_carve(m->render_ws, W, H, &r);
+    CamBlock cb;
+    camera_block(W, H, c.fx, c.fy, c.cx, c.cy, c.R_wc, c.t_wc, cb);
+    GLIC_CUDA_TRY(cudaMemcpyAsync(r.cam, cb.view, 36 * sizeof(float), cudaMemcpyHostToDevice, s));
+    glic_view v{};
+    v.viewmatrix = r.cam; v.projmatrix = r.cam + 16; v.campos = r.cam + 32;
+    v.tan_fovx = cb.tanfovx; v.tan_fovy = cb.tanfovy;
+    v.limx_neg = cb.lim[0]; v.limx_pos = cb.lim[1]; v.limy_neg = cb.lim[2]; v.limy_pos = cb.lim[3];
+    v.width = W; v.height = H;
+    MAP_TRY(activate(m));
+    // the groups are planar: rows [first, P) are the same call on every group pointer offset by `first` rows
+    const size_t first = with_sky ? 0 : m->n_sky;
+    float* g[6];
+    arena_ptrs(m, m->params, m->Pcap, g);
+    for (int attempt = 0; attempt < 4; ++attempt) {           // as forward_settled: an overflow grows the binning and redraws
+        long long* cnt = m->counters_host;
+        MAP_TRY(glic_render((int)(m->P - first), m->D, m->M, g[1] + 3 * first, m->act_scales + 3 * first, 1.0f, m->act_rots + 4 * first,
+                            m->act_opacity + first, g[4] + 3 * first, m->M ? g[5] + (size_t)3 * m->M * first : nullptr, &v,
+                            m->radii + first, m->geom_ws, m->geom_ws.bytes(), r.image_ws, glic_image_bytes(W, H), m->binning_ws,
+                            m->binning_ws.bytes(), r.color, r.T, out[2] ? r.depth : nullptr, out[3] ? r.median : nullptr,
+                            (int64_t*)cnt, s));
+        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+        if (!cnt[2]) break;
+        MAP_TRY(grow_render_binning(m, cnt[0] + cnt[0] / 4));
+        ++m->st.overflow_regrows;
+    }
+    if (out[0]) MAP_TRY(launch_scored_image(H, W, r.color, exposure_index >= 0 ? m->expo_E + 12 * (size_t)exposure_index : nullptr, r.rgb, s));
+    const float* src[4] = {r.rgb, r.T, r.depth, r.median};
+    for (int q = 0; q < 4; ++q)
+        if (out[q]) GLIC_CUDA_TRY(cudaMemcpyAsync(out[q], src[q], sizeof(float) * (q ? HW : 3 * HW), cudaMemcpyDefault, s));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    return GLIC_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1874,15 +1958,7 @@ int glic_mapper_pose_get(glic_mapper* m, int index, float* R_wc9, float* t_wc3, 
 int glic_mapper_pose_set(glic_mapper* m, int index, const float* R_wc9, const float* t_wc3) {
     MAP_TRY(keyframe_index_check(m, true, index, R_wc9, "mapper_pose_set"));
     if (!t_wc3) { set_error("mapper_pose_set: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    for (int j = 0; j < 9; ++j) if (!std::isfinite(R_wc9[j])) { set_error("mapper_pose_set: non-finite entry"); return GLIC_ERR_INVALID_ARGUMENT; }
-    for (int j = 0; j < 3; ++j) if (!std::isfinite(t_wc3[j])) { set_error("mapper_pose_set: non-finite entry"); return GLIC_ERR_INVALID_ARGUMENT; }
-    // a rotation: R^T R = I to float precision and det R = +1
-    double R[9], err = 0.0;
-    for (int j = 0; j < 9; ++j) R[j] = R_wc9[j];
-    for (int a = 0; a < 3; ++a)
-        for (int b = 0; b < 3; ++b) err = std::max(err, std::fabs(R[a] * R[b] + R[3 + a] * R[3 + b] + R[6 + a] * R[6 + b] - (a == b ? 1.0 : 0.0)));
-    const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) + R[2] * (R[3] * R[7] - R[4] * R[6]);
-    if (err > 1e-5 || det < 0.0) { set_error("mapper_pose_set: R_wc is not a rotation (orthonormal, det +1)"); return GLIC_ERR_INVALID_ARGUMENT; }
+    MAP_TRY(pose_check(R_wc9, t_wc3, "mapper_pose_set"));
     return pose_write(m, (size_t)index, R_wc9, t_wc3, false);
 }
 
@@ -1903,6 +1979,30 @@ int glic_mapper_align(glic_mapper* m, int is_train, int index, const glic_align_
     if (m->lpips_w && !glic_lpips_scratch_bytes(H, Ws)) { set_error("mapper_align: LPIPS needs a score region of at least 31x31"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (m->P == 0) { set_error("mapper_align: the map has no rows to align against"); return GLIC_ERR_INVALID_ARGUMENT; }
     return align(m, list[index], is_train != 0, index, *p, out, rgb_host);
+}
+
+int glic_mapper_render_camera(glic_mapper* m, const glic_render_camera* cam, int exposure_index, int with_sky, float* rgb, float* final_T,
+                              float* depth, float* median_depth) {
+    if (!m || !cam || (!rgb && !final_T && !depth && !median_depth)) { set_error("mapper_render_camera: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const glic_render_camera c = *cam;
+    if (c.width < 1 || c.height < 1) { set_error("mapper_render_camera: width and height must be >= 1"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const int64_t tiles = (((int64_t)c.width + TILE - 1) / TILE) * (((int64_t)c.height + TILE - 1) / TILE);
+    if (tiles > GLIC_MAX_TILES) {
+        set_error("mapper_render_camera: " + std::to_string(c.width) + "x" + std::to_string(c.height) + " has " + std::to_string(tiles) +
+                  " tiles of 16x16, more than GLIC_MAX_TILES = " + std::to_string(GLIC_MAX_TILES));
+        return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (!(std::isfinite(c.fx) && c.fx > 0.0f) || !(std::isfinite(c.fy) && c.fy > 0.0f) || !std::isfinite(c.cx) || !std::isfinite(c.cy)) {
+        set_error("mapper_render_camera: fx and fy must be finite and > 0, cx and cy finite"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    MAP_TRY(pose_check(c.R_wc, c.t_wc, "mapper_render_camera"));
+    if (exposure_index != -1 && (!m->expo_on || exposure_index < 0 || exposure_index >= (int)m->train.size())) {
+        set_error("mapper_render_camera: exposure_index must be -1 or a training keyframe index with exposure enabled"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (with_sky != 0 && with_sky != 1) { set_error("mapper_render_camera: with_sky must be 0 or 1"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (m->P == 0) { set_error("mapper_render_camera: the mapper has no rows"); return GLIC_ERR_INVALID_ARGUMENT; }
+    float* const out[4] = {rgb, final_T, depth, median_depth};
+    return render_camera(m, c, exposure_index, with_sky, out);
 }
 
 int glic_mapper_synchronize(glic_mapper* m) {

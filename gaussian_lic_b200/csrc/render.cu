@@ -132,14 +132,23 @@ struct __align__(16) SplatRec { float4 a, b, c; };     // (x, y, conic.x, conic.
 // row cull; everything that differs between the two pixels is evaluated as a pair (f32x2.cuh), in exactly the per-pixel
 // operation order of the scalar formulation (forward.cu:430-453 as pinned in
 // DESIGN.md 3.1), so colour, transmittance and contributor counts keep their bits.
+//
+// INFER (glic_render) is the inference form: the same blend over the same lists in the same operation order, so colour and
+// final T keep their bits, plus the expected depth sum_i T_i alpha_i z_i (unnormalised, like the colour: one more FMA per taken
+// pair, z from the record) and the median depth (z of the first taken splat after which T < 0.5, else 0).  It writes none of
+// the backward's state (checkpoints, bucket_to_tile, n_contrib, max_contrib, pixel_colors); out_depth / out_median may be
+// null.  The training form (INFER = false) compiles every INFER line out.
 constexpr int FWD_THREADS = 128;
 
+template <bool INFER>
 __global__ void __launch_bounds__(FWD_THREADS)
 render_forward_kernel(ViewParams vp, bool no_color, const uint2* __restrict__ ranges,
                       const uint32_t* __restrict__ point_list, const float4* __restrict__ rec,
                       const uint32_t* __restrict__ bucket_offsets, uint32_t* __restrict__ bucket_to_tile,
                       float4* __restrict__ ckpt, uint32_t* __restrict__ n_contrib, uint32_t* __restrict__ max_contrib,
-                      float* __restrict__ pixel_colors, float* __restrict__ out_color, float* __restrict__ out_T) {
+                      float* __restrict__ pixel_colors, float* __restrict__ out_color, float* __restrict__ out_T,
+                      float* __restrict__ out_depth, float* __restrict__ out_median) {
+    if (INFER) no_color = false;                                 // the inference form always blends colour
     __shared__ SplatRec s_rec[2][TILE_PIX];
     __shared__ __align__(8) uint64_t s_bar[2];
     __shared__ uint32_t s_red[FWD_THREADS / 32];
@@ -161,7 +170,7 @@ render_forward_kernel(ViewParams vp, bool no_color, const uint2* __restrict__ ra
 
     if (tid == 0) { mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_fence_init(); }
     uint32_t bbm = 0;
-    if (!no_color) {
+    if (!INFER && !no_color) {
         bbm = tile == 0 ? 0u : bucket_offsets[tile - 1];
         const int nb = (n_splats + BUCKET - 1) / BUCKET;
         for (int b = tid; b < nb; b += FWD_THREADS) bucket_to_tile[bbm + b] = tile;
@@ -187,6 +196,11 @@ render_forward_kernel(ViewParams vp, bool no_color, const uint2* __restrict__ ra
 
     bool done0 = !inside0, done1 = !inside1;
     f2 Tp = f2_bcast(1.0f), Cr = f2_bcast(0.f), Cg = Cr, Cb = Cr;
+    // INFER: a pixel outside the frame is never written and never takes a splat, so it starts at T = 0; the median test below
+    // then stops for its lane as soon as the other pixel is past T = 0.5 (bottom-edge tiles)
+    if (INFER) Tp = f2_pack(inside0 ? 1.0f : 0.0f, inside1 ? 1.0f : 0.0f);
+    f2 Dp = Cr;                             // INFER: expected depth (unnormalised)
+    float med0 = 0.f, med1 = 0.f;           // INFER: median depth (0 until T falls below 0.5)
     uint32_t last0 = 0, last1 = 0;
     int waited = 0;                         // batches whose barrier this thread has consumed
 
@@ -200,7 +214,7 @@ render_forward_kernel(ViewParams vp, bool no_color, const uint2* __restrict__ ra
         const int nb = min(TILE_PIX, n_splats - i * TILE_PIX);
         // one checkpoint per 32-splat bucket, then the bucket's splats
         for (int jb = 0; jb < nb && !(done0 && done1); jb += BUCKET) {
-            if (!no_color) {
+            if (!INFER && !no_color) {
                 float t0, t1, r0, r1, g0, g1, b0, b1;
                 f2_unpack(Tp, t0, t1); f2_unpack(Cr, r0, r1); f2_unpack(Cg, g0, g1); f2_unpack(Cb, b0, b1);
                 float4* k = ckpt + (size_t)bbm * TILE_PIX;
@@ -244,6 +258,15 @@ render_forward_kernel(ViewParams vp, bool no_color, const uint2* __restrict__ ra
                     Cr = f2_fma(Tp, f2_mul(ae, b.z), Cr);
                     Cg = f2_fma(Tp, f2_mul(ae, b.w), Cg);
                     Cb = f2_fma(Tp, f2_mul(ae, c.x), Cb);
+                    if (INFER) {
+                        Dp = f2_fma(Tp, f2_mul(ae, c.y), Dp);
+                        // T only falls: T >= 0.5 before a taken splat and < 0.5 after it marks the first crossing.  Past it
+                        // (most of the pairs of a deep tile) the lane skips the median test altogether
+                        if (fmaxf(t0, t1) >= 0.5f) {
+                            if (!skip0 && t0 >= 0.5f && tt0 < 0.5f) med0 = c.y;
+                            if (!skip1 && t1 >= 0.5f && tt1 < 0.5f) med1 = c.y;
+                        }
+                    }
                 }
                 Tp = f2_pack(skip0 ? t0 : tt0, skip1 ? t1 : tt1);
                 const uint32_t me = (uint32_t)(i * TILE_PIX + j + 1);
@@ -261,6 +284,23 @@ render_forward_kernel(ViewParams vp, bool no_color, const uint2* __restrict__ ra
     float t0, t1, r0, r1, g0, g1, b0, b1;
     f2_unpack(Tp, t0, t1); f2_unpack(Cr, r0, r1); f2_unpack(Cg, g0, g1); f2_unpack(Cb, b0, b1);
     const size_t HW = (size_t)vp.W * vp.H;
+    if (INFER) {
+        float d0, d1;
+        f2_unpack(Dp, d0, d1);
+        if (inside0) {
+            out_T[pid0] = t0;
+            out_color[pid0] = r0; out_color[HW + pid0] = g0; out_color[2 * HW + pid0] = b0;
+            if (out_depth) out_depth[pid0] = d0;
+            if (out_median) out_median[pid0] = med0;
+        }
+        if (inside1) {
+            out_T[pid1] = t1;
+            out_color[pid1] = r1; out_color[HW + pid1] = g1; out_color[2 * HW + pid1] = b1;
+            if (out_depth) out_depth[pid1] = d1;
+            if (out_median) out_median[pid1] = med1;
+        }
+        return;
+    }
     if (inside0) {
         out_T[pid0] = t0;
         if (!no_color) {
@@ -620,10 +660,19 @@ int launch_tile_ranges(int64_t R, const GeomHeader* ghdr, const uint32_t* keys_s
 int launch_render_forward(const ViewParams& vp, bool no_color, const uint32_t* point_list, GeomState g, ImageState img,
                           SampleState smp, float* out_color, float* out_final_T, cudaStream_t s) {
     dim3 grid(vp.grid_x, vp.grid_y), block(FWD_THREADS);
-    render_forward_kernel<<<grid, block, 0, s>>>(vp, no_color, img.ranges, point_list, g.rec, img.bucket_offsets,
-                                                 smp.bucket_to_tile, smp.ckpt,
-                                                 img.n_contrib, img.max_contrib, img.pixel_colors, out_color,
-                                                 out_final_T);
+    render_forward_kernel<false><<<grid, block, 0, s>>>(vp, no_color, img.ranges, point_list, g.rec, img.bucket_offsets,
+                                                        smp.bucket_to_tile, smp.ckpt,
+                                                        img.n_contrib, img.max_contrib, img.pixel_colors, out_color,
+                                                        out_final_T, nullptr, nullptr);
+    GLIC_LAUNCH_CHECK();
+    return GLIC_OK;
+}
+
+int launch_render_infer(const ViewParams& vp, const uint32_t* point_list, GeomState g, ImageState img, float* out_color,
+                        float* out_final_T, float* out_depth, float* out_median, cudaStream_t s) {
+    dim3 grid(vp.grid_x, vp.grid_y), block(FWD_THREADS);
+    render_forward_kernel<true><<<grid, block, 0, s>>>(vp, false, img.ranges, point_list, g.rec, nullptr, nullptr, nullptr,
+                                                       nullptr, nullptr, nullptr, out_color, out_final_T, out_depth, out_median);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }

@@ -495,19 +495,24 @@ int launch_exposure_adam(int S, const int* kf_of_slot, const float* slot_grads, 
 namespace glic {
 namespace {
 
-// clamp both images to [0,1] (gaussian.cpp:756-757) into scratch copies and accumulate the squared error.
-// E (optional, 3 channels): the image is exposed first (see expose()); HW = pixels per plane.
+// element i of the scored image: img exposed by E (optional, 3 channels; see expose()) and clamped to [0,1]
+// (gaussian.cpp:756-757); HW = pixels per plane.  Evaluation and glic_mapper_render_camera both draw their images through it.
+__device__ __forceinline__ float scored_pixel(const float* __restrict__ img, const float* __restrict__ E, size_t HW, size_t i) {
+    float x = img[i];
+    if (E) {
+        const int c = (int)(i / HW);
+        x = expose(img, HW, i - (size_t)c * HW, expo_coef(E, c));
+    }
+    return fminf(fmaxf(x, 0.f), 1.f);
+}
+
+// clamp both images to [0,1] (the image exposed first, scored_pixel) into scratch copies and accumulate the squared error.
 __global__ void __launch_bounds__(256)
 eval_clamp_mse_kernel(size_t N, const float* __restrict__ img, const float* __restrict__ gt, float* __restrict__ a,
                       float* __restrict__ b, double* __restrict__ acc2, const float* __restrict__ E, size_t HW) {
     double se = 0.0;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += (size_t)gridDim.x * blockDim.x) {
-        float x = img[i];
-        if (E) {
-            const int c = (int)(i / HW);
-            x = expose(img, HW, i - (size_t)c * HW, expo_coef(E, c));
-        }
-        x = fminf(fmaxf(x, 0.f), 1.f);
+        const float x = scored_pixel(img, E, HW, i);
         const float y = fminf(fmaxf(gt[i], 0.f), 1.f);
         a[i] = x; b[i] = y;
         const float d = x - y;
@@ -516,6 +521,12 @@ eval_clamp_mse_kernel(size_t N, const float* __restrict__ img, const float* __re
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
     if ((threadIdx.x & 31) == 0 && se != 0.0) atomicAdd(&acc2[0], se);
+}
+
+__global__ void __launch_bounds__(256)
+scored_image_kernel(size_t N, const float* __restrict__ img, const float* __restrict__ E, size_t HW, float* __restrict__ out) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += (size_t)gridDim.x * blockDim.x)
+        out[i] = scored_pixel(img, E, HW, i);
 }
 
 __global__ void __launch_bounds__(256)
@@ -557,6 +568,13 @@ int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, cons
     eval_sum_kernel<<<blocks, 256, 0, s>>>(N, map, acc2);
     GLIC_LAUNCH_CHECK();
     eval_finish_kernel<<<1, 1, 0, s>>>(N, acc2, out2);
+    GLIC_LAUNCH_CHECK();
+    return GLIC_OK;
+}
+
+int launch_scored_image(int H, int W, const float* img, const float* E, float* out, cudaStream_t s) {
+    const size_t N = (size_t)3 * H * W;
+    scored_image_kernel<<<(unsigned)std::min<size_t>((N + 255) / 256, (size_t)NUM_SMS * 8), 256, 0, s>>>(N, img, E, (size_t)H * W, out);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }

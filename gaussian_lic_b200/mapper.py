@@ -270,6 +270,30 @@ class Mapper:
             out["image"] = img
         return out
 
+    def render_camera(self, R_wc, t_wc, width=None, height=None, fx=None, fy=None, cx=None, cy=None, exposure=-1, sky=True,
+                      outputs=("rgb", "final_T", "depth", "median_depth")):
+        """Draw the current map from a camera of the caller's choosing (glic_mapper_render_camera).  R_wc [3,3], t_wc [3] as
+        add_keyframe takes them; the intrinsics and frame size left as None are the configuration's.  exposure: a training
+        keyframe index whose E colours the image (exposure enabled), or -1 for the identity; sky=False leaves the skybox rows
+        out.  Returns a dict of float32 numpy arrays for the requested outputs: rgb [3,H,W] (exposed, clamped to [0,1]),
+        final_T [H,W], depth [H,W] (expected depth, unnormalised: divide by 1 - final_T) and median_depth [H,W]."""
+        c = self.cfg
+        cam = capi.RenderCamera()
+        cam.R_wc[:] = [float(x) for x in np.asarray(R_wc, np.float32).reshape(9)]
+        cam.t_wc[:] = [float(x) for x in np.asarray(t_wc, np.float32).reshape(3)]
+        cam.fx, cam.fy = c.fx if fx is None else float(fx), c.fy if fy is None else float(fy)
+        cam.cx, cam.cy = c.cx if cx is None else float(cx), c.cy if cy is None else float(cy)
+        W, H = self.W if width is None else int(width), self.H if height is None else int(height)
+        cam.width, cam.height = W, H
+        shapes = dict(rgb=(3, H, W), final_T=(H, W), depth=(H, W), median_depth=(H, W))
+        unknown = set(outputs) - set(shapes)
+        if unknown:
+            raise ValueError("unknown outputs: %s" % sorted(unknown))
+        out = {k: np.empty(shapes[k], np.float32) for k in shapes if k in outputs}
+        capi.check(capi.lib.glic_mapper_render_camera(self._h, C.byref(cam), int(exposure), int(bool(sky)),
+                                                      *[_p(out.get(k)) for k in shapes]), "mapper_render_camera")
+        return out
+
     def synchronize(self):
         capi.check(capi.lib.glic_mapper_synchronize(self._h), "mapper_synchronize")
 

@@ -355,6 +355,39 @@ class CRasterizer:
                 break
         return out_color, out_T, radii[:P]
 
+    def render(self, g, view, scale_modifier=1.0, depth=True, median_depth=True, radii=None):
+        """One glic_render call (the inference form of the forward: no sample workspace, nothing saved for a backward) at
+        this rasterizer's size, synchronised; an overflow grows the binning workspace and draws again.  It draws into the
+        workspaces forward() saves its state in, so a backward() belongs to the forward() before any render().  Returns a dict of
+        device tensors: color [3,H,W], final_T [H,W], depth [H,W] (unnormalised expected depth) and median_depth [H,W] when
+        asked for, radii [P], and counters (R, B = 0, overflow) of the last call."""
+        lib = self.lib
+        P = int(g["means"].shape[0])
+        M = int(g["sh"].shape[1]) if g["sh"].numel() else 0
+        f32 = dict(dtype=torch.float32, device=self.dev)
+        out = dict(color=torch.empty(3, self.H, self.W, **f32), final_T=torch.empty(self.H, self.W, **f32),
+                   depth=torch.empty(self.H, self.W, **f32) if depth else None,
+                   median_depth=torch.empty(self.H, self.W, **f32) if median_depth else None)
+        radii = torch.empty(max(P, 1), dtype=torch.int32, device=self.dev) if radii is None else radii
+        self._grow("geom_ws", lib.glic_geom_bytes(P))
+        if self.cap_target == 0:
+            self.cap_target = max(8 * P, 1 << 16)
+        while True:
+            self._grow("binning_ws", lib.glic_binning_bytes(self.cap_target), slack=1.0)
+            capi.check(lib.glic_render(
+                P, int(g["degree"]), M, capi.ptr(g["means"]), capi.ptr(g["scales"]), scale_modifier, capi.ptr(g["rots"]),
+                capi.ptr(g["opacity"]), capi.ptr(g["dc"]), capi.ptr(g["sh"]) if M else None, C.byref(view), capi.ptr(radii),
+                capi.ptr(self.geom_ws), self.geom_ws.numel(), capi.ptr(self.image_ws), self.image_ws.numel(),
+                capi.ptr(self.binning_ws), self.binning_ws.numel(), capi.ptr(out["color"]), capi.ptr(out["final_T"]),
+                capi.ptr(out["depth"]), capi.ptr(out["median_depth"]), capi.ptr(self.counters), self.stream), "render")
+            torch.cuda.synchronize(self.dev)
+            R, B, ovf = (int(x) for x in self.counters.tolist())
+            if not ovf:
+                break
+            self.cap_target = int(R * 1.25) + 4096
+        out["radii"], out["counters"] = radii[:P], (R, B, ovf)
+        return out
+
     def finish(self):
         """Synchronise, publish R / B, and grow the capacity if the last forward overflowed (returns True then)."""
         torch.cuda.synchronize(self.dev)

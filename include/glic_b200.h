@@ -131,6 +131,28 @@ GLIC_API int glic_forward(int P, int sh_degree, int M, const float* means3D, con
                           size_t sample_bytes, float* out_color, float* out_final_T, int64_t* counters_host,
                           void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Render only (inference): the stages of glic_forward up to the blend, unchanged (same preprocess, depth sort, key emission,
+ * tile sort and ranges, hence the same tile lists), then the inference form of the blend.  Per pixel it does the training
+ * blend's work in the training blend's operation order, so out_color and out_final_T equal glic_forward's bit for bit; it
+ * adds two planes and writes none of the state the backward needs (checkpoints, bucket ids, contributor counts, the saved
+ * colour), so there is no sample workspace and no glic_backward after it.
+ *   out_depth[H,W] (may be NULL): expected depth sum_i T_i alpha_i z_i over the splats a pixel takes, z the view-space depth;
+ *     unnormalised like the colour (divide by 1 - out_final_T for the mean depth of what the pixel sees).
+ *   out_median_depth[H,W] (may be NULL): z of the first taken splat after which T < 0.5; 0 where T never falls below 0.5.
+ *   capacity = glic_binning_capacity(binning_bytes, 0, W, H, 1) pairs.  counters_host[3] = {R, 0, overflow} as glic_forward
+ *   with no_color = 1 writes it (asynchronously; overflow != 0: the images are invalid, repeat with room for R pairs).
+ *   No host synchronisation.  P = 0: out_final_T is 1 and every other output 0 (glic_forward writes T = 0 there).  Arguments are checked as glic_forward checks
+ *   them (frame size, GLIC_MAX_TILES, workspaces, null pointers, the 16-byte alignment of rotations).  Profiled under
+ *   GLIC_STAGE_PREPROCESS, _SORT, _EMIT, _RANGES and _RENDER_FWD.
+ * ------------------------------------------------------------------------------------- */
+GLIC_API int glic_render(int P, int sh_degree, int M, const float* means3D, const float* scales, float scale_modifier,
+                         const float* rotations, const float* opacities, const float* dc, const float* sh, const glic_view* view,
+                         int* radii, void* geom_ws, size_t geom_bytes, void* image_ws, size_t image_bytes,
+                         void* binning_ws, size_t binning_bytes, float* out_color, float* out_final_T,
+                         float* out_depth /* may be NULL */, float* out_median_depth /* may be NULL */,
+                         int64_t* counters_host, void* stream);
+
 /* Backward.  Replaces CudaRasterizer::Rasterizer::backward (rasterizer_impl.cu:476-580;
  * backward.cu:138-597) AND the ten torch::zeros of rasterize_points.cu:192-201: every output
  * element is written (exact zeros for culled Gaussians), nothing needs pre-zeroing.
@@ -786,6 +808,37 @@ GLIC_API int glic_mapper_align(glic_mapper* m, int is_train, int index, const gl
  * Rt) | proj[16] (column-major P*Rt) | campos[3] | tan_fovx, tan_fovy | limx_neg, limx_pos, limy_neg, limy_pos. */
 GLIC_API int glic_camera_block(int width, int height, float fx, float fy, float cx, float cy, const float* R_wc /*[9] row-major*/,
                                const float* t_wc /*[3]*/, float* out41);
+/* Rendering the map from any camera: glic_mapper_render_camera(m, cam, exposure_index, with_sky, rgb, final_T, depth,
+ * median_depth) draws the current map (parameters, sky rows, fitted exposures, refined poses as they stand) with glic_render
+ * from a camera the caller chooses: a fly-through, a frame at display resolution, a depth map for meshing or a LiDAR check.
+ *   - camera: glic_camera_block(cam->width, cam->height, fx, fy, cx, cy, R_wc, t_wc), the closed form every keyframe uses;
+ *   - rgb [3,H,W]: the colour with training keyframe exposure_index's E applied (-1: the identity), clamped to [0,1], by the
+ *     device code glic_mapper_render's image goes through; final_T [H,W], depth [H,W] and median_depth [H,W] are glic_render's
+ *     raw planes.  Each output is host or device memory (copied with cudaMemcpyDefault) or NULL; at least one is non-NULL;
+ *   - with_sky = 1 draws every row; 0 only rows [S, P) (glic_mapper_sky_rows), the map without the skybox;
+ *   - at training keyframe k's current float pose (glic_mapper_pose_get, or the stored pose), the configured intrinsics and
+ *     size, exposure_index = k with exposure enabled (-1 otherwise) and with_sky = 1, rgb equals glic_mapper_render(m, 1, k)
+ *     bit for bit; at a held-out keyframe's pose with exposure_index = -1 it equals glic_mapper_render(m, 0, k);
+ *   - with_sky = 0 on a map of sky rows only draws nothing: final_T 1, every other plane 0;
+ *   - binning: the mapper's binning workspace; a frame that overflows it grows it and is drawn again, as evaluation does
+ *     (stats.overflow_regrows counts it).  Only the binning workspace grows, to about 20-32 B per (tile, Gaussian) pair of the
+ *     largest frame drawn, and it is kept; the training's checkpoint (sample) workspace is neither used nor grown;
+ *   - memory: a render workspace kept for the next call, for the largest frame asked for so far: the camera block, an image
+ *     workspace and six planes, about 52 B per pixel.  Everything is reserved before anything runs (failure contract above).
+ * The map is frozen, exactly as under glic_mapper_align: no parameter, moment, statistic, keyframe, pose, camera block, E, Adam
+ * state, sampler state or density-control counter changes, and no stats field but overflow_regrows.  The call drains the
+ * iteration pipeline first and synchronises at the end.  With world > 1 it is rank-local and touches no exchange slot.
+ * Rejected with GLIC_ERR_INVALID_ARGUMENT, changing nothing: a NULL m or cam, or all four outputs NULL; width or height < 1,
+ * or more than GLIC_MAX_TILES tiles; fx or fy not finite and > 0, cx or cy not finite; a non-finite pose, or an R_wc that is
+ * not a rotation (glic_mapper_pose_set's test); exposure_index not -1 and not a training index with exposure enabled;
+ * with_sky not 0 or 1; a mapper with no rows. */
+typedef struct glic_render_camera {
+    float R_wc[9], t_wc[3];            /* row-major, as glic_keyframe */
+    float fx, fy, cx, cy;
+    int width, height;
+} glic_render_camera;
+GLIC_API int glic_mapper_render_camera(glic_mapper* m, const glic_render_camera* cam, int exposure_index, int with_sky,
+                                       float* rgb, float* final_T, float* depth, float* median_depth);
 /* Raw frames (Dataset::addFrame, gaussian.cpp:41-111, and the keyframe hand-off of mapping.cpp:158-174): the host feeds every
  * aligned camera frame with its odometry pose and LiDAR scan; the mapper selects the keyframes, keeps each image as 8 bits
  * in HBM and builds or extends the map on the GPU.  optimize() stays the caller's call (mapping.cpp:178).
