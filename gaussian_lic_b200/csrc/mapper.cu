@@ -17,6 +17,7 @@
 #include "adam_math.cuh"
 
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <cmath>
 #include <cstring>
@@ -110,6 +111,11 @@ void camera_block(int W, int H, double fx, double fy, double cx, double cy, cons
     const float ffx = (float)fx, ffy = (float)fy, fcx = (float)cx, fcy = (float)cy;
     o.lim[0] = -0.15f * W / ffx - fcx / ffx; o.lim[1] = 1.15f * W / ffx - fcx / ffx;
     o.lim[2] = -0.15f * H / ffy - fcy / ffy; o.lim[3] = 1.15f * H / ffy - fcy / ffy;
+}
+
+// the rasterizer's view of a W x H frame from c's scalars and cam, the 36 device floats of c's view | proj | campos
+glic_view make_view(const CamBlock& c, const float* cam, int W, int H) {
+    return glic_view{cam, cam + 16, cam + 32, c.tanfovx, c.tanfovy, c.lim[0], c.lim[1], c.lim[2], c.lim[3], W, H};
 }
 
 // ---- ownership: every CUDA resource of a mapper is a member of one of the two types below, and only they allocate or release
@@ -438,13 +444,32 @@ int reserve(glic_mapper* m, Buf& b, size_t need) { return need <= b.bytes() ? GL
 
 size_t arena_floats(const glic_mapper* m, uint32_t cap) { return glic_packed_floats(cap, (uint32_t)m->M); }
 
-void arena_ptrs(const glic_mapper* m, float* base, uint32_t cap, float* out6[6]) {
+// The six row groups of a packed block of capacity cap (an arena, or with M = 0 the exchange block's gradients), in
+// glic_packed_offsets order; rest is null without SH rest (M = 0)
+struct ArenaRows {
+    float *rot, *xyz, *log_scale, *opacity, *dc, *rest;
+    std::array<float*, 6> groups() const { return {rot, xyz, log_scale, opacity, dc, rest}; }
+};
+ArenaRows arena_rows(float* base, uint32_t cap, int M) {
     size_t off[6];
-    glic_packed_offsets(cap, (uint32_t)m->M, off);
-    for (int q = 0; q < 6; ++q) out6[q] = base + off[q];
+    glic_packed_offsets(cap, (uint32_t)M, off);
+    return {base + off[0], base + off[1], base + off[2], base + off[3], base + off[4], M ? base + off[5] : nullptr};
 }
+// floats per row of each group, in the same order
+std::array<size_t, 6> group_widths(int M) { return {4, 3, 3, 1, 3, (size_t)3 * M}; }
 
 float* geo_ptr(const glic_mapper* m) { return static_cast<float*>(m->xblock.raw()); }
+
+void config_camera_block(const glic_mapper* m, const float* R_wc, const float* t_wc, CamBlock& o, double* T12 = nullptr) {
+    camera_block(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, R_wc, t_wc, o, T12);
+}
+
+int keyframe_at(glic_mapper* m, int is_train, int index, const char* what, const Keyframe*& out) {
+    const auto& list = is_train ? m->train : m->test;
+    if (index < 0 || index >= (int)list.size()) { set_error(std::string(what) + ": keyframe index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
+    out = &list[index];
+    return GLIC_OK;
+}
 
 // view slot s of parity `parity` in region r of the exchange block
 template <typename T = float>
@@ -553,7 +578,7 @@ int pose_write(glic_mapper* m, size_t k, const float* R_wc, const float* t_wc, b
     std::memcpy(R, R_wc, sizeof(R)); std::memcpy(t, t_wc, sizeof(t));
     std::memcpy(kf.R_wc, R, sizeof(R)); std::memcpy(kf.t_wc, t, sizeof(t));
     double T12[12];
-    camera_block(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, kf.R_wc, kf.t_wc, kf.cam, T12);
+    config_camera_block(m, kf.R_wc, kf.t_wc, kf.cam, T12);
     float f12[12];
     std::memcpy(f12, kf.R_wc, 36); std::memcpy(f12 + 9, kf.t_wc, 12);
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
@@ -574,18 +599,23 @@ int dens_reset(glic_mapper* m) {
     return GLIC_OK;
 }
 
+// pose_step_kernel on the first S slots of b, with the configuration's projection, on the mapper's stream
+int launch_pose_kernel(glic_mapper* m, int S, PoseBatch b, const float* slot_grads, double* T, float* pose_f, float* adam_m, float* adam_v,
+                       int* adam_t, float lr_rho, float lr_omega, const unsigned int* skip) {
+    float fov2[2];
+    proj_matrix(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, b.Pm, fov2);
+    pose_step_kernel<<<1, MAX_SLOTS, 0, m->stream>>>(S, b, slot_grads, T, pose_f, adam_m, adam_v, adam_t, lr_rho, lr_omega, skip);
+    GLIC_LAUNCH_CHECK();
+    return GLIC_OK;
+}
+
 int launch_pose_step(glic_mapper* m, const int* views, int parity) {
     PoseBatch b{};
     for (int sl = 0; sl < m->S; ++sl) { b.kf[sl] = views[sl]; b.cam[sl] = m->train[views[sl]].cam_dev; }
-    float fov2[2];
-    proj_matrix(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, b.Pm, fov2);
     StageTimer _t(GLIC_STAGE_ADAM, m->stream);
     const KeyframeAdam& a = m->pose_adam;
-    pose_step_kernel<<<1, MAX_SLOTS, 0, m->stream>>>(m->S, b, slot(m, POSE, parity, 0), m->pose_T, m->pose_f, a.m, a.v, a.t,
-                                                     m->pose_lr_rho, m->pose_lr_omega,
-                                                     reinterpret_cast<const unsigned int*>(geo_ptr(m) + (size_t)11 * m->Pcap));
-    GLIC_LAUNCH_CHECK();
-    return GLIC_OK;
+    return launch_pose_kernel(m, m->S, b, slot(m, POSE, parity, 0), m->pose_T, m->pose_f, a.m, a.v, a.t, m->pose_lr_rho, m->pose_lr_omega,
+                              reinterpret_cast<const unsigned int*>(geo_ptr(m) + (size_t)11 * m->Pcap));
 }
 
 int set_bin_capacity(glic_mapper* m, int64_t pairs, bool exact = false) {
@@ -605,6 +635,13 @@ int grow_render_binning(glic_mapper* m, int64_t pairs) {
     return GLIC_OK;
 }
 
+// after draws skipped on the device for want of room for up to `pairs` pairs: that with a quarter to spare, and at least 1.5x as much
+int regrow_after_skip(glic_mapper* m, int64_t pairs) {
+    MAP_TRY(set_bin_capacity(m, std::max<int64_t>(pairs + pairs / 4, m->bin_cap * 3 / 2)));
+    ++m->st.overflow_regrows;
+    return GLIC_OK;
+}
+
 // lagged, non-blocking look at the pinned binning counters of finished iterations
 int poll_ring(glic_mapper* m, bool wait) {
     for (int r = 0; r < RING; ++r) {
@@ -615,41 +652,43 @@ int poll_ring(glic_mapper* m, bool wait) {
         m->ring_used[r] = false;
         const long long* c = m->counters_host + 4 * r;
         m->st.last_loss = m->loss_host[r];
-        if (c[2]) {                                        // this frame overflowed the binning workspace: it was skipped on the device
-            MAP_TRY(set_bin_capacity(m, std::max<int64_t>(c[0] + c[0] / 4, m->bin_cap * 3 / 2)));
-            ++m->st.overflow_regrows;
-        }
+        if (c[2]) MAP_TRY(regrow_after_skip(m, c[0]));     // this frame overflowed the binning workspace: it was skipped on the device
     }
     return GLIC_OK;
 }
 
 int activate(glic_mapper* m) {
-    float* g[6];
-    arena_ptrs(m, m->params, m->Pcap, g);
-    return glic_activations_forward((int)m->P, g[3], g[2], g[0], m->act_opacity, m->act_scales, m->act_rots, m->stream);
+    const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
+    return glic_activations_forward((int)m->P, a.opacity, a.log_scale, a.rot, m->act_opacity, m->act_scales, m->act_rots, m->stream);
 }
 
-int forward_view(glic_mapper* m, const Keyframe& kf, int no_color, long long* counters) {
-    float* g[6];
-    arena_ptrs(m, m->params, m->Pcap, g);
-    return glic_forward((int)m->P, m->D, m->M, g[1], m->act_scales, 1.0f, m->act_rots, m->act_opacity, g[4], m->M ? g[5] : nullptr, &kf.view,
-                        no_color, m->radii, m->geom_ws, m->geom_ws.bytes(), m->image_ws, m->image_ws.bytes(), m->binning_ws,
-                        m->binning_ws.bytes(), m->sample_ws, m->sample_ws.bytes(), m->color, m->final_T, (int64_t*)counters, m->stream);
+int forward_view(glic_mapper* m, const glic_view& v, int no_color, long long* counters) {
+    const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
+    return glic_forward((int)m->P, m->D, m->M, a.xyz, m->act_scales, 1.0f, m->act_rots, m->act_opacity, a.dc, a.rest, &v, no_color, m->radii,
+                        m->geom_ws, m->geom_ws.bytes(), m->image_ws, m->image_ws.bytes(), m->binning_ws, m->binning_ws.bytes(), m->sample_ws,
+                        m->sample_ws.bytes(), m->color, m->final_T, (int64_t*)counters, m->stream);
 }
 
-// activations and a synchronous forward of kf: a binning overflow grows the workspace and renders again, up to 4 attempts.
-// The caller has drained the ring (poll_ring(wait)), so ring slot 0's pinned counters are free.
-int forward_settled(glic_mapper* m, const Keyframe& kf, int no_color) {
-    MAP_TRY(activate(m));
+// draw(counters), then a synchronisation; a binning overflow grows the workspace by regrow(pairs needed), counts the regrow and
+// draws again, up to 4 attempts.  The caller has drained the ring (poll_ring(wait)), so ring slot 0's pinned counters are free.
+template <typename Draw, typename Regrow>
+int draw_settled(glic_mapper* m, Draw draw, Regrow regrow) {
     for (int attempt = 0; attempt < 4; ++attempt) {
         long long* cnt = m->counters_host;
-        MAP_TRY(forward_view(m, kf, no_color, cnt));
+        MAP_TRY(draw(cnt));
         GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
         if (!cnt[2]) break;
-        MAP_TRY(set_bin_capacity(m, cnt[0] + cnt[0] / 4));
+        MAP_TRY(regrow(cnt[0] + cnt[0] / 4));
         ++m->st.overflow_regrows;
     }
     return GLIC_OK;
+}
+
+// activations and a settled forward of v with the training workspaces
+int forward_settled(glic_mapper* m, const glic_view& v, int no_color) {
+    MAP_TRY(activate(m));
+    return draw_settled(m, [&](long long* cnt) { return forward_view(m, v, no_color, cnt); },
+                        [&](int64_t pairs) { return set_bin_capacity(m, pairs); });
 }
 
 // keyframe kf's float image [3,H,W] into dst on stream s: an add_frame keyframe's 8-bit image decoded from the frame store,
@@ -663,6 +702,22 @@ int load_gt(glic_mapper* m, const Keyframe& kf, float* dst, cudaMemcpyKind kind,
 
 __global__ void overflow_word_kernel(const GeomHeader* ghdr, float* word) { if (ghdr->overflow) *word = 1.0f; }
 
+// the L1 + D-SSIM loss of an H x W image against gt, and its dL/dimg; with E (device, 3x4) the loss of the exposed image, and dL/dE
+int photometric_loss(glic_mapper* m, int H, int W, const float* img, const float* gt, const float* E, float* loss, float* dL_dimg, float* dL_dE) {
+    if (E)
+        return glic_l1_ssim_loss_exposure(H, W, m->cfg.lambda_dssim, img, gt, E, loss, dL_dimg, dL_dE, m->loss_scratch, m->loss_scratch.bytes(),
+                                          m->stream);
+    return glic_l1_ssim_loss(3, H, W, m->cfg.lambda_dssim, img, gt, loss, dL_dimg, m->loss_scratch, m->loss_scratch.bytes(), m->stream);
+}
+
+// the backward of the last forward_view of v from dL_dpix: colour gradients into col, after_render (optional) recorded, then cg's
+int backward_view(glic_mapper* m, const glic_view& v, float* col, const CompactGrads& cg, cudaEvent_t after_render) {
+    const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
+    return glic_backward_compact_internal((int)m->P, m->D, m->M, a.xyz, m->act_scales, m->act_rots, a.rest, &v, m->radii, m->bin_cap, m->geom_ws,
+                                          m->binning_ws, m->image_ws, m->sample_ws, m->dL_dpix, m->g_mean2D, m->g_conic, m->g_opacity, col,
+                                          &cg, after_render, m->stream);
+}
+
 // one optimiser step over the view batch `views` (S keyframe indices, slot-major); this rank renders slots [rank*k, rank*k + k)
 int iteration(glic_mapper* m, const int* views) {
     if (m->P == 0) return GLIC_OK;
@@ -675,15 +730,12 @@ int iteration(glic_mapper* m, const int* views) {
     cudaStream_t s = m->stream;
     const int parity = (int)(m->st.iterations & 1);
     const int W = m->cfg.width, H = m->cfg.height;
-    float* g[6];
-    arena_ptrs(m, m->params, m->Pcap, g);
     float* geo = geo_ptr(m);
+    const ArenaRows a = arena_rows(m->params, m->Pcap, m->M), ga = arena_rows(geo, m->Pcap, 0);
     float* geo_tail = geo + (size_t)11 * m->Pcap;
     GLIC_CUDA_TRY(cudaMemsetAsync(geo_tail, 0, 4 * sizeof(float), s));
     GLIC_CUDA_TRY(cudaMemsetAsync(m->loss_dev, 0, sizeof(float) * 2, s));
     MAP_TRY(activate(m));
-    size_t goff[6];
-    glic_packed_offsets(m->Pcap, 0, goff);
     for (int j = 0; j < m->k; ++j) {
         const int sl = m->cfg.rank * m->k + j;
         const Keyframe& kf = m->train[views[sl]];
@@ -693,7 +745,7 @@ int iteration(glic_mapper* m, const int* views) {
         GLIC_CUDA_TRY(cudaStreamWaitEvent(m->copy_stream, m->gt_free[buf], 0));
         MAP_TRY(load_gt(m, kf, m->gt_dev[buf], cudaMemcpyDefault, m->copy_stream));
         GLIC_CUDA_TRY(cudaEventRecord(m->gt_ready[buf], m->copy_stream));
-        MAP_TRY(forward_view(m, kf, 0, j == m->k - 1 ? m->counters_host + 4 * r : nullptr));
+        MAP_TRY(forward_view(m, kf.view, 0, j == m->k - 1 ? m->counters_host + 4 * r : nullptr));
         uint8_t* fl = slot<uint8_t>(m, FLAGS, parity, sl);
         float* col = slot(m, COLOUR, parity, sl);
         int* rad = m->dens_on ? slot<int>(m, RADII, parity, sl) : nullptr;           // this view's radii for the screen-size statistic
@@ -708,23 +760,18 @@ int iteration(glic_mapper* m, const int* views) {
         }
         GLIC_CUDA_TRY(cudaStreamWaitEvent(s, m->gt_ready[buf], 0));
         // loss of this view (the pinned ring keeps the last local view's value for the statistics)
-        if (m->expo_on)
-            MAP_TRY(glic_l1_ssim_loss_exposure(H, W, m->cfg.lambda_dssim, m->color, m->gt_dev[buf], m->expo_E + 12 * (size_t)views[sl], m->loss_dev + 1,
-                                               m->dL_dpix, slot(m, EXPOSURE, parity, sl), m->loss_scratch, m->loss_scratch.bytes(), s));
-        else
-            MAP_TRY(glic_l1_ssim_loss(3, H, W, m->cfg.lambda_dssim, m->color, m->gt_dev[buf], m->loss_dev + 1, m->dL_dpix, m->loss_scratch, m->loss_scratch.bytes(), s));
+        MAP_TRY(photometric_loss(m, H, W, m->color, m->gt_dev[buf], m->expo_on ? m->expo_E + 12 * (size_t)views[sl] : nullptr, m->loss_dev + 1,
+                                 m->dL_dpix, slot(m, EXPOSURE, parity, sl)));
         GLIC_CUDA_TRY(cudaEventRecord(m->gt_free[buf], s));
         CompactGrads cg;
-        cg.g_rot = reinterpret_cast<float4*>(geo + goff[0]); cg.g_xyz = geo + goff[1]; cg.g_scale = geo + goff[2]; cg.g_opacity = geo + goff[3];
-        cg.opacity = m->act_opacity; cg.dL_dopacity = m->g_opacity; cg.rot_raw = reinterpret_cast<const float4*>(g[0]);
+        cg.g_rot = reinterpret_cast<float4*>(ga.rot); cg.g_xyz = ga.xyz; cg.g_scale = ga.log_scale; cg.g_opacity = ga.opacity;
+        cg.opacity = m->act_opacity; cg.dL_dopacity = m->g_opacity; cg.rot_raw = reinterpret_cast<const float4*>(a.rot);
         cg.accumulate = j > 0;
         cg.pose_partials = m->pose_on ? (double*)m->pose_part : nullptr;        // this view's dL/d(rho, omega), fused into the backward
         cg.pose_grad = m->pose_on ? slot(m, POSE, parity, sl) : nullptr;
         cg.dens_norm = m->dens_on ? geo_tail + 4 : nullptr;                        // this view's statistics, summed over the rank's views
         cg.dens_count = m->dens_on ? geo_tail + 4 + m->Pcap : nullptr;
-        MAP_TRY(glic_backward_compact_internal((int)m->P, m->D, m->M, g[1], m->act_scales, m->act_rots, m->M ? g[5] : nullptr, &kf.view, m->radii,
-                                               m->bin_cap, m->geom_ws, m->binning_ws, m->image_ws, m->sample_ws, m->dL_dpix, m->g_mean2D,
-                                               m->g_conic, m->g_opacity, col, &cg, m->cfg.world > 1 ? (void*)m->ev_col : nullptr, s));
+        MAP_TRY(backward_view(m, kf.view, col, cg, m->cfg.world > 1 ? (cudaEvent_t)m->ev_col : nullptr));
         if (m->cfg.world > 1 && m->pose_on) GLIC_CUDA_TRY(cudaEventRecord(m->ev_pose, s));   // after the pose finish kernel
         if (m->cfg.world > 1) {
             GLIC_CUDA_TRY(cudaStreamWaitEvent(m->push_stream, m->ev_col, 0));
@@ -810,16 +857,30 @@ int keyframe_adam_state(glic_mapper* m, bool pose, int index, float* exp_avg, fl
 // the clamped image (a training keyframe's E applied first; held-out views: identity) and the clamped ground truth stay in the
 // evaluation scratch (eval_clamped).  Asynchronous after the settled forward.
 int render_scored(glic_mapper* m, int is_train, int index, const char* what) {
-    auto& list = is_train ? m->train : m->test;
-    if (index < 0 || index >= (int)list.size()) { set_error(std::string(what) + ": keyframe index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const Keyframe* kf = nullptr;
+    MAP_TRY(keyframe_at(m, is_train, index, what, kf));
     MAP_TRY(poll_ring(m, true));
-    const Keyframe& kf = list[index];
     cudaStream_t s = m->stream;
     const int W = m->cfg.width, H = m->cfg.height;
-    MAP_TRY(forward_settled(m, kf, 0));
-    MAP_TRY(load_gt(m, kf, m->gt_dev[0], cudaMemcpyHostToDevice, s));
+    MAP_TRY(forward_settled(m, kf->view, 0));
+    MAP_TRY(load_gt(m, *kf, m->gt_dev[0], cudaMemcpyHostToDevice, s));
     const float* E = (is_train && m->expo_on) ? m->expo_E + 12 * (size_t)index : nullptr;
     return eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], E, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s);
+}
+
+// the whole clamped image eval_psnr_ssim last scored (eval_clamped) into rgb_host, on the mapper's stream
+int scored_image_to_host(glic_mapper* m, float* rgb_host) {
+    const int W = m->cfg.width, H = m->cfg.height;
+    GLIC_CUDA_TRY(cudaMemcpyAsync(rgb_host, eval_clamped(m->eval_scratch, 3, H, W, 0), sizeof(float) * 3 * (size_t)W * H,
+                                  cudaMemcpyDeviceToHost, m->stream));
+    return GLIC_OK;
+}
+
+// LPIPS of the clamped pair eval_psnr_ssim last scored, W columns wide, into eval_out[2]
+int scored_lpips(glic_mapper* m, int W) {
+    const int H = m->cfg.height;
+    return glic_lpips(H, W, eval_clamped(m->eval_scratch, 3, H, W, 0), eval_clamped(m->eval_scratch, 3, H, W, 1), m->lpips_w, m->eval_out + 2,
+                      m->lpips_scratch, m->lpips_scratch.bytes(), m->stream);
 }
 
 // copies n floats of eval_out to the host and waits for them
@@ -829,29 +890,40 @@ int read_eval_out(glic_mapper* m, float* out, int n) {
     return GLIC_OK;
 }
 
+// a new map of P rows: the binning room for it, reserved before the map is replaced (a failure leaves it as it was), then zero
+// arenas and (with densification on) zero statistics, on the mapper's stream
+int start_map(glic_mapper* m, uint32_t P) {
+    MAP_TRY(set_bin_capacity(m, (int64_t)16 * P));
+    const size_t nfl = arena_floats(m, m->Pcap);
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->params, 0, nfl * 4, m->stream));
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->m1, 0, nfl * 4, m->stream));
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->m2, 0, nfl * 4, m->stream));
+    return dens_reset(m);
+}
+
+// once the mapper's stream has drained: the map is the P rows written since start_map, the first n_sky of them the skybox
+int install_map(glic_mapper* m, uint32_t P, uint32_t n_sky) {
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    m->P = P;
+    m->n_sky = n_sky;
+    m->st.num_gaussians = P;
+    m->initialized = true;
+    return GLIC_OK;
+}
+
 // initialize() (gaussian.cpp:212-304) from device arrays: the sky rows, then the n LiDAR rows.  The caller has validated the
 // arguments, sized the arena for sky_points + n rows and hands sky_ws of glic_skybox_init_bytes(sky_points) bytes.
 int initialize_lidar_core(glic_mapper* m, int n, const float* d_pts, const double* d_col, const float* d_dep, double focal, int sky_points,
                           int sky_radius, void* sky_ws) {
     const uint32_t S = (uint32_t)sky_points, P = S + (uint32_t)n;
-    MAP_TRY(set_bin_capacity(m, (int64_t)16 * P));  // before the map is replaced: a failure leaves it as it was
+    MAP_TRY(start_map(m, P));
     cudaStream_t s = m->stream;
-    const size_t nfl = arena_floats(m, m->Pcap);
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->params, 0, nfl * 4, s));
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->m1, 0, nfl * 4, s));
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->m2, 0, nfl * 4, s));
-    MAP_TRY(dens_reset(m));
-    float* g[6];                                    // rot, xyz, log-scale, opacity, f_dc, f_rest
-    arena_ptrs(m, m->params, m->Pcap, g);
-    MAP_TRY(glic_skybox_init(sky_points, sky_radius, m->cfg.seed, sky_ws, glic_skybox_init_bytes(sky_points), g[1], g[4], g[2], g[0], g[3], nullptr, s));
-    MAP_TRY(glic_lidar_init(n, d_pts, d_col, d_dep, (double)m->cfg.scaling_scale, focal, g[1] + 3 * (size_t)S, g[4] + 3 * (size_t)S,
-                            g[2] + 3 * (size_t)S, g[0] + 4 * (size_t)S, g[3] + S, s));
-    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-    m->P = P;
-    m->n_sky = S;
-    m->st.num_gaussians = P;
-    m->initialized = true;
-    return GLIC_OK;
+    const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
+    MAP_TRY(glic_skybox_init(sky_points, sky_radius, m->cfg.seed, sky_ws, glic_skybox_init_bytes(sky_points), a.xyz, a.dc, a.log_scale, a.rot,
+                             a.opacity, nullptr, s));
+    MAP_TRY(glic_lidar_init(n, d_pts, d_col, d_dep, (double)m->cfg.scaling_scale, focal, a.xyz + 3 * (size_t)S, a.dc + 3 * (size_t)S,
+                            a.log_scale + 3 * (size_t)S, a.rot + 4 * (size_t)S, a.opacity + S, s));
+    return install_map(m, P, S);
 }
 
 // extend()'s workspace after its inputs: outputs (keep_idx, xyz, f_dc, log_scale, rot, opacity) | glic_extend's own
@@ -882,7 +954,7 @@ int extend_core(glic_mapper* m, const Keyframe& kf, int n, const float* d_pts, c
     float *d_xyz = o[0], *d_dc = o[1], *d_ls = o[2], *d_rot = o[3], *d_op = o[4];
     // alpha-only render of the newest keyframe (gaussian.cpp:506-507); the binning capacity is settled synchronously here
     if (m->P) {
-        MAP_TRY(forward_settled(m, kf, 1));
+        MAP_TRY(forward_settled(m, kf.view, 1));
     } else {
         std::vector<float> ones((size_t)W * H, 1.0f);                                       // empty model: alpha = 1 - T = 0
         GLIC_CUDA_TRY(cudaMemcpyAsync(m->final_T, ones.data(), sizeof(float) * ones.size(), cudaMemcpyHostToDevice, s));
@@ -923,15 +995,12 @@ int make_keyframe(glic_mapper* m, const float* R_wc, const float* t_wc, const fl
     std::memcpy(kf.R_wc, R_wc, sizeof(kf.R_wc)); std::memcpy(kf.t_wc, t_wc, sizeof(kf.t_wc));
     kf.image = image;
     kf.bgr = bgr;
-    camera_block(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, kf.R_wc, kf.t_wc, kf.cam);
+    config_camera_block(m, kf.R_wc, kf.t_wc, kf.cam);
     MAP_TRY(kf.cam_dev.allocate(36 * sizeof(float)));
     // view | proj | campos are contiguous; ordered before every use of the block, all of which are on the mapper's stream or after
     // a synchronisation of it
     GLIC_CUDA_TRY(cudaMemcpyAsync(kf.cam_dev, kf.cam.view, 36 * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-    kf.view.viewmatrix = kf.cam_dev; kf.view.projmatrix = kf.cam_dev + 16; kf.view.campos = kf.cam_dev + 32;
-    kf.view.tan_fovx = kf.cam.tanfovx; kf.view.tan_fovy = kf.cam.tanfovy;
-    kf.view.limx_neg = kf.cam.lim[0]; kf.view.limx_pos = kf.cam.lim[1]; kf.view.limy_neg = kf.cam.lim[2]; kf.view.limy_pos = kf.cam.lim[3];
-    kf.view.width = m->cfg.width; kf.view.height = m->cfg.height;
+    kf.view = make_view(kf.cam, kf.cam_dev, m->cfg.width, m->cfg.height);
     return GLIC_OK;
 }
 
@@ -1049,25 +1118,13 @@ int glic_mapper_initialize(glic_mapper* m, uint32_t P, const float* xyz, const f
                            const float* log_scale, const float* rot) {
     if (!m || (P && (!xyz || !f_dc || !opacity_logit || !log_scale || !rot))) { set_error("mapper_initialize: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
     MAP_TRY(set_capacity(m, P));
-    MAP_TRY(set_bin_capacity(m, (int64_t)16 * P));
-    cudaStream_t s = m->stream;
-    const size_t nfl = arena_floats(m, m->Pcap);
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->params, 0, nfl * 4, s));
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->m1, 0, nfl * 4, s));
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->m2, 0, nfl * 4, s));
-    MAP_TRY(dens_reset(m));
-    float* g[6];
-    arena_ptrs(m, m->params, m->Pcap, g);
+    MAP_TRY(start_map(m, P));
+    const auto g = arena_rows(m->params, m->Pcap, m->M).groups();
+    const auto kk = group_widths(m->M);
     const float* src[6] = {rot, xyz, log_scale, opacity_logit, f_dc, f_rest};
-    const size_t kk[6] = {4, 3, 3, 1, 3, (size_t)3 * m->M};
     for (int q = 0; q < 6; ++q)
-        if (P && kk[q] && src[q]) GLIC_CUDA_TRY(cudaMemcpyAsync(g[q], src[q], sizeof(float) * kk[q] * P, cudaMemcpyHostToDevice, s));
-    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-    m->P = P;
-    m->n_sky = 0;
-    m->st.num_gaussians = P;
-    m->initialized = true;
-    return GLIC_OK;
+        if (P && kk[q] && src[q]) GLIC_CUDA_TRY(cudaMemcpyAsync(g[q], src[q], sizeof(float) * kk[q] * P, cudaMemcpyHostToDevice, m->stream));
+    return install_map(m, P, 0);
 }
 
 int glic_mapper_initialize_lidar(glic_mapper* m, int n, const float* points, const double* colors, const float* depth_rsp, double focal,
@@ -1202,16 +1259,15 @@ int glic_mapper_add_frame(glic_mapper* m, const glic_frame* f, int* is_keyframe)
 
 int glic_mapper_keyframe_image(glic_mapper* m, int is_train, int index, float* rgb_host) {
     if (!m || !rgb_host) { set_error("mapper_keyframe_image: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    const auto& list = is_train ? m->train : m->test;
-    if (index < 0 || index >= (int)list.size()) { set_error("mapper_keyframe_image: keyframe index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
-    const Keyframe& kf = list[index];
+    const Keyframe* kf = nullptr;
+    MAP_TRY(keyframe_at(m, is_train, index, "mapper_keyframe_image", kf));
     const size_t bytes = sizeof(float) * 3 * (size_t)m->cfg.width * m->cfg.height;
-    if (!kf.bgr) {
-        GLIC_CUDA_TRY(cudaMemcpy(rgb_host, kf.image, bytes, cudaMemcpyDefault));
+    if (!kf->bgr) {
+        GLIC_CUDA_TRY(cudaMemcpy(rgb_host, kf->image, bytes, cudaMemcpyDefault));
         return GLIC_OK;
     }
     MAP_TRY(poll_ring(m, true));                          // the iterations' use of gt_dev[0] has finished (see render_scored)
-    MAP_TRY(load_gt(m, kf, m->gt_dev[0], cudaMemcpyHostToDevice, m->stream));
+    MAP_TRY(load_gt(m, *kf, m->gt_dev[0], cudaMemcpyHostToDevice, m->stream));
     GLIC_CUDA_TRY(cudaMemcpyAsync(rgb_host, m->gt_dev[0], bytes, cudaMemcpyDeviceToHost, m->stream));
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     return GLIC_OK;
@@ -1302,8 +1358,7 @@ int glic_mapper_evaluate_lpips(glic_mapper* m, int is_train, int index, float* p
     if (!need) { set_error("mapper_evaluate_lpips: LPIPS needs a frame of at least 31x31"); return GLIC_ERR_INVALID_ARGUMENT; }
     MAP_TRY(reserve(m, m->lpips_scratch, need));
     MAP_TRY(render_scored(m, is_train, index, "mapper_evaluate_lpips"));
-    MAP_TRY(glic_lpips(H, W, eval_clamped(m->eval_scratch, 3, H, W, 0), eval_clamped(m->eval_scratch, 3, H, W, 1), m->lpips_w,
-                       m->eval_out + 2, m->lpips_scratch, m->lpips_scratch.bytes(), m->stream));
+    MAP_TRY(scored_lpips(m, W));
     float out3[3] = {0.f, 0.f, 0.f};
     MAP_TRY(read_eval_out(m, out3, 3));
     *psnr = out3[0]; *ssim = out3[1]; *lpips = out3[2];
@@ -1312,10 +1367,8 @@ int glic_mapper_evaluate_lpips(glic_mapper* m, int is_train, int index, float* p
 
 int glic_mapper_render(glic_mapper* m, int is_train, int index, float* rgb_host) {
     if (!m || !rgb_host) { set_error("mapper_render: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    const int W = m->cfg.width, H = m->cfg.height;
     MAP_TRY(render_scored(m, is_train, index, "mapper_render"));
-    GLIC_CUDA_TRY(cudaMemcpyAsync(rgb_host, eval_clamped(m->eval_scratch, 3, H, W, 0), sizeof(float) * 3 * (size_t)W * H,
-                                  cudaMemcpyDeviceToHost, m->stream));
+    MAP_TRY(scored_image_to_host(m, rgb_host));
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     return GLIC_OK;
 }
@@ -1324,18 +1377,16 @@ int glic_mapper_download(glic_mapper* m, float* xyz, float* f_dc, float* f_rest,
                          float* exp_avg_packed, float* exp_avg_sq_packed) {
     if (!m) { set_error("mapper_download: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    float* g[6];
-    arena_ptrs(m, m->params, m->Pcap, g);
+    const auto g = arena_rows(m->params, m->Pcap, m->M).groups();
+    const auto kk = group_widths(m->M);
     float* dst[6] = {rot, xyz, log_scale, opacity_logit, f_dc, f_rest};
-    const size_t kk[6] = {4, 3, 3, 1, 3, (size_t)3 * m->M};
     for (int q = 0; q < 6; ++q)
         if (dst[q] && kk[q] && m->P) GLIC_CUDA_TRY(cudaMemcpy(dst[q], g[q], sizeof(float) * kk[q] * m->P, cudaMemcpyDeviceToHost));
     float* mom[2] = {exp_avg_packed, exp_avg_sq_packed};
     float* srcm[2] = {m->m1, m->m2};
     for (int a = 0; a < 2; ++a) {
         if (!mom[a] || !m->P) continue;
-        float* gm[6];
-        arena_ptrs(m, srcm[a], m->Pcap, gm);
+        const auto gm = arena_rows(srcm[a], m->Pcap, m->M).groups();
         size_t off = 0;                                     // packed (capacity = P) layout: glic_packed_offsets(P, M)
         for (int q = 0; q < 6; ++q) {
             if (kk[q]) GLIC_CUDA_TRY(cudaMemcpy(mom[a] + off, gm[q], sizeof(float) * kk[q] * m->P, cudaMemcpyDeviceToHost));
@@ -1390,11 +1441,11 @@ int density_step(glic_mapper* m, const glic_density_params& p, bool densify, int
     cudaStream_t s = m->stream;
     if (P) {
         MAP_TRY(reserve(m, m->extend_ws, density_scratch_bytes(P)));   // the selection's scratch: the idle extend() staging
-        float* g[6];
-        arena_ptrs(m, m->params, m->Pcap, g);
+        const ArenaRows g = arena_rows(m->params, m->Pcap, m->M);
         const float* no_stats = nullptr;                   // a prune selects no row, with densification on or off
-        const DensitySelect a{P, m->n_sky, densify ? m->dens_accum : no_stats, densify ? m->dens_denom : no_stats, g[2], g[3], m->dens_maxr,
-                              p.grad_threshold, p.percent_dense * p.scene_extent, p.min_opacity, p.max_world_scale, p.max_screen_radius};
+        const DensitySelect a{P, m->n_sky, densify ? m->dens_accum : no_stats, densify ? m->dens_denom : no_stats, g.log_scale, g.opacity,
+                              m->dens_maxr, p.grad_threshold, p.percent_dense * p.scene_extent, p.min_opacity, p.max_world_scale,
+                              p.max_screen_radius};
         MAP_TRY(launch_density_select(a, m->extend_ws, r, s));
     }
     const uint32_t n_clone = r[0], n_split = r[1], kept = r[2], cloned = r[3], split = r[4];
@@ -1592,7 +1643,7 @@ int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_
     // training keyframe's trained E; zero moments and step counts
     AlignState h{};
     CamBlock cb;
-    camera_block(W, H, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, kf.R_wc, kf.t_wc, cb, h.T);
+    config_camera_block(m, kf.R_wc, kf.t_wc, cb, h.T);
     std::memcpy(h.pose_f, kf.R_wc, sizeof(kf.R_wc)); std::memcpy(h.pose_f + 9, kf.t_wc, sizeof(kf.t_wc));
     std::memcpy(h.cam, cb.view, sizeof(h.cam));
     h.E[0] = h.E[5] = h.E[10] = 1.0f;
@@ -1604,9 +1655,7 @@ int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_
         GLIC_CUDA_TRY(cudaMemcpyAsync(st->cam, kf.cam_dev, sizeof(h.cam), cudaMemcpyDeviceToDevice, s));
     }
     if (train && m->expo_on) GLIC_CUDA_TRY(cudaMemcpyAsync(st->E, m->expo_E + 12 * (size_t)index, sizeof(h.E), cudaMemcpyDeviceToDevice, s));
-    Keyframe ak;                                    // the keyframe's view, drawn from the call's own camera block
-    ak.view = kf.view;
-    ak.view.viewmatrix = st->cam; ak.view.projmatrix = st->cam + 16; ak.view.campos = st->cam + 32;
+    const glic_view v = make_view(cb, st->cam, W, H);   // the keyframe's view, drawn from the call's own camera block
     MAP_TRY(load_gt(m, kf, m->gt_dev[0], cudaMemcpyHostToDevice, s));
     const float* gt_fit = m->gt_dev[0];
     if (split) {
@@ -1615,12 +1664,8 @@ int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_
         gt_fit = crops[1];
     }
     MAP_TRY(activate(m));
-    float* g[6];
-    arena_ptrs(m, m->params, m->Pcap, g);
     PoseBatch b{};
     b.cam[0] = st->cam;
-    float fov2[2];
-    proj_matrix(W, H, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, b.Pm, fov2);
     const int slot_kf[1] = {0};
     const unsigned int* skip = reinterpret_cast<const unsigned int*>(&st->overflow);
     CompactGrads cg{};                              // null row pointers: the pose-only backward
@@ -1628,7 +1673,7 @@ int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_
     cg.pose_grad = st->pose_grad;
     const GeomHeader* ghdr = GeomState::carve(m->geom_ws, (int)m->P).hdr;
     for (int it = 0; it < p.iterations; ++it) {
-        MAP_TRY(forward_view(m, ak, 0, nullptr));
+        MAP_TRY(forward_view(m, v, 0, nullptr));
         overflow_word_kernel<<<1, 1, 0, s>>>(ghdr, &st->overflow);
         GLIC_LAUNCH_CHECK();
         const float* img_fit = m->color;
@@ -1639,21 +1684,14 @@ int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_
             img_fit = crops[0];
             dL_fit = crops[2];
         }
-        if (use_expo)
-            MAP_TRY(glic_l1_ssim_loss_exposure(H, Wf, m->cfg.lambda_dssim, img_fit, gt_fit, st->E, &st->loss, dL_fit, st->dE, m->loss_scratch,
-                                               m->loss_scratch.bytes(), s));
-        else
-            MAP_TRY(glic_l1_ssim_loss(3, H, Wf, m->cfg.lambda_dssim, img_fit, gt_fit, &st->loss, dL_fit, m->loss_scratch, m->loss_scratch.bytes(), s));
+        MAP_TRY(photometric_loss(m, H, Wf, img_fit, gt_fit, use_expo ? st->E : nullptr, &st->loss, dL_fit, st->dE));
         if (split) {
             pad_columns_kernel<<<plane_blocks((size_t)3 * H * W), 256, 0, s>>>(H, W, Wf, crops[2], m->dL_dpix);
             GLIC_LAUNCH_CHECK();
         }
-        MAP_TRY(glic_backward_compact_internal((int)m->P, m->D, m->M, g[1], m->act_scales, m->act_rots, m->M ? g[5] : nullptr, &ak.view, m->radii,
-                                               m->bin_cap, m->geom_ws, m->binning_ws, m->image_ws, m->sample_ws, m->dL_dpix, m->g_mean2D,
-                                               m->g_conic, m->g_opacity, col, &cg, nullptr, s));
-        pose_step_kernel<<<1, MAX_SLOTS, 0, s>>>(1, b, st->pose_grad, st->T, st->pose_f, st->pose_m, st->pose_v, &st->pose_t,
-                                                 p.lr_translation, p.lr_rotation, skip);
-        GLIC_LAUNCH_CHECK();
+        MAP_TRY(backward_view(m, v, col, cg, nullptr));
+        MAP_TRY(launch_pose_kernel(m, 1, b, st->pose_grad, st->T, st->pose_f, st->pose_m, st->pose_v, &st->pose_t, p.lr_translation,
+                                   p.lr_rotation, skip));
         if (p.exposure_lr > 0.0f)
             MAP_TRY(launch_exposure_adam(1, slot_kf, st->dE, st->E, st->expo_m, st->expo_v, &st->expo_t, p.exposure_lr, skip, s));
         align_tally_kernel<<<1, 1, 0, s>>>(ghdr, st);
@@ -1661,16 +1699,11 @@ int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_
     }
     GLIC_CUDA_TRY(cudaMemcpyAsync(&h, st, sizeof(h), cudaMemcpyDeviceToHost, s));
     GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-    if (h.skipped) {                                // as poll_ring grows it after an overflowed iteration
-        MAP_TRY(set_bin_capacity(m, std::max<int64_t>((int64_t)h.max_pairs + h.max_pairs / 4, m->bin_cap * 3 / 2)));
-        ++m->st.overflow_regrows;
-    }
+    if (h.skipped) MAP_TRY(regrow_after_skip(m, h.max_pairs));
     // scoring at the fitted camera: the full clamped (exposed) frame, then with split its score columns
-    MAP_TRY(forward_settled(m, ak, 0));
+    MAP_TRY(forward_settled(m, v, 0));
     MAP_TRY(eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], use_expo ? st->E : nullptr, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s));
-    if (rgb_host)
-        GLIC_CUDA_TRY(cudaMemcpyAsync(rgb_host, eval_clamped(m->eval_scratch, 3, H, W, 0), sizeof(float) * 3 * (size_t)W * H,
-                                      cudaMemcpyDeviceToHost, s));
+    if (rgb_host) MAP_TRY(scored_image_to_host(m, rgb_host));
     if (split) {
         for (int q = 0; q < 2; ++q) {
             crop_columns_kernel<<<plane_blocks((size_t)3 * H * Ws), 256, 0, s>>>(H, W, x_score, Ws, eval_clamped(m->eval_scratch, 3, H, W, q), crops[q]);
@@ -1678,9 +1711,7 @@ int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_
         }
         MAP_TRY(eval_psnr_ssim(3, H, Ws, crops[0], crops[1], nullptr, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s));
     }
-    if (m->lpips_w)
-        MAP_TRY(glic_lpips(H, Ws, eval_clamped(m->eval_scratch, 3, H, Ws, 0), eval_clamped(m->eval_scratch, 3, H, Ws, 1), m->lpips_w,
-                           m->eval_out + 2, m->lpips_scratch, m->lpips_scratch.bytes(), s));
+    if (m->lpips_w) MAP_TRY(scored_lpips(m, Ws));
     float out3[3] = {0.f, 0.f, std::numeric_limits<float>::quiet_NaN()};
     MAP_TRY(read_eval_out(m, out3, m->lpips_w ? 3 : 2));
     glic_align_result& r = *out;
@@ -1724,28 +1755,18 @@ int render_camera(glic_mapper* m, const glic_render_camera& c, int exposure_inde
     CamBlock cb;
     camera_block(W, H, c.fx, c.fy, c.cx, c.cy, c.R_wc, c.t_wc, cb);
     GLIC_CUDA_TRY(cudaMemcpyAsync(r.cam, cb.view, 36 * sizeof(float), cudaMemcpyHostToDevice, s));
-    glic_view v{};
-    v.viewmatrix = r.cam; v.projmatrix = r.cam + 16; v.campos = r.cam + 32;
-    v.tan_fovx = cb.tanfovx; v.tan_fovy = cb.tanfovy;
-    v.limx_neg = cb.lim[0]; v.limx_pos = cb.lim[1]; v.limy_neg = cb.lim[2]; v.limy_pos = cb.lim[3];
-    v.width = W; v.height = H;
+    const glic_view v = make_view(cb, r.cam, W, H);
     MAP_TRY(activate(m));
-    // the groups are planar: rows [first, P) are the same call on every group pointer offset by `first` rows
+    // the groups are planar: rows [first, P) are the same call on every group pointer offset by `first` rows (rest stays null
+    // when M = 0)
     const size_t first = with_sky ? 0 : m->n_sky;
-    float* g[6];
-    arena_ptrs(m, m->params, m->Pcap, g);
-    for (int attempt = 0; attempt < 4; ++attempt) {           // as forward_settled: an overflow grows the binning and redraws
-        long long* cnt = m->counters_host;
-        MAP_TRY(glic_render((int)(m->P - first), m->D, m->M, g[1] + 3 * first, m->act_scales + 3 * first, 1.0f, m->act_rots + 4 * first,
-                            m->act_opacity + first, g[4] + 3 * first, m->M ? g[5] + (size_t)3 * m->M * first : nullptr, &v,
-                            m->radii + first, m->geom_ws, m->geom_ws.bytes(), r.image_ws, glic_image_bytes(W, H), m->binning_ws,
-                            m->binning_ws.bytes(), r.color, r.T, out[2] ? r.depth : nullptr, out[3] ? r.median : nullptr,
-                            (int64_t*)cnt, s));
-        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-        if (!cnt[2]) break;
-        MAP_TRY(grow_render_binning(m, cnt[0] + cnt[0] / 4));
-        ++m->st.overflow_regrows;
-    }
+    const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
+    MAP_TRY(draw_settled(m, [&](long long* cnt) {
+        return glic_render((int)(m->P - first), m->D, m->M, a.xyz + 3 * first, m->act_scales + 3 * first, 1.0f, m->act_rots + 4 * first,
+                           m->act_opacity + first, a.dc + 3 * first, a.rest + (size_t)3 * m->M * first, &v, m->radii + first, m->geom_ws,
+                           m->geom_ws.bytes(), r.image_ws, glic_image_bytes(W, H), m->binning_ws, m->binning_ws.bytes(), r.color, r.T,
+                           out[2] ? r.depth : nullptr, out[3] ? r.median : nullptr, (int64_t*)cnt, s);
+    }, [&](int64_t pairs) { return grow_render_binning(m, pairs); }));
     if (out[0]) MAP_TRY(launch_scored_image(H, W, r.color, exposure_index >= 0 ? m->expo_E + 12 * (size_t)exposure_index : nullptr, r.rgb, s));
     const float* src[4] = {r.rgb, r.T, r.depth, r.median};
     for (int q = 0; q < 4; ++q)
@@ -1968,8 +1989,8 @@ int glic_mapper_pose_adam_state(glic_mapper* m, int index, float* exp_avg6, floa
 
 int glic_mapper_align(glic_mapper* m, int is_train, int index, const glic_align_params* p, glic_align_result* out, float* rgb_host) {
     if (!m || !p || !out) { set_error("mapper_align: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    const auto& list = is_train ? m->train : m->test;
-    if (index < 0 || index >= (int)list.size()) { set_error("mapper_align: keyframe index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const Keyframe* kf = nullptr;
+    MAP_TRY(keyframe_at(m, is_train, index, "mapper_align", kf));
     if (p->iterations < 0 || !finite_at_least_zero(p->lr_translation) || !finite_at_least_zero(p->lr_rotation) ||
         !finite_at_least_zero(p->exposure_lr) || (p->split != 0 && p->split != 1)) {
         set_error("mapper_align: iterations must be >= 0, the rates finite and >= 0, split 0 or 1"); return GLIC_ERR_INVALID_ARGUMENT;
@@ -1978,7 +1999,7 @@ int glic_mapper_align(glic_mapper* m, int is_train, int index, const glic_align_
     if (p->split && W < 2) { set_error("mapper_align: split needs a frame at least 2 columns wide"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (m->lpips_w && !glic_lpips_scratch_bytes(H, Ws)) { set_error("mapper_align: LPIPS needs a score region of at least 31x31"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (m->P == 0) { set_error("mapper_align: the map has no rows to align against"); return GLIC_ERR_INVALID_ARGUMENT; }
-    return align(m, list[index], is_train != 0, index, *p, out, rgb_host);
+    return align(m, *kf, is_train != 0, index, *p, out, rgb_host);
 }
 
 int glic_mapper_render_camera(glic_mapper* m, const glic_render_camera* cam, int exposure_index, int with_sky, float* rgb, float* final_T,
