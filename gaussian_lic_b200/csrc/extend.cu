@@ -5,7 +5,8 @@
 // smallest camera depth wins a pixel, the earlier index on ties, exactly the reference's strict `<` rule; points
 // outside the image cannot shadow in-image ones (different map keys) and are dropped by the filter anyway, so the
 // W x H word buffer is the whole map.  Survivors (winner, depth_in_rsp_frame > 0, rendered alpha < 0.99) are compacted in
-// ascending index order by a single-CTA scan and initialised in place.  Checker: the extend restatement of the CPU oracle (oracle/, test infrastructure).
+// ascending index order by a single-CTA scan and initialised in place.  Checkers: tests/extend_oracle.py (exact NumPy
+// restatement of the selection), the CPU oracle's restatement, and torch's own device arithmetic (tests/test_gpu_extend_edges.py).
 #include "common.cuh"
 
 namespace glic {
@@ -14,7 +15,13 @@ namespace {
 struct ExtendCam { float r[9]; float t[3]; float fx, fy, cx, cy; int W, H; };
 
 __device__ __forceinline__ bool extend_pixel(const ExtendCam& c, const float* __restrict__ p, int& px, int& py, float& z) {
-    // torch.matmul(points, R_cw^T) + t, then (x * fx) / z + cx with separate (uncontracted) mul / div / add kernels
+    // ((p0 r0 + p1 r1) + p2 r2) + t, then (x * fx) / z + cx, every step rounded on its own (no contraction).  The reference's
+    // torch.matmul(points, R_cw^T) + t is not one fixed order: measured on an H100 (torch 2.11, TF32 off), its float32 GEMM
+    // gives exactly this order for n <= 16 points and the fma chain fmaf(p2, r2, fmaf(p1, r1, p0 r0)) for every n from 17 to
+    // 4 194 307 tested, so the two round differently on about half the points of a frame.  A point then falls on another
+    // pixel only when an integer lies between its two pixel coordinates, and wins differently only when its depth and its
+    // pixel winner's are within that rounding: 3 of 200 000 and 9 of 1 048 577 random points survive differently
+    // (tests/test_gpu_extend_edges.py prints the counts per case).
     float cam[3];
 #pragma unroll
     for (int r = 0; r < 3; ++r)
@@ -22,13 +29,20 @@ __device__ __forceinline__ bool extend_pixel(const ExtendCam& c, const float* __
     z = cam[2];
     const float fxp = floorf(__fadd_rn(__fdiv_rn(__fmul_rn(cam[0], c.fx), z), c.cx));
     const float fyp = floorf(__fadd_rn(__fdiv_rn(__fmul_rn(cam[1], c.fy), z), c.cy));
-    if (!(fxp >= 0.0f && fxp < (float)c.W && fyp >= 0.0f && fyp < (float)c.H)) return false;   // also rejects NaN
+    // Non-finite coordinates are rejected.  z = +-0 gives +-inf (x != 0) or NaN (x = 0); z = +-inf gives cx for a finite x.
+    // torch's floor().to(int32) on the device saturates +-inf to INT_MAX / INT_MIN, outside the image like here, but turns NaN
+    // into 0: in the reference a NaN coordinate lands on column (or row) 0, where a NaN depth wins the pixel if it comes first
+    // and then blocks every real point (a NaN scan point has a NaN depth_rsp and is not inserted itself), and a point exactly
+    // at the camera centre lands on pixel (0, 0) with depth 0.  Rejecting NaN keeps real points on their pixels.
+    // A zero depth never reaches the z-buffer, so every depth that does is finite or +-inf and non-zero.
+    if (!(fxp >= 0.0f && fxp < (float)c.W && fyp >= 0.0f && fyp < (float)c.H)) return false;
     px = (int)fxp; py = (int)fyp;
     return true;
 }
 
 __device__ __forceinline__ unsigned int orderable(float f) {       // monotone float -> uint (negative depths included)
     f = __fadd_rn(f, 0.0f);                                        // -0.0f -> +0.0f: the reference's float `<` treats them as equal
+                                                                   // (extend_pixel passes no zero depth: monotone for every float anyway)
     const unsigned int b = __float_as_uint(f);
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
@@ -98,9 +112,11 @@ extend_scan_kernel(int n, unsigned int* __restrict__ flag_to_pos, unsigned int* 
     if (tid == 0) *count = carry;
 }
 
+// the reference's tensor ops on the survivors: RGB2SH (rgb - 0.5f) / C0 and scaling_scale * d / focal divide by a scalar, which
+// torch's CUDA division carries out as a multiplication by the scalar's reciprocal, 1.0 / C0 rounded to float once
 __global__ void __launch_bounds__(256)
 extend_init_kernel(int n, const unsigned int* __restrict__ flag_pos, const float* __restrict__ points,
-                   const float* __restrict__ colors, const float* __restrict__ depth_rsp, float scaling_scale, float focal,
+                   const float* __restrict__ colors, const float* __restrict__ depth_rsp, float scaling_scale, float inv_focal,
                    int* __restrict__ keep_idx, float* __restrict__ xyz, float* __restrict__ f_dc, float* __restrict__ log_scale,
                    float* __restrict__ rot, float* __restrict__ opacity_logit) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -109,11 +125,12 @@ extend_init_kernel(int n, const unsigned int* __restrict__ flag_pos, const float
     if (!(fp >> 31)) return;
     const size_t k = fp & 0x7FFFFFFFu;
     keep_idx[k] = i;
-    const float ls = logf(__fdiv_rn(__fmul_rn(scaling_scale, depth_rsp[i]), focal));
+    const float ls = logf(__fmul_rn(__fmul_rn(scaling_scale, depth_rsp[i]), inv_focal));
+    constexpr float inv_C0 = (float)(1.0 / 0.28209479177387814);
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
         xyz[3 * k + c] = points[3 * (size_t)i + c];
-        f_dc[3 * k + c] = __fdiv_rn(__fsub_rn(colors[3 * (size_t)i + c], 0.5f), 0.28209479177387814f);
+        f_dc[3 * k + c] = __fmul_rn(__fsub_rn(colors[3 * (size_t)i + c], 0.5f), inv_C0);
         log_scale[3 * k + c] = ls;
     }
     reinterpret_cast<float4*>(rot)[k] = make_float4(1.0f, 0.0f, 0.0f, 0.0f);
@@ -165,8 +182,9 @@ int glic_extend(int n, const float* points, const float* colors, const float* de
     GLIC_LAUNCH_CHECK();
     extend_scan_kernel<<<1, 1024, 0, s>>>(n, flag, count);
     GLIC_LAUNCH_CHECK();
-    extend_init_kernel<<<blocks, 256, 0, s>>>(n, flag, points, colors, depth_rsp, scaling_scale, (fx + fy) / 2.0f, keep_idx, xyz, f_dc,
-                                              log_scale, rot, opacity_logit);
+    const float focal = (fx + fy) / 2.0f;
+    extend_init_kernel<<<blocks, 256, 0, s>>>(n, flag, points, colors, depth_rsp, scaling_scale, (float)(1.0 / (double)focal), keep_idx,
+                                              xyz, f_dc, log_scale, rot, opacity_logit);
     GLIC_LAUNCH_CHECK();
     unsigned int m = 0;
     GLIC_CUDA_TRY(cudaMemcpyAsync(&m, count, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));

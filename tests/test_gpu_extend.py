@@ -55,7 +55,7 @@ def test_extend_matches_oracle(oracle32, n, W, H, seed):
     assert m == len(want) and np.array_equal(got, want)
     init = oracle32.extend_init(want, pts, cols, rsp, 0.8, fx, fy)
     np.testing.assert_array_equal(xyz[:m].cpu().numpy(), init["xyz"])
-    np.testing.assert_allclose(fdc[:m].cpu().numpy(), init["f_dc"], rtol=2e-7, atol=1e-7)
+    np.testing.assert_array_equal(fdc[:m].cpu().numpy(), init["f_dc"])
     np.testing.assert_allclose(ls[:m].cpu().numpy(), init["log_scale"], rtol=2e-6, atol=2e-7)
     np.testing.assert_array_equal(rot[:m].cpu().numpy(), init["rot"])
     np.testing.assert_allclose(op[:m].cpu().numpy(), init["opacity_logit"], rtol=2e-7)
