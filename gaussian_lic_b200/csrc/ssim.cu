@@ -378,12 +378,23 @@ exposure_adam_kernel(int S, ExpoBatch batch, const float* __restrict__ slot_grad
 
 using namespace glic;
 
+// The planes of one launch run as gridDim.z, which is at most 65535: a larger B*CH (or one that overflows int) is refused
+// before anything is enqueued, rather than failing at the launch after validation has passed.
+static constexpr long long MAX_PLANES = 65535;
+
+static bool planes_ok(long long planes, const char* what) {
+    if (planes <= MAX_PLANES) return true;
+    set_error(std::string(what) + ": " + std::to_string(planes) + " planes; at most 65535 per call");
+    return false;
+}
+
 extern "C" int glic_fused_ssim(int B, int CH, int H, int W, float C1, float C2, const float* img1, const float* img2,
                                float* ssim_map, float* dm_dmu1, float* dm_dsigma1_sq, float* dm_dsigma12, void* stream) {
     if (B < 0 || CH < 0 || H <= 0 || W <= 0 || !img1 || !img2 || !ssim_map) { set_error("fused_ssim: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
     if ((dm_dmu1 != nullptr) != (dm_dsigma1_sq != nullptr) || (dm_dmu1 != nullptr) != (dm_dsigma12 != nullptr)) {
         set_error("fused_ssim: partial maps must be all NULL or all non-NULL"); return GLIC_ERR_INVALID_ARGUMENT;
     }
+    if (!planes_ok((long long)B * CH, "fused_ssim")) return GLIC_ERR_INVALID_ARGUMENT;
     if (B * CH == 0) return GLIC_OK;
     dim3 grid((W + SB - 1) / SB, (H + SB - 1) / SB, B * CH), block(ST);
     ssim_forward_kernel<false><<<grid, block, 0, (cudaStream_t)stream>>>(H, W, C1, C2, img1, img2, ssim_map, dm_dmu1,
@@ -396,9 +407,10 @@ extern "C" int glic_fused_ssim_backward(int B, int CH, int H, int W, float C1, f
                                         const float* img2, const float* dL_dmap, const float* dm_dmu1,
                                         const float* dm_dsigma1_sq, const float* dm_dsigma12, float* dL_dimg1, void* stream) {
     (void)C1; (void)C2;
-    if (H <= 0 || W <= 0 || !img1 || !img2 || !dL_dmap || !dm_dmu1 || !dm_dsigma1_sq || !dm_dsigma12 || !dL_dimg1) {
+    if (B < 0 || CH < 0 || H <= 0 || W <= 0 || !img1 || !img2 || !dL_dmap || !dm_dmu1 || !dm_dsigma1_sq || !dm_dsigma12 || !dL_dimg1) {
         set_error("fused_ssim_backward: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT;
     }
+    if (!planes_ok((long long)B * CH, "fused_ssim_backward")) return GLIC_ERR_INVALID_ARGUMENT;
     if (B * CH == 0) return GLIC_OK;
     dim3 grid((W + SB - 1) / SB, (H + SB - 1) / SB, B * CH), block(ST);
     ssim_backward_kernel<false><<<grid, block, 0, (cudaStream_t)stream>>>(H, W, img1, img2, dL_dmap, dm_dmu1, dm_dsigma1_sq,
@@ -412,6 +424,7 @@ extern "C" size_t glic_loss_scratch_bytes(int CH, int H, int W) { return sizeof(
 extern "C" int glic_l1_ssim_loss(int CH, int H, int W, float lambda_dssim, const float* img, const float* gt, float* loss_out,
                                  float* dL_dimg, void* scratch, size_t scratch_bytes, void* stream) {
     if (CH <= 0 || H <= 0 || W <= 0 || !img || !gt || !loss_out || !scratch) { set_error("l1_ssim_loss: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!planes_ok(CH, "l1_ssim_loss")) return GLIC_ERR_INVALID_ARGUMENT;
     if (scratch_bytes < glic_loss_scratch_bytes(CH, H, W)) { set_error("l1_ssim_loss: scratch too small"); return GLIC_ERR_WORKSPACE; }
     const size_t N = (size_t)CH * H * W;
     float* d1 = static_cast<float*>(scratch);

@@ -280,6 +280,7 @@ GLIC_API int glic_ply_read(const char* path, uint32_t P, uint32_t M, float* xyz,
 /* ---------------------------------------------------------------------------------------
  * Fused SSIM.  Replaces fusedssimCUDA / fusedssim_backwardCUDA (fused-ssim/ssim.cu:186-365).
  * img*: [B,CH,H,W] contiguous.  Partial-derivative maps may be NULL in forward (train = false).
+ * At most 65535 planes (B*CH) per call; more is GLIC_ERR_INVALID_ARGUMENT with nothing enqueued.
  * ------------------------------------------------------------------------------------- */
 GLIC_API int glic_fused_ssim(int B, int CH, int H, int W, float C1, float C2, const float* img1, const float* img2,
                     float* ssim_map, float* dm_dmu1, float* dm_dsigma1_sq, float* dm_dsigma12, void* stream);
@@ -290,7 +291,8 @@ GLIC_API int glic_fused_ssim_backward(int B, int CH, int H, int W, float C1, flo
 
 /* Whole photometric loss of one mapping iteration in two launches (gaussian.cpp:685-691,
  * loss_utils.h:30-33,189-193): L = (1-lambda)*mean|img-gt| + lambda*(1-mean(SSIM)), and
- * dL/dimg.  loss_out: 1 device float (accumulated; zeroed by the call).  scratch: 3*CH*H*W floats. */
+ * dL/dimg.  loss_out: 1 device float (accumulated; zeroed by the call).  scratch: 3*CH*H*W floats.  CH <= 65535.
+ * dL/dimg is bit-reproducible; the loss is not (one float atomicAdd per 32x32 tile, in the order the tiles finish). */
 GLIC_API size_t glic_loss_scratch_bytes(int CH, int H, int W);
 GLIC_API int glic_l1_ssim_loss(int CH, int H, int W, float lambda_dssim, const float* img, const float* gt,
                       float* loss_out, float* dL_dimg, void* scratch, size_t scratch_bytes, void* stream);
