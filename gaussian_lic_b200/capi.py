@@ -115,6 +115,9 @@ def _load():
         "glic_forward_render": (i32, [i32, C.POINTER(View), i32, i64, vp, vp, vp, sz, vp, sz, vp, vp, C.POINTER(i64), vp]),
         "glic_backward": (i32, [i32, i32, i32, vp, vp, f32, vp, vp, vp, C.POINTER(View), vp, i64, vp, vp, vp, vp, vp, f32,
                                 vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+        "glic_deterministic_bytes": (sz, [i64, i32, i32]),
+        "glic_backward_deterministic": (i32, [i32, i32, i32, vp, vp, f32, vp, vp, vp, C.POINTER(View), vp, i64, vp, vp, vp, vp, vp,
+                                              f32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]),
         "glic_sort_pairs_u64_u32": (i32, [i64, i32, vp, vp, vp, vp, vp, sz, vp]),
         "glic_debug_sort_pairs_u32": (i32, [i64, i32, vp, vp, vp, vp, vp, vp, sz, vp]),
         "glic_adam_update": (i32, [vp, vp, vp, vp, vp, f32, f32, f32, f32, u32, u32, vp]),
@@ -210,6 +213,8 @@ def _load():
         "glic_debug_image": (i32, [i32, i32, vp, vp, vp, vp, vp, C.POINTER(i64), vp]),
         "glic_debug_spans": (i32, [i32, vp, C.POINTER(u32), vp]),
         "glic_debug_render_backward": (i32, [i32, C.POINTER(View), i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, vp]),
+        "glic_debug_deterministic_entries": (i32, [i32, C.POINTER(View), i64, vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp,
+                                                   C.POINTER(i64), vp, vp, vp, vp]),
         "glic_debug_pose_backward": (i32, [i32, i32, i32, vp, vp, vp, vp, vp, vp, C.POINTER(View), vp, vp, vp, vp, vp, vp, i32, vp,
                                            vp, vp, vp]),
         "glic_debug_fail_allocation": (i32, [i32]),

@@ -74,6 +74,21 @@ __global__ void debug_keys_kernel(long long R, GeomState g, const uint32_t* tile
     out[i] = ((uint64_t)tile_keys[i] << 32) | (uint64_t)__float_as_uint(g.rec[3 * (size_t)gid + 2].y);
 }
 
+// the deterministic backward's entries in reduction order: sorted positions i < n whose key is a gid (the sentinels sort last)
+__global__ void debug_det_entries_kernel(unsigned n, uint32_t P, const uint32_t* keys, const uint32_t* idx, const float* vals,
+                                         const uint32_t* live_offsets, int T, uint32_t* gid, uint32_t* tile, float* values,
+                                         unsigned int* n_valid) {
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || keys[i] >= P) return;
+    const uint32_t e = idx[i], live = e / BUCKET;
+    int lo = 0, hi = T - 1;                                  // first tile t with live_offsets[t] > live
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (live_offsets[mid] > live) hi = mid; else lo = mid + 1; }
+    gid[i] = keys[i];
+    tile[i] = (uint32_t)lo;
+    for (int j = 0; j < 9; ++j) values[9 * (size_t)i + j] = vals[9 * (size_t)e + j];
+    atomicAdd(n_valid, 1u);
+}
+
 // The stages of glic_forward and glic_render up to the blend, on workspaces carved for `cap` pairs: preprocess, depth sort and scan,
 // key emission, tile sort, tile ranges and, with `buckets`, the bucket offsets of the checkpoints.  Returns the ping-pong half that
 // holds the sorted list, < 0 on error.
@@ -344,27 +359,33 @@ int glic_render(int P, int sh_degree, int M, const float* means3D, const float* 
     return GLIC_OK;
 }
 
-int glic_backward(int P, int sh_degree, int M, const float* means3D, const float* scales, float scale_modifier,
-                  const float* rotations, const float* dc, const float* sh, const glic_view* view, const int* radii,
-                  int64_t R, const void* geom_ws, const void* binning_ws, const void* image_ws, const void* sample_ws,
-                  const float* dL_dpix, float lambda_erank, float* dL_dmeans2D, float* dL_dconic, float* dL_dopacity,
-                  float* dL_dcolors, float* dL_dmeans3D, float* dL_dcov3D, float* dL_ddc, float* dL_dsh, float* dL_dscales,
-                  float* dL_drotations, void* stream) {
-    (void)dc;
+size_t glic_deterministic_bytes(int64_t num_rendered, int width, int height) {
+    size_t b = 0;
+    DetState::carve(nullptr, glic_max_buckets(num_rendered > 0 ? num_rendered : 0, width, height), &b);
+    return b;
+}
+
+// glic_backward and glic_backward_deterministic: det_ws == NULL selects the atomic render backward.  2-D gradient accumulators
+// are filled by atomics (or, deterministic, written for the rows with a contribution): zero them here (11 floats / Gaussian)
+static int backward_impl(const char* what, int P, int sh_degree, int M, const float* means3D, const float* scales, float scale_modifier,
+                         const float* rotations, const float* sh, const glic_view* view, const int* radii, int64_t R,
+                         const void* geom_ws, const void* binning_ws, const void* image_ws, const void* sample_ws,
+                         const float* dL_dpix, float lambda_erank, float* dL_dmeans2D, float* dL_dconic, float* dL_dopacity,
+                         float* dL_dcolors, float* dL_dmeans3D, float* dL_dcov3D, float* dL_ddc, float* dL_dsh, float* dL_dscales,
+                         float* dL_drotations, void* det_ws, cudaStream_t s) {
+    const std::string w(what);
     if (int e = check_view(view)) return e;
-    if (P < 0 || R < 0 || sh_degree < 0 || sh_degree > 3 || M < 0) { set_error("backward: bad sizes"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (P < 0 || R < 0 || sh_degree < 0 || sh_degree > 3 || M < 0) { set_error(w + ": bad sizes"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (P == 0) return GLIC_OK;
     if (!means3D || !scales || !rotations || !radii || !dL_dpix || !dL_dmeans2D || !dL_dconic || !dL_dopacity || !dL_dcolors ||
         !dL_dmeans3D || !dL_dcov3D || !dL_ddc || !dL_dscales || !dL_drotations || (M > 0 && (!sh || !dL_dsh))) {
-        set_error("backward: null pointer"); return GLIC_ERR_INVALID_ARGUMENT;
+        set_error(w + ": null pointer"); return GLIC_ERR_INVALID_ARGUMENT;
     }
-    if (!aligned16(rotations) || !aligned16(dL_drotations)) { set_error("backward: rotations / dL_drotations must be 16-byte aligned"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!geom_ws || !image_ws || (R > 0 && (!binning_ws || !sample_ws))) { set_error("backward: missing saved workspace"); return GLIC_ERR_WORKSPACE; }
-    cudaStream_t s = (cudaStream_t)stream;
+    if (!aligned16(rotations) || !aligned16(dL_drotations)) { set_error(w + ": rotations / dL_drotations must be 16-byte aligned"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!geom_ws || !image_ws || (R > 0 && (!binning_ws || !sample_ws))) { set_error(w + ": missing saved workspace"); return GLIC_ERR_WORKSPACE; }
     const ViewParams vp = make_view_params(view);
     GeomState g = GeomState::carve(const_cast<void*>(geom_ws), P);
     ImageState img = ImageState::carve(const_cast<void*>(image_ws), vp.W, vp.H);
-    // 2-D gradient accumulators are filled by atomics: zero them here (11 floats / Gaussian)
     { StageTimer _t(GLIC_STAGE_ZERO, s);
     GLIC_CUDA_TRY(cudaMemsetAsync(dL_dmeans2D, 0, sizeof(float) * 3 * (size_t)P, s));
     GLIC_CUDA_TRY(cudaMemsetAsync(dL_dconic, 0, sizeof(float) * 4 * (size_t)P, s));
@@ -374,17 +395,45 @@ int glic_backward(int P, int sh_degree, int M, const float* means3D, const float
         BinningState bin = BinningState::carve(const_cast<void*>(binning_ws), R);
         const int64_t max_buckets = glic_max_buckets(R, vp.W, vp.H);
         SampleState smp = SampleState::carve(const_cast<void*>(sample_ws), max_buckets);
-        // the sort's ping-pong parity is a pure function of the pass count
-        const int T = vp.grid_x * vp.grid_y;
-        const int cur = tile_sort_passes(T) & 1;
+        const int cur = tile_sort_passes(vp.grid_x * vp.grid_y) & 1;
         StageTimer _t(GLIC_STAGE_RENDER_BWD, s);
-        if (int e = launch_render_backward(P, vp, max_buckets, bin.vals[cur], g, img, smp, dL_dpix, dL_dmeans2D, dL_dconic,
-                                           dL_dopacity, dL_dcolors, s)) return e;
+        if (int e = det_ws ? launch_render_backward_det(P, vp, max_buckets, bin.vals[cur], g, img, smp, DetState::carve(det_ws, max_buckets),
+                                                        dL_dpix, dL_dmeans2D, dL_dconic, dL_dopacity, dL_dcolors, s)
+                           : launch_render_backward(P, vp, max_buckets, bin.vals[cur], g, img, smp, dL_dpix, dL_dmeans2D, dL_dconic,
+                                                    dL_dopacity, dL_dcolors, s)) return e;
     }
     StageTimer _t(GLIC_STAGE_PREPROCESS_BWD, s);
     return launch_preprocess_backward(P, sh_degree, M, means3D, scales, scale_modifier, rotations, sh, vp, radii, g,
                                       lambda_erank, dL_dmeans2D, dL_dconic, dL_dcolors, dL_dmeans3D, dL_dcov3D, dL_ddc,
                                       dL_dsh, dL_dscales, dL_drotations, s);
+}
+
+int glic_backward_deterministic(int P, int sh_degree, int M, const float* means3D, const float* scales, float scale_modifier,
+                                const float* rotations, const float* dc, const float* sh, const glic_view* view, const int* radii,
+                                int64_t R, const void* geom_ws, const void* binning_ws, const void* image_ws, const void* sample_ws,
+                                const float* dL_dpix, float lambda_erank, float* dL_dmeans2D, float* dL_dconic, float* dL_dopacity,
+                                float* dL_dcolors, float* dL_dmeans3D, float* dL_dcov3D, float* dL_ddc, float* dL_dsh,
+                                float* dL_dscales, float* dL_drotations, void* det_ws, size_t det_bytes, void* stream) {
+    (void)dc;
+    if (int e = check_view(view)) return e;
+    if (P > 0 && R > 0 && (!det_ws || det_bytes < glic_deterministic_bytes(R, view->width, view->height))) {
+        set_error("backward_deterministic: deterministic workspace too small"); return GLIC_ERR_WORKSPACE;
+    }
+    return backward_impl("backward_deterministic", P, sh_degree, M, means3D, scales, scale_modifier, rotations, sh, view, radii, R,
+                         geom_ws, binning_ws, image_ws, sample_ws, dL_dpix, lambda_erank, dL_dmeans2D, dL_dconic, dL_dopacity,
+                         dL_dcolors, dL_dmeans3D, dL_dcov3D, dL_ddc, dL_dsh, dL_dscales, dL_drotations, det_ws, (cudaStream_t)stream);
+}
+
+int glic_backward(int P, int sh_degree, int M, const float* means3D, const float* scales, float scale_modifier,
+                  const float* rotations, const float* dc, const float* sh, const glic_view* view, const int* radii,
+                  int64_t R, const void* geom_ws, const void* binning_ws, const void* image_ws, const void* sample_ws,
+                  const float* dL_dpix, float lambda_erank, float* dL_dmeans2D, float* dL_dconic, float* dL_dopacity,
+                  float* dL_dcolors, float* dL_dmeans3D, float* dL_dcov3D, float* dL_ddc, float* dL_dsh, float* dL_dscales,
+                  float* dL_drotations, void* stream) {
+    (void)dc;
+    return backward_impl("backward", P, sh_degree, M, means3D, scales, scale_modifier, rotations, sh, view, radii, R, geom_ws,
+                         binning_ws, image_ws, sample_ws, dL_dpix, lambda_erank, dL_dmeans2D, dL_dconic, dL_dopacity, dL_dcolors,
+                         dL_dmeans3D, dL_dcov3D, dL_ddc, dL_dsh, dL_dscales, dL_drotations, nullptr, (cudaStream_t)stream);
 }
 
 // Internal (mapper.cu): the backward with the compact gradient form of preprocess_backward.cu.  dL_dcolors is zeroed and
@@ -393,7 +442,7 @@ int glic_backward_compact_internal(int P, int sh_degree, int M, const float* mea
                                    const float* sh, const glic_view* view, const int* radii, int64_t R, const void* geom_ws,
                                    const void* binning_ws, const void* image_ws, const void* sample_ws, const float* dL_dpix,
                                    float* dL_dmeans2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolors,
-                                   const glic::CompactGrads* cg, void* after_render_event, void* stream) {
+                                   const glic::CompactGrads* cg, void* after_render_event, void* stream, void* det_ws) {
     if (int e = check_view(view)) return e;
     if (P <= 0) return GLIC_OK;
     cudaStream_t s = (cudaStream_t)stream;
@@ -419,8 +468,10 @@ int glic_backward_compact_internal(int P, int sh_degree, int M, const float* mea
         const int T = vp.grid_x * vp.grid_y;
         const int cur = tile_sort_passes(T) & 1;
         StageTimer _t(GLIC_STAGE_RENDER_BWD, s);
-        if (int e = launch_render_backward(P, vp, max_buckets, bin.vals[cur], g, img, smp, dL_dpix, dL_dmeans2D, dL_dconic,
-                                           dL_dopacity, dL_dcolors, s)) return e;
+        if (int e = det_ws ? launch_render_backward_det(P, vp, max_buckets, bin.vals[cur], g, img, smp, DetState::carve(det_ws, max_buckets),
+                                                        dL_dpix, dL_dmeans2D, dL_dconic, dL_dopacity, dL_dcolors, s)
+                           : launch_render_backward(P, vp, max_buckets, bin.vals[cur], g, img, smp, dL_dpix, dL_dmeans2D, dL_dconic,
+                                                    dL_dopacity, dL_dcolors, s)) return e;
     }
     // the colour gradients are final here: the multi-GPU push may start while the per-Gaussian backward still runs
     if (after_render_event) GLIC_CUDA_TRY(cudaEventRecord((cudaEvent_t)after_render_event, s));
@@ -496,6 +547,55 @@ int glic_debug_render_backward(int P, const glic_view* view, int64_t R, const vo
     const int cur = tile_sort_passes(vp.grid_x * vp.grid_y) & 1;
     return launch_render_backward(P, vp, max_buckets, bin.vals[cur], g, img, smp, dL_dpix, dL_dmeans2D, dL_dconic, dL_dopacity,
                                   dL_dcolors, (cudaStream_t)stream, exact != 0, counters);
+}
+
+int glic_debug_deterministic_entries(int P, const glic_view* view, int64_t R, const void* geom_ws, const void* binning_ws,
+                                     const void* image_ws, const void* sample_ws, const float* dL_dpix, void* det_ws, size_t det_bytes,
+                                     float* dL_dmeans2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolors, int64_t* count_host,
+                                     uint32_t* gid, uint32_t* tile, float* values, void* stream) {
+    if (int e = check_view(view)) return e;
+    if (P < 0 || R < 0 || !count_host) { set_error("debug_deterministic_entries: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
+    *count_host = 0;
+    if (P == 0) return GLIC_OK;
+    if (!dL_dpix || !dL_dmeans2D || !dL_dconic || !dL_dopacity || !dL_dcolors || !gid || !tile || !values) {
+        set_error("debug_deterministic_entries: null pointer"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (!geom_ws || !image_ws || (R > 0 && (!binning_ws || !sample_ws))) { set_error("debug_deterministic_entries: missing saved workspace"); return GLIC_ERR_WORKSPACE; }
+    if (R > 0 && (!det_ws || det_bytes < glic_deterministic_bytes(R, view->width, view->height))) {
+        set_error("debug_deterministic_entries: deterministic workspace too small"); return GLIC_ERR_WORKSPACE;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    const ViewParams vp = make_view_params(view);
+    GLIC_CUDA_TRY(cudaMemsetAsync(dL_dmeans2D, 0, sizeof(float) * 3 * (size_t)P, s));
+    GLIC_CUDA_TRY(cudaMemsetAsync(dL_dconic, 0, sizeof(float) * 4 * (size_t)P, s));
+    GLIC_CUDA_TRY(cudaMemsetAsync(dL_dopacity, 0, sizeof(float) * (size_t)P, s));
+    GLIC_CUDA_TRY(cudaMemsetAsync(dL_dcolors, 0, sizeof(float) * 3 * (size_t)P, s));
+    if (R == 0) return GLIC_OK;
+    GeomState g = GeomState::carve(const_cast<void*>(geom_ws), P);
+    ImageState img = ImageState::carve(const_cast<void*>(image_ws), vp.W, vp.H);
+    BinningState bin = BinningState::carve(const_cast<void*>(binning_ws), R);
+    const int64_t max_buckets = glic_max_buckets(R, vp.W, vp.H);
+    SampleState smp = SampleState::carve(const_cast<void*>(sample_ws), max_buckets);
+    DetState det = DetState::carve(det_ws, max_buckets);
+    const int cur = tile_sort_passes(vp.grid_x * vp.grid_y) & 1;
+    if (int e = launch_render_backward_det(P, vp, max_buckets, bin.vals[cur], g, img, smp, det, dL_dpix, dL_dmeans2D, dL_dconic,
+                                           dL_dopacity, dL_dcolors, s)) return e;
+    unsigned int* n_valid = det.count;       // reused: the entry count is read by the launches above only
+    const int half = det_sorted_half(P);
+    unsigned int n = 0;
+    GLIC_CUDA_TRY(cudaMemcpyAsync(&n, det.count, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    GLIC_CUDA_TRY(cudaMemsetAsync(n_valid, 0, sizeof(unsigned int), s));
+    if (n > 0) {
+        debug_det_entries_kernel<<<(n + 255) / 256, 256, 0, s>>>(n, (uint32_t)P, det.keys[half], det.idx[half], det.vals, img.live_offsets,
+                                                                 vp.grid_x * vp.grid_y, gid, tile, values, n_valid);
+        GLIC_LAUNCH_CHECK();
+    }
+    unsigned int valid = 0;
+    GLIC_CUDA_TRY(cudaMemcpyAsync(&valid, n_valid, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    *count_host = valid;
+    return GLIC_OK;
 }
 
 int glic_debug_geom(int P, const void* geom_ws, float* depth, float* xy, float* conic_opacity, float* rgb,

@@ -8,6 +8,7 @@
 //               n_contrib[HW] u32 | pixel_colors[3HW] f32
 //   binning_ws: BinHeader | tile keys[2][R] u32 | vals[2][R] u32 | sort temp
 //   sample_ws : bucket_to_tile[Bmax] u32 | ckpt[Bmax*256] float4 (T, C.r, C.g, C.b)
+//   det_ws    : DetState (the deterministic render backward's entries, 32 per bucket)
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -227,6 +228,35 @@ struct SampleState {
     }
 };
 
+// Deterministic render backward (render.cu, launch_render_backward_det): 32 entries per bucket of the sample workspace, each the
+// nine values of one (tile, Gaussian) pair, keyed by gid; the keys and entry indices ping-pong through the stable tile sort.
+//   det_ws: count u32 | keys[2][n] u32 | idx[2][n] u32 | vals[n][9] f32 | sort temp, n = 32 * max_buckets
+struct DetState {
+    unsigned int* count;
+    uint32_t* keys[2];
+    uint32_t* idx[2];
+    float* vals;
+    void* sort_temp;
+    size_t sort_temp_size;
+    int64_t cap;                // entries
+    __host__ static DetState carve(void* ws, int64_t max_buckets, size_t* bytes = nullptr) {
+        const int64_t n = (max_buckets > 0 ? max_buckets : 1) * BUCKET;
+        Carver c(ws);
+        DetState d;
+        d.cap = n;
+        d.count = c.take<unsigned int>(1);
+        d.keys[0] = c.take<uint32_t>(n);
+        d.keys[1] = c.take<uint32_t>(n);
+        d.idx[0] = c.take<uint32_t>(n);
+        d.idx[1] = c.take<uint32_t>(n);
+        d.vals = c.take<float>(9 * (size_t)n);
+        d.sort_temp_size = sort_temp_bytes(n);
+        d.sort_temp = c.take<char>(d.sort_temp_size);
+        if (bytes) *bytes = c.total();
+        return d;
+    }
+};
+
 // getHigherMsb (rasterizer_impl.cu:42-57): number of tile-id bits included in the sort.
 inline uint32_t higher_msb(uint32_t n) {
     uint32_t msb = sizeof(n) * 4, step = msb;
@@ -257,6 +287,10 @@ __host__ __device__ inline int sort_pass_shift(int end_bit, int pass, int max_bi
 }
 // Passes of the tile sort: its sorted pairs end in buffer (passes & 1) of the ping-pong pair.
 inline int tile_sort_passes(int T) { return sort_passes(tile_sort_bits(T)); }
+// key bits of the entry sort: gids 0 .. P-1 and the sentinel P
+inline int det_key_bits(int P) { return 32 - __builtin_clz((unsigned)(P > 0 ? P : 1)); }
+// the ping-pong half that holds the sorted entries (32-bit keys sort with 8-bit digits)
+inline int det_sorted_half(int P) { return sort_passes(det_key_bits(P)) & 1; }
 
 // View parameters passed by value to kernels (pointers stay device pointers).
 struct ViewParams {
@@ -347,6 +381,11 @@ int launch_render_backward(int P, const ViewParams& vp, int64_t max_buckets, con
                            float* dL_dconic /*[P,4]*/, float* dL_dopacity, float* dL_dcolors, cudaStream_t s,
                            bool exact = false /* expf for every pixel, no visit skip (tests) */,
                            unsigned long long* counters = nullptr /* [8], device: the counting form (render.cu BwdCount) */);
+// The deterministic form of launch_render_backward (RP = 8 body, render.cu DetOut): WRITES the four 2-D gradients of every
+// Gaussian with a contribution (rows without one keep what they held: the callers' zeros); independent of grid size and scheduling.
+int launch_render_backward_det(int P, const ViewParams& vp, int64_t max_buckets, const uint32_t* point_list, GeomState g,
+                               ImageState img, SampleState smp, DetState det, const float* dL_dpix, float* dL_dmean2D,
+                               float* dL_dconic, float* dL_dopacity, float* dL_dcolors, cudaStream_t s);
 int launch_preprocess_backward(int P, int D, int M, const float* means, const float* scales, float mod,
                                const float* rots, const float* sh, const ViewParams& vp, const int* radii, GeomState g,
                                float lambda_erank, const float* dL_dmean2D, const float* dL_dconic,
@@ -366,7 +405,8 @@ extern "C" int glic_backward_compact_internal(int P, int sh_degree, int M, const
                                               int64_t R, const void* geom_ws, const void* binning_ws, const void* image_ws,
                                               const void* sample_ws, const float* dL_dpix, float* dL_dmeans2D, float* dL_dconic,
                                               float* dL_dopacity, float* dL_dcolors, const glic::CompactGrads* cg,
-                                              void* after_render_event, void* stream);
+                                              void* after_render_event, void* stream,
+                                              void* det_ws /* NULL: atomic render backward; else glic_deterministic_bytes(R, W, H) */);
 namespace glic {
 int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, float* exp_avg, float* exp_avg_sq, const float* g_geo,
                         uint32_t Pcap_geo, const float* lr6, const float* g_color, const uint8_t* flags, const float* const* campos_dev,
@@ -384,8 +424,14 @@ constexpr int EXPO_MAX_SLOTS = 32;
 int launch_exposure_adam(int S, const int* kf_of_slot_host, const float* slot_grads, float* E, float* exp_avg, float* exp_avg_sq,
                          int* steps, float lr, const unsigned int* skip_flag, cudaStream_t s);
 // glic_eval_psnr_ssim with an optional exposure E (3 channels) applied to img before the clamp
+// fixed (optional, fixed_order_sums_bytes(H, W)): the two sums in a fixed order instead of float64 atomics
 int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, const float* E, float* out2, void* scratch,
-                   size_t scratch_bytes, void* stream);
+                   size_t scratch_bytes, void* stream, void* fixed = nullptr);
+// the native mapper's photometric loss: glic_l1_ssim_loss (3 channels) or, with E, glic_l1_ssim_loss_exposure; partials (optional,
+// fixed_order_sums_bytes(H, W)) sums the loss value in a fixed order instead of with float atomics
+int photometric_loss_sum(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E, float* loss, float* dL_dimg,
+                         float* dL_dE, void* scratch, size_t scratch_bytes, void* partials, cudaStream_t s);
+size_t fixed_order_sums_bytes(int H, int W);
 // out[3][H][W] = img exposed by E (optional) and clamped to [0,1], element for element the image eval_psnr_ssim scores
 int launch_scored_image(int H, int W, const float* img, const float* E, float* out, cudaStream_t s);
 // the clamped (and exposed) images eval_psnr_ssim scored, left in its scratch: which = 0 the image, 1 the ground truth

@@ -350,6 +350,10 @@ struct glic_mapper {
     // ---- per-image buffers ----
     Dev<void> image_ws, binning_ws, sample_ws, loss_scratch, eval_scratch, extend_ws;
     int64_t bin_cap = 0;
+    // GLIC_MAPPER_OPT_DETERMINISTIC: the fixed-order render backward's workspace (glic_deterministic_bytes(bin_cap, W, H), grown
+    // with the binning capacity while the option is on) and the partials of the fixed-order loss and evaluation sums
+    bool deterministic = false;
+    Dev<void> det_ws, det_sums;
     Dev<float> color, final_T, dL_dpix, gt_dev[2], loss_dev, eval_out;
     Dev<unsigned int> vis_acc;
     Event gt_free[2], gt_ready[2], ev_flags, ev_col, ev_push, ring_ev[RING], t0, t1;
@@ -621,8 +625,13 @@ int launch_pose_step(glic_mapper* m, const int* views, int parity) {
 int set_bin_capacity(glic_mapper* m, int64_t pairs, bool exact = false) {
     if (!exact && pairs <= m->bin_cap) return GLIC_OK;
     const size_t binning_bytes = glic_binning_bytes(pairs), sample_bytes = glic_sample_bytes(pairs, m->cfg.width, m->cfg.height);
-    MAP_TRY(grow(m, {{m->binning_ws, binning_bytes}, {m->sample_ws, sample_bytes}}));
-    m->bin_cap = glic_binning_capacity(binning_bytes, sample_bytes, m->cfg.width, m->cfg.height, 0);
+    const int64_t cap = glic_binning_capacity(binning_bytes, sample_bytes, m->cfg.width, m->cfg.height, 0);
+    if (m->deterministic)     // the deterministic workspace follows the capacity, in the same growth
+        MAP_TRY(grow(m, {{m->binning_ws, binning_bytes}, {m->sample_ws, sample_bytes},
+                         {m->det_ws, glic_deterministic_bytes(cap, m->cfg.width, m->cfg.height)}}));
+    else
+        MAP_TRY(grow(m, {{m->binning_ws, binning_bytes}, {m->sample_ws, sample_bytes}}));
+    m->bin_cap = cap;
     return GLIC_OK;
 }
 
@@ -630,8 +639,20 @@ int set_bin_capacity(glic_mapper* m, int64_t pairs, bool exact = false) {
 // as it is.  The training capacity is re-derived from both workspaces exactly as glic_forward derives it, so the backward keeps
 // carving the binning workspace with the capacity the forward used.
 int grow_render_binning(glic_mapper* m, int64_t pairs) {
-    MAP_TRY(reserve(m, m->binning_ws, glic_binning_bytes(pairs)));
-    m->bin_cap = glic_binning_capacity(m->binning_ws.bytes(), m->sample_ws.bytes(), m->cfg.width, m->cfg.height, 0);
+    if (!m->deterministic) {
+        MAP_TRY(reserve(m, m->binning_ws, glic_binning_bytes(pairs)));
+        m->bin_cap = glic_binning_capacity(m->binning_ws.bytes(), m->sample_ws.bytes(), m->cfg.width, m->cfg.height, 0);
+        return GLIC_OK;
+    }
+    // a larger training capacity needs a larger deterministic workspace: both grow together or neither does
+    const size_t bb = std::max(glic_binning_bytes(pairs), m->binning_ws.bytes());
+    const int64_t cap = glic_binning_capacity(bb, m->sample_ws.bytes(), m->cfg.width, m->cfg.height, 0);
+    const size_t db = glic_deterministic_bytes(cap, m->cfg.width, m->cfg.height);
+    std::vector<Grow> list;
+    if (bb > m->binning_ws.bytes()) list.push_back(Grow{m->binning_ws, bb});
+    if (db > m->det_ws.bytes()) list.push_back(Grow{m->det_ws, db});
+    if (!list.empty()) MAP_TRY(grow(m, list));
+    m->bin_cap = cap;
     return GLIC_OK;
 }
 
@@ -704,10 +725,8 @@ __global__ void overflow_word_kernel(const GeomHeader* ghdr, float* word) { if (
 
 // the L1 + D-SSIM loss of an H x W image against gt, and its dL/dimg; with E (device, 3x4) the loss of the exposed image, and dL/dE
 int photometric_loss(glic_mapper* m, int H, int W, const float* img, const float* gt, const float* E, float* loss, float* dL_dimg, float* dL_dE) {
-    if (E)
-        return glic_l1_ssim_loss_exposure(H, W, m->cfg.lambda_dssim, img, gt, E, loss, dL_dimg, dL_dE, m->loss_scratch, m->loss_scratch.bytes(),
-                                          m->stream);
-    return glic_l1_ssim_loss(3, H, W, m->cfg.lambda_dssim, img, gt, loss, dL_dimg, m->loss_scratch, m->loss_scratch.bytes(), m->stream);
+    return photometric_loss_sum(H, W, m->cfg.lambda_dssim, img, gt, E, loss, dL_dimg, dL_dE, m->loss_scratch, m->loss_scratch.bytes(),
+                                m->deterministic ? m->det_sums.raw() : nullptr, m->stream);
 }
 
 // the backward of the last forward_view of v from dL_dpix: colour gradients into col, after_render (optional) recorded, then cg's
@@ -715,7 +734,7 @@ int backward_view(glic_mapper* m, const glic_view& v, float* col, const CompactG
     const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
     return glic_backward_compact_internal((int)m->P, m->D, m->M, a.xyz, m->act_scales, m->act_rots, a.rest, &v, m->radii, m->bin_cap, m->geom_ws,
                                           m->binning_ws, m->image_ws, m->sample_ws, m->dL_dpix, m->g_mean2D, m->g_conic, m->g_opacity, col,
-                                          &cg, after_render, m->stream);
+                                          &cg, after_render, m->stream, m->deterministic ? m->det_ws.raw() : nullptr);
 }
 
 // one optimiser step over the view batch `views` (S keyframe indices, slot-major); this rank renders slots [rank*k, rank*k + k)
@@ -865,7 +884,8 @@ int render_scored(glic_mapper* m, int is_train, int index, const char* what) {
     MAP_TRY(forward_settled(m, kf->view, 0));
     MAP_TRY(load_gt(m, *kf, m->gt_dev[0], cudaMemcpyHostToDevice, s));
     const float* E = (is_train && m->expo_on) ? m->expo_E + 12 * (size_t)index : nullptr;
-    return eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], E, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s);
+    return eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], E, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s,
+                          m->deterministic ? m->det_sums.raw() : nullptr);
 }
 
 // the whole clamped image eval_psnr_ssim last scored (eval_clamped) into rgb_host, on the mapper's stream
@@ -1702,14 +1722,16 @@ int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_
     if (h.skipped) MAP_TRY(regrow_after_skip(m, h.max_pairs));
     // scoring at the fitted camera: the full clamped (exposed) frame, then with split its score columns
     MAP_TRY(forward_settled(m, v, 0));
-    MAP_TRY(eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], use_expo ? st->E : nullptr, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s));
+    MAP_TRY(eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], use_expo ? st->E : nullptr, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s,
+                           m->deterministic ? m->det_sums.raw() : nullptr));
     if (rgb_host) MAP_TRY(scored_image_to_host(m, rgb_host));
     if (split) {
         for (int q = 0; q < 2; ++q) {
             crop_columns_kernel<<<plane_blocks((size_t)3 * H * Ws), 256, 0, s>>>(H, W, x_score, Ws, eval_clamped(m->eval_scratch, 3, H, W, q), crops[q]);
             GLIC_LAUNCH_CHECK();
         }
-        MAP_TRY(eval_psnr_ssim(3, H, Ws, crops[0], crops[1], nullptr, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s));
+        MAP_TRY(eval_psnr_ssim(3, H, Ws, crops[0], crops[1], nullptr, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s,
+                               m->deterministic ? m->det_sums.raw() : nullptr));
     }
     if (m->lpips_w) MAP_TRY(scored_lpips(m, Ws));
     float out3[3] = {0.f, 0.f, std::numeric_limits<float>::quiet_NaN()};
@@ -1909,6 +1931,20 @@ int glic_mapper_set_option(glic_mapper* m, int option, int value) {
             if (value < 1) { set_error("mapper_set_option: binning capacity must be positive"); return GLIC_ERR_INVALID_ARGUMENT; }
             MAP_TRY(poll_ring(m, true));
             return set_bin_capacity(m, value, /*exact=*/true);
+        case GLIC_MAPPER_OPT_DETERMINISTIC: {
+            MAP_TRY(poll_ring(m, true));
+            GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+            if (value) {                                 // both workspaces first, in one growth: a failure changes nothing
+                const int W = m->cfg.width, H = m->cfg.height;
+                const size_t db = glic_deterministic_bytes(m->bin_cap, W, H), sb = fixed_order_sums_bytes(H, W);
+                std::vector<Grow> list;
+                if (db > m->det_ws.bytes()) list.push_back(Grow{m->det_ws, db});
+                if (sb > m->det_sums.bytes()) list.push_back(Grow{m->det_sums, sb});
+                if (!list.empty()) MAP_TRY(grow(m, list));
+            }
+            m->deterministic = value != 0;
+            return GLIC_OK;
+        }
         default: set_error("mapper_set_option: unknown option"); return GLIC_ERR_INVALID_ARGUMENT;
     }
 }

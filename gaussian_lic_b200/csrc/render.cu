@@ -364,8 +364,23 @@ constexpr int BWD_WARPS = 4;              // warps per CTA; every warp owns one 
 // (the former body needs 96 and runs at 5).  !FAST is the former body (expf for every pixel, three suffixes); tests compare the two.  COUNT adds work counters
 // (BwdCount) and is used by tests and scripts/render_bwd_bench.py only.  No visit is skipped for want of a taking pixel:
 // at cfg2, 98 % of the (splat, two row pairs) visits have one, and a per-visit ballot cost more than it saved.
+//
+// DET (the deterministic form, RP = 8 and FAST only; the RP = 4, exact and counting forms stay atomic-only) runs the same body
+// but sends no RED: the nine values of (live bucket `live`, splat k) -- bit for bit what the atomic form would add -- are stored
+// to entry e = 32 live + k of `det` (DetOut), with the splat's gid as the entry's key.  A slot that adds nothing (past n_valid,
+// no visit, or all nine sums exactly zero: the cases the atomic form skips) gets the key `sentinel` = P.  Live buckets are
+// numbered in tile order, so the entry index orders a Gaussian's contributions by ascending tile.  launch_render_backward_det
+// then sorts the keys stably and folds each Gaussian's run (det_reduce_kernel).
 enum BwdCount { BC_LIVE, BC_SPLATS, BC_SPLATS_TAKEN, BC_VISITS, BC_VISITS_TAKEN, BC_CAND, BC_TAKEN, BC_FALLBACK, BC_N };
-template <int BWD_ROWPAIRS, int MIN_CTAS, bool FAST, bool COUNT>
+struct DetOut {
+    uint32_t* keys;           // [cap_live * 32] gid or sentinel
+    uint32_t* idx;            // [cap_live * 32] entry index (the sort's values)
+    float* vals;              // [cap_live * 32][9]
+    unsigned int* count;      // min(32 * live buckets, 32 * cap_live): the entries the sort and the reduction see
+    uint32_t cap_live;        // live buckets the arrays hold; a bucket past it (garbage counts of an overflowed forward) is dropped
+    uint32_t sentinel;
+};
+template <int BWD_ROWPAIRS, int MIN_CTAS, bool FAST, bool COUNT, bool DET = false>
 __global__ void __launch_bounds__(BWD_WARPS * 32, MIN_CTAS)
 render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr, const uint2* __restrict__ ranges,
                        const uint32_t* __restrict__ point_list, const float4* __restrict__ rec,
@@ -373,7 +388,8 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
                        const float4* __restrict__ ckpt, const uint32_t* __restrict__ n_contrib,
                        const float* __restrict__ pixel_colors, const float* __restrict__ dL_dpix,
                        float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic, float* __restrict__ dL_dopacity,
-                       float* __restrict__ dL_dcolors, unsigned long long* __restrict__ counters) {
+                       float* __restrict__ dL_dcolors, unsigned long long* __restrict__ counters, DetOut det) {
+    static_assert(!DET || (BWD_ROWPAIRS == 8 && FAST && !COUNT), "the deterministic form is the production body only");
     __shared__ float4 s_sp[BWD_WARPS][BUCKET][3];            // the bucket's splat records, per warp
     __shared__ uint32_t s_gid[BWD_WARPS][BUCKET];
     __shared__ uint32_t s_rows[BWD_WARPS][BUCKET];           // row pairs each splat can reach (8-bit mask)
@@ -383,6 +399,7 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t n_live = hdr->num_live_buckets;
+    if (DET && blockIdx.x == 0 && threadIdx.x == 0) *det.count = 32u * min(n_live, det.cap_live);
     const size_t HW = (size_t)vp.W * vp.H;
     const float ddelx_dx = 0.5f * vp.W, ddely_dy = 0.5f * vp.H;
     float4 (*sp)[3] = s_sp[warp];
@@ -491,6 +508,7 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
 
         uint32_t todo = __ballot_sync(0xffffffffu, s_rows[warp][lane] != 0);
         if (COUNT && lane == 0) ctr[BC_SPLATS] += __popc(todo);
+        uint32_t emitted = 0;                                    // DET: slots whose nine values were stored (warp-uniform)
         while (todo) {
             const int k = __ffs(todo) - 1;
             todo &= todo - 1;
@@ -626,10 +644,24 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
             v_o += __shfl_xor_sync(0xffffffffu, v_o, 4);
             v_o += __shfl_xor_sync(0xffffffffu, v_o, 2);
             v_o += __shfl_xor_sync(0xffffffffu, v_o, 1);
-            if (i_write) {
+            if constexpr (DET) {
+                // value order of an entry: mean.x, mean.y, conic.x, conic.y, conic.w, colour r, g, b, opacity
+                emitted |= 1u << k;
+                if (i_write && live < det.cap_live) {
+                    const float val = lane == 1 ? v_o : w0;
+                    det.vals[(size_t)9 * (32u * live + (uint32_t)k) + (lane == 1 ? 8 : slot)] = val * (f_op * b.y + f_one);
+                }
+            } else if (i_write) {
                 const size_t gid = s_gid[warp][k];
                 const float val = lane == 1 ? v_o : w0;
                 atomicAdd(dst_base + dst_stride * gid + dst_off, val * (f_op * b.y + f_one));
+            }
+        }
+        if constexpr (DET) {
+            if (live < det.cap_live) {
+                const uint32_t e = 32u * live + (uint32_t)lane;
+                det.keys[e] = (emitted >> lane) & 1u ? s_gid[warp][lane] : det.sentinel;
+                det.idx[e] = e;
             }
         }
     }
@@ -690,7 +722,7 @@ int launch_render_backward(int P, const ViewParams& vp, int64_t max_buckets, con
     static const int rp = getenv("GLIC_BWD_RP") ? atoi(getenv("GLIC_BWD_RP")) : 8;
     using Kern = void (*)(ViewParams, int, ImageHeader*, const uint2*, const uint32_t*, const float4*, const uint32_t*,
                           const uint32_t*, const float4*, const uint32_t*, const float*, const float*, float*, float*, float*, float*,
-                          unsigned long long*);
+                          unsigned long long*, DetOut);
     const int form = exact || counters ? 2 * (int)exact + (counters != nullptr) : rp == 8 ? 0 : 4;
     const Kern kerns[5] = {render_backward_kernel<8, 6, true, false>, render_backward_kernel<8, 6, true, true>,
                            render_backward_kernel<8, 5, false, false>, render_backward_kernel<8, 5, false, true>,
@@ -711,7 +743,117 @@ int launch_render_backward(int P, const ViewParams& vp, int64_t max_buckets, con
     const int64_t need = (max_buckets * parts + BWD_WARPS - 1) / BWD_WARPS;
     kern<<<(unsigned)std::min<int64_t>(blocks, need), BWD_WARPS * 32, 0, s>>>(
         vp, T, img.hdr, img.ranges, point_list, g.rec, img.bucket_offsets, img.live_offsets, smp.ckpt, img.n_contrib,
-        img.pixel_colors, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors, counters);
+        img.pixel_colors, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors, counters, DetOut{});
+    GLIC_LAUNCH_CHECK();
+    return GLIC_OK;
+}
+
+// ---- deterministic render backward: stable sort of the entries by gid, then one fold per Gaussian ---------------------------
+// Association of a Gaussian's contributions v_0 .. v_{n-1} (ascending tile), per value:
+//   chunk c = v_{32c} .. v_{32c+31} (the last one shorter) is left-folded from its first element: s_c = ((v_{32c} + v_{32c+1}) + ...);
+//   the result is the left fold of the chunk sums in chunk order: ((s_0 + s_1) + s_2) + ...
+// For n <= 32 that is the strict left fold.  One warp per window of 32 sorted positions: each lane that heads a run of at most 32
+// entries folds it alone; a longer run is folded by the whole warp, one chunk per lane and 32 chunks per round, and lane order
+// folds the chunk sums.
+__device__ __forceinline__ void det_load9(const float* __restrict__ vals, uint32_t e, float (&v)[9]) {
+#pragma unroll
+    for (int j = 0; j < 9; ++j) v[j] = vals[(size_t)9 * e + j];
+}
+__device__ __forceinline__ void det_store9(uint32_t gid, const float (&s)[9], float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic,
+                                           float* __restrict__ dL_dopacity, float* __restrict__ dL_dcolors) {
+    dL_dmean2D[3 * (size_t)gid + 0] = s[0]; dL_dmean2D[3 * (size_t)gid + 1] = s[1];
+    dL_dconic[4 * (size_t)gid + 0] = s[2]; dL_dconic[4 * (size_t)gid + 1] = s[3]; dL_dconic[4 * (size_t)gid + 3] = s[4];
+    dL_dcolors[3 * (size_t)gid + 0] = s[5]; dL_dcolors[3 * (size_t)gid + 1] = s[6]; dL_dcolors[3 * (size_t)gid + 2] = s[7];
+    dL_dopacity[gid] = s[8];
+}
+
+__global__ void __launch_bounds__(256)
+det_reduce_kernel(const unsigned int* __restrict__ count, uint32_t P, const uint32_t* __restrict__ keys, const uint32_t* __restrict__ idx,
+                  const float* __restrict__ vals, float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic,
+                  float* __restrict__ dL_dopacity, float* __restrict__ dL_dcolors) {
+    const uint32_t n = *count;
+    const int lane = threadIdx.x & 31;
+    const uint32_t warps = gridDim.x * (blockDim.x >> 5);
+    for (uint32_t base = 32u * (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)); base < n; base += 32u * warps) {
+        const uint32_t i = base + lane;
+        const uint32_t key = i < n ? keys[i] : P;
+        const bool head = key < P && (i == 0 || keys[i - 1] != key);
+        const bool is_long = head && i + 32 < n && keys[i + 32] == key;
+        if (head && !is_long) {
+            float s[9], v[9];
+            det_load9(vals, idx[i], s);
+            for (uint32_t j = i + 1; j < n && keys[j] == key; ++j) {
+                det_load9(vals, idx[j], v);
+#pragma unroll
+                for (int q = 0; q < 9; ++q) s[q] = __fadd_rn(s[q], v[q]);
+            }
+            det_store9(key, s, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors);
+        }
+        uint32_t longs = __ballot_sync(0xffffffffu, is_long);
+        while (longs) {
+            const int h = __ffs(longs) - 1;
+            longs &= longs - 1;
+            const uint32_t start = base + (uint32_t)h, gid = __shfl_sync(0xffffffffu, key, h);
+            float tot[9] = {};
+            bool first = true, more = true;
+            for (uint32_t round = 0; more; ++round) {
+                const uint32_t cs = start + 32u * (32u * round + (uint32_t)lane);     // this lane's chunk
+                const bool mine = cs < n && keys[cs] == gid;
+                float s[9] = {}, v[9];
+                if (mine) {
+                    det_load9(vals, idx[cs], s);
+                    for (uint32_t j = cs + 1; j < cs + 32 && j < n && keys[j] == gid; ++j) {
+                        det_load9(vals, idx[j], v);
+#pragma unroll
+                        for (int q = 0; q < 9; ++q) s[q] = __fadd_rn(s[q], v[q]);
+                    }
+                }
+                const uint32_t have = __ballot_sync(0xffffffffu, mine);      // a prefix of the lanes: the run is contiguous
+                for (int l = 0; l < 32 && ((have >> l) & 1u); ++l) {
+#pragma unroll
+                    for (int q = 0; q < 9; ++q) {
+                        const float c = __shfl_sync(0xffffffffu, s[q], l);
+                        tot[q] = first ? c : __fadd_rn(tot[q], c);
+                    }
+                    first = false;
+                }
+                more = have == 0xffffffffu;
+            }
+            if (lane == 0) det_store9(gid, tot, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors);
+        }
+    }
+}
+
+int launch_render_backward_det(int P, const ViewParams& vp, int64_t max_buckets, const uint32_t* point_list, GeomState g,
+                               ImageState img, SampleState smp, DetState det, const float* dL_dpix, float* dL_dmean2D,
+                               float* dL_dconic, float* dL_dopacity, float* dL_dcolors, cudaStream_t s) {
+    if (max_buckets <= 0 || P <= 0) return GLIC_OK;
+    const int T = vp.grid_x * vp.grid_y;
+    live_scan_kernel<<<1, 1024, 0, s>>>(T, img.max_contrib, img.live_offsets, img.hdr);
+    GLIC_LAUNCH_CHECK();
+    const auto kern = render_backward_kernel<8, 6, true, false, true>;
+    static int blocks_per_device[64] = {};
+    int dev = 0;
+    GLIC_CUDA_TRY(cudaGetDevice(&dev));
+    if (dev < 0 || dev >= 64) { set_error("render_backward: device index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!blocks_per_device[dev]) {
+        int sms = NUM_SMS, per_sm = 4;
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, BWD_WARPS * 32, 0);
+        blocks_per_device[dev] = sms * (per_sm > 0 ? per_sm : 1);
+    }
+    const int64_t need = (max_buckets + BWD_WARPS - 1) / BWD_WARPS;
+    const DetOut out{det.keys[0], det.idx[0], det.vals, det.count, (uint32_t)(det.cap / 32), (uint32_t)P};
+    kern<<<(unsigned)std::min<int64_t>(blocks_per_device[dev], need), BWD_WARPS * 32, 0, s>>>(
+        vp, T, img.hdr, img.ranges, point_list, g.rec, img.bucket_offsets, img.live_offsets, smp.ckpt, img.n_contrib,
+        img.pixel_colors, dL_dpix, nullptr, nullptr, nullptr, nullptr, nullptr, out);
+    GLIC_LAUNCH_CHECK();
+    const int cur = launch_sort_pairs32(det.cap, det_key_bits(P), det.keys, det.idx, det.sort_temp, det.sort_temp_size, s, det.count, false);
+    if (cur < 0) return cur;
+    const int64_t windows = (det.cap + 31) / 32;
+    const unsigned blocks = (unsigned)std::min<int64_t>((windows + 7) / 8, (int64_t)NUM_SMS * 16);
+    det_reduce_kernel<<<blocks, 256, 0, s>>>(det.count, (uint32_t)P, det.keys[cur], det.idx[cur], det.vals, dL_dmean2D, dL_dconic,
+                                             dL_dopacity, dL_dcolors);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }

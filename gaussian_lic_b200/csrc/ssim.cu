@@ -60,7 +60,9 @@ __device__ __forceinline__ float expose(const float* __restrict__ img, size_t HW
 // LOSS = true: additionally accumulates (1-lambda)*|a-b| - lambda*ssim, scaled by 1/N, into *loss.
 // EXPO = true: img1 is the three planes of the rendered image and the tile's channel of the exposed image is formed in the
 // halo load (it never exists in global memory); SSIM, its partial maps and the L1 term are those of the exposed image.
-template <bool LOSS, bool EXPO>
+// FIXED (fixed-order sums, the native mapper's deterministic option): the CTA's loss term goes to loss[linear block id] instead of
+// an atomicAdd into loss[0]; loss_finish_kernel sums those partials in a fixed order.
+template <bool LOSS, bool EXPO, bool FIXED = false>
 __device__ __forceinline__ void
 ssim_forward_tile(int H, int W, float C1, float C2, const float* __restrict__ img1, const float* __restrict__ img2,
                   float* __restrict__ ssim_map, float* __restrict__ dm_dmu1, float* __restrict__ dm_dsigma1_sq,
@@ -183,26 +185,28 @@ ssim_forward_tile(int H, int W, float C1, float C2, const float* __restrict__ im
             for (int w = 0; w < ST / 32; ++w) t += red[w];
             if (blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) t = fmaf(t, inv_n, lambda_dssim);
             else t *= inv_n;
-            atomicAdd(loss, t);
+            if (FIXED) loss[(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = t;
+            else atomicAdd(loss, t);
         }
     }
 }
 
-template <bool LOSS>
+template <bool LOSS, bool FIXED = false>
 __global__ void __launch_bounds__(ST)
 ssim_forward_kernel(int H, int W, float C1, float C2, const float* __restrict__ img1, const float* __restrict__ img2,
                     float* __restrict__ ssim_map, float* __restrict__ dm_dmu1, float* __restrict__ dm_dsigma1_sq,
                     float* __restrict__ dm_dsigma12, float lambda_dssim, float inv_n, float* __restrict__ loss) {
-    ssim_forward_tile<LOSS, false>(H, W, C1, C2, img1, img2, ssim_map, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, lambda_dssim, inv_n,
+    ssim_forward_tile<LOSS, false, FIXED>(H, W, C1, C2, img1, img2, ssim_map, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, lambda_dssim, inv_n,
                                    loss, nullptr);
 }
 
 // forward of the exposed loss: the partial maps of SSIM(out, gt) and the loss of out
+template <bool FIXED = false>
 __global__ void __launch_bounds__(ST)
 ssim_loss_exposure_forward_kernel(int H, int W, float C1, float C2, const float* __restrict__ img, const float* __restrict__ gt,
                                   const float* __restrict__ E, float* __restrict__ dm_dmu1, float* __restrict__ dm_dsigma1_sq,
                                   float* __restrict__ dm_dsigma12, float lambda_dssim, float inv_n, float* __restrict__ loss) {
-    ssim_forward_tile<true, true>(H, W, C1, C2, img, gt, nullptr, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, lambda_dssim, inv_n, loss, E);
+    ssim_forward_tile<true, true, FIXED>(H, W, C1, C2, img, gt, nullptr, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, lambda_dssim, inv_n, loss, E);
 }
 
 // dL/dimg1 = conv(dL*dm_dmu1) + 2*img1*conv(dL*dm_dsigma1_sq) + img2*conv(dL*dm_dsigma12)
@@ -372,6 +376,15 @@ exposure_adam_kernel(int S, ExpoBatch batch, const float* __restrict__ slot_grad
     if (j == 0) t[kf] = step;
 }
 
+// out[0] = the G per-CTA loss partials summed in a fixed order (float64, lane-strided, then an xor butterfly): one warp
+__global__ void __launch_bounds__(32) loss_finish_kernel(unsigned G, const float* __restrict__ partials, float* __restrict__ out) {
+    double s = 0.0;
+    for (unsigned b = threadIdx.x; b < G; b += 32) s += (double)partials[b];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (threadIdx.x == 0) out[0] = (float)s;
+}
+
 }  // namespace
 
 }  // namespace glic
@@ -421,8 +434,10 @@ extern "C" int glic_fused_ssim_backward(int B, int CH, int H, int W, float C1, f
 
 extern "C" size_t glic_loss_scratch_bytes(int CH, int H, int W) { return sizeof(float) * 3 * (size_t)CH * H * W + 256; }
 
-extern "C" int glic_l1_ssim_loss(int CH, int H, int W, float lambda_dssim, const float* img, const float* gt, float* loss_out,
-                                 float* dL_dimg, void* scratch, size_t scratch_bytes, void* stream) {
+// partials == NULL: the loss term of every CTA is added atomically into loss_out; otherwise (G floats, G = the forward grid) it
+// is stored per CTA and summed in a fixed order, so the loss value has the same bits on every run
+static int l1_ssim_loss_impl(int CH, int H, int W, float lambda_dssim, const float* img, const float* gt, float* loss_out, float* dL_dimg,
+                             void* scratch, size_t scratch_bytes, float* partials, cudaStream_t s) {
     if (CH <= 0 || H <= 0 || W <= 0 || !img || !gt || !loss_out || !scratch) { set_error("l1_ssim_loss: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (!planes_ok(CH, "l1_ssim_loss")) return GLIC_ERR_INVALID_ARGUMENT;
     if (scratch_bytes < glic_loss_scratch_bytes(CH, H, W)) { set_error("l1_ssim_loss: scratch too small"); return GLIC_ERR_WORKSPACE; }
@@ -432,12 +447,16 @@ extern "C" int glic_l1_ssim_loss(int CH, int H, int W, float lambda_dssim, const
     float* d3 = d2 + N;
     const float C1 = 0.01f * 0.01f, C2 = 0.03f * 0.03f;     // loss_utils.h:130-131
     const float inv_n = (float)(1.0 / (double)N);
-    cudaStream_t s = (cudaStream_t)stream;
-    GLIC_CUDA_TRY(cudaMemsetAsync(loss_out, 0, sizeof(float), s));
     dim3 grid((W + SB - 1) / SB, (H + SB - 1) / SB, CH), block(ST);
+    if (!partials) GLIC_CUDA_TRY(cudaMemsetAsync(loss_out, 0, sizeof(float), s));
     { StageTimer _t(GLIC_STAGE_LOSS_FWD, s);
-    ssim_forward_kernel<true><<<grid, block, 0, s>>>(H, W, C1, C2, img, gt, nullptr, d1, d2, d3, lambda_dssim, inv_n, loss_out); }
+    if (partials) ssim_forward_kernel<true, true><<<grid, block, 0, s>>>(H, W, C1, C2, img, gt, nullptr, d1, d2, d3, lambda_dssim, inv_n, partials);
+    else ssim_forward_kernel<true><<<grid, block, 0, s>>>(H, W, C1, C2, img, gt, nullptr, d1, d2, d3, lambda_dssim, inv_n, loss_out); }
     GLIC_LAUNCH_CHECK();
+    if (partials) {
+        loss_finish_kernel<<<1, 32, 0, s>>>(grid.x * grid.y * grid.z, partials, loss_out);
+        GLIC_LAUNCH_CHECK();
+    }
     if (dL_dimg) {
         StageTimer _t(GLIC_STAGE_LOSS_BWD, s);
         ssim_backward_kernel<true><<<grid, block, 0, s>>>(H, W, img, gt, nullptr, d1, d2, d3, dL_dimg, -lambda_dssim * inv_n,
@@ -445,6 +464,11 @@ extern "C" int glic_l1_ssim_loss(int CH, int H, int W, float lambda_dssim, const
         GLIC_LAUNCH_CHECK();
     }
     return GLIC_OK;
+}
+
+extern "C" int glic_l1_ssim_loss(int CH, int H, int W, float lambda_dssim, const float* img, const float* gt, float* loss_out,
+                                 float* dL_dimg, void* scratch, size_t scratch_bytes, void* stream) {
+    return l1_ssim_loss_impl(CH, H, W, lambda_dssim, img, gt, loss_out, dL_dimg, scratch, scratch_bytes, nullptr, (cudaStream_t)stream);
 }
 
 // scratch: the three partial maps (9 HW floats) | the mix kernel's float64 partial sums (12 per CTA)
@@ -455,9 +479,8 @@ extern "C" size_t glic_loss_exposure_scratch_bytes(int H, int W) {
     return expo_partials_offset(H, W) + sizeof(double) * 12 * (size_t)expo_blocks((size_t)H * W) + 256;
 }
 
-extern "C" int glic_l1_ssim_loss_exposure(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E,
-                                          float* loss_out, float* dL_dimg, float* dL_dE, void* scratch, size_t scratch_bytes,
-                                          void* stream) {
+static int loss_exposure_impl(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E, float* loss_out,
+                              float* dL_dimg, float* dL_dE, void* scratch, size_t scratch_bytes, float* partials, cudaStream_t s) {
     if (H <= 0 || W <= 0 || !img || !gt || !E || !loss_out || !scratch) { set_error("l1_ssim_loss_exposure: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
     if ((dL_dimg == nullptr) != (dL_dE == nullptr)) {
         set_error("l1_ssim_loss_exposure: dL_dimg and dL_dE must be both NULL (loss only) or both non-NULL"); return GLIC_ERR_INVALID_ARGUMENT;
@@ -467,28 +490,49 @@ extern "C" int glic_l1_ssim_loss_exposure(int H, int W, float lambda_dssim, cons
     float* d1 = static_cast<float*>(scratch);
     float* d2 = d1 + N;
     float* d3 = d2 + N;
-    double* partials = reinterpret_cast<double*>(static_cast<char*>(scratch) + expo_partials_offset(H, W));
+    double* expo_partials = reinterpret_cast<double*>(static_cast<char*>(scratch) + expo_partials_offset(H, W));
     const float C1 = 0.01f * 0.01f, C2 = 0.03f * 0.03f;
     const float inv_n = (float)(1.0 / (double)N);
-    cudaStream_t s = (cudaStream_t)stream;
-    GLIC_CUDA_TRY(cudaMemsetAsync(loss_out, 0, sizeof(float), s));
     dim3 grid((W + SB - 1) / SB, (H + SB - 1) / SB, 3), block(ST);
+    if (!partials) GLIC_CUDA_TRY(cudaMemsetAsync(loss_out, 0, sizeof(float), s));
     { StageTimer _t(GLIC_STAGE_LOSS_FWD, s);
-    ssim_loss_exposure_forward_kernel<<<grid, block, 0, s>>>(H, W, C1, C2, img, gt, E, d1, d2, d3, lambda_dssim, inv_n, loss_out); }
+    if (partials) ssim_loss_exposure_forward_kernel<true><<<grid, block, 0, s>>>(H, W, C1, C2, img, gt, E, d1, d2, d3, lambda_dssim, inv_n, partials);
+    else ssim_loss_exposure_forward_kernel<<<grid, block, 0, s>>>(H, W, C1, C2, img, gt, E, d1, d2, d3, lambda_dssim, inv_n, loss_out); }
     GLIC_LAUNCH_CHECK();
+    if (partials) {
+        loss_finish_kernel<<<1, 32, 0, s>>>(grid.x * grid.y * grid.z, partials, loss_out);
+        GLIC_LAUNCH_CHECK();
+    }
     if (dL_dimg) {
         StageTimer _t(GLIC_STAGE_LOSS_BWD, s);
         ssim_loss_exposure_backward_kernel<<<grid, block, 0, s>>>(H, W, img, gt, E, d1, d2, d3, dL_dimg, -lambda_dssim * inv_n,
                                                                   (1.0f - lambda_dssim) * inv_n);
         GLIC_LAUNCH_CHECK();
         const unsigned G = expo_blocks(HW);
-        exposure_mix_kernel<<<G, XT, 0, s>>>(HW, img, E, dL_dimg, partials);
+        exposure_mix_kernel<<<G, XT, 0, s>>>(HW, img, E, dL_dimg, expo_partials);
         GLIC_LAUNCH_CHECK();
-        partials_finish_kernel<12><<<1, 12 * 32, 0, s>>>(G, partials, dL_dE);
+        partials_finish_kernel<12><<<1, 12 * 32, 0, s>>>(G, expo_partials, dL_dE);
         GLIC_LAUNCH_CHECK();
     }
     return GLIC_OK;
 }
+
+extern "C" int glic_l1_ssim_loss_exposure(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E,
+                                          float* loss_out, float* dL_dimg, float* dL_dE, void* scratch, size_t scratch_bytes,
+                                          void* stream) {
+    return loss_exposure_impl(H, W, lambda_dssim, img, gt, E, loss_out, dL_dimg, dL_dE, scratch, scratch_bytes, nullptr, (cudaStream_t)stream);
+}
+
+namespace glic {
+// the native mapper's photometric loss (glic_l1_ssim_loss on 3 channels, or glic_l1_ssim_loss_exposure with E); partials
+// (fixed_order_sums_bytes(H, W)) selects the fixed-order loss sum
+int photometric_loss_sum(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E, float* loss, float* dL_dimg,
+                         float* dL_dE, void* scratch, size_t scratch_bytes, void* partials, cudaStream_t s) {
+    float* p = static_cast<float*>(partials);
+    if (E) return loss_exposure_impl(H, W, lambda_dssim, img, gt, E, loss, dL_dimg, dL_dE, scratch, scratch_bytes, p, s);
+    return l1_ssim_loss_impl(3, H, W, lambda_dssim, img, gt, loss, dL_dimg, scratch, scratch_bytes, p, s);
+}
+}  // namespace glic
 
 namespace glic {
 int launch_exposure_adam(int S, const int* kf_of_slot, const float* slot_grads, float* E, float* m, float* v, int* t, float lr,
@@ -520,6 +564,9 @@ __device__ __forceinline__ float scored_pixel(const float* __restrict__ img, con
 }
 
 // clamp both images to [0,1] (the image exposed first, scored_pixel) into scratch copies and accumulate the squared error.
+// FIXED (the native mapper's deterministic option): each warp stores its float64 sum to acc2[global warp id] instead of adding it
+// atomically; eval_finish_fixed_kernel sums the warps in a fixed order.
+template <bool FIXED = false>
 __global__ void __launch_bounds__(256)
 eval_clamp_mse_kernel(size_t N, const float* __restrict__ img, const float* __restrict__ gt, float* __restrict__ a,
                       float* __restrict__ b, double* __restrict__ acc2, const float* __restrict__ E, size_t HW) {
@@ -533,7 +580,8 @@ eval_clamp_mse_kernel(size_t N, const float* __restrict__ img, const float* __re
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
-    if ((threadIdx.x & 31) == 0 && se != 0.0) atomicAdd(&acc2[0], se);
+    if (FIXED) { if ((threadIdx.x & 31) == 0) acc2[blockIdx.x * 8 + (threadIdx.x >> 5)] = se; }
+    else if ((threadIdx.x & 31) == 0 && se != 0.0) atomicAdd(&acc2[0], se);
 }
 
 __global__ void __launch_bounds__(256)
@@ -542,13 +590,29 @@ scored_image_kernel(size_t N, const float* __restrict__ img, const float* __rest
         out[i] = scored_pixel(img, E, HW, i);
 }
 
+template <bool FIXED = false>
 __global__ void __launch_bounds__(256)
 eval_sum_kernel(size_t N, const float* __restrict__ map, double* __restrict__ acc2) {
     double s = 0.0;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += (size_t)gridDim.x * blockDim.x) s += (double)map[i];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if ((threadIdx.x & 31) == 0) atomicAdd(&acc2[1], s);
+    if (FIXED) { if ((threadIdx.x & 31) == 0) acc2[blockIdx.x * 8 + (threadIdx.x >> 5)] = s; }
+    else if ((threadIdx.x & 31) == 0) atomicAdd(&acc2[1], s);
+}
+
+// eval_finish_kernel on the per-warp partials of the FIXED forms: warps [0, n) of mse and of ssim, summed in a fixed order
+__global__ void __launch_bounds__(32)
+eval_finish_fixed_kernel(size_t N, unsigned n, const double* __restrict__ mse_part, const double* __restrict__ ssim_part, float* __restrict__ out2) {
+    double a = 0.0, b = 0.0;
+    for (unsigned i = threadIdx.x; i < n; i += 32) { a += mse_part[i]; b += ssim_part[i]; }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); b += __shfl_xor_sync(0xffffffffu, b, o); }
+    if (threadIdx.x == 0) {
+        const float mse = (float)(a / (double)N);
+        out2[0] = 10.0f * log10f(1.0f / mse);
+        out2[1] = (float)(b / (double)N);
+    }
 }
 
 __global__ void eval_finish_kernel(size_t N, const double* __restrict__ acc2, float* __restrict__ out2) {
@@ -564,7 +628,7 @@ extern "C" size_t glic_eval_scratch_bytes(int CH, int H, int W) { return sizeof(
 
 namespace glic {
 int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, const float* E, float* out2, void* scratch,
-                   size_t scratch_bytes, void* stream) {
+                   size_t scratch_bytes, void* stream, void* fixed) {
     if (CH <= 0 || H <= 0 || W <= 0 || !img || !gt || !out2 || !scratch || (E && CH != 3)) { set_error("eval_psnr_ssim: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (scratch_bytes < glic_eval_scratch_bytes(CH, H, W)) { set_error("eval_psnr_ssim: scratch too small"); return GLIC_ERR_WORKSPACE; }
     const size_t N = (size_t)CH * H * W;
@@ -573,8 +637,20 @@ int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, cons
     float* a = reinterpret_cast<float*>(static_cast<char*>(scratch) + 256);
     float* b = a + N;
     float* map = b + N;
-    GLIC_CUDA_TRY(cudaMemsetAsync(acc2, 0, 2 * sizeof(double), s));
     const unsigned blocks = (unsigned)std::min<size_t>((N + 255) / 256, (size_t)NUM_SMS * 8);
+    if (fixed) {                                                      // per-warp partials, summed in a fixed order
+        double* mse_part = static_cast<double*>(fixed);
+        double* ssim_part = mse_part + (size_t)NUM_SMS * 8 * 8;
+        eval_clamp_mse_kernel<true><<<blocks, 256, 0, s>>>(N, img, gt, a, b, mse_part, E, (size_t)H * W);
+        GLIC_LAUNCH_CHECK();
+        if (int e = glic_fused_ssim(1, CH, H, W, 0.01f * 0.01f, 0.03f * 0.03f, a, b, map, nullptr, nullptr, nullptr, stream)) return e;
+        eval_sum_kernel<true><<<blocks, 256, 0, s>>>(N, map, ssim_part);
+        GLIC_LAUNCH_CHECK();
+        eval_finish_fixed_kernel<<<1, 32, 0, s>>>(N, blocks * 8, mse_part, ssim_part, out2);
+        GLIC_LAUNCH_CHECK();
+        return GLIC_OK;
+    }
+    GLIC_CUDA_TRY(cudaMemsetAsync(acc2, 0, 2 * sizeof(double), s));
     eval_clamp_mse_kernel<<<blocks, 256, 0, s>>>(N, img, gt, a, b, acc2, E, (size_t)H * W);
     GLIC_LAUNCH_CHECK();
     if (int e = glic_fused_ssim(1, CH, H, W, 0.01f * 0.01f, 0.03f * 0.03f, a, b, map, nullptr, nullptr, nullptr, stream)) return e;
@@ -601,3 +677,12 @@ extern "C" int glic_eval_psnr_ssim(int CH, int H, int W, const float* img, const
                                    size_t scratch_bytes, void* stream) {
     return eval_psnr_ssim(CH, H, W, img, gt, nullptr, out2, scratch, scratch_bytes, stream);
 }
+
+namespace glic {
+// the scratch of the fixed-order sums at H x W (3 channels): the loss's per-CTA partials or the evaluation's per-warp partials
+size_t fixed_order_sums_bytes(int H, int W) {
+    const size_t loss = sizeof(float) * 3 * (size_t)((W + SB - 1) / SB) * ((H + SB - 1) / SB);
+    const size_t eval = sizeof(double) * 2 * (size_t)NUM_SMS * 8 * 8;
+    return std::max(loss, eval) + 256;
+}
+}  // namespace glic

@@ -156,14 +156,28 @@ RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Ten
         ViewHold vh = make_view(viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, limx_neg, limx_pos, limy_neg, limy_pos, H, W);
         // R is the exact num_rendered the forward carved its workspaces with (ctx round trip, rasterizer.cpp)
         const int64_t cap = R;
-        check(glic_backward(P, degree, M, m.data_ptr<float>(), s.data_ptr<float>(), scale_modifier, r.data_ptr<float>(),
-                            d.data_ptr<float>(), M > 0 ? shc.data_ptr<float>() : nullptr, &vh.view, rad.data_ptr<int>(),
-                            cap, gb.data_ptr(), bb.data_ptr(), ib.data_ptr(), sb.data_ptr(), g.data_ptr<float>(), lambda_erank,
-                            dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(), dL_dopacities.data_ptr<float>(),
-                            dL_dcolors.data_ptr<float>(), dL_dmeans3D.data_ptr<float>(), dL_dcov3Ds.data_ptr<float>(),
-                            dL_ddc.data_ptr<float>(), M > 0 ? dL_dsh.data_ptr<float>() : nullptr,
-                            dL_dscales.data_ptr<float>(), dL_drotations.data_ptr<float>(), cur_stream()),
-              "backward");
+        if (at::globalContext().deterministicAlgorithms()) {
+            // torch.use_deterministic_algorithms(True): the fixed-order render backward, its workspace from the caching allocator
+            torch::Tensor det = torch::empty({(int64_t)glic_deterministic_bytes(cap, W, H)}, means3D.options().dtype(torch::kByte));
+            check(glic_backward_deterministic(P, degree, M, m.data_ptr<float>(), s.data_ptr<float>(), scale_modifier, r.data_ptr<float>(),
+                                              d.data_ptr<float>(), M > 0 ? shc.data_ptr<float>() : nullptr, &vh.view, rad.data_ptr<int>(),
+                                              cap, gb.data_ptr(), bb.data_ptr(), ib.data_ptr(), sb.data_ptr(), g.data_ptr<float>(),
+                                              lambda_erank, dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(),
+                                              dL_dopacities.data_ptr<float>(), dL_dcolors.data_ptr<float>(), dL_dmeans3D.data_ptr<float>(),
+                                              dL_dcov3Ds.data_ptr<float>(), dL_ddc.data_ptr<float>(), M > 0 ? dL_dsh.data_ptr<float>() : nullptr,
+                                              dL_dscales.data_ptr<float>(), dL_drotations.data_ptr<float>(), det.data_ptr(),
+                                              (size_t)det.numel(), cur_stream()),
+                  "backward_deterministic");
+        } else {
+            check(glic_backward(P, degree, M, m.data_ptr<float>(), s.data_ptr<float>(), scale_modifier, r.data_ptr<float>(),
+                                d.data_ptr<float>(), M > 0 ? shc.data_ptr<float>() : nullptr, &vh.view, rad.data_ptr<int>(),
+                                cap, gb.data_ptr(), bb.data_ptr(), ib.data_ptr(), sb.data_ptr(), g.data_ptr<float>(), lambda_erank,
+                                dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(), dL_dopacities.data_ptr<float>(),
+                                dL_dcolors.data_ptr<float>(), dL_dmeans3D.data_ptr<float>(), dL_dcov3Ds.data_ptr<float>(),
+                                dL_ddc.data_ptr<float>(), M > 0 ? dL_dsh.data_ptr<float>() : nullptr,
+                                dL_dscales.data_ptr<float>(), dL_drotations.data_ptr<float>(), cur_stream()),
+                  "backward");
+        }
     }
     return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dopacities, dL_dmeans3D, dL_dcov3Ds, dL_ddc, dL_dsh, dL_dscales,
                            dL_drotations);

@@ -197,6 +197,10 @@ class Mapper:
     def set_binning_pairs(self, pairs):
         capi.check(capi.lib.glic_mapper_set_option(self._h, 2, int(pairs)), "mapper_set_option")
 
+    def set_deterministic(self, on):
+        """GLIC_MAPPER_OPT_DETERMINISTIC: fixed-order render backward, loss and evaluation sums (bit-reproducible training)"""
+        capi.check(capi.lib.glic_mapper_set_option(self._h, 3, int(bool(on))), "mapper_set_option")
+
     def enable_exposure(self, exposure_lr=0.001):
         """Train a 3x4 affine exposure per training keyframe from now on (config/fastlivo.yaml:25-26: exposure_lr 0.001)."""
         capi.check(capi.lib.glic_mapper_enable_exposure(self._h, float(exposure_lr)), "mapper_enable_exposure")

@@ -295,6 +295,7 @@ class CRasterizer:
         self.geom_ws = torch.empty(0, **u8)
         self.binning_ws = torch.empty(0, **u8)
         self.sample_ws = torch.empty(0, **u8)
+        self.det_ws = torch.empty(0, **u8)       # glic_backward_deterministic's workspace, grown on first use
         self.loss_scratch = torch.empty(self.lib.glic_loss_scratch_bytes(3, self.H, self.W), **u8)
         self.R = 0
         self.B = 0
@@ -408,16 +409,22 @@ class CRasterizer:
                     dL_ddc=torch.empty(P, 1, 3, **f32), dL_dsh=torch.empty(P, M, 3, **f32),
                     dL_dscales=torch.empty(P, 3, **f32), dL_drots=torch.empty(P, 4, **f32))
 
-    def backward(self, g, view, radii, dL_dpix, grads=None, scale_modifier=1.0, lambda_erank=0.0):
+    def backward(self, g, view, radii, dL_dpix, grads=None, scale_modifier=1.0, lambda_erank=0.0, deterministic=False):
+        """glic_backward on the saved state of the last forward; deterministic=True: glic_backward_deterministic (bit-identical
+        outputs across calls on the same state, contributions added in ascending tile order)."""
         grads = self.alloc_grads() if grads is None else grads
-        capi.check(self.lib.glic_backward(
-            self.P, self.D, self.M, capi.ptr(g["means"]), capi.ptr(g["scales"]), scale_modifier, capi.ptr(g["rots"]),
-            capi.ptr(g["dc"]), capi.ptr(g["sh"]) if self.M else None, C.byref(view), capi.ptr(radii), self.cap,
-            capi.ptr(self.geom_ws), capi.ptr(self.binning_ws), capi.ptr(self.image_ws), capi.ptr(self.sample_ws),
-            capi.ptr(dL_dpix), lambda_erank, capi.ptr(grads["dL_dmeans2D"]), capi.ptr(grads["dL_dconic"]),
-            capi.ptr(grads["dL_dopacity"]), capi.ptr(grads["dL_dcolors"]), capi.ptr(grads["dL_dmeans3D"]),
-            capi.ptr(grads["dL_dcov3D"]), capi.ptr(grads["dL_ddc"]), capi.ptr(grads["dL_dsh"]) if self.M else None,
-            capi.ptr(grads["dL_dscales"]), capi.ptr(grads["dL_drots"]), self.stream), "backward")
+        args = [self.P, self.D, self.M, capi.ptr(g["means"]), capi.ptr(g["scales"]), scale_modifier, capi.ptr(g["rots"]),
+                capi.ptr(g["dc"]), capi.ptr(g["sh"]) if self.M else None, C.byref(view), capi.ptr(radii), self.cap,
+                capi.ptr(self.geom_ws), capi.ptr(self.binning_ws), capi.ptr(self.image_ws), capi.ptr(self.sample_ws),
+                capi.ptr(dL_dpix), lambda_erank, capi.ptr(grads["dL_dmeans2D"]), capi.ptr(grads["dL_dconic"]),
+                capi.ptr(grads["dL_dopacity"]), capi.ptr(grads["dL_dcolors"]), capi.ptr(grads["dL_dmeans3D"]),
+                capi.ptr(grads["dL_dcov3D"]), capi.ptr(grads["dL_ddc"]), capi.ptr(grads["dL_dsh"]) if self.M else None,
+                capi.ptr(grads["dL_dscales"]), capi.ptr(grads["dL_drots"])]
+        if deterministic:
+            ws = self._grow("det_ws", self.lib.glic_deterministic_bytes(self.cap, self.W, self.H), slack=1.0)
+            capi.check(self.lib.glic_backward_deterministic(*args, capi.ptr(ws), ws.numel(), self.stream), "backward_deterministic")
+        else:
+            capi.check(self.lib.glic_backward(*args, self.stream), "backward")
         return grads
 
     def loss(self, img, gt, lambda_dssim=0.2, loss_out=None, dL_dimg=None):
@@ -441,6 +448,25 @@ class CRasterizer:
             capi.ptr(self.sample_ws), capi.ptr(dL_dpix), capi.ptr(grads["dL_dmeans2D"]), capi.ptr(grads["dL_dconic"]),
             capi.ptr(grads["dL_dopacity"]), capi.ptr(grads["dL_dcolors"]), int(exact), capi.ptr(counters), self.stream),
             "debug_render_backward")
+
+    def deterministic_entries(self, view, dL_dpix, grads):
+        """The deterministic render backward alone on the saved state of the last forward (glic_debug_deterministic_entries):
+        writes grads' four 2-D gradient tensors and returns the ordered entry list as device tensors gid [n] int32, tile [n]
+        int32 and values [n, 9] float32 (mean.x, mean.y, conic.x, conic.y, conic.w, colour r, g, b, opacity), in the order the
+        reduction adds them."""
+        ws = self._grow("det_ws", self.lib.glic_deterministic_bytes(self.cap, self.W, self.H), slack=1.0)
+        cap = 32 * max(int(self.lib.glic_max_buckets(self.cap, self.W, self.H)), 1)
+        gid = torch.empty(cap, dtype=torch.int32, device=self.dev)
+        tile = torch.empty(cap, dtype=torch.int32, device=self.dev)
+        values = torch.empty(cap, 9, dtype=torch.float32, device=self.dev)
+        n = C.c_int64(0)
+        capi.check(self.lib.glic_debug_deterministic_entries(
+            self.P, C.byref(view), self.cap, capi.ptr(self.geom_ws), capi.ptr(self.binning_ws), capi.ptr(self.image_ws),
+            capi.ptr(self.sample_ws), capi.ptr(dL_dpix), capi.ptr(ws), ws.numel(), capi.ptr(grads["dL_dmeans2D"]),
+            capi.ptr(grads["dL_dconic"]), capi.ptr(grads["dL_dopacity"]), capi.ptr(grads["dL_dcolors"]), C.byref(n), capi.ptr(gid),
+            capi.ptr(tile), capi.ptr(values), self.stream), "debug_deterministic_entries")
+        n = int(n.value)
+        return gid[:n], tile[:n], values[:n]
 
     # ---- introspection for parity tests -------------------------------------------------------------------
     def debug_state(self):

@@ -170,6 +170,27 @@ GLIC_API int glic_backward(int P, int sh_degree, int M, const float* means3D, co
                   float* dL_dopacity, float* dL_dcolors, float* dL_dmeans3D, float* dL_dcov3D,
                   float* dL_ddc, float* dL_dsh, float* dL_dscales, float* dL_drotations, void* stream);
 
+/* Deterministic backward: glic_backward's arguments and outputs, plus a workspace of glic_deterministic_bytes(num_rendered,
+ * width, height) bytes (num_rendered as glic_backward takes it).  Every output is a function of the saved forward state and
+ * dL_dpix alone: calls on the same state give the same bits, whatever the grid size, scheduling or order of the GPU's work.
+ * The render backward (the production RP = 8 body only) stores each (tile, Gaussian) pair's nine contributions -- bit for bit
+ * the values glic_backward adds atomically -- and adds a Gaussian's contributions in ascending tile index:
+ *   chunks of 32 consecutive contributions are each left-folded from their first element, then the chunk sums are
+ *   left-folded in chunk order; for 32 or fewer contributions that is the strict left fold.
+ * Rows with no contribution are zero.  Agreement with glic_backward: within the reassociation bound of the n contributions.
+ * A short det_ws returns GLIC_ERR_WORKSPACE with nothing enqueued.  The workspace is 32 entries per checkpoint bucket (36 B of
+ * values + 16 B of sort keys and indices each) plus the sort's temp; the GLIC_BWD_RP = 4, exact and counting forms of the debug
+ * hook have no deterministic form. */
+GLIC_API size_t glic_deterministic_bytes(int64_t num_rendered, int width, int height);
+GLIC_API int glic_backward_deterministic(int P, int sh_degree, int M, const float* means3D, const float* scales,
+                  float scale_modifier, const float* rotations, const float* dc, const float* sh,
+                  const glic_view* view, const int* radii, int64_t num_rendered, const void* geom_ws,
+                  const void* binning_ws, const void* image_ws, const void* sample_ws,
+                  const float* dL_dpix, float lambda_erank, float* dL_dmeans2D, float* dL_dconic,
+                  float* dL_dopacity, float* dL_dcolors, float* dL_dmeans3D, float* dL_dcov3D,
+                  float* dL_ddc, float* dL_dsh, float* dL_dscales, float* dL_drotations, void* det_ws, size_t det_bytes,
+                  void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * Stable LSD radix sort of (uint64 key, uint32 value) pairs on key bits [0, end_bit).
  * Replaces cub::DeviceRadixSort::SortPairs<uint64,uint32>(begin_bit=0, end_bit)
@@ -349,6 +370,16 @@ GLIC_API int glic_debug_render_backward(int P, const glic_view* view, int64_t R,
                                         const void* image_ws, const void* sample_ws, const float* dL_dpix, float* dL_dmeans2D,
                                         float* dL_dconic, float* dL_dopacity, float* dL_dcolors, int exact,
                                         unsigned long long* counters, void* stream);
+/* The deterministic render backward alone on the saved state of the last glic_forward (R = its binning capacity): WRITES the
+ * four 2-D gradient buffers as glic_backward_deterministic does (zeroing them first), then copies out the ordered entry list:
+ * *count_host (HOST) = n entries, and for entry i < n gid[i], tile[i] (u32) and values[9 i .. 9 i + 8] (mean.x, mean.y,
+ * conic.x, conic.y, conic.w, colour r, g, b, opacity) in the order the reduction adds them: by gid, then ascending tile.
+ * gid, tile and values (DEVICE) hold 32 * glic_max_buckets(R, W, H) entries.  Synchronises `stream`. */
+GLIC_API int glic_debug_deterministic_entries(int P, const glic_view* view, int64_t R, const void* geom_ws, const void* binning_ws,
+                                              const void* image_ws, const void* sample_ws, const float* dL_dpix, void* det_ws,
+                                              size_t det_bytes, float* dL_dmeans2D, float* dL_dconic, float* dL_dopacity,
+                                              float* dL_dcolors, int64_t* count_host, uint32_t* gid, uint32_t* tile, float* values,
+                                              void* stream);
 /* The mapper's per-Gaussian backward alone, on the saved state of the last glic_forward and given render-backward outputs
  * (device arrays; rotations activated, rot_raw the raw ones, opacity activated).  pose_only = 0: the COMPACT + POSE form of an
  * iteration under pose refinement, writing the 11 geometric floats of every row to g_geo [11 P] (rotation [P,4] | xyz [P,3] |
@@ -707,7 +738,17 @@ GLIC_API int glic_mapper_synchronize(glic_mapper* m);
 /* options: GLIC_MAPPER_OPT_OPTIMIZER (default 1): 0 leaves the Adam launch out of the iteration, so that a benchmark can time
  * the rasterization step (activations, forward, loss, backward, exchange) on its own.  Keyframe images may be device pointers
  * (the copy uses cudaMemcpyDefault): that is how "inputs resident in HBM" is measured. */
-enum { GLIC_MAPPER_OPT_OPTIMIZER = 1, GLIC_MAPPER_OPT_BINNING_PAIRS = 2 /* (tile, Gaussian) pairs the binning workspace holds; grows by itself on overflow */ };
+/* GLIC_MAPPER_OPT_DETERMINISTIC (default 0): 1 makes every later optimize, align, evaluate, evaluate_lpips and render use the
+ * deterministic render backward of glic_backward_deterministic and fixed-order sums for the loss value and the PSNR / SSIM sums;
+ * 0 switches them off again.  Either call drains the pipeline.  With the option on, given the same calls, seeds and inputs, on
+ * the same GPU model and library build, every getter returns the same bits: the parameters, both Adam moments, the poses, E and
+ * their Adam state, the densification statistics, the screen radii, the sky rows, stats (last_loss included) and the density
+ * totals, and the metrics and images of evaluate, render, align and render_camera.  The option costs a workspace that follows the
+ * binning capacity (glic_deterministic_bytes of it), allocated by the call and grown with the capacity under the failure contract
+ * above (a failed allocation returns GLIC_ERR_CUDA and leaves the mapper, the option included, as it was).  With world > 1 every
+ * rank must set it identically; the reduce adds in rank order, so runs then repeat across runs and replicas. */
+enum { GLIC_MAPPER_OPT_OPTIMIZER = 1, GLIC_MAPPER_OPT_BINNING_PAIRS = 2 /* (tile, Gaussian) pairs the binning workspace holds; grows by itself on overflow */,
+       GLIC_MAPPER_OPT_DETERMINISTIC = 3 };
 GLIC_API int glic_mapper_set_option(glic_mapper* m, int option, int value);
 /* Per-keyframe exposure (the reference's apply_exposure / exposure_lr, config/fastlivo.yaml:25-26, which its render()
  * never applies).  Off by default.  glic_mapper_enable_exposure(m, lr) may be called before or between optimize() calls:
