@@ -84,6 +84,10 @@ class RenderCamera(C.Structure):
                 ("cy", C.c_float), ("width", C.c_int), ("height", C.c_int)]
 
 
+class UnseenParams(C.Structure):
+    _fields_ = [("views", C.c_void_p), ("n_views", C.c_int), ("min_weight", C.c_float), ("min_hits", C.c_uint64), ("sky", C.c_int)]
+
+
 def _load():
     if not os.path.isfile(LIB_PATH):
         raise ImportError(
@@ -112,6 +116,7 @@ def _load():
                                vp, vp]),
         "glic_render": (i32, [i32, i32, i32, vp, vp, f32, vp, vp, vp, vp, C.POINTER(View), vp, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp,
                               vp, vp]),
+        "glic_contribution": (i32, [i32, vp, vp, f32, vp, vp, C.POINTER(View), vp, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, vp, vp]),
         "glic_forward_render": (i32, [i32, C.POINTER(View), i32, i64, vp, vp, vp, sz, vp, sz, vp, vp, C.POINTER(i64), vp]),
         "glic_backward": (i32, [i32, i32, i32, vp, vp, f32, vp, vp, vp, C.POINTER(View), vp, i64, vp, vp, vp, vp, vp, f32,
                                 vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
@@ -204,6 +209,8 @@ def _load():
         "glic_mapper_pose_adam_state": (i32, [vp, i32, C.POINTER(f32), C.POINTER(f32), C.POINTER(i32)]),
         "glic_mapper_align": (i32, [vp, i32, i32, C.POINTER(AlignParams), C.POINTER(AlignResult), vp]),
         "glic_mapper_render_camera": (i32, [vp, C.POINTER(RenderCamera), i32, i32, vp, vp, vp, vp]),
+        "glic_mapper_contribution": (i32, [vp, C.POINTER(i32), i32, vp, vp, vp]),
+        "glic_mapper_prune_unseen": (i32, [vp, C.POINTER(UnseenParams), i32, C.POINTER(u32)]),
         "glic_mapper_enable_frames": (i32, [vp, i32, i32, i32]),
         "glic_mapper_add_frame": (i32, [vp, C.POINTER(Frame), C.POINTER(i32)]),
         "glic_mapper_keyframe_image": (i32, [vp, i32, i32, vp]),

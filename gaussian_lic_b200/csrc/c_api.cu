@@ -359,6 +359,42 @@ int glic_render(int P, int sh_degree, int M, const float* means3D, const float* 
     return GLIC_OK;
 }
 
+int glic_contribution(int P, const float* means3D, const float* scales, float scale_modifier, const float* rotations,
+                      const float* opacities, const glic_view* view, int* radii, void* geom_ws, size_t geom_bytes, void* image_ws,
+                      size_t image_bytes, void* binning_ws, size_t binning_bytes, float* max_weight, uint64_t* hits,
+                      uint64_t* ends, float* out_final_T, int64_t* counters_host, void* stream) {
+    if (int e = check_view(view)) return e;
+    if (P < 0) { set_error("contribution: P must be >= 0"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!image_ws || image_bytes < glic_image_bytes(view->width, view->height)) { set_error("contribution: image workspace too small"); return GLIC_ERR_WORKSPACE; }
+    if (P > 0 && (!max_weight || !hits)) { set_error("contribution: null output"); return GLIC_ERR_INVALID_ARGUMENT; }
+    cudaStream_t s = (cudaStream_t)stream;
+    const ViewParams vp = make_view_params(view);
+    const size_t HW = (size_t)vp.W * vp.H;
+    ImageState img = ImageState::carve(image_ws, vp.W, vp.H);
+    if (P == 0) {                                      // glic_forward's outputs for an empty scene; nothing to score
+        if (out_final_T) GLIC_CUDA_TRY(cudaMemsetAsync(out_final_T, 0, sizeof(float) * HW, s));
+        GLIC_CUDA_TRY(cudaMemsetAsync(img.hdr, 0, sizeof(ImageHeader), s));
+        if (counters_host) GLIC_CUDA_TRY(cudaMemcpyAsync(counters_host, img.hdr->counters, 3 * sizeof(long long), cudaMemcpyDeviceToHost, s));
+        return GLIC_OK;
+    }
+    if (!means3D || !scales || !rotations || !opacities || !radii) { set_error("contribution: null input pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!aligned16(rotations)) { set_error("contribution: rotations must be 16-byte aligned"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!geom_ws || geom_bytes < glic_geom_bytes(P)) { set_error("contribution: geometry workspace too small"); return GLIC_ERR_WORKSPACE; }
+    const int64_t cap = glic_binning_capacity(binning_bytes, 0, vp.W, vp.H, 1);
+    if (!binning_ws || cap < 1) { set_error("contribution: binning workspace missing or too small"); return GLIC_ERR_WORKSPACE; }
+    GeomState g = GeomState::carve(geom_ws, P);
+    BinningState bin = BinningState::carve(binning_ws, cap);
+    // glic_forward's stages with no_color = 1, so the lists are its lists; an overflow leaves every range empty (r_eff = 0), so
+    // the blend takes no pair and adds nothing
+    const int cur = bin_view(P, 0, 0, means3D, scales, scale_modifier, rotations, opacities, nullptr, nullptr, vp, true, radii, g, bin,
+                             img, cap, false, s);
+    if (cur < 0) return cur;
+    { StageTimer _t(GLIC_STAGE_RENDER_FWD, s);
+      if (int e = launch_render_score(vp, bin.vals[cur], g, img, max_weight, hits, ends, out_final_T, s)) return e; }
+    if (counters_host) GLIC_CUDA_TRY(cudaMemcpyAsync(counters_host, img.hdr->counters, 3 * sizeof(long long), cudaMemcpyDeviceToHost, s));
+    return GLIC_OK;
+}
+
 size_t glic_deterministic_bytes(int64_t num_rendered, int width, int height) {
     size_t b = 0;
     DetState::carve(nullptr, glic_max_buckets(num_rendered > 0 ? num_rendered : 0, width, height), &b);

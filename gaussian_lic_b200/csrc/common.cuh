@@ -376,6 +376,11 @@ int launch_render_forward(const ViewParams& vp, bool no_color, const uint32_t* p
 // the inference form of the blend (glic_render): colour, final T and, when non-null, expected and median depth; nothing else
 int launch_render_infer(const ViewParams& vp, const uint32_t* point_list, GeomState g, ImageState img, float* out_color,
                         float* out_final_T, float* out_depth, float* out_median, cudaStream_t s);
+// the scoring form of the blend (glic_contribution): accumulates every taken pair's weight into max_weight (max) and hits (count)
+// of its Gaussian, and every pixel it ends into ends (may be null); out_final_T (may be null) as launch_render_forward writes it
+// with no_color
+int launch_render_score(const ViewParams& vp, const uint32_t* point_list, GeomState g, ImageState img, float* max_weight,
+                        uint64_t* hits, uint64_t* ends, float* out_final_T, cudaStream_t s);
 int launch_render_backward(int P, const ViewParams& vp, int64_t max_buckets, const uint32_t* point_list, GeomState g,
                            ImageState img, SampleState smp, const float* dL_dpix, float* dL_dmean2D /*[P,3]*/,
                            float* dL_dconic /*[P,4]*/, float* dL_dopacity, float* dL_dcolors, cudaStream_t s,
@@ -446,6 +451,13 @@ struct DensitySelect {
     const int* maxr;                 // read only when max_screen_radius > 0
     float grad_threshold, clone_max, min_opacity, max_world_scale;
     int max_screen_radius;
+    // glic_mapper_prune_unseen's test: both null (the default), no row goes by it and neither is read
+    const float* score_max = nullptr;
+    const uint64_t* score_hits = nullptr;
+    const uint64_t* score_ends = nullptr;   // pixels the row ends: they count towards min_hits with its hits
+    float min_weight = 0.0f;
+    uint64_t min_hits = 0;
+    int score_sky = 0;               // 1: sky rows can go by it too
 };
 // select: the fate of every row; result_host[6] = {clones, splits, surviving kept rows, surviving clones, surviving split rows,
 // surviving sky rows}, synchronises s; the scratch then holds the index map of the surviving rows (density_index: idx[new] = old)

@@ -390,6 +390,8 @@ struct glic_mapper {
     Dev<char> align_ws;
     // ---- rendering from a caller's camera (glic_mapper_render_camera): its workspace (render_carve) for the largest frame so far
     Dev<char> render_ws;
+    // ---- contribution scores (glic_mapper_contribution / prune_unseen): hits [Pcap] u64 | max_weight [Pcap] f32, sized on first use
+    Dev<char> score_ws;
     // ---- raw frames (glic_mapper_enable_frames / add_frame): the 8-bit image store, chunks of FRAME_CHUNK frames of
     //      frame_stride bytes that never move, and the scan of the frames since the last training keyframe (device arrays
     //      of scan_cap points, grown by doubling) ----
@@ -1452,8 +1454,9 @@ namespace {
 // Otherwise it only prunes: no statistic is read, the statistics (with densification on) move with their rows, dens_calls
 // stays (it keys the children's draws of every later densify), and a call that removes nothing touches nothing.
 // The caller has validated p.  reject_empty: a result without rows is an error (densify on an empty map is not).
+// unseen (optional, a prune only): the scores in score_ws (contribution below) also remove rows, by glic_mapper_prune_unseen's test.
 int density_step(glic_mapper* m, const glic_density_params& p, bool densify, int dry_run, bool reject_empty, glic_density_counts* out,
-                 const char* what) {
+                 const char* what, const glic_unseen_params* unseen = nullptr) {
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     MAP_TRY(poll_ring(m, true));
     const uint32_t P = m->P;
@@ -1463,9 +1466,17 @@ int density_step(glic_mapper* m, const glic_density_params& p, bool densify, int
         MAP_TRY(reserve(m, m->extend_ws, density_scratch_bytes(P)));   // the selection's scratch: the idle extend() staging
         const ArenaRows g = arena_rows(m->params, m->Pcap, m->M);
         const float* no_stats = nullptr;                   // a prune selects no row, with densification on or off
-        const DensitySelect a{P, m->n_sky, densify ? m->dens_accum : no_stats, densify ? m->dens_denom : no_stats, g.log_scale, g.opacity,
-                              m->dens_maxr, p.grad_threshold, p.percent_dense * p.scene_extent, p.min_opacity, p.max_world_scale,
-                              p.max_screen_radius};
+        DensitySelect a{P, m->n_sky, densify ? m->dens_accum : no_stats, densify ? m->dens_denom : no_stats, g.log_scale, g.opacity,
+                        m->dens_maxr, p.grad_threshold, p.percent_dense * p.scene_extent, p.min_opacity, p.max_world_scale,
+                        p.max_screen_radius};
+        if (unseen) {
+            a.score_hits = reinterpret_cast<const uint64_t*>(m->score_ws.raw());
+            a.score_ends = a.score_hits + m->Pcap;
+            a.score_max = reinterpret_cast<const float*>(a.score_hits + 2 * (size_t)m->Pcap);
+            a.min_weight = unseen->min_weight;
+            a.min_hits = unseen->min_hits;
+            a.score_sky = unseen->sky;
+        }
         MAP_TRY(launch_density_select(a, m->extend_ws, r, s));
     }
     const uint32_t n_clone = r[0], n_split = r[1], kept = r[2], cloned = r[3], split = r[4];
@@ -1797,9 +1808,81 @@ int render_camera(glic_mapper* m, const glic_render_camera& c, int exposure_inde
     return GLIC_OK;
 }
 
+// ---- contribution scores (glic_mapper_contribution, glic_mapper_prune_unseen) ------------------------------------------------
+// score_ws: hits [Pcap] u64 | ends [Pcap] u64 | max_weight [Pcap] f32
+size_t score_bytes(uint32_t cap) { return (size_t)cap * (2 * sizeof(uint64_t) + sizeof(float)); }
+
+// a NULL view list (every training keyframe), or n >= 0 training keyframe indices
+int views_check(const glic_mapper* m, const int* views, int n, const char* what) {
+    if (n < 0) { set_error(std::string(what) + ": n_views must be >= 0"); return GLIC_ERR_INVALID_ARGUMENT; }
+    for (int q = 0; views && q < n; ++q)
+        if (views[q] < 0 || views[q] >= (int)m->train.size()) { set_error(std::string(what) + ": view index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
+    return GLIC_OK;
+}
+
+// The scores of every row over training keyframes views[0 .. n) (NULL: all of them) into score_ws, which the caller has
+// reserved (score_bytes(Pcap)) after draining the ring.  Every row is drawn at the keyframe's current camera block, as training
+// draws it; an overflowed view added nothing, so it is redrawn into the same arrays with a larger binning workspace.
+int contribution(glic_mapper* m, const int* views, int n) {
+    cudaStream_t s = m->stream;
+    uint64_t* hits = reinterpret_cast<uint64_t*>(m->score_ws.raw());
+    uint64_t* ends = hits + m->Pcap;
+    float* max_weight = reinterpret_cast<float*>(hits + 2 * (size_t)m->Pcap);
+    GLIC_CUDA_TRY(cudaMemsetAsync(m->score_ws, 0, score_bytes(m->Pcap), s));
+    if (!m->P) return GLIC_OK;
+    MAP_TRY(activate(m));
+    const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
+    const int count = views ? n : (int)m->train.size();
+    for (int q = 0; q < count; ++q) {
+        const glic_view& v = m->train[views ? views[q] : q].view;
+        MAP_TRY(draw_settled(m, [&](long long* cnt) {
+            return glic_contribution((int)m->P, a.xyz, m->act_scales, 1.0f, m->act_rots, m->act_opacity, &v, m->radii, m->geom_ws,
+                                     m->geom_ws.bytes(), m->image_ws, m->image_ws.bytes(), m->binning_ws, m->binning_ws.bytes(), max_weight,
+                                     hits, ends, nullptr, (int64_t*)cnt, s);
+        }, [&](int64_t pairs) { return grow_render_binning(m, pairs); }));
+        // draw_settled gives up after four draws: a view still overflowing then was not scored, and its rows must not go
+        if (m->counters_host[2]) { set_error("mapper_contribution: a view still overflows the binning workspace after regrowing it"); return GLIC_ERR_WORKSPACE; }
+    }
+    return GLIC_OK;
+}
+
 }  // namespace
 
 extern "C" {
+
+int glic_mapper_contribution(glic_mapper* m, const int* views_host, int n_views, float* max_weight, uint64_t* hits, uint64_t* ends) {
+    if (!m || (!max_weight && !hits && !ends)) { set_error("mapper_contribution: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    MAP_TRY(views_check(m, views_host, n_views, "mapper_contribution"));
+    MAP_TRY(poll_ring(m, true));
+    MAP_TRY(reserve(m, m->score_ws, score_bytes(m->Pcap)));
+    MAP_TRY(contribution(m, views_host, n_views));
+    const uint64_t* h = reinterpret_cast<const uint64_t*>(m->score_ws.raw());
+    if (m->P && hits) GLIC_CUDA_TRY(cudaMemcpyAsync(hits, h, sizeof(uint64_t) * m->P, cudaMemcpyDefault, m->stream));
+    if (m->P && ends) GLIC_CUDA_TRY(cudaMemcpyAsync(ends, h + m->Pcap, sizeof(uint64_t) * m->P, cudaMemcpyDefault, m->stream));
+    if (m->P && max_weight) GLIC_CUDA_TRY(cudaMemcpyAsync(max_weight, h + 2 * (size_t)m->Pcap, sizeof(float) * m->P, cudaMemcpyDefault, m->stream));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    return GLIC_OK;
+}
+
+// the scores, then the compaction with no row selected, both size tests and the opacity test off, and the unseen test on
+int glic_mapper_prune_unseen(glic_mapper* m, const glic_unseen_params* p, int dry_run, uint32_t* removed) {
+    if (!m || !p) { set_error("mapper_prune_unseen: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!std::isfinite(p->min_weight) || p->min_weight < 0.0f || p->min_weight > 1.0f) {
+        set_error("mapper_prune_unseen: min_weight must be finite and in [0, 1]"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (p->sky != 0 && p->sky != 1) { set_error("mapper_prune_unseen: sky must be 0 or 1"); return GLIC_ERR_INVALID_ARGUMENT; }
+    MAP_TRY(views_check(m, p->views, p->n_views, "mapper_prune_unseen"));
+    if (m->P) {
+        MAP_TRY(poll_ring(m, true));
+        MAP_TRY(reserve(m, m->score_ws, score_bytes(m->Pcap)));
+        MAP_TRY(reserve(m, m->extend_ws, density_scratch_bytes(m->P)));      // the selection's scratch (density_step)
+        MAP_TRY(contribution(m, p->views, p->n_views));
+    }
+    glic_density_counts k{};
+    MAP_TRY(density_step(m, glic_density_params{0.0f, 0.0f, 0.0f, 0.0f, 0, 0.0f}, false, dry_run, m->P != 0, &k, "mapper_prune_unseen", p));
+    if (removed) *removed = k.pruned;
+    return GLIC_OK;
+}
 
 // the compaction with no row selected and both size tests off; a mapper with no rows has nothing to remove (0, not an error)
 int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, uint32_t* removed) {

@@ -148,6 +148,8 @@ constexpr float SPLIT_LOG_SCALE = 0x1.e148a2p-2f;              // (float)log(1.6
 // predicate: act(logit) < min_opacity, or (non-sky rows) maxr > max_screen_radius > 0, or largest scale > max_world_scale > 0.
 // Clones and children have maxr 0, and the children's scale is their own (the parent's log-scale - log(1.6)).
 // Without statistics (a.accum null) no row is selected; then, with both size tests off, a row's logit is all that is read.
+// With the scores (a.score_max, glic_mapper_prune_unseen, where no row is selected) the row itself also goes when it is not a
+// sky row, or a.score_sky is set, and its max_weight < min_weight or hits + ends < min_hits (the pixels it takes or ends).
 constexpr unsigned FATE_ROW = 4u, FATE_CLONE = 8u, FATE_CHILDREN = 16u;
 
 __device__ __forceinline__ float largest_scale(const float* ls) {
@@ -183,7 +185,8 @@ __device__ __forceinline__ unsigned row_fate(uint32_t r, const DensitySelect& a)
         return cls | (gone ? 0u : FATE_CHILDREN);
     }
     const bool copy_gone = faded || (!sky && world && smax > a.max_world_scale);
-    const bool row_gone = copy_gone || (!sky && a.max_screen_radius > 0 && a.maxr[r] > a.max_screen_radius);
+    const bool unseen = a.score_max && (!sky || a.score_sky) && (a.score_max[r] < a.min_weight || a.score_hits[r] + a.score_ends[r] < a.min_hits);
+    const bool row_gone = copy_gone || unseen || (!sky && a.max_screen_radius > 0 && a.maxr[r] > a.max_screen_radius);
     return cls | (row_gone ? 0u : FATE_ROW) | (cls == 1u && !copy_gone ? FATE_CLONE : 0u);
 }
 

@@ -137,21 +137,36 @@ struct __align__(16) SplatRec { float4 a, b, c; };     // (x, y, conic.x, conic.
 // final T keep their bits, plus the expected depth sum_i T_i alpha_i z_i (unnormalised, like the colour: one more FMA per taken
 // pair, z from the record) and the median depth (z of the first taken splat after which T < 0.5, else 0).  It writes none of
 // the backward's state (checkpoints, bucket_to_tile, n_contrib, max_contrib, pixel_colors); out_depth / out_median may be
-// null.  The training form (INFER = false) compiles every INFER line out.
+// null.
+//
+// SCORE (glic_contribution) is the alpha-only scoring form: the no_color training blend over the same lists in the same operation
+// order, so T and the set of taken (pixel, splat) pairs are the training blend's, bit for bit.  For each taken pair it forms the
+// weight w = fl(T alpha) (T before the splat) and adds it to the splat's two scores: score_max[gid] = max(score_max[gid], w), as
+// atomicMax on the bits of a non-negative float, and score_hits[gid] += 1.  A splat that ends a pixel (T (1 - alpha) < 1e-4) is
+// not taken there, but removing it would let the pixel blend on, so it counts in score_ends[gid] (may be null: not counted).
+// The pairs land first in a shared-memory slot per splat of the 256-splat batch (shared atomics; taken pixels in the low 16
+// bits of the count, ended pixels in the high 16, at most 256 of each), double-buffered by batch parity; after the barrier that
+// ends a batch, each non-empty slot sends one global atomic of each kind it holds and is zeroed.  out_T (may be null) gets the final T; nothing else is
+// written.  The training form compiles every INFER and SCORE line out, INFER every SCORE line.
 constexpr int FWD_THREADS = 128;
+enum FwdForm { FWD_TRAIN, FWD_INFER, FWD_SCORE };
 
-template <bool INFER>
+template <int FORM>
 __global__ void __launch_bounds__(FWD_THREADS)
 render_forward_kernel(ViewParams vp, bool no_color, const uint2* __restrict__ ranges,
                       const uint32_t* __restrict__ point_list, const float4* __restrict__ rec,
                       const uint32_t* __restrict__ bucket_offsets, uint32_t* __restrict__ bucket_to_tile,
                       float4* __restrict__ ckpt, uint32_t* __restrict__ n_contrib, uint32_t* __restrict__ max_contrib,
                       float* __restrict__ pixel_colors, float* __restrict__ out_color, float* __restrict__ out_T,
-                      float* __restrict__ out_depth, float* __restrict__ out_median) {
+                      float* __restrict__ out_depth, float* __restrict__ out_median, unsigned int* __restrict__ score_max,
+                      unsigned long long* __restrict__ score_hits, unsigned long long* __restrict__ score_ends) {
+    constexpr bool INFER = FORM == FWD_INFER, SCORE = FORM == FWD_SCORE;
     if (INFER) no_color = false;                                 // the inference form always blends colour
+    if (SCORE) no_color = true;                                  // the scoring form blends alpha only
     __shared__ SplatRec s_rec[2][TILE_PIX];
     __shared__ __align__(8) uint64_t s_bar[2];
     __shared__ uint32_t s_red[FWD_THREADS / 32];
+    __shared__ uint32_t s_wmax[2][TILE_PIX], s_hits[2][TILE_PIX];    // SCORE: the batch's slots (max weight bits, pixel counts)
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t tile = blockIdx.y * vp.grid_x + blockIdx.x;
@@ -169,6 +184,8 @@ render_forward_kernel(ViewParams vp, bool no_color, const uint2* __restrict__ ra
     const int rounds = (n_splats + TILE_PIX - 1) / TILE_PIX;
 
     if (tid == 0) { mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_fence_init(); }
+    if (SCORE)
+        for (int u = tid; u < 2 * TILE_PIX; u += FWD_THREADS) { (&s_wmax[0][0])[u] = 0u; (&s_hits[0][0])[u] = 0u; }
     uint32_t bbm = 0;
     if (!INFER && !no_color) {
         bbm = tile == 0 ? 0u : bucket_offsets[tile - 1];
@@ -189,6 +206,22 @@ render_forward_kernel(ViewParams vp, bool no_color, const uint2* __restrict__ ra
         }
     };
     if (rounds > 0) prefetch(0);
+    // SCORE: batch r's non-empty slots to the global scores, then zeroed for batch r + 2 (after the barrier that ends batch r)
+    auto score_flush = [&](int r) {
+        const int cnt = min(TILE_PIX, n_splats - r * TILE_PIX);
+        for (int u = tid; u < cnt; u += FWD_THREADS) {
+            const uint32_t h = s_hits[r & 1][u];
+            if (h) {
+                const uint32_t id = point_list[range.x + r * TILE_PIX + u];
+                if (h & 0xFFFFu) {
+                    atomicMax(score_max + id, s_wmax[r & 1][u]);
+                    atomicAdd(score_hits + id, (unsigned long long)(h & 0xFFFFu));
+                }
+                if ((h >> 16) && score_ends) atomicAdd(score_ends + id, (unsigned long long)(h >> 16));
+                s_wmax[r & 1][u] = 0u; s_hits[r & 1][u] = 0u;
+            }
+        }
+    };
 
     // this warp covers tile rows 4w .. 4w+3: splats whose alpha >= 1/255 ellipse cannot reach them are skipped
     // warp-uniformly (conservative half-extent `hy` precomputed per splat => bit-identical results)
@@ -207,6 +240,7 @@ render_forward_kernel(ViewParams vp, bool no_color, const uint2* __restrict__ ra
     for (int i = 0; i < rounds; ++i) {
         // everyone is past batch i-1 (its buffer may be refilled) -- and we may stop if all pixels are done
         if (__syncthreads_count(done0 && done1) == FWD_THREADS) break;
+        if (SCORE && i > 0) score_flush(i - 1);
         if (i + 1 < rounds) prefetch(i + 1);
         mbar_wait(&s_bar[i & 1], (uint32_t)((i >> 1) & 1));
         waited = i + 1;
@@ -249,8 +283,15 @@ render_forward_kernel(ViewParams vp, bool no_color, const uint2* __restrict__ ra
                 float tt0, tt1, t0, t1;
                 f2_unpack(test_T, tt0, tt1);
                 f2_unpack(Tp, t0, t1);
+                const bool end0 = SCORE && !skip0 && tt0 < 0.0001f, end1 = SCORE && !skip1 && tt1 < 0.0001f;
                 if (!skip0 && tt0 < 0.0001f) { done0 = true; skip0 = true; }
                 if (!skip1 && tt1 < 0.0001f) { done1 = true; skip1 = true; }
+                if (SCORE && (!(skip0 && skip1) || end0 || end1)) {
+                    // a positive float's bits order as the float does, so the slot keeps max w as an integer max
+                    const float w0 = skip0 ? 0.0f : __fmul_rn(t0, a0), w1 = skip1 ? 0.0f : __fmul_rn(t1, a1);
+                    if (!(skip0 && skip1)) atomicMax(&s_wmax[i & 1][j], __float_as_uint(fmaxf(w0, w1)));
+                    atomicAdd(&s_hits[i & 1][j], (skip0 ? 0u : 1u) + (skip1 ? 0u : 1u) + (((end0 ? 1u : 0u) + (end1 ? 1u : 0u)) << 16));
+                }
                 if (done0 && done1) break;
                 if (!no_color) {
                     // a pixel that does not take the splat blends with alpha = 0: C = fma(T, 0, C) = C exactly
@@ -284,6 +325,15 @@ render_forward_kernel(ViewParams vp, bool no_color, const uint2* __restrict__ ra
     float t0, t1, r0, r1, g0, g1, b0, b1;
     f2_unpack(Tp, t0, t1); f2_unpack(Cr, r0, r1); f2_unpack(Cg, g0, g1); f2_unpack(Cb, b0, b1);
     const size_t HW = (size_t)vp.W * vp.H;
+    if (SCORE) {
+        __syncthreads();                                          // the last batch's slots are complete
+        if (waited > 0) score_flush(waited - 1);
+        if (out_T) {
+            if (inside0) out_T[pid0] = t0;
+            if (inside1) out_T[pid1] = t1;
+        }
+        return;
+    }
     if (INFER) {
         float d0, d1;
         f2_unpack(Dp, d0, d1);
@@ -692,10 +742,10 @@ int launch_tile_ranges(int64_t R, const GeomHeader* ghdr, const uint32_t* keys_s
 int launch_render_forward(const ViewParams& vp, bool no_color, const uint32_t* point_list, GeomState g, ImageState img,
                           SampleState smp, float* out_color, float* out_final_T, cudaStream_t s) {
     dim3 grid(vp.grid_x, vp.grid_y), block(FWD_THREADS);
-    render_forward_kernel<false><<<grid, block, 0, s>>>(vp, no_color, img.ranges, point_list, g.rec, img.bucket_offsets,
-                                                        smp.bucket_to_tile, smp.ckpt,
-                                                        img.n_contrib, img.max_contrib, img.pixel_colors, out_color,
-                                                        out_final_T, nullptr, nullptr);
+    render_forward_kernel<FWD_TRAIN><<<grid, block, 0, s>>>(vp, no_color, img.ranges, point_list, g.rec, img.bucket_offsets,
+                                                            smp.bucket_to_tile, smp.ckpt,
+                                                            img.n_contrib, img.max_contrib, img.pixel_colors, out_color,
+                                                            out_final_T, nullptr, nullptr, nullptr, nullptr, nullptr);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }
@@ -703,8 +753,21 @@ int launch_render_forward(const ViewParams& vp, bool no_color, const uint32_t* p
 int launch_render_infer(const ViewParams& vp, const uint32_t* point_list, GeomState g, ImageState img, float* out_color,
                         float* out_final_T, float* out_depth, float* out_median, cudaStream_t s) {
     dim3 grid(vp.grid_x, vp.grid_y), block(FWD_THREADS);
-    render_forward_kernel<true><<<grid, block, 0, s>>>(vp, false, img.ranges, point_list, g.rec, nullptr, nullptr, nullptr,
-                                                       nullptr, nullptr, nullptr, out_color, out_final_T, out_depth, out_median);
+    render_forward_kernel<FWD_INFER><<<grid, block, 0, s>>>(vp, false, img.ranges, point_list, g.rec, nullptr, nullptr, nullptr,
+                                                            nullptr, nullptr, nullptr, out_color, out_final_T, out_depth, out_median,
+                                                            nullptr, nullptr, nullptr);
+    GLIC_LAUNCH_CHECK();
+    return GLIC_OK;
+}
+
+int launch_render_score(const ViewParams& vp, const uint32_t* point_list, GeomState g, ImageState img, float* max_weight,
+                        uint64_t* hits, uint64_t* ends, float* out_final_T, cudaStream_t s) {
+    dim3 grid(vp.grid_x, vp.grid_y), block(FWD_THREADS);
+    render_forward_kernel<FWD_SCORE><<<grid, block, 0, s>>>(vp, true, img.ranges, point_list, g.rec, nullptr, nullptr, nullptr,
+                                                            nullptr, nullptr, nullptr, nullptr, out_final_T, nullptr, nullptr,
+                                                            reinterpret_cast<unsigned int*>(max_weight),
+                                                            reinterpret_cast<unsigned long long*>(hits),
+                                                            reinterpret_cast<unsigned long long*>(ends));
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }

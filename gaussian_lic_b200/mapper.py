@@ -321,6 +321,33 @@ class Mapper:
         capi.check(capi.lib.glic_mapper_prune(self._h, float(min_opacity), int(bool(dry_run)), C.byref(out)), "mapper_prune")
         return int(out.value)
 
+    def contribution(self, views=None):
+        """The contribution scores of every row, sky rows included, over training keyframes `views` (None: all of them), each
+        drawn at its current pose (glic_mapper_contribution).  Returns numpy arrays (max_weight [P] float32: the largest
+        T * alpha of any pixel that takes the row; hits [P] uint64: the number of (view, pixel) pairs that take it; ends [P]
+        uint64: the number of (view, pixel) pairs whose blend it ends without being taken)."""
+        P = int(self.stats().num_gaussians)
+        mw, hits, ends = np.zeros(max(P, 1), np.float32), np.zeros(max(P, 1), np.uint64), np.zeros(max(P, 1), np.uint64)
+        arr, n = (None, 0) if views is None else ((C.c_int * len(views))(*[int(v) for v in views]), len(views))
+        capi.check(capi.lib.glic_mapper_contribution(self._h, arr, n, _p(mw), _p(hits), _p(ends)), "mapper_contribution")
+        return mw[:P], hits[:P], ends[:P]
+
+    def prune_unseen(self, min_hits=1, min_weight=0.0, sky=False, views=None, dry_run=False):
+        """Remove every row (sky rows only with sky=True) whose scores over training keyframes `views` (None: all) fall short:
+        hits + ends < min_hits or max_weight < min_weight (glic_mapper_prune_unseen).  The defaults remove exactly the rows that
+        neither take nor end a pixel of any scored view, which changes none of those views' pixels.  The compaction is
+        prune()'s.  dry_run only counts.  Returns the number of rows removed (or that would be)."""
+        p = capi.UnseenParams()
+        keep = None
+        if views is not None:
+            keep = (C.c_int * max(len(views), 1))(*[int(v) for v in views])
+            p.views, p.n_views = C.cast(keep, C.c_void_p), len(views)
+        p.min_weight, p.min_hits, p.sky = float(min_weight), int(min_hits), int(sky)
+        out = C.c_uint32()
+        capi.check(capi.lib.glic_mapper_prune_unseen(self._h, C.byref(p), int(bool(dry_run)), C.byref(out)), "mapper_prune_unseen")
+        del keep
+        return int(out.value)
+
     def enable_densification(self):
         """Gather the view-space gradient statistics densify() selects on, from the next iteration on (world > 1: before
         export_handle())."""

@@ -389,6 +389,32 @@ class CRasterizer:
         out["radii"], out["counters"] = radii[:P], (R, B, ovf)
         return out
 
+    def contribution(self, g, view, max_weight, hits, ends=None, scale_modifier=1.0, final_T=False, radii=None):
+        """One glic_contribution call at this rasterizer's size, synchronised: the view's contribution scores ADDED to max_weight
+        [P] float32 (max), hits [P] int64 (sum of taken pixels) and, when given, ends [P] int64 (sum of pixels the row ends)
+        device tensors; an overflow grows the binning workspace and
+        draws again (the overflowed call added nothing).  It draws into the workspaces forward() uses and publishes R as finish()
+        does, so debug_state() shows this call's lists.  Returns final_T [H,W] (a device tensor) when asked for, else None."""
+        lib = self.lib
+        P = int(g["means"].shape[0])
+        out_T = torch.empty(self.H, self.W, dtype=torch.float32, device=self.dev) if final_T else None
+        radii = torch.empty(max(P, 1), dtype=torch.int32, device=self.dev) if radii is None else radii
+        self._grow("geom_ws", lib.glic_geom_bytes(P))
+        if self.cap_target == 0:
+            self.cap_target = max(8 * P, 1 << 16)
+        while True:
+            self._grow("binning_ws", lib.glic_binning_bytes(self.cap_target), slack=1.0)
+            self.cap = int(lib.glic_binning_capacity(self.binning_ws.numel(), 0, self.W, self.H, 1))
+            capi.check(lib.glic_contribution(
+                P, capi.ptr(g["means"]), capi.ptr(g["scales"]), scale_modifier, capi.ptr(g["rots"]), capi.ptr(g["opacity"]),
+                C.byref(view), capi.ptr(radii), capi.ptr(self.geom_ws), self.geom_ws.numel(), capi.ptr(self.image_ws),
+                self.image_ws.numel(), capi.ptr(self.binning_ws), self.binning_ws.numel(), capi.ptr(max_weight), capi.ptr(hits),
+                capi.ptr(ends), capi.ptr(out_T), capi.ptr(self.counters), self.stream), "contribution")
+            self.P = P
+            if not self.finish():
+                break
+        return out_T
+
     def finish(self):
         """Synchronise, publish R / B, and grow the capacity if the last forward overflowed (returns True then)."""
         torch.cuda.synchronize(self.dev)

@@ -153,6 +153,35 @@ GLIC_API int glic_render(int P, int sh_degree, int M, const float* means3D, cons
                          float* out_depth /* may be NULL */, float* out_median_depth /* may be NULL */,
                          int64_t* counters_host, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Contribution scores: how much each Gaussian adds to a view.  Definitions: for a view and a pixel, walk the pixel's tile list
+ * front to back as the training blend does.  A splat is TAKEN when all of
+ *   power <= 0;   alpha = min(0.99, o expf(power)) >= 1/255;   T (1 - alpha) >= 1e-4
+ * hold (a splat that would push T below 1e-4 ends the pixel and is not taken).  These are the pairs the colour, the contributor
+ * counts and the render backward see.  A taken pair's WEIGHT is w = __fmul_rn(T, alpha), T the pixel's transmittance just
+ * before the splat.  Over a set of views, row i's scores are
+ *   max_weight[i]: the largest w of any taken pair of row i, 0 if none;
+ *   hits[i]:       the number of taken (view, pixel) pairs of row i;
+ *   ends[i]:       the number of (view, pixel) pairs row i ENDS: the splat passes the first two tests but T (1 - alpha) < 1e-4.
+ *                  It is not taken, yet it stops the pixel's blend, so without it the splats behind would be blended there.
+ * All three are order-free (a float max and integer sums): bit-reproducible under any scheduling and independent of view order.
+ * A row with hits = ends = 0 over a set of views changes none of their pixels: at every pixel it is skipped by tests that do not
+ * depend on T, or reached only after the pixel has ended, so removing it leaves every pixel's sequence of blended splats as it was.
+ * glic_contribution scores one view: the stages of glic_forward with no_color = 1 up to the blend, unchanged (the same tile
+ * lists), then an alpha-only form of the blend that ACCUMULATES into the caller's max_weight[P] (max), hits[P] and ends[P] (sums) --
+ * zero them once, then call once per view.  out_final_T (may be NULL) equals glic_forward's final_T bit for bit.  Nothing
+ * else is written; there is no sample workspace and no host synchronisation.
+ *   capacity = glic_binning_capacity(binning_bytes, 0, W, H, 1) pairs; counters_host[3] = {R, 0, overflow} as glic_render
+ *   writes it.  A call that overflows adds nothing to any array, so repeating it with room for R pairs is exact.
+ *   P = 0: nothing is scored, out_final_T is 0 (as glic_forward).  Arguments are checked as glic_render checks them; max_weight
+ *   and hits must be non-NULL when P > 0; ends may be NULL (not counted).  Profiled under GLIC_STAGE_PREPROCESS, _SORT, _EMIT, _RANGES and _RENDER_FWD.
+ * ------------------------------------------------------------------------------------- */
+GLIC_API int glic_contribution(int P, const float* means3D, const float* scales, float scale_modifier, const float* rotations,
+                               const float* opacities, const glic_view* view, int* radii, void* geom_ws, size_t geom_bytes,
+                               void* image_ws, size_t image_bytes, void* binning_ws, size_t binning_bytes,
+                               float* max_weight /*[P], accumulated*/, uint64_t* hits /*[P], accumulated*/,
+                               uint64_t* ends /*[P], accumulated, may be NULL*/, float* out_final_T /* may be NULL */, int64_t* counters_host, void* stream);
+
 /* Backward.  Replaces CudaRasterizer::Rasterizer::backward (rasterizer_impl.cu:476-580;
  * backward.cu:138-597) AND the ten torch::zeros of rasterize_points.cu:192-201: every output
  * element is written (exact zeros for culled Gaussians), nothing needs pre-zeroing.
@@ -882,6 +911,41 @@ typedef struct glic_render_camera {
 } glic_render_camera;
 GLIC_API int glic_mapper_render_camera(glic_mapper* m, const glic_render_camera* cam, int exposure_index, int with_sky,
                                        float* rgb, float* final_T, float* depth, float* median_depth);
+/* Pruning the rows no view blends.  glic_mapper_contribution(m, views_host, n_views, max_weight, hits, ends) computes the
+ * contribution scores (glic_contribution) of every row, sky rows included, over training keyframes views_host[0 .. n_views)
+ * (NULL: every training keyframe; held-out keyframes are never scored, which would leak the test set into the map).  Each view
+ * is drawn at its current camera block (the refined pose under pose refinement), every row drawn, as training draws it; a
+ * view that overflows the binning workspace grows it and is drawn again (stats.overflow_regrows counts it), and only the
+ * binning workspace grows; a view that still overflows after four draws fails the call with GLIC_ERR_WORKSPACE rather than go
+ * unscored.  max_weight [P] floats, hits [P] and ends [P] uint64 are host or device memory (cudaMemcpyDefault); any of them may
+ * be NULL, not all three.  The map is frozen as under glic_mapper_render_camera.  The call drains the iteration pipeline first
+ * and synchronises at the end; with world > 1 it is rank-local and touches no exchange slot.
+ * glic_mapper_prune_unseen(m, p, dry_run, removed) computes the scores over p->views as above and removes every row for which
+ *   (the row is not a sky row, or p->sky = 1) and (max_weight < p->min_weight or hits + ends < p->min_hits);
+ * with min_hits = GLIC_MAPPER_UNSEEN_MIN_HITS and min_weight = 0 that is exactly the rows that neither take nor end a pixel of
+ * any scored view, so no pixel of those views changes: their render, evaluation and render_camera planes at their poses keep
+ * every bit.
+ * The compaction is glic_mapper_prune's (stable order, parameters and both moments bit for
+ * bit, the densification statistics moving with their rows, the sky-row count updated so save_map still writes the non-sky
+ * survivors, the densify call counter untouched, vacated rows zeroed, capacity unchanged).  *removed (may be NULL) gets the
+ * count; dry_run != 0 only counts.  Memory: the score buffers (20 B per row of capacity, kept for the next call) and the
+ * selection scratch are reserved before the scores are computed; the spare arena is allocated, as glic_mapper_prune allocates
+ * it, before the map changes (failure contract above).  Rejected with GLIC_ERR_INVALID_ARGUMENT, changing nothing:
+ * a NULL m or p, n_views < 0, a view index out of range, min_weight not finite or not in [0, 1], sky not 0 or 1, a result with
+ * no rows (dry run or not).  A mapper with no rows returns GLIC_OK with 0 removed.  world > 1: every rank makes the same call
+ * between the same optimize() calls; every rank holds every training keyframe and the scores are order-free, so replicas
+ * remove the same rows with no exchange. */
+#define GLIC_MAPPER_UNSEEN_MIN_HITS 1
+typedef struct glic_unseen_params {
+    const int* views;              /* host, training keyframe indices; NULL: every training keyframe */
+    int n_views;                   /* >= 0; ignored when views is NULL */
+    float min_weight;              /* in [0, 1]: remove rows whose max_weight < min_weight */
+    uint64_t min_hits;             /* remove rows whose hits + ends < min_hits */
+    int sky;                       /* 1: sky rows can be removed too; 0: they stay */
+} glic_unseen_params;
+GLIC_API int glic_mapper_contribution(glic_mapper* m, const int* views_host, int n_views, float* max_weight, uint64_t* hits,
+                                      uint64_t* ends);
+GLIC_API int glic_mapper_prune_unseen(glic_mapper* m, const glic_unseen_params* p, int dry_run, uint32_t* removed);
 /* Raw frames (Dataset::addFrame, gaussian.cpp:41-111, and the keyframe hand-off of mapping.cpp:158-174): the host feeds every
  * aligned camera frame with its odometry pose and LiDAR scan; the mapper selects the keyframes, keeps each image as 8 bits
  * in HBM and builds or extends the map on the GPU.  optimize() stays the caller's call (mapping.cpp:178).
