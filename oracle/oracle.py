@@ -129,6 +129,30 @@ class Oracle:
             _ptr(o["dL_ddc"]), _ptr(o["dL_dsh"]), _ptr(o["dL_dscales"]), _ptr(o["dL_drots"]), _ptr(o["dL_dconic"]))
         return o
 
+    def preprocess_backward(self, g, cam, radii, clamped, dL_dmeans2D, dL_dconic, dL_dcolors, scale_modifier=1.0,
+                            lambda_erank=0.0):
+        """The per-Gaussian backward alone (A.7 + A.8) on given 2-D gradients: dL_dmeans2D [P,>=2], dL_dconic [P,3]
+        (xx, xy, yy), dL_dcolors [P,3], with the forward's radii [P] and clamp bits clamped [P,3].  g as for forward()
+        (an empty sh: no colour backward).  Returns dL_dmeans3D, dL_dcov3D, dL_ddc, dL_dsh, dL_dscales, dL_drots."""
+        P = int(np.asarray(g["means"]).shape[0])
+        M = int(g["sh"].shape[1]) if g["sh"].size else 0
+        a = {k: self._a(g[k]) for k in ("means", "scales", "rots", "dc", "sh")}
+        view, proj, campos, lims = (self._a(cam[k]) for k in ("view", "proj", "campos", "lims"))
+        o = dict(dL_dmeans3D=np.zeros((P, 3), self.dtype), dL_dcov3D=np.zeros((P, 6), self.dtype),
+                 dL_ddc=np.zeros((P, 3), self.dtype), dL_dsh=np.zeros((P, M, 3), self.dtype),
+                 dL_dscales=np.zeros((P, 3), self.dtype), dL_drots=np.zeros((P, 4), self.dtype))
+        r = np.ascontiguousarray(np.asarray(radii).reshape(-1)[:P], np.int32)
+        cl = np.ascontiguousarray(np.asarray(clamped).reshape(P, 3), np.uint8)
+        dm2 = self._a(np.asarray(dL_dmeans2D).reshape(P, -1)[:, :2])
+        dco, dcol = self._a(dL_dconic, (P, 3)), self._a(dL_dcolors, (P, 3))
+        self.lib.glic_oracle_preprocess_backward(
+            C.c_int(P), C.c_int(int(g["degree"])), C.c_int(M), _ptr(a["means"]), _ptr(a["scales"]), self.real(scale_modifier),
+            _ptr(a["rots"]), _ptr(a["dc"]), _ptr(a["sh"]) if M else None, _ptr(view), _ptr(proj), _ptr(campos),
+            C.c_int(cam["W"]), C.c_int(cam["H"]), self.real(cam["tanfovx"]), self.real(cam["tanfovy"]), _ptr(lims), _ptr(r),
+            _ptr(cl), _ptr(dm2), _ptr(dco), _ptr(dcol), self.real(lambda_erank), _ptr(o["dL_dmeans3D"]), _ptr(o["dL_dcov3D"]),
+            _ptr(o["dL_ddc"]), _ptr(o["dL_dsh"]), _ptr(o["dL_dscales"]), _ptr(o["dL_drots"]))
+        return o
+
     def free(self, fwd):
         if fwd.get("state"):
             self.lib.glic_oracle_state_free(C.c_void_p(fwd["state"]))

@@ -92,6 +92,25 @@ class Mag:
     def mean(self, axis=None):
         return Mag(self.v.mean(axis), self.m.mean(axis))
 
+    # The functions below carry the argument's magnitude through to first order and add their own error, counted in
+    # units of their result so that m >= |v| holds after them as it does after the operators above.
+    def sqrt(self):
+        """sqrtf is correctly rounded: d sqrt(x) = dx / (2 sqrt x), plus half the result for its own rounding"""
+        r = np.sqrt(self.v)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            m = np.where(r > 0.0, self.m / (2.0 * r), 0.0)
+        return Mag(r, m + 0.5 * np.abs(r))
+
+    def exp(self, ulps=2.0):
+        """expf is not correctly rounded (CUDA: at most 2 ulp): |e^x| dx, plus `ulps` units of the result"""
+        r = np.exp(self.v)
+        return Mag(r, np.abs(r) * self.m + ulps * np.abs(r))
+
+    def log(self, ulps=2.0):
+        """logf is not correctly rounded (CUDA: at most 1 ulp): dx / |x|, plus `ulps` units of the result"""
+        r = np.log(self.v)
+        return Mag(r, self.m / np.abs(self.v) + ulps * np.abs(r))
+
 
 def conv_array(a):
     """11x11 separable Gaussian over the last two axes, zero padding"""

@@ -74,8 +74,10 @@ def f32_formula_unstable(b32, b64):
     result ~ 1) cancels catastrophically: measured on the needle scene, the f32 oracle misses the f64 dL_dmeans3D by 2e-2
     (identity pose) to 10 (rig view 3) times the tensor's scale, and the CUDA path by as much with its own rounding; dL_dcov3D,
     dL_dscales and dL_drots inherit the same cancellation.  Neither f32 evaluation can pin the other there, so those four are
-    not compared on this scene; the 2-D gradients (where the render kernels and the hy fallback act), opacity and colour
-    gradients still are."""
+    not compared with the f32 oracle on this scene; the 2-D gradients (where the render kernels and the hy fallback act),
+    opacity and colour gradients still are.  test_gpu_preprocess_backward_exact.py pins those four at every row instead:
+    against a float64 restatement fed the kernel's own 2-D gradients, each element within a bound that grows exactly as
+    far as the f32 cancellation can go."""
     a, r = b32["dL_dmeans3D"].astype(np.float64), b64["dL_dmeans3D"].astype(np.float64)
     return np.abs(a - r).max() > GRAD_RTOL * np.abs(r).max()
 
