@@ -153,6 +153,35 @@ class Oracle:
             _ptr(o["dL_ddc"]), _ptr(o["dL_dsh"]), _ptr(o["dL_dscales"]), _ptr(o["dL_drots"]))
         return o
 
+    def render(self, W, H, ranges, point_list, xy, conic_opacity, rgb):
+        """The render forward alone (A.5) on a given state: ranges [T,2], point_list [R], xy [P,2], conic_opacity [P,4],
+        rgb [P,3].  Returns color [3,H,W], final_T [H,W], n_contrib [H*W], max_contrib [T]."""
+        T = ((W + 15) // 16) * ((H + 15) // 16)
+        rg = np.ascontiguousarray(np.asarray(ranges).reshape(T, 2), np.uint32)
+        pl = np.ascontiguousarray(point_list, np.uint32)
+        xy, co, rgb = self._a(xy), self._a(conic_opacity), self._a(rgb)
+        color, final_T = np.zeros((3, H, W), self.dtype), np.zeros((H, W), self.dtype)
+        n_contrib, max_contrib = np.zeros(H * W, np.uint32), np.zeros(T, np.uint32)
+        self.lib.glic_oracle_render(C.c_int(W), C.c_int(H), _ptr(rg), _ptr(pl), _ptr(xy), _ptr(co), _ptr(rgb), None, C.c_int(0),
+                                    _ptr(color), _ptr(final_T), _ptr(n_contrib), _ptr(max_contrib), None, None)
+        return color, final_T, n_contrib, max_contrib
+
+    def render_backward(self, W, H, ranges, point_list, xy, conic_opacity, rgb, n_contrib, color, dL_dpix):
+        """The render backward alone (A.6) on a given state and the forward's n_contrib [H*W] and color [3,H,W].  Returns the
+        2-D gradients dmean2D [P,2] (NDC-scaled), dconic [P,3] (x, y, w), dopacity [P], dcolor [P,3]."""
+        T = ((W + 15) // 16) * ((H + 15) // 16)
+        rg = np.ascontiguousarray(np.asarray(ranges).reshape(T, 2), np.uint32)
+        pl = np.ascontiguousarray(point_list, np.uint32)
+        nc = np.ascontiguousarray(np.asarray(n_contrib).reshape(-1), np.uint32)
+        xy, co, rgb, col, g = (self._a(a) for a in (xy, conic_opacity, rgb, color, dL_dpix))
+        P = xy.shape[0]
+        o = dict(dmean2D=np.zeros((P, 2), self.dtype), dconic=np.zeros((P, 3), self.dtype), dopacity=np.zeros(P, self.dtype),
+                 dcolor=np.zeros((P, 3), self.dtype))
+        self.lib.glic_oracle_render_backward(C.c_int(P), C.c_int(W), C.c_int(H), _ptr(rg), _ptr(pl), _ptr(xy), _ptr(co), _ptr(rgb),
+                                             _ptr(nc), _ptr(col), _ptr(g), _ptr(o["dmean2D"]), _ptr(o["dconic"]),
+                                             _ptr(o["dopacity"]), _ptr(o["dcolor"]))
+        return o
+
     def free(self, fwd):
         if fwd.get("state"):
             self.lib.glic_oracle_state_free(C.c_void_p(fwd["state"]))

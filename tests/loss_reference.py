@@ -111,6 +111,26 @@ class Mag:
         r = np.log(self.v)
         return Mag(r, self.m / np.abs(self.v) + ulps * np.abs(r))
 
+    def rcp(self, ulps=1.0):
+        """1 / x by an approximate reciprocal (rcp.approx.f32: at most 1 ulp): dx / x^2, plus `ulps` units of the result"""
+        r = 1.0 / self.v
+        return Mag(r, self.m * r * r + ulps * np.abs(r))
+
+    def fma(self, b, c):
+        """fmaf(self, b, c): the exact product and sum, rounded once"""
+        return self * b + c
+
+    def minimum(self, o):
+        """fminf: the smaller value, with the larger of the two magnitudes (the operands may be within rounding of each other,
+        so the float32 evaluation may select either)"""
+        o = Mag.of(o)
+        return Mag(np.minimum(self.v, o.v), np.maximum(self.m, o.m))
+
+    @staticmethod
+    def where(cond, a, b):
+        a, b = Mag.of(a), Mag.of(b)
+        return Mag(np.where(cond, a.v, b.v), np.where(cond, a.m, b.m))
+
 
 def conv_array(a):
     """11x11 separable Gaussian over the last two axes, zero padding"""

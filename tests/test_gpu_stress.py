@@ -7,6 +7,10 @@ frames from 1 x 1 to the largest the library accepts, GLIC_MAX_TILES = 65 536 ti
 
 The backward of every stress case runs a second time in a subprocess with GLIC_BWD_RP=4 (two warps per tile): the
 variant is read once per process.
+
+The tensor-scale tolerances here absorb errors confined to a few pixels or pairs.  test_gpu_render_blend_exact.py pins the
+same scenes per element: colour, T and n_contrib at every pixel, and the 2-D gradients per (Gaussian, tile) entry and per
+Gaussian for every backward form, against a float64 restatement that walks every pair without the row cull.
 """
 import os
 import subprocess
