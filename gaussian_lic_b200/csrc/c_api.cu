@@ -63,8 +63,21 @@ __global__ void debug_geom_kernel(int P, GeomState g, float* depth, float* xy, f
     if (clamped) { const unsigned c = g.clamped[i]; clamped[3 * i] = c & 1u; clamped[3 * i + 1] = (c >> 1) & 1u; clamped[3 * i + 2] = (c >> 2) & 1u; }
 }
 
+struct ZeroSpans {
+    static constexpr int MAX = 5;
+    uint32_t* p[MAX];
+    size_t words[MAX];
+};
+
 __global__ void __launch_bounds__(256) fill_kernel(size_t n, float v, float* __restrict__ out) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) out[i] = v;
+}
+
+__global__ void __launch_bounds__(256) zero_spans_kernel(ZeroSpans z) {
+    pdl_enter();
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    for (int k = 0; k < ZeroSpans::MAX; ++k)
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < z.words[k]; i += stride) z.p[k][i] = 0u;
 }
 
 __global__ void debug_keys_kernel(long long R, GeomState g, const uint32_t* tile_keys, const uint32_t* point_list, uint64_t* out) {
@@ -89,12 +102,33 @@ __global__ void debug_det_entries_kernel(unsigned n, uint32_t P, const uint32_t*
     atomicAdd(n_valid, 1u);
 }
 
+int launch_zero_spans(std::initializer_list<ZeroSpan> spans, cudaStream_t s) {
+    if (spans.size() > (size_t)ZeroSpans::MAX) { set_error("zero_spans: too many spans"); return GLIC_ERR_INVALID_ARGUMENT; }
+    ZeroSpans z = {};
+    size_t most = 0;
+    int k = 0;
+    for (const ZeroSpan& sp : spans) {
+        z.p[k] = static_cast<uint32_t*>(sp.p);
+        z.words[k] = sp.bytes / sizeof(uint32_t);
+        most = std::max(most, z.words[k++]);
+    }
+    if (most == 0) return GLIC_OK;
+    GLIC_LAUNCH_PDL(zero_spans_kernel, (unsigned)std::min<size_t>((most + 255) / 256, (size_t)NUM_SMS * 8), 256, 0, s, z);
+    return GLIC_OK;
+}
+
 // The stages of glic_forward and glic_render up to the blend, on workspaces carved for `cap` pairs: preprocess, depth sort and scan,
 // key emission, tile sort, tile ranges and, with `buckets`, the bucket offsets of the checkpoints.  Returns the ping-pong half that
 // holds the sorted list, < 0 on error.
 int bin_view(int P, int sh_degree, int M, const float* means3D, const float* scales, float scale_modifier, const float* rotations,
              const float* opacities, const float* dc, const float* sh, const ViewParams& vp, bool no_color, int* radii, GeomState g,
              BinningState bin, ImageState img, int64_t cap, bool buckets, cudaStream_t s) {
+    const int T = vp.grid_x * vp.grid_y, bit = tile_sort_bits(T);
+    // every word the binning counts into or reads as empty, in one launch: the geometry header, the look-back status words,
+    // both sorts' histograms, tickets and status words, and the tile ranges
+    if (int e = launch_zero_spans({{g.hdr, sizeof(GeomHeader)}, {g.scan_status, GeomState::scan_status_bytes(P)},
+                                   {g.sort_temp, sort_prepare_bytes(P, 32)}, {bin.sort_temp, sort_prepare_bytes(cap, bit)},
+                                   {img.ranges, sizeof(uint2) * (size_t)T}}, s)) return e;
     { StageTimer _t(GLIC_STAGE_PREPROCESS, s);
       if (int e = launch_preprocess_forward(P, sh_degree, M, means3D, scales, scale_modifier, rotations, opacities, dc, sh, vp,
                                             no_color, radii, g, s)) return e; }
@@ -102,18 +136,14 @@ int bin_view(int P, int sh_degree, int M, const float* means3D, const float* sca
       const int cur0 = launch_sort_pairs32(P, 32, g.depth_keys, g.order, g.sort_temp, g.sort_temp_size, s, nullptr, /*hist_ready=*/true);
       if (cur0 < 0) return cur0;
       if (int e = launch_depth_scan(P, g, g.order[cur0], cap, s)) return e; }
-    const int bit = tile_sort_bits(vp.grid_x * vp.grid_y);
     { StageTimer _t(GLIC_STAGE_EMIT, s);
-      if (int e = sort_prepare(cap, bit, bin.sort_temp, s)) return e;        // emit builds the tile sort's digit histograms
       if (int e = launch_emit_keys(P, vp, g, bin.keys[0], bin.vals[0], cap, sort_hist(bin.sort_temp), bit, s)) return e; }
     int cur;
     { StageTimer _t(GLIC_STAGE_SORT, s);
       cur = launch_sort_pairs32(cap, bit, bin.keys, bin.vals, bin.sort_temp, bin.sort_temp_size, s, &g.hdr->r_eff, true);
       if (cur < 0) return cur; }
-    GLIC_CUDA_TRY(cudaMemsetAsync(&bin.hdr->sorted_in_b, cur, 1, s));       // 0/1 in the low byte (header is zero-padded)
-    GLIC_CUDA_TRY(cudaMemsetAsync(reinterpret_cast<char*>(&bin.hdr->sorted_in_b) + 1, 0, 3, s));
     { StageTimer _t(GLIC_STAGE_RANGES, s);
-      if (int e = launch_tile_ranges(cap, g.hdr, bin.keys[cur], vp.grid_x * vp.grid_y, img, buckets, s)) return e; }
+      if (int e = launch_tile_ranges(cap, g.hdr, bin.keys[cur], T, img, buckets, &bin.hdr->sorted_in_b, cur, s)) return e; }
     return cur;
 }
 
@@ -180,6 +210,8 @@ int glic_forward_preprocess(int P, int sh_degree, int M, const float* means3D, c
     cudaStream_t s = (cudaStream_t)stream;
     GeomState g = GeomState::carve(geom_ws, P);
     const ViewParams vp = make_view_params(view);
+    if (int e = launch_zero_spans({{g.hdr, sizeof(GeomHeader)}, {g.scan_status, GeomState::scan_status_bytes(P)},
+                                   {g.sort_temp, sort_prepare_bytes(P, 32)}}, s)) return e;
     { StageTimer _t(GLIC_STAGE_PREPROCESS, s);
     if (int e = launch_preprocess_forward(P, sh_degree, M, means3D, scales, scale_modifier, rotations, opacities, dc, sh, vp,
                                           no_color != 0, radii, g, s)) return e; }
@@ -251,9 +283,9 @@ int glic_forward_render(int P, const glic_view* view, int no_color, int64_t R, v
         { StageTimer _t(GLIC_STAGE_SORT, s); cur = launch_sort_pairs32(R, bit, bin.keys, bin.vals, bin.sort_temp, bin.sort_temp_size, s, nullptr, true); }
         if (cur < 0) return cur;
     }
-    GLIC_CUDA_TRY(cudaMemsetAsync(&bin.hdr->sorted_in_b, cur, 1, s));       // 0/1 in the low byte (header is zero-padded)
-    GLIC_CUDA_TRY(cudaMemsetAsync(reinterpret_cast<char*>(&bin.hdr->sorted_in_b) + 1, 0, 3, s));
-    { StageTimer _t(GLIC_STAGE_RANGES, s); if (int e = launch_tile_ranges(R, nullptr, bin.keys[cur], T, img, !no_color, s)) return e; }
+    GLIC_CUDA_TRY(cudaMemsetAsync(img.ranges, 0, sizeof(uint2) * (size_t)T, s));
+    { StageTimer _t(GLIC_STAGE_RANGES, s);
+      if (int e = launch_tile_ranges(R, nullptr, bin.keys[cur], T, img, !no_color, &bin.hdr->sorted_in_b, cur, s)) return e; }
     { StageTimer _t(GLIC_STAGE_RENDER_FWD, s); if (int e = launch_render_forward(vp, no_color != 0, bin.vals[cur], g, img, smp, out_color, out_final_T, s)) return e; }
     if (num_buckets_host) {
         unsigned int nb = 0;
@@ -485,7 +517,7 @@ int glic_backward_compact_internal(int P, int sh_degree, int M, const float* mea
     const ViewParams vp = make_view_params(view);
     GeomState g = GeomState::carve(const_cast<void*>(geom_ws), P);
     ImageState img = ImageState::carve(const_cast<void*>(image_ws), vp.W, vp.H);
-    { StageTimer _t(GLIC_STAGE_ZERO, s);
+    if (!cg->grads_zeroed) { StageTimer _t(GLIC_STAGE_ZERO, s);
     // conic | mean2D | opacity carved from ONE block (the mapper's capacity layout): one memset over the span when the slack
     // between the live prefixes is small, three otherwise
     const ptrdiff_t span = dL_dconic < dL_dmeans2D && dL_dmeans2D < dL_dopacity ? (dL_dopacity + P) - dL_dconic : -1;

@@ -14,6 +14,8 @@
 #include <stdint.h>
 #include <stddef.h>
 #include <string>
+#include <initializer_list>
+#include <utility>
 
 #include "../../include/glic_b200.h"
 
@@ -59,6 +61,42 @@ extern unsigned long long g_launches;
     do {                                                                                      \
         ++glic::g_launches;                                                                   \
         cudaError_t _e = cudaGetLastError();                                                  \
+        if (_e != cudaSuccess) {                                                              \
+            glic::set_error(std::string("kernel launch: ") + cudaGetErrorString(_e));       \
+            return GLIC_ERR_CUDA;                                                             \
+        }                                                                                     \
+    } while (0)
+
+// ---- programmatic dependent launch (PDL) ------------------------------------------------
+// A kernel launched by GLIC_LAUNCH_PDL may start while the stream's previous kernel is still running.  Every such kernel
+// calls pdl_enter() before anything else: it lets the stream's next kernel launch (that kernel cannot run ahead, it waits
+// the same way), then waits for the previous kernel to complete and its writes to be visible.  Only kernels that call
+// pdl_enter() on every path may be launched this way.  Launched without the attribute, both instructions do nothing.
+__device__ __forceinline__ void pdl_enter() {
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+}
+
+template <typename... KArgs, typename... Args>
+cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = s;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+}
+
+// launch_pdl(kernel, grid, block, smem, stream, args...), counted and checked like GLIC_LAUNCH_CHECK
+#define GLIC_LAUNCH_PDL(...)                                                                  \
+    do {                                                                                      \
+        ++glic::g_launches;                                                                   \
+        cudaError_t _e = glic::launch_pdl(__VA_ARGS__);                                       \
         if (_e != cudaSuccess) {                                                              \
             glic::set_error(std::string("kernel launch: ") + cudaGetErrorString(_e));       \
             return GLIC_ERR_CUDA;                                                             \
@@ -141,6 +179,8 @@ struct GeomState {
         if (bytes) *bytes = c.total();
         return g;
     }
+    // the look-back status words preprocess_forward_kernel's P / PRE_THREADS CTAs use (zeroed before it runs)
+    __host__ static size_t scan_status_bytes(int P) { return sizeof(unsigned long long) * ((P + PRE_THREADS - 1) / PRE_THREADS + 1); }
 };
 
 // Function attributes (opt-in dynamic shared memory) are per device: run `fn` once per (call site, device).
@@ -333,6 +373,9 @@ struct CompactGrads {
     // like the geometric gradients: |(dL/dmean2D.x, .y)| and 1 for a visible row, 0 and 0 for a culled one
     float* dens_norm;         // [P]
     float* dens_count;        // [P]
+    // 1: the render backward's accumulators (dL_dmeans2D, dL_dconic, dL_dopacity, dL_dcolors) are zero in rows [0, P) already
+    // (launch_view_flags zeroed them), so glic_backward_compact_internal does not
+    int grads_zeroed = 0;
 };
 // doubles of the pose-gradient scratch for up to Pcap Gaussians
 size_t pose_partials_count(uint32_t Pcap);
@@ -351,6 +394,12 @@ partials_finish_kernel(unsigned G, const double* __restrict__ partials, float* _
 }
 
 // ---- stage launchers (defined in the .cu files) ------------------------------------------
+// One launch that zeroes up to five spans (bytes a multiple of 4): a chain of dependent launches continues through it, where a
+// memset would end it
+struct ZeroSpan { void* p; size_t bytes; };
+int launch_zero_spans(std::initializer_list<ZeroSpan> spans, cudaStream_t s);
+// The caller zeroes g.hdr, the look-back status words (scan_status_bytes) and the depth sort's temp block
+// (sort_prepare_bytes(P, 32)) first: the kernel counts into all three
 int launch_preprocess_forward(int P, int D, int M, const float* means, const float* scales, float mod,
                               const float* rots, const float* opac, const float* dc, const float* sh,
                               const ViewParams& vp, bool no_color, int* radii, GeomState g, cudaStream_t s);
@@ -367,10 +416,11 @@ int launch_sort_pairs32(int64_t n, int end_bit, uint32_t* keys[2], uint32_t* val
 // per key and pass into sort_hist(temp)[pass * 256 + digit] (digit = bits [sort_pass_shift, + sort_pass_bits) of the key),
 // and the sort is launched with hist_ready = true.
 int sort_prepare(int64_t n, int end_bit, void* temp, cudaStream_t s, int digit_bits = 8);
+size_t sort_prepare_bytes(int64_t n, int end_bit, int digit_bits = 8);     // the bytes sort_prepare zeroes
 uint32_t* sort_hist(void* temp);
-// R: host-side count or capacity; r_dev (optional): device-side true count
+// R: host-side count or capacity; r_dev (optional): device-side true count.  img.ranges must be zero; *sorted_in_b is set to cur
 int launch_tile_ranges(int64_t R, const GeomHeader* ghdr, const uint32_t* tile_keys_sorted, int T, ImageState img, bool buckets,
-                       cudaStream_t s);
+                       unsigned int* sorted_in_b, int cur, cudaStream_t s);
 int launch_render_forward(const ViewParams& vp, bool no_color, const uint32_t* point_list, GeomState g, ImageState img,
                           SampleState smp, float* out_color, float* out_final_T, cudaStream_t s);
 // the inference form of the blend (glic_render): colour, final T and, when non-null, expected and median depth; nothing else
@@ -423,7 +473,13 @@ int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, 
 // radii (with g_dens): [n_slots][Pcap_geo] each slot's screen radii; dens_maxr takes their max over the slots that see the row
 // campos_dev: n_slots host-held device pointers, each slot's camera centre (read on the device)
 // radii_out (optional): the view's radii copied next to its flags (the densification's screen-radius slot)
-int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flags, cudaStream_t s, int* radii_out = nullptr);
+// what one view's loss and render backward accumulate into: the loss word and the per-Gaussian rows (conic [P,4], 16-byte aligned)
+struct ViewZero { float *conic, *mean2D, *opacity, *colors, *loss; };
+int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flags, cudaStream_t s, int* radii_out, float* overflow_word,
+                      const ViewZero& z);
+// glic_activations_forward with zero4[0..3] (optional) zeroed by the same kernel
+int launch_activations_forward(int P, const float* opacity_logit, const float* log_scale, const float* rot_raw, float* opacity,
+                               float* scale, float* rot, float* zero4, cudaStream_t stream);
 // per-keyframe exposure (ssim.cu): one Adam step of every keyframe of a batch of S <= EXPO_MAX_SLOTS slots; slot_grads[S][12]
 constexpr int EXPO_MAX_SLOTS = 32;
 int launch_exposure_adam(int S, const int* kf_of_slot_host, const float* slot_grads, float* E, float* exp_avg, float* exp_avg_sq,
@@ -433,9 +489,10 @@ int launch_exposure_adam(int S, const int* kf_of_slot_host, const float* slot_gr
 int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, const float* E, float* out2, void* scratch,
                    size_t scratch_bytes, void* stream, void* fixed = nullptr);
 // the native mapper's photometric loss: glic_l1_ssim_loss (3 channels) or, with E, glic_l1_ssim_loss_exposure; partials (optional,
-// fixed_order_sums_bytes(H, W)) sums the loss value in a fixed order instead of with float atomics
+// fixed_order_sums_bytes(H, W)) sums the loss value in a fixed order instead of with float atomics; loss_zeroed: *loss is zero
+// already (the float atomics add into it without a memset first)
 int photometric_loss_sum(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E, float* loss, float* dL_dimg,
-                         float* dL_dE, void* scratch, size_t scratch_bytes, void* partials, cudaStream_t s);
+                         float* dL_dE, void* scratch, size_t scratch_bytes, void* partials, cudaStream_t s, bool loss_zeroed = false);
 size_t fixed_order_sums_bytes(int H, int W);
 // out[3][H][W] = img exposed by E (optional) and clamped to [0,1], element for element the image eval_psnr_ssim scores
 int launch_scored_image(int H, int W, const float* img, const float* E, float* out, cudaStream_t s);

@@ -186,6 +186,7 @@ using IpcMapping = Handle<void*, cudaIpcCloseMemHandle>;
 struct Keyframe {                    // move-only: it owns its device camera block
     float R_wc[9], t_wc[3];
     const float* image = nullptr;
+    bool image_on_device = false;    // `image` is memory of the mapper's device: the loss reads it in place
     const uint8_t* bgr = nullptr;    // add_frame keyframes: packed HWC BGR8 in the frame store, decoded where `image` is copied
     CamBlock cam;
     Dev<float> cam_dev;              // view16 | proj16 | campos4
@@ -680,9 +681,10 @@ int poll_ring(glic_mapper* m, bool wait) {
     return GLIC_OK;
 }
 
-int activate(glic_mapper* m) {
+// the activated parameters; zero4[0..3] (optional) zeroed by the same kernel
+int activate(glic_mapper* m, float* zero4 = nullptr) {
     const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
-    return glic_activations_forward((int)m->P, a.opacity, a.log_scale, a.rot, m->act_opacity, m->act_scales, m->act_rots, m->stream);
+    return launch_activations_forward((int)m->P, a.opacity, a.log_scale, a.rot, m->act_opacity, m->act_scales, m->act_rots, zero4, m->stream);
 }
 
 int forward_view(glic_mapper* m, const glic_view& v, int no_color, long long* counters) {
@@ -725,10 +727,12 @@ int load_gt(glic_mapper* m, const Keyframe& kf, float* dst, cudaMemcpyKind kind,
 
 __global__ void overflow_word_kernel(const GeomHeader* ghdr, float* word) { if (ghdr->overflow) *word = 1.0f; }
 
-// the L1 + D-SSIM loss of an H x W image against gt, and its dL/dimg; with E (device, 3x4) the loss of the exposed image, and dL/dE
-int photometric_loss(glic_mapper* m, int H, int W, const float* img, const float* gt, const float* E, float* loss, float* dL_dimg, float* dL_dE) {
+// the L1 + D-SSIM loss of an H x W image against gt, and its dL/dimg; with E (device, 3x4) the loss of the exposed image, and dL/dE;
+// loss_zeroed: *loss is zero already
+int photometric_loss(glic_mapper* m, int H, int W, const float* img, const float* gt, const float* E, float* loss, float* dL_dimg, float* dL_dE,
+                     bool loss_zeroed = false) {
     return photometric_loss_sum(H, W, m->cfg.lambda_dssim, img, gt, E, loss, dL_dimg, dL_dE, m->loss_scratch, m->loss_scratch.bytes(),
-                                m->deterministic ? m->det_sums.raw() : nullptr, m->stream);
+                                m->deterministic ? m->det_sums.raw() : nullptr, m->stream, loss_zeroed);
 }
 
 // the backward of the last forward_view of v from dL_dpix: colour gradients into col, after_render (optional) recorded, then cg's
@@ -754,40 +758,40 @@ int iteration(glic_mapper* m, const int* views) {
     float* geo = geo_ptr(m);
     const ArenaRows a = arena_rows(m->params, m->Pcap, m->M), ga = arena_rows(geo, m->Pcap, 0);
     float* geo_tail = geo + (size_t)11 * m->Pcap;
-    GLIC_CUDA_TRY(cudaMemsetAsync(geo_tail, 0, 4 * sizeof(float), s));
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->loss_dev, 0, sizeof(float) * 2, s));
-    MAP_TRY(activate(m));
+    MAP_TRY(activate(m, geo_tail));
     for (int j = 0; j < m->k; ++j) {
         const int sl = m->cfg.rank * m->k + j;
         const Keyframe& kf = m->train[views[sl]];
-        const int buf = (int)(m->view_counter++ & 1);
         // keyframe image H2D (gaussian.cpp:678), or the 8-bit frame's decode, on the copy stream, overlapping the previous
-        // view's backward / Adam
-        GLIC_CUDA_TRY(cudaStreamWaitEvent(m->copy_stream, m->gt_free[buf], 0));
-        MAP_TRY(load_gt(m, kf, m->gt_dev[buf], cudaMemcpyDefault, m->copy_stream));
-        GLIC_CUDA_TRY(cudaEventRecord(m->gt_ready[buf], m->copy_stream));
+        // view's backward / Adam; an image already in device memory is read where it is
+        const int buf = kf.image_on_device ? -1 : (int)(m->view_counter++ & 1);
+        if (buf >= 0) {
+            GLIC_CUDA_TRY(cudaStreamWaitEvent(m->copy_stream, m->gt_free[buf], 0));
+            MAP_TRY(load_gt(m, kf, m->gt_dev[buf], cudaMemcpyDefault, m->copy_stream));
+            GLIC_CUDA_TRY(cudaEventRecord(m->gt_ready[buf], m->copy_stream));
+        }
         MAP_TRY(forward_view(m, kf.view, 0, j == m->k - 1 ? m->counters_host + 4 * r : nullptr));
         uint8_t* fl = slot<uint8_t>(m, FLAGS, parity, sl);
         float* col = slot(m, COLOUR, parity, sl);
         int* rad = m->dens_on ? slot<int>(m, RADII, parity, sl) : nullptr;           // this view's radii for the screen-size statistic
-        MAP_TRY(launch_view_flags((int)m->P, m->radii, GeomState::carve(m->geom_ws, (int)m->P), fl, s, rad));
-        overflow_word_kernel<<<1, 1, 0, s>>>(GeomState::carve(m->geom_ws, (int)m->P).hdr, geo_tail);
-        GLIC_LAUNCH_CHECK();
+        MAP_TRY(launch_view_flags((int)m->P, m->radii, GeomState::carve(m->geom_ws, (int)m->P), fl, s, rad, geo_tail,
+                                  ViewZero{m->g_conic, m->g_mean2D, m->g_opacity, col, m->loss_dev + 1}));
         if (m->cfg.world > 1) {
             GLIC_CUDA_TRY(cudaEventRecord(m->ev_flags, s));
             GLIC_CUDA_TRY(cudaStreamWaitEvent(m->push_stream, m->ev_flags, 0));
             MAP_TRY(push_to_peers(m, fl, m->P));
             if (rad) MAP_TRY(push_to_peers(m, rad, sizeof(int) * (size_t)m->P));
         }
-        GLIC_CUDA_TRY(cudaStreamWaitEvent(s, m->gt_ready[buf], 0));
+        if (buf >= 0) GLIC_CUDA_TRY(cudaStreamWaitEvent(s, m->gt_ready[buf], 0));
         // loss of this view (the pinned ring keeps the last local view's value for the statistics)
-        MAP_TRY(photometric_loss(m, H, W, m->color, m->gt_dev[buf], m->expo_on ? m->expo_E + 12 * (size_t)views[sl] : nullptr, m->loss_dev + 1,
-                                 m->dL_dpix, slot(m, EXPOSURE, parity, sl)));
-        GLIC_CUDA_TRY(cudaEventRecord(m->gt_free[buf], s));
+        MAP_TRY(photometric_loss(m, H, W, m->color, buf >= 0 ? m->gt_dev[buf] : kf.image, m->expo_on ? m->expo_E + 12 * (size_t)views[sl] : nullptr,
+                                 m->loss_dev + 1, m->dL_dpix, slot(m, EXPOSURE, parity, sl), /*loss_zeroed=*/true));
+        if (buf >= 0) GLIC_CUDA_TRY(cudaEventRecord(m->gt_free[buf], s));
         CompactGrads cg;
         cg.g_rot = reinterpret_cast<float4*>(ga.rot); cg.g_xyz = ga.xyz; cg.g_scale = ga.log_scale; cg.g_opacity = ga.opacity;
         cg.opacity = m->act_opacity; cg.dL_dopacity = m->g_opacity; cg.rot_raw = reinterpret_cast<const float4*>(a.rot);
         cg.accumulate = j > 0;
+        cg.grads_zeroed = 1;
         cg.pose_partials = m->pose_on ? (double*)m->pose_part : nullptr;        // this view's dL/d(rho, omega), fused into the backward
         cg.pose_grad = m->pose_on ? slot(m, POSE, parity, sl) : nullptr;
         cg.dens_norm = m->dens_on ? geo_tail + 4 : nullptr;                        // this view's statistics, summed over the rank's views
@@ -1017,6 +1021,13 @@ int make_keyframe(glic_mapper* m, const float* R_wc, const float* t_wc, const fl
     std::memcpy(kf.R_wc, R_wc, sizeof(kf.R_wc)); std::memcpy(kf.t_wc, t_wc, sizeof(kf.t_wc));
     kf.image = image;
     kf.bgr = bgr;
+    if (image) {
+        cudaPointerAttributes pa = {};
+        int dev = 0;
+        GLIC_CUDA_TRY(cudaPointerGetAttributes(&pa, image));
+        GLIC_CUDA_TRY(cudaGetDevice(&dev));
+        kf.image_on_device = pa.type == cudaMemoryTypeDevice && pa.device == dev;
+    }
     config_camera_block(m, kf.R_wc, kf.t_wc, kf.cam);
     MAP_TRY(kf.cam_dev.allocate(36 * sizeof(float)));
     // view | proj | campos are contiguous; ordered before every use of the block, all of which are on the mapper's stream or after

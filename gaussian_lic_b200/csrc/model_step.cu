@@ -19,12 +19,15 @@ namespace {
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-// torch::sigmoid / torch::exp / torch::nn::functional::normalize (p = 2, eps = 1e-12) of the raw parameters
+// torch::sigmoid / torch::exp / torch::nn::functional::normalize (p = 2, eps = 1e-12) of the raw parameters; zero4 (optional) is
+// zeroed on the way: the mapper's step starts here, and a memset would end its chain of dependent launches
 __global__ void __launch_bounds__(256)
 activations_forward_kernel(int P, const float* __restrict__ opacity_logit, const float* __restrict__ log_scale,
                            const float4* __restrict__ rot_raw, float* __restrict__ opacity, float* __restrict__ scale,
-                           float4* __restrict__ rot) {
+                           float4* __restrict__ rot, float* __restrict__ zero4) {
+    pdl_enter();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (zero4 && i < 4) zero4[i] = 0.0f;
     if (i >= P) return;
     opacity[i] = opacity_activation(opacity_logit[i]);
 #pragma unroll
@@ -250,6 +253,18 @@ arena_append_kernel(uint32_t P, uint32_t n, int K, ArenaLayout L, float* __restr
 }
 
 }  // namespace
+
+int launch_activations_forward(int P, const float* opacity_logit, const float* log_scale, const float* rot_raw, float* opacity,
+                               float* scale, float* rot, float* zero4, cudaStream_t stream) {
+    if (P < 0) { set_error("activations_forward: bad P"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (P == 0) return GLIC_OK;
+    if (!opacity_logit || !log_scale || !rot_raw || !opacity || !scale || !rot) { set_error("activations_forward: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!aligned16(rot_raw) || !aligned16(rot)) { set_error("activations_forward: rotations must be 16-byte aligned"); return GLIC_ERR_INVALID_ARGUMENT; }
+    StageTimer _t(GLIC_STAGE_ADAM, stream);
+    GLIC_LAUNCH_PDL(activations_forward_kernel, (P + 255) / 256, 256, 0, stream, P, opacity_logit, log_scale,
+                    reinterpret_cast<const float4*>(rot_raw), opacity, scale, reinterpret_cast<float4*>(rot), zero4);
+    return GLIC_OK;
+}
 }  // namespace glic
 
 using namespace glic;
@@ -268,15 +283,7 @@ int glic_packed_offsets(uint32_t P, uint32_t M, size_t* offsets6) {
 
 int glic_activations_forward(int P, const float* opacity_logit, const float* log_scale, const float* rot_raw, float* opacity,
                              float* scale, float* rot, void* stream) {
-    if (P < 0) { set_error("activations_forward: bad P"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (P == 0) return GLIC_OK;
-    if (!opacity_logit || !log_scale || !rot_raw || !opacity || !scale || !rot) { set_error("activations_forward: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!aligned16(rot_raw) || !aligned16(rot)) { set_error("activations_forward: rotations must be 16-byte aligned"); return GLIC_ERR_INVALID_ARGUMENT; }
-    StageTimer _t(GLIC_STAGE_ADAM, (cudaStream_t)stream);
-    activations_forward_kernel<<<(P + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
-        P, opacity_logit, log_scale, reinterpret_cast<const float4*>(rot_raw), opacity, scale, reinterpret_cast<float4*>(rot));
-    GLIC_LAUNCH_CHECK();
-    return GLIC_OK;
+    return glic::launch_activations_forward(P, opacity_logit, log_scale, rot_raw, opacity, scale, rot, nullptr, (cudaStream_t)stream);
 }
 
 int glic_activations_backward(int P, const float* opacity, const float* scale, const float* rot_raw, float* dL_dopacity,
@@ -351,20 +358,30 @@ namespace glic {
 namespace {
 __global__ void __launch_bounds__(256)
 view_flags_kernel(int P, const int* __restrict__ radii, const uint8_t* __restrict__ clamped, uint8_t* __restrict__ flags,
-                  int* __restrict__ radii_out) {
+                  int* __restrict__ radii_out, const GeomHeader* __restrict__ ghdr, float* __restrict__ overflow_word, ViewZero z) {
+    pdl_enter();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i == 0) {
+        if (ghdr->overflow) *overflow_word = 1.0f;
+        *z.loss = 0.0f;
+    }
     if (i >= P) return;
     const int r = radii[i];
     flags[i] = r > 0 ? (uint8_t)(0x80u | (clamped[i] & 7u)) : (uint8_t)0;
     if (radii_out) radii_out[i] = r;
+    reinterpret_cast<float4*>(z.conic)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) { z.mean2D[3 * (size_t)i + c] = 0.0f; z.colors[3 * (size_t)i + c] = 0.0f; }
+    z.opacity[i] = 0.0f;
 }
 }  // namespace
 
-// per-view flags byte of the compact exchange: visibility + the forward's colour-clamp bits
-int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flags, cudaStream_t s, int* radii_out) {
+// per-view flags byte of the compact exchange: visibility + the forward's colour-clamp bits; also sets *overflow_word to 1 when the
+// forward overflowed its binning workspace, and zeroes what the view's loss and backward accumulate into (z)
+int launch_view_flags(int P, const int* radii, const GeomState& g, uint8_t* flags, cudaStream_t s, int* radii_out, float* overflow_word,
+                      const ViewZero& z) {
     if (P <= 0) return GLIC_OK;
-    view_flags_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, radii, g.clamped, flags, radii_out);
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(view_flags_kernel, (P + 255) / 256, 256, 0, s, P, radii, g.clamped, flags, radii_out, g.hdr, overflow_word, z);
     return GLIC_OK;
 }
 

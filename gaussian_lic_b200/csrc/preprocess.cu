@@ -377,6 +377,7 @@ preprocess_forward_kernel(int P, int D, int M, const float* __restrict__ means, 
                           float mod, const float4* __restrict__ rots, const float* __restrict__ opac,
                           const float* __restrict__ dc, const float* __restrict__ sh, ViewParams vp, bool no_color,
                           int* __restrict__ radii, GeomState g, uint32_t* __restrict__ depth_hist) {
+    pdl_enter();
     __shared__ float s_view[16], s_proj[16], s_cam[3];
     __shared__ uint32_t s_warp_sum[PRE_THREADS / 32];
     __shared__ uint32_t s_dhist[4 * 256];                   // digit histograms of the depth keys (the P-sized sort's four passes)
@@ -569,6 +570,7 @@ constexpr int SCAN_ITEMS = 4;
 
 __global__ void __launch_bounds__(PRE_THREADS)
 depth_scan_kernel(int P, GeomState g, const uint32_t* __restrict__ order, unsigned int capacity) {
+    pdl_enter();
     __shared__ unsigned s_block;
     __shared__ uint32_t s_warp_sum[PRE_THREADS / 32];
     __shared__ uint32_t s_block_excl;
@@ -629,6 +631,7 @@ depth_scan_kernel(int P, GeomState g, const uint32_t* __restrict__ order, unsign
 __global__ void __launch_bounds__(PRE_THREADS)
 emit_keys_kernel(int P, ViewParams vp, GeomState g, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals, unsigned int capacity,
                  uint32_t* __restrict__ sort_hist, int lo_bits, uint32_t hi_mask) {
+    pdl_enter();
     __shared__ WalkSmem walk;
     __shared__ uint32_t s_hist[2 * 256];
     for (int i = threadIdx.x; i < 2 * 256; i += PRE_THREADS) s_hist[i] = 0;
@@ -669,27 +672,20 @@ int launch_preprocess_forward(int P, int D, int M, const float* means, const flo
                               const float* rots, const float* opac, const float* dc, const float* sh,
                               const ViewParams& vp, bool no_color, int* radii, GeomState g, cudaStream_t s) {
     const int blocks = (P + PRE_THREADS - 1) / PRE_THREADS;
-    // header (ticket/total) and the emit kernel's look-back status words start at zero
-    GLIC_CUDA_TRY(cudaMemsetAsync(g.hdr, 0, sizeof(GeomHeader), s));
-    GLIC_CUDA_TRY(cudaMemsetAsync(g.scan_status, 0, sizeof(unsigned long long) * (blocks + 1), s));
-    if (int e = sort_prepare(P, 32, g.sort_temp, s)) return e;       // the depth sort's histograms are built by this kernel
     const size_t dyn = sizeof(float) * (PRE_THREADS / 32) * 32 * SH_ROW_MAX + sizeof(WalkSmem);
     static bool attr_set[64] = {};
     if (first_use_on_device(attr_set)) {
         GLIC_CUDA_TRY(cudaFuncSetAttribute(preprocess_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
     }
-    preprocess_forward_kernel<<<blocks, PRE_THREADS, dyn, s>>>(P, D, M, means, scales, mod,
-                                                             reinterpret_cast<const float4*>(rots), opac, dc, sh, vp,
-                                                             no_color, radii, g, sort_hist(g.sort_temp));
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(preprocess_forward_kernel, blocks, PRE_THREADS, dyn, s, P, D, M, means, scales, mod,
+                    reinterpret_cast<const float4*>(rots), opac, dc, sh, vp, no_color, radii, g, sort_hist(g.sort_temp));
     return GLIC_OK;
 }
 
 int launch_depth_scan(int P, GeomState g, const uint32_t* order, int64_t capacity, cudaStream_t s) {
     const unsigned int cap = (unsigned int)std::min<int64_t>(capacity, 0xFFFFFFFFll);
     const int per_cta = PRE_THREADS * SCAN_ITEMS;
-    depth_scan_kernel<<<(P + per_cta - 1) / per_cta, PRE_THREADS, 0, s>>>(P, g, order, cap);
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(depth_scan_kernel, (P + per_cta - 1) / per_cta, PRE_THREADS, 0, s, P, g, order, cap);
     return GLIC_OK;
 }
 
@@ -701,9 +697,8 @@ int launch_emit_keys(int P, const ViewParams& vp, GeomState g, uint32_t* tile_ke
     // the sort's digit split: one pass of end_bit bits, or two of sort_pass_bits(end_bit, 0) + sort_pass_bits(end_bit, 1)
     const int lo_bits = sort_pass_bits(end_bit, 0);
     const uint32_t hi_mask = sort_passes(end_bit) > 1 ? (1u << sort_pass_bits(end_bit, 1)) - 1u : 0u;
-    emit_keys_kernel<<<(P + PRE_THREADS - 1) / PRE_THREADS, PRE_THREADS, 0, s>>>(P, vp, g, tile_keys, vals, cap, sort_hist_out, lo_bits,
-                                                                                  hi_mask);
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(emit_keys_kernel, (P + PRE_THREADS - 1) / PRE_THREADS, PRE_THREADS, 0, s, P, vp, g, tile_keys, vals, cap,
+                    sort_hist_out, lo_bits, hi_mask);
     return GLIC_OK;
 }
 

@@ -53,6 +53,7 @@ preprocess_backward_kernel(int P, int D, int M, const float* __restrict__ means,
                            const float* __restrict__ dL_dcolors, float* __restrict__ dL_dmeans3D,
                            float* __restrict__ dL_dcov3D, float* __restrict__ dL_ddc, float* __restrict__ dL_dsh,
                            float* __restrict__ dL_dscales, float4* __restrict__ dL_drots, CompactGrads cg) {
+    pdl_enter();
     __shared__ float s_view[16], s_proj[16], s_cam[3];
     __shared__ __align__(16) float s_sh[PB_THREADS / 32][32 * SH_ROW_MAX];    // SH rows in, dL/dSH rows out
     static_assert(COMPACT || !POSE, "the pose gradient is a compact-form output");
@@ -364,11 +365,10 @@ int launch_preprocess_backward(int P, int D, int M, const float* means, const fl
                                float lambda_erank, const float* dL_dmean2D, const float* dL_dconic,
                                const float* dL_dcolors, float* dL_dmeans3D, float* dL_dcov3D, float* dL_ddc,
                                float* dL_dsh, float* dL_dscales, float* dL_drots, cudaStream_t s) {
-    preprocess_backward_kernel<false><<<(P + PB_THREADS - 1) / PB_THREADS, PB_THREADS, 0, s>>>(
-        P, D, M, means, scales, mod, reinterpret_cast<const float4*>(rots), sh, vp, radii, g.clamped, lambda_erank,
-        dL_dmean2D, dL_dconic, dL_dcolors, dL_dmeans3D, dL_dcov3D, dL_ddc, dL_dsh, dL_dscales,
-        reinterpret_cast<float4*>(dL_drots), CompactGrads{});
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(preprocess_backward_kernel<false>, (P + PB_THREADS - 1) / PB_THREADS, PB_THREADS, 0, s,
+                    P, D, M, means, scales, mod, reinterpret_cast<const float4*>(rots), sh, vp, radii, g.clamped, lambda_erank,
+                    dL_dmean2D, dL_dconic, dL_dcolors, dL_dmeans3D, dL_dcov3D, dL_ddc, dL_dsh, dL_dscales,
+                    reinterpret_cast<float4*>(dL_drots), CompactGrads{});
     return GLIC_OK;
 }
 
@@ -378,18 +378,16 @@ static int launch_compact(int P, int D, int M, const float* means, const float* 
                    const float* dL_dcolors, const CompactGrads& cg, cudaStream_t s) {
     const unsigned blocks = (P + PB_THREADS - 1) / PB_THREADS;
     if (cg.pose_partials) {
-        preprocess_backward_kernel<true, true, DENS, POSE_ONLY><<<blocks, PB_THREADS, 0, s>>>(
-            P, D, M, means, scales, mod, reinterpret_cast<const float4*>(rots), sh, vp, radii, g.clamped, 0.0f,
-            dL_dmean2D, dL_dconic, dL_dcolors, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cg);
-        GLIC_LAUNCH_CHECK();
+        GLIC_LAUNCH_PDL(preprocess_backward_kernel<true, true, DENS, POSE_ONLY>, blocks, PB_THREADS, 0, s,
+                        P, D, M, means, scales, mod, reinterpret_cast<const float4*>(rots), sh, vp, radii, g.clamped, 0.0f,
+                        dL_dmean2D, dL_dconic, dL_dcolors, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cg);
         partials_finish_kernel<6><<<1, 6 * 32, 0, s>>>(blocks, cg.pose_partials, cg.pose_grad);
         GLIC_LAUNCH_CHECK();
         return GLIC_OK;
     }
-    preprocess_backward_kernel<true, false, DENS><<<(P + PB_THREADS - 1) / PB_THREADS, PB_THREADS, 0, s>>>(
-        P, D, M, means, scales, mod, reinterpret_cast<const float4*>(rots), sh, vp, radii, g.clamped, 0.0f,
-        dL_dmean2D, dL_dconic, dL_dcolors, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cg);
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(preprocess_backward_kernel<true, false, DENS>, (P + PB_THREADS - 1) / PB_THREADS, PB_THREADS, 0, s,
+                    P, D, M, means, scales, mod, reinterpret_cast<const float4*>(rots), sh, vp, radii, g.clamped, 0.0f,
+                    dL_dmean2D, dL_dconic, dL_dcolors, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cg);
     return GLIC_OK;
 }
 

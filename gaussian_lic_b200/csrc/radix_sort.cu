@@ -85,6 +85,7 @@ template <typename KeyT, int RB>
 __global__ void __launch_bounds__(256)
 sort_histogram_kernel(const KeyT* __restrict__ keys, int64_t n, const unsigned int* __restrict__ n_dev, int passes, int end_bit,
                       uint32_t* __restrict__ hist) {
+    pdl_enter();
     constexpr int RADIX = 1 << RB;
     if (n_dev) n = min(n, (int64_t)*n_dev);
     __shared__ uint32_t sh[MAX_PASSES * RADIX];
@@ -108,6 +109,7 @@ sort_histogram_kernel(const KeyT* __restrict__ keys, int64_t n, const unsigned i
 
 // ---- 2. exclusive scan of each pass's bins --------------------------------------------
 __global__ void __launch_bounds__(RADIX_MAX) sort_scan_hist_kernel(uint32_t* __restrict__ hist) {
+    pdl_enter();
     __shared__ uint32_t warp_tot[RADIX_MAX / 32];
     uint32_t* h = hist + blockIdx.x * blockDim.x;          // blockDim.x = bins of this sort's widest digit
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -148,6 +150,7 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
                      KeyT* __restrict__ keys_out, uint32_t* __restrict__ vals_out, int64_t n, const unsigned int* __restrict__ n_dev,
                      int shift, int bits, const uint32_t* __restrict__ digit_base, uint32_t* __restrict__ status,
                      uint32_t* __restrict__ ticket) {
+    pdl_enter();
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr int SORT_TILE = SORT_THREADS * SORT_ITEMS;
     constexpr int RADIX_BITS = RB, RADIX = 1 << RB;
@@ -323,10 +326,13 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
 }  // namespace
 
 // zeroes the histograms, tickets and look-back status words of a sort of n pairs on bits [0, end_bit)
+size_t sort_prepare_bytes(int64_t n, int end_bit, int digit_bits) {
+    return n <= 0 ? 0 : sizeof(uint32_t) * (MAX_PASSES * RADIX_MAX + 32 + (size_t)sort_blocks(n) * sort_live_digits(end_bit, digit_bits));
+}
+
 int sort_prepare(int64_t n, int end_bit, void* temp, cudaStream_t s, int digit_bits) {
     if (n <= 0) return GLIC_OK;
-    const size_t used = sizeof(uint32_t) * (MAX_PASSES * RADIX_MAX + 32 + (size_t)sort_blocks(n) * sort_live_digits(end_bit, digit_bits));
-    GLIC_CUDA_TRY(cudaMemsetAsync(temp, 0, used, s));
+    GLIC_CUDA_TRY(cudaMemsetAsync(temp, 0, sort_prepare_bytes(n, end_bit, digit_bits), s));
     return GLIC_OK;
 }
 
@@ -350,10 +356,9 @@ static int run_passes(int64_t n, int passes, int end_bit, int64_t blocks, KeyT* 
     uint32_t* status = t.status;
     for (int p = 0; p < passes; ++p) {
         const int bits = sort_pass_bits(end_bit, p, RB);
-        onesweep_pass_kernel<KeyT, ITEMS, RB><<<(unsigned)blocks, SORT_THREADS, sizeof(PassSmem<KeyT, ITEMS, RB>), s>>>(
-            keys[cur], vals[cur], keys[cur ^ 1], vals[cur ^ 1], n, n_dev, sort_pass_shift(end_bit, p, RB), bits, t.hist + p * BINS,
-            status, t.tickets + p);
-        GLIC_LAUNCH_CHECK();
+        GLIC_LAUNCH_PDL(onesweep_pass_kernel<KeyT, ITEMS, RB>, (unsigned)blocks, SORT_THREADS, sizeof(PassSmem<KeyT, ITEMS, RB>), s,
+                        keys[cur], vals[cur], keys[cur ^ 1], vals[cur ^ 1], n, n_dev, sort_pass_shift(end_bit, p, RB), bits,
+                        t.hist + p * BINS, status, t.tickets + p);
         status += (size_t)blocks << bits;     // each pass's status words cover its live digits only
         cur ^= 1;
     }
@@ -389,12 +394,10 @@ static int launch_sort_pairs_t(int64_t n, int end_bit, KeyT* keys[2], uint32_t* 
     if (!hist_ready) {
         if (int e = sort_prepare(n, end_bit, temp, s, rb)) return e;
         int hist_blocks = (int)std::min<int64_t>((n + 256 * 16 - 1) / (256 * 16), (int64_t)NUM_SMS * 8);
-        if (rb == 9) sort_histogram_kernel<KeyT, 9><<<hist_blocks, 256, 0, s>>>(keys[0], n, n_dev, passes, end_bit, t.hist);
-        else sort_histogram_kernel<KeyT, 8><<<hist_blocks, 256, 0, s>>>(keys[0], n, n_dev, passes, end_bit, t.hist);
-        GLIC_LAUNCH_CHECK();
+        GLIC_LAUNCH_PDL(rb == 9 ? sort_histogram_kernel<KeyT, 9> : sort_histogram_kernel<KeyT, 8>, hist_blocks, 256, 0, s,
+                        keys[0], n, n_dev, passes, end_bit, t.hist);
     }
-    sort_scan_hist_kernel<<<passes, 1 << rb, 0, s>>>(t.hist);
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(sort_scan_hist_kernel, passes, 1 << rb, 0, s, t.hist);
     if (rb == 9) {
         if constexpr (sizeof(KeyT) == 8) return run_passes<KeyT, SORT_ITEMS_BIG, 9>(n, passes, end_bit, sort_blocks_big(n), keys, vals, t, s, n_dev);
     }

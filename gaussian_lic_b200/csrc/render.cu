@@ -32,6 +32,7 @@ namespace glic {
 __global__ void __launch_bounds__(256)
 tile_ranges_kernel(int64_t R, const unsigned int* __restrict__ r_dev, const uint32_t* __restrict__ keys, uint32_t T,
                    uint2* __restrict__ ranges) {
+    pdl_enter();
     if (r_dev) R = min(R, (int64_t)*r_dev);
     const int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;     // four consecutive sorted keys per thread
     if (i0 >= R) return;
@@ -109,7 +110,8 @@ __device__ __forceinline__ uint32_t cta_scan_tiles(int T, Load load, Store store
 // bucket_offsets = inclusive scan of ceil(n_t / 32)
 __global__ void __launch_bounds__(1024)
 bucket_scan_kernel(int T, const uint2* __restrict__ ranges, uint32_t* __restrict__ bucket_offsets, ImageHeader* hdr,
-                   long long R, const GeomHeader* __restrict__ ghdr, int buckets) {
+                   long long R, const GeomHeader* __restrict__ ghdr, int buckets, unsigned int* __restrict__ sorted_in_b, int cur) {
+    pdl_enter();
     const uint32_t total = cta_scan_tiles(
         T, [&](int t) { if (!buckets) return 0u; const uint2 r = ranges[t]; return (r.y - r.x + BUCKET - 1) / BUCKET; },
         [&](int t, uint32_t v) { bucket_offsets[t] = v; });
@@ -118,6 +120,7 @@ bucket_scan_kernel(int T, const uint2* __restrict__ ranges, uint32_t* __restrict
         if (ghdr) { R = ghdr->r_eff; true_R = ghdr->total; ovf = ghdr->overflow; }
         hdr->num_buckets = total; hdr->num_rendered = R;
         hdr->counters[0] = true_R; hdr->counters[1] = total; hdr->counters[2] = ovf; hdr->counters[3] = 0;
+        *sorted_in_b = (unsigned int)cur;
     }
 }
 
@@ -388,6 +391,7 @@ render_forward_kernel(ViewParams vp, bool no_color, const uint2* __restrict__ ra
 // launch geometry depends on a device-side count.
 __global__ void __launch_bounds__(1024)
 live_scan_kernel(int T, const uint32_t* __restrict__ max_contrib, uint32_t* __restrict__ live_offsets, ImageHeader* hdr) {
+    pdl_enter();
     const uint32_t total = cta_scan_tiles(T, [&](int t) { return (max_contrib[t] + BUCKET - 1) / BUCKET; },
                                           [&](int t, uint32_t v) { live_offsets[t] = v; });
     if (threadIdx.x == 0) { hdr->num_live_buckets = total; hdr->bwd_ticket = 0; }
@@ -439,6 +443,7 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
                        const float* __restrict__ pixel_colors, const float* __restrict__ dL_dpix,
                        float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic, float* __restrict__ dL_dopacity,
                        float* __restrict__ dL_dcolors, unsigned long long* __restrict__ counters, DetOut det) {
+    pdl_enter();
     static_assert(!DET || (BWD_ROWPAIRS == 8 && FAST && !COUNT), "the deterministic form is the production body only");
     __shared__ float4 s_sp[BWD_WARPS][BUCKET][3];            // the bucket's splat records, per warp
     __shared__ uint32_t s_gid[BWD_WARPS][BUCKET];
@@ -727,15 +732,13 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
 
 // ---- launchers ------------------------------------------------------------------------------
 int launch_tile_ranges(int64_t R, const GeomHeader* ghdr, const uint32_t* keys_sorted, int T, ImageState img, bool buckets,
-                       cudaStream_t s) {
+                       unsigned int* sorted_in_b, int cur, cudaStream_t s) {
     const unsigned int* r_dev = ghdr ? &ghdr->r_eff : nullptr;
-    GLIC_CUDA_TRY(cudaMemsetAsync(img.ranges, 0, sizeof(uint2) * (size_t)T, s));
     if (R > 0) {
-        tile_ranges_kernel<<<(unsigned)((R + 1023) / 1024), 256, 0, s>>>(R, r_dev, keys_sorted, (uint32_t)T, img.ranges);
-        GLIC_LAUNCH_CHECK();
+        GLIC_LAUNCH_PDL(tile_ranges_kernel, (unsigned)((R + 1023) / 1024), 256, 0, s, R, r_dev, keys_sorted, (uint32_t)T, img.ranges);
     }
-    bucket_scan_kernel<<<1, 1024, 0, s>>>(T, img.ranges, img.bucket_offsets, img.hdr, (long long)R, ghdr, buckets ? 1 : 0);
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(bucket_scan_kernel, 1, 1024, 0, s, T, img.ranges, img.bucket_offsets, img.hdr, (long long)R, ghdr, buckets ? 1 : 0,
+                    sorted_in_b, cur);
     return GLIC_OK;
 }
 
@@ -778,8 +781,7 @@ int launch_render_backward(int P, const ViewParams& vp, int64_t max_buckets, con
     (void)P; (void)smp.bucket_to_tile;
     if (max_buckets <= 0) return GLIC_OK;
     const int T = vp.grid_x * vp.grid_y;
-    live_scan_kernel<<<1, 1024, 0, s>>>(T, img.max_contrib, img.live_offsets, img.hdr);
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(live_scan_kernel, 1, 1024, 0, s, T, img.max_contrib, img.live_offsets, img.hdr);
     // RP = row pairs per lane (8: one warp per bucket's whole tile, 4: two warps share it; the exact and counting forms exist
     // for RP = 8 only).  The occupancy-derived grid size is a property of the DEVICE and the kernel: cached per device.
     static const int rp = getenv("GLIC_BWD_RP") ? atoi(getenv("GLIC_BWD_RP")) : 8;
@@ -804,10 +806,9 @@ int launch_render_backward(int P, const ViewParams& vp, int64_t max_buckets, con
     const int blocks = blocks_per_device[form][dev];
     const int parts = form == 4 ? 2 : 1;
     const int64_t need = (max_buckets * parts + BWD_WARPS - 1) / BWD_WARPS;
-    kern<<<(unsigned)std::min<int64_t>(blocks, need), BWD_WARPS * 32, 0, s>>>(
-        vp, T, img.hdr, img.ranges, point_list, g.rec, img.bucket_offsets, img.live_offsets, smp.ckpt, img.n_contrib,
-        img.pixel_colors, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors, counters, DetOut{});
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(kern, (unsigned)std::min<int64_t>(blocks, need), BWD_WARPS * 32, 0, s, vp, T, img.hdr, img.ranges, point_list, g.rec,
+                    img.bucket_offsets, img.live_offsets, smp.ckpt, img.n_contrib, img.pixel_colors, dL_dpix, dL_dmean2D, dL_dconic,
+                    dL_dopacity, dL_dcolors, counters, DetOut{});
     return GLIC_OK;
 }
 
@@ -834,6 +835,7 @@ __global__ void __launch_bounds__(256)
 det_reduce_kernel(const unsigned int* __restrict__ count, uint32_t P, const uint32_t* __restrict__ keys, const uint32_t* __restrict__ idx,
                   const float* __restrict__ vals, float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic,
                   float* __restrict__ dL_dopacity, float* __restrict__ dL_dcolors) {
+    pdl_enter();
     const uint32_t n = *count;
     const int lane = threadIdx.x & 31;
     const uint32_t warps = gridDim.x * (blockDim.x >> 5);
@@ -892,8 +894,7 @@ int launch_render_backward_det(int P, const ViewParams& vp, int64_t max_buckets,
                                float* dL_dconic, float* dL_dopacity, float* dL_dcolors, cudaStream_t s) {
     if (max_buckets <= 0 || P <= 0) return GLIC_OK;
     const int T = vp.grid_x * vp.grid_y;
-    live_scan_kernel<<<1, 1024, 0, s>>>(T, img.max_contrib, img.live_offsets, img.hdr);
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(live_scan_kernel, 1, 1024, 0, s, T, img.max_contrib, img.live_offsets, img.hdr);
     const auto kern = render_backward_kernel<8, 6, true, false, true>;
     static int blocks_per_device[64] = {};
     int dev = 0;
@@ -907,17 +908,15 @@ int launch_render_backward_det(int P, const ViewParams& vp, int64_t max_buckets,
     }
     const int64_t need = (max_buckets + BWD_WARPS - 1) / BWD_WARPS;
     const DetOut out{det.keys[0], det.idx[0], det.vals, det.count, (uint32_t)(det.cap / 32), (uint32_t)P};
-    kern<<<(unsigned)std::min<int64_t>(blocks_per_device[dev], need), BWD_WARPS * 32, 0, s>>>(
-        vp, T, img.hdr, img.ranges, point_list, g.rec, img.bucket_offsets, img.live_offsets, smp.ckpt, img.n_contrib,
-        img.pixel_colors, dL_dpix, nullptr, nullptr, nullptr, nullptr, nullptr, out);
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(kern, (unsigned)std::min<int64_t>(blocks_per_device[dev], need), BWD_WARPS * 32, 0, s, vp, T, img.hdr, img.ranges,
+                    point_list, g.rec, img.bucket_offsets, img.live_offsets, smp.ckpt, img.n_contrib, img.pixel_colors, dL_dpix, nullptr,
+                    nullptr, nullptr, nullptr, nullptr, out);
     const int cur = launch_sort_pairs32(det.cap, det_key_bits(P), det.keys, det.idx, det.sort_temp, det.sort_temp_size, s, det.count, false);
     if (cur < 0) return cur;
     const int64_t windows = (det.cap + 31) / 32;
     const unsigned blocks = (unsigned)std::min<int64_t>((windows + 7) / 8, (int64_t)NUM_SMS * 16);
-    det_reduce_kernel<<<blocks, 256, 0, s>>>(det.count, (uint32_t)P, det.keys[cur], det.idx[cur], det.vals, dL_dmean2D, dL_dconic,
-                                             dL_dopacity, dL_dcolors);
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(det_reduce_kernel, blocks, 256, 0, s, det.count, (uint32_t)P, det.keys[cur], det.idx[cur], det.vals, dL_dmean2D,
+                    dL_dconic, dL_dopacity, dL_dcolors);
     return GLIC_OK;
 }
 

@@ -196,6 +196,7 @@ __global__ void __launch_bounds__(ST)
 ssim_forward_kernel(int H, int W, float C1, float C2, const float* __restrict__ img1, const float* __restrict__ img2,
                     float* __restrict__ ssim_map, float* __restrict__ dm_dmu1, float* __restrict__ dm_dsigma1_sq,
                     float* __restrict__ dm_dsigma12, float lambda_dssim, float inv_n, float* __restrict__ loss) {
+    pdl_enter();
     ssim_forward_tile<LOSS, false, FIXED>(H, W, C1, C2, img1, img2, ssim_map, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, lambda_dssim, inv_n,
                                    loss, nullptr);
 }
@@ -206,6 +207,7 @@ __global__ void __launch_bounds__(ST)
 ssim_loss_exposure_forward_kernel(int H, int W, float C1, float C2, const float* __restrict__ img, const float* __restrict__ gt,
                                   const float* __restrict__ E, float* __restrict__ dm_dmu1, float* __restrict__ dm_dsigma1_sq,
                                   float* __restrict__ dm_dsigma12, float lambda_dssim, float inv_n, float* __restrict__ loss) {
+    pdl_enter();
     ssim_forward_tile<true, true, FIXED>(H, W, C1, C2, img, gt, nullptr, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, lambda_dssim, inv_n, loss, E);
 }
 
@@ -292,6 +294,7 @@ ssim_backward_kernel(int H, int W, const float* __restrict__ img1, const float* 
                      const float* __restrict__ dL_dmap, const float* __restrict__ dm_dmu1,
                      const float* __restrict__ dm_dsigma1_sq, const float* __restrict__ dm_dsigma12,
                      float* __restrict__ dL_dimg1, float dl_const, float l1_scale) {
+    pdl_enter();
     ssim_backward_tile<CONST_DL, false>(H, W, img1, img2, dL_dmap, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, dL_dimg1, dl_const, l1_scale,
                                         nullptr);
 }
@@ -302,6 +305,7 @@ ssim_loss_exposure_backward_kernel(int H, int W, const float* __restrict__ img, 
                                    const float* __restrict__ E, const float* __restrict__ dm_dmu1,
                                    const float* __restrict__ dm_dsigma1_sq, const float* __restrict__ dm_dsigma12,
                                    float* __restrict__ dL_dout, float dl_const, float l1_scale) {
+    pdl_enter();
     ssim_backward_tile<true, true>(H, W, img, gt, nullptr, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, dL_dout, dl_const, l1_scale, E);
 }
 
@@ -317,6 +321,7 @@ inline unsigned expo_blocks(size_t HW) { return (unsigned)std::min<size_t>((HW +
 __global__ void __launch_bounds__(XT)
 exposure_mix_kernel(size_t HW, const float* __restrict__ img, const float* __restrict__ E, float* __restrict__ dL,
                     double* __restrict__ partials) {
+    pdl_enter();
     __shared__ double red[XT / 32][12];
     float e[12];
 #pragma unroll
@@ -378,6 +383,7 @@ exposure_adam_kernel(int S, ExpoBatch batch, const float* __restrict__ slot_grad
 
 // out[0] = the G per-CTA loss partials summed in a fixed order (float64, lane-strided, then an xor butterfly): one warp
 __global__ void __launch_bounds__(32) loss_finish_kernel(unsigned G, const float* __restrict__ partials, float* __restrict__ out) {
+    pdl_enter();
     double s = 0.0;
     for (unsigned b = threadIdx.x; b < G; b += 32) s += (double)partials[b];
 #pragma unroll
@@ -410,9 +416,8 @@ extern "C" int glic_fused_ssim(int B, int CH, int H, int W, float C1, float C2, 
     if (!planes_ok((long long)B * CH, "fused_ssim")) return GLIC_ERR_INVALID_ARGUMENT;
     if (B * CH == 0) return GLIC_OK;
     dim3 grid((W + SB - 1) / SB, (H + SB - 1) / SB, B * CH), block(ST);
-    ssim_forward_kernel<false><<<grid, block, 0, (cudaStream_t)stream>>>(H, W, C1, C2, img1, img2, ssim_map, dm_dmu1,
-                                                                          dm_dsigma1_sq, dm_dsigma12, 0.f, 0.f, nullptr);
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(ssim_forward_kernel<false>, grid, block, 0, (cudaStream_t)stream, H, W, C1, C2, img1, img2, ssim_map, dm_dmu1,
+                    dm_dsigma1_sq, dm_dsigma12, 0.f, 0.f, nullptr);
     return GLIC_OK;
 }
 
@@ -426,9 +431,8 @@ extern "C" int glic_fused_ssim_backward(int B, int CH, int H, int W, float C1, f
     if (!planes_ok((long long)B * CH, "fused_ssim_backward")) return GLIC_ERR_INVALID_ARGUMENT;
     if (B * CH == 0) return GLIC_OK;
     dim3 grid((W + SB - 1) / SB, (H + SB - 1) / SB, B * CH), block(ST);
-    ssim_backward_kernel<false><<<grid, block, 0, (cudaStream_t)stream>>>(H, W, img1, img2, dL_dmap, dm_dmu1, dm_dsigma1_sq,
-                                                                           dm_dsigma12, dL_dimg1, 0.f, 0.f);
-    GLIC_LAUNCH_CHECK();
+    GLIC_LAUNCH_PDL(ssim_backward_kernel<false>, grid, block, 0, (cudaStream_t)stream, H, W, img1, img2, dL_dmap, dm_dmu1,
+                    dm_dsigma1_sq, dm_dsigma12, dL_dimg1, 0.f, 0.f);
     return GLIC_OK;
 }
 
@@ -437,7 +441,7 @@ extern "C" size_t glic_loss_scratch_bytes(int CH, int H, int W) { return sizeof(
 // partials == NULL: the loss term of every CTA is added atomically into loss_out; otherwise (G floats, G = the forward grid) it
 // is stored per CTA and summed in a fixed order, so the loss value has the same bits on every run
 static int l1_ssim_loss_impl(int CH, int H, int W, float lambda_dssim, const float* img, const float* gt, float* loss_out, float* dL_dimg,
-                             void* scratch, size_t scratch_bytes, float* partials, cudaStream_t s) {
+                             void* scratch, size_t scratch_bytes, float* partials, cudaStream_t s, bool loss_zeroed = false) {
     if (CH <= 0 || H <= 0 || W <= 0 || !img || !gt || !loss_out || !scratch) { set_error("l1_ssim_loss: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (!planes_ok(CH, "l1_ssim_loss")) return GLIC_ERR_INVALID_ARGUMENT;
     if (scratch_bytes < glic_loss_scratch_bytes(CH, H, W)) { set_error("l1_ssim_loss: scratch too small"); return GLIC_ERR_WORKSPACE; }
@@ -448,20 +452,15 @@ static int l1_ssim_loss_impl(int CH, int H, int W, float lambda_dssim, const flo
     const float C1 = 0.01f * 0.01f, C2 = 0.03f * 0.03f;     // loss_utils.h:130-131
     const float inv_n = (float)(1.0 / (double)N);
     dim3 grid((W + SB - 1) / SB, (H + SB - 1) / SB, CH), block(ST);
-    if (!partials) GLIC_CUDA_TRY(cudaMemsetAsync(loss_out, 0, sizeof(float), s));
+    if (!partials && !loss_zeroed) GLIC_CUDA_TRY(cudaMemsetAsync(loss_out, 0, sizeof(float), s));
     { StageTimer _t(GLIC_STAGE_LOSS_FWD, s);
-    if (partials) ssim_forward_kernel<true, true><<<grid, block, 0, s>>>(H, W, C1, C2, img, gt, nullptr, d1, d2, d3, lambda_dssim, inv_n, partials);
-    else ssim_forward_kernel<true><<<grid, block, 0, s>>>(H, W, C1, C2, img, gt, nullptr, d1, d2, d3, lambda_dssim, inv_n, loss_out); }
-    GLIC_LAUNCH_CHECK();
-    if (partials) {
-        loss_finish_kernel<<<1, 32, 0, s>>>(grid.x * grid.y * grid.z, partials, loss_out);
-        GLIC_LAUNCH_CHECK();
-    }
+    if (partials) GLIC_LAUNCH_PDL(ssim_forward_kernel<true, true>, grid, block, 0, s, H, W, C1, C2, img, gt, nullptr, d1, d2, d3, lambda_dssim, inv_n, partials);
+    else GLIC_LAUNCH_PDL(ssim_forward_kernel<true>, grid, block, 0, s, H, W, C1, C2, img, gt, nullptr, d1, d2, d3, lambda_dssim, inv_n, loss_out); }
+    if (partials) GLIC_LAUNCH_PDL(loss_finish_kernel, 1, 32, 0, s, grid.x * grid.y * grid.z, partials, loss_out);
     if (dL_dimg) {
         StageTimer _t(GLIC_STAGE_LOSS_BWD, s);
-        ssim_backward_kernel<true><<<grid, block, 0, s>>>(H, W, img, gt, nullptr, d1, d2, d3, dL_dimg, -lambda_dssim * inv_n,
-                                                          (1.0f - lambda_dssim) * inv_n);
-        GLIC_LAUNCH_CHECK();
+        GLIC_LAUNCH_PDL(ssim_backward_kernel<true>, grid, block, 0, s, H, W, img, gt, nullptr, d1, d2, d3, dL_dimg, -lambda_dssim * inv_n,
+                        (1.0f - lambda_dssim) * inv_n);
     }
     return GLIC_OK;
 }
@@ -480,7 +479,8 @@ extern "C" size_t glic_loss_exposure_scratch_bytes(int H, int W) {
 }
 
 static int loss_exposure_impl(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E, float* loss_out,
-                              float* dL_dimg, float* dL_dE, void* scratch, size_t scratch_bytes, float* partials, cudaStream_t s) {
+                              float* dL_dimg, float* dL_dE, void* scratch, size_t scratch_bytes, float* partials, cudaStream_t s,
+                              bool loss_zeroed = false) {
     if (H <= 0 || W <= 0 || !img || !gt || !E || !loss_out || !scratch) { set_error("l1_ssim_loss_exposure: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
     if ((dL_dimg == nullptr) != (dL_dE == nullptr)) {
         set_error("l1_ssim_loss_exposure: dL_dimg and dL_dE must be both NULL (loss only) or both non-NULL"); return GLIC_ERR_INVALID_ARGUMENT;
@@ -494,23 +494,17 @@ static int loss_exposure_impl(int H, int W, float lambda_dssim, const float* img
     const float C1 = 0.01f * 0.01f, C2 = 0.03f * 0.03f;
     const float inv_n = (float)(1.0 / (double)N);
     dim3 grid((W + SB - 1) / SB, (H + SB - 1) / SB, 3), block(ST);
-    if (!partials) GLIC_CUDA_TRY(cudaMemsetAsync(loss_out, 0, sizeof(float), s));
+    if (!partials && !loss_zeroed) GLIC_CUDA_TRY(cudaMemsetAsync(loss_out, 0, sizeof(float), s));
     { StageTimer _t(GLIC_STAGE_LOSS_FWD, s);
-    if (partials) ssim_loss_exposure_forward_kernel<true><<<grid, block, 0, s>>>(H, W, C1, C2, img, gt, E, d1, d2, d3, lambda_dssim, inv_n, partials);
-    else ssim_loss_exposure_forward_kernel<<<grid, block, 0, s>>>(H, W, C1, C2, img, gt, E, d1, d2, d3, lambda_dssim, inv_n, loss_out); }
-    GLIC_LAUNCH_CHECK();
-    if (partials) {
-        loss_finish_kernel<<<1, 32, 0, s>>>(grid.x * grid.y * grid.z, partials, loss_out);
-        GLIC_LAUNCH_CHECK();
-    }
+    if (partials) GLIC_LAUNCH_PDL(ssim_loss_exposure_forward_kernel<true>, grid, block, 0, s, H, W, C1, C2, img, gt, E, d1, d2, d3, lambda_dssim, inv_n, partials);
+    else GLIC_LAUNCH_PDL(ssim_loss_exposure_forward_kernel<false>, grid, block, 0, s, H, W, C1, C2, img, gt, E, d1, d2, d3, lambda_dssim, inv_n, loss_out); }
+    if (partials) GLIC_LAUNCH_PDL(loss_finish_kernel, 1, 32, 0, s, grid.x * grid.y * grid.z, partials, loss_out);
     if (dL_dimg) {
         StageTimer _t(GLIC_STAGE_LOSS_BWD, s);
-        ssim_loss_exposure_backward_kernel<<<grid, block, 0, s>>>(H, W, img, gt, E, d1, d2, d3, dL_dimg, -lambda_dssim * inv_n,
-                                                                  (1.0f - lambda_dssim) * inv_n);
-        GLIC_LAUNCH_CHECK();
+        GLIC_LAUNCH_PDL(ssim_loss_exposure_backward_kernel, grid, block, 0, s, H, W, img, gt, E, d1, d2, d3, dL_dimg, -lambda_dssim * inv_n,
+                        (1.0f - lambda_dssim) * inv_n);
         const unsigned G = expo_blocks(HW);
-        exposure_mix_kernel<<<G, XT, 0, s>>>(HW, img, E, dL_dimg, expo_partials);
-        GLIC_LAUNCH_CHECK();
+        GLIC_LAUNCH_PDL(exposure_mix_kernel, G, XT, 0, s, HW, img, E, dL_dimg, expo_partials);
         partials_finish_kernel<12><<<1, 12 * 32, 0, s>>>(G, expo_partials, dL_dE);
         GLIC_LAUNCH_CHECK();
     }
@@ -527,10 +521,10 @@ namespace glic {
 // the native mapper's photometric loss (glic_l1_ssim_loss on 3 channels, or glic_l1_ssim_loss_exposure with E); partials
 // (fixed_order_sums_bytes(H, W)) selects the fixed-order loss sum
 int photometric_loss_sum(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E, float* loss, float* dL_dimg,
-                         float* dL_dE, void* scratch, size_t scratch_bytes, void* partials, cudaStream_t s) {
+                         float* dL_dE, void* scratch, size_t scratch_bytes, void* partials, cudaStream_t s, bool loss_zeroed) {
     float* p = static_cast<float*>(partials);
-    if (E) return loss_exposure_impl(H, W, lambda_dssim, img, gt, E, loss, dL_dimg, dL_dE, scratch, scratch_bytes, p, s);
-    return l1_ssim_loss_impl(3, H, W, lambda_dssim, img, gt, loss, dL_dimg, scratch, scratch_bytes, p, s);
+    if (E) return loss_exposure_impl(H, W, lambda_dssim, img, gt, E, loss, dL_dimg, dL_dE, scratch, scratch_bytes, p, s, loss_zeroed);
+    return l1_ssim_loss_impl(3, H, W, lambda_dssim, img, gt, loss, dL_dimg, scratch, scratch_bytes, p, s, loss_zeroed);
 }
 }  // namespace glic
 
