@@ -161,6 +161,12 @@ def _load():
         "glic_p2p_check": (i32, [vp, sz, sz, vp]),
         "glic_eval_scratch_bytes": (sz, [i32, i32, i32]),
         "glic_eval_psnr_ssim": (i32, [i32, i32, i32, vp, vp, vp, vp, sz, vp]),
+        "glic_mask_words_per_row": (i32, [i32]),
+        "glic_pack_mask": (i32, [i32, i32, vp, vp, vp, vp]),
+        "glic_loss_masked_scratch_bytes": (sz, [i32, i32]),
+        "glic_l1_ssim_loss_masked": (i32, [i32, i32, f32, vp, vp, vp, vp, i32, i32, u32, i32, vp, vp, vp, vp, sz, vp]),
+        "glic_eval_masked_scratch_bytes": (sz, [i32, i32, i32]),
+        "glic_eval_psnr_ssim_masked": (i32, [i32, i32, i32, vp, vp, vp, vp, i32, i32, u32, i32, vp, vp, sz, vp]),
         "glic_lpips_weight_floats": (sz, []),
         "glic_lpips_read_weights": (i32, [C.c_char_p, vp]),
         "glic_lpips_scratch_bytes": (sz, [i32, i32]),
@@ -214,6 +220,9 @@ def _load():
         "glic_mapper_enable_frames": (i32, [vp, i32, i32, i32]),
         "glic_mapper_add_frame": (i32, [vp, C.POINTER(Frame), C.POINTER(i32)]),
         "glic_mapper_keyframe_image": (i32, [vp, i32, i32, vp]),
+        "glic_mapper_add_frame_masked": (i32, [vp, C.POINTER(Frame), vp, C.POINTER(i32)]),
+        "glic_mapper_set_keyframe_mask": (i32, [vp, i32, i32, vp]),
+        "glic_mapper_keyframe_mask": (i32, [vp, i32, i32, vp, C.POINTER(u32)]),
         "glic_mapper_frames_get": (i32, [vp, C.POINTER(FrameStats)]),
         "glic_debug_geom": (i32, [i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "glic_debug_binning": (i32, [i32, vp, i64, i64, vp, vp, vp, vp]),

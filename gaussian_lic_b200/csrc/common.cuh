@@ -484,15 +484,32 @@ int launch_activations_forward(int P, const float* opacity_logit, const float* l
 constexpr int EXPO_MAX_SLOTS = 32;
 int launch_exposure_adam(int S, const int* kf_of_slot_host, const float* slot_grads, float* E, float* exp_avg, float* exp_avg_sq,
                          int* steps, float lr, const unsigned int* skip_flag, cudaStream_t s);
+// A view of a bit-packed valid-pixel mask (glic_pack_mask): pixel (y, x) of the viewed H x W region is used when bit c & 31 of
+// words[y * words_per_row + (c >> 5)] is set, c = x0 + x.  x0 lets a column crop read its frame's mask in place.
+struct MaskView {
+    const uint32_t* words;
+    int words_per_row, x0;
+};
+__device__ __forceinline__ bool mask_bit(const MaskView& m, int y, int x) {
+    const int c = m.x0 + x;
+    return (m.words[(size_t)y * m.words_per_row + (c >> 5)] >> (c & 31)) & 1u;
+}
 // glic_eval_psnr_ssim with an optional exposure E (3 channels) applied to img before the clamp
 // fixed (optional, fixed_order_sums_bytes(H, W)): the two sums in a fixed order instead of float64 atomics
+// mask (optional, `valid` > 0 pixels set): both clamped images are 0 at masked pixels, and MSE and the SSIM mean are taken over
+// the CH * valid used elements
 int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, const float* E, float* out2, void* scratch,
-                   size_t scratch_bytes, void* stream, void* fixed = nullptr);
+                   size_t scratch_bytes, void* stream, void* fixed = nullptr, const MaskView* mask = nullptr, uint32_t valid = 0);
 // the native mapper's photometric loss: glic_l1_ssim_loss (3 channels) or, with E, glic_l1_ssim_loss_exposure; partials (optional,
 // fixed_order_sums_bytes(H, W)) sums the loss value in a fixed order instead of with float atomics; loss_zeroed: *loss is zero
-// already (the float atomics add into it without a memset first)
+// already (the float atomics add into it without a memset first); mask (optional, `valid` > 0 pixels set): the masked loss of
+// glic_l1_ssim_loss_masked
 int photometric_loss_sum(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E, float* loss, float* dL_dimg,
-                         float* dL_dE, void* scratch, size_t scratch_bytes, void* partials, cudaStream_t s, bool loss_zeroed = false);
+                         float* dL_dE, void* scratch, size_t scratch_bytes, void* partials, cudaStream_t s, bool loss_zeroed = false,
+                         const MaskView* mask = nullptr, uint32_t valid = 0);
+// glic_pack_mask: bits and count of a device byte mask [H][W], on stream s
+int launch_pack_mask(int H, int W, const uint8_t* valid, uint32_t* words, uint32_t* count, cudaStream_t s);
+inline int mask_words_per_row(int W) { return (W + 31) / 32; }
 size_t fixed_order_sums_bytes(int H, int W);
 // out[3][H][W] = img exposed by E (optional) and clamped to [0,1], element for element the image eval_psnr_ssim scores
 int launch_scored_image(int H, int W, const float* img, const float* E, float* out, cudaStream_t s);

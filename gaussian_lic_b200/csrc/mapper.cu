@@ -191,7 +191,25 @@ struct Keyframe {                    // move-only: it owns its device camera blo
     CamBlock cam;
     Dev<float> cam_dev;              // view16 | proj16 | campos4
     glic_view view;
+    // valid-pixel mask (glic_mapper_set_keyframe_mask): the packed bits, the number of used pixels (0: no mask) and how many
+    // of them lie in columns [0, W/2) (glic_mapper_align's split fit region)
+    Dev<uint32_t> mask;
+    uint32_t mask_valid = 0, mask_valid_left = 0;
 };
+
+// the view of kf's whole mask from column x0 on, or nullptr when kf has none
+const MaskView* keyframe_mask(const Keyframe& kf, int W, MaskView& mv, int x0 = 0) {
+    if (!kf.mask_valid) return nullptr;
+    mv = MaskView{kf.mask, mask_words_per_row(W), x0};
+    return &mv;
+}
+
+// final_T = 0 at the masked pixels of an H x W frame: extend() then takes them as covered and seeds nothing there
+__global__ void __launch_bounds__(256) mask_final_T_kernel(int H, int W, MaskView mk, float* __restrict__ T) {
+    const size_t n = (size_t)H * W;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        if (!mask_bit(mk, (int)(i / W), (int)(i % W))) T[i] = 0.0f;
+}
 
 inline uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
 
@@ -729,10 +747,11 @@ __global__ void overflow_word_kernel(const GeomHeader* ghdr, float* word) { if (
 
 // the L1 + D-SSIM loss of an H x W image against gt, and its dL/dimg; with E (device, 3x4) the loss of the exposed image, and dL/dE;
 // loss_zeroed: *loss is zero already
+// mask (optional, `valid` used pixels): the masked loss
 int photometric_loss(glic_mapper* m, int H, int W, const float* img, const float* gt, const float* E, float* loss, float* dL_dimg, float* dL_dE,
-                     bool loss_zeroed = false) {
+                     bool loss_zeroed = false, const MaskView* mask = nullptr, uint32_t valid = 0) {
     return photometric_loss_sum(H, W, m->cfg.lambda_dssim, img, gt, E, loss, dL_dimg, dL_dE, m->loss_scratch, m->loss_scratch.bytes(),
-                                m->deterministic ? m->det_sums.raw() : nullptr, m->stream, loss_zeroed);
+                                m->deterministic ? m->det_sums.raw() : nullptr, m->stream, loss_zeroed, mask, valid);
 }
 
 // the backward of the last forward_view of v from dL_dpix: colour gradients into col, after_render (optional) recorded, then cg's
@@ -783,9 +802,11 @@ int iteration(glic_mapper* m, const int* views) {
             if (rad) MAP_TRY(push_to_peers(m, rad, sizeof(int) * (size_t)m->P));
         }
         if (buf >= 0) GLIC_CUDA_TRY(cudaStreamWaitEvent(s, m->gt_ready[buf], 0));
-        // loss of this view (the pinned ring keeps the last local view's value for the statistics)
+        // loss of this view (the pinned ring keeps the last local view's value for the statistics), under its keyframe's mask
+        MaskView mv;
         MAP_TRY(photometric_loss(m, H, W, m->color, buf >= 0 ? m->gt_dev[buf] : kf.image, m->expo_on ? m->expo_E + 12 * (size_t)views[sl] : nullptr,
-                                 m->loss_dev + 1, m->dL_dpix, slot(m, EXPOSURE, parity, sl), /*loss_zeroed=*/true));
+                                 m->loss_dev + 1, m->dL_dpix, slot(m, EXPOSURE, parity, sl), /*loss_zeroed=*/true, keyframe_mask(kf, W, mv),
+                                 kf.mask_valid));
         if (buf >= 0) GLIC_CUDA_TRY(cudaEventRecord(m->gt_free[buf], s));
         CompactGrads cg;
         cg.g_rot = reinterpret_cast<float4*>(ga.rot); cg.g_xyz = ga.xyz; cg.g_scale = ga.log_scale; cg.g_opacity = ga.opacity;
@@ -880,8 +901,9 @@ int keyframe_adam_state(glic_mapper* m, bool pose, int index, float* exp_avg, fl
 
 // renders keyframe `index` and scores it (evaluateVisualQuality, gaussian.cpp:754-760): PSNR / SSIM land in eval_out[0..1], and
 // the clamped image (a training keyframe's E applied first; held-out views: identity) and the clamped ground truth stay in the
-// evaluation scratch (eval_clamped).  Asynchronous after the settled forward.
-int render_scored(glic_mapper* m, int is_train, int index, const char* what) {
+// evaluation scratch (eval_clamped).  masked: under the keyframe's mask (if it has one), the masked scores of eval_psnr_ssim and a
+// clamped pair that is 0 at masked pixels.  Asynchronous after the settled forward.
+int render_scored(glic_mapper* m, int is_train, int index, const char* what, bool masked) {
     const Keyframe* kf = nullptr;
     MAP_TRY(keyframe_at(m, is_train, index, what, kf));
     MAP_TRY(poll_ring(m, true));
@@ -890,8 +912,9 @@ int render_scored(glic_mapper* m, int is_train, int index, const char* what) {
     MAP_TRY(forward_settled(m, kf->view, 0));
     MAP_TRY(load_gt(m, *kf, m->gt_dev[0], cudaMemcpyHostToDevice, s));
     const float* E = (is_train && m->expo_on) ? m->expo_E + 12 * (size_t)index : nullptr;
+    MaskView mv;
     return eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], E, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s,
-                          m->deterministic ? m->det_sums.raw() : nullptr);
+                          m->deterministic ? m->det_sums.raw() : nullptr, masked ? keyframe_mask(*kf, W, mv) : nullptr, kf->mask_valid);
 }
 
 // the whole clamped image eval_psnr_ssim last scored (eval_clamped) into rgb_host, on the mapper's stream
@@ -985,6 +1008,11 @@ int extend_core(glic_mapper* m, const Keyframe& kf, int n, const float* d_pts, c
         std::vector<float> ones((size_t)W * H, 1.0f);                                       // empty model: alpha = 1 - T = 0
         GLIC_CUDA_TRY(cudaMemcpyAsync(m->final_T, ones.data(), sizeof(float) * ones.size(), cudaMemcpyHostToDevice, s));
         GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    }
+    MaskView mv;
+    if (const MaskView* mk = keyframe_mask(kf, W, mv)) {           // no point is seeded at a masked pixel
+        mask_final_T_kernel<<<(unsigned)std::min<size_t>(((size_t)W * H + 255) / 256, (size_t)NUM_SMS * 8), 256, 0, s>>>(H, W, *mk, m->final_T);
+        GLIC_LAUNCH_CHECK();
     }
     float view[16];
     std::memcpy(view, kf.cam.view, sizeof(view));
@@ -1084,6 +1112,41 @@ int scan_handoff(glic_mapper* m, const Keyframe& kf, int n) {
     scan_colour_kernel<float><<<blocks, 256, 0, s>>>(3 * n, m->scan_rgb, d_col);
     GLIC_LAUNCH_CHECK();
     return extend_core(m, kf, n, m->scan_xyz, d_col, m->scan_depth, ws);
+}
+
+// the mask checks of set_keyframe_mask and add_frame_masked, before anything is reserved: a mask with no used pixel is refused
+int mask_check(const glic_mapper* m, const uint8_t* valid, const char* what) {
+    const size_t n = (size_t)m->cfg.width * m->cfg.height;
+    if (std::find_if(valid, valid + n, [](uint8_t v) { return v != 0; }) == valid + n) {
+        set_error(std::string(what) + ": the mask has no valid pixel"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    return GLIC_OK;
+}
+
+// packs the host byte mask `valid` (checked by mask_check) into kf's mask: a new bit buffer and a staging buffer are allocated
+// first, so a failure leaves kf's mask as it was; the bits and the count are made on the device, and the mapper's stream is drained
+// before the new buffer replaces the old one (which iterations in flight may still read)
+int pack_keyframe_mask(glic_mapper* m, Keyframe& kf, const uint8_t* valid) {
+    const int W = m->cfg.width, H = m->cfg.height;
+    const size_t n = (size_t)W * H, words = (size_t)H * mask_words_per_row(W);
+    Dev<uint32_t> bits;
+    Dev<uint8_t> staging;                                  // the bytes | the count
+    MAP_TRY(bits.allocate(words * sizeof(uint32_t)));
+    MAP_TRY(staging.allocate(((n + 255) & ~size_t(255)) + 256));
+    uint32_t* d_count = reinterpret_cast<uint32_t*>(staging + ((n + 255) & ~size_t(255)));
+    cudaStream_t s = m->stream;
+    uint32_t count = 0;
+    GLIC_CUDA_TRY(cudaMemcpyAsync(staging, valid, n, cudaMemcpyHostToDevice, s));
+    MAP_TRY(launch_pack_mask(H, W, staging, bits, d_count, s));
+    GLIC_CUDA_TRY(cudaMemcpyAsync(&count, d_count, sizeof(count), cudaMemcpyDeviceToHost, s));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    uint32_t left = 0;
+    for (int y = 0; y < H; ++y)
+        for (int x = 0; x < W / 2; ++x) left += valid[(size_t)y * W + x] != 0;
+    kf.mask = std::move(bits);
+    kf.mask_valid = count;
+    kf.mask_valid_left = left;
+    return GLIC_OK;
 }
 
 int scheduled_density_step(glic_mapper* m);    // optimize()'s density control, with glic_mapper_densify_and_prune below
@@ -1229,8 +1292,11 @@ int glic_mapper_enable_frames(glic_mapper* m, int select_every_k_frame, int sky_
     return GLIC_OK;
 }
 
-int glic_mapper_add_frame(glic_mapper* m, const glic_frame* f, int* is_keyframe) {
+int glic_mapper_add_frame(glic_mapper* m, const glic_frame* f, int* is_keyframe) { return glic_mapper_add_frame_masked(m, f, nullptr, is_keyframe); }
+
+int glic_mapper_add_frame_masked(glic_mapper* m, const glic_frame* f, const uint8_t* valid, int* is_keyframe) {
     if (!m || !f || !f->bgr || (f->n_points > 0 && (!f->xyz || !f->rgb))) { set_error("mapper_add_frame: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (valid) MAP_TRY(mask_check(m, valid, "mapper_add_frame_masked"));
     if (!m->frames_on) { set_error("mapper_add_frame: frames are not enabled (glic_mapper_enable_frames)"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (f->row_bytes < 3 * (size_t)m->cfg.width || f->n_points < 0) { set_error("mapper_add_frame: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
     const size_t pending = (size_t)m->fst.pending_points + (size_t)f->n_points;
@@ -1260,6 +1326,7 @@ int glic_mapper_add_frame(glic_mapper* m, const glic_frame* f, int* is_keyframe)
     uint8_t* dst = m->frame_chunks[idx / FRAME_CHUNK] + (idx % FRAME_CHUNK) * m->frame_stride;
     Keyframe kf;
     MAP_TRY(make_keyframe(m, R_wc, t_wc, nullptr, dst, kf));
+    if (valid) MAP_TRY(pack_keyframe_mask(m, kf, valid));  // before the hand-off: its extend() leaves the masked pixels out
     if (train) {
         if (m->expo_on || m->pose_on) MAP_TRY(reserve_keyframe_rows(m, m->train.size() + 1));
         MAP_TRY(handoff_reserve(m, (int)pending));
@@ -1303,6 +1370,36 @@ int glic_mapper_keyframe_image(glic_mapper* m, int is_train, int index, float* r
     MAP_TRY(load_gt(m, *kf, m->gt_dev[0], cudaMemcpyHostToDevice, m->stream));
     GLIC_CUDA_TRY(cudaMemcpyAsync(rgb_host, m->gt_dev[0], bytes, cudaMemcpyDeviceToHost, m->stream));
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    return GLIC_OK;
+}
+
+int glic_mapper_set_keyframe_mask(glic_mapper* m, int is_train, int index, const uint8_t* valid) {
+    if (!m) { set_error("mapper_set_keyframe_mask: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const Keyframe* kf = nullptr;
+    MAP_TRY(keyframe_at(m, is_train, index, "mapper_set_keyframe_mask", kf));
+    Keyframe& k = (is_train ? m->train : m->test)[index];
+    if (!valid) {                                          // clear: the iterations in flight may still read the old bits
+        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+        k.mask = Dev<uint32_t>();
+        k.mask_valid = k.mask_valid_left = 0;
+        return GLIC_OK;
+    }
+    MAP_TRY(mask_check(m, valid, "mapper_set_keyframe_mask"));
+    return pack_keyframe_mask(m, k, valid);
+}
+
+int glic_mapper_keyframe_mask(glic_mapper* m, int is_train, int index, uint8_t* out, uint32_t* valid_count) {
+    if (!m || !valid_count) { set_error("mapper_keyframe_mask: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const Keyframe* kf = nullptr;
+    MAP_TRY(keyframe_at(m, is_train, index, "mapper_keyframe_mask", kf));
+    *valid_count = kf->mask_valid;
+    if (!out || !kf->mask_valid) return GLIC_OK;
+    const int W = m->cfg.width, H = m->cfg.height, wpr = mask_words_per_row(W);
+    std::vector<uint32_t> bits((size_t)H * wpr);
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    GLIC_CUDA_TRY(cudaMemcpy(bits.data(), kf->mask, bits.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    for (int y = 0; y < H; ++y)
+        for (int x = 0; x < W; ++x) out[(size_t)y * W + x] = (bits[(size_t)y * wpr + (x >> 5)] >> (x & 31)) & 1u;
     return GLIC_OK;
 }
 
@@ -1366,7 +1463,7 @@ int glic_mapper_optimize(glic_mapper* m, const int* views_host, int n_views) {
 
 int glic_mapper_evaluate(glic_mapper* m, int is_train, int index, float* psnr, float* ssim) {
     if (!m || !psnr || !ssim) { set_error("mapper_evaluate: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    MAP_TRY(render_scored(m, is_train, index, "mapper_evaluate"));
+    MAP_TRY(render_scored(m, is_train, index, "mapper_evaluate", true));
     float out2[2] = {0.f, 0.f};
     MAP_TRY(read_eval_out(m, out2, 2));
     *psnr = out2[0]; *ssim = out2[1];
@@ -1390,7 +1487,7 @@ int glic_mapper_evaluate_lpips(glic_mapper* m, int is_train, int index, float* p
     const size_t need = glic_lpips_scratch_bytes(H, W);
     if (!need) { set_error("mapper_evaluate_lpips: LPIPS needs a frame of at least 31x31"); return GLIC_ERR_INVALID_ARGUMENT; }
     MAP_TRY(reserve(m, m->lpips_scratch, need));
-    MAP_TRY(render_scored(m, is_train, index, "mapper_evaluate_lpips"));
+    MAP_TRY(render_scored(m, is_train, index, "mapper_evaluate_lpips", true));
     MAP_TRY(scored_lpips(m, W));
     float out3[3] = {0.f, 0.f, 0.f};
     MAP_TRY(read_eval_out(m, out3, 3));
@@ -1400,7 +1497,7 @@ int glic_mapper_evaluate_lpips(glic_mapper* m, int is_train, int index, float* p
 
 int glic_mapper_render(glic_mapper* m, int is_train, int index, float* rgb_host) {
     if (!m || !rgb_host) { set_error("mapper_render: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    MAP_TRY(render_scored(m, is_train, index, "mapper_render"));
+    MAP_TRY(render_scored(m, is_train, index, "mapper_render", false));
     MAP_TRY(scored_image_to_host(m, rgb_host));
     GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
     return GLIC_OK;
@@ -1672,6 +1769,15 @@ int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_
     const bool split = p.split != 0;
     const int Wf = split ? W / 2 : W, x_score = split ? W / 2 : 0, Ws = W - x_score;     // fit and score columns
     const bool use_expo = p.exposure_lr > 0.0f || (train && m->expo_on);                  // the loss applies E
+    // under the keyframe's mask: the fit loss and both scores are masked, each region read from the mask in place
+    MaskView fit_mv, full_mv, score_mv;
+    const MaskView* fit_mask = keyframe_mask(kf, W, fit_mv);
+    const MaskView* full_mask = keyframe_mask(kf, W, full_mv);
+    const MaskView* score_mask = keyframe_mask(kf, W, score_mv, x_score);
+    const uint32_t fit_valid = split ? kf.mask_valid_left : kf.mask_valid, score_valid = kf.mask_valid - (split ? kf.mask_valid_left : 0);
+    if (kf.mask_valid && (fit_valid == 0 || score_valid == 0)) {
+        set_error("mapper_align: the keyframe's mask leaves no valid pixel in the fit or the score columns"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
     cudaStream_t s = m->stream;
     MAP_TRY(poll_ring(m, true));
     MAP_TRY(reserve(m, m->align_ws, align_carve(nullptr, m->Pcap, W, H, split, nullptr, nullptr, nullptr, nullptr)));
@@ -1726,7 +1832,7 @@ int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_
             img_fit = crops[0];
             dL_fit = crops[2];
         }
-        MAP_TRY(photometric_loss(m, H, Wf, img_fit, gt_fit, use_expo ? st->E : nullptr, &st->loss, dL_fit, st->dE));
+        MAP_TRY(photometric_loss(m, H, Wf, img_fit, gt_fit, use_expo ? st->E : nullptr, &st->loss, dL_fit, st->dE, false, fit_mask, fit_valid));
         if (split) {
             pad_columns_kernel<<<plane_blocks((size_t)3 * H * W), 256, 0, s>>>(H, W, Wf, crops[2], m->dL_dpix);
             GLIC_LAUNCH_CHECK();
@@ -1745,7 +1851,7 @@ int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_
     // scoring at the fitted camera: the full clamped (exposed) frame, then with split its score columns
     MAP_TRY(forward_settled(m, v, 0));
     MAP_TRY(eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], use_expo ? st->E : nullptr, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s,
-                           m->deterministic ? m->det_sums.raw() : nullptr));
+                           m->deterministic ? m->det_sums.raw() : nullptr, full_mask, kf.mask_valid));
     if (rgb_host) MAP_TRY(scored_image_to_host(m, rgb_host));
     if (split) {
         for (int q = 0; q < 2; ++q) {
@@ -1753,7 +1859,7 @@ int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_
             GLIC_LAUNCH_CHECK();
         }
         MAP_TRY(eval_psnr_ssim(3, H, Ws, crops[0], crops[1], nullptr, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s,
-                               m->deterministic ? m->det_sums.raw() : nullptr));
+                               m->deterministic ? m->det_sums.raw() : nullptr, score_mask, score_valid));
     }
     if (m->lpips_w) MAP_TRY(scored_lpips(m, Ws));
     float out3[3] = {0.f, 0.f, std::numeric_limits<float>::quiet_NaN()};

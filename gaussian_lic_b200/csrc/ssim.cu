@@ -62,12 +62,14 @@ __device__ __forceinline__ float expose(const float* __restrict__ img, size_t HW
 // halo load (it never exists in global memory); SSIM, its partial maps and the L1 term are those of the exposed image.
 // FIXED (fixed-order sums, the native mapper's deterministic option): the CTA's loss term goes to loss[linear block id] instead of
 // an atomicAdd into loss[0]; loss_finish_kernel sums those partials in a fixed order.
-template <bool LOSS, bool EXPO, bool FIXED = false>
+// MASK (glic_l1_ssim_loss_masked): a pixel whose bit in mk is clear loads as 0 in both images (a select: nothing read there can
+// leak), exactly like the zero padding outside the frame, and adds no L1 / SSIM term to the loss.
+template <bool LOSS, bool EXPO, bool FIXED = false, bool MASK = false>
 __device__ __forceinline__ void
 ssim_forward_tile(int H, int W, float C1, float C2, const float* __restrict__ img1, const float* __restrict__ img2,
                   float* __restrict__ ssim_map, float* __restrict__ dm_dmu1, float* __restrict__ dm_dsigma1_sq,
                   float* __restrict__ dm_dsigma12, float lambda_dssim, float inv_n, float* __restrict__ loss,
-                  const float* __restrict__ E) {
+                  const float* __restrict__ E, MaskView mk = MaskView{nullptr, 0, 0}) {
     __shared__ float s1[SH_][SH_ + 1];
     __shared__ float s2[SH_][SH_ + 1];
     __shared__ float2 h01[SH_][SB + 1];          // horizontal pass of (x, y)
@@ -79,8 +81,32 @@ ssim_forward_tile(int H, int W, float C1, float C2, const float* __restrict__ im
     const float* a = img1 + (EXPO ? 0 : plane);
     const float* b = img2 + plane;
     const int x0 = blockIdx.x * SB, y0 = blockIdx.y * SB;
+    const uint32_t* vbits = nullptr;
 
-    if (EXPO) {
+    if (MASK) {
+        // the centre rows' mask bits, columns x0 .. x0 + 31 of row y0 + r in bit r of vrow: the loss term reads them here
+        // rather than through the view's pointer, which would otherwise stay live across the convolutions
+        __shared__ uint32_t vrow[SB];
+        if (tid < SB) {
+            const int y = y0 + tid, c = mk.x0 + x0, w = c >> 5, sh = c & 31;
+            uint32_t bits = 0u;
+            if (y < H) {
+                const uint32_t* row = mk.words + (size_t)y * mk.words_per_row;
+                bits = __funnelshift_r(row[w], (sh && w + 1 < mk.words_per_row) ? row[w + 1] : 0u, sh);
+            }
+            vrow[tid] = bits;
+        }
+        vbits = vrow;
+        const ExpoCoef e = EXPO ? expo_coef(E, blockIdx.z) : ExpoCoef{};
+        for (int i = tid; i < SH_ * SH_; i += ST) {
+            const int ly = i / SH_, lx = i % SH_;
+            const int y = y0 + ly - HALO, x = x0 + lx - HALO;
+            const bool use = x >= 0 && y >= 0 && x < W && y < H && mask_bit(mk, y, x);
+            const size_t p = (size_t)y * W + x;
+            s1[ly][lx] = use ? (EXPO ? expose(a, (size_t)H * W, p, e) : a[p]) : 0.0f;
+            s2[ly][lx] = use ? b[p] : 0.0f;
+        }
+    } else if (EXPO) {
         const ExpoCoef e = expo_coef(E, blockIdx.z);
         for (int i = tid; i < SH_ * SH_; i += ST) {
             const int ly = i / SH_, lx = i % SH_;
@@ -171,7 +197,8 @@ ssim_forward_tile(int H, int W, float C1, float C2, const float* __restrict__ im
                 dm_dsigma1_sq[gi] = ((-Cq * Dq) / (A * B * B));
                 dm_dsigma12[gi] = ((2.0f * Cq) / (A * B));
             }
-            if (LOSS) part += (1.0f - lambda_dssim) * fabsf(s1[ry + HALO][tx + HALO] - s2[ry + HALO][tx + HALO]) - lambda_dssim * m;
+            if (LOSS && (!MASK || ((vbits[ry] >> tx) & 1u)))
+                part += (1.0f - lambda_dssim) * fabsf(s1[ry + HALO][tx + HALO] - s2[ry + HALO][tx + HALO]) - lambda_dssim * m;
         }
     }
     if (LOSS) {
@@ -214,12 +241,14 @@ ssim_loss_exposure_forward_kernel(int H, int W, float C1, float C2, const float*
 // dL/dimg1 = conv(dL*dm_dmu1) + 2*img1*conv(dL*dm_dsigma1_sq) + img2*conv(dL*dm_dsigma12)
 // CONST_DL: dL_dmap is the constant `dl_const` (fused loss) and the L1 sign term is added.
 // EXPO: img1 is the three planes of the rendered image; the result is dL/dout at the exposed image out (see expose()).
-template <bool CONST_DL, bool EXPO>
+// MASK: a masked pixel carries no SSIM term (its dL/dmap is 0 as a halo pixel) and gets dL/dimg1 = +0 (a select).
+template <bool CONST_DL, bool EXPO, bool MASK = false>
 __device__ __forceinline__ void
 ssim_backward_tile(int H, int W, const float* __restrict__ img1, const float* __restrict__ img2,
                    const float* __restrict__ dL_dmap, const float* __restrict__ dm_dmu1,
                    const float* __restrict__ dm_dsigma1_sq, const float* __restrict__ dm_dsigma12,
-                   float* __restrict__ dL_dimg1, float dl_const, float l1_scale, const float* __restrict__ E) {
+                   float* __restrict__ dL_dimg1, float dl_const, float l1_scale, const float* __restrict__ E,
+                   MaskView mk = MaskView{nullptr, 0, 0}) {
     __shared__ float s[3][SH_][SH_ + 1];
     __shared__ float h[3][SH_][SB + 1];
     const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
@@ -229,7 +258,7 @@ ssim_backward_tile(int H, int W, const float* __restrict__ img1, const float* __
         const int ly = i / SH_, lx = i % SH_;
         const int y = y0 + ly - HALO, x = x0 + lx - HALO;
         float v0 = 0.f, v1 = 0.f, v2 = 0.f;
-        if (x >= 0 && y >= 0 && x < W && y < H) {
+        if (x >= 0 && y >= 0 && x < W && y < H && (!MASK || mask_bit(mk, y, x))) {
             const size_t gi = plane + (size_t)y * W + x;
             const float dl = CONST_DL ? dl_const : dL_dmap[gi];
             v0 = dm_dmu1[gi] * dl; v1 = dm_dsigma1_sq[gi] * dl; v2 = dm_dsigma12[gi] * dl;
@@ -283,7 +312,7 @@ ssim_backward_tile(int H, int W, const float* __restrict__ img1, const float* __
                 const float d = p1 - p2;
                 out += l1_scale * (d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f));
             }
-            dL_dimg1[gi] = out;
+            dL_dimg1[gi] = (MASK && !mask_bit(mk, py, px)) ? 0.0f : out;
         }
     }
 }
@@ -307,6 +336,41 @@ ssim_loss_exposure_backward_kernel(int H, int W, const float* __restrict__ img, 
                                    float* __restrict__ dL_dout, float dl_const, float l1_scale) {
     pdl_enter();
     ssim_backward_tile<true, true>(H, W, img, gt, nullptr, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, dL_dout, dl_const, l1_scale, E);
+}
+
+// the masked loss (glic_l1_ssim_loss_masked): forward of the 3-plane image (EXPO: exposed by E) against gt, with the
+// fixed-order (FIXED) or atomic loss sum, and its backward (dL/dimg, or with EXPO dL/dout for exposure_mix_kernel)
+template <bool EXPO, bool FIXED>
+__global__ void __launch_bounds__(ST)
+ssim_loss_masked_forward_kernel(int H, int W, float C1, float C2, const float* __restrict__ img, const float* __restrict__ gt,
+                                const float* __restrict__ E, MaskView mk, float* __restrict__ dm_dmu1, float* __restrict__ dm_dsigma1_sq,
+                                float* __restrict__ dm_dsigma12, float lambda_dssim, float inv_n, float* __restrict__ loss) {
+    pdl_enter();
+    ssim_forward_tile<true, EXPO, FIXED, true>(H, W, C1, C2, img, gt, nullptr, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, lambda_dssim, inv_n,
+                                               loss, E, mk);
+}
+
+template <bool EXPO>
+__global__ void __launch_bounds__(ST)
+ssim_loss_masked_backward_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt, const float* __restrict__ E,
+                                 MaskView mk, const float* __restrict__ dm_dmu1, const float* __restrict__ dm_dsigma1_sq,
+                                 const float* __restrict__ dm_dsigma12, float* __restrict__ dL_dout, float dl_const, float l1_scale) {
+    pdl_enter();
+    ssim_backward_tile<true, EXPO, true>(H, W, img, gt, nullptr, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, dL_dout, dl_const, l1_scale, E, mk);
+}
+
+// glic_pack_mask: one warp per 32-column word of a row, its bits by ballot; the valid pixels counted in integers (exact)
+__global__ void __launch_bounds__(256)
+pack_mask_kernel(int H, int W, int wpr, const uint8_t* __restrict__ valid, uint32_t* __restrict__ words, unsigned int* __restrict__ count) {
+    const int lane = threadIdx.x & 31;
+    const size_t n = (size_t)H * wpr, warps = ((size_t)gridDim.x * blockDim.x) >> 5;
+    unsigned int c = 0;
+    for (size_t w = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < n; w += warps) {   // warp-uniform
+        const int y = (int)(w / wpr), x = (int)(w % wpr) * 32 + lane;
+        const unsigned int bits = __ballot_sync(0xffffffffu, x < W && valid[(size_t)y * W + x] != 0);
+        if (lane == 0) { words[w] = bits; c += __popc(bits); }
+    }
+    if (lane == 0 && c) atomicAdd(count, c);
 }
 
 constexpr int XT = 256;             // threads of the exposure mix kernel
@@ -440,8 +504,10 @@ extern "C" size_t glic_loss_scratch_bytes(int CH, int H, int W) { return sizeof(
 
 // partials == NULL: the loss term of every CTA is added atomically into loss_out; otherwise (G floats, G = the forward grid) it
 // is stored per CTA and summed in a fixed order, so the loss value has the same bits on every run
+// mask (3 planes, `valid` > 0 pixels set): the masked loss of glic_l1_ssim_loss_masked
 static int l1_ssim_loss_impl(int CH, int H, int W, float lambda_dssim, const float* img, const float* gt, float* loss_out, float* dL_dimg,
-                             void* scratch, size_t scratch_bytes, float* partials, cudaStream_t s, bool loss_zeroed = false) {
+                             void* scratch, size_t scratch_bytes, float* partials, cudaStream_t s, bool loss_zeroed = false,
+                             const MaskView* mask = nullptr, uint32_t valid = 0) {
     if (CH <= 0 || H <= 0 || W <= 0 || !img || !gt || !loss_out || !scratch) { set_error("l1_ssim_loss: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (!planes_ok(CH, "l1_ssim_loss")) return GLIC_ERR_INVALID_ARGUMENT;
     if (scratch_bytes < glic_loss_scratch_bytes(CH, H, W)) { set_error("l1_ssim_loss: scratch too small"); return GLIC_ERR_WORKSPACE; }
@@ -450,9 +516,21 @@ static int l1_ssim_loss_impl(int CH, int H, int W, float lambda_dssim, const flo
     float* d2 = d1 + N;
     float* d3 = d2 + N;
     const float C1 = 0.01f * 0.01f, C2 = 0.03f * 0.03f;     // loss_utils.h:130-131
-    const float inv_n = (float)(1.0 / (double)N);
+    const float inv_n = (float)(1.0 / (double)(mask ? (size_t)CH * valid : N));     // N_w = CH * valid: today's 1/N when all are set
     dim3 grid((W + SB - 1) / SB, (H + SB - 1) / SB, CH), block(ST);
     if (!partials && !loss_zeroed) GLIC_CUDA_TRY(cudaMemsetAsync(loss_out, 0, sizeof(float), s));
+    if (mask) {
+        { StageTimer _t(GLIC_STAGE_LOSS_FWD, s);
+        if (partials) GLIC_LAUNCH_PDL(ssim_loss_masked_forward_kernel<false, true>, grid, block, 0, s, H, W, C1, C2, img, gt, nullptr, *mask, d1, d2, d3, lambda_dssim, inv_n, partials);
+        else GLIC_LAUNCH_PDL(ssim_loss_masked_forward_kernel<false, false>, grid, block, 0, s, H, W, C1, C2, img, gt, nullptr, *mask, d1, d2, d3, lambda_dssim, inv_n, loss_out); }
+        if (partials) GLIC_LAUNCH_PDL(loss_finish_kernel, 1, 32, 0, s, grid.x * grid.y * grid.z, partials, loss_out);
+        if (dL_dimg) {
+            StageTimer _t(GLIC_STAGE_LOSS_BWD, s);
+            GLIC_LAUNCH_PDL(ssim_loss_masked_backward_kernel<false>, grid, block, 0, s, H, W, img, gt, nullptr, *mask, d1, d2, d3, dL_dimg,
+                            -lambda_dssim * inv_n, (1.0f - lambda_dssim) * inv_n);
+        }
+        return GLIC_OK;
+    }
     { StageTimer _t(GLIC_STAGE_LOSS_FWD, s);
     if (partials) GLIC_LAUNCH_PDL(ssim_forward_kernel<true, true>, grid, block, 0, s, H, W, C1, C2, img, gt, nullptr, d1, d2, d3, lambda_dssim, inv_n, partials);
     else GLIC_LAUNCH_PDL(ssim_forward_kernel<true>, grid, block, 0, s, H, W, C1, C2, img, gt, nullptr, d1, d2, d3, lambda_dssim, inv_n, loss_out); }
@@ -480,7 +558,7 @@ extern "C" size_t glic_loss_exposure_scratch_bytes(int H, int W) {
 
 static int loss_exposure_impl(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E, float* loss_out,
                               float* dL_dimg, float* dL_dE, void* scratch, size_t scratch_bytes, float* partials, cudaStream_t s,
-                              bool loss_zeroed = false) {
+                              bool loss_zeroed = false, const MaskView* mask = nullptr, uint32_t valid = 0) {
     if (H <= 0 || W <= 0 || !img || !gt || !E || !loss_out || !scratch) { set_error("l1_ssim_loss_exposure: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
     if ((dL_dimg == nullptr) != (dL_dE == nullptr)) {
         set_error("l1_ssim_loss_exposure: dL_dimg and dL_dE must be both NULL (loss only) or both non-NULL"); return GLIC_ERR_INVALID_ARGUMENT;
@@ -492,17 +570,22 @@ static int loss_exposure_impl(int H, int W, float lambda_dssim, const float* img
     float* d3 = d2 + N;
     double* expo_partials = reinterpret_cast<double*>(static_cast<char*>(scratch) + expo_partials_offset(H, W));
     const float C1 = 0.01f * 0.01f, C2 = 0.03f * 0.03f;
-    const float inv_n = (float)(1.0 / (double)N);
+    const float inv_n = (float)(1.0 / (double)(mask ? 3 * (size_t)valid : N));
     dim3 grid((W + SB - 1) / SB, (H + SB - 1) / SB, 3), block(ST);
     if (!partials && !loss_zeroed) GLIC_CUDA_TRY(cudaMemsetAsync(loss_out, 0, sizeof(float), s));
     { StageTimer _t(GLIC_STAGE_LOSS_FWD, s);
-    if (partials) GLIC_LAUNCH_PDL(ssim_loss_exposure_forward_kernel<true>, grid, block, 0, s, H, W, C1, C2, img, gt, E, d1, d2, d3, lambda_dssim, inv_n, partials);
+    if (mask && partials) GLIC_LAUNCH_PDL(ssim_loss_masked_forward_kernel<true, true>, grid, block, 0, s, H, W, C1, C2, img, gt, E, *mask, d1, d2, d3, lambda_dssim, inv_n, partials);
+    else if (mask) GLIC_LAUNCH_PDL(ssim_loss_masked_forward_kernel<true, false>, grid, block, 0, s, H, W, C1, C2, img, gt, E, *mask, d1, d2, d3, lambda_dssim, inv_n, loss_out);
+    else if (partials) GLIC_LAUNCH_PDL(ssim_loss_exposure_forward_kernel<true>, grid, block, 0, s, H, W, C1, C2, img, gt, E, d1, d2, d3, lambda_dssim, inv_n, partials);
     else GLIC_LAUNCH_PDL(ssim_loss_exposure_forward_kernel<false>, grid, block, 0, s, H, W, C1, C2, img, gt, E, d1, d2, d3, lambda_dssim, inv_n, loss_out); }
     if (partials) GLIC_LAUNCH_PDL(loss_finish_kernel, 1, 32, 0, s, grid.x * grid.y * grid.z, partials, loss_out);
     if (dL_dimg) {
         StageTimer _t(GLIC_STAGE_LOSS_BWD, s);
-        GLIC_LAUNCH_PDL(ssim_loss_exposure_backward_kernel, grid, block, 0, s, H, W, img, gt, E, d1, d2, d3, dL_dimg, -lambda_dssim * inv_n,
-                        (1.0f - lambda_dssim) * inv_n);
+        // under a mask dL/dout is +0 at masked pixels, so the mix below and dL/dE need no mask of their own
+        if (mask) GLIC_LAUNCH_PDL(ssim_loss_masked_backward_kernel<true>, grid, block, 0, s, H, W, img, gt, E, *mask, d1, d2, d3, dL_dimg,
+                                  -lambda_dssim * inv_n, (1.0f - lambda_dssim) * inv_n);
+        else GLIC_LAUNCH_PDL(ssim_loss_exposure_backward_kernel, grid, block, 0, s, H, W, img, gt, E, d1, d2, d3, dL_dimg, -lambda_dssim * inv_n,
+                             (1.0f - lambda_dssim) * inv_n);
         const unsigned G = expo_blocks(HW);
         GLIC_LAUNCH_PDL(exposure_mix_kernel, G, XT, 0, s, HW, img, E, dL_dimg, expo_partials);
         partials_finish_kernel<12><<<1, 12 * 32, 0, s>>>(G, expo_partials, dL_dE);
@@ -521,12 +604,54 @@ namespace glic {
 // the native mapper's photometric loss (glic_l1_ssim_loss on 3 channels, or glic_l1_ssim_loss_exposure with E); partials
 // (fixed_order_sums_bytes(H, W)) selects the fixed-order loss sum
 int photometric_loss_sum(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E, float* loss, float* dL_dimg,
-                         float* dL_dE, void* scratch, size_t scratch_bytes, void* partials, cudaStream_t s, bool loss_zeroed) {
+                         float* dL_dE, void* scratch, size_t scratch_bytes, void* partials, cudaStream_t s, bool loss_zeroed,
+                         const MaskView* mask, uint32_t valid) {
     float* p = static_cast<float*>(partials);
-    if (E) return loss_exposure_impl(H, W, lambda_dssim, img, gt, E, loss, dL_dimg, dL_dE, scratch, scratch_bytes, p, s, loss_zeroed);
-    return l1_ssim_loss_impl(3, H, W, lambda_dssim, img, gt, loss, dL_dimg, scratch, scratch_bytes, p, s, loss_zeroed);
+    if (E) return loss_exposure_impl(H, W, lambda_dssim, img, gt, E, loss, dL_dimg, dL_dE, scratch, scratch_bytes, p, s, loss_zeroed, mask, valid);
+    return l1_ssim_loss_impl(3, H, W, lambda_dssim, img, gt, loss, dL_dimg, scratch, scratch_bytes, p, s, loss_zeroed, mask, valid);
+}
+
+int launch_pack_mask(int H, int W, const uint8_t* valid, uint32_t* words, uint32_t* count, cudaStream_t s) {
+    const size_t n = (size_t)H * mask_words_per_row(W);
+    GLIC_CUDA_TRY(cudaMemsetAsync(count, 0, sizeof(uint32_t), s));
+    pack_mask_kernel<<<(unsigned)std::min<size_t>((n + 7) / 8, (size_t)NUM_SMS * 8), 256, 0, s>>>(H, W, mask_words_per_row(W), valid, words,
+                                                                                                  count);
+    GLIC_LAUNCH_CHECK();
+    return GLIC_OK;
 }
 }  // namespace glic
+
+extern "C" int glic_mask_words_per_row(int W) { return W > 0 ? mask_words_per_row(W) : 0; }
+
+extern "C" int glic_pack_mask(int H, int W, const uint8_t* valid, uint32_t* words, uint32_t* count, void* stream) {
+    if (H <= 0 || W <= 0 || !valid || !words || !count) { set_error("pack_mask: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
+    return launch_pack_mask(H, W, valid, words, count, (cudaStream_t)stream);
+}
+
+// the masked loss's scratch: the exposed loss's | the fixed-order loss partials
+extern "C" size_t glic_loss_masked_scratch_bytes(int H, int W) {
+    if (H <= 0 || W <= 0) return 0;
+    return glic_loss_exposure_scratch_bytes(H, W) + fixed_order_sums_bytes(H, W);
+}
+
+extern "C" int glic_l1_ssim_loss_masked(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E,
+                                        const uint32_t* mask_words, int words_per_row, int mask_x0, uint32_t valid_count,
+                                        int fixed_order, float* loss_out, float* dL_dimg, float* dL_dE, void* scratch,
+                                        size_t scratch_bytes, void* stream) {
+    if (H <= 0 || W <= 0 || !scratch || (E && ((dL_dimg == nullptr) != (dL_dE == nullptr)))) {
+        set_error("l1_ssim_loss_masked: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (mask_words && (valid_count == 0 || (uint64_t)valid_count > (uint64_t)H * W || mask_x0 < 0 || words_per_row < 1 ||
+                       (int64_t)mask_x0 + W > 32 * (int64_t)words_per_row)) {
+        set_error("l1_ssim_loss_masked: bad mask view, or a mask with no valid pixel"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (scratch_bytes < glic_loss_masked_scratch_bytes(H, W)) { set_error("l1_ssim_loss_masked: scratch too small"); return GLIC_ERR_WORKSPACE; }
+    const size_t lb = glic_loss_exposure_scratch_bytes(H, W);
+    void* partials = fixed_order ? static_cast<char*>(scratch) + lb : nullptr;
+    const MaskView mv{mask_words, words_per_row, mask_x0};
+    return photometric_loss_sum(H, W, lambda_dssim, img, gt, E, loss_out, dL_dimg, dL_dE, scratch, lb, partials, (cudaStream_t)stream, false,
+                                mask_words ? &mv : nullptr, valid_count);
+}
 
 namespace glic {
 int launch_exposure_adam(int S, const int* kf_of_slot, const float* slot_grads, float* E, float* m, float* v, int* t, float lr,
@@ -595,6 +720,43 @@ eval_sum_kernel(size_t N, const float* __restrict__ map, double* __restrict__ ac
     else if ((threadIdx.x & 31) == 0) atomicAdd(&acc2[1], s);
 }
 
+// The masked evaluation (eval_psnr_ssim with a mask): the clamped pair is written with 0 in both images at masked pixels, and only
+// used pixels enter the two sums (a masked one adds +0.0, which leaves a float64 sum's bits as they are).  W: the row length of
+// the planes, HW = H * W.
+template <bool FIXED>
+__global__ void __launch_bounds__(256)
+eval_clamp_mse_masked_kernel(size_t N, const float* __restrict__ img, const float* __restrict__ gt, float* __restrict__ a,
+                             float* __restrict__ b, double* __restrict__ acc2, const float* __restrict__ E, size_t HW, int W, MaskView mk) {
+    double se = 0.0;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t p = i % HW;
+        const bool use = mask_bit(mk, (int)(p / W), (int)(p % W));
+        const float x = use ? scored_pixel(img, E, HW, i) : 0.f;
+        const float y = use ? fminf(fmaxf(gt[i], 0.f), 1.f) : 0.f;
+        a[i] = x; b[i] = y;
+        const float d = x - y;
+        se += (double)(d * d);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
+    if (FIXED) { if ((threadIdx.x & 31) == 0) acc2[blockIdx.x * 8 + (threadIdx.x >> 5)] = se; }
+    else if ((threadIdx.x & 31) == 0 && se != 0.0) atomicAdd(&acc2[0], se);
+}
+
+template <bool FIXED>
+__global__ void __launch_bounds__(256)
+eval_sum_masked_kernel(size_t N, const float* __restrict__ map, double* __restrict__ acc2, size_t HW, int W, MaskView mk) {
+    double s = 0.0;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t p = i % HW;
+        s += mask_bit(mk, (int)(p / W), (int)(p % W)) ? (double)map[i] : 0.0;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (FIXED) { if ((threadIdx.x & 31) == 0) acc2[blockIdx.x * 8 + (threadIdx.x >> 5)] = s; }
+    else if ((threadIdx.x & 31) == 0) atomicAdd(&acc2[1], s);
+}
+
 // eval_finish_kernel on the per-warp partials of the FIXED forms: warps [0, n) of mse and of ssim, summed in a fixed order
 __global__ void __launch_bounds__(32)
 eval_finish_fixed_kernel(size_t N, unsigned n, const double* __restrict__ mse_part, const double* __restrict__ ssim_part, float* __restrict__ out2) {
@@ -621,11 +783,42 @@ __global__ void eval_finish_kernel(size_t N, const double* __restrict__ acc2, fl
 extern "C" size_t glic_eval_scratch_bytes(int CH, int H, int W) { return sizeof(float) * 3 * (size_t)CH * H * W + 256; }
 
 namespace glic {
+namespace {
+// eval_psnr_ssim under a mask, after its checks: the masked clamp, the SSIM map of the masked pair, its masked sum; both means
+// over the Nw = CH * valid used elements
+int eval_psnr_ssim_masked(int CH, int H, int W, const float* img, const float* gt, const float* E, float* out2, void* scratch, void* stream,
+                          void* fixed, MaskView mk, size_t Nw) {
+    const size_t N = (size_t)CH * H * W, HW = (size_t)H * W;
+    cudaStream_t s = (cudaStream_t)stream;
+    double* acc2 = static_cast<double*>(scratch);
+    float* a = reinterpret_cast<float*>(static_cast<char*>(scratch) + 256);
+    float* b = a + N;
+    float* map = b + N;
+    const unsigned blocks = (unsigned)std::min<size_t>((N + 255) / 256, (size_t)NUM_SMS * 8);
+    double* mse_part = fixed ? static_cast<double*>(fixed) : acc2;
+    double* ssim_part = fixed ? mse_part + (size_t)NUM_SMS * 8 * 8 : acc2;
+    if (!fixed) GLIC_CUDA_TRY(cudaMemsetAsync(acc2, 0, 2 * sizeof(double), s));
+    if (fixed) eval_clamp_mse_masked_kernel<true><<<blocks, 256, 0, s>>>(N, img, gt, a, b, mse_part, E, HW, W, mk);
+    else eval_clamp_mse_masked_kernel<false><<<blocks, 256, 0, s>>>(N, img, gt, a, b, acc2, E, HW, W, mk);
+    GLIC_LAUNCH_CHECK();
+    if (int e = glic_fused_ssim(1, CH, H, W, 0.01f * 0.01f, 0.03f * 0.03f, a, b, map, nullptr, nullptr, nullptr, stream)) return e;
+    if (fixed) eval_sum_masked_kernel<true><<<blocks, 256, 0, s>>>(N, map, ssim_part, HW, W, mk);
+    else eval_sum_masked_kernel<false><<<blocks, 256, 0, s>>>(N, map, acc2, HW, W, mk);
+    GLIC_LAUNCH_CHECK();
+    if (fixed) eval_finish_fixed_kernel<<<1, 32, 0, s>>>(Nw, blocks * 8, mse_part, ssim_part, out2);
+    else eval_finish_kernel<<<1, 1, 0, s>>>(Nw, acc2, out2);
+    GLIC_LAUNCH_CHECK();
+    return GLIC_OK;
+}
+}  // namespace
+
 int eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, const float* E, float* out2, void* scratch,
-                   size_t scratch_bytes, void* stream, void* fixed) {
+                   size_t scratch_bytes, void* stream, void* fixed, const MaskView* mask, uint32_t valid) {
     if (CH <= 0 || H <= 0 || W <= 0 || !img || !gt || !out2 || !scratch || (E && CH != 3)) { set_error("eval_psnr_ssim: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (scratch_bytes < glic_eval_scratch_bytes(CH, H, W)) { set_error("eval_psnr_ssim: scratch too small"); return GLIC_ERR_WORKSPACE; }
+    if (mask && valid == 0) { set_error("eval_psnr_ssim: a mask with no valid pixel"); return GLIC_ERR_INVALID_ARGUMENT; }
     const size_t N = (size_t)CH * H * W;
+    if (mask) return eval_psnr_ssim_masked(CH, H, W, img, gt, E, out2, scratch, stream, fixed, *mask, (size_t)CH * valid);
     cudaStream_t s = (cudaStream_t)stream;
     double* acc2 = static_cast<double*>(scratch);                     // first 256 bytes: the two accumulators
     float* a = reinterpret_cast<float*>(static_cast<char*>(scratch) + 256);
@@ -670,6 +863,26 @@ const float* eval_clamped(const void* scratch, int CH, int H, int W, int which) 
 extern "C" int glic_eval_psnr_ssim(int CH, int H, int W, const float* img, const float* gt, float* out2, void* scratch,
                                    size_t scratch_bytes, void* stream) {
     return eval_psnr_ssim(CH, H, W, img, gt, nullptr, out2, scratch, scratch_bytes, stream);
+}
+
+extern "C" size_t glic_eval_masked_scratch_bytes(int CH, int H, int W) {
+    if (CH <= 0 || H <= 0 || W <= 0) return 0;
+    return ((glic_eval_scratch_bytes(CH, H, W) + 255) & ~size_t(255)) + fixed_order_sums_bytes(H, W);
+}
+
+extern "C" int glic_eval_psnr_ssim_masked(int CH, int H, int W, const float* img, const float* gt, const float* E,
+                                          const uint32_t* mask_words, int words_per_row, int mask_x0, uint32_t valid_count,
+                                          int fixed_order, float* out2, void* scratch, size_t scratch_bytes, void* stream) {
+    if (CH <= 0 || H <= 0 || W <= 0 || !scratch) { set_error("eval_psnr_ssim_masked: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (mask_words && (valid_count == 0 || (uint64_t)valid_count > (uint64_t)H * W || mask_x0 < 0 || words_per_row < 1 ||
+                       (int64_t)mask_x0 + W > 32 * (int64_t)words_per_row)) {
+        set_error("eval_psnr_ssim_masked: bad mask view, or a mask with no valid pixel"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (scratch_bytes < glic_eval_masked_scratch_bytes(CH, H, W)) { set_error("eval_psnr_ssim_masked: scratch too small"); return GLIC_ERR_WORKSPACE; }
+    const size_t eb = (glic_eval_scratch_bytes(CH, H, W) + 255) & ~size_t(255);
+    const MaskView mv{mask_words, words_per_row, mask_x0};
+    return eval_psnr_ssim(CH, H, W, img, gt, E, out2, scratch, eb, stream, fixed_order ? static_cast<char*>(scratch) + eb : nullptr,
+                          mask_words ? &mv : nullptr, valid_count);
 }
 
 namespace glic {

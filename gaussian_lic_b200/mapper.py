@@ -109,11 +109,12 @@ class Mapper:
         capi.check(capi.lib.glic_mapper_enable_frames(self._h, int(select_every_k_frame), int(sky_points), int(sky_radius)),
                    "mapper_enable_frames")
 
-    def add_frame(self, q_wc, t_wc, bgr, xyz, rgb):
+    def add_frame(self, q_wc, t_wc, bgr, xyz, rgb, mask=None):
         """Dataset::addFrame (gaussian.cpp:41-111) and the keyframe hand-off of mapping.cpp:158-174 on the GPU.  q_wc: (x, y, z, w)
         odometry orientation; t_wc: position; bgr: [H,W,3] uint8 BGR8 image (a row-padded view such as a[:, :W] of a wider
-        array is passed with its row stride); xyz: [n,3] float32 world points; rgb: [n,3] uint8.  Returns True for a
-        training keyframe, False for a held-out one."""
+        array is passed with its row stride); xyz: [n,3] float32 world points; rgb: [n,3] uint8; mask (optional): the frame's
+        [H,W] valid-pixel map (nonzero / True = used, see set_mask), set before the hand-off so that its extend() seeds
+        nothing at a masked pixel.  Returns True for a training keyframe, False for a held-out one."""
         f = capi.Frame()
         f.q_wc[:] = [float(x) for x in np.asarray(q_wc, np.float64).reshape(4)]
         f.t_wc[:] = [float(x) for x in np.asarray(t_wc, np.float64).reshape(3)]
@@ -127,8 +128,32 @@ class Mapper:
             raise ValueError("xyz and rgb must have the same number of points")
         f.n_points, f.xyz, f.rgb = int(pts.shape[0]), _p(pts), _p(col)
         out = C.c_int()
-        capi.check(capi.lib.glic_mapper_add_frame(self._h, C.byref(f), C.byref(out)), "mapper_add_frame")
+        if mask is None:
+            capi.check(capi.lib.glic_mapper_add_frame(self._h, C.byref(f), C.byref(out)), "mapper_add_frame")
+        else:
+            valid = self._mask_bytes(mask)
+            capi.check(capi.lib.glic_mapper_add_frame_masked(self._h, C.byref(f), _p(valid), C.byref(out)), "mapper_add_frame_masked")
         return bool(out.value)
+
+    def _mask_bytes(self, mask):
+        m = np.asarray(mask)
+        if m.shape != (self.H, self.W):
+            raise ValueError("mask must be a [%d,%d] array" % (self.H, self.W))
+        return np.ascontiguousarray(m != 0, dtype=np.uint8)
+
+    def set_mask(self, is_train, index, valid):
+        """Set (valid: [H,W] array, nonzero / True = the pixel is used) or clear (valid=None) a keyframe's valid-pixel mask.  The
+        loss, evaluate / evaluate_lpips, align and extend() leave masked pixels out (include/glic_b200.h, "Per-keyframe
+        valid-pixel masks"); a mask with no used pixel is refused."""
+        v = None if valid is None else self._mask_bytes(valid)
+        capi.check(capi.lib.glic_mapper_set_keyframe_mask(self._h, int(bool(is_train)), int(index), _p(v)), "mapper_set_keyframe_mask")
+
+    def mask(self, is_train, index):
+        """-> (the stored [H,W] uint8 0/1 mask, or None when the keyframe has none; the number of used pixels)"""
+        n = C.c_uint32()
+        out = np.empty((self.H, self.W), np.uint8)
+        capi.check(capi.lib.glic_mapper_keyframe_mask(self._h, int(bool(is_train)), int(index), _p(out), C.byref(n)), "mapper_keyframe_mask")
+        return (out if n.value else None), int(n.value)
 
     def keyframe_image(self, index, train=True):
         """The [3,H,W] float32 image the loss sees for a keyframe (decoded from 8 bits for add_frame keyframes)."""

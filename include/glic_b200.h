@@ -363,6 +363,41 @@ GLIC_API int glic_l1_ssim_loss_exposure(int H, int W, float lambda_dssim, const 
                                         float* loss_out, float* dL_dimg, float* dL_dE_dev, void* scratch, size_t scratch_bytes,
                                         void* stream);
 
+/* Valid-pixel masks.  A mask marks the pixels of a frame that the loss and the evaluation use (1) and leave out (0): moving
+ * objects, the rig's own platform.  On the device it is bit-packed: row y is glic_mask_words_per_row(W) uint32 words, pixel
+ * (y, x) is bit x & 31 of word y * words_per_row + (x >> 5); the pad bits of a row's last word are 0.  A view of a mask is
+ * (words, words_per_row, x0): the viewed H x W region's pixel (y, x) is the mask's pixel (y, x0 + x), so a column crop reads
+ * its frame's mask in place.
+ *   glic_pack_mask: valid_dev [H][W] bytes (nonzero = used) into words_dev (H * words_per_row words) and count_dev (1 device
+ *   uint32, the number of used pixels, an exact integer sum), on `stream`.
+ *
+ * The masked loss, with a the image (exposed by E_dev when given), b = gt and w the mask:
+ *     a' = w ? a : 0,  b' = w ? b : 0   (a select: NaN or Inf under the mask never enters; the masked pixels act exactly
+ *                                         like the SSIM's zero padding at the frame border)
+ *     L  = (1-lambda) * sum_used |a'-b'| / Nw + lambda * (1 - sum_used SSIM(a', b') / Nw),   Nw = 3 * valid_count
+ *     dL/da = w ? dL/da' : +0
+ * An all-ones mask gives glic_l1_ssim_loss / glic_l1_ssim_loss_exposure bit for bit (loss value, dL/dimg and dL/dE).
+ *   glic_l1_ssim_loss_masked: 3 channels; E_dev NULL or the 12 floats of glic_l1_ssim_loss_exposure (then dL_dimg and dL_dE_dev
+ *   are both NULL or both set, as there); valid_count = the view's used pixels (> 0, or GLIC_ERR_INVALID_ARGUMENT before any
+ *   launch); fixed_order = 1: the loss value summed in a fixed order (bit-reproducible, as the mapper's deterministic option);
+ *   mask_words = NULL: the unmasked loss (the same kernels as glic_l1_ssim_loss / _exposure).  scratch:
+ *   glic_loss_masked_scratch_bytes(H, W).
+ *   glic_eval_psnr_ssim_masked: glic_eval_psnr_ssim's scores (with E_dev, of the exposed image, CH = 3) where both clamped
+ *   images are 0 under the mask and MSE and the SSIM mean are taken over the CH * valid_count used elements (the SSIM map
+ *   itself is that of the masked pair).  fixed_order = 1: both sums in a fixed order.  scratch:
+ *   glic_eval_masked_scratch_bytes(CH, H, W). */
+GLIC_API int glic_mask_words_per_row(int W);
+GLIC_API int glic_pack_mask(int H, int W, const uint8_t* valid_dev, uint32_t* words_dev, uint32_t* count_dev, void* stream);
+GLIC_API size_t glic_loss_masked_scratch_bytes(int H, int W);
+GLIC_API int glic_l1_ssim_loss_masked(int H, int W, float lambda_dssim, const float* img, const float* gt, const float* E_dev,
+                                      const uint32_t* mask_words, int words_per_row, int mask_x0, uint32_t valid_count,
+                                      int fixed_order, float* loss_out, float* dL_dimg, float* dL_dE_dev, void* scratch,
+                                      size_t scratch_bytes, void* stream);
+GLIC_API size_t glic_eval_masked_scratch_bytes(int CH, int H, int W);
+GLIC_API int glic_eval_psnr_ssim_masked(int CH, int H, int W, const float* img, const float* gt, const float* E_dev,
+                                        const uint32_t* mask_words, int words_per_row, int mask_x0, uint32_t valid_count,
+                                        int fixed_order, float* out2, void* scratch, size_t scratch_bytes, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * simple-knn.  Replaces SimpleKNN::knn (simple-knn/simple_knn.cu:185-221): mean of the three
  * smallest squared distances to other points.  points[P,3] -> mean_dists[P].
@@ -990,6 +1025,35 @@ GLIC_API int glic_mapper_enable_frames(glic_mapper* m, int select_every_k_frame,
 GLIC_API int glic_mapper_add_frame(glic_mapper* m, const glic_frame* f, int* is_keyframe /* may be NULL */);
 GLIC_API int glic_mapper_keyframe_image(glic_mapper* m, int is_train, int index, float* rgb_host /* [3,H,W] */);
 GLIC_API int glic_mapper_frames_get(glic_mapper* m, glic_frame_stats* out);
+
+/* Per-keyframe valid-pixel masks: leave moving objects and the rig's own platform out of the map.  A mask is a host [H][W]
+ * byte map of one keyframe, nonzero = the pixel is used; it is kept bit-packed on the device (glic_pack_mask: H *
+ * ceil(W / 32) words, 259 200 bytes at 1920x1080).  Where it is used, with the semantics of glic_l1_ssim_loss_masked:
+ *   - every training iteration's loss of the keyframe: the ground truth under the mask has no influence on any bit of
+ *     training, and dL/dimg is +0 there, so exposure, pose refinement, the densification statistics and the multi-GPU
+ *     exchange follow from the masked dL/dimg unchanged;
+ *   - glic_mapper_evaluate / evaluate_lpips: PSNR and SSIM of glic_eval_psnr_ssim_masked; LPIPS is taken on the same clamped
+ *     pair, which is 0 in both images under the mask, with its usual mean over every pixel;
+ *   - glic_mapper_align: the fit loss and the scores, each over its own columns of the mask; a mask that leaves the fit or the
+ *     score columns without a used pixel is refused (GLIC_ERR_INVALID_ARGUMENT); rgb_host is the scored image, 0 under the mask;
+ *   - extend() on the newest training keyframe (glic_mapper_extend, and add_frame's hand-off): no point is inserted at a masked
+ *     pixel.  Exactly: the selection is that of glic_extend with final_T set to 0 at the masked pixels.
+ * Not affected: glic_mapper_render, glic_mapper_render_camera, contribution scoring and prune_unseen, save_map.  A mapper
+ * with no mask on any keyframe enqueues exactly the launches it did before masks existed.  With world > 1 every rank sets
+ * the same masks, as it adds the same keyframes.  Under GLIC_MAPPER_OPT_DETERMINISTIC the masked loss and evaluation use
+ * their fixed-order sums: the same calls give the same bits.
+ *   glic_mapper_set_keyframe_mask(m, is_train, index, valid): sets (valid != NULL) or clears (valid = NULL) the mask of a
+ *   keyframe.  Packs and counts on the device and synchronises.  A NULL mapper, an index out of range or a mask with no used
+ *   pixel return GLIC_ERR_INVALID_ARGUMENT; a failed allocation returns GLIC_ERR_CUDA; either way nothing changes.
+ *   glic_mapper_keyframe_mask(m, is_train, index, out, valid_count): *valid_count = the used pixels (0: no mask); out
+ *   (optional, [H][W] bytes) receives the stored mask as 0 / 1 when there is one and is left as it is otherwise.  Synchronises.
+ *   glic_mapper_add_frame_masked(m, f, valid, is_keyframe): glic_mapper_add_frame with the frame's mask (valid NULL: none), set
+ *   before the keyframe hand-off so that its extend() leaves the masked pixels out; a held-out frame keeps its mask for the
+ *   evaluation and the alignment.  A mask with no used pixel is refused like the other bad arguments, changing nothing. */
+GLIC_API int glic_mapper_set_keyframe_mask(glic_mapper* m, int is_train, int index, const uint8_t* valid /* host [H][W] or NULL */);
+GLIC_API int glic_mapper_keyframe_mask(glic_mapper* m, int is_train, int index, uint8_t* out /* may be NULL */, uint32_t* valid_count);
+GLIC_API int glic_mapper_add_frame_masked(glic_mapper* m, const glic_frame* f, const uint8_t* valid /* host [H][W] or NULL */,
+                                          int* is_keyframe /* may be NULL */);
 
 /* ---------------------------------------------------------------------------------------
  * Stage timing (cudaEvent pairs recorded on the launching stream around each stage; off by
