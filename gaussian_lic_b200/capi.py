@@ -88,6 +88,19 @@ class UnseenParams(C.Structure):
     _fields_ = [("views", C.c_void_p), ("n_views", C.c_int), ("min_weight", C.c_float), ("min_hits", C.c_uint64), ("sky", C.c_int)]
 
 
+class TsdfGrid(C.Structure):
+    _fields_ = [("origin", C.c_float * 3), ("voxel_size", C.c_float), ("dims", C.c_int * 3), ("data", C.c_void_p)]
+
+
+class MeshParams(C.Structure):
+    _fields_ = [("views", C.c_void_p), ("n_views", C.c_int), ("origin", C.c_float * 3), ("voxel_size", C.c_float), ("dims", C.c_int * 3),
+                ("trunc", C.c_float), ("max_depth", C.c_float)]
+
+
+class MeshCounts(C.Structure):
+    _fields_ = [("vertices", C.c_uint32), ("faces", C.c_uint32), ("observed_voxels", C.c_uint64)]
+
+
 def _load():
     if not os.path.isfile(LIB_PATH):
         raise ImportError(
@@ -224,6 +237,16 @@ def _load():
         "glic_mapper_set_keyframe_mask": (i32, [vp, i32, i32, vp]),
         "glic_mapper_keyframe_mask": (i32, [vp, i32, i32, vp, C.POINTER(u32)]),
         "glic_mapper_frames_get": (i32, [vp, C.POINTER(FrameStats)]),
+        "glic_tsdf_bytes": (sz, [C.POINTER(i32)]),
+        "glic_tsdf_clear": (i32, [C.POINTER(TsdfGrid), vp]),
+        "glic_tsdf_integrate": (i32, [C.POINTER(TsdfGrid), vp, i32, i32, f32, f32, f32, f32, vp, vp, vp, i32, f32, f32, vp]),
+        "glic_mesh_scratch_bytes": (sz, [C.POINTER(i32)]),
+        "glic_mesh_count": (i32, [C.POINTER(TsdfGrid), vp, sz, C.POINTER(C.c_uint64), vp]),
+        "glic_mesh_extract": (i32, [C.POINTER(TsdfGrid), vp, sz, vp, vp, vp, vp]),
+        "glic_mesh_ply_write": (i32, [C.c_char_p, u32, vp, vp, u32, vp]),
+        "glic_mapper_extract_mesh": (i32, [vp, C.POINTER(MeshParams), C.POINTER(MeshCounts)]),
+        "glic_mapper_mesh_get": (i32, [vp, C.POINTER(MeshCounts), vp, vp, vp]),
+        "glic_mapper_save_mesh": (i32, [vp, C.c_char_p]),
         "glic_debug_geom": (i32, [i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "glic_debug_binning": (i32, [i32, vp, i64, i64, vp, vp, vp, vp]),
         "glic_debug_image": (i32, [i32, i32, vp, vp, vp, vp, vp, C.POINTER(i64), vp]),

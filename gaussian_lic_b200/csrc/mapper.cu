@@ -15,6 +15,7 @@
 //     Adam launch on the same bytes.  With densification on, the view's statistics ride along as two more rows (13 floats).
 #include "common.cuh"
 #include "adam_math.cuh"
+#include "mesh.cuh"
 
 #include <algorithm>
 #include <array>
@@ -411,6 +412,12 @@ struct glic_mapper {
     Dev<char> render_ws;
     // ---- contribution scores (glic_mapper_contribution / prune_unseen): hits [Pcap] u64 | max_weight [Pcap] f32, sized on first use
     Dev<char> score_ws;
+    // ---- the last mesh of glic_mapper_extract_mesh: xyz [V,3] f32, rgb [V,3] u8, faces [F,3] i32 (empty until the first call)
+    bool mesh_ready = false;
+    glic_mesh_counts mesh_counts{};
+    Dev<float> mesh_xyz;
+    Dev<uint8_t> mesh_rgb;
+    Dev<int32_t> mesh_faces;
     // ---- raw frames (glic_mapper_enable_frames / add_frame): the 8-bit image store, chunks of FRAME_CHUNK frames of
     //      frame_stride bytes that never move, and the scan of the frames since the last training keyframe (device arrays
     //      of scan_cap points, grown by doubling) ----
@@ -1963,9 +1970,110 @@ int contribution(glic_mapper* m, const int* views, int n) {
     return GLIC_OK;
 }
 
+// ---- meshing (glic_mapper_extract_mesh) ------------------------------------------------------------------------------------
+// the grid of p's geometry over `data`
+glic_tsdf_grid mesh_grid(const glic_mesh_params& p, void* data) {
+    glic_tsdf_grid g;
+    for (int a = 0; a < 3; ++a) { g.origin[a] = p.origin[a]; g.dims[a] = p.dims[a]; }
+    g.voxel_size = p.voxel_size;
+    g.data = data;
+    return g;
+}
+
+// glic_mapper_extract_mesh after its checks.  The grid and the scratch are this call's own; the render workspace is
+// glic_mapper_render_camera's; the new mesh replaces the previous one only once it is complete.
+int extract_mesh(glic_mapper* m, const glic_mesh_params& p, glic_mesh_counts* out) {
+    const int W = m->cfg.width, H = m->cfg.height;
+    cudaStream_t s = m->stream;
+    MAP_TRY(poll_ring(m, true));
+    MAP_TRY(reserve(m, m->render_ws, render_carve(nullptr, W, H, nullptr)));
+    Buf grid_buf, scratch;
+    MAP_TRY(grid_buf.allocate(glic_tsdf_bytes(p.dims)));
+    MAP_TRY(scratch.allocate(glic_mesh_scratch_bytes(p.dims)));
+    const glic_tsdf_grid grid = mesh_grid(p, grid_buf.raw());
+    MAP_TRY(glic_tsdf_clear(&grid, s));
+    RenderPlanes r;
+    render_carve(m->render_ws, W, H, &r);
+    MAP_TRY(activate(m));
+    const size_t first = m->n_sky;
+    const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
+    const int count = p.views ? p.n_views : (int)m->train.size();
+    for (int q = 0; q < count; ++q) {
+        const Keyframe& kf = m->train[p.views ? p.views[q] : q];
+        MAP_TRY(draw_settled(m, [&](long long* cnt) {
+            return glic_render((int)(m->P - first), m->D, m->M, a.xyz + 3 * first, m->act_scales + 3 * first, 1.0f, m->act_rots + 4 * first,
+                               m->act_opacity + first, a.dc + 3 * first, a.rest + (size_t)3 * m->M * first, &kf.view, m->radii + first,
+                               m->geom_ws, m->geom_ws.bytes(), r.image_ws, glic_image_bytes(W, H), m->binning_ws, m->binning_ws.bytes(),
+                               r.color, r.T, nullptr, r.median, (int64_t*)cnt, s);
+        }, [&](int64_t pairs) { return grow_render_binning(m, pairs); }));
+        if (m->counters_host[2]) { set_error("mapper_extract_mesh: a view still overflows the binning workspace after regrowing it"); return GLIC_ERR_WORKSPACE; }
+        MAP_TRY(launch_scored_image(H, W, r.color, nullptr, r.rgb, s));
+        MAP_TRY(glic_tsdf_integrate(&grid, kf.cam_dev, W, H, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, r.median, r.rgb,
+                                    kf.mask_valid ? (const uint32_t*)kf.mask : nullptr, mask_words_per_row(W), p.trunc, p.max_depth, s));
+    }
+    uint64_t t[3];
+    MAP_TRY(mesh_count(grid, scratch.raw(), scratch.bytes(), t, s));
+    if (t[1] > 0xFFFFFFFFull) { set_error("mapper_extract_mesh: more than 2^32 - 1 faces"); return GLIC_ERR_INVALID_ARGUMENT; }
+    Dev<float> xyz;
+    Dev<uint8_t> rgb;
+    Dev<int32_t> faces;
+    MAP_TRY(xyz.allocate(12 * t[0]));
+    MAP_TRY(rgb.allocate(3 * t[0]));
+    MAP_TRY(faces.allocate(12 * t[1]));
+    MAP_TRY(glic_mesh_extract(&grid, scratch.raw(), scratch.bytes(), xyz, rgb, faces, s));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    m->mesh_xyz = std::move(xyz);
+    m->mesh_rgb = std::move(rgb);
+    m->mesh_faces = std::move(faces);
+    m->mesh_counts = glic_mesh_counts{(uint32_t)t[0], (uint32_t)t[1], t[2]};
+    m->mesh_ready = true;
+    if (out) *out = m->mesh_counts;
+    return GLIC_OK;
+}
+
 }  // namespace
 
 extern "C" {
+
+int glic_mapper_extract_mesh(glic_mapper* m, const glic_mesh_params* p, glic_mesh_counts* out) {
+    if (!m || !p) { set_error("mapper_extract_mesh: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!glic_tsdf_bytes(p->dims)) {
+        set_error("mapper_extract_mesh: every grid dimension must be in [2, 2048], with fewer than 2^31 lattice points"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (!(std::isfinite(p->voxel_size) && p->voxel_size > 0.0f) || !std::isfinite(p->origin[0]) || !std::isfinite(p->origin[1]) ||
+        !std::isfinite(p->origin[2])) {
+        set_error("mapper_extract_mesh: voxel_size must be finite and > 0, the origin finite"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (!(std::isfinite(p->trunc) && p->trunc > 0.0f)) { set_error("mapper_extract_mesh: trunc must be finite and > 0"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!(std::isfinite(p->max_depth) && p->max_depth >= 0.0f)) {
+        set_error("mapper_extract_mesh: max_depth must be finite and >= 0"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    MAP_TRY(views_check(m, p->views, p->n_views, "mapper_extract_mesh"));
+    if (m->P <= m->n_sky) { set_error("mapper_extract_mesh: the mapper has no non-sky rows"); return GLIC_ERR_INVALID_ARGUMENT; }
+    return extract_mesh(m, *p, out);
+}
+
+int glic_mapper_mesh_get(glic_mapper* m, glic_mesh_counts* counts, float* xyz, uint8_t* rgb, int32_t* faces) {
+    if (!m) { set_error("mapper_mesh_get: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (counts) *counts = m->mesh_counts;
+    const size_t V = m->mesh_counts.vertices, F = m->mesh_counts.faces;
+    if (xyz && V) GLIC_CUDA_TRY(cudaMemcpyAsync(xyz, m->mesh_xyz, 12 * V, cudaMemcpyDefault, m->stream));
+    if (rgb && V) GLIC_CUDA_TRY(cudaMemcpyAsync(rgb, m->mesh_rgb, 3 * V, cudaMemcpyDefault, m->stream));
+    if (faces && F) GLIC_CUDA_TRY(cudaMemcpyAsync(faces, m->mesh_faces, 12 * F, cudaMemcpyDefault, m->stream));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    return GLIC_OK;
+}
+
+int glic_mapper_save_mesh(glic_mapper* m, const char* path) {
+    if (!m || !path) { set_error("mapper_save_mesh: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!m->mesh_ready) { set_error("mapper_save_mesh: no mesh extracted yet (glic_mapper_extract_mesh)"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const glic_mesh_counts c = m->mesh_counts;
+    std::vector<float> xyz(3 * (size_t)c.vertices);
+    std::vector<uint8_t> rgb(3 * (size_t)c.vertices);
+    std::vector<int32_t> faces(3 * (size_t)c.faces);
+    MAP_TRY(glic_mapper_mesh_get(m, nullptr, xyz.data(), rgb.data(), faces.data()));
+    return glic_mesh_ply_write(path, c.vertices, xyz.data(), rgb.data(), c.faces, faces.data());
+}
 
 int glic_mapper_contribution(glic_mapper* m, const int* views_host, int n_views, float* max_weight, uint64_t* hits, uint64_t* ends) {
     if (!m || (!max_weight && !hits && !ends)) { set_error("mapper_contribution: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }

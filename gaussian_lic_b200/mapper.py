@@ -323,6 +323,40 @@ class Mapper:
                                                       *[_p(out.get(k)) for k in shapes]), "mapper_render_camera")
         return out
 
+    def extract_mesh(self, origin, voxel_size, dims, trunc, max_depth=0.0, views=None):
+        """A coloured triangle mesh of the map (glic_mapper_extract_mesh): the median depth and the colour of the map without
+        its sky rows, drawn at each of training keyframes `views` (None: all of them) and fused into a dense TSDF grid of dims
+        (nx, ny, nz) lattice points from origin with spacing voxel_size (truncation trunc; depths beyond max_depth > 0 left
+        out), then naive surface nets.  Returns a dict of numpy arrays vertices [V,3] float32, colors [V,3] uint8 and faces
+        [F,3] int32 (outward winding), and the counts vertices, faces and observed_voxels.  The mesh also stays in the mapper
+        for save_mesh()."""
+        p = capi.MeshParams()
+        keep = None
+        if views is not None:
+            keep = (C.c_int * max(len(views), 1))(*[int(v) for v in views])
+            p.views, p.n_views = C.cast(keep, C.c_void_p), len(views)
+        p.origin[:] = [float(x) for x in np.asarray(origin, np.float32).reshape(3)]
+        p.voxel_size = float(voxel_size)
+        p.dims[:] = [int(x) for x in dims]
+        p.trunc, p.max_depth = float(trunc), float(max_depth)
+        counts = capi.MeshCounts()
+        capi.check(capi.lib.glic_mapper_extract_mesh(self._h, C.byref(p), C.byref(counts)), "mapper_extract_mesh")
+        del keep
+        return self.mesh()
+
+    def mesh(self):
+        """The last extracted mesh as extract_mesh() returns it (empty arrays before any)."""
+        c = capi.MeshCounts()
+        capi.check(capi.lib.glic_mapper_mesh_get(self._h, C.byref(c), None, None, None), "mapper_mesh_get")
+        V, F = int(c.vertices), int(c.faces)
+        xyz, rgb, faces = np.empty((V, 3), np.float32), np.empty((V, 3), np.uint8), np.empty((F, 3), np.int32)
+        capi.check(capi.lib.glic_mapper_mesh_get(self._h, None, _p(xyz), _p(rgb), _p(faces)), "mapper_mesh_get")
+        return dict(vertices=xyz, colors=rgb, faces=faces, n_vertices=V, n_faces=F, observed_voxels=int(c.observed_voxels))
+
+    def save_mesh(self, path):
+        """Write the last extracted mesh as a binary little-endian PLY (x y z float, red green blue uchar, vertex_indices)."""
+        capi.check(capi.lib.glic_mapper_save_mesh(self._h, str(path).encode()), "mapper_save_mesh")
+
     def synchronize(self):
         capi.check(capi.lib.glic_mapper_synchronize(self._h), "mapper_synchronize")
 

@@ -210,6 +210,57 @@ def skybox_init(n, radius, seed, device="cuda:0", uniforms=False, stream=None):
     return out
 
 
+# ---- meshing (include/glic_b200.h "Meshing") -------------------------------------------------------------------------
+def tsdf_grid(origin, voxel_size, dims, device="cuda:0", stream=None):
+    """A cleared TSDF grid: returns (capi.TsdfGrid, its data tensor).  The data is planar tsdf[N] | weight[N] | colour[3][N]
+    float32, N = nx ny nz, lattice point (i, j, k) at index i + nx (j + ny k); view it with tsdf_planes()."""
+    d = (C.c_int * 3)(*[int(x) for x in dims])
+    nbytes = capi.lib.glic_tsdf_bytes(d)
+    if not nbytes:
+        raise capi.GlicError("tsdf_grid: every dimension must be in [2, 2048], with fewer than 2^31 lattice points")
+    data = torch.empty(nbytes // 4, dtype=torch.float32, device=device)
+    g = capi.TsdfGrid()
+    g.origin[:] = [float(x) for x in origin]
+    g.voxel_size, g.dims[:], g.data = float(voxel_size), [int(x) for x in dims], data.data_ptr()
+    capi.check(capi.lib.glic_tsdf_clear(C.byref(g), stream), "tsdf_clear")
+    return g, data
+
+
+def tsdf_planes(data, dims):
+    """(tsdf [nz,ny,nx], weight [nz,ny,nx], colour [3,nz,ny,nx]) views of a grid's data tensor"""
+    nx, ny, nz = (int(x) for x in dims)
+    N = nx * ny * nz
+    return data[:N].view(nz, ny, nx), data[N:2 * N].view(nz, ny, nx), data[2 * N:].view(3, nz, ny, nx)
+
+
+def tsdf_integrate(grid, viewmatrix, W, H, fx, fy, cx, cy, depth, rgb=None, mask_words=None, words_per_row=0, trunc=0.1, max_depth=0.0,
+                   stream=None):
+    """Fuse one view into grid (glic_tsdf_integrate).  viewmatrix: 16 column-major float32 CUDA values of a camera block;
+    depth [H,W], rgb [3,H,W] (None: colour untouched) float32 CUDA tensors; mask_words (optional) a glic_pack_mask int32 CUDA
+    tensor of words_per_row words per row.  Asynchronous."""
+    capi.check(capi.lib.glic_tsdf_integrate(C.byref(grid), capi.ptr(viewmatrix.contiguous()), int(W), int(H), float(fx), float(fy),
+                                            float(cx), float(cy), capi.ptr(depth.contiguous()),
+                                            capi.ptr(None if rgb is None else rgb.contiguous()), capi.ptr(mask_words),
+                                            int(words_per_row), float(trunc), float(max_depth), stream), "tsdf_integrate")
+
+
+def mesh_extract(grid, device="cuda:0", stream=None):
+    """Surface nets of grid (glic_mesh_count + glic_mesh_extract): returns CUDA tensors (xyz [V,3] float32, rgb [V,3] uint8,
+    faces [F,3] int32).  Synchronises once, for the counts."""
+    dev = torch.device(device)
+    need = capi.lib.glic_mesh_scratch_bytes(grid.dims)
+    scratch = torch.empty(max(need, 1), dtype=torch.uint8, device=dev)
+    counts = (C.c_uint64 * 2)()
+    capi.check(capi.lib.glic_mesh_count(C.byref(grid), capi.ptr(scratch), need, counts, stream), "mesh_count")
+    V, F = int(counts[0]), int(counts[1])
+    xyz = torch.empty(max(V, 1), 3, dtype=torch.float32, device=dev)
+    rgb = torch.empty(max(V, 1), 3, dtype=torch.uint8, device=dev)
+    faces = torch.empty(max(F, 1), 3, dtype=torch.int32, device=dev)
+    capi.check(capi.lib.glic_mesh_extract(C.byref(grid), capi.ptr(scratch), need, capi.ptr(xyz), capi.ptr(rgb), capi.ptr(faces), stream),
+               "mesh_extract")
+    return xyz[:V], rgb[:V], faces[:F]
+
+
 # ---- render() and the model getters it uses (rasterizer/renderer.cpp:21-88; gaussian.cpp:147-175) ------------------
 class GaussianParams:
     """The six raw parameter tensors of GaussianModel with its activation getters (sigmoid / exp / normalize)."""

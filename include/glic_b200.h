@@ -1056,6 +1056,112 @@ GLIC_API int glic_mapper_add_frame_masked(glic_mapper* m, const glic_frame* f, c
                                           int* is_keyframe /* may be NULL */);
 
 /* ---------------------------------------------------------------------------------------
+ * Meshing (no counterpart in the reference): a coloured triangle mesh from depth maps, by TSDF fusion into a dense voxel grid and
+ * naive surface nets, for collision checking, inspection, measurement or a viewer that does not draw splats.  Every step below
+ * is one correctly rounded float operation, in the order written, with no contraction (the fmas are xform_row's own); nothing is
+ * accumulated with atomics, so each output depends only on the inputs and the call order, and two identical call sequences give
+ * identical bits.
+ *   Grid: glic_tsdf_grid, data = DEVICE memory of glic_tsdf_bytes(dims) = 20 N bytes, planar tsdf[N] | weight[N] | colour[3][N]
+ *   (f32), N = nx ny nz.  Lattice point (i, j, k) has index i + nx (j + ny k) and world position o + s (i, j, k), each coordinate
+ *   __fadd_rn(o.x, __fmul_rn(s, (float)i)).  Every dimension in [2, 2048] with N < 2^31; voxel_size finite and > 0, origin
+ *   finite.  glic_tsdf_bytes and glic_mesh_scratch_bytes return 0 for other dims.  glic_tsdf_clear zeroes it: unobserved
+ *   everywhere.
+ *   glic_tsdf_integrate fuses one W x H view.  viewmatrix_dev: the 16 column-major floats of a camera block (device memory, so
+ *   a mapper keyframe's refined block needs no host round trip); depth [H,W]; rgb [3,H,W] or NULL (colour left untouched);
+ *   mask_words a bit-packed mask of glic_pack_mask's layout (words_per_row >= glic_mask_words_per_row(W)) or NULL.  Per lattice
+ *   point p at world position (X, Y, Z):
+ *     1. (x, y, z) = rows 0..2 of the view matrix applied to (X, Y, Z, 1) as the renderer does it (xform_row, geom_math.cuh:
+ *        m[12+r] + fma(Z, m[8+r], fma(X, m[r], Y m[4+r]))), so z is the view-space depth the renderer reports; skip unless z > 0;
+ *     2. u = fx (x / z) + cx, v = fy (y / z) + cy; skip unless 0 <= u < W and 0 <= v < H (float comparisons: NaN skips);
+ *        px = (int)floorf(u), py = (int)floorf(v) (pixel px covers u in [px, px + 1), the renderer's convention);
+ *     3. skip a masked-out pixel; d = depth[py][px]; skip unless d > 0 and (max_depth == 0 or d <= max_depth): NaN skips, and so
+ *        does 0, the median depth of a pixel whose T never falls below 0.5;
+ *     4. sdf = d - z; skip unless sdf >= -trunc;
+ *     5. t = fminf(1, sdf / trunc); with w the stored weight: tsdf = (tsdf w + t) / (w + 1), each colour channel
+ *        col = (col w + rgb[c][py][px]) / (w + 1), weight = w + 1.
+ *   A skipped point is neither read nor written.
+ *   Extraction (naive surface nets): a lattice point is INSIDE iff tsdf < 0 and OBSERVED iff weight > 0.  Cell (i, j, k) has
+ *   corners (i + a, j + b, k + c), a, b, c in {0, 1}; it is ACTIVE iff all 8 corners are observed and they are not all on one
+ *   side.  Its 12 edges go in this order: the x-edges for (b, c) = (0,0), (1,0), (0,1), (1,1), the y-edges for (a, c) in the
+ *   same order, then the z-edges for (a, b).  An edge from A to B (B the upper end) CROSSES when exactly one end is inside, at
+ *   f = tA / (tA - tB).  The cell's vertex offset is the left fold, in edge order, of the crossing points in voxel units from the
+ *   cell's lower corner, divided by the number of crossings; the vertex is o + s ((float)i + off) per axis, and its colour the
+ *   same mean of cA + f (cB - cA), stored as __float2int_rn(fminf(fmaxf(c, 0), 1) 255).  Vertex ids are the ranks of the active
+ *   cells in ascending linear index (of the lower corner).  Every lattice edge from L to L + e_a with both ends observed and
+ *   exactly one inside, whose four cells with lower corners L - e_b - e_c, L - e_c, L, L - e_b ((a, b, c) cyclic) exist and are
+ *   active, makes the quad of their vertices in that order, reversed unless L is inside (normals point out, into free space),
+ *   split into the triangles (q0, q1, q2) and (q0, q2, q3).  Faces are ordered by 3 index(L) + a.
+ *   glic_mesh_count(grid, scratch, bytes, counts_host, stream): counts_host[2] (HOST) = {vertices V, faces F}; the scans stay in
+ *   the scratch (glic_mesh_scratch_bytes(dims): about N / 4 bytes); synchronises once.  glic_mesh_extract then fills xyz [V,3]
+ *   f32, rgb [V,3] u8 and faces [F,3] i32 (device, all non-NULL) from them, asynchronously; the grid must be as it was counted.
+ *   glic_mesh_ply_write(path, V, xyz, rgb, F, faces): HOST arrays to a binary little-endian PLY, element vertex V (float x y z,
+ *   uchar red green blue), element face F (property list uchar int vertex_indices); an I/O failure returns
+ *   GLIC_ERR_INVALID_ARGUMENT with the path in glic_last_error, as glic_ply_write does.
+ *   Every call checks its arguments before it enqueues anything: a NULL pointer, bad dims, a bad voxel size or origin, a frame
+ *   under 1x1 or above GLIC_MAX_TILES tiles, fx or fy not finite and > 0, cx or cy not finite, trunc not finite and > 0, max_depth
+ *   not finite and >= 0 or a short words_per_row return GLIC_ERR_INVALID_ARGUMENT; a scratch under glic_mesh_scratch_bytes
+ *   returns GLIC_ERR_WORKSPACE.
+ * ------------------------------------------------------------------------------------- */
+typedef struct glic_tsdf_grid {
+    float origin[3];               /* world position of lattice point (0, 0, 0) */
+    float voxel_size;              /* lattice spacing */
+    int dims[3];                   /* nx, ny, nz */
+    void* data;                    /* device, glic_tsdf_bytes(dims) bytes */
+} glic_tsdf_grid;
+GLIC_API size_t glic_tsdf_bytes(const int* dims /*[3]*/);
+GLIC_API int glic_tsdf_clear(const glic_tsdf_grid* grid, void* stream);
+GLIC_API int glic_tsdf_integrate(const glic_tsdf_grid* grid, const float* viewmatrix_dev, int W, int H, float fx, float fy, float cx,
+                                 float cy, const float* depth, const float* rgb /* may be NULL */, const uint32_t* mask_words /* may be NULL */,
+                                 int words_per_row, float trunc, float max_depth, void* stream);
+GLIC_API size_t glic_mesh_scratch_bytes(const int* dims /*[3]*/);
+GLIC_API int glic_mesh_count(const glic_tsdf_grid* grid, void* scratch, size_t scratch_bytes, uint64_t* counts_host /*[2]*/, void* stream);
+GLIC_API int glic_mesh_extract(const glic_tsdf_grid* grid, const void* scratch, size_t scratch_bytes, float* xyz, uint8_t* rgb,
+                               int32_t* faces, void* stream);
+GLIC_API int glic_mesh_ply_write(const char* path, uint32_t V, const float* xyz, const uint8_t* rgb, uint32_t F, const int32_t* faces);
+
+/* Meshing the map.  glic_mapper_extract_mesh(m, p, out) is exactly this composition:
+ *   1. clear a grid of p's origin, voxel_size and dims;
+ *   2. for each listed training keyframe k (p->views[0 .. n_views), NULL: every training keyframe; held-out keyframes are not
+ *      used), in list order: draw the map WITHOUT the sky rows at k's current camera block (the refined pose under pose
+ *      refinement), the configured intrinsics and size, by glic_mapper_render_camera's path with exposure_index -1 (the map's
+ *      colour, not the frame's brightness); take its median depth and its clamped rgb; glic_tsdf_integrate them with k's view
+ *      matrix, the configured fx, fy, cx, cy, p's trunc and max_depth and k's mask when it has one (masked pixels, moving objects
+ *      say, are not baked into the mesh);
+ *   3. glic_mesh_count and glic_mesh_extract.
+ * A view whose draw overflows the binning workspace grows it and is drawn again, as evaluation does (stats.overflow_regrows
+ * counts it); a view that still overflows after four draws fails the call with GLIC_ERR_WORKSPACE.  *out (may be NULL): the
+ * vertex and face counts and the number of observed lattice points (weight > 0).  The mesh (xyz, rgb8, faces) stays in the
+ * mapper's device memory until the next successful extract_mesh or destroy: glic_mapper_mesh_get copies it out (cudaMemcpyDefault,
+ * so host or device memory; any pointer may be NULL; counts = the last call's *out, zeros before any) and glic_mapper_save_mesh
+ * writes it with glic_mesh_ply_write (GLIC_ERR_INVALID_ARGUMENT before any extract_mesh).  Memory while the call runs: the grid
+ * (20 B per lattice point: 2.7 GB for 512^3) and the extraction scratch, both released when it returns, the render workspace of
+ * glic_mapper_render_camera (kept), then the new mesh (15 B per vertex + 12 B per face, kept); the grid, the scratch and the render
+ * workspace are reserved before anything runs, and a failed allocation returns GLIC_ERR_CUDA with the previous mesh and the mapper
+ * as they were (failure contract above).
+ * The map is frozen exactly as under glic_mapper_render_camera; no stats field but overflow_regrows changes.  The call drains the
+ * iteration pipeline first and synchronises at the end.  With world > 1 it is rank-local and touches no exchange slot.  A mapper
+ * that never calls it allocates and enqueues nothing for it.  Rejected with GLIC_ERR_INVALID_ARGUMENT, changing nothing: a NULL m
+ * or p, what glic_tsdf_integrate rejects in the grid, trunc and max_depth, n_views < 0, a view index out of range, a mapper with
+ * no non-sky rows. */
+typedef struct glic_mesh_params {
+    const int* views;              /* host, training keyframe indices; NULL: every training keyframe */
+    int n_views;                   /* >= 0; ignored when views is NULL */
+    float origin[3];
+    float voxel_size;
+    int dims[3];
+    float trunc;                   /* > 0: the truncation distance, world units */
+    float max_depth;               /* > 0: depths beyond it are not fused; 0: no limit */
+} glic_mesh_params;
+typedef struct glic_mesh_counts {
+    uint32_t vertices, faces;
+    uint64_t observed_voxels;
+} glic_mesh_counts;
+GLIC_API int glic_mapper_extract_mesh(glic_mapper* m, const glic_mesh_params* p, glic_mesh_counts* out /* may be NULL */);
+GLIC_API int glic_mapper_mesh_get(glic_mapper* m, glic_mesh_counts* counts, float* xyz /*[V,3]*/, uint8_t* rgb /*[V,3]*/,
+                                  int32_t* faces /*[F,3]*/);
+GLIC_API int glic_mapper_save_mesh(glic_mapper* m, const char* path);
+
+/* ---------------------------------------------------------------------------------------
  * Stage timing (cudaEvent pairs recorded on the launching stream around each stage; off by
  * default).  glic_profile_enable(1) starts recording and resets the accumulators;
  * glic_profile_read() synchronises the recorded events and returns, per stage, the summed
