@@ -101,6 +101,14 @@ class MeshCounts(C.Structure):
     _fields_ = [("vertices", C.c_uint32), ("faces", C.c_uint32), ("observed_voxels", C.c_uint64)]
 
 
+class RigidCorrection(C.Structure):
+    _fields_ = [("R", C.c_double * 9), ("t", C.c_double * 3), ("q", C.c_double * 4), ("sh", C.c_double * 83)]
+
+
+class PoseCorrection(C.Structure):
+    _fields_ = [("is_train", C.c_int), ("index", C.c_int), ("R_wc", C.c_float * 9), ("t_wc", C.c_float * 3)]
+
+
 def _load():
     if not os.path.isfile(LIB_PATH):
         raise ImportError(
@@ -247,6 +255,12 @@ def _load():
         "glic_mapper_extract_mesh": (i32, [vp, C.POINTER(MeshParams), C.POINTER(MeshCounts)]),
         "glic_mapper_mesh_get": (i32, [vp, C.POINTER(MeshCounts), vp, vp, vp]),
         "glic_mapper_save_mesh": (i32, [vp, C.c_char_p]),
+        "glic_pose_correction_record": (i32, [C.POINTER(f32), C.POINTER(f32), C.POINTER(f32), C.POINTER(f32), i32,
+                                              C.POINTER(RigidCorrection)]),
+        "glic_sh_rotation": (i32, [C.POINTER(C.c_double), i32, C.POINTER(C.c_double)]),
+        "glic_mapper_anchors": (i32, [vp, vp]),
+        "glic_mapper_set_anchors": (i32, [vp, vp]),
+        "glic_mapper_correct_poses": (i32, [vp, i32, C.POINTER(PoseCorrection), C.POINTER(u32)]),
         "glic_debug_geom": (i32, [i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "glic_debug_binning": (i32, [i32, vp, i64, i64, vp, vp, vp, vp]),
         "glic_debug_image": (i32, [i32, i32, vp, vp, vp, vp, vp, C.POINTER(i64), vp]),

@@ -16,6 +16,7 @@
 #include "common.cuh"
 #include "adam_math.cuh"
 #include "mesh.cuh"
+#include "pose_correction.cuh"
 
 #include <algorithm>
 #include <array>
@@ -248,6 +249,16 @@ __device__ void se3_exp(const double u[6], double R[9], double t[3]) {
     for (int i = 0; i < 3; ++i) t[i] = V[3 * i] * u[0] + V[3 * i + 1] * u[1] + V[3 * i + 2] * u[2];
 }
 
+// The float pose (R_wc = R_cw^T, t_wc = -R_cw^T t_cw) of the float64 T_cw = Rn (row-major) | tn into f (R_wc | t_wc), and the
+// camera block of that float pose into cam: the pose step and glic_mapper_correct_poses re-derive a refined keyframe here
+__device__ __forceinline__ void pose_derive(const double* Rn, const double* tn, const float* Pm, float* f, float* cam) {
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) f[3 * i + j] = (float)Rn[3 * j + i];
+        f[9 + i] = (float)(-(Rn[i] * tn[0] + Rn[3 + i] * tn[1] + Rn[6 + i] * tn[2]));
+    }
+    pose_camera(f, f + 9, Pm, cam, nullptr);
+}
+
 struct PoseBatch {
     int kf[MAX_SLOTS];                // keyframe of each slot
     float* cam[MAX_SLOTS];            // its device camera block
@@ -287,12 +298,26 @@ pose_step_kernel(int S, PoseBatch b, const float* __restrict__ slot_grads /* [S]
     }
     for (int e = 0; e < 9; ++e) Tk[e] = Rn[e];
     for (int i = 0; i < 3; ++i) Tk[9 + i] = tn[i];
-    float* f = pose_f + 12 * (size_t)kf;
-    for (int i = 0; i < 3; ++i) {
-        for (int j = 0; j < 3; ++j) f[3 * i + j] = (float)Rn[3 * j + i];
-        f[9 + i] = (float)(-(Rn[i] * tn[0] + Rn[3 + i] * tn[1] + Rn[6 + i] * tn[2]));
-    }
-    pose_camera(f, f + 9, b.Pm, b.cam[s], nullptr);
+    pose_derive(Rn, tn, b.Pm, pose_f + 12 * (size_t)kf, b.cam[s]);
+}
+
+// glic_mapper_correct_poses under pose refinement: slot s < S moves keyframe b.kf[s] by its record dT = [R | t]:
+// T_cw <- T_cw dT^-1 = R_cw R^T | t_cw - (R_cw R^T) t, then the float pose and the camera block as the pose step derives them
+__global__ void __launch_bounds__(MAX_SLOTS)
+pose_correct_kernel(int S, PoseBatch b, const glic_rigid_correction* __restrict__ table, double* __restrict__ T, float* __restrict__ pose_f) {
+    const int s = threadIdx.x;
+    if (s >= S) return;
+    const int kf = b.kf[s];
+    const double* R = table[kf].R;
+    const double* t = table[kf].t;
+    double* Tk = T + 12 * (size_t)kf;
+    double Rn[9], tn[3];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) Rn[3 * i + j] = dadd(dadd(dmul(Tk[3 * i], R[3 * j]), dmul(Tk[3 * i + 1], R[3 * j + 1])), dmul(Tk[3 * i + 2], R[3 * j + 2]));
+    for (int i = 0; i < 3; ++i) tn[i] = dadd(Tk[9 + i], -dadd(dadd(dmul(Rn[3 * i], t[0]), dmul(Rn[3 * i + 1], t[1])), dmul(Rn[3 * i + 2], t[2])));
+    for (int e = 0; e < 9; ++e) Tk[e] = Rn[e];
+    for (int i = 0; i < 3; ++i) Tk[9 + i] = tn[i];
+    pose_derive(Rn, tn, b.Pm, pose_f + 12 * (size_t)kf, b.cam[s]);
 }
 
 // ---- raw frames (glic_mapper_add_frame; Dataset::addFrame, gaussian.cpp:41-111) -------------------------------------------
@@ -357,6 +382,7 @@ struct glic_mapper {
     uint32_t P = 0, Pcap = 0;
     uint32_t n_sky = 0;                   // rows [0, n_sky) are the skybox (glic_mapper_initialize_lidar): left out of save_map
     Dev<float> params, m1, m2;
+    Dev<int32_t> anchor;                  // [Pcap]: the training keyframe each row moves with (glic_mapper_correct_poses), or -1
     Dev<float> act_opacity, act_scales, act_rots;
     Dev<int> radii;
     Dev<float> g_conic;                   // the render backward's 2-D gradient accumulators: conic [4 Pcap] | mean2D [3 Pcap] | opacity
@@ -539,7 +565,8 @@ int push_to_peers(glic_mapper* m, const void* local, size_t bytes) {
 }
 
 // grows everything whose size depends on the Gaussian capacity, all of it allocated before any old buffer is released; the
-// arenas keep their live rows and every new buffer but pose_part starts zeroed, so rows [P, Pcap) of the arenas stay zero
+// arenas and the anchors keep their live rows and every new buffer but pose_part and the anchors starts zeroed, so rows [P, Pcap)
+// of the arenas stay zero
 int set_capacity(glic_mapper* m, uint32_t cap) {
     cap = round_up(std::max<uint32_t>(cap, 256), 256);
     if (cap <= m->Pcap) return GLIC_OK;
@@ -556,7 +583,8 @@ int set_capacity(glic_mapper* m, uint32_t cap) {
                               {m->act_opacity, (size_t)cap * 4, 0, true}, {m->act_scales, (size_t)cap * 12, 0, true},
                               {m->act_rots, (size_t)cap * 16, 0, true}, {m->radii, (size_t)cap * 4, 0, true},
                               {m->g_conic, (size_t)cap * (16 + 12 + 4), 0, true}, {m->geom_ws, glic_geom_bytes((int)cap), 0, true},
-                              {m->xblock, x.bytes, 0, true}, {m->pose_part, pose_partials_count(cap) * sizeof(double)}};
+                              {m->xblock, x.bytes, 0, true}, {m->pose_part, pose_partials_count(cap) * sizeof(double)},
+                              {m->anchor, (size_t)cap * 4, (size_t)m->P * 4}};
     if (m->dens_on)                                       // the statistics keep their live rows
         for (Buf* b : {(Buf*)&m->dens_accum, (Buf*)&m->dens_denom, (Buf*)&m->dens_maxr}) list.push_back({*b, (size_t)cap * 4, (size_t)m->P * 4, true});
     MAP_TRY(grow(m, list, regrow));
@@ -969,8 +997,9 @@ int install_map(glic_mapper* m, uint32_t P, uint32_t n_sky) {
 
 // initialize() (gaussian.cpp:212-304) from device arrays: the sky rows, then the n LiDAR rows.  The caller has validated the
 // arguments, sized the arena for sky_points + n rows and hands sky_ws of glic_skybox_init_bytes(sky_points) bytes.
+// anchor: the LiDAR rows' (the sky rows take -1)
 int initialize_lidar_core(glic_mapper* m, int n, const float* d_pts, const double* d_col, const float* d_dep, double focal, int sky_points,
-                          int sky_radius, void* sky_ws) {
+                          int sky_radius, void* sky_ws, int32_t anchor) {
     const uint32_t S = (uint32_t)sky_points, P = S + (uint32_t)n;
     MAP_TRY(start_map(m, P));
     cudaStream_t s = m->stream;
@@ -979,6 +1008,7 @@ int initialize_lidar_core(glic_mapper* m, int n, const float* d_pts, const doubl
                              a.opacity, nullptr, s));
     MAP_TRY(glic_lidar_init(n, d_pts, d_col, d_dep, (double)m->cfg.scaling_scale, focal, a.xyz + 3 * (size_t)S, a.dc + 3 * (size_t)S,
                             a.log_scale + 3 * (size_t)S, a.rot + 4 * (size_t)S, a.opacity + S, s));
+    MAP_TRY(launch_fill_anchors(m->anchor, 0, S, P, anchor, s));
     return install_map(m, P, S);
 }
 
@@ -997,10 +1027,11 @@ size_t extend_core_carve(void* ws, int n, int W, int H, int** keep, float** out5
     return c.total();
 }
 
-// extend() (gaussian.cpp:499-638) on training keyframe kf, the newest, from device arrays of n > 0 points.  The caller has
-// drained the ring, sized the arena for P + n rows, recorded m->t0 before staging its inputs and hands ws of
-// extend_core_carve(nullptr, n, W, H, ...) bytes.
-int extend_core(glic_mapper* m, const Keyframe& kf, int n, const float* d_pts, const float* d_col, const float* d_dep, void* ws) {
+// extend() (gaussian.cpp:499-638) on training keyframe kf, the newest, from device arrays of n > 0 points; the new rows take
+// anchor `anchor`.  The caller has drained the ring, sized the arena for P + n rows, recorded m->t0 before staging its inputs and
+// hands ws of extend_core_carve(nullptr, n, W, H, ...) bytes.
+int extend_core(glic_mapper* m, const Keyframe& kf, int n, const float* d_pts, const float* d_col, const float* d_dep, void* ws,
+                int32_t anchor) {
     cudaStream_t s = m->stream;
     const int W = m->cfg.width, H = m->cfg.height;
     int* d_keep = nullptr;
@@ -1034,6 +1065,7 @@ int extend_core(glic_mapper* m, const Keyframe& kf, int n, const float* d_pts, c
     MAP_TRY(glic_extend(n, d_pts, d_col, d_dep, Rcw, tcw, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, W, H, m->final_T, m->cfg.scaling_scale,
                         d_ws, glic_extend_bytes(n, W, H), d_keep, d_xyz, d_dc, d_ls, d_rot, d_op, &count, s));
     MAP_TRY(glic_arena_append(m->params, m->m1, m->m2, m->P, m->Pcap, (uint32_t)m->M, (uint32_t)count, d_xyz, d_dc, d_ls, d_rot, d_op, s));
+    MAP_TRY(launch_fill_anchors(m->anchor, m->P, m->P, m->P + (uint32_t)count, anchor, s));
     GLIC_CUDA_TRY(cudaEventRecord(m->t1, s));
     GLIC_CUDA_TRY(cudaStreamSynchronize(s));
     cudaEventElapsedTime(&m->st.ms_extend, m->t0, m->t1);
@@ -1097,7 +1129,8 @@ int handoff_reserve(glic_mapper* m, int n) {
     return reserve(m, m->extend_ws, c.total());
 }
 
-// mapping.cpp:158-174 at training keyframe kf: the n accumulated scan points initialize the map, or extend it.  Everything is
+// mapping.cpp:158-174 at training keyframe kf: the n accumulated scan points initialize the map, or extend it.  kf joins the
+// training list right after, so its rows are anchored to index train.size().  Everything is
 // reserved (handoff_reserve); the one allocation left is a binning regrow, which comes before the map changes.
 int scan_handoff(glic_mapper* m, const Keyframe& kf, int n) {
     cudaStream_t s = m->stream;
@@ -1110,7 +1143,7 @@ int scan_handoff(glic_mapper* m, const Keyframe& kf, int n) {
         scan_colour_kernel<double><<<blocks, 256, 0, s>>>(3 * n, m->scan_rgb, d_col);
         GLIC_LAUNCH_CHECK();
         const double focal = ((double)m->cfg.fx + (double)m->cfg.fy) / 2;
-        return initialize_lidar_core(m, n, m->scan_xyz, d_col, m->scan_depth, focal, S, m->frame_sky_radius, sky_ws);
+        return initialize_lidar_core(m, n, m->scan_xyz, d_col, m->scan_depth, focal, S, m->frame_sky_radius, sky_ws, (int32_t)m->train.size());
     }
     if (n == 0) { m->st.last_inserted = 0; return GLIC_OK; }
     float* d_col = c.take<float>((size_t)3 * n);
@@ -1118,7 +1151,7 @@ int scan_handoff(glic_mapper* m, const Keyframe& kf, int n) {
     GLIC_CUDA_TRY(cudaEventRecord(m->t0, s));
     scan_colour_kernel<float><<<blocks, 256, 0, s>>>(3 * n, m->scan_rgb, d_col);
     GLIC_LAUNCH_CHECK();
-    return extend_core(m, kf, n, m->scan_xyz, d_col, m->scan_depth, ws);
+    return extend_core(m, kf, n, m->scan_xyz, d_col, m->scan_depth, ws, (int32_t)m->train.size());
 }
 
 // the mask checks of set_keyframe_mask and add_frame_masked, before anything is reserved: a mask with no used pixel is refused
@@ -1227,6 +1260,7 @@ int glic_mapper_initialize(glic_mapper* m, uint32_t P, const float* xyz, const f
     const float* src[6] = {rot, xyz, log_scale, opacity_logit, f_dc, f_rest};
     for (int q = 0; q < 6; ++q)
         if (P && kk[q] && src[q]) GLIC_CUDA_TRY(cudaMemcpyAsync(g[q], src[q], sizeof(float) * kk[q] * P, cudaMemcpyHostToDevice, m->stream));
+    MAP_TRY(launch_fill_anchors(m->anchor, 0, P, P, -1, m->stream));
     return install_map(m, P, 0);
 }
 
@@ -1249,7 +1283,7 @@ int glic_mapper_initialize_lidar(glic_mapper* m, int n, const float* points, con
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_pts, points, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, s));
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_col, colors, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, s));
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_dep, depth_rsp, sizeof(float) * n, cudaMemcpyHostToDevice, s));
-    return initialize_lidar_core(m, n, d_pts, d_col, d_dep, focal, sky_points, sky_radius, d_sky);
+    return initialize_lidar_core(m, n, d_pts, d_col, d_dep, focal, sky_points, sky_radius, d_sky, (int32_t)m->train.size() - 1);
 }
 
 int glic_mapper_sky_rows(glic_mapper* m, uint32_t* out) {
@@ -1282,7 +1316,7 @@ int glic_mapper_extend(glic_mapper* m, int n, const float* points, const float* 
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_pts, points, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, s));
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_col, colors, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, s));
     GLIC_CUDA_TRY(cudaMemcpyAsync(d_dep, depth_rsp, sizeof(float) * n, cudaMemcpyHostToDevice, s));
-    return extend_core(m, m->train.back(), n, d_pts, d_col, d_dep, ws);
+    return extend_core(m, m->train.back(), n, d_pts, d_col, d_dep, ws, (int32_t)m->train.size() - 1);
 }
 
 int glic_mapper_enable_frames(glic_mapper* m, int select_every_k_frame, int sky_points, int sky_radius) {
@@ -1609,9 +1643,11 @@ int density_step(glic_mapper* m, const glic_density_params& p, bool densify, int
             MAP_TRY(set_capacity(m, std::max<uint32_t>((uint32_t)rows, 2 * m->Pcap)));
         }
         Dev<float> spare, spare_stats[3];
+        Dev<int32_t> spare_anchor;
         const bool move_stats = !densify && m->dens_on;
         const size_t bytes = arena_floats(m, m->Pcap) * sizeof(float);
         MAP_TRY(spare.allocate(bytes));
+        MAP_TRY(spare_anchor.allocate((size_t)m->Pcap * 4));
         if (move_stats)
             for (Dev<float>& b : spare_stats) MAP_TRY(b.allocate((size_t)m->Pcap * 4));
         GLIC_CUDA_TRY(cudaMemsetAsync(spare, 0, bytes, s));
@@ -1621,6 +1657,9 @@ int density_step(glic_mapper* m, const glic_density_params& p, bool densify, int
             MAP_TRY(launch_gather_rows(*arena, spare, m->Pcap, m->M, written, arena == &m->params ? (uint32_t)rows : kept, idx, s));
             std::swap(*arena, spare);
         }
+        // the anchors follow the params gather: every result row, clones and split children from their parents
+        MAP_TRY(launch_gather_words(m->anchor, spare_anchor, written, (uint32_t)rows, idx, s));
+        std::swap(m->anchor, spare_anchor);
         MAP_TRY(launch_densify_children(m->params, m->Pcap, m->M, kept + cloned, split, m->extend_ws, P, n_split, m->cfg.seed, m->dens_calls, s));
         if (move_stats) {                                  // the statistics move with their rows (and their spares are zero)
             Buf* stats[3] = {&m->dens_accum, &m->dens_denom, &m->dens_maxr};
@@ -2031,6 +2070,58 @@ int extract_mesh(glic_mapper* m, const glic_mesh_params& p, glic_mesh_counts* ou
     return GLIC_OK;
 }
 
+// ---- pose corrections (glic_mapper_correct_poses) ----------------------------------------------------------------------------
+// After the checks: the records, one allocation (a failure changes nothing), the row pass, the keyframes.
+int correct_poses(glic_mapper* m, int n, const glic_pose_correction* c, uint32_t* moved) {
+    cudaStream_t s = m->stream;
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    MAP_TRY(poll_ring(m, true));
+    const size_t nt = m->train.size();
+    std::vector<glic_rigid_correction> table(nt);
+    for (glic_rigid_correction& r : table) r.q[0] = CORRECTION_NONE;
+    std::vector<int> corrected;                          // the listed training keyframes, in list order
+    for (int i = 0; i < n; ++i) {
+        if (!c[i].is_train) continue;
+        const Keyframe& kf = m->train[c[i].index];
+        MAP_TRY(glic_pose_correction_record(kf.R_wc, kf.t_wc, c[i].R_wc, c[i].t_wc, m->D, &table[c[i].index]));
+        corrected.push_back(c[i].index);
+    }
+    // device: the table indexed by keyframe | the moved-row count
+    Carver cv(nullptr);
+    cv.take<glic_rigid_correction>(nt); cv.take<uint32_t>(1);
+    Buf buf;
+    MAP_TRY(buf.allocate(cv.total()));
+    cv = Carver(buf.raw());
+    glic_rigid_correction* d_table = cv.take<glic_rigid_correction>(nt);
+    uint32_t* d_moved = cv.take<uint32_t>(1);
+    if (nt) GLIC_CUDA_TRY(cudaMemcpyAsync(d_table, table.data(), nt * sizeof(glic_rigid_correction), cudaMemcpyHostToDevice, s));
+    GLIC_CUDA_TRY(cudaMemsetAsync(d_moved, 0, sizeof(uint32_t), s));
+    if (!corrected.empty()) MAP_TRY(launch_correct_rows(m->D, m->P, m->Pcap, m->params, m->anchor, d_table, (int)nt, d_moved, s));
+    if (m->pose_on) {                                    // the refined masters move with their keyframes, MAX_SLOTS per launch
+        for (size_t first = 0; first < corrected.size(); first += MAX_SLOTS) {
+            PoseBatch b{};
+            const int S = (int)std::min<size_t>(MAX_SLOTS, corrected.size() - first);
+            for (int sl = 0; sl < S; ++sl) { b.kf[sl] = corrected[first + sl]; b.cam[sl] = m->train[b.kf[sl]].cam_dev; }
+            float fov2[2];
+            proj_matrix(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, b.Pm, fov2);
+            pose_correct_kernel<<<1, MAX_SLOTS, 0, s>>>(S, b, d_table, m->pose_T, m->pose_f);
+            GLIC_LAUNCH_CHECK();
+        }
+    }
+    // the given poses; the camera blocks of keyframes without a refined master are rebuilt from them as make_keyframe builds them
+    for (int i = 0; i < n; ++i) {
+        Keyframe& kf = (c[i].is_train ? m->train : m->test)[c[i].index];
+        std::memcpy(kf.R_wc, c[i].R_wc, sizeof(kf.R_wc)); std::memcpy(kf.t_wc, c[i].t_wc, sizeof(kf.t_wc));
+        config_camera_block(m, kf.R_wc, kf.t_wc, kf.cam);
+        if (!(c[i].is_train && m->pose_on)) GLIC_CUDA_TRY(cudaMemcpyAsync(kf.cam_dev, kf.cam.view, 36 * sizeof(float), cudaMemcpyHostToDevice, s));
+    }
+    uint32_t count = 0;
+    GLIC_CUDA_TRY(cudaMemcpyAsync(&count, d_moved, sizeof(count), cudaMemcpyDeviceToHost, s));
+    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
+    if (moved) *moved = count;
+    return GLIC_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -2329,6 +2420,39 @@ int glic_mapper_pose_set(glic_mapper* m, int index, const float* R_wc9, const fl
 
 int glic_mapper_pose_adam_state(glic_mapper* m, int index, float* exp_avg6, float* exp_avg_sq6, int* step) {
     return keyframe_adam_state(m, true, index, exp_avg6, exp_avg_sq6, step, "mapper_pose_adam_state");
+}
+
+int glic_mapper_anchors(glic_mapper* m, int32_t* out) {
+    if (!m || !out) { set_error("mapper_anchors: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    if (m->P) GLIC_CUDA_TRY(cudaMemcpy(out, m->anchor, (size_t)m->P * 4, cudaMemcpyDeviceToHost));
+    return GLIC_OK;
+}
+
+int glic_mapper_set_anchors(glic_mapper* m, const int32_t* in) {
+    if (!m || (!in && m->P)) { set_error("mapper_set_anchors: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const int32_t n = (int32_t)m->train.size();
+    for (uint32_t i = 0; i < m->P; ++i)
+        if (in[i] < -1 || in[i] >= n) { set_error("mapper_set_anchors: an anchor is neither -1 nor a training keyframe index"); return GLIC_ERR_INVALID_ARGUMENT; }
+    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    if (m->P) GLIC_CUDA_TRY(cudaMemcpy(m->anchor, in, (size_t)m->P * 4, cudaMemcpyHostToDevice));
+    return GLIC_OK;
+}
+
+int glic_mapper_correct_poses(glic_mapper* m, int n, const glic_pose_correction* c, uint32_t* moved) {
+    if (!m || n < 0 || (n > 0 && !c)) { set_error("mapper_correct_poses: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
+    std::vector<char> seen_train(m->train.size(), 0), seen_test(m->test.size(), 0);
+    for (int i = 0; i < n; ++i) {
+        const Keyframe* kf = nullptr;
+        MAP_TRY(keyframe_at(m, c[i].is_train, c[i].index, "mapper_correct_poses", kf));
+        MAP_TRY(pose_check(c[i].R_wc, c[i].t_wc, "mapper_correct_poses"));
+        char& seen = (c[i].is_train ? seen_train : seen_test)[c[i].index];
+        if (seen) { set_error("mapper_correct_poses: a keyframe is listed twice"); return GLIC_ERR_INVALID_ARGUMENT; }
+        seen = 1;
+    }
+    if (moved) *moved = 0;
+    if (n == 0) return GLIC_OK;
+    return correct_poses(m, n, c, moved);
 }
 
 int glic_mapper_align(glic_mapper* m, int is_train, int index, const glic_align_params* p, glic_align_result* out, float* rgb_host) {

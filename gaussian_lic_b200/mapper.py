@@ -41,6 +41,39 @@ def camera_block(W, H, fx, fy, cx, cy, R_wc, t_wc):
                 tanfovy=float(o[36]), lims=o[37:41].copy())
 
 
+def _f32x(a, n):
+    return (C.c_float * n)(*[float(x) for x in np.asarray(a, np.float32).reshape(n)])
+
+
+def _sh_blocks(sh, degree):
+    """the band matrices A_1 .. A_degree of a record's sh[83], as float64 arrays"""
+    out, off = [], 0
+    for l in range(1, 4):
+        n = 2 * l + 1
+        if l <= degree:
+            out.append(np.array(sh[off:off + n * n], np.float64).reshape(n, n))
+        off += n * n
+    return out
+
+
+def pose_correction_record(R_old, t_old, R_new, t_new, degree=3):
+    """glic_pose_correction_record: the rigid correction from a keyframe's old pose to its new one (R_wc [3,3], t_wc [3], taken
+    as float32).  Returns dict R [3,3], t [3], q [4] (r, x, y, z) float64 and sh, the list of band matrices A_1 .. A_degree."""
+    r = capi.RigidCorrection()
+    capi.check(capi.lib.glic_pose_correction_record(_f32x(R_old, 9), _f32x(t_old, 3), _f32x(R_new, 9), _f32x(t_new, 3), int(degree),
+                                                    C.byref(r)), "pose_correction_record")
+    return dict(R=np.array(r.R[:], np.float64).reshape(3, 3), t=np.array(r.t[:], np.float64), q=np.array(r.q[:], np.float64),
+                sh=_sh_blocks(r.sh, degree))
+
+
+def sh_rotation(q, degree=3):
+    """glic_sh_rotation: the band matrices A_1 .. A_degree of R(q) for a unit quaternion q = (r, x, y, z) (float64)."""
+    qq = (C.c_double * 4)(*[float(x) for x in np.asarray(q, np.float64).reshape(4)])
+    out = (C.c_double * 83)()
+    capi.check(capi.lib.glic_sh_rotation(qq, int(degree), out), "sh_rotation")
+    return _sh_blocks(out, degree)
+
+
 class Mapper:
     def __init__(self, W, H, fx, fy, cx, cy, sh_degree=3, capacity=0, max_iters=100, seed=0, rank=0, world=1, views_per_rank=1,
                  **lrs):
@@ -275,6 +308,32 @@ class Mapper:
         m1, m2, t = (C.c_float * 6)(), (C.c_float * 6)(), C.c_int()
         capi.check(capi.lib.glic_mapper_pose_adam_state(self._h, int(index), m1, m2, C.byref(t)), "mapper_pose_adam_state")
         return np.array(m1[:], np.float32), np.array(m2[:], np.float32), int(t.value)
+
+    def anchors(self):
+        """anchor [P] int32: the training keyframe each row moves with under correct_poses, or -1 (never moves)."""
+        P = int(self.stats().num_gaussians)
+        out = np.zeros(max(P, 1), np.int32)
+        capi.check(capi.lib.glic_mapper_anchors(self._h, out.ctypes.data_as(C.c_void_p)), "mapper_anchors")
+        return out[:P]
+
+    def set_anchors(self, anchors):
+        """Overwrite every row's anchor (-1, or a training keyframe index); anything else is refused and nothing changes."""
+        a = np.ascontiguousarray(anchors, dtype=np.int32).reshape(-1)
+        if a.shape[0] != int(self.stats().num_gaussians):
+            raise ValueError("set_anchors needs one anchor per row")
+        capi.check(capi.lib.glic_mapper_set_anchors(self._h, a.ctypes.data_as(C.c_void_p)), "mapper_set_anchors")
+
+    def correct_poses(self, corrections):
+        """Move keyframes to corrected poses and the rows anchored to them with them (glic_mapper_correct_poses).
+        corrections: a list of (is_train, index, R_wc [3,3], t_wc [3]).  Returns the number of rows moved."""
+        arr = (capi.PoseCorrection * max(len(corrections), 1))()
+        for e, (is_train, index, R, t) in zip(arr, corrections):
+            e.is_train, e.index = int(bool(is_train)), int(index)
+            e.R_wc[:] = [float(x) for x in np.asarray(R, np.float32).reshape(9)]
+            e.t_wc[:] = [float(x) for x in np.asarray(t, np.float32).reshape(3)]
+        moved = C.c_uint32()
+        capi.check(capi.lib.glic_mapper_correct_poses(self._h, len(corrections), arr, C.byref(moved)), "mapper_correct_poses")
+        return int(moved.value)
 
     def align(self, index, train=False, iterations=100, lr_translation=1e-3, lr_rotation=1e-3, exposure_lr=0.0, split=False,
               image=False):

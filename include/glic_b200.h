@@ -1162,6 +1162,91 @@ GLIC_API int glic_mapper_mesh_get(glic_mapper* m, glic_mesh_counts* counts, floa
 GLIC_API int glic_mapper_save_mesh(glic_mapper* m, const char* path);
 
 /* ---------------------------------------------------------------------------------------
+ * Pose corrections: moving the map with corrected keyframe poses (loop closure, a smoother's
+ * revision, a re-anchored trajectory).
+ *
+ * Anchors.  Every row of the map carries anchor[i]: the index of a training keyframe, or -1 (the row never moves).  Rows made by
+ * the glic_mapper_add_frame hand-off (initialize or extend) take the index of the training keyframe handed off (under
+ * glic_mapper_add_frame_masked too: it is the keyframe pushed right after the hand-off); rows of glic_mapper_extend and the LiDAR
+ * rows of glic_mapper_initialize_lidar take the newest training keyframe, or -1 when there is none; skybox rows and the rows of
+ * glic_mapper_initialize take -1.  Growth keeps the column; every compaction (prune, prune_unseen, densify, densify_and_prune,
+ * the density schedule) gathers it with the arenas, so clones and split children take their parent's anchor.  Anchors are not in
+ * glic_mapper_save_map's file.  glic_mapper_anchors copies anchor[0 .. P) to host memory; glic_mapper_set_anchors overwrites it
+ * from host memory (for maps not built through extend, say a PLY loaded by the caller): every value must be -1 or a training
+ * keyframe index in range, otherwise GLIC_ERR_INVALID_ARGUMENT and nothing changes.
+ *
+ * The correction record of one keyframe, float64, computed on the host from its old and its new pose (R_wc row-major, t_wc, the
+ * floats glic_keyframe takes); every operation below rounds once (host code is built without FMA):
+ *   R = dR = R_new R_old^T:   R[3i+j] = (R_new[3i] R_old[3j] + R_new[3i+1] R_old[3j+1]) + R_new[3i+2] R_old[3j+2]
+ *   t = t_new - dR t_old:     t[i] = t_new[i] - ((R[3i] t_old[0] + R[3i+1] t_old[1]) + R[3i+2] t_old[2])
+ *   q = (r, x, y, z), the unit quaternion of dR in the convention of R(q) = [1-2(yy+zz) 2(xy-rz) 2(xz+ry); 2(xy+rz) 1-2(xx+zz)
+ *       2(yz-rx); 2(xz-ry) 2(yz+rx) 1-2(xx+yy)] (Hamilton product: R(a (x) b) = R(a) R(b)).  With tr = (R0 + R4) + R8, the first
+ *       strictly largest of (tr, R0, R4, R8) picks the branch (a tie goes to the earlier one):
+ *         tr: r = sqrt(1 + tr) / 2,           s = 0.25 / r, x = (R7 - R5) s, y = (R2 - R6) s, z = (R3 - R1) s
+ *         R0: x = sqrt(((1 + R0) - R4) - R8) / 2, s = 0.25 / x, r = (R7 - R5) s, y = (R1 + R3) s, z = (R2 + R6) s
+ *         R4: y = sqrt(((1 - R0) + R4) - R8) / 2, s = 0.25 / y, r = (R2 - R6) s, x = (R1 + R3) s, z = (R5 + R7) s
+ *         R8: z = sqrt(((1 - R0) - R4) + R8) / 2, s = 0.25 / z, r = (R3 - R1) s, x = (R2 + R6) s, y = (R5 + R7) s
+ *       then q is divided by n = sqrt(((r r + x x) + y y) + z z), and negated when r < 0, or when r == 0 and the first non-zero of
+ *       (x, y, z) is negative (r = +0 after the sign rule).
+ *   sh = the band rotation matrices of R(q) (glic_sh_rotation(q)): A_1 (3x3) at sh[0], A_2 (5x5) at sh[9], A_3 (7x7) at sh[34],
+ *       row-major, in this library's SH-rest order and signs; entries of bands above `degree` are 0.
+ * glic_sh_rotation(q, degree, out), the band-matrix builder of the record, is also exported on its own: it gives the matrices of any
+ * unit quaternion, so a caller (or a test) can check them, or rotate SH coefficients it holds, without going through two poses.  For a
+ * unit q, A_l[m][n] = integral over the unit sphere of b_m(d) b_n(R(q)^T d), so that
+ * sum_m (A_l c)_m b_m(d) = sum_n c_n b_n(R(q)^T d) for every unit d and coefficient vector c of band l: the colour a moved splat
+ * shows towards R(q) d is the colour it showed towards d.  b_k are the SH-rest basis polynomials of the renderer (degree 1: -c1 y,
+ * c1 z, -c1 x, then degree 2 and 3 in the same order) with their constants in float64.  The integral is a product quadrature
+ * exact for polynomials of degree <= 7 (4-point Gauss-Legendre in z times 8 equally spaced azimuths), so A_l is exact up to
+ * rounding.  It is built from R(q) rather than dR because dR, the product of two float rotations, is orthonormal only to float
+ * precision; R(q) is the rotation the row's quaternion gets.
+ *
+ * glic_mapper_correct_poses(m, n, c, moved): c[0 .. n) each give the corrected pose of one keyframe, training (is_train != 0) or
+ * held-out.  Checked before anything changes (GLIC_ERR_INVALID_ARGUMENT, nothing changed): n >= 0, c non-NULL when n > 0, every
+ * index in range, every pose a rotation with finite entries (the test of glic_mapper_pose_set), no keyframe listed twice.  n = 0
+ * is a no-op.  The call drains the iteration pipeline, then:
+ *   1. for every listed training keyframe k, the record from its current given pose (the one last passed to add or to
+ *      glic_mapper_pose_set; not a refined pose) to the new one;
+ *   2. one pass over rows [0, P): a row whose anchor is a corrected keyframe gets, in float64 with one rounding per operation and
+ *      one final rounding to float,
+ *        xyz'_i = fl32(((R[3i] x + R[3i+1] y) + R[3i+2] z) + t[i]),
+ *        rot' = fl32(q (x) rot) on the stored (unnormalised) quaternion: r' = ((qr rr - qx rx) - qy ry) - qz rz,
+ *          x' = ((qr rx + qx rr) + qy rz) - qz ry, y' = ((qr ry - qx rz) + qy rr) + qz rx, z' = ((qr rz + qx ry) - qy rx) + qz rr,
+ *        every band l and channel ch of the SH rest (stored [M][3]): c'_m = fl32(sum_n A_l[m][n] c_n), summed from n = 0 up,
+ *      and dc, log-scale and opacity unchanged.  Every other row and rows [P, capacity) are not written.  The Adam moments of
+ *      every row stay as they are (as under glic_mapper_pose_set);
+ *   3. every listed keyframe's given pose becomes the new one.  Without pose refinement (and for held-out keyframes) its camera
+ *      block is rebuilt from it, exactly as at glic_mapper_add_keyframe.  With pose refinement a training keyframe's float64 master
+ *      becomes T_cw' = T_cw dT^-1 (R_cw' = R_cw dR^T, t_cw' = t_cw - R_cw' t), which keeps the refinement's offset in the
+ *      keyframe's own frame, and its float pose and device camera block are re-derived from it by the pose step's code; its Adam
+ *      state is kept.
+ * *moved (may be NULL): the number of rows written.  Exposure, masks, the densification statistics, contribution scores and the
+ * last mesh are left as they are (extract the mesh again).  The update is elementwise, so replicas that make the same call stay
+ * bit-identical without an exchange, and deterministic training stays bit-reproducible.  Memory: one table of
+ * sizeof(glic_rigid_correction) per training keyframe, released when the call returns; a failed allocation returns GLIC_ERR_CUDA
+ * with the mapper as it was.
+ * Not covered: computing the corrections, blending several keyframes' corrections per row, moving the skybox, transforming
+ * Adam moments, re-seeding scan points still pending from frames not yet handed off, anchors in the PLY.
+ * ------------------------------------------------------------------------------------- */
+typedef struct glic_rigid_correction {
+    double R[9];                   /* dR, row-major */
+    double t[3];
+    double q[4];                   /* (r, x, y, z), unit, r >= 0 */
+    double sh[9 + 25 + 49];        /* A_1 | A_2 | A_3, row-major */
+} glic_rigid_correction;
+typedef struct glic_pose_correction {
+    int is_train;                  /* non-zero: a training keyframe; 0: held-out */
+    int index;
+    float R_wc[9];                 /* the corrected pose, as glic_keyframe takes it */
+    float t_wc[3];
+} glic_pose_correction;
+GLIC_API int glic_pose_correction_record(const float* R_old /*[9]*/, const float* t_old /*[3]*/, const float* R_new /*[9]*/,
+                                         const float* t_new /*[3]*/, int degree, glic_rigid_correction* out);
+GLIC_API int glic_sh_rotation(const double* q /*[4], unit*/, int degree, double* out /*[83]*/);
+GLIC_API int glic_mapper_anchors(glic_mapper* m, int32_t* out /*[P]*/);
+GLIC_API int glic_mapper_set_anchors(glic_mapper* m, const int32_t* in /*[P]*/);
+GLIC_API int glic_mapper_correct_poses(glic_mapper* m, int n, const glic_pose_correction* c, uint32_t* moved /* may be NULL */);
+
+/* ---------------------------------------------------------------------------------------
  * Stage timing (cudaEvent pairs recorded on the launching stream around each stage; off by
  * default).  glic_profile_enable(1) starts recording and resets the accumulators;
  * glic_profile_read() synchronises the recorded events and returns, per stage, the summed
