@@ -313,16 +313,16 @@ inline uint32_t higher_msb(uint32_t n) {
 // order is the same either way (a stable sort on a bit every key has clear).
 inline int tile_sort_bits(int T) { return (int)higher_msb((uint32_t)(T - 1)); }
 
-// Digit split of the LSD radix sorts (radix_sort.cu): ceil(end_bit / max_bits) passes, the key bits spread evenly over them
+// Digit split of the LSD radix sorts (radix_sort.cu): ceil(end_bit / 8) passes, the key bits spread evenly over them
 // (the wider digits first), so that no pass carries digits no key can have: 13 tile bits -> 7 + 6, 16 -> 8 + 8, 32 -> 4 x 8,
 // 45 -> 8,8,8,7,7,7.  Producer kernels that build the sort's histograms count the same digits.
-__host__ __device__ inline int sort_passes(int end_bit, int max_bits = 8) { return (end_bit + max_bits - 1) / max_bits; }
-__host__ __device__ inline int sort_pass_bits(int end_bit, int pass, int max_bits = 8) {
-    const int p = sort_passes(end_bit, max_bits);
+__host__ __device__ inline int sort_passes(int end_bit) { return (end_bit + 7) / 8; }
+__host__ __device__ inline int sort_pass_bits(int end_bit, int pass) {
+    const int p = sort_passes(end_bit);
     return end_bit / p + (pass < end_bit % p ? 1 : 0);
 }
-__host__ __device__ inline int sort_pass_shift(int end_bit, int pass, int max_bits = 8) {
-    const int p = sort_passes(end_bit, max_bits);
+__host__ __device__ inline int sort_pass_shift(int end_bit, int pass) {
+    const int p = sort_passes(end_bit);
     return pass * (end_bit / p) + (pass < end_bit % p ? pass : end_bit % p);
 }
 // Passes of the tile sort: its sorted pairs end in buffer (passes & 1) of the ping-pong pair.
@@ -415,8 +415,8 @@ int launch_sort_pairs32(int64_t n, int end_bit, uint32_t* keys[2], uint32_t* val
 // A producer kernel may build the digit histograms itself: sort_prepare() zeroes the temp block, the producer adds one count
 // per key and pass into sort_hist(temp)[pass * 256 + digit] (digit = bits [sort_pass_shift, + sort_pass_bits) of the key),
 // and the sort is launched with hist_ready = true.
-int sort_prepare(int64_t n, int end_bit, void* temp, cudaStream_t s, int digit_bits = 8);
-size_t sort_prepare_bytes(int64_t n, int end_bit, int digit_bits = 8);     // the bytes sort_prepare zeroes
+int sort_prepare(int64_t n, int end_bit, void* temp, cudaStream_t s);
+size_t sort_prepare_bytes(int64_t n, int end_bit);     // the bytes sort_prepare zeroes
 uint32_t* sort_hist(void* temp);
 // R: host-side count or capacity; r_dev (optional): device-side true count.  img.ranges must be zero; *sorted_in_b is set to cur
 int launch_tile_ranges(int64_t R, const GeomHeader* ghdr, const uint32_t* tile_keys_sorted, int T, ImageState img, bool buckets,

@@ -125,10 +125,12 @@ unsigned long long p2p_timeout_ns() {
     return ns;
 }
 
+constexpr int P2P_CTAS_PER_SM = 2;        // CTAs of p2p_reduce_kernel per SM, at most
+
 template <int WORLD, int UNROLL>
-void launch_reduce(const PeerBufs& pb, size_t lo4, size_t hi4, size_t vis_off, size_t vlo4, size_t vhi4, int ctas_per_sm, cudaStream_t s) {
+void launch_reduce(const PeerBufs& pb, size_t lo4, size_t hi4, size_t vis_off, size_t vlo4, size_t vhi4, cudaStream_t s) {
     const size_t work = std::max((hi4 - lo4 + UNROLL - 1) / UNROLL, vhi4 - vlo4);
-    const unsigned blocks = (unsigned)std::max<size_t>(1, std::min<size_t>((work + 511) / 512, (size_t)NUM_SMS * ctas_per_sm));
+    const unsigned blocks = (unsigned)std::max<size_t>(1, std::min<size_t>((work + 511) / 512, (size_t)NUM_SMS * P2P_CTAS_PER_SM));
     p2p_reduce_kernel<WORLD, UNROLL><<<blocks, 512, 0, s>>>(pb, lo4, hi4, vis_off, vlo4, vhi4, 1.0f / (float)WORLD);
 }
 
@@ -239,15 +241,10 @@ int glic_p2p_allreduce_mean(int rank, int world, void* const* bufs_host, size_t 
     { StageTimer _t(GLIC_STAGE_ALLREDUCE, s);
       p2p_barrier_kernel<<<1, 32, 0, s>>>(pb, rank, world, flag_off, p2p_timeout_ns());         // every peer's gradients are complete
       GLIC_LAUNCH_CHECK();
-      static const int ctas = getenv("GLIC_P2P_CTAS") ? atoi(getenv("GLIC_P2P_CTAS")) : 2;   // tuning knob
-      static const int unr = getenv("GLIC_P2P_UNROLL") ? atoi(getenv("GLIC_P2P_UNROLL")) : 4;
-#define GLIC_P2P_CASE(WD) case WD: if (unr >= 4 && WD <= 4) launch_reduce<WD, 4>(pb, lo4, hi4, f_bytes, vlo4, vhi4, ctas, s); \
-                                   else if (unr >= 2) launch_reduce<WD, 2>(pb, lo4, hi4, f_bytes, vlo4, vhi4, ctas, s); \
-                                   else launch_reduce<WD, 1>(pb, lo4, hi4, f_bytes, vlo4, vhi4, ctas, s); break;
-      switch (world) {
-          GLIC_P2P_CASE(1) GLIC_P2P_CASE(2) GLIC_P2P_CASE(3) GLIC_P2P_CASE(4) GLIC_P2P_CASE(5) GLIC_P2P_CASE(6) GLIC_P2P_CASE(7) GLIC_P2P_CASE(8)
-      }
-#undef GLIC_P2P_CASE
+      // UNROLL 16-byte loads in flight per peer: 4 up to 4 ranks, 2 above (at most 16 per thread)
+#define GLIC_P2P_MEAN(WD) case WD: launch_reduce<WD, WD <= 4 ? 4 : 2>(pb, lo4, hi4, f_bytes, vlo4, vhi4, s); break;
+      switch (world) { GLIC_P2P_MEAN(1) GLIC_P2P_MEAN(2) GLIC_P2P_MEAN(3) GLIC_P2P_MEAN(4) GLIC_P2P_MEAN(5) GLIC_P2P_MEAN(6) GLIC_P2P_MEAN(7) GLIC_P2P_MEAN(8) }
+#undef GLIC_P2P_MEAN
       GLIC_LAUNCH_CHECK();
       p2p_barrier_kernel<<<1, 32, 0, s>>>(pb, rank, world, flag_off, p2p_timeout_ns());      // every slice has been written everywhere
       GLIC_LAUNCH_CHECK(); }
@@ -302,7 +299,7 @@ int glic_p2p_reduce_adam(int rank, int world, void* const* bufs_host, uint32_t P
     { StageTimer _t(GLIC_STAGE_ALLREDUCE, s);
       p2p_barrier_kernel<<<1, 32, 0, s>>>(pb, rank, world, flag_off, p2p_timeout_ns());          // every peer's gradients and visibility are complete
       GLIC_LAUNCH_CHECK();
-#define GLIC_P2P_VIS(WD) case WD: launch_reduce<WD, 1>(pb, 0, 0, f_bytes, vlo4, vhi4, 2, s); break;
+#define GLIC_P2P_VIS(WD) case WD: launch_reduce<WD, 1>(pb, 0, 0, f_bytes, vlo4, vhi4, s); break;
       switch (world) { GLIC_P2P_VIS(1) GLIC_P2P_VIS(2) GLIC_P2P_VIS(3) GLIC_P2P_VIS(4) GLIC_P2P_VIS(5) GLIC_P2P_VIS(6) GLIC_P2P_VIS(7) GLIC_P2P_VIS(8) }
 #undef GLIC_P2P_VIS
       GLIC_LAUNCH_CHECK();

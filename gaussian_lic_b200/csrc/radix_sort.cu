@@ -18,7 +18,6 @@
 // Algorithmic HBM traffic: (8 + 24*passes) B per pair (152 B @ 45 bits).
 #include "common.cuh"
 #include <algorithm>
-#include <cstdlib>
 
 namespace glic {
 
@@ -26,8 +25,14 @@ size_t sort_temp_bytes(int64_t n);
 
 namespace {
 
-constexpr int RADIX_BITS_MAX = 9;                      // the 64-bit-key sort takes 9-bit digits when that saves a pass (45 bits: 5 instead of 6)
-constexpr int RADIX_MAX = 1 << RADIX_BITS_MAX;
+// Widest digit of a pass.  A pass is bound by the warp-synchronous ranking (one ballot per digit bit and item), not by its
+// 24 B/pair of HBM traffic, so 9-bit digits cost more than the pass they save on 64-bit keys (measured, NOTES.md).
+constexpr int RADIX_BITS = 8;
+constexpr int RADIX = 1 << RADIX_BITS;
+// Words the temp block reserves per pass for the histograms and, per CTA, for the status words: 512, twice the bins of
+// the widest digit.  The reservation sets sort_temp_bytes and, through it, the workspace sizes and the binning capacity
+// a workspace yields.
+constexpr int RADIX_RESERVED = 512;
 constexpr int SORT_THREADS = 256;
 constexpr int SORT_WARPS = SORT_THREADS / 32;
 constexpr int SORT_ITEMS_BIG = 16;                     // 4096 pairs per CTA: the R-sized tile sort
@@ -40,19 +45,18 @@ constexpr uint32_t FLAG_PREFIX = 2u << 30;
 constexpr uint32_t VALUE_MASK = (1u << 30) - 1;
 
 struct SortTemp {
-    uint32_t* hist;     // [MAX_PASSES][1 << max digit bits]  digit histograms -> exclusive offsets
+    uint32_t* hist;     // [MAX_PASSES][RADIX]  digit histograms -> exclusive offsets (MAX_PASSES * RADIX_RESERVED words reserved)
     uint32_t* tickets;  // [MAX_PASSES]
     uint32_t* status;   // per pass p: [blocks][1 << sort_pass_bits(p)], passes packed back to back
 };
 
 __host__ inline int sort_items(int64_t n) { return n < SORT_SMALL_LIMIT ? SORT_ITEMS_SMALL : SORT_ITEMS_BIG; }
 __host__ inline int64_t sort_blocks(int64_t n) { const int64_t tile = (int64_t)SORT_THREADS * sort_items(n); return (n + tile - 1) / tile; }
-__host__ inline int64_t sort_blocks_big(int64_t n) { const int64_t tile = (int64_t)SORT_THREADS * SORT_ITEMS_BIG; return (n + tile - 1) / tile; }
 
 // live digits of all passes together: the status words one CTA needs over the whole sort
-__host__ inline int64_t sort_live_digits(int end_bit, int max_bits) {
+__host__ inline int64_t sort_live_digits(int end_bit) {
     int64_t d = 0;
-    for (int p = 0; p < sort_passes(end_bit, max_bits); ++p) d += (int64_t)1 << sort_pass_bits(end_bit, p, max_bits);
+    for (int p = 0; p < sort_passes(end_bit); ++p) d += (int64_t)1 << sort_pass_bits(end_bit, p);
     return d;
 }
 
@@ -60,7 +64,7 @@ __host__ inline SortTemp carve_sort_temp(void* temp) {
     char* p = static_cast<char*>(temp);
     SortTemp t;
     t.hist = reinterpret_cast<uint32_t*>(p);
-    t.tickets = t.hist + MAX_PASSES * RADIX_MAX;
+    t.tickets = t.hist + MAX_PASSES * RADIX_RESERVED;
     t.status = t.tickets + 32;
     return t;
 }
@@ -81,12 +85,11 @@ __device__ __forceinline__ void cp_async4(void* smem_dst, const void* gmem_src) 
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // ---- 1. all-pass histogram --------------------------------------------------------------
-template <typename KeyT, int RB>
+template <typename KeyT>
 __global__ void __launch_bounds__(256)
 sort_histogram_kernel(const KeyT* __restrict__ keys, int64_t n, const unsigned int* __restrict__ n_dev, int passes, int end_bit,
                       uint32_t* __restrict__ hist) {
     pdl_enter();
-    constexpr int RADIX = 1 << RB;
     if (n_dev) n = min(n, (int64_t)*n_dev);
     __shared__ uint32_t sh[MAX_PASSES * RADIX];
     for (int i = threadIdx.x; i < passes * RADIX; i += blockDim.x) sh[i] = 0;
@@ -95,8 +98,8 @@ sort_histogram_kernel(const KeyT* __restrict__ keys, int64_t n, const unsigned i
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
         const KeyT k = keys[i];
         for (int p = 0; p < passes; ++p) {
-            const int bits = sort_pass_bits(end_bit, p, RB);
-            const uint32_t d = (uint32_t)(k >> sort_pass_shift(end_bit, p, RB)) & ((1u << bits) - 1u);
+            const int bits = sort_pass_bits(end_bit, p);
+            const uint32_t d = (uint32_t)(k >> sort_pass_shift(end_bit, p)) & ((1u << bits) - 1u);
             atomicAdd(&sh[p * RADIX + d], 1u);
         }
     }
@@ -108,10 +111,10 @@ sort_histogram_kernel(const KeyT* __restrict__ keys, int64_t n, const unsigned i
 }
 
 // ---- 2. exclusive scan of each pass's bins --------------------------------------------
-__global__ void __launch_bounds__(RADIX_MAX) sort_scan_hist_kernel(uint32_t* __restrict__ hist) {
+__global__ void __launch_bounds__(RADIX_RESERVED) sort_scan_hist_kernel(uint32_t* __restrict__ hist) {
     pdl_enter();
-    __shared__ uint32_t warp_tot[RADIX_MAX / 32];
-    uint32_t* h = hist + blockIdx.x * blockDim.x;          // blockDim.x = bins of this sort's widest digit
+    __shared__ uint32_t warp_tot[RADIX_RESERVED / 32];
+    uint32_t* h = hist + blockIdx.x * blockDim.x;          // blockDim.x = RADIX: one pass's bins
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t v = h[tid];
     uint32_t incl = v;
@@ -128,10 +131,9 @@ __global__ void __launch_bounds__(RADIX_MAX) sort_scan_hist_kernel(uint32_t* __r
 }
 
 // ---- 3. one onesweep pass -------------------------------------------------------------------
-template <typename KeyT, int SORT_ITEMS, int RB>
+template <typename KeyT, int SORT_ITEMS>
 struct __align__(16) PassSmem {
     static constexpr int SORT_TILE = SORT_THREADS * SORT_ITEMS;
-    static constexpr int RADIX = 1 << RB;
     KeyT keys[SORT_TILE];
     uint32_t vals[SORT_TILE];
     uint32_t warp_cnt[SORT_WARPS][RADIX];
@@ -142,9 +144,9 @@ struct __align__(16) PassSmem {
     uint32_t block_id;
 };
 
-// RB: widest digit the kernel is built for (8, or 9 for the opt-in 64-bit variant); `bits` <= RB: this pass's digit width.
-// Only the 1 << bits live digits are counted, published and looked back on; `status` holds [blocks][1 << bits] words.
-template <typename KeyT, int SORT_ITEMS, int RB>
+// `bits` <= RADIX_BITS: this pass's digit width.  Only the 1 << bits live digits are counted, published and looked back on;
+// `status` holds [blocks][1 << bits] words.
+template <typename KeyT, int SORT_ITEMS>
 __global__ void __launch_bounds__(SORT_THREADS, SORT_ITEMS <= 4 ? 6 : (sizeof(KeyT) == 4 ? 4 : 3))
 onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restrict__ vals_in,
                      KeyT* __restrict__ keys_out, uint32_t* __restrict__ vals_out, int64_t n, const unsigned int* __restrict__ n_dev,
@@ -153,9 +155,8 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
     pdl_enter();
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr int SORT_TILE = SORT_THREADS * SORT_ITEMS;
-    constexpr int RADIX_BITS = RB, RADIX = 1 << RB;
-    constexpr int DPT = RADIX > SORT_THREADS ? RADIX / SORT_THREADS : 1;   // digits owned by one thread in the per-digit phase
-    PassSmem<KeyT, SORT_ITEMS, RB>& sm = *reinterpret_cast<PassSmem<KeyT, SORT_ITEMS, RB>*>(smem_raw);
+    static_assert(RADIX == SORT_THREADS, "the per-digit phase gives each thread one digit");
+    PassSmem<KeyT, SORT_ITEMS>& sm = *reinterpret_cast<PassSmem<KeyT, SORT_ITEMS>*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nd = 1 << bits;                               // live digits of this pass
     const uint32_t dmask = (uint32_t)nd - 1u;
@@ -186,13 +187,9 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
         if (wbase + j * 32 + lane < count) atomicAdd(&sm.tile_cnt[(uint32_t)(k[j] >> shift) & dmask], 1u);
     __syncthreads();
     // -- publish the tile's digit counts before ranking it: successors' look-backs need not wait for this CTA's ranking
-    uint32_t tot[DPT];
-#pragma unroll
-    for (int e = 0; e < DPT; ++e) {
-        const int d = tid * DPT + e;
-        tot[e] = d < nd ? sm.tile_cnt[d] : 0u;
-        if (d < nd) st_volatile(status + (size_t)block * nd + d, (block == 0 ? FLAG_PREFIX : FLAG_AGG) | tot[e]);
-    }
+    //    (thread t owns digit t here and in the per-digit phase)
+    const uint32_t tot = tid < nd ? sm.tile_cnt[tid] : 0u;
+    if (tid < nd) st_volatile(status + (size_t)block * nd + tid, (block == 0 ? FLAG_PREFIX : FLAG_AGG) | tot);
 
     // -- stable rank inside the warp's digit streams
     const uint32_t lt_mask = (1u << lane) - 1u;
@@ -203,7 +200,7 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
         const uint32_t d = (uint32_t)(k[j] >> shift) & dmask;
         const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
         uint32_t r = 0;
-        // peers from RB ballots, with no branch on `bits` (the bits past it are clear in every d and change nothing): the
+        // peers from RADIX_BITS ballots, with no branch on `bits` (the bits past it are clear in every d and change nothing): the
         // branch-free cascade measured faster than skipping the dead ballots.  Cost is independent of the digit
         // distribution; MATCH.ANY measured ~1.35x slower per pass on H100
         uint32_t bpeers = vmask;
@@ -226,25 +223,19 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
     }
     __syncthreads();
 
-    // -- per digit (thread t owns digits t*DPT .. t*DPT + DPT-1): warp bases, CTA-local placement, look-back
+    // -- per digit (thread t owns digit t): warp bases, CTA-local placement, look-back
     {
-        uint32_t mine = 0;
+        if (tid < nd) {
+            uint32_t t = 0;
 #pragma unroll
-        for (int e = 0; e < DPT; ++e) {
-            const int d = tid * DPT + e;
-            if (d < nd) {
-                uint32_t t = 0;
-#pragma unroll
-                for (int w = 0; w < SORT_WARPS; ++w) {
-                    const uint32_t c = sm.warp_cnt[w][d];
-                    sm.warp_cnt[w][d] = t;
-                    t += c;
-                }
+            for (int w = 0; w < SORT_WARPS; ++w) {
+                const uint32_t c = sm.warp_cnt[w][tid];
+                sm.warp_cnt[w][tid] = t;
+                t += c;
             }
-            mine += tot[e];
         }
         // CTA-local exclusive scan over digits (placement inside the staged tile)
-        uint32_t incl = mine;
+        uint32_t incl = tot;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
             const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
@@ -254,19 +245,16 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
         __syncthreads();
         uint32_t dbase = 0;
         for (int w = 0; w < warp; ++w) dbase += sm.warp_tot[w];
-        uint32_t excl = dbase + incl - mine;
-#pragma unroll
-        for (int e = 0; e < DPT; ++e) {
-            const int d = tid * DPT + e;
-            if (d >= nd) break;
-            sm.digit_excl[d] = excl;
+        const uint32_t excl = dbase + incl - tot;
+        if (tid < nd) {
+            sm.digit_excl[tid] = excl;
             // decoupled look-back for this digit (its aggregate went out before the ranking)
             uint32_t prev = 0;
             if (block > 0) {
                 int64_t b = block - 1;
                 unsigned spins = 0;
                 while (true) {
-                    const uint32_t s = ld_volatile(status + (size_t)b * nd + d);
+                    const uint32_t s = ld_volatile(status + (size_t)b * nd + tid);
                     const uint32_t f = s & ~VALUE_MASK;
                     if (f == 0) {
                         if (++spins > (1u << 26)) __trap();   // fail loudly rather than hang the GPU
@@ -276,10 +264,9 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
                     if (f == FLAG_PREFIX) break;
                     --b;
                 }
-                st_volatile(status + (size_t)block * nd + d, FLAG_PREFIX | (prev + tot[e]));
+                st_volatile(status + (size_t)block * nd + tid, FLAG_PREFIX | (prev + tot));
             }
-            sm.global_base[d] = digit_base[d] + prev - excl;
-            excl += tot[e];
+            sm.global_base[tid] = digit_base[tid] + prev - excl;
         }
     }
     __syncthreads();
@@ -326,13 +313,13 @@ onesweep_pass_kernel(const KeyT* __restrict__ keys_in, const uint32_t* __restric
 }  // namespace
 
 // zeroes the histograms, tickets and look-back status words of a sort of n pairs on bits [0, end_bit)
-size_t sort_prepare_bytes(int64_t n, int end_bit, int digit_bits) {
-    return n <= 0 ? 0 : sizeof(uint32_t) * (MAX_PASSES * RADIX_MAX + 32 + (size_t)sort_blocks(n) * sort_live_digits(end_bit, digit_bits));
+size_t sort_prepare_bytes(int64_t n, int end_bit) {
+    return n <= 0 ? 0 : sizeof(uint32_t) * (MAX_PASSES * RADIX_RESERVED + 32 + (size_t)sort_blocks(n) * sort_live_digits(end_bit));
 }
 
-int sort_prepare(int64_t n, int end_bit, void* temp, cudaStream_t s, int digit_bits) {
+int sort_prepare(int64_t n, int end_bit, void* temp, cudaStream_t s) {
     if (n <= 0) return GLIC_OK;
-    GLIC_CUDA_TRY(cudaMemsetAsync(temp, 0, sort_prepare_bytes(n, end_bit, digit_bits), s));
+    GLIC_CUDA_TRY(cudaMemsetAsync(temp, 0, sort_prepare_bytes(n, end_bit), s));
     return GLIC_OK;
 }
 
@@ -340,40 +327,28 @@ uint32_t* sort_hist(void* temp) { return static_cast<uint32_t*>(temp); }      //
 
 size_t sort_temp_bytes(int64_t n) {
     const size_t blocks = (size_t)sort_blocks(n > 0 ? n : 1);
-    return sizeof(uint32_t) * (MAX_PASSES * RADIX_MAX + 32 + (size_t)MAX_PASSES * blocks * RADIX_MAX) + 256;
+    return sizeof(uint32_t) * (MAX_PASSES * RADIX_RESERVED + 32 + (size_t)MAX_PASSES * blocks * RADIX_RESERVED) + 256;
 }
 
-template <typename KeyT, int ITEMS, int RB>
+template <typename KeyT, int ITEMS>
 static int run_passes(int64_t n, int passes, int end_bit, int64_t blocks, KeyT* keys[2], uint32_t* vals[2], const SortTemp& t, cudaStream_t s,
                       const unsigned int* n_dev) {
-    constexpr int BINS = 1 << RB;
     static bool attr_set[64] = {};
     if (first_use_on_device(attr_set)) {
-        GLIC_CUDA_TRY(cudaFuncSetAttribute(onesweep_pass_kernel<KeyT, ITEMS, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)sizeof(PassSmem<KeyT, ITEMS, RB>)));
+        GLIC_CUDA_TRY(cudaFuncSetAttribute(onesweep_pass_kernel<KeyT, ITEMS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)sizeof(PassSmem<KeyT, ITEMS>)));
     }
     int cur = 0;
     uint32_t* status = t.status;
     for (int p = 0; p < passes; ++p) {
-        const int bits = sort_pass_bits(end_bit, p, RB);
-        GLIC_LAUNCH_PDL(onesweep_pass_kernel<KeyT, ITEMS, RB>, (unsigned)blocks, SORT_THREADS, sizeof(PassSmem<KeyT, ITEMS, RB>), s,
-                        keys[cur], vals[cur], keys[cur ^ 1], vals[cur ^ 1], n, n_dev, sort_pass_shift(end_bit, p, RB), bits,
-                        t.hist + p * BINS, status, t.tickets + p);
+        const int bits = sort_pass_bits(end_bit, p);
+        GLIC_LAUNCH_PDL(onesweep_pass_kernel<KeyT, ITEMS>, (unsigned)blocks, SORT_THREADS, sizeof(PassSmem<KeyT, ITEMS>), s,
+                        keys[cur], vals[cur], keys[cur ^ 1], vals[cur ^ 1], n, n_dev, sort_pass_shift(end_bit, p), bits,
+                        t.hist + p * RADIX, status, t.tickets + p);
         status += (size_t)blocks << bits;     // each pass's status words cover its live digits only
         cur ^= 1;
     }
     return cur;
-}
-
-// Widest digit of a sort.  The pass kernel is generic (up to 8- or 9-bit digits; GLIC_SORT_DIGIT_BITS=9 selects the wider
-// one for 64-bit keys when it saves a pass), but 8 stays the default: a pass is bound by the warp-synchronous ranking (one
-// ballot per digit bit and item), not by its 24 B/pair of HBM traffic, so a wider digit costs more than the saved pass
-// returns.
-template <typename KeyT>
-static inline int sort_digit_bits(int end_bit) {
-    static const int want = getenv("GLIC_SORT_DIGIT_BITS") ? atoi(getenv("GLIC_SORT_DIGIT_BITS")) : 8;
-    if (want == 9 && sizeof(KeyT) == 8 && sort_passes(end_bit, 9) < sort_passes(end_bit, 8)) return 9;
-    return 8;
 }
 
 // hist_ready: the caller zeroed the temp block with sort_prepare() and a producer kernel already accumulated the digit
@@ -385,24 +360,19 @@ static int launch_sort_pairs_t(int64_t n, int end_bit, KeyT* keys[2], uint32_t* 
     if (end_bit < 1 || end_bit > (int)(8 * sizeof(KeyT))) { set_error("sort: end_bit out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (n >= (int64_t)VALUE_MASK) { set_error("sort: n too large"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (n <= 0) return 0;
-    const int rb = hist_ready ? 8 : sort_digit_bits<KeyT>(end_bit);
-    const int passes = sort_passes(end_bit, rb);
+    const int passes = sort_passes(end_bit);
     if (passes > MAX_PASSES) { set_error("sort: too many passes"); return GLIC_ERR_INVALID_ARGUMENT; }
     if (temp_bytes < sort_temp_bytes(n)) { set_error("sort: temp too small"); return GLIC_ERR_WORKSPACE; }
     const int64_t blocks = sort_blocks(n);
     SortTemp t = carve_sort_temp(temp);
     if (!hist_ready) {
-        if (int e = sort_prepare(n, end_bit, temp, s, rb)) return e;
+        if (int e = sort_prepare(n, end_bit, temp, s)) return e;
         int hist_blocks = (int)std::min<int64_t>((n + 256 * 16 - 1) / (256 * 16), (int64_t)NUM_SMS * 8);
-        GLIC_LAUNCH_PDL(rb == 9 ? sort_histogram_kernel<KeyT, 9> : sort_histogram_kernel<KeyT, 8>, hist_blocks, 256, 0, s,
-                        keys[0], n, n_dev, passes, end_bit, t.hist);
+        GLIC_LAUNCH_PDL(sort_histogram_kernel<KeyT>, hist_blocks, 256, 0, s, keys[0], n, n_dev, passes, end_bit, t.hist);
     }
-    GLIC_LAUNCH_PDL(sort_scan_hist_kernel, passes, 1 << rb, 0, s, t.hist);
-    if (rb == 9) {
-        if constexpr (sizeof(KeyT) == 8) return run_passes<KeyT, SORT_ITEMS_BIG, 9>(n, passes, end_bit, sort_blocks_big(n), keys, vals, t, s, n_dev);
-    }
-    return sort_items(n) == SORT_ITEMS_SMALL ? run_passes<KeyT, SORT_ITEMS_SMALL, 8>(n, passes, end_bit, blocks, keys, vals, t, s, n_dev)
-                                             : run_passes<KeyT, SORT_ITEMS_BIG, 8>(n, passes, end_bit, blocks, keys, vals, t, s, n_dev);
+    GLIC_LAUNCH_PDL(sort_scan_hist_kernel, passes, RADIX, 0, s, t.hist);
+    return sort_items(n) == SORT_ITEMS_SMALL ? run_passes<KeyT, SORT_ITEMS_SMALL>(n, passes, end_bit, blocks, keys, vals, t, s, n_dev)
+                                             : run_passes<KeyT, SORT_ITEMS_BIG>(n, passes, end_bit, blocks, keys, vals, t, s, n_dev);
 }
 
 int launch_sort_pairs(int64_t n, int end_bit, uint64_t* keys[2], uint32_t* vals[2], void* temp, size_t temp_bytes,

@@ -397,13 +397,15 @@ live_scan_kernel(int T, const uint32_t* __restrict__ max_contrib, uint32_t* __re
     if (threadIdx.x == 0) { hdr->num_live_buckets = total; hdr->bwd_ticket = 0; }
 }
 
-constexpr int BWD_WARPS = 4;              // warps per CTA; every warp owns one (live bucket, tile part) at a time
+constexpr int BWD_WARPS = 4;              // warps per CTA; every warp owns one live bucket at a time
+constexpr int BWD_ROWPAIRS = TILE / 2;    // row pairs of a tile: a lane owns one pixel of each
 
 // Backward of the blend, pixel-major inside a 32-splat bucket (replaces PerGaussianRenderCUDA, backward.cu:400-597).
 //
-// One warp per (LIVE bucket, tile part) in a persistent grid-stride loop; a part is RP consecutive row pairs of the 16x16
-// tile (RP = 8: whole tile, RP = 4: half), and lane l owns the RP pixels (column l & 15, rows 2j + (l >> 4)) of its part.  Every pixel restarts from the bucket's checkpoint (T, C) and walks the bucket's splats in list order
-// exactly like the forward, so T and the colour prefix need no hand-over between lanes and the eight pixels of a lane
+// One warp per LIVE bucket in a persistent grid-stride loop, covering the bucket's whole 16x16 tile: lane l owns the 8
+// pixels (column l & 15, rows 2j + (l >> 4), j = 0..7), one per row pair.  Every pixel restarts from the bucket's
+// checkpoint (T, C) and walks the bucket's splats in list order exactly like the forward, so T and the colour prefix
+// need no hand-over between lanes and the eight pixels of a lane
 // are eight independent dependency chains.  A (splat, row pair) is visited only if the splat's alpha >= 1/255 ellipse can
 // reach those rows (the forward's conservative half-extent test => skipped pairs contribute exactly zero) and some pixel
 // of the pair got this far.  The nine per-splat sums are accumulated over the lane's pixels in registers, combined across
@@ -419,7 +421,7 @@ constexpr int BWD_WARPS = 4;              // warps per CTA; every warp owns one 
 // (BwdCount) and is used by tests and scripts/render_bwd_bench.py only.  No visit is skipped for want of a taking pixel:
 // at cfg2, 98 % of the (splat, two row pairs) visits have one, and a per-visit ballot cost more than it saved.
 //
-// DET (the deterministic form, RP = 8 and FAST only; the RP = 4, exact and counting forms stay atomic-only) runs the same body
+// DET (the deterministic form, FAST only; the exact and counting forms stay atomic-only) runs the same body
 // but sends no RED: the nine values of (live bucket `live`, splat k) -- bit for bit what the atomic form would add -- are stored
 // to entry e = 32 live + k of `det` (DetOut), with the splat's gid as the entry's key.  A slot that adds nothing (past n_valid,
 // no visit, or all nine sums exactly zero: the cases the atomic form skips) gets the key `sentinel` = P.  Live buckets are
@@ -434,7 +436,7 @@ struct DetOut {
     uint32_t cap_live;        // live buckets the arrays hold; a bucket past it (garbage counts of an overflowed forward) is dropped
     uint32_t sentinel;
 };
-template <int BWD_ROWPAIRS, int MIN_CTAS, bool FAST, bool COUNT, bool DET = false>
+template <int MIN_CTAS, bool FAST, bool COUNT, bool DET = false>
 __global__ void __launch_bounds__(BWD_WARPS * 32, MIN_CTAS)
 render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr, const uint2* __restrict__ ranges,
                        const uint32_t* __restrict__ point_list, const float4* __restrict__ rec,
@@ -444,7 +446,7 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
                        float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic, float* __restrict__ dL_dopacity,
                        float* __restrict__ dL_dcolors, unsigned long long* __restrict__ counters, DetOut det) {
     pdl_enter();
-    static_assert(!DET || (BWD_ROWPAIRS == 8 && FAST && !COUNT), "the deterministic form is the production body only");
+    static_assert(!DET || (FAST && !COUNT), "the deterministic form is the production body only");
     __shared__ float4 s_sp[BWD_WARPS][BUCKET][3];            // the bucket's splat records, per warp
     __shared__ uint32_t s_gid[BWD_WARPS][BUCKET];
     __shared__ uint32_t s_rows[BWD_WARPS][BUCKET];           // row pairs each splat can reach (8-bit mask)
@@ -470,15 +472,12 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
     const bool i_write = (lane & 3) == 0 || lane == 1;
     unsigned ctr[BC_N] = {};                                     // COUNT only: this lane's share of the counters
 
-    constexpr int PARTS = (TILE / 2) / BWD_ROWPAIRS;
-    // work items are handed out dynamically (one ticket per warp and item): buckets differ by more than 10x in cost
+    // live buckets are handed out dynamically (one ticket per warp and bucket): buckets differ by more than 10x in cost
     for (;;) {
-        uint32_t item = 0;
-        if (lane == 0) item = atomicAdd(&hdr->bwd_ticket, 1u);
-        item = __shfl_sync(0xffffffffu, item, 0);
-        if (item >= n_live * PARTS) break;
-        const uint32_t live = item / PARTS;
-        const int part = (int)(item % PARTS);
+        uint32_t live = 0;
+        if (lane == 0) live = atomicAdd(&hdr->bwd_ticket, 1u);
+        live = __shfl_sync(0xffffffffu, live, 0);
+        if (live >= n_live) break;
         // tile of this live bucket: first t with live_offsets[t] > live -- 32-ary search, one probe per lane
         int lo = 0, cnt = T_tiles;
         while (cnt > 1) {
@@ -497,11 +496,11 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
         const int bucket_start = bucket_in_tile * BUCKET;
         const int n_valid = min(BUCKET, n_splats - bucket_start);
         const int tile_x = tile % vp.grid_x, tile_y = tile / vp.grid_x;
-        const int row0 = tile_y * TILE + 2 * BWD_ROWPAIRS * part;       // first tile row of this part
+        const int row0 = tile_y * TILE;
         const int qx = tile_x * TILE + (lane & (TILE - 1)), qy0 = row0 + (lane >> 4);
         const float pfx = (float)qx;
 
-        // this lane's 8 pixels, as RP/2 PAIRS of row pairs (p <-> rows 2(2p) + h and 2(2p+1) + h, h = lane >> 4): contributors left
+        // this lane's 8 pixels, as 4 PAIRS of row pairs (p <-> rows 2(2p) + h and 2(2p+1) + h, h = lane >> 4): contributors left
         // inside this bucket (0 = never got here) and the restart state, kept as fp32 pairs (f32x2.cuh)
         constexpr int NP = BWD_ROWPAIRS / 2;
         int rel[BWD_ROWPAIRS];
@@ -524,7 +523,7 @@ render_backward_kernel(ViewParams vp, int T_tiles, ImageHeader* __restrict__ hdr
 #pragma unroll
                 for (int e = 0; e < 7; ++e) st[h][e] = 0.f;
                 if (rel[j] > 0) {
-                    const float4 k4 = ckpt[(size_t)bucket * TILE_PIX + (part * BWD_ROWPAIRS + j) * 32 + lane];
+                    const float4 k4 = ckpt[(size_t)bucket * TILE_PIX + j * 32 + lane];
                     st[h][0] = k4.x;
                     st[h][1] = k4.y - pixel_colors[qi]; st[h][2] = k4.z - pixel_colors[HW + qi]; st[h][3] = k4.w - pixel_colors[2 * HW + qi];
                     st[h][4] = dL_dpix[qi]; st[h][5] = dL_dpix[HW + qi]; st[h][6] = dL_dpix[2 * HW + qi];
@@ -782,18 +781,15 @@ int launch_render_backward(int P, const ViewParams& vp, int64_t max_buckets, con
     if (max_buckets <= 0) return GLIC_OK;
     const int T = vp.grid_x * vp.grid_y;
     GLIC_LAUNCH_PDL(live_scan_kernel, 1, 1024, 0, s, T, img.max_contrib, img.live_offsets, img.hdr);
-    // RP = row pairs per lane (8: one warp per bucket's whole tile, 4: two warps share it; the exact and counting forms exist
-    // for RP = 8 only).  The occupancy-derived grid size is a property of the DEVICE and the kernel: cached per device.
-    static const int rp = getenv("GLIC_BWD_RP") ? atoi(getenv("GLIC_BWD_RP")) : 8;
+    // The occupancy-derived grid size is a property of the DEVICE and the kernel: cached per device.
     using Kern = void (*)(ViewParams, int, ImageHeader*, const uint2*, const uint32_t*, const float4*, const uint32_t*,
                           const uint32_t*, const float4*, const uint32_t*, const float*, const float*, float*, float*, float*, float*,
                           unsigned long long*, DetOut);
-    const int form = exact || counters ? 2 * (int)exact + (counters != nullptr) : rp == 8 ? 0 : 4;
-    const Kern kerns[5] = {render_backward_kernel<8, 6, true, false>, render_backward_kernel<8, 6, true, true>,
-                           render_backward_kernel<8, 5, false, false>, render_backward_kernel<8, 5, false, true>,
-                           render_backward_kernel<4, 6, true, false>};
+    const int form = 2 * (int)exact + (counters != nullptr);
+    const Kern kerns[4] = {render_backward_kernel<6, true, false>, render_backward_kernel<6, true, true>,
+                           render_backward_kernel<5, false, false>, render_backward_kernel<5, false, true>};
     const Kern kern = kerns[form];
-    static int blocks_per_device[5][64] = {};
+    static int blocks_per_device[4][64] = {};
     int dev = 0;
     GLIC_CUDA_TRY(cudaGetDevice(&dev));
     if (dev < 0 || dev >= 64) { set_error("render_backward: device index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
@@ -804,8 +800,7 @@ int launch_render_backward(int P, const ViewParams& vp, int64_t max_buckets, con
         blocks_per_device[form][dev] = sms * (per_sm > 0 ? per_sm : 1);
     }
     const int blocks = blocks_per_device[form][dev];
-    const int parts = form == 4 ? 2 : 1;
-    const int64_t need = (max_buckets * parts + BWD_WARPS - 1) / BWD_WARPS;
+    const int64_t need = (max_buckets + BWD_WARPS - 1) / BWD_WARPS;
     GLIC_LAUNCH_PDL(kern, (unsigned)std::min<int64_t>(blocks, need), BWD_WARPS * 32, 0, s, vp, T, img.hdr, img.ranges, point_list, g.rec,
                     img.bucket_offsets, img.live_offsets, smp.ckpt, img.n_contrib, img.pixel_colors, dL_dpix, dL_dmean2D, dL_dconic,
                     dL_dopacity, dL_dcolors, counters, DetOut{});
@@ -895,7 +890,7 @@ int launch_render_backward_det(int P, const ViewParams& vp, int64_t max_buckets,
     if (max_buckets <= 0 || P <= 0) return GLIC_OK;
     const int T = vp.grid_x * vp.grid_y;
     GLIC_LAUNCH_PDL(live_scan_kernel, 1, 1024, 0, s, T, img.max_contrib, img.live_offsets, img.hdr);
-    const auto kern = render_backward_kernel<8, 6, true, false, true>;
+    const auto kern = render_backward_kernel<6, true, false, true>;
     static int blocks_per_device[64] = {};
     int dev = 0;
     GLIC_CUDA_TRY(cudaGetDevice(&dev));

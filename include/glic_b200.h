@@ -202,14 +202,14 @@ GLIC_API int glic_backward(int P, int sh_degree, int M, const float* means3D, co
 /* Deterministic backward: glic_backward's arguments and outputs, plus a workspace of glic_deterministic_bytes(num_rendered,
  * width, height) bytes (num_rendered as glic_backward takes it).  Every output is a function of the saved forward state and
  * dL_dpix alone: calls on the same state give the same bits, whatever the grid size, scheduling or order of the GPU's work.
- * The render backward (the production RP = 8 body only) stores each (tile, Gaussian) pair's nine contributions -- bit for bit
+ * The render backward (the production body only) stores each (tile, Gaussian) pair's nine contributions -- bit for bit
  * the values glic_backward adds atomically -- and adds a Gaussian's contributions in ascending tile index:
  *   chunks of 32 consecutive contributions are each left-folded from their first element, then the chunk sums are
  *   left-folded in chunk order; for 32 or fewer contributions that is the strict left fold.
  * Rows with no contribution are zero.  Agreement with glic_backward: within the reassociation bound of the n contributions.
  * A short det_ws returns GLIC_ERR_WORKSPACE with nothing enqueued.  The workspace is 32 entries per checkpoint bucket (36 B of
- * values + 16 B of sort keys and indices each) plus the sort's temp; the GLIC_BWD_RP = 4, exact and counting forms of the debug
- * hook have no deterministic form. */
+ * values + 16 B of sort keys and indices each) plus the sort's temp; the exact and counting forms of the debug hook have no
+ * deterministic form. */
 GLIC_API size_t glic_deterministic_bytes(int64_t num_rendered, int width, int height);
 GLIC_API int glic_backward_deterministic(int P, int sh_degree, int M, const float* means3D, const float* scales,
                   float scale_modifier, const float* rotations, const float* dc, const float* sh,

@@ -42,9 +42,7 @@ nc.packed.flat.normal_()
 ms_nccl = timed(lambda: nc(radii))
 payload = ex.packed.payload_bytes()
 if rank == 0:
-    print(json.dumps({"world": world, "payload_bytes": payload, "ctas": os.environ.get("GLIC_P2P_CTAS", "2"),
-                      "unroll": os.environ.get("GLIC_P2P_UNROLL", "4"), "p2p_ms": round(ms_p2p, 4),
-                      "nccl_ms": round(ms_nccl, 4),
+    print(json.dumps({"world": world, "payload_bytes": payload, "p2p_ms": round(ms_p2p, 4), "nccl_ms": round(ms_nccl, 4),
                       "p2p_busbw_GBs": round(2 * (world - 1) / world * payload / ms_p2p / 1e6, 1),
                       "nccl_busbw_GBs": round(2 * (world - 1) / world * payload / ms_nccl / 1e6, 1)}))
 ex.close()

@@ -31,7 +31,7 @@ def card():
 
 
 def short(name):
-    """'void glic::(anonymous namespace)::onesweep_pass_kernel<unsigned int, 16, 8>(...)' -> 'onesweep_pass_kernel<unsigned int, 16, 8>'"""
+    """'void glic::(anonymous namespace)::onesweep_pass_kernel<unsigned int, 16>(...)' -> 'onesweep_pass_kernel<unsigned int, 16>'"""
     n = re.sub(r"^void\s+", "", name).replace("(anonymous namespace)::", "")
     depth, cut, ns = 0, len(n), 0
     for i, ch in enumerate(n):

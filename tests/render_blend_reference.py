@@ -52,8 +52,8 @@ EXACT = dict(amin=1.0 / 255.0, tmin=1e-4, amax=0.99)
 
 # |float32 kernel - v| <= c * 2^-24 * m per element.  Over every case of tests/test_gpu_render_blend_exact.py on an H100
 # (sm_90a) the largest err / bound with these constants was 0.39 (C), 0.15 (T), and per (Gaussian, tile) entry 0.044 (mean),
-# 0.047 (conic), 0.12 (colour) and 0.047 (opacity); the per-Gaussian sums of every atomic and deterministic form, RP = 4
-# included, stayed below 0.04 of their bound.  The float32 evaluation of test_render_blend_reference_host.py stays within the same ranges.
+# 0.047 (conic), 0.12 (colour) and 0.047 (opacity); the per-Gaussian sums of every atomic and deterministic form stayed
+# below 0.04 of their bound.  The float32 evaluation of test_render_blend_reference_host.py stays within the same ranges.
 BOUND = dict(C=4.0, T=4.0, mean=8.0, conic=8.0, opacity=8.0, color=4.0)
 PAIR_KEYS = ("mean", "mean", "conic", "conic", "conic", "color", "color", "color", "opacity")
 # half-width of the band around a decision threshold, in units of 2^-24 * m of the quantity decided on

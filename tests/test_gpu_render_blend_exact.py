@@ -15,16 +15,12 @@ the count.
 - Backward per (Gaussian, tile): CRasterizer.deterministic_entries gives, bit for bit, what the atomic form adds for each
   bucket; every entry is held to the restated tile contribution.  A pair that one side has and the other lacks counts as zero
   on the lacking side.  A large frame (cfg2) is checked on a sample of tiles this way.
-- Backward per Gaussian, for render_backward(exact=False) (production), render_backward(exact=True), the 2-D outputs of
-  backward() and of backward(deterministic=True), and RP = 4 (GLIC_BWD_RP=4, in a subprocess): the summed bound plus
-  (5 + adds) * 2^-24 * sum m, where 5 is the depth of the in-warp sum and adds = tiles touched x parts (the deterministic
-  fold adds fewer).
+- Backward per Gaussian, for render_backward(exact=False) (production), render_backward(exact=True) and the 2-D outputs of
+  backward() and of backward(deterministic=True): the summed bound plus (5 + adds) * 2^-24 * sum m, where 5 is the depth of
+  the in-warp sum and adds = tiles touched (the deterministic fold adds fewer).
 
 Run with -s to see max(err / bound) per output and form, the flagged pixels and the paths each case reached.
 """
-import os
-import subprocess
-import sys
 import time
 
 import numpy as np
@@ -39,7 +35,6 @@ pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
 
 DEV = "cuda:0"
-RP = int(os.environ.get("GLIC_BWD_RP", "8"))
 FOLD = 5.0                       # roundings of the in-warp sum (32 lanes) before an entry leaves the warp
 TWO_D = ("dL_dmeans2D", "dL_dconic", "dL_dopacity", "dL_dcolors")
 
@@ -150,21 +145,21 @@ class Case:
         if forms:
             v, m, n = rb.per_gaussian(bw, pl, self.P)
 
-            def per_gaussian(grads, parts):
-                return _max_by_key(rb.ratio(_two_d(grads), v, rb.pair_bound(m, FOLD + n * parts)))
+            def per_gaussian(grads):
+                return _max_by_key(rb.ratio(_two_d(grads), v, rb.pair_bound(m, FOLD + n)))
             for name, exact in (("atomic", False), ("exact", True)):
                 grads = self.r.alloc_grads()
                 for k in TWO_D:
                     grads[k].zero_()
                 self.r.render_backward(self.view, dLt, grads, exact=exact)
                 torch.cuda.synchronize()
-                ratios[name] = per_gaussian(grads, 1 if exact else 8 // RP)
+                ratios[name] = per_gaussian(grads)
             grads = self.r.backward(self.gd, self.view, self.radii, dLt)
             torch.cuda.synchronize()
-            ratios["backward"] = per_gaussian(grads, 8 // RP)
+            ratios["backward"] = per_gaussian(grads)
             grads = self.r.backward(self.gd, self.view, self.radii, dLt, deterministic=True)
             torch.cuda.synchronize()
-            ratios["deterministic"] = per_gaussian(grads, 1)
+            ratios["deterministic"] = per_gaussian(grads)
         return ratios, info
 
     def paths(self):
@@ -176,8 +171,8 @@ class Case:
 
 
 def _report(name, fwd, bwd, info, paths):
-    print("\n%s (GLIC_BWD_RP=%d)\n    forward %s\n    %s\n    %s\n    paths %s" % (
-        name, RP, "  ".join("%s %.3f" % kv for kv in fwd.items()),
+    print("\n%s\n    forward %s\n    %s\n    %s\n    paths %s" % (
+        name, "  ".join("%s %.3f" % kv for kv in fwd.items()),
         "\n    ".join("%-13s %s" % (f, "  ".join("%s %.3f" % kv for kv in r.items())) for f, r in bwd.items()), info, paths))
     worst = max([max(fwd.values())] + [max(r.values()) for r in bwd.values()])
     assert worst <= 1.0, (name, fwd, bwd)
@@ -283,17 +278,3 @@ def test_cfg2_sampled_tiles():
         return np.array(sorted(tiles))
     c = run_case("cfg2 view 1, sampled tiles", g, cam, tiles=sample, forms=False)
     assert c.fw["tiles"].size >= 64
-
-
-@pytest.mark.skipif(os.environ.get("GLIC_BWD_RP") is not None, reason="already inside the GLIC_BWD_RP subprocess")
-def test_two_warps_per_tile():
-    """the atomic forms with render_backward_kernel<4, 6> (GLIC_BWD_RP=4: two warps share a tile's bucket, two adds per
-    (Gaussian, tile)) on the small scenes, the stress scenes and the one-hot patterns"""
-    here = os.path.dirname(os.path.abspath(__file__))
-    env = dict(os.environ, GLIC_BWD_RP="4")
-    p = subprocess.run([sys.executable, "-m", "pytest", "-q", "-s", "-x", "-p", "no:cacheprovider", "-m", "gpu",
-                        os.path.join(here, "test_gpu_render_blend_exact.py"), "-k", "small_scene or stress_scene or one_hot"],
-                       cwd=here, env=env, capture_output=True, text=True)
-    print(p.stdout[-20000:], p.stderr[-2000:])
-    assert p.returncode == 0, p.stdout[-4000:]
-    assert "%d passed" % (20 + len(STRESS_CASES) + 3) in p.stdout

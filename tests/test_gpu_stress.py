@@ -5,17 +5,10 @@ grad_close), on the scenes of synthetic.make_stress_scene -- needle-shaped splat
 of splats, depth ties, view-edge culls and clamps (tests/test_stress_scenes.py checks that each reaches its path) -- and on
 frames from 1 x 1 to the largest the library accepts, GLIC_MAX_TILES = 65 536 tiles.
 
-The backward of every stress case runs a second time in a subprocess with GLIC_BWD_RP=4 (two warps per tile): the
-variant is read once per process.
-
 The tensor-scale tolerances here absorb errors confined to a few pixels or pairs.  test_gpu_render_blend_exact.py pins the
 same scenes per element: colour, T and n_contrib at every pixel, and the 2-D gradients per (Gaussian, tile) entry and per
 Gaussian for every backward form, against a float64 restatement that walks every pair without the row cull.
 """
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
@@ -117,7 +110,7 @@ def test_stress_matches_oracle(oracle32, oracle64, kind, opaque, view, pp):
     st = oracle32.state(f)
     d = check_forward(r, color, T, radii, f, st)
     c = path_counters(d, f, st)
-    print("path counters %s (GLIC_BWD_RP=%s): %s" % (kind + ("-high" if opaque else ""), os.environ.get("GLIC_BWD_RP", "8"), c))
+    print("path counters %s: %s" % (kind + ("-high" if opaque else ""), c))
     if kind == "big" and view == 0:
         # the arena overflowed part-way through: some rects stored spans, the later ones had their rows recomputed
         assert c["span_count"] > c["span_cap"] and big_rect_rows(st["xy"], f["radii"], cam["W"], cam["H"]) > c["span_cap"]
@@ -135,19 +128,6 @@ def test_stress_matches_oracle(oracle32, oracle64, kind, opaque, view, pp):
         skip = NEEDLE_UNSTABLE
     check_backward(grads, b, f, skip=skip)
     oracle32.free(f)
-
-
-@pytest.mark.skipif(os.environ.get("GLIC_BWD_RP") is not None, reason="already inside the GLIC_BWD_RP subprocess")
-def test_stress_backward_two_warps_per_tile():
-    """render_backward_kernel<4, 6> (GLIC_BWD_RP=4, two warps share a tile's bucket) against the oracle on every stress case"""
-    here = os.path.dirname(os.path.abspath(__file__))
-    env = dict(os.environ, GLIC_BWD_RP="4")
-    p = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-p", "no:cacheprovider", "-m", "gpu",
-                        os.path.join(here, "test_gpu_stress.py"), "-k", "test_stress_matches_oracle"],
-                       cwd=here, env=env, capture_output=True, text=True)
-    print(p.stdout[-4000:], p.stderr[-2000:])
-    assert p.returncode == 0, p.stdout[-4000:]
-    assert "%d passed" % len(CASES) in p.stdout
 
 
 @pytest.mark.parametrize("kind,view,pp", [("needles", 0, (0.0, 0.0)), ("big", 0, (0.0, 0.0)), ("big", 5, (17.5, -9.25))])
