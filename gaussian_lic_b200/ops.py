@@ -577,6 +577,17 @@ class CRasterizer:
         d["span_count"], d["span_cap"] = int(spans[0]), int(spans[1])
         return d
 
+    def debug_render_state(self, R):
+        """debug_state() of the lists the last render() drew, R = its counters[0]: glic_render carves the binning workspace
+        with the capacity glic_binning_capacity(binning_bytes, 0, W, H, 1), which need not be the forward's.  The rasterizer's
+        own R and capacity (those of the last forward, which backward() uses) are left as they were."""
+        saved = self.R, self.cap
+        self.R, self.cap = int(R), int(self.lib.glic_binning_capacity(self.binning_ws.numel(), 0, self.W, self.H, 1))
+        try:
+            return self.debug_state()
+        finally:
+            self.R, self.cap = saved
+
 
 def sort_pairs(keys, vals, end_bit):
     """Stable sort of (int64-viewed u64 keys, int32-viewed u32 values) device tensors on bits [0,end_bit)."""

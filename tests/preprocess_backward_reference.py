@@ -228,6 +228,39 @@ def _xform_row(m, r, x, y, z):
     return m[12 + r] + (z * m[8 + r] + (x * m[r] + y * m[4 + r]))
 
 
+def ewa_forward(A, v, lims, fx, fy, mod_, px, py, pz, sraw, q, dilation=True):
+    """geom_math.cuh cov3d_from_scale_rot and cov2d_project: the activated scale times mod, R(q), M = S R, the cov3D V =
+    M^T M, the view-space position, the clamped ratios, T = J W and the 2-D covariance (a, b, c), with its 0.3 dilation"""
+    s = [mod_ * si for si in sraw]
+    r, x, y, z = q
+    yy, zz, xz, rx, rz = y * y, z * z, x * z, r * x, r * z
+    R = [A.ka(1) - (yy + zz) * 2, (x * y - rz) * 2, (r * y + xz) * 2,
+         (x * y + rz) * 2, A.ka(1) - (x * x + zz) * 2, (y * z - rx) * 2,
+         (xz - r * y) * 2, (y * z + rx) * 2, A.ka(1) - (x * x + yy) * 2]
+    Mm = [s[i % 3] * R[i] for i in range(9)]
+    V = [Mm[0] * Mm[0] + Mm[1] * Mm[1] + Mm[2] * Mm[2], Mm[3] * Mm[0] + Mm[4] * Mm[1] + Mm[5] * Mm[2],
+         Mm[6] * Mm[0] + Mm[7] * Mm[1] + Mm[8] * Mm[2], Mm[3] * Mm[3] + Mm[4] * Mm[4] + Mm[5] * Mm[5],
+         Mm[6] * Mm[3] + Mm[7] * Mm[4] + Mm[8] * Mm[5], Mm[6] * Mm[6] + Mm[7] * Mm[7] + Mm[8] * Mm[8]]
+    tx, ty, tz = (_xform_row(v, j, px, py, pz) for j in range(3))
+    txtz, tytz = tx / tz, ty / tz
+    lx, ly = A.clip(txtz, lims[0], lims[1]), A.clip(tytz, lims[2], lims[3])
+    tz2 = tz * tz
+    J00, J11 = fx / tz, fy / tz
+    J02, J12 = (fx * (lx * -tz)) / tz2, (fy * (ly * -tz)) / tz2
+    T00, T01, T02 = v[2] * J02 + v[0] * J00, v[6] * J02 + v[4] * J00, v[10] * J02 + v[8] * J00
+    T10, T11, T12 = v[2] * J12 + v[1] * J11, v[6] * J12 + v[5] * J11, v[10] * J12 + v[9] * J11
+    A00, A01 = T00 * V[0] + T01 * V[1] + T02 * V[2], T10 * V[0] + T11 * V[1] + T12 * V[2]
+    A10, A11 = T00 * V[1] + T01 * V[3] + T02 * V[4], T10 * V[1] + T11 * V[3] + T12 * V[4]
+    A20, A21 = T00 * V[2] + T01 * V[4] + T02 * V[5], T10 * V[2] + T11 * V[4] + T12 * V[5]
+    a = A00 * T00 + A10 * T01 + A20 * T02
+    b = A01 * T00 + A11 * T01 + A21 * T02
+    c = A01 * T10 + A11 * T11 + A21 * T12
+    if dilation:
+        a, c = a + A.ka(0.3), c + A.ka(0.3)
+    return dict(s=s, R=R, Mm=Mm, V=V, tz=tz, txtz=txtz, tytz=tytz, lx=lx, ly=ly, T=(T00, T01, T02, T10, T11, T12), a=a, b=b,
+                c=c)
+
+
 def _band(A, q, thresholds):
     """rows whose float64 branch quantity q lies within BAND * 2^-24 * m of a threshold"""
     if not A.mag:
@@ -289,30 +322,10 @@ def _backward(g, cam, radii, clamped, dmean2D, dconic, dcolors, mod=1.0, lambda_
     band = {}
 
     # ---- forward quantities, recomputed (geom_math.cuh cov3d_from_scale_rot, cov2d_project) ---------------------------------
-    s = [mod_ * si for si in sraw]
-    r, x, y, z = q
-    yy, zz, xz, rx, rz = y * y, z * z, x * z, r * x, r * z
-    R = [A.ka(1) - (yy + zz) * 2, (x * y - rz) * 2, (r * y + xz) * 2,
-         (x * y + rz) * 2, A.ka(1) - (x * x + zz) * 2, (y * z - rx) * 2,
-         (xz - r * y) * 2, (y * z + rx) * 2, A.ka(1) - (x * x + yy) * 2]
-    Mm = [s[i % 3] * R[i] for i in range(9)]
-    V = [Mm[0] * Mm[0] + Mm[1] * Mm[1] + Mm[2] * Mm[2], Mm[3] * Mm[0] + Mm[4] * Mm[1] + Mm[5] * Mm[2],
-         Mm[6] * Mm[0] + Mm[7] * Mm[1] + Mm[8] * Mm[2], Mm[3] * Mm[3] + Mm[4] * Mm[4] + Mm[5] * Mm[5],
-         Mm[6] * Mm[3] + Mm[7] * Mm[4] + Mm[8] * Mm[5], Mm[6] * Mm[6] + Mm[7] * Mm[7] + Mm[8] * Mm[8]]
-    tx, ty, tz = (_xform_row(v, j, px, py, pz) for j in range(3))
-    txtz, tytz = tx / tz, ty / tz
-    lx, ly = A.clip(txtz, lims[0], lims[1]), A.clip(tytz, lims[2], lims[3])
-    tz2 = tz * tz
-    J00, J11 = fx / tz, fy / tz
-    J02, J12 = (fx * (lx * -tz)) / tz2, (fy * (ly * -tz)) / tz2
-    T00, T01, T02 = v[2] * J02 + v[0] * J00, v[6] * J02 + v[4] * J00, v[10] * J02 + v[8] * J00
-    T10, T11, T12 = v[2] * J12 + v[1] * J11, v[6] * J12 + v[5] * J11, v[10] * J12 + v[9] * J11
-    A00, A01 = T00 * V[0] + T01 * V[1] + T02 * V[2], T10 * V[0] + T11 * V[1] + T12 * V[2]
-    A10, A11 = T00 * V[1] + T01 * V[3] + T02 * V[4], T10 * V[1] + T11 * V[3] + T12 * V[4]
-    A20, A21 = T00 * V[2] + T01 * V[4] + T02 * V[5], T10 * V[2] + T11 * V[4] + T12 * V[5]
-    a = A00 * T00 + A10 * T01 + A20 * T02 + A.ka(0.3)
-    b = A01 * T00 + A11 * T01 + A21 * T02
-    c = A01 * T10 + A11 * T11 + A21 * T12 + A.ka(0.3)
+    e = ewa_forward(A, v, lims, fx, fy, mod_, px, py, pz, sraw, q)
+    s, R, Mm, V, tz, txtz, tytz, lx, ly = (e[kk] for kk in ("s", "R", "Mm", "V", "tz", "txtz", "tytz", "lx", "ly"))
+    T00, T01, T02, T10, T11, T12 = e["T"]
+    a, b, c = e["a"], e["b"], e["c"]
 
     # ---- EWA backward --------------------------------------------------------------------------------------------------------
     tv = A.val(txtz)
