@@ -101,6 +101,24 @@ class MeshCounts(C.Structure):
     _fields_ = [("vertices", C.c_uint32), ("faces", C.c_uint32), ("observed_voxels", C.c_uint64)]
 
 
+class BlockSet(C.Structure):
+    _fields_ = [("capacity", C.c_uint32), ("data", C.c_void_p)]
+
+
+class SparseTsdf(C.Structure):
+    _fields_ = [("origin", C.c_float * 3), ("voxel_size", C.c_float), ("n_blocks", C.c_uint32), ("data", C.c_void_p)]
+
+
+class SparseMeshCounts(C.Structure):
+    _fields_ = [("vertices", C.c_uint32), ("faces", C.c_uint32), ("observed_voxels", C.c_uint64), ("blocks", C.c_uint32),
+                ("clipped_pixels", C.c_uint32), ("lattice_lo", C.c_int32 * 3), ("lattice_hi", C.c_int32 * 3)]
+
+
+class SparseMeshParams(C.Structure):
+    _fields_ = [("views", C.c_void_p), ("n_views", C.c_int), ("origin", C.c_float * 3), ("voxel_size", C.c_float), ("trunc", C.c_float),
+                ("max_depth", C.c_float), ("max_blocks", C.c_uint32)]
+
+
 class RigidCorrection(C.Structure):
     _fields_ = [("R", C.c_double * 9), ("t", C.c_double * 3), ("q", C.c_double * 4), ("sh", C.c_double * 83)]
 
@@ -255,6 +273,20 @@ def _load():
         "glic_mapper_extract_mesh": (i32, [vp, C.POINTER(MeshParams), C.POINTER(MeshCounts)]),
         "glic_mapper_mesh_get": (i32, [vp, C.POINTER(MeshCounts), vp, vp, vp]),
         "glic_mapper_save_mesh": (i32, [vp, C.c_char_p]),
+        "glic_block_set_bytes": (sz, [u32]),
+        "glic_block_set_clear": (i32, [C.POINTER(BlockSet), vp]),
+        "glic_block_set_copy": (i32, [C.POINTER(BlockSet), C.POINTER(BlockSet), vp]),
+        "glic_block_set_insert": (i32, [C.POINTER(BlockSet), C.POINTER(f32), f32, vp, i32, i32, f32, f32, f32, f32, vp, vp, i32, f32, f32,
+                                        C.POINTER(C.c_int64), vp]),
+        "glic_sparse_tsdf_bytes": (sz, [u32]),
+        "glic_sparse_tsdf_init": (i32, [C.POINTER(SparseTsdf), C.POINTER(BlockSet), vp]),
+        "glic_sparse_tsdf_integrate": (i32, [C.POINTER(SparseTsdf), vp, i32, i32, f32, f32, f32, f32, vp, vp, vp, i32, f32, f32, vp]),
+        "glic_sparse_mesh_scratch_bytes": (sz, [u32]),
+        "glic_sparse_mesh_extract_bytes": (sz, [u32, u32]),
+        "glic_sparse_mesh_count": (i32, [C.POINTER(SparseTsdf), vp, sz, C.POINTER(SparseMeshCounts), vp]),
+        "glic_sparse_mesh_extract": (i32, [C.POINTER(SparseTsdf), vp, sz, C.POINTER(SparseMeshCounts), vp, sz, vp, vp, vp, vp]),
+        "glic_debug_sparse_tsdf": (i32, [C.POINTER(SparseTsdf), vp, vp, vp]),
+        "glic_mapper_extract_mesh_sparse": (i32, [vp, C.POINTER(SparseMeshParams), C.POINTER(SparseMeshCounts)]),
         "glic_pose_correction_record": (i32, [C.POINTER(f32), C.POINTER(f32), C.POINTER(f32), C.POINTER(f32), i32,
                                               C.POINTER(RigidCorrection)]),
         "glic_sh_rotation": (i32, [C.POINTER(C.c_double), i32, C.POINTER(C.c_double)]),

@@ -181,10 +181,7 @@ __device__ __forceinline__ uint32_t block_exclusive(uint32_t v, uint32_t* warp_t
     return before + incl - v;
 }
 
-__global__ void __launch_bounds__(MESH_THREADS)
-tsdf_integrate_kernel(Grid g, const float* __restrict__ view, int W, int H, float fx, float fy, float cx, float cy,
-                      const float* __restrict__ depth, const float* __restrict__ rgb, const uint32_t* __restrict__ mask, int wpr,
-                      float trunc, float max_depth) {
+__global__ void __launch_bounds__(MESH_THREADS) tsdf_integrate_kernel(Grid g, FuseView f) {
     const uint32_t p = blockIdx.x * MESH_THREADS + threadIdx.x;
     if (p >= g.N) return;
     int ijk[3];
@@ -192,30 +189,7 @@ tsdf_integrate_kernel(Grid g, const float* __restrict__ view, int W, int H, floa
     const float X = fadd(g.o[0], fmul(g.s, (float)ijk[0]));
     const float Y = fadd(g.o[1], fmul(g.s, (float)ijk[1]));
     const float Z = fadd(g.o[2], fmul(g.s, (float)ijk[2]));
-    const float z = xform_row(view, 2, X, Y, Z);
-    if (!(z > 0.0f)) return;
-    const float x = xform_row(view, 0, X, Y, Z), y = xform_row(view, 1, X, Y, Z);
-    const float u = fadd(fmul(fx, __fdiv_rn(x, z)), cx), v = fadd(fmul(fy, __fdiv_rn(y, z)), cy);
-    if (!(u >= 0.0f && u < (float)W && v >= 0.0f && v < (float)H)) return;
-    const int px = (int)floorf(u), py = (int)floorf(v);
-    if (mask && !((mask[(size_t)py * wpr + (px >> 5)] >> (px & 31)) & 1u)) return;
-    const size_t pix = (size_t)py * W + px;
-    const float d = depth[pix];
-    if (!(d > 0.0f) || (max_depth != 0.0f && !(d <= max_depth))) return;
-    const float sdf = fsub(d, z);
-    if (!(sdf >= -trunc)) return;
-    const float t = fminf(1.0f, __fdiv_rn(sdf, trunc));
-    const float w = g.weight[p], w1 = fadd(w, 1.0f);
-    g.tsdf[p] = __fdiv_rn(fadd(fmul(g.tsdf[p], w), t), w1);
-    if (rgb) {
-        const size_t HW = (size_t)W * H;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            float* cp = g.col + (size_t)c * g.N + p;
-            *cp = __fdiv_rn(fadd(fmul(*cp, w), rgb[c * HW + pix]), w1);
-        }
-    }
-    g.weight[p] = w1;
+    tsdf_update(f, X, Y, Z, g.tsdf + p, g.weight + p, g.col + p, g.N);
 }
 
 // act bits, and per tile: tile[0][t] = active cells, tile[2][t] = observed lattice points
@@ -320,10 +294,6 @@ __device__ __forceinline__ uint32_t vertex_id(const MeshScratch& m, uint32_t C) 
     return m.wpre[C >> 5] + (uint32_t)__popc(m.act[C >> 5] & ((1u << (C & 31)) - 1u));
 }
 
-// corner A of each of the cell's 12 edges in the fixed edge order: the x-edges for (b, c) = (0,0), (1,0), (0,1), (1,1), then the
-// y-edges for (a, c), then the z-edges for (a, b); edge e's other end is A + (1 << (e / 4))
-__constant__ int EDGE_A[12] = {0, 2, 4, 6, 0, 1, 4, 5, 0, 1, 2, 3};
-
 // the vertex (world position) and colour (uint8) of active cell L
 __device__ __forceinline__ void cell_vertex(const Grid& g, uint32_t L, const int ijk[3], float xyz[3], uint8_t rgb[3]) {
     float t[8], col[3][8];
@@ -334,33 +304,7 @@ __device__ __forceinline__ void cell_vertex(const Grid& g, uint32_t L, const int
 #pragma unroll
         for (int ch = 0; ch < 3; ++ch) col[ch][q] = g.col[(size_t)ch * g.N + c];
     }
-    float sp[3] = {0.f, 0.f, 0.f}, sc[3] = {0.f, 0.f, 0.f};
-    int n = 0;
-#pragma unroll
-    for (int e = 0; e < 12; ++e) {
-        const int ax = e >> 2, A = EDGE_A[e], B = A + (1 << ax);
-        const float tA = t[A], tB = t[B];
-        if ((tA < 0.0f) == (tB < 0.0f)) continue;
-        const float f = __fdiv_rn(tA, fsub(tA, tB));
-        float p[3] = {(float)(A & 1), (float)((A >> 1) & 1), (float)(A >> 2)};
-        p[ax] = f;
-        float cc[3];
-#pragma unroll
-        for (int ch = 0; ch < 3; ++ch) cc[ch] = fadd(col[ch][A], fmul(f, fsub(col[ch][B], col[ch][A])));
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            sp[a] = n ? fadd(sp[a], p[a]) : p[a];
-            sc[a] = n ? fadd(sc[a], cc[a]) : cc[a];
-        }
-        ++n;
-    }
-    const float fn = (float)n;
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        xyz[a] = fadd(g.o[a], fmul(g.s, fadd((float)ijk[a], __fdiv_rn(sp[a], fn))));
-        const float c = fminf(fmaxf(__fdiv_rn(sc[a], fn), 0.0f), 1.0f);
-        rgb[a] = (uint8_t)__float2int_rn(fmul(c, 255.0f));
-    }
+    surface_vertex(t, col, ijk, g.o, g.s, xyz, rgb);
 }
 
 __global__ void __launch_bounds__(MESH_THREADS)
@@ -420,6 +364,26 @@ int scratch_check(const glic_tsdf_grid* g, void* scratch, size_t bytes, const ch
 
 }  // namespace
 
+int fuse_view_check(const FuseView& f, const char* what) {
+    const std::string w(what);
+    if (!f.view || !f.depth) { set_error(w + ": null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (f.W < 1 || f.H < 1) { set_error(w + ": width and height must be >= 1"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const int64_t tiles = (((int64_t)f.W + TILE - 1) / TILE) * (((int64_t)f.H + TILE - 1) / TILE);
+    if (tiles > GLIC_MAX_TILES) {
+        set_error(w + ": " + std::to_string(f.W) + "x" + std::to_string(f.H) + " has more than GLIC_MAX_TILES tiles of 16x16");
+        return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (!(std::isfinite(f.fx) && f.fx > 0.0f) || !(std::isfinite(f.fy) && f.fy > 0.0f) || !std::isfinite(f.cx) || !std::isfinite(f.cy)) {
+        set_error(w + ": fx and fy must be finite and > 0, cx and cy finite"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    if (!(std::isfinite(f.trunc) && f.trunc > 0.0f)) { set_error(w + ": trunc must be finite and > 0"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (!(std::isfinite(f.max_depth) && f.max_depth >= 0.0f)) { set_error(w + ": max_depth must be finite and >= 0"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (f.mask && f.wpr < mask_words_per_row(f.W)) {
+        set_error(w + ": words_per_row must be at least glic_mask_words_per_row(W)"); return GLIC_ERR_INVALID_ARGUMENT;
+    }
+    return GLIC_OK;
+}
+
 int mesh_count(const glic_tsdf_grid& gg, void* scratch, size_t scratch_bytes, uint64_t totals3[3], cudaStream_t s) {
     MeshScratch m;
     if (const int e = scratch_check(&gg, scratch, scratch_bytes, "mesh_count", &m)) return e;
@@ -472,24 +436,10 @@ int glic_tsdf_integrate(const glic_tsdf_grid* grid, const float* viewmatrix_dev,
                         const float* depth, const float* rgb, const uint32_t* mask_words, int words_per_row, float trunc, float max_depth,
                         void* stream) {
     if (const int e = grid_check(grid, "tsdf_integrate")) return e;
-    if (!viewmatrix_dev || !depth) { set_error("tsdf_integrate: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (W < 1 || H < 1) { set_error("tsdf_integrate: width and height must be >= 1"); return GLIC_ERR_INVALID_ARGUMENT; }
-    const int64_t tiles = (((int64_t)W + TILE - 1) / TILE) * (((int64_t)H + TILE - 1) / TILE);
-    if (tiles > GLIC_MAX_TILES) {
-        set_error("tsdf_integrate: " + std::to_string(W) + "x" + std::to_string(H) + " has more than GLIC_MAX_TILES tiles of 16x16");
-        return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (!(std::isfinite(fx) && fx > 0.0f) || !(std::isfinite(fy) && fy > 0.0f) || !std::isfinite(cx) || !std::isfinite(cy)) {
-        set_error("tsdf_integrate: fx and fy must be finite and > 0, cx and cy finite"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (!(std::isfinite(trunc) && trunc > 0.0f)) { set_error("tsdf_integrate: trunc must be finite and > 0"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!(std::isfinite(max_depth) && max_depth >= 0.0f)) { set_error("tsdf_integrate: max_depth must be finite and >= 0"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (mask_words && words_per_row < mask_words_per_row(W)) {
-        set_error("tsdf_integrate: words_per_row must be at least glic_mask_words_per_row(W)"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
+    const FuseView f{viewmatrix_dev, W, H, fx, fy, cx, cy, depth, rgb, mask_words, words_per_row, trunc, max_depth};
+    if (const int e = fuse_view_check(f, "tsdf_integrate")) return e;
     const Grid g = device_grid(*grid);
-    tsdf_integrate_kernel<<<(g.N + MESH_THREADS - 1) / MESH_THREADS, MESH_THREADS, 0, (cudaStream_t)stream>>>(
-        g, viewmatrix_dev, W, H, fx, fy, cx, cy, depth, rgb, mask_words, words_per_row, trunc, max_depth);
+    tsdf_integrate_kernel<<<(g.N + MESH_THREADS - 1) / MESH_THREADS, MESH_THREADS, 0, (cudaStream_t)stream>>>(g, f);
     GLIC_LAUNCH_CHECK();
     return GLIC_OK;
 }

@@ -403,6 +403,25 @@ class Mapper:
         del keep
         return self.mesh()
 
+    def extract_mesh_sparse(self, origin, voxel_size, trunc, max_depth=0.0, views=None, max_blocks=0):
+        """extract_mesh() over a sparse block grid (glic_mapper_extract_mesh_sparse): only the 8^3-voxel blocks near some view's
+        observed surface are stored, on a lattice aligned to origin with spacing voxel_size and no box, so a map of any extent can
+        be meshed; the mesh equals extract_mesh()'s with a box holding those blocks.  max_blocks > 0 refuses a map that needs more
+        blocks (GlicError) before the grid is allocated.  Returns the counts as a dict (vertices, faces, observed_voxels, blocks,
+        clipped_pixels, lattice_lo, lattice_hi: the inclusive lattice box of the blocks); the mesh itself is read with mesh()."""
+        p = capi.SparseMeshParams()
+        keep = None
+        if views is not None:
+            keep = (C.c_int * max(len(views), 1))(*[int(v) for v in views])
+            p.views, p.n_views = C.cast(keep, C.c_void_p), len(views)
+        p.origin[:] = [float(x) for x in np.asarray(origin, np.float32).reshape(3)]
+        p.voxel_size, p.trunc, p.max_depth, p.max_blocks = float(voxel_size), float(trunc), float(max_depth), int(max_blocks)
+        c = capi.SparseMeshCounts()
+        capi.check(capi.lib.glic_mapper_extract_mesh_sparse(self._h, C.byref(p), C.byref(c)), "mapper_extract_mesh_sparse")
+        del keep
+        return dict(vertices=int(c.vertices), faces=int(c.faces), observed_voxels=int(c.observed_voxels), blocks=int(c.blocks),
+                    clipped_pixels=int(c.clipped_pixels), lattice_lo=tuple(c.lattice_lo), lattice_hi=tuple(c.lattice_hi))
+
     def mesh(self):
         """The last extracted mesh as extract_mesh() returns it (empty arrays before any)."""
         c = capi.MeshCounts()

@@ -261,6 +261,86 @@ def mesh_extract(grid, device="cuda:0", stream=None):
     return xyz[:V], rgb[:V], faces[:F]
 
 
+# ---- sparse meshing (include/glic_b200.h "Sparse meshing") ----------------------------------------------------------
+def block_set(capacity, device="cuda:0", stream=None):
+    """An empty block set of `capacity` blocks: returns (capi.BlockSet, its data tensor)."""
+    nbytes = capi.lib.glic_block_set_bytes(int(capacity))
+    if not nbytes:
+        raise capi.GlicError("block_set: capacity must be in [1, 2^24]")
+    data = torch.empty(nbytes, dtype=torch.uint8, device=device)
+    s = capi.BlockSet(int(capacity), data.data_ptr())
+    capi.check(capi.lib.glic_block_set_clear(C.byref(s), stream), "block_set_clear")
+    return s, data
+
+
+def block_set_copy(src, dst, stream=None):
+    """Rehash src into dst (a set of at least twice src's capacity; glic_block_set_copy).  Asynchronous."""
+    capi.check(capi.lib.glic_block_set_copy(C.byref(src), C.byref(dst), stream), "block_set_copy")
+
+
+def block_set_insert(set_, origin, voxel_size, viewmatrix, W, H, fx, fy, cx, cy, depth, mask_words=None, words_per_row=0, trunc=0.1,
+                     max_depth=0.0, stream=None):
+    """Add one view's blocks to set_ (glic_block_set_insert); arguments as tsdf_integrate takes them.  Synchronises and returns
+    (blocks in the set, clipped pixels of this call, overflow)."""
+    o = (C.c_float * 3)(*[float(x) for x in origin])
+    cnt = (C.c_int64 * 3)()
+    capi.check(capi.lib.glic_block_set_insert(C.byref(set_), o, float(voxel_size), capi.ptr(viewmatrix.contiguous()), int(W), int(H),
+                                              float(fx), float(fy), float(cx), float(cy), capi.ptr(depth.contiguous()), capi.ptr(mask_words),
+                                              int(words_per_row), float(trunc), float(max_depth), cnt, stream), "block_set_insert")
+    torch.cuda.synchronize()
+    return int(cnt[0]), int(cnt[1]), int(cnt[2])
+
+
+def sparse_tsdf(origin, voxel_size, set_, n_blocks, device="cuda:0", stream=None):
+    """The sparse grid of set_'s n_blocks blocks (its block count), cleared: returns (capi.SparseTsdf, its data tensor)."""
+    nbytes = capi.lib.glic_sparse_tsdf_bytes(int(n_blocks))
+    if not nbytes and n_blocks:
+        raise capi.GlicError("sparse_tsdf: more than 2^23 - 1 blocks")
+    data = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=device)
+    g = capi.SparseTsdf()
+    g.origin[:] = [float(x) for x in origin]
+    g.voxel_size, g.n_blocks, g.data = float(voxel_size), int(n_blocks), data.data_ptr()
+    capi.check(capi.lib.glic_sparse_tsdf_init(C.byref(g), C.byref(set_), stream), "sparse_tsdf_init")
+    return g, data
+
+
+def sparse_tsdf_integrate(grid, viewmatrix, W, H, fx, fy, cx, cy, depth, rgb=None, mask_words=None, words_per_row=0, trunc=0.1,
+                          max_depth=0.0, stream=None):
+    """Fuse one view into a sparse grid (glic_sparse_tsdf_integrate), as tsdf_integrate takes it.  Asynchronous."""
+    capi.check(capi.lib.glic_sparse_tsdf_integrate(C.byref(grid), capi.ptr(viewmatrix.contiguous()), int(W), int(H), float(fx), float(fy),
+                                                   float(cx), float(cy), capi.ptr(depth.contiguous()),
+                                                   capi.ptr(None if rgb is None else rgb.contiguous()), capi.ptr(mask_words),
+                                                   int(words_per_row), float(trunc), float(max_depth), stream), "sparse_tsdf_integrate")
+
+
+def sparse_tsdf_planes(grid, device="cuda:0", stream=None):
+    """(sorted block keys [n] int64, pool [n, 5, 512] float32: tsdf, weight, colour x3) of a sparse grid (glic_debug_sparse_tsdf)"""
+    n = int(grid.n_blocks)
+    keys = torch.empty(max(n, 1), dtype=torch.int64, device=device)
+    pool = torch.empty(max(n, 1), 5, 512, dtype=torch.float32, device=device)
+    capi.check(capi.lib.glic_debug_sparse_tsdf(C.byref(grid), capi.ptr(keys), capi.ptr(pool), stream), "debug_sparse_tsdf")
+    return keys[:n], pool[:n]
+
+
+def sparse_mesh_extract(grid, device="cuda:0", stream=None):
+    """Surface nets of a sparse grid (glic_sparse_mesh_count + glic_sparse_mesh_extract): returns CUDA tensors (xyz [V,3] float32,
+    rgb [V,3] uint8, faces [F,3] int32) and the capi.SparseMeshCounts.  Synchronises once, for the counts."""
+    dev = torch.device(device)
+    need = capi.lib.glic_sparse_mesh_scratch_bytes(grid.n_blocks)
+    scratch = torch.empty(max(need, 1), dtype=torch.uint8, device=dev)
+    counts = capi.SparseMeshCounts()
+    capi.check(capi.lib.glic_sparse_mesh_count(C.byref(grid), capi.ptr(scratch), need, C.byref(counts), stream), "sparse_mesh_count")
+    V, F = int(counts.vertices), int(counts.faces)
+    ws_bytes = capi.lib.glic_sparse_mesh_extract_bytes(V, F)
+    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+    xyz = torch.empty(max(V, 1), 3, dtype=torch.float32, device=dev)
+    rgb = torch.empty(max(V, 1), 3, dtype=torch.uint8, device=dev)
+    faces = torch.empty(max(F, 1), 3, dtype=torch.int32, device=dev)
+    capi.check(capi.lib.glic_sparse_mesh_extract(C.byref(grid), capi.ptr(scratch), need, C.byref(counts), capi.ptr(ws), ws_bytes,
+                                                 capi.ptr(xyz), capi.ptr(rgb), capi.ptr(faces), stream), "sparse_mesh_extract")
+    return xyz[:V], rgb[:V], faces[:F], counts
+
+
 # ---- render() and the model getters it uses (rasterizer/renderer.cpp:21-88; gaussian.cpp:147-175) ------------------
 class GaussianParams:
     """The six raw parameter tensors of GaussianModel with its activation getters (sigmoid / exp / normalize)."""

@@ -1162,6 +1162,125 @@ GLIC_API int glic_mapper_mesh_get(glic_mapper* m, glic_mesh_counts* counts, floa
 GLIC_API int glic_mapper_save_mesh(glic_mapper* m, const char* path);
 
 /* ---------------------------------------------------------------------------------------
+ * Sparse meshing (no counterpart in the reference): the TSDF of "Meshing" stored only in the 8^3-voxel blocks near some view's
+ * observed surface, so a map hundreds of metres long meshes at a few centimetres.  Its mesh equals the dense grid's bit for bit
+ * whenever a dense grid of the same origin and voxel size can hold the same blocks (the equivalence below).
+ *   Lattice: point (i, j, k), integers in [-2^19, 2^19), at world position __fadd_rn(o.x, __fmul_rn(s, (float)i)) per axis (the
+ *   dense grid's formula, with no box).  Block (bi, bj, bk) holds the points with floor(i / 8) = bi (floor division on negatives),
+ *   and so on; its key is ((bk + 2^16) << 34) | ((bj + 2^16) << 17) | (bi + 2^16).  A block is allocated or not; every point of an
+ *   allocated block takes exactly the per-point update of "Meshing" (steps 1-5); a point of no allocated block is unobserved
+ *   (weight 0) and is never read or written.
+ *   Allocation rule (the block set of one view): a pixel (px, py) is USED when step 3's tests pass (not masked, d = depth[py][px]
+ *   > 0, max_depth == 0 or d <= max_depth).  For a used pixel, in float64, each operation rounded once in the order written: the
+ *   8 corners (u, v, z), u in {px, px + 1}, v in {py, py + 1}, z in {d, d + trunc}; camera point c = ((u - cx) z / fx,
+ *   (v - cy) z / fy, z); world point X_a = (R_0a (c_0 - t_0) + R_1a (c_1 - t_1)) + R_2a (c_2 - t_2) with R_ra = view[4a + r],
+ *   t_r = view[12 + r]; per axis the range [lo, hi] of the 8 X_a; lattice range floor((lo - o) / s) - 2 .. ceil((hi - o) / s) + 2;
+ *   every block meeting that range is in the view's set.  Where the range leaves the lattice (or a corner is not finite) the
+ *   part outside is dropped and the pixel counts as CLIPPED.  A grid's block set is the union over the views inserted, in any
+ *   order.  (The margin of 2: a point gets t < 0 only from a used pixel whose frustum piece z in (d, d + trunc] it lies in;
+ *   surface nets reads the +-1 neighbourhood of such points; one voxel covers that, the other rounding.  DESIGN.md.)
+ *   Equivalence: insert views V_1..V_n, build the grid, then integrate them in some order; integrate the same views in the same
+ *   order into a dense grid of origin o and voxel size s whose box holds every allocated block.  If no pixel was clipped, every
+ *   point of every allocated block holds the dense grid's tsdf, weight and colour bit for bit; the meshes (vertices xyz and rgb,
+ *   faces) are equal element for element, vertices by ascending (k, j, i) of their cell's lower corner and faces by ascending
+ *   (k, j, i, axis) of their lattice edge (the dense orders on any box); and the sparse count of observed points is <= the
+ *   dense one (the dense grid also holds free space far from every surface).  Every insertion must come before the grid is
+ *   built: a block made after a view was integrated would miss that view's free-space updates.
+ *   Block set: glic_block_set, data = DEVICE memory of glic_block_set_bytes(capacity) = 32 + 16 capacity bytes (a hash of 2
+ *   capacity key slots), capacity in [1, 2^24] (0 bytes otherwise).  glic_block_set_clear empties it.  glic_block_set_insert
+ *   adds one view's blocks (W, H, intrinsics, depth, mask_words, words_per_row, trunc and max_depth as glic_tsdf_integrate takes
+ *   them; origin[3] (HOST) and voxel_size as the grid's) and writes counters_host[3] = {blocks in the set, clipped pixels of this
+ *   call, overflow} ASYNCHRONOUSLY, as glic_forward writes its counters (valid after a stream synchronise).  The count is exact, and
+ *   overflow != 0 exactly when the set's blocks would exceed its capacity; the set then holds part of this view's blocks (and up
+ *   to twice its capacity).  glic_block_set_copy(src, dst) rehashes src into dst (another set of at least twice src's capacity,
+ *   cleared first), and repeating the insertion into dst gives the set a call that never overflowed gives.
+ *   Grid: glic_sparse_tsdf, data = DEVICE memory of glic_sparse_tsdf_bytes(n_blocks) (0 above 2^23 - 1 blocks):
+ *   keys[n] u64 ascending | neighbours[27 n] u32 | pool, block b's points at pool + 2560 b, planar tsdf[512] | weight[512] |
+ *   colour[3][512], point (x, y, z) of the block at x + 8 y + 64 z: 10 KiB + 116 B per block (the pool region is at least the
+ *   sort workspace of n keys, which only matters below a few blocks).  glic_sparse_tsdf_init(grid, set) builds it from the set:
+ *   n_blocks must be the set's block count (counters_host[0] of its last insertion); the keys are compacted and sorted with
+ *   glic_sort_pairs_u64_u32, block slot = rank of its key (so the layout depends on the set alone), every point is cleared.
+ *   glic_sparse_tsdf_integrate takes glic_tsdf_integrate's view arguments, one thread per point of every allocated block.
+ *   glic_sparse_mesh_count(grid, scratch, bytes, counts_host, stream): scratch of glic_sparse_mesh_scratch_bytes(n_blocks) (64 B
+ *   per block: the active-cell bits), *counts_host (HOST) = vertices, faces, observed points, blocks and the lattice bounding box
+ *   of the allocated blocks (inclusive; lo 0 and hi -1 for none); clipped_pixels is 0 there (the mapper fills it).  Synchronises
+ *   once.  glic_sparse_mesh_extract(grid, scratch, bytes, counts, ws, ws_bytes, xyz, rgb, faces): counts as counted, ws of
+ *   glic_sparse_mesh_extract_bytes(vertices, faces) (32 B per vertex and per quad, plus the sort's temp), fills xyz [V,3] f32,
+ *   rgb [V,3] u8 and faces [F,3] i32 asynchronously; the grid must be as it was counted.  Nothing depends on which CTA finishes
+ *   first.  glic_debug_sparse_tsdf copies the sorted keys [n] and the pool [n * 2560] (any memory) for tests.
+ *   Every call checks its arguments before it enqueues anything: what glic_tsdf_integrate rejects, a NULL set, a capacity out of
+ *   range, a copy into a smaller or the same set, a NULL counts pointer or output return GLIC_ERR_INVALID_ARGUMENT; a short
+ *   scratch or workspace GLIC_ERR_WORKSPACE.
+ * ------------------------------------------------------------------------------------- */
+typedef struct glic_block_set {
+    uint32_t capacity;             /* blocks it can hold */
+    void* data;                    /* device, glic_block_set_bytes(capacity) bytes */
+} glic_block_set;
+typedef struct glic_sparse_tsdf {
+    float origin[3];               /* world position of lattice point (0, 0, 0) */
+    float voxel_size;
+    uint32_t n_blocks;
+    void* data;                    /* device, glic_sparse_tsdf_bytes(n_blocks) bytes */
+} glic_sparse_tsdf;
+typedef struct glic_sparse_mesh_counts {
+    uint32_t vertices, faces;
+    uint64_t observed_voxels;
+    uint32_t blocks;
+    uint32_t clipped_pixels;       /* pixels whose lattice range was clipped (glic_mapper_extract_mesh_sparse; 0 from glic_sparse_mesh_count) */
+    int32_t lattice_lo[3], lattice_hi[3];  /* inclusive lattice bounding box of the allocated blocks */
+} glic_sparse_mesh_counts;
+GLIC_API size_t glic_block_set_bytes(uint32_t capacity);
+GLIC_API int glic_block_set_clear(const glic_block_set* set, void* stream);
+GLIC_API int glic_block_set_copy(const glic_block_set* src, const glic_block_set* dst, void* stream);
+GLIC_API int glic_block_set_insert(const glic_block_set* set, const float* origin /*[3], host*/, float voxel_size, const float* viewmatrix_dev,
+                                   int W, int H, float fx, float fy, float cx, float cy, const float* depth,
+                                   const uint32_t* mask_words /* may be NULL */, int words_per_row, float trunc, float max_depth,
+                                   int64_t* counters_host /*[3]*/, void* stream);
+GLIC_API size_t glic_sparse_tsdf_bytes(uint32_t n_blocks);
+GLIC_API int glic_sparse_tsdf_init(const glic_sparse_tsdf* grid, const glic_block_set* set, void* stream);
+GLIC_API int glic_sparse_tsdf_integrate(const glic_sparse_tsdf* grid, const float* viewmatrix_dev, int W, int H, float fx, float fy, float cx,
+                                        float cy, const float* depth, const float* rgb /* may be NULL */,
+                                        const uint32_t* mask_words /* may be NULL */, int words_per_row, float trunc, float max_depth,
+                                        void* stream);
+GLIC_API size_t glic_sparse_mesh_scratch_bytes(uint32_t n_blocks);
+GLIC_API size_t glic_sparse_mesh_extract_bytes(uint32_t vertices, uint32_t faces);
+GLIC_API int glic_sparse_mesh_count(const glic_sparse_tsdf* grid, void* scratch, size_t scratch_bytes, glic_sparse_mesh_counts* counts_host,
+                                    void* stream);
+GLIC_API int glic_sparse_mesh_extract(const glic_sparse_tsdf* grid, void* scratch, size_t scratch_bytes, const glic_sparse_mesh_counts* counts,
+                                      void* extract_ws, size_t extract_bytes, float* xyz, uint8_t* rgb, int32_t* faces, void* stream);
+GLIC_API int glic_debug_sparse_tsdf(const glic_sparse_tsdf* grid, uint64_t* keys, float* data, void* stream);
+
+/* Sparse meshing of the map.  glic_mapper_extract_mesh_sparse(m, p, out) is exactly this composition:
+ *   1. pass 1: for each listed training keyframe (p->views as glic_mapper_extract_mesh takes them), draw the map without the sky
+ *      exactly as glic_mapper_extract_mesh draws it and glic_block_set_insert its median depth under its mask, with p's origin,
+ *      voxel_size, trunc and max_depth; an insertion that overflows grows the set (glic_block_set_copy into twice the capacity)
+ *      and is repeated;
+ *   2. glic_sparse_tsdf_init a grid of the set's blocks;
+ *   3. pass 2: draw every listed view again and glic_sparse_tsdf_integrate its median depth and clamped rgb (the inference draw
+ *      is deterministic, so both passes see the same planes);
+ *   4. glic_sparse_mesh_count and glic_sparse_mesh_extract.
+ * max_blocks > 0 caps the set: a set of more blocks returns GLIC_ERR_WORKSPACE before the grid is allocated, changing nothing;
+ * so does a set of more than 2^23 - 1 blocks.
+ * *out (may be NULL): vertices, faces, observed points, blocks, the pixels clipped in pass 1 and the lattice bounding box.  On the
+ * same map, glic_mapper_extract_mesh with the same views, origin, voxel_size, trunc and max_depth and dims covering that box
+ * (lo >= 0) gives the same mesh arrays when nothing was clipped.  Everything else is glic_mapper_extract_mesh's contract: the
+ * frozen map, the drain, rank-local, the binning redraw (GLIC_ERR_WORKSPACE after four draws), the failure contract (the grid,
+ * scratch and set are this call's own and released when it returns; the pool is allocated after pass 1, once its size is known,
+ * and before the map or the previous mesh changes), and the new mesh replaces the last one only once it is complete, so
+ * glic_mapper_mesh_get and glic_mapper_save_mesh serve both calls.  A mapper that never calls it allocates and enqueues nothing
+ * for it.  Rejected with GLIC_ERR_INVALID_ARGUMENT, changing nothing: what glic_mapper_extract_mesh rejects but dims. */
+typedef struct glic_sparse_mesh_params {
+    const int* views;              /* host, training keyframe indices; NULL: every training keyframe */
+    int n_views;
+    float origin[3];               /* the lattice's alignment; there is no box */
+    float voxel_size;
+    float trunc;
+    float max_depth;
+    uint32_t max_blocks;           /* 0: no limit */
+} glic_sparse_mesh_params;
+GLIC_API int glic_mapper_extract_mesh_sparse(glic_mapper* m, const glic_sparse_mesh_params* p, glic_sparse_mesh_counts* out /* may be NULL */);
+
+/* ---------------------------------------------------------------------------------------
  * Pose corrections: moving the map with corrected keyframe poses (loop closure, a smoother's
  * revision, a re-anchored trajectory).
  *
