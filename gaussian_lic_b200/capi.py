@@ -293,6 +293,9 @@ def _load():
         "glic_mapper_anchors": (i32, [vp, vp]),
         "glic_mapper_set_anchors": (i32, [vp, vp]),
         "glic_mapper_correct_poses": (i32, [vp, i32, C.POINTER(PoseCorrection), C.POINTER(u32)]),
+        "glic_mapper_save_checkpoint": (i32, [vp, C.c_char_p]),
+        "glic_mapper_checkpoint_config": (i32, [C.c_char_p, C.POINTER(MapperConfig)]),
+        "glic_mapper_load_checkpoint": (i32, [vp, C.c_char_p]),
         "glic_debug_geom": (i32, [i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "glic_debug_binning": (i32, [i32, vp, i64, i64, vp, vp, vp, vp]),
         "glic_debug_image": (i32, [i32, i32, vp, vp, vp, vp, vp, C.POINTER(i64), vp]),

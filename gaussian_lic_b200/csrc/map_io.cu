@@ -148,3 +148,344 @@ int glic_ply_write_packed(const char* path, uint32_t P, uint32_t M, const float*
 }
 
 }  // extern "C"
+
+// ---- mapper checkpoints (include/glic_b200.h "Checkpoints"): the file's framing, its fixed fields and their validation.  Host-only
+// code: mapper.cu moves the arrays between the file and the device.
+#include "checkpoint.h"
+
+#include <cerrno>
+#include <sstream>
+#include <unistd.h>
+
+namespace glic {
+namespace ckpt {
+
+namespace {
+
+constexpr char MAGIC[8] = {'G', 'L', 'I', 'C', 'C', 'K', 'P', 'T'};
+constexpr int MAX_SLOTS = 32;                    // mapper.cu: world * views_per_rank
+constexpr uint32_t MAX_RNG_TEXT = 1u << 16;
+
+int bad(const std::string& why) { set_error("checkpoint: " + why); return GLIC_ERR_INVALID_ARGUMENT; }
+
+// a cursor over fixed fields read from the file
+struct Get {
+    const uint8_t* p;
+    const uint8_t* end;
+    template <typename T> T get() {
+        T v;
+        std::memcpy(&v, p, sizeof(T));
+        p += sizeof(T);
+        return v;
+    }
+    template <typename T> void get_n(T* v, size_t n) { std::memcpy(v, p, n * sizeof(T)); p += n * sizeof(T); }
+};
+
+struct Reader {
+    FILE* f = nullptr;
+    uint64_t size = 0;
+    ~Reader() { if (f) std::fclose(f); }
+    // n bytes at offset off into out (the caller has checked that they lie in the file)
+    int at(uint64_t off, size_t n, std::vector<uint8_t>& out) {
+        out.resize(n);
+        if (fseeko(f, (off_t)off, SEEK_SET) != 0 || std::fread(out.data(), 1, n, f) != n) return bad("read error");
+        return GLIC_OK;
+    }
+};
+
+bool config_valid(const glic_mapper_config& c) {
+    return c.width > 0 && c.height > 0 && c.sh_degree >= 0 && c.sh_degree <= 3 && c.world >= 1 && c.world <= 8 && c.rank >= 0 &&
+           c.rank < c.world && c.views_per_rank >= 1 && c.world * c.views_per_rank <= MAX_SLOTS && c.capacity >= 256 &&
+           c.capacity % 256 == 0 && c.max_iters > 0;
+}
+
+int get_config(const uint8_t* h, glic_mapper_config& c) {
+    if (std::memcmp(h, MAGIC, 8) != 0) return bad("not a mapper checkpoint (bad magic)");
+    uint32_t version;
+    std::memcpy(&version, h + 8, 4);
+    if (version != VERSION) return bad("unsupported version " + std::to_string(version));
+    Get g{h + 12, h + HEADER_BYTES};
+    c.width = g.get<int32_t>(); c.height = g.get<int32_t>();
+    c.fx = g.get<float>(); c.fy = g.get<float>(); c.cx = g.get<float>(); c.cy = g.get<float>();
+    c.sh_degree = g.get<int32_t>();
+    c.position_lr = g.get<float>(); c.feature_lr = g.get<float>(); c.opacity_lr = g.get<float>(); c.scaling_lr = g.get<float>();
+    c.rotation_lr = g.get<float>(); c.lambda_dssim = g.get<float>(); c.scaling_scale = g.get<float>();
+    c.capacity = g.get<uint32_t>(); c.max_iters = g.get<int32_t>(); c.seed = g.get<uint64_t>();
+    c.rank = g.get<int32_t>(); c.world = g.get<int32_t>(); c.views_per_rank = g.get<int32_t>();
+    if (!config_valid(c)) return bad("configuration out of range");
+    return GLIC_OK;
+}
+
+int read_header(Reader& r, const char* path, glic_mapper_config& c) {
+    r.f = std::fopen(path, "rb");
+    if (!r.f) return bad(std::string("cannot open ") + path);
+    if (fseeko(r.f, 0, SEEK_END) != 0) return bad("cannot seek");
+    r.size = (uint64_t)ftello(r.f);
+    if (r.size < HEADER_BYTES) return bad("truncated header");
+    std::vector<uint8_t> h;
+    if (int e = r.at(0, HEADER_BYTES, h)) return e;
+    return get_config(h.data(), c);
+}
+
+}  // namespace
+
+void put_config(Bytes& b, const glic_mapper_config& c) {
+    b.put<int32_t>(c.width).put<int32_t>(c.height).put(c.fx).put(c.fy).put(c.cx).put(c.cy).put<int32_t>(c.sh_degree);
+    b.put(c.position_lr).put(c.feature_lr).put(c.opacity_lr).put(c.scaling_lr).put(c.rotation_lr).put(c.lambda_dssim).put(c.scaling_scale);
+    b.put<uint32_t>(c.capacity).put<int32_t>(c.max_iters).put<uint64_t>(c.seed).put<int32_t>(c.rank).put<int32_t>(c.world)
+     .put<int32_t>(c.views_per_rank);
+}
+
+void put_stats(Bytes& b, const glic_mapper_stats& s) {
+    b.put(s.num_gaussians).put(s.capacity).put(s.iterations).put(s.last_inserted).put(s.last_loss).put(s.mean_visible)
+     .put(s.overflow_regrows).put(s.ms_extend).put(s.ms_optimize);
+}
+
+void put_schedule(Bytes& b, uint32_t on, const glic_density_schedule& s, const glic_density_counts& t, uint32_t steps, uint32_t resets) {
+    b.put(on).put(s.densify_from).put(s.densify_until).put(s.densify_interval).put(s.opacity_reset_interval).put(s.grad_threshold)
+     .put(s.percent_dense).put(s.min_opacity).put(s.reset_opacity).put(s.screen_radius).put(s.world_scale_factor).put(s.scene_extent);
+    b.put(t.cloned).put(t.split).put(t.pruned).put(t.rows).put(steps).put(resets);
+}
+
+void put_frame_stats(Bytes& b, const glic_frame_stats& s) {
+    b.put(s.frames).put(s.train).put(s.test).put(s.pending_points).put(s.image_bytes);
+}
+
+Writer::~Writer() {
+    if (f_) { std::fclose(f_); std::remove(tmp_.c_str()); }
+}
+
+int Writer::open(const char* path) {
+    path_ = path;
+    tmp_ = path_ + ".tmp";
+    f_ = std::fopen(tmp_.c_str(), "wb");
+    if (!f_) return bad("cannot create " + tmp_);
+    return GLIC_OK;
+}
+
+int Writer::header(const glic_mapper_config& cfg) {
+    Bytes b;
+    b.put_n(MAGIC, 8).put(VERSION);
+    put_config(b, cfg);
+    return write(b.b.data(), b.b.size());
+}
+
+int Writer::begin(Section s, uint64_t length) {
+    if (open_section_) return bad("internal: a section was left open");
+    Bytes b;
+    b.put(TAGS[s]).put<uint32_t>(0).put(length);
+    if (int e = write(b.b.data(), b.b.size())) return e;
+    left_ = length;
+    open_section_ = true;
+    return GLIC_OK;
+}
+
+int Writer::write(const void* p, size_t n) {
+    if (open_section_) {
+        if (n > left_) return bad("internal: a section is longer than its declared length");
+        left_ -= n;
+    }
+    if (n && std::fwrite(p, 1, n, f_) != n) return bad("short write to " + tmp_ + ": " + std::strerror(errno));
+    return GLIC_OK;
+}
+
+int Writer::end() {
+    if (!open_section_ || left_) return bad("internal: a section is shorter than its declared length");
+    open_section_ = false;
+    return GLIC_OK;
+}
+
+int Writer::commit() {
+    if (open_section_) return bad("internal: a section was left open");
+    Bytes b;
+    b.put(END_TAG).put<uint32_t>(0).put<uint64_t>(0);
+    if (int e = write(b.b.data(), b.b.size())) return e;
+    if (std::fflush(f_) != 0 || fsync(fileno(f_)) != 0) return bad("cannot flush " + tmp_ + ": " + std::strerror(errno));
+    const int closed = std::fclose(f_);
+    f_ = nullptr;
+    if (closed != 0 || std::rename(tmp_.c_str(), path_.c_str()) != 0) {
+        std::remove(tmp_.c_str());
+        return bad("cannot replace " + path_ + ": " + std::strerror(errno));
+    }
+    return GLIC_OK;
+}
+
+int read_info(const char* path, Info& o) {
+    Reader r;
+    if (int e = read_header(r, path, o.cfg)) return e;
+    const int W = o.cfg.width, H = o.cfg.height, M = (o.cfg.sh_degree + 1) * (o.cfg.sh_degree + 1) - 1;
+    // the section table: every tag known and present once, every length inside the file, the end marker last
+    uint64_t off[N_SECTIONS], len[N_SECTIONS];
+    bool seen[N_SECTIONS] = {};
+    uint64_t pos = HEADER_BYTES;
+    std::vector<uint8_t> buf;
+    for (;;) {
+        if (r.size - pos < FRAME_BYTES) return bad("truncated file (section frame)");
+        if (int e = r.at(pos, FRAME_BYTES, buf)) return e;
+        Get g{buf.data(), buf.data() + FRAME_BYTES};
+        const uint32_t tag = g.get<uint32_t>(), zero = g.get<uint32_t>();
+        const uint64_t n = g.get<uint64_t>();
+        pos += FRAME_BYTES;
+        if (zero != 0) return bad("bad section frame");
+        if (tag == END_TAG) {
+            if (n != 0) return bad("bad end marker");
+            if (pos != r.size) return bad("trailing bytes after the end marker");
+            break;
+        }
+        int s = 0;
+        while (s < N_SECTIONS && TAGS[s] != tag) ++s;
+        if (s == N_SECTIONS) return bad("unknown section");
+        if (seen[s]) return bad("duplicated section");
+        if (n > r.size - pos) return bad("truncated file (section longer than the file)");
+        seen[s] = true; off[s] = pos; len[s] = n;
+        pos += n;
+    }
+    for (int s : {MAP, COUNTERS, KEYFRAMES, SCHEDULE})
+        if (!seen[s]) return bad("missing section");
+    auto fixed = [&](Section s, size_t n, std::vector<uint8_t>& b) -> int {
+        if (len[s] < n) return bad("section length disagrees with its counts");
+        return r.at(off[s], n, b);
+    };
+    auto length_is = [&](Section s, uint64_t want) { return len[s] == want ? GLIC_OK : bad("section length disagrees with its counts"); };
+    // CNTR
+    if (int e = fixed(COUNTERS, 92, buf)) return e;
+    {
+        Get g{buf.data(), buf.data() + buf.size()};
+        glic_mapper_stats& s = o.st;
+        s.num_gaussians = g.get<uint32_t>(); s.capacity = g.get<uint32_t>(); s.iterations = g.get<uint64_t>();
+        s.last_inserted = g.get<uint32_t>(); s.last_loss = g.get<float>(); s.mean_visible = g.get<double>();
+        s.overflow_regrows = g.get<uint32_t>(); s.ms_extend = g.get<float>(); s.ms_optimize = g.get<float>();
+        o.view_counter = g.get<uint64_t>(); o.bin_cap = g.get<int64_t>(); o.binning_bytes = g.get<uint64_t>(); o.sample_bytes = g.get<uint64_t>();
+        o.optimizer = g.get<uint32_t>(); o.deterministic = g.get<uint32_t>(); o.flags = g.get<uint32_t>();
+        const uint32_t rng_len = g.get<uint32_t>();
+        if (rng_len > MAX_RNG_TEXT) return bad("view sampler state too long");
+        if (int e = length_is(COUNTERS, counters_bytes(rng_len))) return e;
+        if (o.optimizer > 1 || o.deterministic > 1 || (o.flags & ~F_ALL) || o.bin_cap < 0) return bad("counters out of range");
+        std::vector<uint8_t> text;
+        if (int e = r.at(off[COUNTERS] + 92, rng_len, text)) return e;
+        std::istringstream in(std::string(text.begin(), text.end()));
+        in >> o.rng;
+        if (in.fail() || (in >> std::ws, !in.eof())) return bad("unreadable view sampler state");
+    }
+    const bool expo = o.flags & F_EXPOSURE, pose = o.flags & F_POSE, dens = o.flags & F_DENSIFICATION, frames = o.flags & F_FRAMES;
+    const bool want[N_SECTIONS] = {true, true, true, expo, pose, dens, true, frames};
+    for (int s = 0; s < N_SECTIONS; ++s)
+        if (seen[s] != want[s]) return bad(seen[s] ? "section of a feature that is off" : "missing section");
+    // MAP
+    if (int e = fixed(MAP, 12, buf)) return e;
+    {
+        Get g{buf.data(), buf.data() + buf.size()};
+        o.P = g.get<uint32_t>(); o.Pcap = g.get<uint32_t>(); o.n_sky = g.get<uint32_t>();
+        if (o.P > o.Pcap || o.n_sky > o.P) return bad("row counts out of range");
+        if (o.Pcap != o.cfg.capacity || o.st.capacity != o.Pcap || o.st.num_gaussians != o.P) return bad("row counts disagree between sections");
+        if (int e = length_is(MAP, map_bytes(o.P, M))) return e;
+        o.map_off = off[MAP] + 12;
+    }
+    // FRMS (before the keyframes, which refer to its frame store)
+    const uint64_t stride = frame_stride(W, H);
+    if (frames) {
+        if (int e = fixed(FRAMES, 36, buf)) return e;
+        Get g{buf.data(), buf.data() + buf.size()};
+        o.frame_k = g.get<int32_t>(); o.sky_points = g.get<int32_t>(); o.sky_radius = g.get<int32_t>();
+        glic_frame_stats& s = o.fst;
+        s.frames = g.get<uint32_t>(); s.train = g.get<uint32_t>(); s.test = g.get<uint32_t>(); s.pending_points = g.get<uint32_t>();
+        s.image_bytes = g.get<uint64_t>();
+        if (int e = length_is(FRAMES, frames_bytes(s.pending_points))) return e;
+        if (o.frame_k < 1 || o.sky_points < 0 || (o.sky_points > 0 && o.sky_radius <= 0) || (uint64_t)s.train + s.test != s.frames ||
+            s.image_bytes != (uint64_t)((s.frames + FRAME_CHUNK - 1) / FRAME_CHUNK) * FRAME_CHUNK * stride ||
+            (uint64_t)s.pending_points + (uint64_t)o.sky_points > INT32_MAX / 4)
+            return bad("frame settings out of range");
+        o.frames_off = off[FRAMES] + 36;
+    }
+    // KEYF: walk the records
+    if (int e = fixed(KEYFRAMES, 8, buf)) return e;
+    {
+        Get g{buf.data(), buf.data() + buf.size()};
+        o.n_train = g.get<uint32_t>(); o.n_test = g.get<uint32_t>();
+        uint64_t at = off[KEYFRAMES] + 8, end = off[KEYFRAMES] + len[KEYFRAMES];
+        const uint64_t n = (uint64_t)o.n_train + o.n_test;
+        if (n > (end - at) / KEYFRAME_RECORD_BYTES) return bad("section length disagrees with its counts");
+        o.kf.resize(n);
+        std::vector<uint8_t> used(frames ? o.fst.frames : 0, 0);
+        uint64_t n_frames = 0;
+        for (Keyframe& k : o.kf) {
+            if (end - at < KEYFRAME_RECORD_BYTES) return bad("section length disagrees with its counts");
+            if (int e = r.at(at, KEYFRAME_RECORD_BYTES, buf)) return e;
+            Get q{buf.data(), buf.data() + buf.size()};
+            q.get_n(k.R_wc, 9); q.get_n(k.t_wc, 3); q.get_n(k.cam, 42); q.get_n(k.cam_dev, 36);
+            k.kind = q.get<uint32_t>(); k.frame = q.get<uint32_t>(); k.mask_valid = q.get<uint32_t>(); k.mask_valid_left = q.get<uint32_t>();
+            if (k.kind > IMAGE_DEVICE || k.mask_valid > (uint64_t)W * H || k.mask_valid_left > k.mask_valid) return bad("keyframe record out of range");
+            if (k.kind == IMAGE_BGR8) {
+                if (!frames || k.frame >= o.fst.frames || used[k.frame]) return bad("keyframe frame index out of range");
+                used[k.frame] = 1;
+                ++n_frames;
+            } else if (k.frame != NO_FRAME) {
+                return bad("keyframe record out of range");
+            }
+            const uint64_t b = keyframe_bytes(k.kind, k.mask_valid, W, H);
+            if (end - at < b) return bad("section length disagrees with its counts");
+            k.image_off = at + KEYFRAME_RECORD_BYTES;
+            k.mask_off = k.image_off + (k.kind == IMAGE_BGR8 ? 3 : 12) * (uint64_t)W * H;
+            at += b;
+        }
+        if (at != end) return bad("section length disagrees with its counts");
+        if (frames && n_frames != o.fst.frames) return bad("keyframe counts disagree between sections");
+    }
+    // EXPO, POSE
+    if (expo) {
+        if (int e = fixed(EXPOSURE, 8, buf)) return e;
+        Get g{buf.data(), buf.data() + buf.size()};
+        o.expo_lr = g.get<float>();
+        const uint32_t n = g.get<uint32_t>();
+        if (n != o.n_train) return bad("keyframe counts disagree between sections");
+        if (int e = length_is(EXPOSURE, exposure_bytes(n))) return e;
+        o.expo_off = off[EXPOSURE] + 8;
+    }
+    if (pose) {
+        if (int e = fixed(POSE, 12, buf)) return e;
+        Get g{buf.data(), buf.data() + buf.size()};
+        o.pose_lr_rho = g.get<float>(); o.pose_lr_omega = g.get<float>();
+        const uint32_t n = g.get<uint32_t>();
+        if (n != o.n_train) return bad("keyframe counts disagree between sections");
+        if (int e = length_is(POSE, pose_bytes(n))) return e;
+        o.pose_off = off[POSE] + 12;
+    }
+    // DENS
+    if (dens) {
+        if (int e = fixed(DENSIFICATION, 12, buf)) return e;
+        Get g{buf.data(), buf.data() + buf.size()};
+        o.dens_calls = g.get<uint64_t>();
+        if (g.get<uint32_t>() != o.P) return bad("row counts disagree between sections");
+        if (int e = length_is(DENSIFICATION, densification_bytes(o.P))) return e;
+        o.dens_off = off[DENSIFICATION] + 12;
+    }
+    // SCHD
+    if (int e = length_is(SCHEDULE, SCHEDULE_BYTES)) return e;
+    if (int e = fixed(SCHEDULE, SCHEDULE_BYTES, buf)) return e;
+    {
+        Get g{buf.data(), buf.data() + buf.size()};
+        glic_density_schedule& s = o.sched;
+        o.sched_on = g.get<uint32_t>();
+        s.densify_from = g.get<uint32_t>(); s.densify_until = g.get<uint32_t>(); s.densify_interval = g.get<uint32_t>();
+        s.opacity_reset_interval = g.get<uint32_t>(); s.grad_threshold = g.get<float>(); s.percent_dense = g.get<float>();
+        s.min_opacity = g.get<float>(); s.reset_opacity = g.get<float>(); s.screen_radius = g.get<int32_t>();
+        s.world_scale_factor = g.get<float>(); s.scene_extent = g.get<float>();
+        glic_density_counts& t = o.sched_totals;
+        t.cloned = g.get<uint32_t>(); t.split = g.get<uint32_t>(); t.pruned = g.get<uint32_t>(); t.rows = g.get<uint32_t>();
+        o.sched_steps = g.get<uint32_t>(); o.sched_resets = g.get<uint32_t>();
+        if (o.sched_on > 1 || (o.sched_on && (!dens || s.densify_interval == 0))) return bad("density schedule out of range");
+    }
+    return GLIC_OK;
+}
+
+}  // namespace ckpt
+}  // namespace glic
+
+extern "C" int glic_mapper_checkpoint_config(const char* path, glic_mapper_config* out) {
+    if (!path || !out) { set_error("mapper_checkpoint_config: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
+    glic::ckpt::Reader r;
+    glic_mapper_config c{};
+    if (int e = glic::ckpt::read_header(r, path, c)) return e;
+    *out = c;
+    return GLIC_OK;
+}

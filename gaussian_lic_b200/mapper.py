@@ -74,6 +74,13 @@ def sh_rotation(q, degree=3):
     return _sh_blocks(out, degree)
 
 
+def checkpoint_config(path):
+    """The configuration (capi.MapperConfig, capacity = the saved arena capacity) of a checkpoint file; host only."""
+    cfg = capi.MapperConfig()
+    capi.check(capi.lib.glic_mapper_checkpoint_config(str(path).encode(), C.byref(cfg)), "mapper_checkpoint_config")
+    return cfg
+
+
 class Mapper:
     def __init__(self, W, H, fx, fy, cx, cy, sh_degree=3, capacity=0, max_iters=100, seed=0, rank=0, world=1, views_per_rank=1,
                  **lrs):
@@ -84,12 +91,32 @@ class Mapper:
             setattr(cfg, k, float(v))
         cfg.capacity, cfg.max_iters, cfg.seed = int(capacity), int(max_iters), int(seed)
         cfg.rank, cfg.world, cfg.views_per_rank = int(rank), int(world), int(views_per_rank)
+        self._create(cfg)
+
+    def _create(self, cfg):
         self.cfg = cfg
-        self.M = (sh_degree + 1) ** 2 - 1
-        self.W, self.H = int(W), int(H)
+        self.M = (cfg.sh_degree + 1) ** 2 - 1
+        self.W, self.H = int(cfg.width), int(cfg.height)
         self._h = C.c_void_p()
         self._keep = []                                   # host arrays the C++ side points into
         capi.check(capi.lib.glic_mapper_create(C.byref(cfg), C.byref(self._h)), "mapper_create")
+
+    @classmethod
+    def from_checkpoint(cls, path, lpips=None):
+        """A new mapper that continues from a file of save_checkpoint(): created with the file's configuration (checkpoint_config),
+        with the LPIPS weights of `lpips` (a glic_lpips weight file; they are not in the checkpoint) loaded, then restored.  The
+        restored mapper owns its keyframe images.  With world > 1, export_handle() / connect() follow."""
+        m = cls.__new__(cls)
+        m._h = C.c_void_p()
+        m._create(checkpoint_config(path))
+        try:
+            if lpips is not None:
+                m.load_lpips(lpips)
+            m.load_checkpoint(path)
+        except Exception:
+            m.close()
+            raise
+        return m
 
     def close(self):
         if self._h:
@@ -243,6 +270,16 @@ class Mapper:
 
     def save_map(self, path):
         capi.check(capi.lib.glic_mapper_save_map(self._h, str(path).encode()), "mapper_save_map")
+
+    def save_checkpoint(self, path):
+        """Write the whole mapper state to `path` (include/glic_b200.h "Checkpoints"): via <path>.tmp, renamed over path once
+        complete, so an existing file survives a failed save.  Changes nothing in the mapper."""
+        capi.check(capi.lib.glic_mapper_save_checkpoint(self._h, str(path).encode()), "mapper_save_checkpoint")
+
+    def load_checkpoint(self, path):
+        """Restore a checkpoint into this mapper, which must be fresh (created, with no rows, keyframes or features) and have the
+        file's configuration but for the capacity (see from_checkpoint)."""
+        capi.check(capi.lib.glic_mapper_load_checkpoint(self._h, str(path).encode()), "mapper_load_checkpoint")
 
     def stats(self):
         st = capi.MapperStats()

@@ -1366,6 +1366,81 @@ GLIC_API int glic_mapper_set_anchors(glic_mapper* m, const int32_t* in /*[P]*/);
 GLIC_API int glic_mapper_correct_poses(glic_mapper* m, int n, const glic_pose_correction* c, uint32_t* moved /* may be NULL */);
 
 /* ---------------------------------------------------------------------------------------
+ * Checkpoints: the mapper's whole state in one file, and a new mapper (in a new process, on another machine) that continues
+ * from it.
+ *
+ * Resume: glic_mapper_checkpoint_config(path, &cfg) -> glic_mapper_create(&cfg) -> [glic_mapper_load_lpips, glic_mapper_set_option]
+ * -> glic_mapper_load_checkpoint -> (world > 1: glic_mapper_export / glic_mapper_connect) -> carry on.  A restored mapper returns
+ * what the saved one returned from every getter, bit for bit, and under GLIC_MAPPER_OPT_DETERMINISTIC it trains on exactly as the
+ * saved one would have (same GPU model and library build).  Without the option the restored state is still exact; continued
+ * training differs as any two runs do (float atomics).
+ *
+ * glic_mapper_save_checkpoint(m, path): drains the iteration pipeline (the lagged overflow ring included) and synchronises, then
+ * writes the file; it changes nothing in the mapper.  The arrays stream through a pinned staging buffer of two 8 MiB chunks (the
+ * device-to-host copy of one, on the copy stream, overlaps the write of the other), so host memory does not grow with the map or
+ * the keyframes; float keyframe images in host memory are written from where the caller keeps them.  The file is written as
+ * <path>.tmp in the same directory, flushed (fflush, fsync) and renamed over path: on any failure the temporary file is removed and
+ * an existing file at path is left as it was.  A connected mapper (world > 1) may save; each rank writes its own file.
+ * glic_mapper_checkpoint_config(path, out): host only, no device: the configuration of the fixed header, capacity = the saved arena
+ * capacity.  A missing or unreadable file, a short header, a bad magic or version, or a configuration glic_mapper_create would
+ * refuse (or a capacity that is not a positive multiple of 256) return GLIC_ERR_INVALID_ARGUMENT.
+ * glic_mapper_load_checkpoint(m, path): m must be fresh: created, with no rows (no initialize), no keyframe, no feature enabled
+ * (exposure, pose refinement, densification, frames) and not exported; load_lpips and set_option before it are allowed, and the
+ * file's options replace them.  The configuration must equal the file's in every field but capacity (floats by their bits); the
+ * mapper takes the saved capacity.  The whole file is validated before anything is allocated; GLIC_ERR_INVALID_ARGUMENT, with the
+ * mapper still fresh, for: a bad magic or version, a section frame with a non-zero reserved word, a missing, duplicated or unknown
+ * section (or one of a feature the counters say is off), a section length that disagrees with its counts, P > capacity, sky rows >
+ * P, counts that disagree between sections (rows, keyframes, frames), a truncated file or bytes after the end marker, an
+ * out-of-range field, a configuration mismatch, or a mapper that is not fresh.  Every allocation (keyframes, frame store, then the
+ * arenas and workspaces at the saved capacity, the binning workspaces at their saved sizes, the deterministic workspace as
+ * set_option sizes it) is made before any state is swapped in: a failed one returns GLIC_ERR_CUDA and leaves the mapper fresh, so a
+ * second load can succeed.  Float keyframe images keep their memory class in mapper-owned memory (device memory read in place by
+ * the loss, or pinned host memory), released by glic_mapper_destroy; 8-bit frames go back into the frame store and the pending scan
+ * into the scan buffers.  Synchronises.  With world > 1, rank and world must match the file (they are configuration fields) and
+ * the load comes before glic_mapper_export.
+ * Not saved: the LPIPS weights (a file the caller has: call glic_mapper_load_lpips again), the last mesh (derived: extract it
+ * again), and every workspace's contents (scratch that each call rewrites before reading).
+ *
+ * The file (version 1, little-endian, no padding; u32 / i32 / u64 / i64 / f32 / f64 are the usual fixed-width types):
+ *   header, 96 bytes: u8 magic[8] = "GLICCKPT" | u32 version = 1 | the glic_mapper_config fields in declaration order, one by one:
+ *     i32 width, height | f32 fx, fy, cx, cy | i32 sh_degree | f32 position_lr, feature_lr, opacity_lr, scaling_lr, rotation_lr,
+ *     lambda_dssim, scaling_scale | u32 capacity (the arena capacity Pcap) | i32 max_iters | u64 seed | i32 rank, world,
+ *     views_per_rank
+ *   then sections, each: u32 tag (four ASCII bytes) | u32 0 | u64 length (bytes of payload that follow), in any order, each at
+ *   most once; then the end marker "END " | 0 | 0, which ends the file.  M = (sh_degree + 1)^2 - 1; P = rows; n = training
+ *   keyframes.
+ *   "MAP " (always), 12 + P (12 (14 + 3M) + 4) bytes: u32 P, Pcap, n_sky | for each of params, exp_avg, exp_avg_sq: f32 rows
+ *     [0, P) of rot [P][4], xyz [P][3], log_scale [P][3], opacity [P], f_dc [P][3], f_rest [P][M][3] | i32 anchor [P]
+ *   "CNTR" (always), 92 + L bytes: glic_mapper_stats field by field (u32 num_gaussians, capacity | u64 iterations | u32
+ *     last_inserted | f32 last_loss | f64 mean_visible | u32 overflow_regrows | f32 ms_extend, ms_optimize) | u64 view_counter
+ *     (images sent through the double buffer) | i64 bin_cap (the binning capacity in pairs: a frame needing more is skipped, so it
+ *     changes training) | u64 binning and sample workspace bytes (bin_cap is the largest capacity both hold) | u32 optimizer,
+ *     deterministic (GLIC_MAPPER_OPT_* values, 0 or 1) | u32 flags (1 initialized, 2 exposure, 4 pose refinement, 8 densification,
+ *     16 frames) | u32 L | u8 [L] the view sampler's std::mt19937_64 as its operator<< writes it (decimal words)
+ *   "KEYF" (always): u32 n, n_test | n + n_test records, training then held-out, each: f32 R_wc[9], t_wc[3] | f32 cam[42], the host
+ *     camera block (view16 proj16 campos4 tanfovx tanfovy lim4) | f32 cam_dev[36], the device camera block copied back verbatim
+ *     (view16 proj16 campos4) | u32 image kind (0: 8-bit add_frame image, 1: float image in host memory, 2: float image in
+ *     device memory) | u32 frame (kind 0: its slot in the frame store, in add_frame order; else 0xFFFFFFFF) | u32 mask_valid,
+ *     mask_valid_left | the image: kind 0 u8 [H][W][3] BGR, else f32 [3][H][W] | u32 mask words [H][(W + 31) / 32] when mask_valid
+ *     > 0 (bit x & 31 of word x >> 5 of a row: pixel x used)
+ *   "EXPO" (exposure on), 8 + 148 n bytes: f32 exposure_lr | u32 n | f32 E [n][12], exp_avg [n][12], exp_avg_sq [n][12] | i32
+ *     step [n]
+ *   "POSE" (pose refinement on), 12 + 196 n bytes: f32 lr_translation, lr_rotation | u32 n | f64 T_cw [n][12] (R_cw row-major |
+ *     t_cw) | f32 pose [n][12] (R_wc | t_wc) | f32 exp_avg [n][6], exp_avg_sq [n][6] | i32 step [n]
+ *   "DENS" (densification on), 12 + 12 P bytes: u64 densify calls so far | u32 P | f32 grad_accum [P], denom [P] | i32 max screen
+ *     radius [P]
+ *   "SCHD" (always), 72 bytes: u32 schedule set | glic_density_schedule field by field | glic_density_counts totals field by field
+ *     | u32 steps, resets
+ *   "FRMS" (frames on), 36 + 19 p bytes: i32 select_every_k_frame, sky_points, sky_radius | glic_frame_stats field by field (u32
+ *     frames, train, test, pending_points p | u64 image_bytes) | the pending scan: f32 xyz [p][3] | u8 rgb [p][3] | f32 depth [p]
+ * Bytes per row at degree 3: 712 (+ 12 with densification); per keyframe at 1920x1080: 6.22 MB (8-bit) or 24.9 MB (float), plus
+ * 259 200 per mask.
+ * ------------------------------------------------------------------------------------- */
+GLIC_API int glic_mapper_save_checkpoint(glic_mapper* m, const char* path);
+GLIC_API int glic_mapper_checkpoint_config(const char* path, glic_mapper_config* out);   /* host only, no device */
+GLIC_API int glic_mapper_load_checkpoint(glic_mapper* m, const char* path);
+
+/* ---------------------------------------------------------------------------------------
  * Stage timing (cudaEvent pairs recorded on the launching stream around each stage; off by
  * default).  glic_profile_enable(1) starts recording and resets the accumulators;
  * glic_profile_read() synchronises the recorded events and returns, per stage, the summed
