@@ -15,7 +15,7 @@ OBJ = os.path.join(PKG, "_build")
 LIB = os.path.join(PKG, "libglic_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 HOST_CXX = "/usr/bin/g++"
-CU_SOURCES = ["c_api.cu", "preprocess.cu", "radix_sort.cu", "render.cu", "preprocess_backward.cu", "ssim.cu", "adam_knn.cu", "p2p.cu", "model_step.cu", "map_io.cu", "extend.cu", "initialize.cu", "frames.cu", "lpips.cu", "prune.cu", "mesh.cu", "sparse_mesh.cu", "pose_correction.cu", "mapper.cu"]
+CU_SOURCES = ["c_api.cu", "preprocess.cu", "radix_sort.cu", "render.cu", "preprocess_backward.cu", "ssim.cu", "adam_knn.cu", "p2p.cu", "model_step.cu", "map_io.cu", "extend.cu", "initialize.cu", "frames.cu", "lpips.cu", "prune.cu", "mesh.cu", "sparse_mesh.cu", "pose_correction.cu", "mapper.cu", "mapper_density.cu", "mapper_views.cu", "mapper_mesh.cu", "mapper_checkpoint.cu"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-ccbin", HOST_CXX,
               "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 

@@ -1,6 +1,6 @@
 // checkpoint.h -- the mapper checkpoint file (include/glic_b200.h "Checkpoints"): what map_io.cu's host-only reader hands
-// mapper.cu, and the writer's framing.  No CUDA here: map_io.cu reads and writes the file, mapper.cu moves the bytes between it
-// and the device.
+// mapper_checkpoint.cu, and the writer's framing.  No CUDA here: map_io.cu reads and writes the file, mapper_checkpoint.cu moves
+// the bytes between it and the device.
 #pragma once
 
 #include "../../include/glic_b200.h"
@@ -33,6 +33,19 @@ constexpr uint32_t END_TAG = fourcc("END ");
 enum : uint32_t { F_INITIALIZED = 1, F_EXPOSURE = 2, F_POSE = 4, F_DENSIFICATION = 8, F_FRAMES = 16, F_ALL = 31 };
 enum : uint32_t { IMAGE_BGR8 = 0, IMAGE_HOST = 1, IMAGE_DEVICE = 2 };
 
+// Bytes per row of each array of the per-row sections, in file order.  The mapper's buffer groups (mapper_state.cuh) are sized,
+// saved and loaded with these widths, so the mapper and the reader agree on every section's length.
+constexpr size_t EXPOSURE_ROW[] = {48, 48, 48, 4};        // E [3x4] f32 | Adam m, v [12] f32 | step i32
+constexpr size_t POSE_ROW[] = {96, 48, 24, 24, 4};        // T_cw [12] f64 | R_wc, t_wc [12] f32 | Adam m, v [6] f32 | step i32
+constexpr size_t DENSIFICATION_ROW[] = {4, 4, 4};         // gradient-norm sum f32 | view count f32 | largest screen radius i32
+constexpr size_t SCAN_ROW[] = {12, 3, 4};                 // pending scan point: xyz [3] f32 | rgb [3] u8 | depth f32
+template <size_t N>
+constexpr uint64_t row_bytes(const size_t (&widths)[N]) {
+    uint64_t sum = 0;
+    for (size_t w : widths) sum += w;
+    return sum;
+}
+
 // the section lengths the counts imply
 inline uint64_t map_bytes(uint64_t P, int M) { return 12 + P * (3 * 4 * (14 + 3 * (uint64_t)M) + 4); }
 inline uint64_t counters_bytes(uint64_t rng_len) { return 92 + rng_len; }
@@ -40,11 +53,11 @@ inline uint64_t keyframe_bytes(uint32_t kind, uint32_t mask_valid, int W, int H)
     const uint64_t HW = (uint64_t)W * H;
     return KEYFRAME_RECORD_BYTES + (kind == IMAGE_BGR8 ? 3 * HW : 12 * HW) + (mask_valid ? 4 * (uint64_t)H * ((W + 31) / 32) : 0);
 }
-inline uint64_t exposure_bytes(uint64_t n) { return 8 + 148 * n; }
-inline uint64_t pose_bytes(uint64_t n) { return 12 + 196 * n; }
-inline uint64_t densification_bytes(uint64_t P) { return 12 + 12 * P; }
+inline uint64_t exposure_bytes(uint64_t n) { return 8 + row_bytes(EXPOSURE_ROW) * n; }
+inline uint64_t pose_bytes(uint64_t n) { return 12 + row_bytes(POSE_ROW) * n; }
+inline uint64_t densification_bytes(uint64_t P) { return 12 + row_bytes(DENSIFICATION_ROW) * P; }
 constexpr uint64_t SCHEDULE_BYTES = 72;
-inline uint64_t frames_bytes(uint64_t pending) { return 36 + 19 * pending; }
+inline uint64_t frames_bytes(uint64_t pending) { return 36 + row_bytes(SCAN_ROW) * pending; }
 inline uint64_t frame_stride(int W, int H) { return (3 * (uint64_t)W * H + 255) & ~(uint64_t)255; }
 
 struct Keyframe {

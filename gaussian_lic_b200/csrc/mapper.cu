@@ -13,10 +13,8 @@
 //     copy engines over NVLink as soon as the render backward has produced them (overlapping the per-Gaussian backward),
 //     the 11 geometric floats are mean-reduced in place by the two-shot kernel of p2p.cu; every replica then runs the same
 //     Adam launch on the same bytes.  With densification on, the view's statistics ride along as two more rows (13 floats).
-#include "common.cuh"
+#include "mapper_state.cuh"
 #include "adam_math.cuh"
-#include "checkpoint.h"
-#include "mesh.cuh"
 #include "pose_correction.cuh"
 
 #include <algorithm>
@@ -26,26 +24,12 @@
 #include <cstring>
 #include <functional>
 #include <initializer_list>
-#include <limits>
 #include <memory>
 #include <nv/target>
-#include <random>
-#include <sstream>
 #include <utility>
 #include <vector>
 
-using namespace glic;
-
-namespace {
-
-constexpr int MAX_SLOTS = 32;        // world * views_per_rank
-static_assert(MAX_SLOTS <= EXPO_MAX_SLOTS, "the exposure step takes every slot of a batch");
-constexpr int RING = 8;              // pinned result ring (loss, binning counters)
-
-struct CamBlock {                    // what the rasterizer gets per view (camera.h:38-110, renderer.cpp:31-54)
-    float view[16], proj[16], campos[4];
-    float tanfovx, tanfovy, lim[4];
-};
+namespace mapper_impl {
 
 // the pose-independent projection P of camera.h (row-major), with the FoV from the intrinsics (float members)
 void proj_matrix(int W, int H, double fx, double fy, double cx, double cy, float* Pm, float* fov2) {
@@ -106,7 +90,7 @@ __host__ __device__ void pose_camera(const float* R_wc, const float* t_wc, const
 
 // camera.h:38-110 in closed form: FoV from the intrinsics (float members), pose_camera, the asymmetric clamp limits of :63-66
 void camera_block(int W, int H, double fx, double fy, double cx, double cy, const float* R_wc, const float* t_wc, CamBlock& o,
-                  double* T12 = nullptr) {
+                  double* T12) {
     float Pm[16], fov2[2];
     proj_matrix(W, H, fx, fy, cx, cy, Pm, fov2);
     pose_camera(R_wc, t_wc, Pm, o.view, T12);                         // view | proj | campos are contiguous
@@ -122,88 +106,11 @@ glic_view make_view(const CamBlock& c, const float* cam, int W, int H) {
     return glic_view{cam, cam + 16, cam + 32, c.tanfovx, c.tanfovy, c.lim[0], c.lim[1], c.lim[2], c.lim[3], W, H};
 }
 
-// ---- ownership: every CUDA resource of a mapper is a member of one of the two types below, and only they allocate or release
-// one.  The members release themselves, so destroying a mapper is a drain and a delete, and a failed create needs no cleanup.
 std::atomic<int> fail_countdown{0};          // glic_debug_fail_allocation
 std::atomic<int64_t> live_allocations{0};    // glic_debug_mapper_allocations
 
-// One device (or pinned host) allocation of a known size, move-only, released by its destructor
-class Buf {
-public:
-    Buf() = default;
-    Buf(Buf&& o) noexcept { *this = std::move(o); }
-    Buf& operator=(Buf&& o) noexcept {
-        if (this != &o) { release(); p_ = std::exchange(o.p_, nullptr); bytes_ = std::exchange(o.bytes_, 0); pinned_ = o.pinned_; }
-        return *this;
-    }
-    ~Buf() { release(); }
-    void* raw() const { return p_; }
-    size_t bytes() const { return bytes_; }
-    // on an empty Buf: `bytes` of device memory (of pinned host memory with `pinned`), not initialised
-    int allocate(size_t bytes, bool pinned = false) {
-        int n = fail_countdown.load();
-        while (n > 0 && !fail_countdown.compare_exchange_weak(n, n - 1)) {}
-        const cudaError_t e = n == 1 ? cudaErrorMemoryAllocation
-                            : pinned ? cudaHostAlloc(&p_, bytes, cudaHostAllocDefault) : cudaMalloc(&p_, bytes ? bytes : 256);
-        if (e != cudaSuccess) {
-            p_ = nullptr;
-            cudaGetLastError();                      // not left for the next launch check to report
-            set_error("mapper: allocation of " + std::to_string(bytes) + " bytes failed: " + cudaGetErrorString(e));
-            return GLIC_ERR_CUDA;
-        }
-        bytes_ = bytes; pinned_ = pinned; ++live_allocations;
-        return GLIC_OK;
-    }
-private:
-    void release() {
-        if (!p_) return;
-        if (pinned_) cudaFreeHost(p_); else cudaFree(p_);
-        --live_allocations; p_ = nullptr; bytes_ = 0;
-    }
-    void* p_ = nullptr;
-    size_t bytes_ = 0;
-    bool pinned_ = false;
-};
-// a Buf of T that converts to T*, so the launches take it as they would a raw pointer
-template <typename T>
-struct Dev : Buf {
-    operator T*() const { return static_cast<T*>(raw()); }
-};
-
-// a stream, an event or an IPC mapping, move-only, destroyed by its destructor
-template <typename H, cudaError_t (*Destroy)(H)>
-class Handle {
-public:
-    Handle() = default;
-    explicit Handle(H h) : h_(h) {}
-    Handle(Handle&& o) noexcept : h_(std::exchange(o.h_, nullptr)) {}
-    Handle& operator=(Handle&& o) noexcept { std::swap(h_, o.h_); return *this; }
-    ~Handle() { if (h_) Destroy(h_); }
-    operator H() const { return h_; }
-private:
-    H h_ = nullptr;
-};
-using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
-using Event = Handle<cudaEvent_t, cudaEventDestroy>;
-using IpcMapping = Handle<void*, cudaIpcCloseMemHandle>;
-
-struct Keyframe {                    // move-only: it owns its device camera block
-    float R_wc[9], t_wc[3];
-    const float* image = nullptr;
-    bool image_on_device = false;    // `image` is memory of the mapper's device: the loss reads it in place
-    Buf owned_image;                 // a float image restored from a checkpoint (device or pinned host memory): `image` points here
-    const uint8_t* bgr = nullptr;    // add_frame keyframes: packed HWC BGR8 in the frame store, decoded where `image` is copied
-    CamBlock cam;
-    Dev<float> cam_dev;              // view16 | proj16 | campos4
-    glic_view view;
-    // valid-pixel mask (glic_mapper_set_keyframe_mask): the packed bits, the number of used pixels (0: no mask) and how many
-    // of them lie in columns [0, W/2) (glic_mapper_align's split fit region)
-    Dev<uint32_t> mask;
-    uint32_t mask_valid = 0, mask_valid_left = 0;
-};
-
 // the view of kf's whole mask from column x0 on, or nullptr when kf has none
-const MaskView* keyframe_mask(const Keyframe& kf, int W, MaskView& mv, int x0 = 0) {
+const MaskView* keyframe_mask(const Keyframe& kf, int W, MaskView& mv, int x0) {
     if (!kf.mask_valid) return nullptr;
     mv = MaskView{kf.mask, mask_words_per_row(W), x0};
     return &mv;
@@ -262,12 +169,6 @@ __device__ __forceinline__ void pose_derive(const double* Rn, const double* tn, 
     pose_camera(f, f + 9, Pm, cam, nullptr);
 }
 
-struct PoseBatch {
-    int kf[MAX_SLOTS];                // keyframe of each slot
-    float* cam[MAX_SLOTS];            // its device camera block
-    float Pm[16];                     // the pose-independent projection (row-major)
-};
-
 // One thread per slot; the first slot that holds a keyframe steps it with the batch gradient of keyframe_batch_grad and
 // torch_adam_delta, as the exposure step does.  A set overflow word leaves the pose, m, v and t unchanged; an update of
 // exactly zero leaves the pose and its camera block unchanged.
@@ -324,7 +225,6 @@ pose_correct_kernel(int S, PoseBatch b, const glic_rigid_correction* __restrict_
 }
 
 // ---- raw frames (glic_mapper_add_frame; Dataset::addFrame, gaussian.cpp:41-111) -------------------------------------------
-constexpr size_t FRAME_CHUNK = ckpt::FRAME_CHUNK;    // frames per device allocation of the 8-bit image store
 
 // Eigen::Quaterniond(w, x, y, z).toRotationMatrix() in Eigen's operation order, without normalisation; q = (x, y, z, w).
 // Host code: x86-64 is compiled without FMA, so every operation rounds once.
@@ -358,132 +258,10 @@ __global__ void __launch_bounds__(256) scan_colour_kernel(int n3, const uint8_t*
     if (i < n3) out[i] = (T)__ddiv_rn((double)rgb[i], 255.0);
 }
 
-// Regions of the exchange block that hold one slot per (parity, view slot), in layout order
-enum SlotRegion { COLOUR, FLAGS, EXPOSURE, POSE, RADII, N_REGIONS };
-
-// Adam state of a per-training-keyframe parameter of `width` floats: moments [cap][width], step counts [cap]
-struct KeyframeAdam {
-    int width;
-    Dev<float> m, v;
-    Dev<int> t;
-};
-
-// The exchange block: geo[11*Pcap + 4 (+ 2*Pcap)] | flags words | one region [2][S] of slots per SlotRegion.  With densification
-// on, the reduced region ends in the batch's statistics rows: norms [Pcap] | view counts [Pcap], at 11*Pcap + 4.
-struct XLayout {
-    size_t n_geo = 0;                // floats in the reduced region (11*Pcap + 4; the tail holds the collective overflow word)
-    size_t bytes = 0, slot_off[N_REGIONS] = {}, slot_bytes[N_REGIONS] = {};
-};
-
-}  // namespace
-
-struct glic_mapper {
-    glic_mapper_config cfg{};
-    int dev = 0, D = 0, M = 0, S = 1, k = 1;
-    Stream stream, copy_stream, push_stream;
-    // ---- arenas (capacity Pcap) ----
-    uint32_t P = 0, Pcap = 0;
-    uint32_t n_sky = 0;                   // rows [0, n_sky) are the skybox (glic_mapper_initialize_lidar): left out of save_map
-    Dev<float> params, m1, m2;
-    Dev<int32_t> anchor;                  // [Pcap]: the training keyframe each row moves with (glic_mapper_correct_poses), or -1
-    Dev<float> act_opacity, act_scales, act_rots;
-    Dev<int> radii;
-    Dev<float> g_conic;                   // the render backward's 2-D gradient accumulators: conic [4 Pcap] | mean2D [3 Pcap] | opacity
-    float *g_mean2D = nullptr, *g_opacity = nullptr;
-    Dev<void> geom_ws;
-    Dev<char> xblock;
-    XLayout x;
-    void* peers[8] = {nullptr};
-    bool connected = false;
-    std::vector<IpcMapping> opened;
-    // ---- per-image buffers ----
-    Dev<void> image_ws, binning_ws, sample_ws, loss_scratch, eval_scratch, extend_ws;
-    int64_t bin_cap = 0;
-    // GLIC_MAPPER_OPT_DETERMINISTIC: the fixed-order render backward's workspace (glic_deterministic_bytes(bin_cap, W, H), grown
-    // with the binning capacity while the option is on) and the partials of the fixed-order loss and evaluation sums
-    bool deterministic = false;
-    Dev<void> det_ws, det_sums;
-    Dev<float> color, final_T, dL_dpix, gt_dev[2], loss_dev, eval_out;
-    Dev<unsigned int> vis_acc;
-    Event gt_free[2], gt_ready[2], ev_flags, ev_col, ev_push, ring_ev[RING], t0, t1;
-    Dev<long long> counters_host;         // pinned [RING][4]
-    Dev<float> loss_host;                 // pinned [RING]
-    bool ring_used[RING] = {false};
-    // ---- keyframes ----
-    std::vector<Keyframe> train, test;
-    std::mt19937_64 rng;
-    uint64_t view_counter = 0;
-    glic_mapper_stats st{};
-    bool run_optimizer = true;            // GLIC_MAPPER_OPT_OPTIMIZER (benchmarks time the rasterization step alone with it off)
-    // ---- per-training-keyframe rows of the exposure and the pose refinement, kf_cap of each, allocated for both features
-    //      once either is enabled (enabling one initialises its rows of the existing keyframes) ----
-    size_t kf_cap = 0;
-    // exposure (glic_mapper_enable_exposure): E [kf_cap][12] and its Adam state
-    bool expo_on = false;
-    float expo_lr = 0.f;
-    Dev<float> expo_E;
-    KeyframeAdam expo_adam{12};
-    // pose refinement (glic_mapper_enable_pose_refinement): float64 T_cw [kf_cap][12] (R_cw row-major | t_cw), the float pose
-    // [kf_cap][12] (R_wc | t_wc) and the Adam state of the 6-vector
-    bool pose_on = false;
-    float pose_lr_rho = 0.f, pose_lr_omega = 0.f;
-    Dev<double> pose_T;
-    Dev<float> pose_f;
-    KeyframeAdam pose_adam{6};
-    Dev<double> pose_part;                // per-CTA partials of the pose-gradient reduction (pose_partials_count(Pcap))
-    Event ev_pose;
-    // ---- LPIPS of the evaluation (glic_mapper_load_lpips): weight payload and glic_lpips's scratch, sized on first use ----
-    Dev<float> lpips_w;
-    Dev<void> lpips_scratch;
-    // ---- test-time alignment (glic_mapper_align): its workspace (align_carve), sized on first use ----
-    Dev<char> align_ws;
-    // ---- rendering from a caller's camera (glic_mapper_render_camera): its workspace (render_carve) for the largest frame so far
-    Dev<char> render_ws;
-    // ---- contribution scores (glic_mapper_contribution / prune_unseen): hits [Pcap] u64 | max_weight [Pcap] f32, sized on first use
-    Dev<char> score_ws;
-    // ---- the last mesh of glic_mapper_extract_mesh: xyz [V,3] f32, rgb [V,3] u8, faces [F,3] i32 (empty until the first call)
-    bool mesh_ready = false;
-    glic_mesh_counts mesh_counts{};
-    Dev<float> mesh_xyz;
-    Dev<uint8_t> mesh_rgb;
-    Dev<int32_t> mesh_faces;
-    // ---- raw frames (glic_mapper_enable_frames / add_frame): the 8-bit image store, chunks of FRAME_CHUNK frames of
-    //      frame_stride bytes that never move, and the scan of the frames since the last training keyframe (device arrays
-    //      of scan_cap points, grown by doubling) ----
-    bool initialized = false;             // initialize or initialize_lidar has run (the next scan extends the map)
-    bool frames_on = false;
-    int frame_k = 1, frame_sky_points = 0, frame_sky_radius = 0;
-    std::vector<Dev<uint8_t>> frame_chunks;
-    size_t frame_stride = 0;
-    Dev<float> scan_xyz, scan_depth;
-    Dev<uint8_t> scan_rgb;
-    size_t scan_cap = 0;
-    glic_frame_stats fst{};
-    // ---- densification (glic_mapper_enable_densification): per-row statistics [Pcap] each, and the number of real densify
-    //      calls so far (the key of the split children's generator) ----
-    bool dens_on = false;
-    bool exported = false;                // glic_mapper_export has run: the exchange block can no longer move
-    Dev<float> dens_accum, dens_denom;
-    Dev<int> dens_maxr;                   // the largest screen radius of each row since the statistics last restarted
-    uint64_t dens_calls = 0;
-    // ---- the density-control schedule of optimize() (glic_mapper_set_density_schedule) and what it has done since it was set
-    bool sched_on = false;
-    glic_density_schedule sched{};
-    glic_density_counts sched_totals{};
-    uint32_t sched_steps = 0, sched_resets = 0;
-};
-
-namespace {
-
-#define MAP_TRY(expr) do { int _e = (expr); if (_e != GLIC_OK) return _e; } while (0)
-
-// One buffer of a growth: its new size, the prefix of its old contents it keeps, and whether it starts zeroed
-struct Grow { Buf& buf; size_t bytes, keep = 0; bool zero = false; };
-
 // The one way a mapper's buffers grow: allocate every new buffer; on the mapper's stream zero those that start zeroed and copy the
 // kept prefixes (then `fill`, which set_capacity uses to regrow the arenas into the new buffers); synchronise; only then swap the
 // new buffers in and release the old.  A failed allocation leaves every buffer as it was.
-int grow(glic_mapper* m, const std::vector<Grow>& list, const std::function<int(Buf*)>& fill = nullptr) {
+int grow(glic_mapper* m, const std::vector<Grow>& list, const std::function<int(Buf*)>& fill) {
     std::vector<Buf> fresh(list.size());
     Buf* b = fresh.data();
     for (const Grow& g : list) MAP_TRY((b++)->allocate(g.bytes));
@@ -505,12 +283,6 @@ int reserve(glic_mapper* m, Buf& b, size_t need) { return need <= b.bytes() ? GL
 
 size_t arena_floats(const glic_mapper* m, uint32_t cap) { return glic_packed_floats(cap, (uint32_t)m->M); }
 
-// The six row groups of a packed block of capacity cap (an arena, or with M = 0 the exchange block's gradients), in
-// glic_packed_offsets order; rest is null without SH rest (M = 0)
-struct ArenaRows {
-    float *rot, *xyz, *log_scale, *opacity, *dc, *rest;
-    std::array<float*, 6> groups() const { return {rot, xyz, log_scale, opacity, dc, rest}; }
-};
 ArenaRows arena_rows(float* base, uint32_t cap, int M) {
     size_t off[6];
     glic_packed_offsets(cap, (uint32_t)M, off);
@@ -521,7 +293,7 @@ std::array<size_t, 6> group_widths(int M) { return {4, 3, 3, 1, 3, (size_t)3 * M
 
 float* geo_ptr(const glic_mapper* m) { return static_cast<float*>(m->xblock.raw()); }
 
-void config_camera_block(const glic_mapper* m, const float* R_wc, const float* t_wc, CamBlock& o, double* T12 = nullptr) {
+void config_camera_block(const glic_mapper* m, const float* R_wc, const float* t_wc, CamBlock& o, double* T12) {
     camera_block(m->cfg.width, m->cfg.height, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, R_wc, t_wc, o, T12);
 }
 
@@ -567,36 +339,20 @@ int push_to_peers(glic_mapper* m, const void* local, size_t bytes) {
     return GLIC_OK;
 }
 
-// grows everything whose size depends on the Gaussian capacity, all of it allocated before any old buffer is released; the
-// arenas and the anchors keep their live rows and every new buffer but pose_part and the anchors starts zeroed, so rows [P, Pcap)
-// of the arenas stay zero
+// grows everything whose size depends on the Gaussian capacity (capacity_buffers), all of it allocated before any old buffer is
+// released
 int set_capacity(glic_mapper* m, uint32_t cap) {
     cap = round_up(std::max<uint32_t>(cap, 256), 256);
     if (cap <= m->Pcap) return GLIC_OK;
     if (m->connected) { set_error("mapper: the arena capacity is fixed once the exchange blocks are connected (world > 1); create the mapper with a larger capacity"); return GLIC_ERR_WORKSPACE; }
-    const size_t arena = arena_floats(m, cap) * sizeof(float);
-    const XLayout x = xblock_layout(m->S, cap, m->dens_on);
     auto regrow = [&](Buf* fresh) -> int {
         const float* old[3] = {m->params, m->m1, m->m2};
         for (int a = 0; a < 3 && m->P; ++a)
             MAP_TRY(glic_arena_regrow(old[a], m->Pcap, static_cast<float*>(fresh[a].raw()), cap, (uint32_t)m->M, m->P, m->stream));
         return GLIC_OK;
     };
-    std::vector<Grow> list = {{m->params, arena, 0, true}, {m->m1, arena, 0, true}, {m->m2, arena, 0, true},
-                              {m->act_opacity, (size_t)cap * 4, 0, true}, {m->act_scales, (size_t)cap * 12, 0, true},
-                              {m->act_rots, (size_t)cap * 16, 0, true}, {m->radii, (size_t)cap * 4, 0, true},
-                              {m->g_conic, (size_t)cap * (16 + 12 + 4), 0, true}, {m->geom_ws, glic_geom_bytes((int)cap), 0, true},
-                              {m->xblock, x.bytes, 0, true}, {m->pose_part, pose_partials_count(cap) * sizeof(double)},
-                              {m->anchor, (size_t)cap * 4, (size_t)m->P * 4}};
-    if (m->dens_on)                                       // the statistics keep their live rows
-        for (Buf* b : {(Buf*)&m->dens_accum, (Buf*)&m->dens_denom, (Buf*)&m->dens_maxr}) list.push_back({*b, (size_t)cap * 4, (size_t)m->P * 4, true});
-    MAP_TRY(grow(m, list, regrow));
-    m->g_mean2D = m->g_conic + (size_t)cap * 4;           // conic first: float4-aligned
-    m->g_opacity = m->g_mean2D + (size_t)cap * 3;
-    m->x = x;
-    m->peers[m->cfg.rank] = m->xblock;
-    m->Pcap = cap;
-    m->st.capacity = cap;
+    MAP_TRY(grow(m, capacity_buffers(m, cap, m->dens_on), regrow));
+    adopt_capacity(m, cap, xblock_layout(m->S, cap, m->dens_on));
     return GLIC_OK;
 }
 
@@ -604,10 +360,10 @@ int set_capacity(glic_mapper* m, uint32_t cap) {
 int reserve_keyframe_rows(glic_mapper* m, size_t n) {
     if (n <= m->kf_cap) return GLIC_OK;
     const size_t cap = std::max<size_t>({n, 2 * m->kf_cap, 64}), old = m->kf_cap;
-    auto rows = [&](Buf& b, size_t row_bytes) { return Grow{b, cap * row_bytes, old * row_bytes, true}; };
-    MAP_TRY(grow(m, {rows(m->expo_E, 12 * sizeof(float)), rows(m->expo_adam.m, 12 * sizeof(float)), rows(m->expo_adam.v, 12 * sizeof(float)),
-                     rows(m->expo_adam.t, sizeof(int)), rows(m->pose_T, 12 * sizeof(double)), rows(m->pose_f, 12 * sizeof(float)),
-                     rows(m->pose_adam.m, 6 * sizeof(float)), rows(m->pose_adam.v, 6 * sizeof(float)), rows(m->pose_adam.t, sizeof(int))}));
+    std::vector<Grow> list;
+    grow_rows(list, exposure_rows(m), cap, old, true);
+    grow_rows(list, pose_rows(m), cap, old, true);
+    MAP_TRY(grow(m, list));
     m->kf_cap = cap;
     return GLIC_OK;
 }
@@ -656,9 +412,7 @@ int pose_write(glic_mapper* m, size_t k, const float* R_wc, const float* t_wc, b
 // zero statistics for every row, on the mapper's stream (a no-op with densification off)
 int dens_reset(glic_mapper* m) {
     if (!m->dens_on) return GLIC_OK;
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->dens_accum, 0, (size_t)m->Pcap * 4, m->stream));
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->dens_denom, 0, (size_t)m->Pcap * 4, m->stream));
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->dens_maxr, 0, (size_t)m->Pcap * 4, m->stream));
+    for (const Rows& r : densification_rows(m)) GLIC_CUDA_TRY(cudaMemsetAsync(r.buf.raw(), 0, (size_t)m->Pcap * r.bytes, m->stream));
     return GLIC_OK;
 }
 
@@ -738,7 +492,7 @@ int poll_ring(glic_mapper* m, bool wait) {
 }
 
 // the activated parameters; zero4[0..3] (optional) zeroed by the same kernel
-int activate(glic_mapper* m, float* zero4 = nullptr) {
+int activate(glic_mapper* m, float* zero4) {
     const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
     return launch_activations_forward((int)m->P, a.opacity, a.log_scale, a.rot, m->act_opacity, m->act_scales, m->act_rots, zero4, m->stream);
 }
@@ -748,21 +502,6 @@ int forward_view(glic_mapper* m, const glic_view& v, int no_color, long long* co
     return glic_forward((int)m->P, m->D, m->M, a.xyz, m->act_scales, 1.0f, m->act_rots, m->act_opacity, a.dc, a.rest, &v, no_color, m->radii,
                         m->geom_ws, m->geom_ws.bytes(), m->image_ws, m->image_ws.bytes(), m->binning_ws, m->binning_ws.bytes(), m->sample_ws,
                         m->sample_ws.bytes(), m->color, m->final_T, (int64_t*)counters, m->stream);
-}
-
-// draw(counters), then a synchronisation; a binning overflow grows the workspace by regrow(pairs needed), counts the regrow and
-// draws again, up to 4 attempts.  The caller has drained the ring (poll_ring(wait)), so ring slot 0's pinned counters are free.
-template <typename Draw, typename Regrow>
-int draw_settled(glic_mapper* m, Draw draw, Regrow regrow) {
-    for (int attempt = 0; attempt < 4; ++attempt) {
-        long long* cnt = m->counters_host;
-        MAP_TRY(draw(cnt));
-        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-        if (!cnt[2]) break;
-        MAP_TRY(regrow(cnt[0] + cnt[0] / 4));
-        ++m->st.overflow_regrows;
-    }
-    return GLIC_OK;
 }
 
 // activations and a settled forward of v with the training workspaces
@@ -781,13 +520,11 @@ int load_gt(glic_mapper* m, const Keyframe& kf, float* dst, cudaMemcpyKind kind,
     return GLIC_OK;
 }
 
-__global__ void overflow_word_kernel(const GeomHeader* ghdr, float* word) { if (ghdr->overflow) *word = 1.0f; }
-
 // the L1 + D-SSIM loss of an H x W image against gt, and its dL/dimg; with E (device, 3x4) the loss of the exposed image, and dL/dE;
 // loss_zeroed: *loss is zero already
 // mask (optional, `valid` used pixels): the masked loss
 int photometric_loss(glic_mapper* m, int H, int W, const float* img, const float* gt, const float* E, float* loss, float* dL_dimg, float* dL_dE,
-                     bool loss_zeroed = false, const MaskView* mask = nullptr, uint32_t valid = 0) {
+                     bool loss_zeroed, const MaskView* mask, uint32_t valid) {
     return photometric_loss_sum(H, W, m->cfg.lambda_dssim, img, gt, E, loss, dL_dimg, dL_dE, m->loss_scratch, m->loss_scratch.bytes(),
                                 m->deterministic ? m->det_sums.raw() : nullptr, m->stream, loss_zeroed, mask, valid);
 }
@@ -1192,9 +929,7 @@ int pack_keyframe_mask(glic_mapper* m, Keyframe& kf, const uint8_t* valid) {
     return GLIC_OK;
 }
 
-int scheduled_density_step(glic_mapper* m);    // optimize()'s density control, with glic_mapper_densify_and_prune below
-
-}  // namespace
+}  // namespace mapper_impl
 
 extern "C" {
 
@@ -1363,8 +1098,9 @@ int glic_mapper_add_frame_masked(glic_mapper* m, const glic_frame* f, const uint
     }
     if (pending > m->scan_cap) {
         const size_t cap = std::max<size_t>({pending, 2 * m->scan_cap, 4096});
-        MAP_TRY(grow(m, {{m->scan_xyz, cap * 3 * sizeof(float), have * 3 * sizeof(float)}, {m->scan_rgb, cap * 3, have * 3},
-                         {m->scan_depth, cap * sizeof(float), have * sizeof(float)}}));
+        std::vector<Grow> list;
+        grow_rows(list, scan_rows(m), cap, have, false);
+        MAP_TRY(grow(m, list));
         m->scan_cap = cap;
     }
     uint8_t* dst = m->frame_chunks[idx / FRAME_CHUNK] + (idx % FRAME_CHUNK) * m->frame_stride;
@@ -1570,601 +1306,9 @@ int glic_mapper_download(glic_mapper* m, float* xyz, float* f_dc, float* f_rest,
     return GLIC_OK;
 }
 
-int glic_mapper_enable_densification(glic_mapper* m) {
-    if (!m) { set_error("mapper_enable_densification: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (m->dens_on) return GLIC_OK;
-    if (m->cfg.world > 1 && (m->exported || m->connected)) {
-        set_error("mapper_enable_densification: with world > 1 it must come before glic_mapper_export (the exchange block grows)");
-        return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    MAP_TRY(poll_ring(m, true));
-    // the exchange block gains the two statistics rows and the radius slots; every new buffer starts zeroed
-    const XLayout x = xblock_layout(m->S, m->Pcap, true);
-    MAP_TRY(grow(m, {{m->xblock, x.bytes, 0, true}, {m->dens_accum, (size_t)m->Pcap * 4, 0, true}, {m->dens_denom, (size_t)m->Pcap * 4, 0, true},
-                     {m->dens_maxr, (size_t)m->Pcap * 4, 0, true}}));
-    m->x = x;
-    m->peers[m->cfg.rank] = m->xblock;
-    m->dens_on = true;
-    return GLIC_OK;
-}
-
 }  // extern "C"
 
-namespace {
-
-// The one stable compaction of the arenas (prune.cu), behind glic_mapper_densify_and_prune, glic_mapper_densify (min_opacity 0,
-// both size tests off) and glic_mapper_prune (no row selected, both size tests off): select, reserve (capacity, then the
-// spares), gather each arena into a spare one of the same capacity and swap, write the children's xyz and log-scale.  The
-// spare is allocated once, before anything changes, and rotates: params -> spare, the old params buffer then takes m1, the old
-// m1 buffer m2, and the old m2 buffer is freed.  Peak extra memory: one arena (glic_packed_floats(Pcap, M) floats); the
-// selection's scratch (12 B per row and five counts per 1024 rows) lives in the extend() staging buffer, which keeps it.  The
-// params gather takes every result row, the moments only the kept rows (the new rows' moments are zero), and each writes output
-// rows [0, max(rows, P)): rows [P, Pcap) of every arena are zero already (allocation, initialize, append and regrow keep them
-// so), so the rows a prune vacates end up zero like them.
-// densify: the call densifies, so it selects by the statistics, zeroes them and advances dens_calls even when no row changes.
-// Otherwise it only prunes: no statistic is read, the statistics (with densification on) move with their rows, dens_calls
-// stays (it keys the children's draws of every later densify), and a call that removes nothing touches nothing.
-// The caller has validated p.  reject_empty: a result without rows is an error (densify on an empty map is not).
-// unseen (optional, a prune only): the scores in score_ws (contribution below) also remove rows, by glic_mapper_prune_unseen's test.
-int density_step(glic_mapper* m, const glic_density_params& p, bool densify, int dry_run, bool reject_empty, glic_density_counts* out,
-                 const char* what, const glic_unseen_params* unseen = nullptr) {
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    MAP_TRY(poll_ring(m, true));
-    const uint32_t P = m->P;
-    uint32_t r[6] = {0, 0, 0, 0, 0, 0};                // clones, splits, surviving kept rows, clones, split rows, sky rows
-    cudaStream_t s = m->stream;
-    if (P) {
-        MAP_TRY(reserve(m, m->extend_ws, density_scratch_bytes(P)));   // the selection's scratch: the idle extend() staging
-        const ArenaRows g = arena_rows(m->params, m->Pcap, m->M);
-        const float* no_stats = nullptr;                   // a prune selects no row, with densification on or off
-        DensitySelect a{P, m->n_sky, densify ? m->dens_accum : no_stats, densify ? m->dens_denom : no_stats, g.log_scale, g.opacity,
-                        m->dens_maxr, p.grad_threshold, p.percent_dense * p.scene_extent, p.min_opacity, p.max_world_scale,
-                        p.max_screen_radius};
-        if (unseen) {
-            a.score_hits = reinterpret_cast<const uint64_t*>(m->score_ws.raw());
-            a.score_ends = a.score_hits + m->Pcap;
-            a.score_max = reinterpret_cast<const float*>(a.score_hits + 2 * (size_t)m->Pcap);
-            a.min_weight = unseen->min_weight;
-            a.min_hits = unseen->min_hits;
-            a.score_sky = unseen->sky;
-        }
-        MAP_TRY(launch_density_select(a, m->extend_ws, r, s));
-    }
-    const uint32_t n_clone = r[0], n_split = r[1], kept = r[2], cloned = r[3], split = r[4];
-    const uint64_t unpruned = (uint64_t)P + n_clone + n_split, rows = (uint64_t)kept + cloned + 2 * (uint64_t)split;
-    if (reject_empty && rows == 0) {
-        set_error(std::string(what) + ": the result has no rows (an empty map cannot be trained)");
-        return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (!dry_run && (n_clone || n_split || rows != P)) {
-        if (rows > m->Pcap) {
-            if (m->connected) {
-                set_error(std::string(what) + ": the result does not fit the capacity, which is fixed once the exchange blocks are connected (world > 1); prune first");
-                return GLIC_ERR_WORKSPACE;
-            }
-            MAP_TRY(set_capacity(m, std::max<uint32_t>((uint32_t)rows, 2 * m->Pcap)));
-        }
-        Dev<float> spare, spare_stats[3];
-        Dev<int32_t> spare_anchor;
-        const bool move_stats = !densify && m->dens_on;
-        const size_t bytes = arena_floats(m, m->Pcap) * sizeof(float);
-        MAP_TRY(spare.allocate(bytes));
-        MAP_TRY(spare_anchor.allocate((size_t)m->Pcap * 4));
-        if (move_stats)
-            for (Dev<float>& b : spare_stats) MAP_TRY(b.allocate((size_t)m->Pcap * 4));
-        GLIC_CUDA_TRY(cudaMemsetAsync(spare, 0, bytes, s));
-        const uint32_t* idx = density_index(m->extend_ws, P);
-        const uint32_t written = std::max<uint32_t>((uint32_t)rows, P);   // the rows a prune vacates become zero
-        for (Dev<float>* arena : {&m->params, &m->m1, &m->m2}) {
-            MAP_TRY(launch_gather_rows(*arena, spare, m->Pcap, m->M, written, arena == &m->params ? (uint32_t)rows : kept, idx, s));
-            std::swap(*arena, spare);
-        }
-        // the anchors follow the params gather: every result row, clones and split children from their parents
-        MAP_TRY(launch_gather_words(m->anchor, spare_anchor, written, (uint32_t)rows, idx, s));
-        std::swap(m->anchor, spare_anchor);
-        MAP_TRY(launch_densify_children(m->params, m->Pcap, m->M, kept + cloned, split, m->extend_ws, P, n_split, m->cfg.seed, m->dens_calls, s));
-        if (move_stats) {                                  // the statistics move with their rows (and their spares are zero)
-            Buf* stats[3] = {&m->dens_accum, &m->dens_denom, &m->dens_maxr};
-            for (int q = 0; q < 3; ++q) {
-                GLIC_CUDA_TRY(cudaMemsetAsync(spare_stats[q], 0, (size_t)m->Pcap * 4, s));
-                MAP_TRY(launch_gather_words(stats[q]->raw(), spare_stats[q], written, kept, idx, s));
-                std::swap(*stats[q], static_cast<Buf&>(spare_stats[q]));
-            }
-        }
-        m->P = (uint32_t)rows;
-        m->n_sky = r[5];
-        m->st.num_gaussians = m->P;
-    }
-    if (!dry_run) {
-        if (densify) MAP_TRY(dens_reset(m));                       // densification_postfix: the statistics start again
-        GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-        if (densify) ++m->dens_calls;
-    }
-    if (out) *out = glic_density_counts{n_clone, n_split, (uint32_t)(unpruned - rows), (uint32_t)rows};
-    return GLIC_OK;
-}
-
-// getNerfppNorm's radius over the training keyframes' camera centres (their device poses under pose refinement), in double
-int scene_extent(glic_mapper* m, float* out) {
-    const size_t n = m->train.size();
-    *out = 0.0f;
-    if (n == 0) return GLIC_OK;
-    std::vector<double> c(3 * n);
-    if (m->pose_on) {
-        std::vector<float> f12(12 * n);
-        GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-        GLIC_CUDA_TRY(cudaMemcpy(f12.data(), m->pose_f, f12.size() * sizeof(float), cudaMemcpyDeviceToHost));
-        for (size_t k = 0; k < n; ++k) for (int i = 0; i < 3; ++i) c[3 * k + i] = f12[12 * k + 9 + i];
-    } else {
-        for (size_t k = 0; k < n; ++k) for (int i = 0; i < 3; ++i) c[3 * k + i] = m->train[k].t_wc[i];
-    }
-    double mean[3] = {0.0, 0.0, 0.0}, far = 0.0;
-    for (size_t k = 0; k < n; ++k) for (int i = 0; i < 3; ++i) mean[i] += c[3 * k + i];
-    for (int i = 0; i < 3; ++i) mean[i] /= (double)n;
-    for (size_t k = 0; k < n; ++k) {
-        const double dx = c[3 * k] - mean[0], dy = c[3 * k + 1] - mean[1], dz = c[3 * k + 2] - mean[2];
-        far = std::max(far, std::sqrt(dx * dx + dy * dy + dz * dz));
-    }
-    *out = (float)(1.1 * far);
-    return GLIC_OK;
-}
-
-// the schedule's work after the iteration that made stats.iterations = n (glic_mapper_set_density_schedule)
-int scheduled_density_step(glic_mapper* m) {
-    const glic_density_schedule& c = m->sched;
-    const uint64_t n = m->st.iterations;
-    if (c.densify_from < n && n < c.densify_until && n % c.densify_interval == 0) {
-        float extent = c.scene_extent;
-        if (!(extent > 0.0f)) MAP_TRY(scene_extent(m, &extent));
-        if (extent > 0.0f) {                                        // one keyframe, or all at one place: no step
-            const bool sizes = c.opacity_reset_interval > 0 && n > c.opacity_reset_interval;
-            const glic_density_params p{c.grad_threshold, c.percent_dense, extent, c.min_opacity, sizes ? c.screen_radius : 0,
-                                        sizes ? c.world_scale_factor * extent : 0.0f};
-            glic_density_counts k{};
-            MAP_TRY(glic_mapper_densify_and_prune(m, &p, 0, &k));
-            m->sched_totals.cloned += k.cloned;
-            m->sched_totals.split += k.split;
-            m->sched_totals.pruned += k.pruned;
-            m->sched_totals.rows = k.rows;
-            ++m->sched_steps;
-        }
-    }
-    if (c.opacity_reset_interval > 0 && n < c.densify_until && n % c.opacity_reset_interval == 0) {
-        MAP_TRY(glic_mapper_reset_opacity(m, c.reset_opacity));
-        ++m->sched_resets;
-    }
-    return GLIC_OK;
-}
-
-bool finite_at_least_zero(float x) { return std::isfinite(x) && x >= 0.0f; }
-
-// ---- test-time alignment (glic_mapper_align) ------------------------------------------------------------------------------
-// The call's one-row state on the device: the pose and exposure being fitted with their Adam states, laid out as
-// pose_step_kernel and exposure_adam_kernel index them (keyframe 0 of one-row arrays); the last iteration's gradients, loss and
-// overflow word; and the tally of the iterations.
-struct AlignState {
-    double T[12];                     // float64 T_cw = R_cw (row-major) | t_cw
-    float pose_f[12];                 // R_wc | t_wc
-    float cam[36];                    // view16 | proj16 | campos4 of pose_f
-    float pose_m[6], pose_v[6];
-    float E[12], expo_m[12], expo_v[12];
-    float pose_grad[8];               // dL/d(rho, omega) (6 used)
-    float dE[12];                     // dL/dE
-    float loss;                       // fit-region loss
-    float overflow;                   // overflow_word_kernel's word: non-zero skips both steps
-    int pose_t, expo_t;
-    int steps, skipped;
-    float first_loss, last_loss;
-    unsigned int max_pairs;           // the largest (tile, Gaussian) pair count of a skipped iteration
-};
-
-// closes an alignment iteration: counted as stepped (with its loss) or skipped (with its pair count); the word is cleared
-__global__ void align_tally_kernel(const GeomHeader* __restrict__ ghdr, AlignState* __restrict__ st) {
-    if (st->overflow != 0.0f) {
-        ++st->skipped;
-        st->max_pairs = max(st->max_pairs, ghdr->total);
-    } else {
-        if (st->steps == 0) st->first_loss = st->loss;
-        st->last_loss = st->loss;
-        ++st->steps;
-    }
-    st->overflow = 0.0f;
-}
-
-// dst[3][H][w] = columns [x0, x0 + w) of src[3][H][W]
-__global__ void __launch_bounds__(256)
-crop_columns_kernel(int H, int W, int x0, int w, const float* __restrict__ src, float* __restrict__ dst) {
-    const size_t n = (size_t)3 * H * w;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const size_t row = i / w;
-        dst[i] = src[row * W + x0 + (i - row * w)];
-    }
-}
-
-// dst[3][H][W] = src[3][H][w] in columns [0, w), zero in the others
-__global__ void __launch_bounds__(256)
-pad_columns_kernel(int H, int W, int w, const float* __restrict__ src, float* __restrict__ dst) {
-    const size_t n = (size_t)3 * H * W;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const size_t row = i / W, x = i - row * W;
-        dst[i] = x < (size_t)w ? src[row * w + x] : 0.0f;
-    }
-}
-
-unsigned plane_blocks(size_t n) { return (unsigned)std::min<size_t>((n + 255) / 256, (size_t)NUM_SMS * 8); }
-
-// The workspace of glic_mapper_align: colour gradients [3 Pcap] | pose partials | with split, three planes [3][H][W - W/2]
-// (rendered and ground-truth crops, the fit crop's dL/dpixel) | the one-row state
-size_t align_carve(void* ws, uint32_t Pcap, int W, int H, bool split, float** col, double** part, float** crops, AlignState** st) {
-    Carver c(ws);
-    float* a = c.take<float>((size_t)3 * Pcap);
-    double* b = c.take<double>(pose_partials_count(Pcap));
-    for (int q = 0; q < 3; ++q) {
-        float* x = c.take<float>(split ? (size_t)3 * H * (W - W / 2) : 0);
-        if (crops) crops[q] = x;
-    }
-    AlignState* t = c.take<AlignState>(1);
-    if (col) *col = a;
-    if (part) *part = b;
-    if (st) *st = t;
-    return c.total();
-}
-
-// glic_mapper_align after its checks: reserve, start state, the fit loop (enqueued without a host synchronisation), the
-// overflow regrow, the scoring
-int align(glic_mapper* m, const Keyframe& kf, bool train, int index, const glic_align_params& p, glic_align_result* out, float* rgb_host) {
-    const int W = m->cfg.width, H = m->cfg.height;
-    const bool split = p.split != 0;
-    const int Wf = split ? W / 2 : W, x_score = split ? W / 2 : 0, Ws = W - x_score;     // fit and score columns
-    const bool use_expo = p.exposure_lr > 0.0f || (train && m->expo_on);                  // the loss applies E
-    // under the keyframe's mask: the fit loss and both scores are masked, each region read from the mask in place
-    MaskView fit_mv, full_mv, score_mv;
-    const MaskView* fit_mask = keyframe_mask(kf, W, fit_mv);
-    const MaskView* full_mask = keyframe_mask(kf, W, full_mv);
-    const MaskView* score_mask = keyframe_mask(kf, W, score_mv, x_score);
-    const uint32_t fit_valid = split ? kf.mask_valid_left : kf.mask_valid, score_valid = kf.mask_valid - (split ? kf.mask_valid_left : 0);
-    if (kf.mask_valid && (fit_valid == 0 || score_valid == 0)) {
-        set_error("mapper_align: the keyframe's mask leaves no valid pixel in the fit or the score columns"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    cudaStream_t s = m->stream;
-    MAP_TRY(poll_ring(m, true));
-    MAP_TRY(reserve(m, m->align_ws, align_carve(nullptr, m->Pcap, W, H, split, nullptr, nullptr, nullptr, nullptr)));
-    if (use_expo) MAP_TRY(reserve(m, m->loss_scratch, glic_loss_exposure_scratch_bytes(H, Wf)));
-    if (m->lpips_w) MAP_TRY(reserve(m, m->lpips_scratch, glic_lpips_scratch_bytes(H, Ws)));
-    float *col = nullptr, *crops[3] = {nullptr, nullptr, nullptr};
-    double* part = nullptr;
-    AlignState* st = nullptr;
-    align_carve(m->align_ws, m->Pcap, W, H, split, &col, &part, crops, &st);
-    // start: the stored pose (its camera block is the keyframe's), or a training keyframe's refined one; E = [I | 0], or a
-    // training keyframe's trained E; zero moments and step counts
-    AlignState h{};
-    CamBlock cb;
-    config_camera_block(m, kf.R_wc, kf.t_wc, cb, h.T);
-    std::memcpy(h.pose_f, kf.R_wc, sizeof(kf.R_wc)); std::memcpy(h.pose_f + 9, kf.t_wc, sizeof(kf.t_wc));
-    std::memcpy(h.cam, cb.view, sizeof(h.cam));
-    h.E[0] = h.E[5] = h.E[10] = 1.0f;
-    h.first_loss = h.last_loss = std::numeric_limits<float>::quiet_NaN();
-    GLIC_CUDA_TRY(cudaMemcpyAsync(st, &h, sizeof(h), cudaMemcpyHostToDevice, s));
-    if (train && m->pose_on) {
-        GLIC_CUDA_TRY(cudaMemcpyAsync(st->T, m->pose_T + 12 * (size_t)index, sizeof(h.T), cudaMemcpyDeviceToDevice, s));
-        GLIC_CUDA_TRY(cudaMemcpyAsync(st->pose_f, m->pose_f + 12 * (size_t)index, sizeof(h.pose_f), cudaMemcpyDeviceToDevice, s));
-        GLIC_CUDA_TRY(cudaMemcpyAsync(st->cam, kf.cam_dev, sizeof(h.cam), cudaMemcpyDeviceToDevice, s));
-    }
-    if (train && m->expo_on) GLIC_CUDA_TRY(cudaMemcpyAsync(st->E, m->expo_E + 12 * (size_t)index, sizeof(h.E), cudaMemcpyDeviceToDevice, s));
-    const glic_view v = make_view(cb, st->cam, W, H);   // the keyframe's view, drawn from the call's own camera block
-    MAP_TRY(load_gt(m, kf, m->gt_dev[0], cudaMemcpyHostToDevice, s));
-    const float* gt_fit = m->gt_dev[0];
-    if (split) {
-        crop_columns_kernel<<<plane_blocks((size_t)3 * H * Wf), 256, 0, s>>>(H, W, 0, Wf, m->gt_dev[0], crops[1]);
-        GLIC_LAUNCH_CHECK();
-        gt_fit = crops[1];
-    }
-    MAP_TRY(activate(m));
-    PoseBatch b{};
-    b.cam[0] = st->cam;
-    const int slot_kf[1] = {0};
-    const unsigned int* skip = reinterpret_cast<const unsigned int*>(&st->overflow);
-    CompactGrads cg{};                              // null row pointers: the pose-only backward
-    cg.pose_partials = part;
-    cg.pose_grad = st->pose_grad;
-    const GeomHeader* ghdr = GeomState::carve(m->geom_ws, (int)m->P).hdr;
-    for (int it = 0; it < p.iterations; ++it) {
-        MAP_TRY(forward_view(m, v, 0, nullptr));
-        overflow_word_kernel<<<1, 1, 0, s>>>(ghdr, &st->overflow);
-        GLIC_LAUNCH_CHECK();
-        const float* img_fit = m->color;
-        float* dL_fit = m->dL_dpix;
-        if (split) {
-            crop_columns_kernel<<<plane_blocks((size_t)3 * H * Wf), 256, 0, s>>>(H, W, 0, Wf, m->color, crops[0]);
-            GLIC_LAUNCH_CHECK();
-            img_fit = crops[0];
-            dL_fit = crops[2];
-        }
-        MAP_TRY(photometric_loss(m, H, Wf, img_fit, gt_fit, use_expo ? st->E : nullptr, &st->loss, dL_fit, st->dE, false, fit_mask, fit_valid));
-        if (split) {
-            pad_columns_kernel<<<plane_blocks((size_t)3 * H * W), 256, 0, s>>>(H, W, Wf, crops[2], m->dL_dpix);
-            GLIC_LAUNCH_CHECK();
-        }
-        MAP_TRY(backward_view(m, v, col, cg, nullptr));
-        MAP_TRY(launch_pose_kernel(m, 1, b, st->pose_grad, st->T, st->pose_f, st->pose_m, st->pose_v, &st->pose_t, p.lr_translation,
-                                   p.lr_rotation, skip));
-        if (p.exposure_lr > 0.0f)
-            MAP_TRY(launch_exposure_adam(1, slot_kf, st->dE, st->E, st->expo_m, st->expo_v, &st->expo_t, p.exposure_lr, skip, s));
-        align_tally_kernel<<<1, 1, 0, s>>>(ghdr, st);
-        GLIC_LAUNCH_CHECK();
-    }
-    GLIC_CUDA_TRY(cudaMemcpyAsync(&h, st, sizeof(h), cudaMemcpyDeviceToHost, s));
-    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-    if (h.skipped) MAP_TRY(regrow_after_skip(m, h.max_pairs));
-    // scoring at the fitted camera: the full clamped (exposed) frame, then with split its score columns
-    MAP_TRY(forward_settled(m, v, 0));
-    MAP_TRY(eval_psnr_ssim(3, H, W, m->color, m->gt_dev[0], use_expo ? st->E : nullptr, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s,
-                           m->deterministic ? m->det_sums.raw() : nullptr, full_mask, kf.mask_valid));
-    if (rgb_host) MAP_TRY(scored_image_to_host(m, rgb_host));
-    if (split) {
-        for (int q = 0; q < 2; ++q) {
-            crop_columns_kernel<<<plane_blocks((size_t)3 * H * Ws), 256, 0, s>>>(H, W, x_score, Ws, eval_clamped(m->eval_scratch, 3, H, W, q), crops[q]);
-            GLIC_LAUNCH_CHECK();
-        }
-        MAP_TRY(eval_psnr_ssim(3, H, Ws, crops[0], crops[1], nullptr, m->eval_out, m->eval_scratch, m->eval_scratch.bytes(), s,
-                               m->deterministic ? m->det_sums.raw() : nullptr, score_mask, score_valid));
-    }
-    if (m->lpips_w) MAP_TRY(scored_lpips(m, Ws));
-    float out3[3] = {0.f, 0.f, std::numeric_limits<float>::quiet_NaN()};
-    MAP_TRY(read_eval_out(m, out3, m->lpips_w ? 3 : 2));
-    glic_align_result& r = *out;
-    std::memcpy(r.R_wc, h.pose_f, sizeof(r.R_wc)); std::memcpy(r.t_wc, h.pose_f + 9, sizeof(r.t_wc));
-    std::memcpy(r.E, h.E, sizeof(r.E));
-    r.psnr = out3[0]; r.ssim = out3[1]; r.lpips = out3[2];
-    r.first_loss = h.first_loss; r.last_loss = h.last_loss;
-    std::memcpy(r.pose_exp_avg, h.pose_m, sizeof(r.pose_exp_avg)); std::memcpy(r.pose_exp_avg_sq, h.pose_v, sizeof(r.pose_exp_avg_sq));
-    std::memcpy(r.expo_exp_avg, h.expo_m, sizeof(r.expo_exp_avg)); std::memcpy(r.expo_exp_avg_sq, h.expo_v, sizeof(r.expo_exp_avg_sq));
-    r.steps = h.steps; r.skipped = h.skipped;
-    return GLIC_OK;
-}
-
-// The workspace of glic_mapper_render_camera: the camera block (view16 | proj16 | campos4) | an image workspace | glic_render's
-// colour, final T, depth and median depth planes | the scored colour
-struct RenderPlanes { float* cam; void* image_ws; float *color, *T, *depth, *median, *rgb; };
-size_t render_carve(void* ws, int W, int H, RenderPlanes* out) {
-    const size_t HW = (size_t)W * H;
-    Carver c(ws);
-    RenderPlanes r;
-    r.cam = c.take<float>(36);
-    r.image_ws = c.take<char>(glic_image_bytes(W, H));
-    r.color = c.take<float>(3 * HW);
-    r.T = c.take<float>(HW);
-    r.depth = c.take<float>(HW);
-    r.median = c.take<float>(HW);
-    r.rgb = c.take<float>(3 * HW);
-    if (out) *out = r;
-    return c.total();
-}
-
-// glic_mapper_render_camera after its checks: out = rgb, final_T, depth, median_depth (each may be NULL)
-int render_camera(glic_mapper* m, const glic_render_camera& c, int exposure_index, int with_sky, float* const out[4]) {
-    const int W = c.width, H = c.height;
-    const size_t HW = (size_t)W * H;
-    cudaStream_t s = m->stream;
-    MAP_TRY(poll_ring(m, true));
-    MAP_TRY(reserve(m, m->render_ws, render_carve(nullptr, W, H, nullptr)));
-    RenderPlanes r;
-    render_carve(m->render_ws, W, H, &r);
-    CamBlock cb;
-    camera_block(W, H, c.fx, c.fy, c.cx, c.cy, c.R_wc, c.t_wc, cb);
-    GLIC_CUDA_TRY(cudaMemcpyAsync(r.cam, cb.view, 36 * sizeof(float), cudaMemcpyHostToDevice, s));
-    const glic_view v = make_view(cb, r.cam, W, H);
-    MAP_TRY(activate(m));
-    // the groups are planar: rows [first, P) are the same call on every group pointer offset by `first` rows (rest stays null
-    // when M = 0)
-    const size_t first = with_sky ? 0 : m->n_sky;
-    const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
-    MAP_TRY(draw_settled(m, [&](long long* cnt) {
-        return glic_render((int)(m->P - first), m->D, m->M, a.xyz + 3 * first, m->act_scales + 3 * first, 1.0f, m->act_rots + 4 * first,
-                           m->act_opacity + first, a.dc + 3 * first, a.rest + (size_t)3 * m->M * first, &v, m->radii + first, m->geom_ws,
-                           m->geom_ws.bytes(), r.image_ws, glic_image_bytes(W, H), m->binning_ws, m->binning_ws.bytes(), r.color, r.T,
-                           out[2] ? r.depth : nullptr, out[3] ? r.median : nullptr, (int64_t*)cnt, s);
-    }, [&](int64_t pairs) { return grow_render_binning(m, pairs); }));
-    if (out[0]) MAP_TRY(launch_scored_image(H, W, r.color, exposure_index >= 0 ? m->expo_E + 12 * (size_t)exposure_index : nullptr, r.rgb, s));
-    const float* src[4] = {r.rgb, r.T, r.depth, r.median};
-    for (int q = 0; q < 4; ++q)
-        if (out[q]) GLIC_CUDA_TRY(cudaMemcpyAsync(out[q], src[q], sizeof(float) * (q ? HW : 3 * HW), cudaMemcpyDefault, s));
-    GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-    return GLIC_OK;
-}
-
-// ---- contribution scores (glic_mapper_contribution, glic_mapper_prune_unseen) ------------------------------------------------
-// score_ws: hits [Pcap] u64 | ends [Pcap] u64 | max_weight [Pcap] f32
-size_t score_bytes(uint32_t cap) { return (size_t)cap * (2 * sizeof(uint64_t) + sizeof(float)); }
-
-// a NULL view list (every training keyframe), or n >= 0 training keyframe indices
-int views_check(const glic_mapper* m, const int* views, int n, const char* what) {
-    if (n < 0) { set_error(std::string(what) + ": n_views must be >= 0"); return GLIC_ERR_INVALID_ARGUMENT; }
-    for (int q = 0; views && q < n; ++q)
-        if (views[q] < 0 || views[q] >= (int)m->train.size()) { set_error(std::string(what) + ": view index out of range"); return GLIC_ERR_INVALID_ARGUMENT; }
-    return GLIC_OK;
-}
-
-// The scores of every row over training keyframes views[0 .. n) (NULL: all of them) into score_ws, which the caller has
-// reserved (score_bytes(Pcap)) after draining the ring.  Every row is drawn at the keyframe's current camera block, as training
-// draws it; an overflowed view added nothing, so it is redrawn into the same arrays with a larger binning workspace.
-int contribution(glic_mapper* m, const int* views, int n) {
-    cudaStream_t s = m->stream;
-    uint64_t* hits = reinterpret_cast<uint64_t*>(m->score_ws.raw());
-    uint64_t* ends = hits + m->Pcap;
-    float* max_weight = reinterpret_cast<float*>(hits + 2 * (size_t)m->Pcap);
-    GLIC_CUDA_TRY(cudaMemsetAsync(m->score_ws, 0, score_bytes(m->Pcap), s));
-    if (!m->P) return GLIC_OK;
-    MAP_TRY(activate(m));
-    const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
-    const int count = views ? n : (int)m->train.size();
-    for (int q = 0; q < count; ++q) {
-        const glic_view& v = m->train[views ? views[q] : q].view;
-        MAP_TRY(draw_settled(m, [&](long long* cnt) {
-            return glic_contribution((int)m->P, a.xyz, m->act_scales, 1.0f, m->act_rots, m->act_opacity, &v, m->radii, m->geom_ws,
-                                     m->geom_ws.bytes(), m->image_ws, m->image_ws.bytes(), m->binning_ws, m->binning_ws.bytes(), max_weight,
-                                     hits, ends, nullptr, (int64_t*)cnt, s);
-        }, [&](int64_t pairs) { return grow_render_binning(m, pairs); }));
-        // draw_settled gives up after four draws: a view still overflowing then was not scored, and its rows must not go
-        if (m->counters_host[2]) { set_error("mapper_contribution: a view still overflows the binning workspace after regrowing it"); return GLIC_ERR_WORKSPACE; }
-    }
-    return GLIC_OK;
-}
-
-// ---- meshing (glic_mapper_extract_mesh) ------------------------------------------------------------------------------------
-// the grid of p's geometry over `data`
-glic_tsdf_grid mesh_grid(const glic_mesh_params& p, void* data) {
-    glic_tsdf_grid g;
-    for (int a = 0; a < 3; ++a) { g.origin[a] = p.origin[a]; g.dims[a] = p.dims[a]; }
-    g.voxel_size = p.voxel_size;
-    g.data = data;
-    return g;
-}
-
-// keyframe kf drawn as glic_mapper_extract_mesh draws it, without the sky rows: its median depth into r.median and, with rgb,
-// its clamped colour into r.rgb
-int draw_mesh_view(glic_mapper* m, const Keyframe& kf, const RenderPlanes& r, bool rgb, const char* what) {
-    const int W = m->cfg.width, H = m->cfg.height;
-    cudaStream_t s = m->stream;
-    const size_t first = m->n_sky;
-    const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
-    MAP_TRY(draw_settled(m, [&](long long* cnt) {
-        return glic_render((int)(m->P - first), m->D, m->M, a.xyz + 3 * first, m->act_scales + 3 * first, 1.0f, m->act_rots + 4 * first,
-                           m->act_opacity + first, a.dc + 3 * first, a.rest + (size_t)3 * m->M * first, &kf.view, m->radii + first,
-                           m->geom_ws, m->geom_ws.bytes(), r.image_ws, glic_image_bytes(W, H), m->binning_ws, m->binning_ws.bytes(),
-                           r.color, r.T, nullptr, r.median, (int64_t*)cnt, s);
-    }, [&](int64_t pairs) { return grow_render_binning(m, pairs); }));
-    if (m->counters_host[2]) { set_error(std::string(what) + ": a view still overflows the binning workspace after regrowing it"); return GLIC_ERR_WORKSPACE; }
-    if (rgb) MAP_TRY(launch_scored_image(H, W, r.color, nullptr, r.rgb, s));
-    return GLIC_OK;
-}
-
-// the new mesh of V vertices and F faces replaces the last one once `extract` has filled it
-template <typename Extract>
-int replace_mesh(glic_mapper* m, const glic_mesh_counts& c, Extract extract) {
-    Dev<float> xyz;
-    Dev<uint8_t> rgb;
-    Dev<int32_t> faces;
-    MAP_TRY(xyz.allocate(12 * (size_t)c.vertices));
-    MAP_TRY(rgb.allocate(3 * (size_t)c.vertices));
-    MAP_TRY(faces.allocate(12 * (size_t)c.faces));
-    MAP_TRY(extract((float*)xyz, (uint8_t*)rgb, (int32_t*)faces));
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    m->mesh_xyz = std::move(xyz);
-    m->mesh_rgb = std::move(rgb);
-    m->mesh_faces = std::move(faces);
-    m->mesh_counts = c;
-    m->mesh_ready = true;
-    return GLIC_OK;
-}
-
-// glic_mapper_extract_mesh after its checks.  The grid and the scratch are this call's own; the render workspace is
-// glic_mapper_render_camera's; the new mesh replaces the previous one only once it is complete.
-int extract_mesh(glic_mapper* m, const glic_mesh_params& p, glic_mesh_counts* out) {
-    const int W = m->cfg.width, H = m->cfg.height;
-    cudaStream_t s = m->stream;
-    MAP_TRY(poll_ring(m, true));
-    MAP_TRY(reserve(m, m->render_ws, render_carve(nullptr, W, H, nullptr)));
-    Buf grid_buf, scratch;
-    MAP_TRY(grid_buf.allocate(glic_tsdf_bytes(p.dims)));
-    MAP_TRY(scratch.allocate(glic_mesh_scratch_bytes(p.dims)));
-    const glic_tsdf_grid grid = mesh_grid(p, grid_buf.raw());
-    MAP_TRY(glic_tsdf_clear(&grid, s));
-    RenderPlanes r;
-    render_carve(m->render_ws, W, H, &r);
-    MAP_TRY(activate(m));
-    const int count = p.views ? p.n_views : (int)m->train.size();
-    for (int q = 0; q < count; ++q) {
-        const Keyframe& kf = m->train[p.views ? p.views[q] : q];
-        MAP_TRY(draw_mesh_view(m, kf, r, true, "mapper_extract_mesh"));
-        MAP_TRY(glic_tsdf_integrate(&grid, kf.cam_dev, W, H, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, r.median, r.rgb,
-                                    kf.mask_valid ? (const uint32_t*)kf.mask : nullptr, mask_words_per_row(W), p.trunc, p.max_depth, s));
-    }
-    uint64_t t[3];
-    MAP_TRY(mesh_count(grid, scratch.raw(), scratch.bytes(), t, s));
-    if (t[1] > 0xFFFFFFFFull) { set_error("mapper_extract_mesh: more than 2^32 - 1 faces"); return GLIC_ERR_INVALID_ARGUMENT; }
-    MAP_TRY(replace_mesh(m, glic_mesh_counts{(uint32_t)t[0], (uint32_t)t[1], t[2]}, [&](float* xyz, uint8_t* rgb, int32_t* faces) {
-        return glic_mesh_extract(&grid, scratch.raw(), scratch.bytes(), xyz, rgb, faces, s);
-    }));
-    if (out) *out = m->mesh_counts;
-    return GLIC_OK;
-}
-
-// glic_mapper_extract_mesh_sparse after its checks: pass 1 builds the block set (grown and the insertion repeated on overflow),
-// then the grid, pass 2 integrates, then count and extract.  The set, the grid and the scratch are this call's own.
-constexpr uint32_t SPARSE_FIRST_CAPACITY = 1u << 16;
-constexpr uint32_t SPARSE_MAX_BLOCKS = (1u << 23) - 1;  // glic_sparse_tsdf_bytes' largest grid; sets double up to 2^24
-
-int extract_mesh_sparse(glic_mapper* m, const glic_sparse_mesh_params& p, glic_sparse_mesh_counts* out) {
-    const int W = m->cfg.width, H = m->cfg.height;
-    cudaStream_t s = m->stream;
-    MAP_TRY(poll_ring(m, true));
-    MAP_TRY(reserve(m, m->render_ws, render_carve(nullptr, W, H, nullptr)));
-    Buf set_buf;
-    MAP_TRY(set_buf.allocate(glic_block_set_bytes(SPARSE_FIRST_CAPACITY)));
-    glic_block_set set{SPARSE_FIRST_CAPACITY, set_buf.raw()};
-    MAP_TRY(glic_block_set_clear(&set, s));
-    RenderPlanes r;
-    render_carve(m->render_ws, W, H, &r);
-    MAP_TRY(activate(m));
-    const int count = p.views ? p.n_views : (int)m->train.size();
-    const int words = mask_words_per_row(W);
-    const uint64_t limit = p.max_blocks ? std::min(p.max_blocks, SPARSE_MAX_BLOCKS) : SPARSE_MAX_BLOCKS;
-    uint64_t clipped = 0, blocks = 0;
-    for (int q = 0; q < count; ++q) {
-        const Keyframe& kf = m->train[p.views ? p.views[q] : q];
-        MAP_TRY(draw_mesh_view(m, kf, r, false, "mapper_extract_mesh_sparse"));
-        for (;;) {
-            const int64_t* c = (const int64_t*)m->counters_host.raw();
-            MAP_TRY(glic_block_set_insert(&set, p.origin, p.voxel_size, kf.cam_dev, W, H, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, r.median,
-                                          kf.mask_valid ? (const uint32_t*)kf.mask : nullptr, words, p.trunc, p.max_depth,
-                                          (int64_t*)m->counters_host.raw(), s));
-            GLIC_CUDA_TRY(cudaStreamSynchronize(s));
-            // the count is exact, and an overflow means more blocks than the capacity
-            const bool over = c[2] != 0;
-            blocks = (uint64_t)c[0];
-            if ((over && set.capacity >= limit) || (!over && blocks > limit)) {
-                set_error("mapper_extract_mesh_sparse: the map needs more than " + std::to_string(limit) + " blocks" +
-                          (p.max_blocks ? " (max_blocks)" : ""));
-                return GLIC_ERR_WORKSPACE;
-            }
-            if (!over) { clipped += (uint64_t)c[1]; break; }
-            Buf bigger;
-            MAP_TRY(bigger.allocate(glic_block_set_bytes(2 * set.capacity)));
-            const glic_block_set next{2 * set.capacity, bigger.raw()};
-            MAP_TRY(glic_block_set_copy(&set, &next, s));
-            GLIC_CUDA_TRY(cudaStreamSynchronize(s));       // the old set is read until the copy ends
-            set_buf = std::move(bigger);
-            set = next;
-        }
-    }
-    Buf grid_buf, scratch;
-    MAP_TRY(grid_buf.allocate(glic_sparse_tsdf_bytes((uint32_t)blocks)));
-    MAP_TRY(scratch.allocate(glic_sparse_mesh_scratch_bytes((uint32_t)blocks)));
-    glic_sparse_tsdf grid;
-    for (int a = 0; a < 3; ++a) grid.origin[a] = p.origin[a];
-    grid.voxel_size = p.voxel_size;
-    grid.n_blocks = (uint32_t)blocks;
-    grid.data = grid_buf.raw();
-    MAP_TRY(glic_sparse_tsdf_init(&grid, &set, s));
-    for (int q = 0; q < count; ++q) {
-        const Keyframe& kf = m->train[p.views ? p.views[q] : q];
-        MAP_TRY(draw_mesh_view(m, kf, r, true, "mapper_extract_mesh_sparse"));
-        MAP_TRY(glic_sparse_tsdf_integrate(&grid, kf.cam_dev, W, H, m->cfg.fx, m->cfg.fy, m->cfg.cx, m->cfg.cy, r.median, r.rgb,
-                                           kf.mask_valid ? (const uint32_t*)kf.mask : nullptr, words, p.trunc, p.max_depth, s));
-    }
-    glic_sparse_mesh_counts c;
-    MAP_TRY(glic_sparse_mesh_count(&grid, scratch.raw(), scratch.bytes(), &c, s));
-    c.clipped_pixels = (uint32_t)std::min<uint64_t>(clipped, 0xFFFFFFFFull);
-    Buf ws;
-    MAP_TRY(ws.allocate(glic_sparse_mesh_extract_bytes(c.vertices, c.faces)));
-    MAP_TRY(replace_mesh(m, glic_mesh_counts{c.vertices, c.faces, c.observed_voxels}, [&](float* xyz, uint8_t* rgb, int32_t* faces) {
-        return glic_sparse_mesh_extract(&grid, scratch.raw(), scratch.bytes(), &c, ws.raw(), ws.bytes(), xyz, rgb, faces, s);
-    }));
-    if (out) *out = c;
-    return GLIC_OK;
-}
+namespace mapper_impl {
 
 // ---- pose corrections (glic_mapper_correct_poses) ----------------------------------------------------------------------------
 // After the checks: the records, one allocation (a failure changes nothing), the row pass, the keyframes.
@@ -2218,596 +1362,9 @@ int correct_poses(glic_mapper* m, int n, const glic_pose_correction* c, uint32_t
     return GLIC_OK;
 }
 
-// ---- checkpoints (glic_mapper_save_checkpoint, glic_mapper_load_checkpoint) ------------------------------------------------
-// The file's framing, fixed fields and validation are map_io.cu's (checkpoint.h); here the arrays move between it and the device
-// through two pinned chunks: while one chunk is written (read), the copy of the other is in flight.
-constexpr size_t CKPT_CHUNK = size_t(8) << 20;
-
-int make_events(Event (&ev)[2]) {
-    for (Event& e : ev) {
-        cudaEvent_t h = nullptr;
-        GLIC_CUDA_TRY(cudaEventCreateWithFlags(&h, cudaEventDisableTiming));
-        e = Event(h);
-    }
-    return GLIC_OK;
-}
-
-// A section's bytes in file order: device spans are copied on `s` into the current chunk, which is written once full while the
-// other chunk fills; host bytes are written in place once every device byte before them is.
-class SaveStream {
-public:
-    SaveStream(ckpt::Writer& w, cudaStream_t s, char* stage, const Event (&ev)[2]) : w_(w), s_(s), ev_{ev[0], ev[1]} {
-        buf_[0] = stage; buf_[1] = stage + CKPT_CHUNK;
-    }
-    int begin(ckpt::Section sec, uint64_t length) { MAP_TRY(flush()); return w_.begin(sec, length); }
-    int end() { MAP_TRY(flush()); return w_.end(); }
-    int device(const void* src, size_t n) {
-        const char* p = static_cast<const char*>(src);
-        while (n) {
-            const size_t k = std::min(n, CKPT_CHUNK - fill_);
-            GLIC_CUDA_TRY(cudaMemcpyAsync(buf_[cur_] + fill_, p, k, cudaMemcpyDeviceToHost, s_));
-            fill_ += k; p += k; n -= k;
-            if (fill_ == CKPT_CHUNK) MAP_TRY(submit());
-        }
-        return GLIC_OK;
-    }
-    int host(const void* p, size_t n) { MAP_TRY(flush()); return w_.write(p, n); }
-    int host(const ckpt::Bytes& b) { return host(b.b.data(), b.b.size()); }
-    int flush() { MAP_TRY(submit()); return drain(); }
-private:
-    // the current chunk's copies are enqueued: write the other chunk, then fill that one
-    int submit() {
-        if (!fill_) return GLIC_OK;
-        GLIC_CUDA_TRY(cudaEventRecord(ev_[cur_], s_));
-        MAP_TRY(drain());
-        pending_ = fill_; cur_ ^= 1; fill_ = 0;
-        return GLIC_OK;
-    }
-    int drain() {                                  // writes the submitted chunk (the one that is not current)
-        if (!pending_) return GLIC_OK;
-        GLIC_CUDA_TRY(cudaEventSynchronize(ev_[cur_ ^ 1]));
-        MAP_TRY(w_.write(buf_[cur_ ^ 1], pending_));
-        pending_ = 0;
-        return GLIC_OK;
-    }
-    ckpt::Writer& w_;
-    cudaStream_t s_;
-    cudaEvent_t ev_[2];
-    char* buf_[2];
-    int cur_ = 0;
-    size_t fill_ = 0, pending_ = 0;
-};
-
-// File bytes at given offsets into device memory (read into one chunk while the other's copy on `s` is in flight) or host memory
-class LoadStream {
-public:
-    LoadStream(cudaStream_t s, char* stage, const Event (&ev)[2]) : s_(s), ev_{ev[0], ev[1]} { buf_[0] = stage; buf_[1] = stage + CKPT_CHUNK; }
-    ~LoadStream() { if (f_) std::fclose(f_); }
-    int open(const char* path) {
-        f_ = std::fopen(path, "rb");
-        if (!f_) { set_error(std::string("checkpoint: cannot open ") + path); return GLIC_ERR_INVALID_ARGUMENT; }
-        return GLIC_OK;
-    }
-    int device(uint64_t off, void* dst, size_t n) {
-        MAP_TRY(seek(off));
-        char* d = static_cast<char*>(dst);
-        while (n) {
-            const size_t k = std::min(n, CKPT_CHUNK);
-            if (busy_[cur_]) GLIC_CUDA_TRY(cudaEventSynchronize(ev_[cur_]));
-            MAP_TRY(read(buf_[cur_], k));
-            GLIC_CUDA_TRY(cudaMemcpyAsync(d, buf_[cur_], k, cudaMemcpyHostToDevice, s_));
-            GLIC_CUDA_TRY(cudaEventRecord(ev_[cur_], s_));
-            busy_[cur_] = true; cur_ ^= 1; d += k; n -= k;
-        }
-        return GLIC_OK;
-    }
-    int host(uint64_t off, void* dst, size_t n) { MAP_TRY(seek(off)); return read(dst, n); }
-private:
-    int seek(uint64_t off) {
-        if (off == pos_) return GLIC_OK;
-        if (fseeko(f_, (off_t)off, SEEK_SET) != 0) { set_error("checkpoint: cannot seek"); return GLIC_ERR_INVALID_ARGUMENT; }
-        pos_ = off;
-        return GLIC_OK;
-    }
-    int read(void* p, size_t n) {
-        if (n && std::fread(p, 1, n, f_) != n) { set_error("checkpoint: truncated file"); return GLIC_ERR_INVALID_ARGUMENT; }
-        pos_ += n;
-        return GLIC_OK;
-    }
-    FILE* f_ = nullptr;
-    uint64_t pos_ = 0;
-    cudaStream_t s_;
-    cudaEvent_t ev_[2];
-    char* buf_[2];
-    bool busy_[2] = {false, false};
-    int cur_ = 0;
-};
-
-static_assert(sizeof(CamBlock) == 42 * sizeof(float), "the host camera block is 42 floats in the file");
-
-uint32_t image_kind(const Keyframe& kf) { return kf.bgr ? ckpt::IMAGE_BGR8 : kf.image_on_device ? ckpt::IMAGE_DEVICE : ckpt::IMAGE_HOST; }
-
-// the slot of an add_frame keyframe's image in the frame store
-uint32_t frame_index(const glic_mapper* m, const uint8_t* bgr) {
-    for (size_t c = 0; c < m->frame_chunks.size(); ++c) {
-        const uint8_t* base = m->frame_chunks[c];
-        if (bgr >= base && bgr < base + FRAME_CHUNK * m->frame_stride) return (uint32_t)(c * FRAME_CHUNK + (size_t)(bgr - base) / m->frame_stride);
-    }
-    return ckpt::NO_FRAME;
-}
-
-uint32_t feature_flags(const glic_mapper* m) {
-    return (m->initialized ? ckpt::F_INITIALIZED : 0) | (m->expo_on ? ckpt::F_EXPOSURE : 0) | (m->pose_on ? ckpt::F_POSE : 0) |
-           (m->dens_on ? ckpt::F_DENSIFICATION : 0) | (m->frames_on ? ckpt::F_FRAMES : 0);
-}
-
-// glic_mapper_save_checkpoint after its checks: the drain, the staging, then every section in file order
-int save_checkpoint(glic_mapper* m, const char* path) {
-    using namespace ckpt;
-    const int W = m->cfg.width, H = m->cfg.height;
-    const size_t HW = (size_t)W * H, P = m->P, mask_bytes = sizeof(uint32_t) * (size_t)H * mask_words_per_row(W);
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    MAP_TRY(poll_ring(m, true));
-    Buf stage;
-    MAP_TRY(stage.allocate(2 * CKPT_CHUNK, true));
-    Event ev[2];
-    MAP_TRY(make_events(ev));
-    Writer w;
-    MAP_TRY(w.open(path));
-    glic_mapper_config cfg = m->cfg;
-    cfg.capacity = m->Pcap;                                  // a restored mapper is created at the saved capacity
-    MAP_TRY(w.header(cfg));
-    SaveStream out(w, m->copy_stream, static_cast<char*>(stage.raw()), ev);
-    // the map: the live rows of the six groups of each arena, then the anchors
-    MAP_TRY(out.begin(MAP, map_bytes(P, m->M)));
-    MAP_TRY(out.host(Bytes().put(m->P).put(m->Pcap).put(m->n_sky)));
-    const auto kk = group_widths(m->M);
-    for (float* arena : {(float*)m->params, (float*)m->m1, (float*)m->m2}) {
-        const auto g = arena_rows(arena, m->Pcap, m->M).groups();
-        for (int q = 0; q < 6; ++q) MAP_TRY(out.device(g[q], sizeof(float) * kk[q] * P));
-    }
-    MAP_TRY(out.device(m->anchor, sizeof(int32_t) * P));
-    MAP_TRY(out.end());
-    // the counters, the options and the view sampler
-    {
-        std::ostringstream os;
-        os << m->rng;
-        const std::string rng = os.str();
-        Bytes b;
-        put_stats(b, m->st);
-        b.put(m->view_counter).put<int64_t>(m->bin_cap).put<uint64_t>(m->binning_ws.bytes()).put<uint64_t>(m->sample_ws.bytes())
-         .put<uint32_t>(m->run_optimizer).put<uint32_t>(m->deterministic).put(feature_flags(m)).put<uint32_t>((uint32_t)rng.size())
-         .put_n(rng.data(), rng.size());
-        MAP_TRY(out.begin(COUNTERS, counters_bytes(rng.size())));
-        MAP_TRY(out.host(b));
-        MAP_TRY(out.end());
-    }
-    // the keyframes, training then held-out
-    uint64_t kf_bytes = 8;
-    for (const auto* list : {&m->train, &m->test})
-        for (const Keyframe& kf : *list) kf_bytes += keyframe_bytes(image_kind(kf), kf.mask_valid, W, H);
-    MAP_TRY(out.begin(KEYFRAMES, kf_bytes));
-    MAP_TRY(out.host(Bytes().put((uint32_t)m->train.size()).put((uint32_t)m->test.size())));
-    for (const auto* list : {&m->train, &m->test})
-        for (const Keyframe& kf : *list) {
-            const uint32_t kind = image_kind(kf);
-            MAP_TRY(out.host(Bytes().put_n(kf.R_wc, 9).put_n(kf.t_wc, 3).put_n(reinterpret_cast<const float*>(&kf.cam), 42)));
-            MAP_TRY(out.device(kf.cam_dev, 36 * sizeof(float)));   // verbatim: pose refinement and corrections move it on the device
-            MAP_TRY(out.host(Bytes().put(kind).put(kind == IMAGE_BGR8 ? frame_index(m, kf.bgr) : NO_FRAME).put(kf.mask_valid)
-                                    .put(kf.mask_valid_left)));
-            if (kind == IMAGE_BGR8) MAP_TRY(out.device(kf.bgr, 3 * HW));
-            else if (kind == IMAGE_DEVICE) MAP_TRY(out.device(kf.image, sizeof(float) * 3 * HW));
-            else MAP_TRY(out.host(kf.image, sizeof(float) * 3 * HW));   // read where the caller keeps it
-            if (kf.mask_valid) MAP_TRY(out.device(kf.mask, mask_bytes));
-        }
-    MAP_TRY(out.end());
-    const size_t n = m->train.size();
-    if (m->expo_on) {
-        MAP_TRY(out.begin(ckpt::EXPOSURE, exposure_bytes(n)));
-        MAP_TRY(out.host(Bytes().put(m->expo_lr).put((uint32_t)n)));
-        const KeyframeAdam& a = m->expo_adam;
-        MAP_TRY(out.device(m->expo_E, 48 * n)); MAP_TRY(out.device(a.m, 48 * n)); MAP_TRY(out.device(a.v, 48 * n)); MAP_TRY(out.device(a.t, 4 * n));
-        MAP_TRY(out.end());
-    }
-    if (m->pose_on) {
-        MAP_TRY(out.begin(ckpt::POSE, pose_bytes(n)));
-        MAP_TRY(out.host(Bytes().put(m->pose_lr_rho).put(m->pose_lr_omega).put((uint32_t)n)));
-        const KeyframeAdam& a = m->pose_adam;
-        MAP_TRY(out.device(m->pose_T, 96 * n)); MAP_TRY(out.device(m->pose_f, 48 * n));
-        MAP_TRY(out.device(a.m, 24 * n)); MAP_TRY(out.device(a.v, 24 * n)); MAP_TRY(out.device(a.t, 4 * n));
-        MAP_TRY(out.end());
-    }
-    if (m->dens_on) {
-        MAP_TRY(out.begin(DENSIFICATION, densification_bytes(P)));
-        MAP_TRY(out.host(Bytes().put<uint64_t>(m->dens_calls).put(m->P)));
-        MAP_TRY(out.device(m->dens_accum, 4 * P)); MAP_TRY(out.device(m->dens_denom, 4 * P)); MAP_TRY(out.device(m->dens_maxr, 4 * P));
-        MAP_TRY(out.end());
-    }
-    {
-        Bytes b;
-        put_schedule(b, m->sched_on, m->sched, m->sched_totals, m->sched_steps, m->sched_resets);
-        MAP_TRY(out.begin(SCHEDULE, SCHEDULE_BYTES));
-        MAP_TRY(out.host(b));
-        MAP_TRY(out.end());
-    }
-    if (m->frames_on) {
-        const size_t p = m->fst.pending_points;
-        Bytes b;
-        b.put<int32_t>(m->frame_k).put<int32_t>(m->frame_sky_points).put<int32_t>(m->frame_sky_radius);
-        put_frame_stats(b, m->fst);
-        MAP_TRY(out.begin(FRAMES, frames_bytes(p)));
-        MAP_TRY(out.host(b));
-        MAP_TRY(out.device(m->scan_xyz, 12 * p)); MAP_TRY(out.device(m->scan_rgb, 3 * p)); MAP_TRY(out.device(m->scan_depth, 4 * p));
-        MAP_TRY(out.end());
-    }
-    return w.commit();
-}
-
-// created, and nothing since that leaves a trace in the state a checkpoint holds (load_lpips and set_option aside)
-bool mapper_fresh(const glic_mapper* m) {
-    return !m->initialized && m->P == 0 && m->train.empty() && m->test.empty() && !m->expo_on && !m->pose_on && !m->dens_on &&
-           !m->frames_on && !m->sched_on && !m->exported && !m->connected;
-}
-
-// every field but the capacity, floats by their bits
-bool same_config(const glic_mapper_config& a, const glic_mapper_config& b) {
-    ckpt::Bytes x, y;
-    glic_mapper_config a1 = a, b1 = b;
-    a1.capacity = b1.capacity = 0;
-    ckpt::put_config(x, a1);
-    ckpt::put_config(y, b1);
-    return x.b == y.b;
-}
-
-// glic_mapper_load_checkpoint after its checks: validate the whole file, allocate everything (keyframes first, then the mapper's
-// buffers in one growth whose fill streams the file in), and only then set the scalars
-int load_checkpoint(glic_mapper* m, const char* path) {
-    using namespace ckpt;
-    if (!mapper_fresh(m)) {
-        set_error("mapper_load_checkpoint: the mapper is not fresh (load into a mapper that is only created, with no rows, keyframes or "
-                  "features, before glic_mapper_export)");
-        return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    auto in = std::make_unique<Info>();
-    MAP_TRY(read_info(path, *in));
-    if (!same_config(in->cfg, m->cfg)) {
-        set_error("mapper_load_checkpoint: the mapper's configuration differs from the checkpoint's (create it from "
-                  "glic_mapper_checkpoint_config)");
-        return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    const int W = m->cfg.width, H = m->cfg.height;
-    const size_t HW = (size_t)W * H, mask_bytes = sizeof(uint32_t) * (size_t)H * mask_words_per_row(W);
-    if (glic_binning_capacity(in->binning_bytes, in->sample_bytes, W, H, 0) != in->bin_cap) {
-        set_error("checkpoint: the binning workspaces do not give the saved binning capacity"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    const bool expo = in->flags & F_EXPOSURE, pose = in->flags & F_POSE, dens = in->flags & F_DENSIFICATION, frames = in->flags & F_FRAMES;
-    const uint64_t stride = frame_stride(W, H);
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    MAP_TRY(poll_ring(m, true));
-    // 1. the staging, the frame store and the keyframes, outside the mapper
-    Buf stage;
-    MAP_TRY(stage.allocate(2 * CKPT_CHUNK, true));
-    Event ev[2];
-    MAP_TRY(make_events(ev));
-    std::vector<Dev<uint8_t>> chunks(frames ? (in->fst.frames + FRAME_CHUNK - 1) / FRAME_CHUNK : 0);
-    for (Dev<uint8_t>& c : chunks) MAP_TRY(c.allocate(FRAME_CHUNK * stride));
-    std::vector<Keyframe> kfs(in->kf.size());
-    for (size_t i = 0; i < kfs.size(); ++i) {
-        const ckpt::Keyframe& r = in->kf[i];
-        Keyframe& k = kfs[i];
-        std::memcpy(k.R_wc, r.R_wc, sizeof(k.R_wc)); std::memcpy(k.t_wc, r.t_wc, sizeof(k.t_wc));
-        std::memcpy(&k.cam, r.cam, sizeof(k.cam));
-        MAP_TRY(k.cam_dev.allocate(36 * sizeof(float)));
-        if (r.kind == IMAGE_BGR8) {
-            k.bgr = chunks[r.frame / FRAME_CHUNK] + (r.frame % FRAME_CHUNK) * stride;
-        } else {                                             // the image keeps its memory class, now owned by the mapper
-            MAP_TRY(k.owned_image.allocate(sizeof(float) * 3 * HW, r.kind == IMAGE_HOST));
-            k.image = static_cast<const float*>(k.owned_image.raw());
-            k.image_on_device = r.kind == IMAGE_DEVICE;
-        }
-        if (r.mask_valid) MAP_TRY(k.mask.allocate(mask_bytes));
-        k.mask_valid = r.mask_valid;
-        k.mask_valid_left = r.mask_valid_left;
-        k.view = make_view(k.cam, k.cam_dev, W, H);
-    }
-    // 2. the mapper's buffers at the saved capacity, as set_capacity, enable_densification, set_option, enable_exposure and
-    //    add_frame size them; zeroed where they start zeroed
-    const uint32_t cap = in->Pcap, P = in->P, n = in->n_train, pending = frames ? in->fst.pending_points : 0;
-    const XLayout x = xblock_layout(m->S, cap, dens);
-    const size_t arena = arena_floats(m, cap) * sizeof(float);
-    const size_t kf_cap = (expo || pose) ? std::max<size_t>(n, 64) : 0;
-    std::vector<Grow> list = {{m->params, arena, 0, true}, {m->m1, arena, 0, true}, {m->m2, arena, 0, true},
-                              {m->act_opacity, (size_t)cap * 4, 0, true}, {m->act_scales, (size_t)cap * 12, 0, true},
-                              {m->act_rots, (size_t)cap * 16, 0, true}, {m->radii, (size_t)cap * 4, 0, true},
-                              {m->g_conic, (size_t)cap * (16 + 12 + 4), 0, true}, {m->geom_ws, glic_geom_bytes((int)cap), 0, true},
-                              {m->xblock, x.bytes, 0, true}, {m->pose_part, pose_partials_count(cap) * sizeof(double)},
-                              {m->anchor, (size_t)cap * 4}, {m->binning_ws, (size_t)in->binning_bytes}, {m->sample_ws, (size_t)in->sample_bytes}};
-    if (dens)
-        for (Buf* b : {(Buf*)&m->dens_accum, (Buf*)&m->dens_denom, (Buf*)&m->dens_maxr}) list.push_back({*b, (size_t)cap * 4, 0, true});
-    if (in->deterministic) {
-        list.push_back({m->det_ws, glic_deterministic_bytes(in->bin_cap, W, H)});
-        list.push_back({m->det_sums, fixed_order_sums_bytes(H, W)});
-    }
-    if (expo && glic_loss_exposure_scratch_bytes(H, W) > m->loss_scratch.bytes()) list.push_back({m->loss_scratch, glic_loss_exposure_scratch_bytes(H, W)});
-    for (auto [b, row] : std::initializer_list<std::pair<Buf*, size_t>>{
-             {&m->expo_E, 48}, {&m->expo_adam.m, 48}, {&m->expo_adam.v, 48}, {&m->expo_adam.t, 4}, {&m->pose_T, 96}, {&m->pose_f, 48},
-             {&m->pose_adam.m, 24}, {&m->pose_adam.v, 24}, {&m->pose_adam.t, 4}})
-        if (kf_cap) list.push_back({*b, kf_cap * row, 0, true});
-    if (pending) {
-        list.push_back({m->scan_xyz, (size_t)pending * 12});
-        list.push_back({m->scan_rgb, (size_t)pending * 3});
-        list.push_back({m->scan_depth, (size_t)pending * 4});
-    }
-    auto fill = [&](Buf* fresh) -> int {
-        auto at = [&](const Buf& b) -> char* {
-            for (size_t i = 0; i < list.size(); ++i) if (&list[i].buf == &b) return static_cast<char*>(fresh[i].raw());
-            return nullptr;
-        };
-        LoadStream L(m->stream, static_cast<char*>(stage.raw()), ev);
-        MAP_TRY(L.open(path));
-        const auto kk = group_widths(m->M);
-        uint64_t off = in->map_off;
-        for (const Buf* a : {(const Buf*)&m->params, (const Buf*)&m->m1, (const Buf*)&m->m2}) {
-            const auto g = arena_rows(reinterpret_cast<float*>(at(*a)), cap, m->M).groups();
-            for (int q = 0; q < 6; ++q) {
-                MAP_TRY(L.device(off, g[q], sizeof(float) * kk[q] * P));
-                off += sizeof(float) * kk[q] * P;
-            }
-        }
-        MAP_TRY(L.device(off, at(m->anchor), sizeof(int32_t) * P));
-        for (size_t i = 0; i < kfs.size(); ++i) {
-            const ckpt::Keyframe& r = in->kf[i];
-            Keyframe& k = kfs[i];
-            GLIC_CUDA_TRY(cudaMemcpyAsync(k.cam_dev, r.cam_dev, sizeof(r.cam_dev), cudaMemcpyHostToDevice, m->stream));
-            if (r.kind == IMAGE_BGR8) MAP_TRY(L.device(r.image_off, const_cast<uint8_t*>(k.bgr), 3 * HW));
-            else if (r.kind == IMAGE_DEVICE) MAP_TRY(L.device(r.image_off, k.owned_image.raw(), sizeof(float) * 3 * HW));
-            else MAP_TRY(L.host(r.image_off, k.owned_image.raw(), sizeof(float) * 3 * HW));
-            if (r.mask_valid) MAP_TRY(L.device(r.mask_off, k.mask, mask_bytes));
-        }
-        // consecutive arrays of one section
-        auto arrays = [&](uint64_t o, std::initializer_list<std::pair<void*, size_t>> dst) -> int {
-            for (const auto& [p, bytes] : dst) { MAP_TRY(L.device(o, p, bytes)); o += bytes; }
-            return GLIC_OK;
-        };
-        if (expo) MAP_TRY(arrays(in->expo_off, {{at(m->expo_E), 48 * (size_t)n}, {at(m->expo_adam.m), 48 * (size_t)n},
-                                                {at(m->expo_adam.v), 48 * (size_t)n}, {at(m->expo_adam.t), 4 * (size_t)n}}));
-        if (pose) MAP_TRY(arrays(in->pose_off, {{at(m->pose_T), 96 * (size_t)n}, {at(m->pose_f), 48 * (size_t)n}, {at(m->pose_adam.m), 24 * (size_t)n},
-                                                {at(m->pose_adam.v), 24 * (size_t)n}, {at(m->pose_adam.t), 4 * (size_t)n}}));
-        if (dens) MAP_TRY(arrays(in->dens_off, {{at(m->dens_accum), 4 * (size_t)P}, {at(m->dens_denom), 4 * (size_t)P}, {at(m->dens_maxr), 4 * (size_t)P}}));
-        if (pending) MAP_TRY(arrays(in->frames_off, {{at(m->scan_xyz), 12 * (size_t)pending}, {at(m->scan_rgb), 3 * (size_t)pending},
-                                                     {at(m->scan_depth), 4 * (size_t)pending}}));
-        return GLIC_OK;
-    };
-    // a failed read returns with copies in flight into the new buffers: they finish before the buffers are released
-    MAP_TRY(grow(m, list, [&](Buf* fresh) { const int e = fill(fresh); if (e) cudaStreamSynchronize(m->stream); return e; }));
-    // 3. the state: nothing below can fail
-    for (size_t i = 0; i < kfs.size(); ++i) (i < n ? m->train : m->test).push_back(std::move(kfs[i]));
-    m->frame_chunks = std::move(chunks);
-    m->cfg.capacity = cap;
-    m->Pcap = cap; m->P = P; m->n_sky = in->n_sky;
-    m->x = x;
-    m->g_mean2D = m->g_conic + (size_t)cap * 4;
-    m->g_opacity = m->g_mean2D + (size_t)cap * 3;
-    m->peers[m->cfg.rank] = m->xblock;
-    m->st = in->st;
-    m->view_counter = in->view_counter;
-    m->rng = in->rng;
-    m->bin_cap = in->bin_cap;
-    m->run_optimizer = in->optimizer != 0;
-    m->deterministic = in->deterministic != 0;
-    m->initialized = in->flags & F_INITIALIZED;
-    m->kf_cap = kf_cap;
-    m->expo_on = expo; m->expo_lr = in->expo_lr;
-    m->pose_on = pose; m->pose_lr_rho = in->pose_lr_rho; m->pose_lr_omega = in->pose_lr_omega;
-    m->dens_on = dens; m->dens_calls = in->dens_calls;
-    m->sched_on = in->sched_on != 0; m->sched = in->sched; m->sched_totals = in->sched_totals;
-    m->sched_steps = in->sched_steps; m->sched_resets = in->sched_resets;
-    m->frames_on = frames;
-    if (frames) {
-        m->frame_k = in->frame_k; m->frame_sky_points = in->sky_points; m->frame_sky_radius = in->sky_radius;
-        m->frame_stride = stride;
-        m->fst = in->fst;
-        m->scan_cap = pending;
-    }
-    return GLIC_OK;
-}
-
-}  // namespace
+}  // namespace mapper_impl
 
 extern "C" {
-
-int glic_mapper_extract_mesh(glic_mapper* m, const glic_mesh_params* p, glic_mesh_counts* out) {
-    if (!m || !p) { set_error("mapper_extract_mesh: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!glic_tsdf_bytes(p->dims)) {
-        set_error("mapper_extract_mesh: every grid dimension must be in [2, 2048], with fewer than 2^31 lattice points"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (!(std::isfinite(p->voxel_size) && p->voxel_size > 0.0f) || !std::isfinite(p->origin[0]) || !std::isfinite(p->origin[1]) ||
-        !std::isfinite(p->origin[2])) {
-        set_error("mapper_extract_mesh: voxel_size must be finite and > 0, the origin finite"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (!(std::isfinite(p->trunc) && p->trunc > 0.0f)) { set_error("mapper_extract_mesh: trunc must be finite and > 0"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!(std::isfinite(p->max_depth) && p->max_depth >= 0.0f)) {
-        set_error("mapper_extract_mesh: max_depth must be finite and >= 0"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    MAP_TRY(views_check(m, p->views, p->n_views, "mapper_extract_mesh"));
-    if (m->P <= m->n_sky) { set_error("mapper_extract_mesh: the mapper has no non-sky rows"); return GLIC_ERR_INVALID_ARGUMENT; }
-    return extract_mesh(m, *p, out);
-}
-
-int glic_mapper_extract_mesh_sparse(glic_mapper* m, const glic_sparse_mesh_params* p, glic_sparse_mesh_counts* out) {
-    if (!m || !p) { set_error("mapper_extract_mesh_sparse: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!(std::isfinite(p->voxel_size) && p->voxel_size > 0.0f) || !std::isfinite(p->origin[0]) || !std::isfinite(p->origin[1]) ||
-        !std::isfinite(p->origin[2])) {
-        set_error("mapper_extract_mesh_sparse: voxel_size must be finite and > 0, the origin finite"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (!(std::isfinite(p->trunc) && p->trunc > 0.0f)) { set_error("mapper_extract_mesh_sparse: trunc must be finite and > 0"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!(std::isfinite(p->max_depth) && p->max_depth >= 0.0f)) {
-        set_error("mapper_extract_mesh_sparse: max_depth must be finite and >= 0"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    MAP_TRY(views_check(m, p->views, p->n_views, "mapper_extract_mesh_sparse"));
-    if (m->P <= m->n_sky) { set_error("mapper_extract_mesh_sparse: the mapper has no non-sky rows"); return GLIC_ERR_INVALID_ARGUMENT; }
-    return extract_mesh_sparse(m, *p, out);
-}
-
-int glic_mapper_mesh_get(glic_mapper* m, glic_mesh_counts* counts, float* xyz, uint8_t* rgb, int32_t* faces) {
-    if (!m) { set_error("mapper_mesh_get: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (counts) *counts = m->mesh_counts;
-    const size_t V = m->mesh_counts.vertices, F = m->mesh_counts.faces;
-    if (xyz && V) GLIC_CUDA_TRY(cudaMemcpyAsync(xyz, m->mesh_xyz, 12 * V, cudaMemcpyDefault, m->stream));
-    if (rgb && V) GLIC_CUDA_TRY(cudaMemcpyAsync(rgb, m->mesh_rgb, 3 * V, cudaMemcpyDefault, m->stream));
-    if (faces && F) GLIC_CUDA_TRY(cudaMemcpyAsync(faces, m->mesh_faces, 12 * F, cudaMemcpyDefault, m->stream));
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    return GLIC_OK;
-}
-
-int glic_mapper_save_mesh(glic_mapper* m, const char* path) {
-    if (!m || !path) { set_error("mapper_save_mesh: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!m->mesh_ready) { set_error("mapper_save_mesh: no mesh extracted yet (glic_mapper_extract_mesh)"); return GLIC_ERR_INVALID_ARGUMENT; }
-    const glic_mesh_counts c = m->mesh_counts;
-    std::vector<float> xyz(3 * (size_t)c.vertices);
-    std::vector<uint8_t> rgb(3 * (size_t)c.vertices);
-    std::vector<int32_t> faces(3 * (size_t)c.faces);
-    MAP_TRY(glic_mapper_mesh_get(m, nullptr, xyz.data(), rgb.data(), faces.data()));
-    return glic_mesh_ply_write(path, c.vertices, xyz.data(), rgb.data(), c.faces, faces.data());
-}
-
-int glic_mapper_contribution(glic_mapper* m, const int* views_host, int n_views, float* max_weight, uint64_t* hits, uint64_t* ends) {
-    if (!m || (!max_weight && !hits && !ends)) { set_error("mapper_contribution: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    MAP_TRY(views_check(m, views_host, n_views, "mapper_contribution"));
-    MAP_TRY(poll_ring(m, true));
-    MAP_TRY(reserve(m, m->score_ws, score_bytes(m->Pcap)));
-    MAP_TRY(contribution(m, views_host, n_views));
-    const uint64_t* h = reinterpret_cast<const uint64_t*>(m->score_ws.raw());
-    if (m->P && hits) GLIC_CUDA_TRY(cudaMemcpyAsync(hits, h, sizeof(uint64_t) * m->P, cudaMemcpyDefault, m->stream));
-    if (m->P && ends) GLIC_CUDA_TRY(cudaMemcpyAsync(ends, h + m->Pcap, sizeof(uint64_t) * m->P, cudaMemcpyDefault, m->stream));
-    if (m->P && max_weight) GLIC_CUDA_TRY(cudaMemcpyAsync(max_weight, h + 2 * (size_t)m->Pcap, sizeof(float) * m->P, cudaMemcpyDefault, m->stream));
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    return GLIC_OK;
-}
-
-// the scores, then the compaction with no row selected, both size tests and the opacity test off, and the unseen test on
-int glic_mapper_prune_unseen(glic_mapper* m, const glic_unseen_params* p, int dry_run, uint32_t* removed) {
-    if (!m || !p) { set_error("mapper_prune_unseen: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!std::isfinite(p->min_weight) || p->min_weight < 0.0f || p->min_weight > 1.0f) {
-        set_error("mapper_prune_unseen: min_weight must be finite and in [0, 1]"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (p->sky != 0 && p->sky != 1) { set_error("mapper_prune_unseen: sky must be 0 or 1"); return GLIC_ERR_INVALID_ARGUMENT; }
-    MAP_TRY(views_check(m, p->views, p->n_views, "mapper_prune_unseen"));
-    if (m->P) {
-        MAP_TRY(poll_ring(m, true));
-        MAP_TRY(reserve(m, m->score_ws, score_bytes(m->Pcap)));
-        MAP_TRY(reserve(m, m->extend_ws, density_scratch_bytes(m->P)));      // the selection's scratch (density_step)
-        MAP_TRY(contribution(m, p->views, p->n_views));
-    }
-    glic_density_counts k{};
-    MAP_TRY(density_step(m, glic_density_params{0.0f, 0.0f, 0.0f, 0.0f, 0, 0.0f}, false, dry_run, m->P != 0, &k, "mapper_prune_unseen", p));
-    if (removed) *removed = k.pruned;
-    return GLIC_OK;
-}
-
-// the compaction with no row selected and both size tests off; a mapper with no rows has nothing to remove (0, not an error)
-int glic_mapper_prune(glic_mapper* m, float min_opacity, int dry_run, uint32_t* removed) {
-    if (!m) { set_error("mapper_prune: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!std::isfinite(min_opacity) || min_opacity < 0.0f || min_opacity > 1.0f) {
-        set_error("mapper_prune: min_opacity must be finite and in [0, 1]"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    glic_density_counts k{};
-    MAP_TRY(density_step(m, glic_density_params{0.0f, 0.0f, 0.0f, min_opacity, 0, 0.0f}, false, dry_run, m->P != 0, &k, "mapper_prune"));
-    if (removed) *removed = k.pruned;
-    return GLIC_OK;
-}
-
-int glic_mapper_densify(glic_mapper* m, float grad_threshold, float percent_dense, float scene_extent, int dry_run, uint32_t* cloned,
-                        uint32_t* split) {
-    if (!m) { set_error("mapper_densify: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!m->dens_on) { set_error("mapper_densify: densification is not enabled (glic_mapper_enable_densification)"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!finite_at_least_zero(grad_threshold) || !finite_at_least_zero(percent_dense) || !std::isfinite(scene_extent) || !(scene_extent > 0.0f)) {
-        set_error("mapper_densify: grad_threshold and percent_dense must be finite and >= 0, scene_extent finite and > 0");
-        return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    glic_density_counts k{};
-    MAP_TRY(density_step(m, glic_density_params{grad_threshold, percent_dense, scene_extent, 0.0f, 0, 0.0f}, true, dry_run, false, &k, "mapper_densify"));
-    if (cloned) *cloned = k.cloned;
-    if (split) *split = k.split;
-    return GLIC_OK;
-}
-
-int glic_mapper_densify_and_prune(glic_mapper* m, const glic_density_params* p, int dry_run, glic_density_counts* out) {
-    if (!m || !p) { set_error("mapper_densify_and_prune: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!m->dens_on) { set_error("mapper_densify_and_prune: densification is not enabled (glic_mapper_enable_densification)"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!finite_at_least_zero(p->grad_threshold) || !finite_at_least_zero(p->percent_dense) || !std::isfinite(p->scene_extent) ||
-        !(p->scene_extent > 0.0f) || !finite_at_least_zero(p->min_opacity) || p->min_opacity > 1.0f || p->max_screen_radius < 0 ||
-        !finite_at_least_zero(p->max_world_scale)) {
-        set_error("mapper_densify_and_prune: grad_threshold, percent_dense and max_world_scale must be finite and >= 0, scene_extent finite "
-                  "and > 0, min_opacity in [0, 1], max_screen_radius >= 0");
-        return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    return density_step(m, *p, true, dry_run, true, out, "mapper_densify_and_prune");
-}
-
-int glic_mapper_screen_radii(glic_mapper* m, int32_t* out) {
-    if (!m || !out) { set_error("mapper_screen_radii: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!m->dens_on) { set_error("mapper_screen_radii: densification is not enabled (glic_mapper_enable_densification)"); return GLIC_ERR_INVALID_ARGUMENT; }
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    if (m->P) GLIC_CUDA_TRY(cudaMemcpy(out, m->dens_maxr, (size_t)m->P * 4, cudaMemcpyDeviceToHost));
-    return GLIC_OK;
-}
-
-// Inria's reset_opacity on the non-sky rows: one kernel (prune.cu) after the pipeline drains
-int glic_mapper_reset_opacity(glic_mapper* m, float max_opacity) {
-    if (!m) { set_error("mapper_reset_opacity: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!std::isfinite(max_opacity) || !(max_opacity > 0.0f) || !(max_opacity < 1.0f)) {
-        set_error("mapper_reset_opacity: max_opacity must be finite and in (0, 1)"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    MAP_TRY(poll_ring(m, true));
-    const double r = (double)max_opacity;
-    MAP_TRY(launch_reset_opacity(m->n_sky, m->P, m->Pcap, m->M, m->params, m->m1, m->m2, max_opacity, (float)std::log(r / (1.0 - r)), m->stream));
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    return GLIC_OK;
-}
-
-int glic_mapper_set_density_schedule(glic_mapper* m, const glic_density_schedule* c) {
-    if (!m) { set_error("mapper_set_density_schedule: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (c) {
-        if (!m->dens_on) { set_error("mapper_set_density_schedule: densification is not enabled (glic_mapper_enable_densification)"); return GLIC_ERR_INVALID_ARGUMENT; }
-        if (c->densify_interval == 0 || !finite_at_least_zero(c->grad_threshold) || !finite_at_least_zero(c->percent_dense) ||
-            !finite_at_least_zero(c->min_opacity) || c->min_opacity > 1.0f || !std::isfinite(c->reset_opacity) || !(c->reset_opacity > 0.0f) ||
-            !(c->reset_opacity < 1.0f) || c->screen_radius < 0 || !finite_at_least_zero(c->world_scale_factor) || !finite_at_least_zero(c->scene_extent)) {
-            set_error("mapper_set_density_schedule: densify_interval must be >= 1, grad_threshold, percent_dense, world_scale_factor and "
-                      "scene_extent finite and >= 0, min_opacity in [0, 1], reset_opacity in (0, 1), screen_radius >= 0");
-            return GLIC_ERR_INVALID_ARGUMENT;
-        }
-        m->sched = *c;
-    }
-    m->sched_on = c != nullptr;
-    m->sched_totals = glic_density_counts{};
-    m->sched_steps = m->sched_resets = 0;
-    return GLIC_OK;
-}
-
-int glic_mapper_scene_extent(glic_mapper* m, float* out) {
-    if (!m || !out) { set_error("mapper_scene_extent: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    return scene_extent(m, out);
-}
-
-int glic_mapper_density_totals(glic_mapper* m, glic_density_counts* out, uint32_t* steps, uint32_t* resets) {
-    if (!m) { set_error("mapper_density_totals: null mapper"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (out) *out = m->sched_totals;
-    if (steps) *steps = m->sched_steps;
-    if (resets) *resets = m->sched_resets;
-    return GLIC_OK;
-}
-
-int glic_mapper_densify_stats(glic_mapper* m, float* grad_accum, float* denom) {
-    if (!m || !grad_accum || !denom) { set_error("mapper_densify_stats: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!m->dens_on) { set_error("mapper_densify_stats: densification is not enabled (glic_mapper_enable_densification)"); return GLIC_ERR_INVALID_ARGUMENT; }
-    GLIC_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    if (!m->P) return GLIC_OK;
-    GLIC_CUDA_TRY(cudaMemcpy(grad_accum, m->dens_accum, (size_t)m->P * 4, cudaMemcpyDeviceToHost));
-    GLIC_CUDA_TRY(cudaMemcpy(denom, m->dens_denom, (size_t)m->P * 4, cudaMemcpyDeviceToHost));
-    return GLIC_OK;
-}
 
 int glic_mapper_save_map(glic_mapper* m, const char* path) {
     if (!m || !path) { set_error("mapper_save_map: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
@@ -2819,16 +1376,6 @@ int glic_mapper_save_map(glic_mapper* m, const char* path) {
     // is the consistently sliced one.
     return glic_ply_write(path, (uint32_t)(P - S), (uint32_t)M, xyz.data() + 3 * S, dc.data() + 3 * S, rest.data() + 3 * M * S, op.data() + S,
                           ls.data() + 3 * S, rot.data() + 4 * S);
-}
-
-int glic_mapper_save_checkpoint(glic_mapper* m, const char* path) {
-    if (!m || !path) { set_error("mapper_save_checkpoint: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    return save_checkpoint(m, path);
-}
-
-int glic_mapper_load_checkpoint(glic_mapper* m, const char* path) {
-    if (!m || !path) { set_error("mapper_load_checkpoint: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    return load_checkpoint(m, path);
 }
 
 int glic_mapper_stats_get(glic_mapper* m, glic_mapper_stats* out) {
@@ -2968,45 +1515,6 @@ int glic_mapper_correct_poses(glic_mapper* m, int n, const glic_pose_correction*
     if (moved) *moved = 0;
     if (n == 0) return GLIC_OK;
     return correct_poses(m, n, c, moved);
-}
-
-int glic_mapper_align(glic_mapper* m, int is_train, int index, const glic_align_params* p, glic_align_result* out, float* rgb_host) {
-    if (!m || !p || !out) { set_error("mapper_align: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    const Keyframe* kf = nullptr;
-    MAP_TRY(keyframe_at(m, is_train, index, "mapper_align", kf));
-    if (p->iterations < 0 || !finite_at_least_zero(p->lr_translation) || !finite_at_least_zero(p->lr_rotation) ||
-        !finite_at_least_zero(p->exposure_lr) || (p->split != 0 && p->split != 1)) {
-        set_error("mapper_align: iterations must be >= 0, the rates finite and >= 0, split 0 or 1"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    const int W = m->cfg.width, H = m->cfg.height, Ws = W - (p->split ? W / 2 : 0);
-    if (p->split && W < 2) { set_error("mapper_align: split needs a frame at least 2 columns wide"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (m->lpips_w && !glic_lpips_scratch_bytes(H, Ws)) { set_error("mapper_align: LPIPS needs a score region of at least 31x31"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (m->P == 0) { set_error("mapper_align: the map has no rows to align against"); return GLIC_ERR_INVALID_ARGUMENT; }
-    return align(m, *kf, is_train != 0, index, *p, out, rgb_host);
-}
-
-int glic_mapper_render_camera(glic_mapper* m, const glic_render_camera* cam, int exposure_index, int with_sky, float* rgb, float* final_T,
-                              float* depth, float* median_depth) {
-    if (!m || !cam || (!rgb && !final_T && !depth && !median_depth)) { set_error("mapper_render_camera: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    const glic_render_camera c = *cam;
-    if (c.width < 1 || c.height < 1) { set_error("mapper_render_camera: width and height must be >= 1"); return GLIC_ERR_INVALID_ARGUMENT; }
-    const int64_t tiles = (((int64_t)c.width + TILE - 1) / TILE) * (((int64_t)c.height + TILE - 1) / TILE);
-    if (tiles > GLIC_MAX_TILES) {
-        set_error("mapper_render_camera: " + std::to_string(c.width) + "x" + std::to_string(c.height) + " has " + std::to_string(tiles) +
-                  " tiles of 16x16, more than GLIC_MAX_TILES = " + std::to_string(GLIC_MAX_TILES));
-        return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (!(std::isfinite(c.fx) && c.fx > 0.0f) || !(std::isfinite(c.fy) && c.fy > 0.0f) || !std::isfinite(c.cx) || !std::isfinite(c.cy)) {
-        set_error("mapper_render_camera: fx and fy must be finite and > 0, cx and cy finite"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    MAP_TRY(pose_check(c.R_wc, c.t_wc, "mapper_render_camera"));
-    if (exposure_index != -1 && (!m->expo_on || exposure_index < 0 || exposure_index >= (int)m->train.size())) {
-        set_error("mapper_render_camera: exposure_index must be -1 or a training keyframe index with exposure enabled"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (with_sky != 0 && with_sky != 1) { set_error("mapper_render_camera: with_sky must be 0 or 1"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (m->P == 0) { set_error("mapper_render_camera: the mapper has no rows"); return GLIC_ERR_INVALID_ARGUMENT; }
-    float* const out[4] = {rgb, final_T, depth, median_depth};
-    return render_camera(m, c, exposure_index, with_sky, out);
 }
 
 int glic_mapper_synchronize(glic_mapper* m) {
