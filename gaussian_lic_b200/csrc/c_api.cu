@@ -48,6 +48,11 @@ static int check_view(const glic_view* v) {
     return GLIC_OK;
 }
 
+static int fail(int status, const char* name, const char* what) {
+    set_error(std::string(name) + ": " + what);
+    return status;
+}
+
 // ---- debug copy-out kernels ---------------------------------------------------------------
 __global__ void debug_geom_kernel(int P, GeomState g, float* depth, float* xy, float* conic_opacity, float* rgb,
                                   uint32_t* tiles, uint32_t* offsets, uint8_t* clamped) {
@@ -147,6 +152,152 @@ int bin_view(int P, int sh_degree, int M, const float* means3D, const float* sca
     return cur;
 }
 
+// The Gaussians one draw preprocesses.  With no_color, dc and sh are not read.
+struct Scene {
+    int P, sh_degree, M;
+    const float *means3D, *scales; float scale_modifier; const float *rotations, *opacities, *dc, *sh;
+    bool no_color; int* radii;
+};
+
+// The scene checks of a draw, in the order they fire: the view and the sizes; then the SH coefficients and the image workspace;
+// then, for P > 0 only, the inputs and the geometry workspace.  `name` prefixes every message.
+static int check_sizes(const char* name, const glic_view* view, const Scene& sc) {
+    if (int e = check_view(view)) return e;
+    if (sc.P < 0 || sc.sh_degree < 0 || sc.sh_degree > 3 || sc.M < 0) return fail(GLIC_ERR_INVALID_ARGUMENT, name, "bad P / sh_degree / M");
+    return GLIC_OK;
+}
+static int check_image(const char* name, const glic_view* view, const Scene& sc, const void* image_ws, size_t image_bytes) {
+    if (!sc.no_color && (sc.sh_degree + 1) * (sc.sh_degree + 1) - 1 > sc.M)
+        return fail(GLIC_ERR_INVALID_ARGUMENT, name, "sh has fewer coefficients than sh_degree needs");
+    if (!image_ws || image_bytes < glic_image_bytes(view->width, view->height)) return fail(GLIC_ERR_WORKSPACE, name, "image workspace too small");
+    return GLIC_OK;
+}
+static int check_inputs(const char* name, const Scene& sc, const void* geom_ws, size_t geom_bytes) {
+    if (!sc.means3D || !sc.scales || !sc.rotations || !sc.opacities || !sc.radii ||
+        (!sc.no_color && (!sc.dc || (sc.M > 0 && sc.sh_degree > 0 && !sc.sh)))) return fail(GLIC_ERR_INVALID_ARGUMENT, name, "null input pointer");
+    if (!aligned16(sc.rotations)) return fail(GLIC_ERR_INVALID_ARGUMENT, name, "rotations must be 16-byte aligned");
+    if (!geom_ws || geom_bytes < glic_geom_bytes(sc.P)) return fail(GLIC_ERR_WORKSPACE, name, "geometry workspace too small");
+    return GLIC_OK;
+}
+
+// The blend form of a draw, as render_forward_kernel's FORM: training (glic_forward: with colour, the checkpoints into the sample
+// workspace and the bucket offsets), inference (glic_render: colour and depth planes) or scoring (glic_contribution)
+enum DrawForm { DRAW_TRAIN, DRAW_INFER, DRAW_SCORE };
+
+// What one draw writes.  Null planes are not written.
+struct Draw {
+    const char* name;
+    DrawForm form;
+    float empty_T;                  // every pixel's T in an empty scene
+    bool missing_output;            // the caller's own output check failed
+    float *color, *final_T, *depth, *median_depth, *max_weight;
+    uint64_t *hits, *ends;
+    void* sample_ws;                // DRAW_TRAIN with colour only: the checkpoints
+    size_t sample_bytes;
+};
+
+// The planes of an empty scene: T = d.empty_T, every other plane 0
+static int write_empty(const Draw& d, size_t HW, cudaStream_t s) {
+    if (d.final_T && d.empty_T == 0.f) {
+        GLIC_CUDA_TRY(cudaMemsetAsync(d.final_T, 0, sizeof(float) * HW, s));
+    } else if (d.final_T) {
+        fill_kernel<<<(unsigned)std::min<size_t>((HW + 255) / 256, (size_t)NUM_SMS * 8), 256, 0, s>>>(HW, d.empty_T, d.final_T);
+        GLIC_LAUNCH_CHECK();
+    }
+    if (d.color) GLIC_CUDA_TRY(cudaMemsetAsync(d.color, 0, sizeof(float) * 3 * HW, s));
+    if (d.depth) GLIC_CUDA_TRY(cudaMemsetAsync(d.depth, 0, sizeof(float) * HW, s));
+    if (d.median_depth) GLIC_CUDA_TRY(cudaMemsetAsync(d.median_depth, 0, sizeof(float) * HW, s));
+    return GLIC_OK;
+}
+
+// glic_forward, glic_render and glic_contribution: the scene checks, then bin_view on workspaces carved for the largest capacity
+// they hold, one blend and the counters {R, B, overflow} copied to counters_host
+static int draw(const Draw& d, const Scene& sc, const glic_view* view, void* geom_ws, size_t geom_bytes, void* image_ws,
+                size_t image_bytes, void* binning_ws, size_t binning_bytes, int64_t* counters_host, cudaStream_t s) {
+    if (int e = check_sizes(d.name, view, sc)) return e;
+    if (int e = check_image(d.name, view, sc, image_ws, image_bytes)) return e;
+    if (d.missing_output) return fail(GLIC_ERR_INVALID_ARGUMENT, d.name, "null output");
+    const ViewParams vp = make_view_params(view);
+    ImageState img = ImageState::carve(image_ws, vp.W, vp.H);
+    if (sc.P == 0) {
+        if (int e = write_empty(d, (size_t)vp.W * vp.H, s)) return e;
+        GLIC_CUDA_TRY(cudaMemsetAsync(img.hdr, 0, sizeof(ImageHeader), s));
+    } else {
+        if (int e = check_inputs(d.name, sc, geom_ws, geom_bytes)) return e;
+        const bool samples = d.form == DRAW_TRAIN && !sc.no_color;
+        const int64_t cap = glic_binning_capacity(binning_bytes, samples ? d.sample_bytes : 0, vp.W, vp.H, !samples);
+        if (!binning_ws || cap < 1 || (samples && !d.sample_ws))
+            return fail(GLIC_ERR_WORKSPACE, d.name, d.form == DRAW_TRAIN ? "binning / sample workspace missing or too small"
+                                                                         : "binning workspace missing or too small");
+        GeomState g = GeomState::carve(geom_ws, sc.P);
+        BinningState bin = BinningState::carve(binning_ws, cap);
+        SampleState smp = SampleState::carve(samples ? d.sample_ws : nullptr, samples ? glic_max_buckets(cap, vp.W, vp.H) : 0);
+        const int cur = bin_view(sc.P, sc.sh_degree, sc.M, sc.means3D, sc.scales, sc.scale_modifier, sc.rotations, sc.opacities, sc.dc,
+                                 sc.sh, vp, sc.no_color, sc.radii, g, bin, img, cap, samples, s);
+        if (cur < 0) return cur;
+        StageTimer _t(GLIC_STAGE_RENDER_FWD, s);
+        const uint32_t* list = bin.vals[cur];
+        const int e = d.form == DRAW_TRAIN ? launch_render_forward(vp, sc.no_color, list, g, img, smp, d.color, d.final_T, s)
+                    : d.form == DRAW_INFER ? launch_render_infer(vp, list, g, img, d.color, d.final_T, d.depth, d.median_depth, s)
+                                           : launch_render_score(vp, list, g, img, d.max_weight, d.hits, d.ends, d.final_T, s);
+        if (e) return e;
+    }
+    if (counters_host) GLIC_CUDA_TRY(cudaMemcpyAsync(counters_host, img.hdr->counters, 3 * sizeof(long long), cudaMemcpyDeviceToHost, s));
+    return GLIC_OK;
+}
+
+// The state a forward left for its backward in the caller's workspaces, carved for R pairs; the sorted list is bin.vals[cur]
+struct Saved { GeomState g; ImageState img; BinningState bin; SampleState smp; int64_t max_buckets; int cur; };
+static Saved carve_saved(int P, const ViewParams& vp, int64_t R, const void* geom_ws, const void* image_ws, const void* binning_ws,
+                         const void* sample_ws) {
+    const int64_t max_buckets = glic_max_buckets(R, vp.W, vp.H);
+    return {GeomState::carve(const_cast<void*>(geom_ws), P), ImageState::carve(const_cast<void*>(image_ws), vp.W, vp.H),
+            BinningState::carve(const_cast<void*>(binning_ws), R), SampleState::carve(const_cast<void*>(sample_ws), max_buckets),
+            max_buckets, tile_sort_passes(vp.grid_x * vp.grid_y) & 1};
+}
+
+// The render backward of a saved forward: deterministic with det_ws (glic_deterministic_bytes), atomic without
+static int render_backward(int P, const ViewParams& vp, const Saved& sv, void* det_ws, const float* dL_dpix, float* dL_dmeans2D,
+                           float* dL_dconic, float* dL_dopacity, float* dL_dcolors, cudaStream_t s) {
+    StageTimer _t(GLIC_STAGE_RENDER_BWD, s);
+    const uint32_t* list = sv.bin.vals[sv.cur];
+    if (det_ws)
+        return launch_render_backward_det(P, vp, sv.max_buckets, list, sv.g, sv.img, sv.smp, DetState::carve(det_ws, sv.max_buckets),
+                                          dL_dpix, dL_dmeans2D, dL_dconic, dL_dopacity, dL_dcolors, s);
+    return launch_render_backward(P, vp, sv.max_buckets, list, sv.g, sv.img, sv.smp, dL_dpix, dL_dmeans2D, dL_dconic, dL_dopacity,
+                                  dL_dcolors, s);
+}
+
+int backward_compact(int P, int sh_degree, int M, const float* means3D, const float* scales, const float* rotations, const float* sh,
+                     const glic_view* view, const int* radii, int64_t R, const void* geom_ws, const void* binning_ws,
+                     const void* image_ws, const void* sample_ws, const float* dL_dpix, float* dL_dmeans2D, float* dL_dconic,
+                     float* dL_dopacity, float* dL_dcolors, const CompactGrads& cg, cudaEvent_t after_render, cudaStream_t s,
+                     void* det_ws) {
+    if (int e = check_view(view)) return e;
+    if (P <= 0) return GLIC_OK;
+    const ViewParams vp = make_view_params(view);
+    const Saved sv = carve_saved(P, vp, R, geom_ws, image_ws, binning_ws, sample_ws);
+    if (!cg.grads_zeroed) { StageTimer _t(GLIC_STAGE_ZERO, s);
+    // conic | mean2D | opacity carved from ONE block (the mapper's capacity layout): one memset over the span when the slack
+    // between the live prefixes is small, three otherwise
+    const ptrdiff_t span = dL_dconic < dL_dmeans2D && dL_dmeans2D < dL_dopacity ? (dL_dopacity + P) - dL_dconic : -1;
+    if (span > 0 && span <= 10 * (ptrdiff_t)P) {
+        GLIC_CUDA_TRY(cudaMemsetAsync(dL_dconic, 0, sizeof(float) * (size_t)span, s));
+    } else {
+        GLIC_CUDA_TRY(cudaMemsetAsync(dL_dmeans2D, 0, sizeof(float) * 3 * (size_t)P, s));
+        GLIC_CUDA_TRY(cudaMemsetAsync(dL_dconic, 0, sizeof(float) * 4 * (size_t)P, s));
+        GLIC_CUDA_TRY(cudaMemsetAsync(dL_dopacity, 0, sizeof(float) * (size_t)P, s));
+    }
+    GLIC_CUDA_TRY(cudaMemsetAsync(dL_dcolors, 0, sizeof(float) * 3 * (size_t)P, s)); }
+    if (R > 0)
+        if (int e = render_backward(P, vp, sv, det_ws, dL_dpix, dL_dmeans2D, dL_dconic, dL_dopacity, dL_dcolors, s)) return e;
+    // the colour gradients are final here: the multi-GPU push may start while the per-Gaussian backward still runs
+    if (after_render) GLIC_CUDA_TRY(cudaEventRecord(after_render, s));
+    StageTimer _t(GLIC_STAGE_PREPROCESS_BWD, s);
+    return launch_preprocess_backward_compact(P, sh_degree, M, means3D, scales, 1.0f, rotations, sh, vp, radii, sv.g, dL_dmeans2D,
+                                              dL_dconic, dL_dcolors, cg, s);
+}
+
 }  // namespace glic
 
 using namespace glic;
@@ -195,18 +346,14 @@ int glic_forward_preprocess(int P, int sh_degree, int M, const float* means3D, c
                             const float* rotations, const float* opacities, const float* dc, const float* sh,
                             const glic_view* view, int no_color, int* radii, void* geom_ws, size_t geom_bytes,
                             void* image_ws, size_t image_bytes, int64_t* num_rendered_host, void* stream) {
-    if (int e = check_view(view)) return e;
-    if (P < 0 || sh_degree < 0 || sh_degree > 3 || M < 0) { set_error("forward_preprocess: bad P / sh_degree / M"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!num_rendered_host) { set_error("forward_preprocess: num_rendered_host is NULL"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const char* name = "forward_preprocess";
+    const Scene sc{P, sh_degree, M, means3D, scales, scale_modifier, rotations, opacities, dc, sh, no_color != 0, radii};
+    if (int e = check_sizes(name, view, sc)) return e;
+    if (!num_rendered_host) return fail(GLIC_ERR_INVALID_ARGUMENT, name, "num_rendered_host is NULL");
     *num_rendered_host = 0;
-    if (!no_color && (sh_degree + 1) * (sh_degree + 1) - 1 > M) { set_error("forward_preprocess: sh has fewer coefficients than sh_degree needs"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!image_ws || image_bytes < glic_image_bytes(view->width, view->height)) { set_error("forward_preprocess: image workspace too small"); return GLIC_ERR_WORKSPACE; }
+    if (int e = check_image(name, view, sc, image_ws, image_bytes)) return e;
     if (P == 0) return GLIC_OK;
-    if (!means3D || !scales || !rotations || !opacities || !radii || (!no_color && (!dc || (M > 0 && sh_degree > 0 && !sh)))) {
-        set_error("forward_preprocess: null input pointer"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (!aligned16(rotations)) { set_error("forward_preprocess: rotations must be 16-byte aligned"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!geom_ws || geom_bytes < glic_geom_bytes(P)) { set_error("forward_preprocess: geometry workspace too small"); return GLIC_ERR_WORKSPACE; }
+    if (int e = check_inputs(name, sc, geom_ws, geom_bytes)) return e;
     cudaStream_t s = (cudaStream_t)stream;
     GeomState g = GeomState::carve(geom_ws, P);
     const ViewParams vp = make_view_params(view);
@@ -253,21 +400,22 @@ int glic_forward_render(int P, const glic_view* view, int no_color, int64_t R, v
                         void* binning_ws, size_t binning_bytes, void* sample_ws, size_t sample_bytes, float* out_color,
                         float* out_final_T, int64_t* num_buckets_host, void* stream) {
     if (int e = check_view(view)) return e;
-    if (P < 0 || R < 0 || !image_ws || !out_final_T || (!no_color && !out_color)) { set_error("forward_render: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const char* name = "forward_render";
+    if (P < 0 || R < 0 || !image_ws || !out_final_T || (!no_color && !out_color)) return fail(GLIC_ERR_INVALID_ARGUMENT, name, "bad arguments");
     cudaStream_t s = (cudaStream_t)stream;
     const ViewParams vp = make_view_params(view);
     const int T = vp.grid_x * vp.grid_y;
     const size_t HW = (size_t)vp.W * vp.H;
     if (num_buckets_host) *num_buckets_host = 0;
     if (P == 0) {   // rasterize_points.cu:110: zero outputs
-        GLIC_CUDA_TRY(cudaMemsetAsync(out_final_T, 0, sizeof(float) * HW, s));
-        if (out_color) GLIC_CUDA_TRY(cudaMemsetAsync(out_color, 0, sizeof(float) * 3 * HW, s));
-        return GLIC_OK;
+        Draw d{name, DRAW_TRAIN, 0.f};
+        d.color = out_color; d.final_T = out_final_T;
+        return write_empty(d, HW, s);
     }
-    if (!geom_ws) { set_error("forward_render: geometry workspace is NULL"); return GLIC_ERR_WORKSPACE; }
-    if (!binning_ws || binning_bytes < glic_binning_bytes(R)) { set_error("forward_render: binning workspace too small"); return GLIC_ERR_WORKSPACE; }
+    if (!geom_ws) return fail(GLIC_ERR_WORKSPACE, name, "geometry workspace is NULL");
+    if (!binning_ws || binning_bytes < glic_binning_bytes(R)) return fail(GLIC_ERR_WORKSPACE, name, "binning workspace too small");
     const int64_t max_buckets = no_color ? 0 : glic_max_buckets(R, vp.W, vp.H);
-    if (!no_color && (!sample_ws || sample_bytes < glic_sample_bytes(R, vp.W, vp.H))) { set_error("forward_render: sample workspace too small"); return GLIC_ERR_WORKSPACE; }
+    if (!no_color && (!sample_ws || sample_bytes < glic_sample_bytes(R, vp.W, vp.H))) return fail(GLIC_ERR_WORKSPACE, name, "sample workspace too small");
     GeomState g = GeomState::carve(geom_ws, P);
     ImageState img = ImageState::carve(image_ws, vp.W, vp.H);
     BinningState bin = BinningState::carve(binning_ws, R);
@@ -312,40 +460,10 @@ int glic_forward(int P, int sh_degree, int M, const float* means3D, const float*
                  int no_color, int* radii, void* geom_ws, size_t geom_bytes, void* image_ws, size_t image_bytes, void* binning_ws,
                  size_t binning_bytes, void* sample_ws, size_t sample_bytes, float* out_color, float* out_final_T,
                  int64_t* counters_host, void* stream) {
-    if (int e = check_view(view)) return e;
-    if (P < 0 || sh_degree < 0 || sh_degree > 3 || M < 0) { set_error("forward: bad P / sh_degree / M"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!no_color && (sh_degree + 1) * (sh_degree + 1) - 1 > M) { set_error("forward: sh has fewer coefficients than sh_degree needs"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!image_ws || image_bytes < glic_image_bytes(view->width, view->height)) { set_error("forward: image workspace too small"); return GLIC_ERR_WORKSPACE; }
-    if (!out_final_T || (!no_color && !out_color)) { set_error("forward: null output"); return GLIC_ERR_INVALID_ARGUMENT; }
-    cudaStream_t s = (cudaStream_t)stream;
-    const ViewParams vp = make_view_params(view);
-    const size_t HW = (size_t)vp.W * vp.H;
-    ImageState img = ImageState::carve(image_ws, vp.W, vp.H);
-    if (P == 0) {
-        GLIC_CUDA_TRY(cudaMemsetAsync(out_final_T, 0, sizeof(float) * HW, s));
-        if (out_color) GLIC_CUDA_TRY(cudaMemsetAsync(out_color, 0, sizeof(float) * 3 * HW, s));
-        GLIC_CUDA_TRY(cudaMemsetAsync(img.hdr, 0, sizeof(ImageHeader), s));
-        if (counters_host) GLIC_CUDA_TRY(cudaMemcpyAsync(counters_host, img.hdr->counters, 3 * sizeof(long long), cudaMemcpyDeviceToHost, s));
-        return GLIC_OK;
-    }
-    if (!means3D || !scales || !rotations || !opacities || !radii || (!no_color && (!dc || (M > 0 && sh_degree > 0 && !sh)))) {
-        set_error("forward: null input pointer"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (!aligned16(rotations)) { set_error("forward: rotations must be 16-byte aligned"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!geom_ws || geom_bytes < glic_geom_bytes(P)) { set_error("forward: geometry workspace too small"); return GLIC_ERR_WORKSPACE; }
-    const int64_t cap = glic_binning_capacity(binning_bytes, sample_bytes, vp.W, vp.H, no_color);
-    if (!binning_ws || cap < 1 || (!no_color && !sample_ws)) { set_error("forward: binning / sample workspace missing or too small"); return GLIC_ERR_WORKSPACE; }
-    GeomState g = GeomState::carve(geom_ws, P);
-    BinningState bin = BinningState::carve(binning_ws, cap);
-    const int64_t max_buckets = no_color ? 0 : glic_max_buckets(cap, vp.W, vp.H);
-    SampleState smp = SampleState::carve(no_color ? nullptr : sample_ws, max_buckets);
-    const int cur = bin_view(P, sh_degree, M, means3D, scales, scale_modifier, rotations, opacities, dc, sh, vp, no_color != 0, radii, g, bin,
-                             img, cap, !no_color, s);
-    if (cur < 0) return cur;
-    { StageTimer _t(GLIC_STAGE_RENDER_FWD, s);
-      if (int e = launch_render_forward(vp, no_color != 0, bin.vals[cur], g, img, smp, out_color, out_final_T, s)) return e; }
-    if (counters_host) GLIC_CUDA_TRY(cudaMemcpyAsync(counters_host, img.hdr->counters, 3 * sizeof(long long), cudaMemcpyDeviceToHost, s));
-    return GLIC_OK;
+    Draw d{"forward", DRAW_TRAIN, 0.f, !out_final_T || (!no_color && !out_color)};
+    d.color = out_color; d.final_T = out_final_T; d.sample_ws = sample_ws; d.sample_bytes = sample_bytes;
+    const Scene sc{P, sh_degree, M, means3D, scales, scale_modifier, rotations, opacities, dc, sh, no_color != 0, radii};
+    return draw(d, sc, view, geom_ws, geom_bytes, image_ws, image_bytes, binning_ws, binning_bytes, counters_host, (cudaStream_t)stream);
 }
 
 int glic_render(int P, int sh_degree, int M, const float* means3D, const float* scales, float scale_modifier,
@@ -353,42 +471,12 @@ int glic_render(int P, int sh_degree, int M, const float* means3D, const float* 
                 int* radii, void* geom_ws, size_t geom_bytes, void* image_ws, size_t image_bytes, void* binning_ws,
                 size_t binning_bytes, float* out_color, float* out_final_T, float* out_depth, float* out_median_depth,
                 int64_t* counters_host, void* stream) {
-    if (int e = check_view(view)) return e;
-    if (P < 0 || sh_degree < 0 || sh_degree > 3 || M < 0) { set_error("render: bad P / sh_degree / M"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if ((sh_degree + 1) * (sh_degree + 1) - 1 > M) { set_error("render: sh has fewer coefficients than sh_degree needs"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!image_ws || image_bytes < glic_image_bytes(view->width, view->height)) { set_error("render: image workspace too small"); return GLIC_ERR_WORKSPACE; }
-    if (!out_color || !out_final_T) { set_error("render: null output"); return GLIC_ERR_INVALID_ARGUMENT; }
-    cudaStream_t s = (cudaStream_t)stream;
-    const ViewParams vp = make_view_params(view);
-    const size_t HW = (size_t)vp.W * vp.H;
-    ImageState img = ImageState::carve(image_ws, vp.W, vp.H);
-    if (P == 0) {                                      // nothing to draw: T = 1 (nothing covers a pixel), every other plane 0
-        fill_kernel<<<(unsigned)std::min<size_t>((HW + 255) / 256, (size_t)NUM_SMS * 8), 256, 0, s>>>(HW, 1.0f, out_final_T);
-        GLIC_LAUNCH_CHECK();
-        GLIC_CUDA_TRY(cudaMemsetAsync(out_color, 0, sizeof(float) * 3 * HW, s));
-        if (out_depth) GLIC_CUDA_TRY(cudaMemsetAsync(out_depth, 0, sizeof(float) * HW, s));
-        if (out_median_depth) GLIC_CUDA_TRY(cudaMemsetAsync(out_median_depth, 0, sizeof(float) * HW, s));
-        GLIC_CUDA_TRY(cudaMemsetAsync(img.hdr, 0, sizeof(ImageHeader), s));
-        if (counters_host) GLIC_CUDA_TRY(cudaMemcpyAsync(counters_host, img.hdr->counters, 3 * sizeof(long long), cudaMemcpyDeviceToHost, s));
-        return GLIC_OK;
-    }
-    if (!means3D || !scales || !rotations || !opacities || !radii || !dc || (M > 0 && sh_degree > 0 && !sh)) {
-        set_error("render: null input pointer"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (!aligned16(rotations)) { set_error("render: rotations must be 16-byte aligned"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!geom_ws || geom_bytes < glic_geom_bytes(P)) { set_error("render: geometry workspace too small"); return GLIC_ERR_WORKSPACE; }
-    const int64_t cap = glic_binning_capacity(binning_bytes, 0, vp.W, vp.H, 1);     // no sample workspace: nothing is saved
-    if (!binning_ws || cap < 1) { set_error("render: binning workspace missing or too small"); return GLIC_ERR_WORKSPACE; }
-    GeomState g = GeomState::carve(geom_ws, P);
-    BinningState bin = BinningState::carve(binning_ws, cap);
-    // glic_forward's stages up to the blend, so the tile lists are its lists; no checkpoints, so no bucket offsets
-    const int cur = bin_view(P, sh_degree, M, means3D, scales, scale_modifier, rotations, opacities, dc, sh, vp, false, radii, g, bin, img,
-                             cap, false, s);
-    if (cur < 0) return cur;
-    { StageTimer _t(GLIC_STAGE_RENDER_FWD, s);
-      if (int e = launch_render_infer(vp, bin.vals[cur], g, img, out_color, out_final_T, out_depth, out_median_depth, s)) return e; }
-    if (counters_host) GLIC_CUDA_TRY(cudaMemcpyAsync(counters_host, img.hdr->counters, 3 * sizeof(long long), cudaMemcpyDeviceToHost, s));
-    return GLIC_OK;
+    // glic_forward's stages up to the blend, so the tile lists are its lists; no checkpoints, so no bucket offsets.  An empty
+    // scene has T = 1 (nothing covers a pixel)
+    Draw d{"render", DRAW_INFER, 1.f, !out_color || !out_final_T};
+    d.color = out_color; d.final_T = out_final_T; d.depth = out_depth; d.median_depth = out_median_depth;
+    const Scene sc{P, sh_degree, M, means3D, scales, scale_modifier, rotations, opacities, dc, sh, false, radii};
+    return draw(d, sc, view, geom_ws, geom_bytes, image_ws, image_bytes, binning_ws, binning_bytes, counters_host, (cudaStream_t)stream);
 }
 
 int glic_contribution(int P, const float* means3D, const float* scales, float scale_modifier, const float* rotations,
@@ -396,35 +484,13 @@ int glic_contribution(int P, const float* means3D, const float* scales, float sc
                       size_t image_bytes, void* binning_ws, size_t binning_bytes, float* max_weight, uint64_t* hits,
                       uint64_t* ends, float* out_final_T, int64_t* counters_host, void* stream) {
     if (int e = check_view(view)) return e;
-    if (P < 0) { set_error("contribution: P must be >= 0"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!image_ws || image_bytes < glic_image_bytes(view->width, view->height)) { set_error("contribution: image workspace too small"); return GLIC_ERR_WORKSPACE; }
-    if (P > 0 && (!max_weight || !hits)) { set_error("contribution: null output"); return GLIC_ERR_INVALID_ARGUMENT; }
-    cudaStream_t s = (cudaStream_t)stream;
-    const ViewParams vp = make_view_params(view);
-    const size_t HW = (size_t)vp.W * vp.H;
-    ImageState img = ImageState::carve(image_ws, vp.W, vp.H);
-    if (P == 0) {                                      // glic_forward's outputs for an empty scene; nothing to score
-        if (out_final_T) GLIC_CUDA_TRY(cudaMemsetAsync(out_final_T, 0, sizeof(float) * HW, s));
-        GLIC_CUDA_TRY(cudaMemsetAsync(img.hdr, 0, sizeof(ImageHeader), s));
-        if (counters_host) GLIC_CUDA_TRY(cudaMemcpyAsync(counters_host, img.hdr->counters, 3 * sizeof(long long), cudaMemcpyDeviceToHost, s));
-        return GLIC_OK;
-    }
-    if (!means3D || !scales || !rotations || !opacities || !radii) { set_error("contribution: null input pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!aligned16(rotations)) { set_error("contribution: rotations must be 16-byte aligned"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!geom_ws || geom_bytes < glic_geom_bytes(P)) { set_error("contribution: geometry workspace too small"); return GLIC_ERR_WORKSPACE; }
-    const int64_t cap = glic_binning_capacity(binning_bytes, 0, vp.W, vp.H, 1);
-    if (!binning_ws || cap < 1) { set_error("contribution: binning workspace missing or too small"); return GLIC_ERR_WORKSPACE; }
-    GeomState g = GeomState::carve(geom_ws, P);
-    BinningState bin = BinningState::carve(binning_ws, cap);
+    if (P < 0) return fail(GLIC_ERR_INVALID_ARGUMENT, "contribution", "P must be >= 0");
     // glic_forward's stages with no_color = 1, so the lists are its lists; an overflow leaves every range empty (r_eff = 0), so
-    // the blend takes no pair and adds nothing
-    const int cur = bin_view(P, 0, 0, means3D, scales, scale_modifier, rotations, opacities, nullptr, nullptr, vp, true, radii, g, bin,
-                             img, cap, false, s);
-    if (cur < 0) return cur;
-    { StageTimer _t(GLIC_STAGE_RENDER_FWD, s);
-      if (int e = launch_render_score(vp, bin.vals[cur], g, img, max_weight, hits, ends, out_final_T, s)) return e; }
-    if (counters_host) GLIC_CUDA_TRY(cudaMemcpyAsync(counters_host, img.hdr->counters, 3 * sizeof(long long), cudaMemcpyDeviceToHost, s));
-    return GLIC_OK;
+    // the blend takes no pair and adds nothing.  An empty scene has glic_forward's outputs and nothing to score
+    Draw d{"contribution", DRAW_SCORE, 0.f, P > 0 && (!max_weight || !hits)};
+    d.final_T = out_final_T; d.max_weight = max_weight; d.hits = hits; d.ends = ends;
+    const Scene sc{P, 0, 0, means3D, scales, scale_modifier, rotations, opacities, nullptr, nullptr, true, radii};
+    return draw(d, sc, view, geom_ws, geom_bytes, image_ws, image_bytes, binning_ws, binning_bytes, counters_host, (cudaStream_t)stream);
 }
 
 size_t glic_deterministic_bytes(int64_t num_rendered, int width, int height) {
@@ -441,37 +507,25 @@ static int backward_impl(const char* what, int P, int sh_degree, int M, const fl
                          const float* dL_dpix, float lambda_erank, float* dL_dmeans2D, float* dL_dconic, float* dL_dopacity,
                          float* dL_dcolors, float* dL_dmeans3D, float* dL_dcov3D, float* dL_ddc, float* dL_dsh, float* dL_dscales,
                          float* dL_drotations, void* det_ws, cudaStream_t s) {
-    const std::string w(what);
     if (int e = check_view(view)) return e;
-    if (P < 0 || R < 0 || sh_degree < 0 || sh_degree > 3 || M < 0) { set_error(w + ": bad sizes"); return GLIC_ERR_INVALID_ARGUMENT; }
+    if (P < 0 || R < 0 || sh_degree < 0 || sh_degree > 3 || M < 0) return fail(GLIC_ERR_INVALID_ARGUMENT, what, "bad sizes");
     if (P == 0) return GLIC_OK;
     if (!means3D || !scales || !rotations || !radii || !dL_dpix || !dL_dmeans2D || !dL_dconic || !dL_dopacity || !dL_dcolors ||
-        !dL_dmeans3D || !dL_dcov3D || !dL_ddc || !dL_dscales || !dL_drotations || (M > 0 && (!sh || !dL_dsh))) {
-        set_error(w + ": null pointer"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (!aligned16(rotations) || !aligned16(dL_drotations)) { set_error(w + ": rotations / dL_drotations must be 16-byte aligned"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!geom_ws || !image_ws || (R > 0 && (!binning_ws || !sample_ws))) { set_error(w + ": missing saved workspace"); return GLIC_ERR_WORKSPACE; }
+        !dL_dmeans3D || !dL_dcov3D || !dL_ddc || !dL_dscales || !dL_drotations || (M > 0 && (!sh || !dL_dsh)))
+        return fail(GLIC_ERR_INVALID_ARGUMENT, what, "null pointer");
+    if (!aligned16(rotations) || !aligned16(dL_drotations)) return fail(GLIC_ERR_INVALID_ARGUMENT, what, "rotations / dL_drotations must be 16-byte aligned");
+    if (!geom_ws || !image_ws || (R > 0 && (!binning_ws || !sample_ws))) return fail(GLIC_ERR_WORKSPACE, what, "missing saved workspace");
     const ViewParams vp = make_view_params(view);
-    GeomState g = GeomState::carve(const_cast<void*>(geom_ws), P);
-    ImageState img = ImageState::carve(const_cast<void*>(image_ws), vp.W, vp.H);
+    const Saved sv = carve_saved(P, vp, R, geom_ws, image_ws, binning_ws, sample_ws);
     { StageTimer _t(GLIC_STAGE_ZERO, s);
     GLIC_CUDA_TRY(cudaMemsetAsync(dL_dmeans2D, 0, sizeof(float) * 3 * (size_t)P, s));
     GLIC_CUDA_TRY(cudaMemsetAsync(dL_dconic, 0, sizeof(float) * 4 * (size_t)P, s));
     GLIC_CUDA_TRY(cudaMemsetAsync(dL_dopacity, 0, sizeof(float) * (size_t)P, s));
     GLIC_CUDA_TRY(cudaMemsetAsync(dL_dcolors, 0, sizeof(float) * 3 * (size_t)P, s)); }
-    if (R > 0) {
-        BinningState bin = BinningState::carve(const_cast<void*>(binning_ws), R);
-        const int64_t max_buckets = glic_max_buckets(R, vp.W, vp.H);
-        SampleState smp = SampleState::carve(const_cast<void*>(sample_ws), max_buckets);
-        const int cur = tile_sort_passes(vp.grid_x * vp.grid_y) & 1;
-        StageTimer _t(GLIC_STAGE_RENDER_BWD, s);
-        if (int e = det_ws ? launch_render_backward_det(P, vp, max_buckets, bin.vals[cur], g, img, smp, DetState::carve(det_ws, max_buckets),
-                                                        dL_dpix, dL_dmeans2D, dL_dconic, dL_dopacity, dL_dcolors, s)
-                           : launch_render_backward(P, vp, max_buckets, bin.vals[cur], g, img, smp, dL_dpix, dL_dmeans2D, dL_dconic,
-                                                    dL_dopacity, dL_dcolors, s)) return e;
-    }
+    if (R > 0)
+        if (int e = render_backward(P, vp, sv, det_ws, dL_dpix, dL_dmeans2D, dL_dconic, dL_dopacity, dL_dcolors, s)) return e;
     StageTimer _t(GLIC_STAGE_PREPROCESS_BWD, s);
-    return launch_preprocess_backward(P, sh_degree, M, means3D, scales, scale_modifier, rotations, sh, vp, radii, g,
+    return launch_preprocess_backward(P, sh_degree, M, means3D, scales, scale_modifier, rotations, sh, vp, radii, sv.g,
                                       lambda_erank, dL_dmeans2D, dL_dconic, dL_dcolors, dL_dmeans3D, dL_dcov3D, dL_ddc,
                                       dL_dsh, dL_dscales, dL_drotations, s);
 }
@@ -484,9 +538,8 @@ int glic_backward_deterministic(int P, int sh_degree, int M, const float* means3
                                 float* dL_dscales, float* dL_drotations, void* det_ws, size_t det_bytes, void* stream) {
     (void)dc;
     if (int e = check_view(view)) return e;
-    if (P > 0 && R > 0 && (!det_ws || det_bytes < glic_deterministic_bytes(R, view->width, view->height))) {
-        set_error("backward_deterministic: deterministic workspace too small"); return GLIC_ERR_WORKSPACE;
-    }
+    if (P > 0 && R > 0 && (!det_ws || det_bytes < glic_deterministic_bytes(R, view->width, view->height)))
+        return fail(GLIC_ERR_WORKSPACE, "backward_deterministic", "deterministic workspace too small");
     return backward_impl("backward_deterministic", P, sh_degree, M, means3D, scales, scale_modifier, rotations, sh, view, radii, R,
                          geom_ws, binning_ws, image_ws, sample_ws, dL_dpix, lambda_erank, dL_dmeans2D, dL_dconic, dL_dopacity,
                          dL_dcolors, dL_dmeans3D, dL_dcov3D, dL_ddc, dL_dsh, dL_dscales, dL_drotations, det_ws, (cudaStream_t)stream);
@@ -504,59 +557,13 @@ int glic_backward(int P, int sh_degree, int M, const float* means3D, const float
                          dL_dmeans3D, dL_dcov3D, dL_ddc, dL_dsh, dL_dscales, dL_drotations, nullptr, (cudaStream_t)stream);
 }
 
-// Internal (mapper.cu): the backward with the compact gradient form of preprocess_backward.cu.  dL_dcolors is zeroed and
-// accumulated like the other 2-D gradients but may live anywhere (the mapper points it into its exchange block).
-int glic_backward_compact_internal(int P, int sh_degree, int M, const float* means3D, const float* scales, const float* rotations,
-                                   const float* sh, const glic_view* view, const int* radii, int64_t R, const void* geom_ws,
-                                   const void* binning_ws, const void* image_ws, const void* sample_ws, const float* dL_dpix,
-                                   float* dL_dmeans2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolors,
-                                   const glic::CompactGrads* cg, void* after_render_event, void* stream, void* det_ws) {
-    if (int e = check_view(view)) return e;
-    if (P <= 0) return GLIC_OK;
-    cudaStream_t s = (cudaStream_t)stream;
-    const ViewParams vp = make_view_params(view);
-    GeomState g = GeomState::carve(const_cast<void*>(geom_ws), P);
-    ImageState img = ImageState::carve(const_cast<void*>(image_ws), vp.W, vp.H);
-    if (!cg->grads_zeroed) { StageTimer _t(GLIC_STAGE_ZERO, s);
-    // conic | mean2D | opacity carved from ONE block (the mapper's capacity layout): one memset over the span when the slack
-    // between the live prefixes is small, three otherwise
-    const ptrdiff_t span = dL_dconic < dL_dmeans2D && dL_dmeans2D < dL_dopacity ? (dL_dopacity + P) - dL_dconic : -1;
-    if (span > 0 && span <= 10 * (ptrdiff_t)P) {
-        GLIC_CUDA_TRY(cudaMemsetAsync(dL_dconic, 0, sizeof(float) * (size_t)span, s));
-    } else {
-        GLIC_CUDA_TRY(cudaMemsetAsync(dL_dmeans2D, 0, sizeof(float) * 3 * (size_t)P, s));
-        GLIC_CUDA_TRY(cudaMemsetAsync(dL_dconic, 0, sizeof(float) * 4 * (size_t)P, s));
-        GLIC_CUDA_TRY(cudaMemsetAsync(dL_dopacity, 0, sizeof(float) * (size_t)P, s));
-    }
-    GLIC_CUDA_TRY(cudaMemsetAsync(dL_dcolors, 0, sizeof(float) * 3 * (size_t)P, s)); }
-    if (R > 0) {
-        BinningState bin = BinningState::carve(const_cast<void*>(binning_ws), R);
-        const int64_t max_buckets = glic_max_buckets(R, vp.W, vp.H);
-        SampleState smp = SampleState::carve(const_cast<void*>(sample_ws), max_buckets);
-        const int T = vp.grid_x * vp.grid_y;
-        const int cur = tile_sort_passes(T) & 1;
-        StageTimer _t(GLIC_STAGE_RENDER_BWD, s);
-        if (int e = det_ws ? launch_render_backward_det(P, vp, max_buckets, bin.vals[cur], g, img, smp, DetState::carve(det_ws, max_buckets),
-                                                        dL_dpix, dL_dmeans2D, dL_dconic, dL_dopacity, dL_dcolors, s)
-                           : launch_render_backward(P, vp, max_buckets, bin.vals[cur], g, img, smp, dL_dpix, dL_dmeans2D, dL_dconic,
-                                                    dL_dopacity, dL_dcolors, s)) return e;
-    }
-    // the colour gradients are final here: the multi-GPU push may start while the per-Gaussian backward still runs
-    if (after_render_event) GLIC_CUDA_TRY(cudaEventRecord((cudaEvent_t)after_render_event, s));
-    StageTimer _t(GLIC_STAGE_PREPROCESS_BWD, s);
-    return launch_preprocess_backward_compact(P, sh_degree, M, means3D, scales, 1.0f, rotations, sh, vp, radii, g, dL_dmeans2D,
-                                              dL_dconic, dL_dcolors, *cg, s);
-}
-
 int glic_debug_pose_backward(int P, int sh_degree, int M, const float* means3D, const float* scales, const float* rotations,
                              const float* rot_raw, const float* opacity, const float* sh, const glic_view* view, const int* radii,
                              const void* geom_ws, const float* dL_dmeans2D, const float* dL_dconic, const float* dL_dopacity,
                              const float* dL_dcolors, int pose_only, float* g_geo, void* partials, float* pose6, void* stream) {
     if (int e = check_view(view)) return e;
     if (P <= 0 || !means3D || !scales || !rotations || !radii || !geom_ws || !dL_dmeans2D || !dL_dconic || !dL_dcolors || !partials ||
-        !pose6 || (!pose_only && (!g_geo || !rot_raw || !opacity || !dL_dopacity))) {
-        set_error("debug_pose_backward: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
+        !pose6 || (!pose_only && (!g_geo || !rot_raw || !opacity || !dL_dopacity))) return fail(GLIC_ERR_INVALID_ARGUMENT, "debug_pose_backward", "bad arguments");
     CompactGrads cg{};
     if (!pose_only) {                                   // the mapper's compact block: rotation | xyz | log-scale | opacity logit
         cg.g_rot = reinterpret_cast<float4*>(g_geo);
@@ -602,19 +609,15 @@ int glic_debug_render_backward(int P, const glic_view* view, int64_t R, const vo
                                float* dL_dconic, float* dL_dopacity, float* dL_dcolors, int exact, unsigned long long* counters,
                                void* stream) {
     if (int e = check_view(view)) return e;
-    if (P < 0 || R < 0) { set_error("debug_render_backward: bad sizes"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const char* name = "debug_render_backward";
+    if (P < 0 || R < 0) return fail(GLIC_ERR_INVALID_ARGUMENT, name, "bad sizes");
     if (P == 0 || R == 0) return GLIC_OK;
-    if (!dL_dpix || !dL_dmeans2D || !dL_dconic || !dL_dopacity || !dL_dcolors) { set_error("debug_render_backward: null pointer"); return GLIC_ERR_INVALID_ARGUMENT; }
-    if (!geom_ws || !image_ws || !binning_ws || !sample_ws) { set_error("debug_render_backward: missing saved workspace"); return GLIC_ERR_WORKSPACE; }
+    if (!dL_dpix || !dL_dmeans2D || !dL_dconic || !dL_dopacity || !dL_dcolors) return fail(GLIC_ERR_INVALID_ARGUMENT, name, "null pointer");
+    if (!geom_ws || !image_ws || !binning_ws || !sample_ws) return fail(GLIC_ERR_WORKSPACE, name, "missing saved workspace");
     const ViewParams vp = make_view_params(view);
-    GeomState g = GeomState::carve(const_cast<void*>(geom_ws), P);
-    ImageState img = ImageState::carve(const_cast<void*>(image_ws), vp.W, vp.H);
-    BinningState bin = BinningState::carve(const_cast<void*>(binning_ws), R);
-    const int64_t max_buckets = glic_max_buckets(R, vp.W, vp.H);
-    SampleState smp = SampleState::carve(const_cast<void*>(sample_ws), max_buckets);
-    const int cur = tile_sort_passes(vp.grid_x * vp.grid_y) & 1;
-    return launch_render_backward(P, vp, max_buckets, bin.vals[cur], g, img, smp, dL_dpix, dL_dmeans2D, dL_dconic, dL_dopacity,
-                                  dL_dcolors, (cudaStream_t)stream, exact != 0, counters);
+    const Saved sv = carve_saved(P, vp, R, geom_ws, image_ws, binning_ws, sample_ws);
+    return launch_render_backward(P, vp, sv.max_buckets, sv.bin.vals[sv.cur], sv.g, sv.img, sv.smp, dL_dpix, dL_dmeans2D, dL_dconic,
+                                  dL_dopacity, dL_dcolors, (cudaStream_t)stream, exact != 0, counters);
 }
 
 int glic_debug_deterministic_entries(int P, const glic_view* view, int64_t R, const void* geom_ws, const void* binning_ws,
@@ -622,16 +625,15 @@ int glic_debug_deterministic_entries(int P, const glic_view* view, int64_t R, co
                                      float* dL_dmeans2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolors, int64_t* count_host,
                                      uint32_t* gid, uint32_t* tile, float* values, void* stream) {
     if (int e = check_view(view)) return e;
-    if (P < 0 || R < 0 || !count_host) { set_error("debug_deterministic_entries: bad arguments"); return GLIC_ERR_INVALID_ARGUMENT; }
+    const char* name = "debug_deterministic_entries";
+    if (P < 0 || R < 0 || !count_host) return fail(GLIC_ERR_INVALID_ARGUMENT, name, "bad arguments");
     *count_host = 0;
     if (P == 0) return GLIC_OK;
-    if (!dL_dpix || !dL_dmeans2D || !dL_dconic || !dL_dopacity || !dL_dcolors || !gid || !tile || !values) {
-        set_error("debug_deterministic_entries: null pointer"); return GLIC_ERR_INVALID_ARGUMENT;
-    }
-    if (!geom_ws || !image_ws || (R > 0 && (!binning_ws || !sample_ws))) { set_error("debug_deterministic_entries: missing saved workspace"); return GLIC_ERR_WORKSPACE; }
-    if (R > 0 && (!det_ws || det_bytes < glic_deterministic_bytes(R, view->width, view->height))) {
-        set_error("debug_deterministic_entries: deterministic workspace too small"); return GLIC_ERR_WORKSPACE;
-    }
+    if (!dL_dpix || !dL_dmeans2D || !dL_dconic || !dL_dopacity || !dL_dcolors || !gid || !tile || !values)
+        return fail(GLIC_ERR_INVALID_ARGUMENT, name, "null pointer");
+    if (!geom_ws || !image_ws || (R > 0 && (!binning_ws || !sample_ws))) return fail(GLIC_ERR_WORKSPACE, name, "missing saved workspace");
+    if (R > 0 && (!det_ws || det_bytes < glic_deterministic_bytes(R, view->width, view->height)))
+        return fail(GLIC_ERR_WORKSPACE, name, "deterministic workspace too small");
     cudaStream_t s = (cudaStream_t)stream;
     const ViewParams vp = make_view_params(view);
     GLIC_CUDA_TRY(cudaMemsetAsync(dL_dmeans2D, 0, sizeof(float) * 3 * (size_t)P, s));
@@ -639,15 +641,10 @@ int glic_debug_deterministic_entries(int P, const glic_view* view, int64_t R, co
     GLIC_CUDA_TRY(cudaMemsetAsync(dL_dopacity, 0, sizeof(float) * (size_t)P, s));
     GLIC_CUDA_TRY(cudaMemsetAsync(dL_dcolors, 0, sizeof(float) * 3 * (size_t)P, s));
     if (R == 0) return GLIC_OK;
-    GeomState g = GeomState::carve(const_cast<void*>(geom_ws), P);
-    ImageState img = ImageState::carve(const_cast<void*>(image_ws), vp.W, vp.H);
-    BinningState bin = BinningState::carve(const_cast<void*>(binning_ws), R);
-    const int64_t max_buckets = glic_max_buckets(R, vp.W, vp.H);
-    SampleState smp = SampleState::carve(const_cast<void*>(sample_ws), max_buckets);
-    DetState det = DetState::carve(det_ws, max_buckets);
-    const int cur = tile_sort_passes(vp.grid_x * vp.grid_y) & 1;
-    if (int e = launch_render_backward_det(P, vp, max_buckets, bin.vals[cur], g, img, smp, det, dL_dpix, dL_dmeans2D, dL_dconic,
-                                           dL_dopacity, dL_dcolors, s)) return e;
+    const Saved sv = carve_saved(P, vp, R, geom_ws, image_ws, binning_ws, sample_ws);
+    DetState det = DetState::carve(det_ws, sv.max_buckets);
+    if (int e = launch_render_backward_det(P, vp, sv.max_buckets, sv.bin.vals[sv.cur], sv.g, sv.img, sv.smp, det, dL_dpix, dL_dmeans2D,
+                                           dL_dconic, dL_dopacity, dL_dcolors, s)) return e;
     unsigned int* n_valid = det.count;       // reused: the entry count is read by the launches above only
     const int half = det_sorted_half(P);
     unsigned int n = 0;
@@ -655,7 +652,7 @@ int glic_debug_deterministic_entries(int P, const glic_view* view, int64_t R, co
     GLIC_CUDA_TRY(cudaStreamSynchronize(s));
     GLIC_CUDA_TRY(cudaMemsetAsync(n_valid, 0, sizeof(unsigned int), s));
     if (n > 0) {
-        debug_det_entries_kernel<<<(n + 255) / 256, 256, 0, s>>>(n, (uint32_t)P, det.keys[half], det.idx[half], det.vals, img.live_offsets,
+        debug_det_entries_kernel<<<(n + 255) / 256, 256, 0, s>>>(n, (uint32_t)P, det.keys[half], det.idx[half], det.vals, sv.img.live_offsets,
                                                                  vp.grid_x * vp.grid_y, gid, tile, values, n_valid);
         GLIC_LAUNCH_CHECK();
     }

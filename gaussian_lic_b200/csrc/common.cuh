@@ -374,7 +374,7 @@ struct CompactGrads {
     float* dens_norm;         // [P]
     float* dens_count;        // [P]
     // 1: the render backward's accumulators (dL_dmeans2D, dL_dconic, dL_dopacity, dL_dcolors) are zero in rows [0, P) already
-    // (launch_view_flags zeroed them), so glic_backward_compact_internal does not
+    // (launch_view_flags zeroed them), so backward_compact does not
     int grads_zeroed = 0;
 };
 // doubles of the pose-gradient scratch for up to Pcap Gaussians
@@ -452,17 +452,15 @@ int launch_preprocess_backward_compact(int P, int D, int M, const float* means, 
                                        const float* dL_dmean2D, const float* dL_dconic, const float* dL_dcolors,
                                        const CompactGrads& cg, cudaStream_t s);
 
-}  // namespace glic
-
-// internal cross-file entry points (not part of the C ABI)
-extern "C" int glic_backward_compact_internal(int P, int sh_degree, int M, const float* means3D, const float* scales,
-                                              const float* rotations, const float* sh, const glic_view* view, const int* radii,
-                                              int64_t R, const void* geom_ws, const void* binning_ws, const void* image_ws,
-                                              const void* sample_ws, const float* dL_dpix, float* dL_dmeans2D, float* dL_dconic,
-                                              float* dL_dopacity, float* dL_dcolors, const glic::CompactGrads* cg,
-                                              void* after_render_event, void* stream,
-                                              void* det_ws /* NULL: atomic render backward; else glic_deterministic_bytes(R, W, H) */);
-namespace glic {
+// The backward of the last forward into the compact gradient form of preprocess_backward.cu (the mapper's).  dL_dcolors is zeroed
+// and accumulated like the other 2-D gradients but may live anywhere (the mapper points it into its exchange block).
+// after_render (optional) is recorded once the colour gradients are final; det_ws: NULL for the atomic render backward, else
+// glic_deterministic_bytes(R, W, H) for the deterministic one.
+int backward_compact(int P, int sh_degree, int M, const float* means3D, const float* scales, const float* rotations, const float* sh,
+                     const glic_view* view, const int* radii, int64_t R, const void* geom_ws, const void* binning_ws,
+                     const void* image_ws, const void* sample_ws, const float* dL_dpix, float* dL_dmeans2D, float* dL_dconic,
+                     float* dL_dopacity, float* dL_dcolors, const CompactGrads& cg, cudaEvent_t after_render, cudaStream_t s,
+                     void* det_ws);
 int launch_adam_compact(uint32_t P, uint32_t Pcap, int D, int M, float* params, float* exp_avg, float* exp_avg_sq, const float* g_geo,
                         uint32_t Pcap_geo, const float* lr6, const float* g_color, const uint8_t* flags, const float* const* campos_dev,
                         int n_slots, float grad_scale, float color_scale, float b1, float b2, float eps, const unsigned int* skip_flag,

@@ -532,9 +532,9 @@ int photometric_loss(glic_mapper* m, int H, int W, const float* img, const float
 // the backward of the last forward_view of v from dL_dpix: colour gradients into col, after_render (optional) recorded, then cg's
 int backward_view(glic_mapper* m, const glic_view& v, float* col, const CompactGrads& cg, cudaEvent_t after_render) {
     const ArenaRows a = arena_rows(m->params, m->Pcap, m->M);
-    return glic_backward_compact_internal((int)m->P, m->D, m->M, a.xyz, m->act_scales, m->act_rots, a.rest, &v, m->radii, m->bin_cap, m->geom_ws,
-                                          m->binning_ws, m->image_ws, m->sample_ws, m->dL_dpix, m->g_mean2D, m->g_conic, m->g_opacity, col,
-                                          &cg, after_render, m->stream, m->deterministic ? m->det_ws.raw() : nullptr);
+    return glic::backward_compact((int)m->P, m->D, m->M, a.xyz, m->act_scales, m->act_rots, a.rest, &v, m->radii, m->bin_cap, m->geom_ws,
+                                  m->binning_ws, m->image_ws, m->sample_ws, m->dL_dpix, m->g_mean2D, m->g_conic, m->g_opacity, col, cg,
+                                  after_render, m->stream, m->deterministic ? m->det_ws.raw() : nullptr);
 }
 
 // one optimiser step over the view batch `views` (S keyframe indices, slot-major); this rank renders slots [rank*k, rank*k + k)

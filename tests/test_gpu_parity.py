@@ -107,6 +107,86 @@ def test_empty_and_tiny_inputs():
                                    z(5, 1, 3), z(5, 15, 3), 3, torch.as_tensor(cam["campos"]).cuda(), False, False, False)
 
 
+def test_empty_scene_outputs_of_every_draw():
+    """P = 0 through the five draw entry points of the C ABI: every output plane, the host counters, the image header and the
+    launches, starting from NaN planes, junk counters and a junk header.  glic_render writes T = 1 (nothing covers a pixel); the
+    others write T = 0 as rasterize_points.cu:110 does."""
+    import ctypes as C
+    from gaussian_lic_b200 import capi
+    lib = capi.lib
+    W, H = 64, 48
+    _, cam = small_scene(1, W, H, 1, 3)
+    dev = "cuda"
+    t = lambda a: torch.as_tensor(a, dtype=torch.float32).to(dev)
+    vm, pm, cp = t(cam["view"]), t(cam["proj"]), t(cam["campos"])
+    lims = [float(x) for x in cam["lims"]]
+    view = capi.View(vm.data_ptr(), pm.data_ptr(), cp.data_ptr(), cam["tanfovx"], cam["tanfovy"], *lims, W, H)
+    ws = lambda n: torch.empty(max(int(n), 16), dtype=torch.uint8, device=dev)
+    geom, image = ws(lib.glic_geom_bytes(0)), ws(lib.glic_image_bytes(W, H))
+    binning, sample = ws(lib.glic_binning_bytes(64)), ws(lib.glic_sample_bytes(64, W, H))
+    nan = lambda *s: torch.full(s, float("nan"), device=dev)
+    JUNK = -7
+
+    def run(call):
+        image.fill_(0xFF)                                 # the header reads num_rendered = -1, num_buckets = 2^32 - 1
+        counters = (C.c_int64 * 3)(JUNK, JUNK, JUNK)
+        host = C.c_int64(JUNK)
+        torch.cuda.synchronize()
+        before = lib.glic_launch_count()
+        assert call(counters, host) == 0, lib.glic_last_error()
+        torch.cuda.synchronize()
+        hdr = (C.c_int64 * 2)()
+        assert lib.glic_debug_image(W, H, image.data_ptr(), None, None, None, None, hdr, None) == 0
+        torch.cuda.synchronize()
+        return lib.glic_launch_count() - before, list(counters), host.value, list(hdr)
+
+    ptr = lambda x: None if x is None else x.data_ptr()
+    JUNK_HDR = [-1, 2 ** 32 - 1]
+    zero, ones = torch.zeros(H, W, device=dev), torch.ones(H, W, device=dev)
+    for no_color in (0, 1):
+        # glic_forward_preprocess: nothing to launch; R = 0 and the header untouched
+        launches, counters, host, hdr = run(lambda c, h: lib.glic_forward_preprocess(
+            0, 3, 15, None, None, 1.0, None, None, None, None, C.byref(view), no_color, None, None, 0, image.data_ptr(),
+            image.numel(), C.byref(h), None))
+        assert (launches, host, hdr) == (0, 0, JUNK_HDR)
+        # glic_forward_render: T and colour zeroed, B = 0, the header untouched
+        color, T = nan(3, H, W), nan(H, W)
+        launches, counters, host, hdr = run(lambda c, h: lib.glic_forward_render(
+            0, C.byref(view), no_color, 0, geom.data_ptr(), image.data_ptr(), binning.data_ptr(), binning.numel(), sample.data_ptr(),
+            sample.numel(), color.data_ptr(), T.data_ptr(), C.byref(h), None))
+        assert (launches, host, hdr) == (0, 0, JUNK_HDR)
+        assert torch.equal(T, zero) and not color.any()
+        # glic_forward: T and colour zeroed, the counters and the header zero; with no_color a missing colour plane is allowed
+        for color in ((nan(3, H, W), None) if no_color else (nan(3, H, W),)):
+            T = nan(H, W)
+            launches, counters, host, hdr = run(lambda c, h: lib.glic_forward(
+                0, 3, 15, None, None, 1.0, None, None, None, None, C.byref(view), no_color, None, geom.data_ptr(), geom.numel(),
+                image.data_ptr(), image.numel(), binning.data_ptr(), binning.numel(), sample.data_ptr(), sample.numel(), ptr(color),
+                T.data_ptr(), c, None))
+            assert (launches, counters, hdr) == (0, [0, 0, 0], [0, 0])
+            assert torch.equal(T, zero) and (color is None or not color.any())
+    # glic_render: T = 1 by one fill launch, colour and the optional depth planes zeroed, the counters and the header zero
+    for depths in (True, False):
+        color, T = nan(3, H, W), nan(H, W)
+        depth, median = (nan(H, W), nan(H, W)) if depths else (None, None)
+        launches, counters, host, hdr = run(lambda c, h: lib.glic_render(
+            0, 3, 15, None, None, 1.0, None, None, None, None, C.byref(view), None, geom.data_ptr(), geom.numel(), image.data_ptr(),
+            image.numel(), binning.data_ptr(), binning.numel(), color.data_ptr(), T.data_ptr(), ptr(depth), ptr(median), c, None))
+        assert (launches, counters, hdr) == (1, [0, 0, 0], [0, 0])
+        assert torch.equal(T, ones) and not color.any()
+        assert depth is None or (not depth.any() and not median.any())
+    # glic_contribution: T zeroed when asked for, the scores untouched, the counters and the header zero
+    for with_T in (True, False):
+        mw, hits, ends = nan(4), torch.full((4,), 5, dtype=torch.int64, device=dev), torch.full((H * W,), 6, dtype=torch.int64, device=dev)
+        T = nan(H, W) if with_T else None
+        launches, counters, host, hdr = run(lambda c, h: lib.glic_contribution(
+            0, None, None, 1.0, None, None, C.byref(view), None, geom.data_ptr(), geom.numel(), image.data_ptr(), image.numel(),
+            binning.data_ptr(), binning.numel(), mw.data_ptr(), hits.data_ptr(), ends.data_ptr(), ptr(T), c, None))
+        assert (launches, counters, hdr) == (0, [0, 0, 0], [0, 0])
+        assert T is None or torch.equal(T, zero)
+        assert torch.isnan(mw).all() and (hits == 5).all() and (ends == 6).all()
+
+
 def test_torch_shim_autograd_matches_capi(oracle32):
     """The reference-facing symbols (LibTorch shim) driven like rasterizer.cpp / renderer.cpp."""
     from gaussian_lic_b200 import ops
